@@ -17,12 +17,13 @@
 // A K-block of a tile is therefore ONE contiguous byte range that one thread moves with
 // cp.async.bulk (TMA) straight into shared memory; no thread ever touches operand data on the way in.
 //
-// Roles (9 warps, one CTA per SM, persistent over a device-side list of work units):
-//   warps 0-7  two consumer warpgroups: warpgroup w owns rows 64w .. 64w+63 of the tile, issues
-//              wgmma.m64n64k16 per 64-column slice from the shared-memory ring into a
-//              register accumulator of up to 64 x 256, then runs the epilogue straight from registers:
-//              bias + CELU | * CELU'(stored activation) | final layer + gradient seed | plain
-//   warp  8    producer: one lane arms the mbarrier (expect_tx) and issues the bulk copies
+// Roles (3 warpgroups, one CTA per SM, persistent over a device-side list of work units):
+//   warp  0     producer: one lane arms the mbarrier (expect_tx) and issues the bulk copies (warps 1-3 only
+//               hand their registers over to the consumers and exit)
+//   warps 4-11  two consumer warpgroups: warpgroup w owns rows 64w .. 64w+63 of the tile, issues
+//               wgmma.m64n64k16 per 64-column slice from the shared-memory ring into a
+//               register accumulator of up to 64 x 256, then runs the epilogue straight from registers:
+//               bias + CELU | * CELU'(stored activation) | final layer + gradient seed | plain
 // Ring: STAGES slots of (A block + B block of up to 256 rows); the producer runs ahead across units, so
 // the loads of the next unit overlap the epilogue of the current one.
 //
@@ -37,6 +38,8 @@
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -54,8 +57,12 @@ constexpr int A_BLOCK_BYTES = OPND_BLOCK_BYTES;  // 16 / 24 KB: [p1 | p2 (| p3)]
 constexpr int STAGE_BYTES = A_BLOCK_BYTES + PARTS * TN_MAX * ROW_BYTES;  // 48 / 72 KB
 constexpr int STAGES = ANI_OPND_FP16X2 ? 4 : 3;                         // 192 / 216 KB of the 227 KB
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;                 // + alignment of the ring
-constexpr int NUM_CONSUMER_WARPS = 8, PROD_WARP = 8;
-constexpr int THREADS = (NUM_CONSUMER_WARPS + 1) * 32;  // 288: up to 224 registers per thread
+// warpgroup 0 is the producer (one issuing warp), warpgroups 1 and 2 the consumers.  The launch gives every thread 168
+// registers; the producer warpgroup hands all but PROD_REGS back and the consumers take them (2 x 232 + 40 = 504 of the
+// 512 per lane of a sub-partition): room for the 128-register accumulator and the epilogue's prefetched activations.
+constexpr int NUM_CONSUMER_WARPS = 8, PROD_WARP = 0;
+constexpr int THREADS = (NUM_CONSUMER_WARPS + 4) * 32;  // 384
+constexpr int PROD_REGS = 40, CONS_REGS = 232;
 constexpr int MAX_PHASES = 6;
 constexpr int CHAIN_MAX_D = 8;
 constexpr long long SPIN_LIMIT = 6000000000LL;  // ~3 s of clock64 ticks
@@ -164,6 +171,15 @@ __device__ __forceinline__ void red_release_gpu(int32_t* p, int v) {
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 // named barrier of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+// per-thread register budget of the executing warpgroup (all four of its warps execute it)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+// L2 prefetch of a contiguous global range (multiple of 16 bytes)
+__device__ __forceinline__ void prefetch_l2(const void* src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+}
 
 // bounded wait for `*counter >= need` (one thread); raises the status word instead of hanging
 __device__ __forceinline__ void wait_counter(const int32_t* counter, int need, int32_t* status) {
@@ -398,8 +414,11 @@ struct Walk {
     j = 0;
     nt = -1;
   }
+  // CHAIN: F->chain, known at compile time (the producer warp: no registers for the state of the other order)
+  __device__ __forceinline__ bool next(Unit& x) { return F->chain ? next<true>(x) : next<false>(x); }
+  template <bool CHAIN>
   __device__ __forceinline__ bool next(Unit& x) {
-    if (!F->chain) {
+    if (!CHAIN) {
       u += G;
       if (u >= total) return false;
       int t = u, q = 0;
@@ -474,6 +493,16 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
     }
   }
   const int ngroups = tl.bn / 32;
+  // EPI_MUL_DCELU: the stored activation of the next (32-column group, row half) is loaded before the current one is
+  // computed and stored in its place.  (Loads may not pass stores into the same buffer, so without this every step
+  // would wait for a full global round trip.)  [step parity][piece]: chunk q of every piece of the row
+  uint4 ybuf[2][PARTS];
+  auto load_y = [&](int g, int h, uint4 (&dst)[PARTS]) {
+    const unsigned char* blk = ct + (size_t)g * A_BLOCK_BYTES + swz_off(r0 + 8 * h, q);
+#pragma unroll
+    for (int p = 0; p < PARTS; ++p) dst[p] = *reinterpret_cast<const uint4*>(blk + p * A_PART_BYTES);
+  };
+  if (EPI == EPI_MUL_DCELU) load_y(0, 0, ybuf[0]);
 #pragma unroll
   for (int g = 0; g < TN_MAX / 32; ++g) {
     if (g >= ngroups) break;
@@ -481,13 +510,18 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = r0 + 8 * h;
-      // stored activation of this row's 32 columns (EPI_MUL_DCELU): chunk q of every piece, transposed to pairs
+      if (EPI == EPI_MUL_DCELU) {
+        if (h == 0)
+          load_y(g, 1, ybuf[1]);
+        else if (g + 1 < ngroups)
+          load_y(g + 1, 0, ybuf[0]);
+      }
+      // stored activation of this row's 32 columns (EPI_MUL_DCELU), transposed to pairs
       uint32_t yw[PARTS][4];
       if (EPI == EPI_MUL_DCELU) {
-        const unsigned char* blk = ct + (size_t)g * A_BLOCK_BYTES + swz_off(row, q);
 #pragma unroll
         for (int p = 0; p < PARTS; ++p) {
-          const uint4 v = *reinterpret_cast<const uint4*>(blk + p * A_PART_BYTES);
+          const uint4 v = ybuf[h][p];
           yw[p][0] = v.x, yw[p][1] = v.y, yw[p][2] = v.z, yw[p][3] = v.w;
           quad_transpose(yw[p], lane);
         }
@@ -593,90 +627,107 @@ __global__ void __launch_bounds__(THREADS, 1) k_gemm_wg(const __grid_constant__ 
   // everything below may: wait for the previous grid to complete and flush.  No-ops in a plain launch.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  Walk walk;
-  walk.init(F, tms, (int)gridDim.x, (int)blockIdx.x);
-
-  if (warp == PROD_WARP) {
+  if (warp < 4) {
+    setmaxnreg_dec<PROD_REGS>();
+    if (warp != PROD_WARP) return;
     // ================================ producer (TMA) ================================
-    uint32_t stage = 0, phase = 0;
-    int tloc = 0;
-    Unit un;
-    while (walk.next(un)) {
-      const Args& args = F.ph[un.p];
-      const TileMap& tm = tms[un.p];
-      const Tile& tl = un.tl;
-      const Species& sp = args.sp[tl.s];
-      const int nkb = tm.kb_count >= 0 ? tm.kb_count : (sp.K + TK - 1) / TK;
-      if (lane == 0) {
-        stamp(tloc, 0, 0);
-        wait_inputs(F, tms, un.p, tl);
-        if (F.sync) fence_proxy_async_all();
-      }
-      __syncwarp();
-      const int nkb_all = sp.b_kb_moff ? sp.b_kblocks : (sp.K + TK - 1) / TK;  // K-blocks of the stored B operand
-      const int kb_boff = tl.mem * sp.b_kb_moff;                               // split-K: this member's first K-block
-      // A: [row tile][32-column block][p1 | p2 | p3]; this GEMM starts at column member * a_moff
-      const unsigned char* At =
-          args.A + ((size_t)tl.rt * args.a_kblocks + (size_t)(tl.mem * sp.a_moff) / TK) * A_BLOCK_BYTES;
-      // B: [member][n tile][k block][p1 bn x 64 B | p2 | p3]
-      const unsigned char* Bm = sp.Bt + (sp.b_kb_moff ? (size_t)0 : (size_t)tl.mem * sp.N * nkb_all * (PARTS * ROW_BYTES));
-      const uint32_t b_bytes = (uint32_t)tl.bn * ROW_BYTES;  // one piece of the tile's B rows
-      const bool dense = tm.nb_count < 0 || args.b_compact;
-      // the packed B tile this one lies in
-      const int n0p = tl.n0 / TN_MAX * TN_MAX, bnp = min(TN_MAX, (args.b_compact ? tm.n_eff[tl.s] : sp.N) - n0p);
-      // gathered column blocks (layer-1 backward): lane -> (live block q, piece)
-      const int gq = lane / PARTS, gpart = lane % PARTS;
-      size_t g_src = 0;
-      int g_bns = 0;
-      const bool g_active = !dense && lane < PARTS * (tl.bn / 32);
-      if (g_active) {
-        const int row0 = tm.nb[tl.n0 / 32 + gq] * 32;
-        const int n0s = row0 / TN_MAX * TN_MAX;
-        g_bns = min(TN_MAX, sp.N - n0s);
-        g_src = (size_t)n0s * nkb_all * (PARTS * ROW_BYTES) + (size_t)(row0 - n0s) * ROW_BYTES +
-                (size_t)gpart * g_bns * ROW_BYTES;
-      }
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&empty[stage], phase ^ 1);
-        unsigned char* st = smem + stage * STAGE_BYTES;
-        const int kbi = tm.kb_count >= 0 ? tm.kb[kb] : kb;
-        const int kbb = kbi + kb_boff;
+    // one loop per list order: the walk state of the other order would not fit the producer's registers
+    auto produce = [&](auto chain) {
+      Walk walk;
+      walk.init(F, tms, (int)gridDim.x, (int)blockIdx.x);
+      uint32_t stage = 0, phase = 0;
+      int tloc = 0;
+      Unit un;
+      while (walk.template next<decltype(chain)::value>(un)) {
+        const Args& args = F.ph[un.p];
+        const TileMap& tm = tms[un.p];
+        const Tile& tl = un.tl;
+        const Species& sp = args.sp[tl.s];
+        const int nkb = tm.kb_count >= 0 ? tm.kb_count : (sp.K + TK - 1) / TK;
         if (lane == 0) {
-          mbar_arrive_expect_tx(&full[stage], A_BLOCK_BYTES + PARTS * b_bytes);
-          bulk_g2s(st, At + (size_t)kbi * A_BLOCK_BYTES, A_BLOCK_BYTES, &full[stage]);
-          if (dense) {
-            if (tl.bn == bnp) {  // the pieces are adjacent in global memory and in shared memory: one copy
-              bulk_g2s(st + A_BLOCK_BYTES, Bm + ((size_t)tl.n0 * nkb_all + (size_t)kbb * tl.bn) * (PARTS * ROW_BYTES),
-                       PARTS * b_bytes, &full[stage]);
-            } else {             // a column tile inside a packed 256-row B tile: one copy per piece
+          stamp(tloc, 0, 0);
+          wait_inputs(F, tms, un.p, tl);
+          if (F.sync) fence_proxy_async_all();
+          // the stored activation the dCELU epilogue reads: contiguous 32-column blocks of this tile, on their way to L2
+          // while the main loop runs
+          if (F.epi[un.p] == EPI_MUL_DCELU)
+            prefetch_l2(static_cast<const unsigned char*>(args.C) +
+                            ((size_t)tl.rt * args.c_kblocks + (size_t)(tl.mem * sp.c_moff + tl.n0) / TK) * A_BLOCK_BYTES,
+                        (uint32_t)(tl.bn / TK) * A_BLOCK_BYTES);
+        }
+        __syncwarp();
+        const int nkb_all = sp.b_kb_moff ? sp.b_kblocks : (sp.K + TK - 1) / TK;  // K-blocks of the stored B operand
+        const int kb_boff = tl.mem * sp.b_kb_moff;                               // split-K: this member's first K-block
+        // A: [row tile][32-column block][p1 | p2 | p3]; this GEMM starts at column member * a_moff
+        const unsigned char* At =
+            args.A + ((size_t)tl.rt * args.a_kblocks + (size_t)(tl.mem * sp.a_moff) / TK) * A_BLOCK_BYTES;
+        // B: [member][n tile][k block][p1 bn x 64 B | p2 | p3]
+        const unsigned char* Bm = sp.Bt + (sp.b_kb_moff ? (size_t)0 : (size_t)tl.mem * sp.N * nkb_all * (PARTS * ROW_BYTES));
+        const uint32_t b_bytes = (uint32_t)tl.bn * ROW_BYTES;  // one piece of the tile's B rows
+        const bool dense = tm.nb_count < 0 || args.b_compact;
+        // the packed B tile this one lies in
+        const int n0p = tl.n0 / TN_MAX * TN_MAX, bnp = min(TN_MAX, (args.b_compact ? tm.n_eff[tl.s] : sp.N) - n0p);
+        // gathered column blocks (layer-1 backward): lane -> (live block q, piece)
+        const int gq = lane / PARTS, gpart = lane % PARTS;
+        size_t g_src = 0;
+        int g_bns = 0;
+        const bool g_active = !dense && lane < PARTS * (tl.bn / 32);
+        if (g_active) {
+          const int row0 = tm.nb[tl.n0 / 32 + gq] * 32;
+          const int n0s = row0 / TN_MAX * TN_MAX;
+          g_bns = min(TN_MAX, sp.N - n0s);
+          g_src = (size_t)n0s * nkb_all * (PARTS * ROW_BYTES) + (size_t)(row0 - n0s) * ROW_BYTES +
+                  (size_t)gpart * g_bns * ROW_BYTES;
+        }
+        for (int kb = 0; kb < nkb; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          unsigned char* st = smem + stage * STAGE_BYTES;
+          const int kbi = tm.kb_count >= 0 ? tm.kb[kb] : kb;
+          const int kbb = kbi + kb_boff;
+          if (lane == 0) {
+            mbar_arrive_expect_tx(&full[stage], A_BLOCK_BYTES + PARTS * b_bytes);
+            bulk_g2s(st, At + (size_t)kbi * A_BLOCK_BYTES, A_BLOCK_BYTES, &full[stage]);
+            if (dense) {
+              if (tl.bn == bnp) {  // the pieces are adjacent in global memory and in shared memory: one copy
+                bulk_g2s(st + A_BLOCK_BYTES, Bm + ((size_t)tl.n0 * nkb_all + (size_t)kbb * tl.bn) * (PARTS * ROW_BYTES),
+                         PARTS * b_bytes, &full[stage]);
+              } else {             // a column tile inside a packed 256-row B tile: one copy per piece
 #pragma unroll
-              for (int p = 0; p < PARTS; ++p)
-                bulk_g2s(st + A_BLOCK_BYTES + p * b_bytes,
-                         Bm + ((size_t)n0p * nkb_all + (size_t)kbb * bnp) * (PARTS * ROW_BYTES) +
-                             (size_t)p * bnp * ROW_BYTES + (size_t)(tl.n0 - n0p) * ROW_BYTES,
-                         b_bytes, &full[stage]);
+                for (int p = 0; p < PARTS; ++p)
+                  bulk_g2s(st + A_BLOCK_BYTES + p * b_bytes,
+                           Bm + ((size_t)n0p * nkb_all + (size_t)kbb * bnp) * (PARTS * ROW_BYTES) +
+                               (size_t)p * bnp * ROW_BYTES + (size_t)(tl.n0 - n0p) * ROW_BYTES,
+                           b_bytes, &full[stage]);
+              }
             }
           }
+          __syncwarp();
+          if (g_active)
+            bulk_g2s(st + A_BLOCK_BYTES + gpart * b_bytes + gq * 32 * ROW_BYTES,
+                     Bm + g_src + (size_t)kbb * g_bns * (PARTS * ROW_BYTES), 32 * ROW_BYTES, &full[stage]);
+          __syncwarp();
+          if (lane == 0 && kb == 0) stamp(tloc, 0, 1);
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
         }
-        __syncwarp();
-        if (g_active)
-          bulk_g2s(st + A_BLOCK_BYTES + gpart * b_bytes + gq * 32 * ROW_BYTES,
-                   Bm + g_src + (size_t)kbb * g_bns * (PARTS * ROW_BYTES), 32 * ROW_BYTES, &full[stage]);
-        __syncwarp();
-        if (lane == 0 && kb == 0) stamp(tloc, 0, 1);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
+        if (lane == 0) stamp(tloc, 0, 2);
+        ++tloc;
       }
-      if (lane == 0) stamp(tloc, 0, 2);
-      ++tloc;
-    }
+    };
+    if (F.chain)
+      produce(std::true_type{});
+    else
+      produce(std::false_type{});
     return;
   }
 
   // ================================ consumers ================================
-  const int wg = warp >> 2, warp_in_wg = warp & 3;
+  setmaxnreg_inc<CONS_REGS>();
+  Walk walk;
+  walk.init(F, tms, (int)gridDim.x, (int)blockIdx.x);
+  const int wg = (warp >> 2) - 1, warp_in_wg = warp & 3;
   const bool leader = (threadIdx.x & 127) == 0;
   uint32_t stage = 0, phase = 0;
   float omax = 0.f;  // largest |scaled value| this thread handed to the half-precision split

@@ -492,9 +492,10 @@ class Engine:
         self.side_stream = os.environ.get("ANI_B200_SIDE_STREAM", "0") != "0"
         self.overlap_reduce = os.environ.get("ANI_B200_OVERLAP_REDUCE", "1") != "0"
         # The MLP of a step: ONE persistent data-flow launch or the six chained launches of the same GEMM kernel
-        # (csrc/gemm_tc.cuh).  The data-flow list avoids the per-launch tile-count quantisation of long lists; for short
-        # lists (< 3 waves) the chained launches hand a row tile over more cheaply than an L2 counter.  "auto" applies
-        # that rule; ANI_B200_MLP_FUSED=0 / 1 forces one of them.
+        # (csrc/gemm_tc.cuh).  The data-flow list avoids the launch boundaries and the per-launch tile-count quantisation;
+        # on the H100 it is as fast or faster from one wave of units per layer up (water 10 k, 50 k-atom protein, GDB
+        # batch of 256), while below a wave (water 1 k) the chained launches are as fast and hand a row tile over
+        # without an L2 counter.  "auto" applies that rule; ANI_B200_MLP_FUSED=0 / 1 forces one of them.
         self.mlp_mode = os.environ.get("ANI_B200_MLP_FUSED", "auto")
         self._num_sms = torch.cuda.get_device_properties(self.device).multi_processor_count
         self._side_stream: tp.Optional[torch.cuda.Stream] = None
@@ -787,8 +788,7 @@ class Engine:
         if self.mlp_mode in ("0", "1"):
             return self.mlp_mode == "1"
         units = (-(-owned // TILE) + 1) * self.nets.num_members     # per layer: row tiles x members (>= 1 column tile)
-        waves = units / self._num_sms
-        return waves >= 3.0 and waves / math.ceil(waves) < 0.9
+        return units >= self._num_sms
 
     def note_composition(self, ws: Workspace) -> None:
         """Before a graph capture (the shape has already run eagerly): read the element mask of the last
