@@ -617,6 +617,42 @@ def water_box(n_molecules: int, seed: int = 0, density: float = 0.1,
     return z, idx, coords, cell, pbc
 
 
+def seven_element_box(n_atoms: int = 1200, seed: int = 11, density: float = 0.1,
+                      dtype: torch.dtype = torch.float64):
+    """Periodic box with all seven ANI-2x elements (H C N O S F Cl): random-walk chains of 4-12 atoms in the style
+    of ``conformer_batch`` (bonds 1.1-1.5 A), every contact >= 0.9 A under the minimum image, ~0.1 atoms / A^3.
+    Every element pair is present, so every 32-column block of the AEV is live.
+    Returns (elem_idx (1,N), coords (1,N,3), cell, pbc)."""
+    rng = np.random.default_rng(seed)
+    L = (n_atoms / density) ** (1.0 / 3.0)
+    pts = np.zeros((0, 3))
+
+    def free(p):
+        d = pts - p
+        d -= L * np.round(d / L)
+        return len(pts) == 0 or float((d * d).sum(1).min()) >= 0.81
+
+    while len(pts) < n_atoms:
+        start = rng.uniform(0.0, L, 3)
+        if not free(start):
+            continue
+        chain = [start]
+        pts = np.vstack([pts, start])
+        n = int(rng.integers(4, 13))
+        for _ in range(50):
+            if len(chain) >= n or len(pts) >= n_atoms:
+                break
+            d = rng.normal(size=3)
+            p = (chain[int(rng.integers(0, len(chain)))] + d / np.linalg.norm(d) * rng.uniform(1.1, 1.5)) % L
+            if free(p):
+                chain.append(p)
+                pts = np.vstack([pts, p])
+    species = rng.choice(7, size=n_atoms, p=[0.45, 0.25, 0.08, 0.1, 0.04, 0.04, 0.04])
+    species[rng.permutation(n_atoms)[:7]] = np.arange(7)    # every element at least once
+    return (torch.tensor(species).view(1, -1), torch.tensor(pts, dtype=dtype).view(1, -1, 3),
+            torch.eye(3, dtype=dtype) * L, torch.tensor([True, True, True]))
+
+
 def conformer_batch(n_conf: int = 256, a_min: int = 9, a_max: int = 26, seed: int = 1234,
                     dtype: torch.dtype = torch.float32):
     """GDB-11-like padded batch (SURVEY.md 8d config 3): random-walk chains of H/C/N/O,

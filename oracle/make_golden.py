@@ -10,6 +10,7 @@ TEST INFRASTRUCTURE ONLY; runs only in the build container (the GPU box has no
   4. stores inputs + reference outputs as a small fixture.
 
 Usage:  python oracle/make_golden.py            (writes tests/golden/)
+        python oracle/make_golden.py --case sevenel_pbc_ani2x   (only the named cases, comma-separated)
 """
 from __future__ import annotations
 
@@ -102,7 +103,8 @@ def run_reference(aevc, ens, idx, coords, cell, pbc):
     }
 
 
-def main():
+def main(only=None):
+    """``only``: names of the cases to (re)write; all of them by default."""
     torchani = import_reference()
     import oracle.ani_oracle as orc
 
@@ -154,6 +156,12 @@ def main():
     s, x, _ = read_xyz(os.path.join(RES, "small.xyz"))
     cases.append(dict(name="small264_nopbc_ani2x", kind="2x", nl="cell_list", idx=T([[sym2[a] for a in s]]),
                       coords=T(x).unsqueeze(0), cell=None, pbc=None, compact=True))
+    # 11. periodic box with all seven ANI-2x elements (H C N O S F Cl): every element pair, every AEV block live
+    sidx, scoords, scell, spbc = orc.seven_element_box(1200, seed=11)
+    cases.append(dict(name="sevenel_pbc_ani2x", kind="2x", nl="cell_list", idx=sidx, coords=scoords, cell=scell,
+                      pbc=spbc, compact=True))
+    if only:
+        cases = [c for c in cases if c["name"] in only]
 
     seed = 1234
     w2 = orc.make_weights(orc.SYMBOLS_2X, orc.DIMS_2X, 1008, 8, seed, torch.float64)
@@ -198,6 +206,8 @@ def main():
             rec["distances"] = ref["distances"].numpy()[order]
         np.savez_compressed(os.path.join(out_dir, c["name"] + ".npz"), **rec)
 
+    if only:
+        return
     # ---- loop-level oracle vs vectorised oracle on tiny systems (independent restatement)
     spec = orc.aev_spec_2x()
     s, x, cell = read_xyz(os.path.join(RES, "water-0.8nm.xyz"))
@@ -252,5 +262,7 @@ def main_stress():
 if __name__ == "__main__":
     if "--stress" in sys.argv:
         main_stress()
+    elif "--case" in sys.argv:
+        main(only=sys.argv[sys.argv.index("--case") + 1].split(","))
     else:
         main()

@@ -9,7 +9,8 @@ import oracle.ani_oracle as orc
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")
 GOLDEN_CASES = ["ch4_ani1x", "kat2x5_ani2x", "water30_pbc_ani2x", "benzene_pbc_ani2x", "tightcell_pbc_ani2x",
-                "randbatch_ani2x", "small264_nopbc_ani2x", "water999_pbc_ani2x", "6w8h_triclinic_ani2x", "1c17_chunk_hcnos_ani2x"]
+                "randbatch_ani2x", "small264_nopbc_ani2x", "water999_pbc_ani2x", "6w8h_triclinic_ani2x", "1c17_chunk_hcnos_ani2x",
+                "sevenel_pbc_ani2x"]
 
 # Parity bars (BASELINE.json north_star): AEV and atomic energies within 1e-5 relative, forces within
 # 1e-4 Ha/A, judged against the float64 oracle.  "Relative" is applied element-wise with an absolute

@@ -88,6 +88,40 @@ def test_golden_cases(engines, name):
     ws = eng.workspace(*species.shape)
     n_real = int((species >= 0).sum())
     assert int(ws.nbr_cnt[:n_real].sum().item()) == 2 * int(rec["num_pairs"])
+    if name == "sevenel_pbc_ani2x":   # every element pair present: every 32-column block of layer 1 is live
+        assert int(ws.aev_blocks[0]) == 32
+
+
+def test_composition_change_under_a_captured_graph():
+    """A problem shape captured into a CUDA graph with two elements (water: H and O) and replayed with all seven.
+    At capture time Engine.note_composition sizes the shared-memory gradient table of the AEV backward for two
+    elements; on the replay the other element pairs are read from global memory.  The replay must still match the
+    float64 oracle at the golden bars."""
+    from torchani_b200.engine import Engine, PackedNetworks, constants_2x
+    dev = torch.device("cuda:0")
+    rec = load_golden("sevenel_pbc_ani2x")
+    species, coords, cell, pbc = golden_inputs(rec, torch.float32)
+    consts = constants_2x()
+    m = oracle_model("2x")
+    nets = PackedNetworks([[wm[s] for s in m.symbols] for wm in m.weights], consts.out_dim, dev)
+    eng = Engine(consts, nets, [m.sae[s] for s in m.symbols])
+    co, ce = coords.to(dev), cell.to(dev)
+    water = torch.where(species == 0, 0, 3).to(dev)     # the same atoms as H and O only
+    for _ in range(eng.graph_after + 1):                 # eager uses, then the capture
+        eng.step(water, co, ce, True)
+    eng.check_status()
+    ws = eng.workspace(*species.shape)
+    assert len(eng._graphs) == 1 and ws.max_elements == 2
+    res = eng.step(species.to(dev), co, ce, True)       # a replay of that graph, now with seven elements
+    torch.cuda.synchronize()
+    eng.check_status()
+    assert len(eng._graphs) == 1 and int(ws.aev_blocks[0]) == 32
+    ref = orc.compute(oracle_model("2x", torch.float64, "cell_list"), species, coords.double(), cell.double(), pbc)
+    assert_close("member atomic energies", res.member_atomic.cpu().numpy(), ref["member_atomic"].numpy(),
+                 E_RTOL, E_ATOL)
+    assert_close("total energies", res.energies.cpu().numpy(), ref["energy"].numpy(), 0.0, 2e-7 * species.numel())
+    assert_close("forces", -res.grad.cpu().numpy(), ref["forces"].numpy(), 0.0, F_ATOL)
+    assert np.abs(-res.grad.cpu().numpy() - rec["forces"]).max() < F_ATOL
 
 
 def test_conformer_batch_256(engines):

@@ -241,6 +241,13 @@ __device__ __forceinline__ float celu(float x, const CeluConst& c) {
 __device__ __forceinline__ float dcelu_from_out(float y, const CeluConst& c) {
   return y > 0.f ? 1.0f : fmaf(y, c.inv_alpha, 1.0f);
 }
+// running max of |v| in which a NaN sticks (fmaxf drops it): an inf/NaN operand piece turns the products into NaN,
+// and that must raise ANI_STATUS_OPERAND_RANGE like any other value out of range
+__device__ __forceinline__ float max_abs_nan(float m, float v) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(m), "f"(fabsf(v)));
+  return r;
+}
 
 // ---- tile enumeration -----------------------------------------------------------------------
 // Row tiles of one species are contiguous; tile t -> (species, row tile, member, n0, bn).
@@ -295,6 +302,7 @@ __device__ __forceinline__ void build_tile_map(const Args& a, TileMap& tm) {
   // Short lists (less than half a wave of 256-column tiles: 1 k-atom systems, multi-GPU shards): split every
   // accumulator into two column tiles -- twice the CTAs at work, each with half the main loop and half the epilogue,
   // which is what the latency of the layer chain is made of.  (Tiles never straddle a packed 256-row B tile.)
+  // tests/test_gpu_mlp.py restates this rule (layer1_forward_tiles) to assert which side its cases run: change both.
   if (a.allow_narrow && wide > 0 && 2 * wide <= (int)gridDim.x) {
     for (int s = 0; s < S; ++s) {
       tm.tn[s] = tm.n_eff[s] > TN_MAX ? TN_MAX / 2 : max(32, ((tm.n_eff[s] / 32 + 1) / 2) * 32);
@@ -555,7 +563,7 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
           }
           if (EPI != EPI_PLAIN) {
             v *= args.out_scale;
-            omax = fmaxf(omax, fabsf(v));
+            omax = max_abs_nan(omax, v);
           }
           o[j][e] = v;
         }

@@ -285,6 +285,7 @@ static int mlp_common(const ani_mlp_model* model, int rows_cap, const int32_t* r
 // rest of the sum goes through vector REDs into dx).  1 = round 1 (one unit per member: most parallelism, 8 partial
 // sums per element); larger groups halve / quarter the RED traffic and the per-unit ramp at the price of fewer units.
 // By row capacity (larger systems have units to spare) unless ANI_B200_L1B_GROUP pins it.
+// tests/test_gpu_mlp.py restates this rule (l1b_group) to assert which group each of its cases runs: change both.
 static int l1b_group(int M, int rows_cap) {
   static const int env = []() {
     const char* e = getenv("ANI_B200_L1B_GROUP");
