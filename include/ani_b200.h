@@ -384,6 +384,15 @@ int ani_b200_mlp_step(const ani_mlp_model* model, const void* x, float* dx, int 
                       const int32_t* layout_info, const int32_t* aev_blocks, void* act1, void* act2, void* act3,
                       float* e_member, int want_backward, int32_t* sync_i32, int32_t* status, void* stream);
 
+/*    The same step with gradients (want_backward == 1) as one launch that keeps every intermediate of a      */
+/*    (row tile, member) chain in shared memory (csrc/mlp_resident.cuh): act1 / act2 receive the activations   */
+/*    a1 / a2 (tiled, scaled like the forward's), e_member and dx as above; no act3, no gradient pieces in     */
+/*    global memory, no counters.  ANI_ERR_UNSUPPORTED in the 3 x bf16 build and for models with a hidden      */
+/*    width above 256.                                                                                         */
+int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void* x, float* dx, int rows_cap,
+                               const int32_t* row_atom, const int32_t* layout_info, const int32_t* aev_blocks,
+                               void* act1, void* act2, float* e_member, int32_t* status, void* stream);
+
 /* 7. Scatter per-member atomic energies back to input order and reduce per conformer.      */
 /*      atomic_out f32[n] (mean over active members, 0 for padding; flat input order)         */
 /*      member_atomic_out f32[M][n] or NULL                                                    */

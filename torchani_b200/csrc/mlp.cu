@@ -17,6 +17,7 @@
 
 #include "common.cuh"
 #include "gemm_tc.cuh"
+#include "mlp_resident.cuh"
 
 namespace ani {
 
@@ -235,10 +236,9 @@ extern "C" int ani_b200_pack_b_operand(const float* src, int n, int k, int ld_sr
   return ANI_OK;
 }
 
-// shared argument checks + the launch-invariant part of the GEMM arguments
-static int mlp_common(const ani_mlp_model* model, int rows_cap, const int32_t* row_atom, const int32_t* layout_info,
-                      void* act1, void* act2, void* act3, int32_t* status, tc::Args& ta) {
-  if (!model || !row_atom || !layout_info || !act1 || !act2 || !act3) return ANI_ERR_BAD_ARG;
+// argument checks of the model and the row capacity
+static int check_model(const ani_mlp_model* model, int rows_cap) {
+  if (!model) return ANI_ERR_BAD_ARG;
   const int S = model->num_species, M = model->num_members;
   if (S < 1 || S > ANI_MAX_SPECIES || M < 1 || M > ANI_MAX_MEMBERS) return ANI_ERR_BAD_ARG;
   if (rows_cap < ANI_TILE_ROWS || rows_cap % ANI_TILE_ROWS) return ANI_ERR_BAD_ARG;
@@ -254,6 +254,16 @@ static int mlp_common(const ani_mlp_model* model, int rows_cap, const int32_t* r
     for (int l = 0; l < 3; ++l)
       if (ANI_OPND_FP16X2 && !(p.w_scale[l] > 0.f)) return ANI_ERR_BAD_ARG;
   }
+  return ANI_OK;
+}
+
+// shared argument checks + the launch-invariant part of the GEMM arguments
+static int mlp_common(const ani_mlp_model* model, int rows_cap, const int32_t* row_atom, const int32_t* layout_info,
+                      void* act1, void* act2, void* act3, int32_t* status, tc::Args& ta) {
+  if (!model || !row_atom || !layout_info || !act1 || !act2 || !act3) return ANI_ERR_BAD_ARG;
+  const int rc = check_model(model, rows_cap);
+  if (rc != ANI_OK) return rc;
+  const int S = model->num_species, M = model->num_members;
   ta.layout_info = layout_info;
   ta.kblocks = nullptr;
   ta.nblocks = nullptr;
@@ -583,6 +593,93 @@ extern "C" int ani_b200_mlp_step(const ani_mlp_model* model, const void* x, floa
   }
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
+}
+
+// ---- the whole MLP of a step as ONE launch of resident chains (mlp_resident.cuh) ----------------------------------
+extern "C" int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void* x, float* dx, int rows_cap,
+                                          const int32_t* row_atom, const int32_t* layout_info,
+                                          const int32_t* aev_blocks, void* act1, void* act2, float* e_member,
+                                          int32_t* status, void* stream) {
+  if (!x || !dx || !e_member || !row_atom || !layout_info || !act1 || !act2) return ANI_ERR_BAD_ARG;
+  const int rc = check_model(model, rows_cap);
+  if (rc != ANI_OK) return rc;
+#if !ANI_OPND_FP16X2
+  return ANI_ERR_UNSUPPORTED;  // 3 x bf16 K-blocks are 24 KB: R would need 192 KB
+#else
+  const int S = model->num_species, M = model->num_members, ldx = model->ldx;
+  for (int s = 0; s < S; ++s) {
+    const ani_mlp_species& p = model->sp[s];
+    if (p.h1 > tc::RES_KBLOCKS * tc::TK || p.h2 > tc::RES_KBLOCKS * tc::TK || p.h3 > tc::RES_KBLOCKS * tc::TK)
+      return ANI_ERR_UNSUPPORTED;
+  }
+  if (ldx / 32 > tc::MAX_BLOCKS) return ANI_ERR_UNSUPPORTED;
+  static tc::ResArgs F;   // ~2 KB: built in place, passed by value (__grid_constant__)
+  const float sv = OPND_SCALE_VALUE, sg = OPND_SCALE_GRAD;
+  const bool compact = use_b1_compact(model, aev_blocks);
+  F.x = static_cast<const unsigned char*>(x);
+  F.act1 = static_cast<unsigned char*>(act1);
+  F.act2 = static_cast<unsigned char*>(act2);
+  F.dx = dx;
+  F.e_member = e_member;
+  F.layout_info = layout_info;
+  F.row_atom = row_atom;
+  F.blocks = aev_blocks;
+  F.kbx = ldx / 32;
+  F.kb1 = M * model->h1_max / 32;
+  F.kb2 = M * model->h2_max / 32;
+  F.ldx = ldx;
+  F.rows_cap = rows_cap;
+  F.members = M;
+  F.num_species = S;
+  F.b_compact = compact;
+  F.alpha = model->celu_alpha;
+  F.status = status;
+  for (int m = 0; m < ANI_MAX_MEMBERS; ++m) F.member_scale[m] = m < M ? model->member_scale[m] : 0.f;
+  for (int s = 0; s < S; ++s) {
+    const ani_mlp_species& p = model->sp[s];
+    tc::ResSpecies& r = F.sp[s];
+    r.B[0] = static_cast<const unsigned char*>(p.t_f1);
+    r.B[1] = static_cast<const unsigned char*>(p.t_f2);
+    r.B[2] = static_cast<const unsigned char*>(p.t_f3);
+    r.B[3] = static_cast<const unsigned char*>(p.t_b3);
+    r.B[4] = static_cast<const unsigned char*>(p.t_b2);
+    r.B[5] = compact ? b1_compact_ptr(model, s) : static_cast<const unsigned char*>(p.t_b1);
+    r.bias[0] = p.b1;
+    r.bias[1] = p.b2;
+    r.bias[2] = p.b3;
+    r.w4 = p.w4;
+    r.b4 = p.b4;
+    r.h1 = p.h1;
+    r.h2 = p.h2;
+    r.h3 = p.h3;
+    const float acc[tc::RES_PHASES] = {sv * wsc(p, 0), sv * wsc(p, 1), sv * wsc(p, 2),
+                                       sg * wsc(p, 2), sg * wsc(p, 1), sg * wsc(p, 0)};
+    for (int q = 0; q < tc::RES_PHASES; ++q) r.acc_scale[q] = 1.0f / acc[q];
+  }
+  // the longest chains first (one chain = the six GEMMs of one row tile and member)
+  auto cost = [&](int s) {
+    const ani_mlp_species& p = model->sp[s];
+    return (long long)ldx * p.h1 + (long long)p.h1 * p.h2 + (long long)p.h2 * p.h3;
+  };
+  for (int s = 0; s < S; ++s) F.order[s] = s;
+  for (int i = 1; i < S; ++i)
+    for (int j = i; j > 0 && cost(F.order[j]) > cost(F.order[j - 1]); --j) {
+      const int t = F.order[j];
+      F.order[j] = F.order[j - 1];
+      F.order[j - 1] = t;
+    }
+  static const bool attr = []() {
+    return cudaFuncSetAttribute(tc::k_mlp_resident, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::RES_SMEM_BYTES) ==
+           cudaSuccess;
+  }();
+  (void)attr;
+  cudaStream_t st = (cudaStream_t)stream;
+  // zero the live blocks of dx (the members' REDs accumulate into it) and gather the compact W1^T operands
+  launch_zero_compact(model, M > 1 ? dx : nullptr, layout_info, aev_blocks, st);
+  tc::k_mlp_resident<<<num_sms(), tc::THREADS, tc::RES_SMEM_BYTES, st>>>(F);
+  ANI_CUDA_CHECK_LAUNCH();
+  return ANI_OK;
+#endif
 }
 
 extern "C" int ani_b200_mlp_forward_backward(const ani_mlp_model* model, const void* x, float* dx, int rows_cap,

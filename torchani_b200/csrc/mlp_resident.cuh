@@ -1,0 +1,445 @@
+// The whole ensemble MLP of a step with every intermediate resident in shared memory (sm_90a, 2 x fp16 build).
+//
+// A chain is one (128-row tile, member) pair.  One persistent CTA per SM runs whole chains, each as six phases back to
+// back, and hands every layer's output to the next layer through a resident region R of shared memory instead of
+// global memory:
+//
+//   phase  A operand                B operand (ring)               epilogue
+//   0      x live K-blocks (ring)   W1_m                           a1 = CELU(.)  -> R and act1 (for phase 4)
+//   1      R                        W2_m                           a2 = CELU(.)  -> R and act2 (for phase 3)
+//   2      R                        W3_m                           head: e_member; G3 -> R
+//   3      R                        W3_m^T                         G2 = (.) * CELU'(act2) -> R
+//   4      R                        W2_m^T                         G1 = (.) * CELU'(act1) -> R
+//   5      R                        W1^T (member m's K-blocks),    dE/dAEV: vector REDs into dx (M > 1) or stores
+//                                   <= 256 live columns per tile
+//
+// R is 8 K-blocks (256 columns) in the tiled-operand layout of common.cuh, so the wgmma descriptors of gemm_tc.cuh read
+// it unchanged.  Consumer warpgroup w reads and writes only rows 64w .. 64w+63 of R: a phase's output goes into R after
+// the warpgroup's last wgmma of that phase has retired, and a warpgroup barrier after fence.proxy.async makes it
+// visible to the next phase's wgmma.  The dCELU loads of phases 3 and 4 read back what the same thread stored in phases
+// 1 and 0 (tile_epilogue's thread -> (row, chunk) map is the same in every phase).  The only inputs are x (an earlier
+// launch) and the weights, so nothing waits on another CTA: the producer streams B (and x in phase 0) ahead across
+// phase and chain boundaries, limited only by the free ring slots.
+//
+// Shared memory: R 128 KB + a ring of six 16 KB slots + 1 KB alignment = 230,400 B.  A K-block takes one slot for
+// the x block of phase 0 and one per 128 rows of B.
+// The 3 x bf16 build would need 192 KB for R and does not compile this kernel.
+#pragma once
+#include "gemm_tc.cuh"
+
+namespace ani {
+namespace tc {
+
+constexpr int RES_KBLOCKS = 8;   // widest layer of an eligible model: 256 columns
+constexpr int RES_PHASES = 6;
+#if ANI_OPND_FP16X2
+constexpr int RES_BYTES = RES_KBLOCKS * A_BLOCK_BYTES;                  // 128 KB
+// Ring of 16 KB slots: one x K-block, or 128 rows of a B K-block ([p1 128 x 64 B | p2 128 x 64 B]).  A K-block takes
+// 1-3 slots, so phases 1-5 keep two K-blocks of B in flight where 48 KB stages would keep one.
+constexpr int RES_SLOT_BYTES = A_BLOCK_BYTES;
+constexpr int RES_SLOTS = 6;
+constexpr int RES_HALF = TN_MAX / 2;                                    // B rows per slot
+constexpr int RES_SMEM_BYTES = RES_BYTES + RES_SLOTS * RES_SLOT_BYTES + 1024;
+static_assert(RES_SMEM_BYTES <= 232448 - 1024, "resident MLP: shared memory over the per-block limit");
+static_assert(PARTS * RES_HALF * ROW_BYTES == RES_SLOT_BYTES, "a slot holds 128 B rows of every piece");
+#endif
+
+struct ResSpecies {
+  const unsigned char* B[RES_PHASES];  // tiled B operands of the phases: W1, W2, W3, W3^T, W2^T per member; W1^T shared
+  const float* bias[3];                // [M][h] per layer
+  const float* w4;                     // [M][h3]
+  const float* b4;                     // [M]
+  int h1, h2, h3;
+  float acc_scale[RES_PHASES];         // 1 / (scale of A x scale of B) of every phase
+};
+
+struct ResArgs {
+  const unsigned char* x;              // tiled AEV operand, kbx K-blocks per row tile
+  unsigned char* act1;                 // tiled a1 [row tile][kb1], member m at column m * h1
+  unsigned char* act2;                 // tiled a2 [row tile][kb2]
+  float* dx;                           // plain [rows_cap][ldx]
+  float* e_member;                     // [M][rows_cap]
+  const int32_t* layout_info;          // [4 + S + 1]: ..., first row tile of species s, total row tiles
+  const int32_t* row_atom;             // [rows_cap], -1 for padding rows
+  const int32_t* blocks;               // live 32-column AEV blocks [count, ids...] or nullptr (all live)
+  int kbx, kb1, kb2, ldx, rows_cap, members, num_species;
+  int b_compact;                       // with `blocks`: B[5] holds only the live column blocks (mlp.cu b1_compact)
+  float alpha;
+  int32_t* status;
+  int order[ANI_MAX_SPECIES];          // species by decreasing chain length: the longest chains start first
+  float member_scale[ANI_MAX_MEMBERS];
+  ResSpecies sp[ANI_MAX_SPECIES];
+};
+
+#if ANI_OPND_FP16X2
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// 16-byte store into R by its shared-window address (a generic store would take the global-memory path)
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+
+// chain c of the list: species in `order`, then row tile, then member.  false: past the end
+__device__ __forceinline__ bool res_chain(const ResArgs& a, const int* first, int c, int& s, int& rt, int& m) {
+  for (int i = 0; i < a.num_species; ++i) {
+    const int t = a.order[i];
+    const int n = (first[t + 1] - first[t]) * a.members;
+    if (c < n) {
+      s = t;
+      rt = first[t] + c / a.members;
+      m = c % a.members;
+      return true;
+    }
+    c -= n;
+  }
+  return false;
+}
+
+// The r-th chain of this CTA: round r of gridDim.x chains, every other round in reverse CTA order.  The list is sorted
+// longest first, so a CTA that took one of the first (longest) chains of a round takes one of the last (shortest) of
+// the next: with 2-3 chains per CTA (a GDB batch of 256: H, C, N, O) the busiest CTA gets H + N + O instead of H + C + O.
+__device__ __forceinline__ int res_chain_id(int r) {
+  return r * (int)gridDim.x + ((r & 1) ? (int)gridDim.x - 1 - (int)blockIdx.x : (int)blockIdx.x);
+}
+
+// K-blocks of the A operand and output columns of phase p (nblk < 0: every AEV block is live)
+__device__ __forceinline__ void res_phase(const ResArgs& a, const ResSpecies& sp, int p, int nblk, int& nkb, int& n) {
+  switch (p) {
+    case 0: nkb = nblk >= 0 ? nblk : a.kbx; n = sp.h1; break;
+    case 1: nkb = sp.h1 / TK; n = sp.h2; break;
+    case 2: nkb = sp.h2 / TK; n = sp.h3; break;
+    case 3: nkb = sp.h3 / TK; n = sp.h2; break;
+    case 4: nkb = sp.h2 / TK; n = sp.h1; break;
+    default: nkb = sp.h1 / TK; n = nblk >= 0 ? nblk * TK : a.ldx; break;
+  }
+}
+
+// ---- epilogue of one consumer warpgroup and phase P: 64 rows x bn columns from the accumulator registers ----
+// Same register -> (row, column) map as tile_epilogue (gemm_tc.cuh).
+template <int P>
+__device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies& sp, int rt, int m, int n0, int bn,
+                                             float (&acc)[4][32], uint32_t res, const int* blk, int nblk, int wg,
+                                             int lane, int warp_in_wg, float& omax) {
+  constexpr bool ACT = P <= 1, HEAD = P == 2, DCELU = P == 3 || P == 4, PLAIN = P == 5;
+  const CeluConst cc{a.alpha, 1.0f / a.alpha, 1.4426950408889634f / a.alpha};
+  const int q = lane & 3;
+  const int r0 = 64 * wg + 16 * warp_in_wg + (lane >> 2);  // rows r0 and r0 + 8 of the tile
+  const float acc_scale = sp.acc_scale[P];
+  const float out_scale = ACT ? OPND_SCALE_VALUE : OPND_SCALE_GRAD;
+  // the global copy of a1 / a2: written by phases 0 / 1, read back for CELU' by phases 4 / 3
+  unsigned char* ct = nullptr;
+  if (P == 0 || P == 4) ct = a.act1 + ((size_t)rt * a.kb1 + (size_t)(m * sp.h1) / TK) * A_BLOCK_BYTES;
+  if (P == 1 || P == 3) ct = a.act2 + ((size_t)rt * a.kb2 + (size_t)(m * sp.h2) / TK) * A_BLOCK_BYTES;
+  const float* bias = P <= 2 ? sp.bias[P] + (size_t)m * (P == 0 ? sp.h1 : P == 1 ? sp.h2 : sp.h3) : nullptr;
+  const float* w4 = HEAD ? sp.w4 + (size_t)m * sp.h3 : nullptr;
+  float e_acc[2] = {0.f, 0.f}, seed[2] = {0.f, 0.f};
+  bool row_valid[2] = {false, false};
+  if (HEAD) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      row_valid[h] = a.row_atom[rt * TM + r0 + 8 * h] >= 0;
+      seed[h] = row_valid[h] ? a.member_scale[m] : 0.f;
+    }
+  }
+  const int ngroups = bn / 32;
+  // dCELU: the stored activation of the next (32-column group, row half) is loaded before the current one is computed
+  uint4 ybuf[2][PARTS];
+  auto load_y = [&](int g, int h, uint4 (&dst)[PARTS]) {
+    const unsigned char* b = ct + (size_t)g * A_BLOCK_BYTES + swz_off(r0 + 8 * h, q);
+#pragma unroll
+    for (int p = 0; p < PARTS; ++p) dst[p] = *reinterpret_cast<const uint4*>(b + p * A_PART_BYTES);
+  };
+  if (DCELU) load_y(0, 0, ybuf[0]);
+  // One loop iteration per 32-column group, NOT unrolled: the body is compiled once per phase instead of eight times.
+  // Unrolled, the kernel was 23 k instructions and its epilogues took twice as long on the H100, most likely because
+  // every epilogue ran from a cold instruction cache.  The group's 16 accumulator registers are selected into `ag`
+  // first (static register names).
+#pragma unroll 1
+  for (int g = 0; g < ngroups; ++g) {
+    float ag[16];
+    switch (g) {
+#define ANI_RES_PICK(G)                                                     \
+  case G:                                                                   \
+    _Pragma("unroll") for (int i = 0; i < 16; ++i) ag[i] = acc[(G) >> 1][((G) & 1) * 16 + i]; \
+    break;
+      ANI_RES_PICK(0) ANI_RES_PICK(1) ANI_RES_PICK(2) ANI_RES_PICK(3)
+      ANI_RES_PICK(4) ANI_RES_PICK(5) ANI_RES_PICK(6)
+      default: ANI_RES_PICK(7)
+#undef ANI_RES_PICK
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      if (DCELU) {
+        if (h == 0)
+          load_y(g, 1, ybuf[1]);
+        else if (g + 1 < ngroups)
+          load_y(g + 1, 0, ybuf[0]);
+      }
+      uint32_t yw[PARTS][4];
+      if (DCELU) {
+#pragma unroll
+        for (int p = 0; p < PARTS; ++p) {
+          const uint4 v = ybuf[h][p];
+          yw[p][0] = v.x, yw[p][1] = v.y, yw[p][2] = v.z, yw[p][3] = v.w;
+          quad_transpose(yw[p], lane);
+        }
+      }
+      uint32_t w[PARTS][4];
+      float o[4][2];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int col = 32 * g + 8 * j + 2 * q;  // column inside the tile
+        float2 b2 = make_float2(0.f, 0.f), w2 = make_float2(0.f, 0.f), y2 = make_float2(0.f, 0.f);
+        if (P <= 2) b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
+        if (HEAD) w2 = __ldg(reinterpret_cast<const float2*>(w4 + col));
+        if (DCELU) {
+          uint32_t pw[PARTS];
+#pragma unroll
+          for (int p = 0; p < PARTS; ++p) pw[p] = yw[p][j];
+          y2 = join_pair(pw);
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float v = ag[4 * j + 2 * h + e] * acc_scale;
+          const float bb = e ? b2.y : b2.x, ww = e ? w2.y : w2.x, yy = e ? y2.y : y2.x;
+          if (ACT) {
+            v = celu(v + bb, cc);
+          } else if (DCELU) {
+            v *= dcelu_from_out(yy * (1.0f / OPND_SCALE_VALUE), cc);
+          } else if (HEAD) {
+            const float av = celu(v + bb, cc);
+            e_acc[h] = fmaf(av, ww, e_acc[h]);
+            v = seed[h] * ww * dcelu_from_out(av, cc);
+          }
+          if (!PLAIN) {
+            v *= out_scale;
+            omax = max_abs_nan(omax, v);
+          }
+          o[j][e] = v;
+        }
+        if (!PLAIN) {
+          uint32_t pw[PARTS];
+          split_pair(o[j][0], o[j][1], pw);
+#pragma unroll
+          for (int p = 0; p < PARTS; ++p) w[p][j] = pw[p];
+        }
+      }
+      if (PLAIN) {
+        float* dst_row = a.dx + (size_t)(rt * TM + row) * a.ldx;
+        // live column blocks map back to their place: group g of the tile is live block n0 / 32 + g
+        const int col0 = nblk >= 0 ? blk[n0 / 32 + g] * 32 : n0 + g * 32;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          float* dst = dst_row + col0 + 8 * j + 2 * q;
+          if (a.members > 1)
+            red_add_v2(dst, o[j][0], o[j][1]);
+          else
+            *reinterpret_cast<float2*>(dst) = make_float2(o[j][0], o[j][1]);
+        }
+      } else {
+        const uint32_t off = (uint32_t)g * A_BLOCK_BYTES + swz_off(row, q);
+#pragma unroll
+        for (int p = 0; p < PARTS; ++p) {
+          quad_transpose(w[p], lane);
+          const uint4 v = make_uint4(w[p][0], w[p][1], w[p][2], w[p][3]);
+          st_shared_v4(res + off + p * A_PART_BYTES, v);
+          if (ACT) *reinterpret_cast<uint4*>(ct + off + p * A_PART_BYTES) = v;
+        }
+      }
+    }
+  }
+  if (HEAD) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float e = e_acc[h];
+      e += __shfl_xor_sync(ANI_FULL_MASK, e, 1);
+      e += __shfl_xor_sync(ANI_FULL_MASK, e, 2);
+      if (q == 0) a.e_member[(size_t)m * a.rows_cap + rt * TM + r0 + 8 * h] = row_valid[h] ? e + sp.b4[m] : 0.f;
+    }
+  }
+}
+
+// ---- the kernel: one persistent CTA per SM, chains res_chain_id(0), res_chain_id(1), ... ----
+__global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_constant__ ResArgs F) {
+  extern __shared__ unsigned char smem_raw[];
+  // 1024-byte aligned (swizzle groups are 8 rows x 64 B): R, then the ring
+  unsigned char* res = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  unsigned char* ring = res + RES_BYTES;
+  __shared__ int s_first[ANI_MAX_SPECIES + 1];
+  __shared__ int s_blk[MAX_BLOCKS];
+  __shared__ __align__(8) uint64_t full[RES_SLOTS], empty[RES_SLOTS];
+  const int warp = __shfl_sync(ANI_FULL_MASK, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
+  const int nblk = F.blocks ? min(F.blocks[0], MAX_BLOCKS) : -1;
+  if (threadIdx.x <= F.num_species) s_first[threadIdx.x] = F.layout_info[4 + threadIdx.x];
+  if ((int)threadIdx.x < nblk) s_blk[threadIdx.x] = F.blocks[1 + threadIdx.x];
+  if (threadIdx.x == 32) {
+    for (int i = 0; i < RES_SLOTS; ++i) {
+      mbar_init(&full[i], 1);                     // the expect_tx arrival of the producer lane (+ the bytes)
+      mbar_init(&empty[i], NUM_CONSUMER_WARPS);   // one arrival per consumer warp
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  int s, rt, m;
+  if (warp < 4) {
+    setmaxnreg_dec<PROD_REGS>();
+    if (warp != PROD_WARP) return;
+    // ================================ producer (TMA) ================================
+    uint32_t u = 0;  // ring slots handed out so far: slot u % RES_SLOTS, use u / RES_SLOTS of that slot
+    for (int r = 0; res_chain(F, s_first, res_chain_id(r), s, rt, m); ++r) {
+      const ResSpecies& sp = F.sp[s];
+      for (int p = 0; p < RES_PHASES; ++p) {
+        int nkb, n;
+        res_phase(F, sp, p, nblk, nkb, n);
+        // K-blocks of the stored B operand; phase 5 (W1^T of all members) starts member m at K-block m * h1 / 32
+        const int nkb_all = p == 0 ? F.kbx : p == 5 ? F.members * sp.h1 / TK : nkb;
+        const int kb_boff = p == 5 ? m * sp.h1 / TK : 0;
+        const unsigned char* Bm = sp.B[p] + (p == 5 ? (size_t)0 : (size_t)m * n * nkb_all * (PARTS * ROW_BYTES));
+        // the stored activation the dCELU epilogue reads, on its way to L2 while the main loop runs
+        if (lane == 0 && (p == 3 || p == 4))
+          prefetch_l2(p == 4 ? F.act1 + ((size_t)rt * F.kb1 + (size_t)(m * sp.h1) / TK) * A_BLOCK_BYTES
+                             : F.act2 + ((size_t)rt * F.kb2 + (size_t)(m * sp.h2) / TK) * A_BLOCK_BYTES,
+                      (uint32_t)(n / TK) * A_BLOCK_BYTES);
+        // phase 5 without the compact operand: lane -> (live block, piece) of a gathered 2 KB copy
+        const bool gather = p == 5 && nblk >= 0 && !F.b_compact;
+        for (int n0 = 0; n0 < n; n0 += TN_MAX) {
+          const int bn = min(TN_MAX, n - n0);
+          // slots of one K-block: the x block (phase 0), then one per 128 rows of B
+          const int nh = (bn + RES_HALF - 1) / RES_HALF, a_sl = p == 0 ? 1 : 0;
+          const int gq = lane / PARTS, gpart = lane % PARTS;
+          const bool g_active = gather && lane < PARTS * (bn / 32);
+          size_t g_src = 0;
+          int g_bns = 0;
+          if (g_active) {
+            const int row0 = s_blk[n0 / 32 + gq] * 32, n0s = row0 / TN_MAX * TN_MAX;
+            g_bns = min(TN_MAX, F.ldx - n0s);
+            g_src = (size_t)n0s * nkb_all * (PARTS * ROW_BYTES) + (size_t)(row0 - n0s) * ROW_BYTES +
+                    (size_t)gpart * g_bns * ROW_BYTES;
+          }
+          for (int kb = 0; kb < nkb; ++kb) {
+            for (int j = 0; j < a_sl + nh; ++j)
+              mbar_wait(&empty[(u + j) % RES_SLOTS], (((u + j) / RES_SLOTS) & 1) ^ 1);
+            const int kbi = p == 0 && nblk >= 0 ? s_blk[kb] : kb;
+            const int kbb = kbi + kb_boff;
+            // B K-block in global memory: [p1 bn x 64 B | p2 bn x 64 B]
+            const unsigned char* bsrc = Bm + ((size_t)n0 * nkb_all + (size_t)kbb * bn) * (PARTS * ROW_BYTES);
+            if (lane == 0) {
+              if (p == 0) {
+                const int sl = u % RES_SLOTS;
+                mbar_arrive_expect_tx(&full[sl], A_BLOCK_BYTES);
+                bulk_g2s(ring + sl * RES_SLOT_BYTES, F.x + ((size_t)rt * F.kbx + kbi) * A_BLOCK_BYTES, A_BLOCK_BYTES,
+                         &full[sl]);
+              }
+              for (int h = 0; h < nh; ++h) {
+                const int sl = (u + a_sl + h) % RES_SLOTS;
+                const uint32_t rows = (uint32_t)min(RES_HALF, bn - h * RES_HALF);
+                mbar_arrive_expect_tx(&full[sl], PARTS * rows * ROW_BYTES);
+                if (!gather)
+#pragma unroll
+                  for (int pp = 0; pp < PARTS; ++pp)
+                    bulk_g2s(ring + sl * RES_SLOT_BYTES + pp * A_PART_BYTES,
+                             bsrc + ((size_t)pp * bn + h * RES_HALF) * ROW_BYTES, rows * ROW_BYTES, &full[sl]);
+              }
+            }
+            __syncwarp();
+            if (g_active)
+              bulk_g2s(ring + ((u + gq / 4) % RES_SLOTS) * RES_SLOT_BYTES + gpart * A_PART_BYTES +
+                           (gq % 4) * 32 * ROW_BYTES,
+                       Bm + g_src + (size_t)kbb * g_bns * (PARTS * ROW_BYTES), 32 * ROW_BYTES,
+                       &full[(u + gq / 4) % RES_SLOTS]);
+            __syncwarp();
+            u += a_sl + nh;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ================================ consumers ================================
+  setmaxnreg_inc<CONS_REGS>();
+  const int wg = (warp >> 2) - 1, warp_in_wg = warp & 3;
+  const uint32_t res_u32 = smem_u32(res), res_a = res_u32 + wg * (64 / 8) * GROUP_BYTES;  // this warpgroup's rows of R
+  uint32_t u = 0;    // ring slots consumed so far, in the producer's order
+  float omax = 0.f;  // largest |scaled value| this thread handed to the half-precision split
+  for (int r = 0; __shfl_sync(ANI_FULL_MASK, (int)res_chain(F, s_first, res_chain_id(r), s, rt, m), 0); ++r) {
+    const ResSpecies& sp = F.sp[s];
+#pragma unroll 1
+    for (int p = 0; p < RES_PHASES; ++p) {
+      int nkb_, n_;
+      res_phase(F, sp, p, nblk, nkb_, n_);
+      const int nkb = __shfl_sync(ANI_FULL_MASK, nkb_, 0), n = __shfl_sync(ANI_FULL_MASK, n_, 0);
+      for (int n0 = 0; n0 < n; n0 += TN_MAX) {
+        const int bn = min(TN_MAX, n - n0);
+        const int a_sl = p == 0 ? 1 : 0, nslot = a_sl + (bn + RES_HALF - 1) / RES_HALF;
+        // 64-column slices; a 32-column remainder is computed as a whole slice into columns nobody reads (rows of its
+        // slot that this K-block did not fill)
+        const int nsl = (bn + 63) / 64;
+        float acc[4][32];
+#pragma unroll
+        for (int cc = 0; cc < 4; ++cc)
+#pragma unroll
+          for (int i = 0; i < 32; ++i) acc[cc][i] = 0.f;
+        uint32_t prev = 0;
+        for (int kb = 0; kb < nkb; ++kb) {
+          for (int j = 0; j < nslot; ++j) mbar_wait(&full[(u + j) % RES_SLOTS], ((u + j) / RES_SLOTS) & 1);
+          const uint32_t sa = p == 0 ? smem_u32(ring + (u % RES_SLOTS) * RES_SLOT_BYTES) + wg * (64 / 8) * GROUP_BYTES
+                                     : res_a + kb * A_BLOCK_BYTES;
+          // B rows 0-127 and 128-255
+          const uint32_t sb0 = smem_u32(ring + ((u + a_sl) % RES_SLOTS) * RES_SLOT_BYTES);
+          const uint32_t sb1 = smem_u32(ring + ((u + a_sl + 1) % RES_SLOTS) * RES_SLOT_BYTES);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < TK / 16; ++k) {
+            const uint32_t adv = 32u * k;  // 16 pieces = 32 B along the swizzle row
+            uint64_t da[PARTS];
+#pragma unroll
+            for (int pp = 0; pp < PARTS; ++pp) da[pp] = make_desc(sa + pp * A_PART_BYTES + adv);
+#pragma unroll
+            for (int cc = 0; cc < 4; ++cc) {
+              if (cc >= nsl) break;
+              uint64_t db[PARTS];
+#pragma unroll
+              for (int pp = 0; pp < PARTS; ++pp)
+                db[pp] = make_desc((cc < 2 ? sb0 : sb1) + pp * A_PART_BYTES + (cc & 1) * (64 / 8) * GROUP_BYTES + adv);
+              // smallest terms first
+              wgmma_n64(acc[cc], da[1], db[0]);
+              wgmma_n64(acc[cc], da[0], db[1]);
+              wgmma_n64(acc[cc], da[0], db[0]);
+            }
+          }
+          wgmma_commit();
+          // the previous K-block's products have retired: its slots go back to the producer
+          wgmma_wait<1>();
+          if (kb > 0 && lane == 0)
+            for (int j = 0; j < nslot; ++j) mbar_arrive(&empty[(prev + j) % RES_SLOTS]);
+          prev = u;
+          u += nslot;
+        }
+        wgmma_wait<0>();
+        if (nkb > 0 && lane == 0)
+          for (int j = 0; j < nslot; ++j) mbar_arrive(&empty[(prev + j) % RES_SLOTS]);
+        // every warp of the warpgroup is done reading R before any of them overwrites it
+        if (p < 5) wg_bar(wg);
+        switch (p) {
+          case 0: res_epilogue<0>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 1: res_epilogue<1>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 2: res_epilogue<2>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 3: res_epilogue<3>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 4: res_epilogue<4>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          default: res_epilogue<5>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+        }
+        // this warpgroup's rows of the phase's output, visible to the next phase's wgmma
+        if (p < 5) {
+          fence_proxy_async_shared();
+          wg_bar(wg);
+        }
+      }
+    }
+  }
+  if (F.status && !(omax <= OPND_HALF_MAX)) atomicOr(F.status, ANI_STATUS_OPERAND_RANGE);
+}
+#endif  // ANI_OPND_FP16X2
+
+}  // namespace tc
+}  // namespace ani

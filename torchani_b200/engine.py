@@ -497,6 +497,13 @@ class Engine:
         # batch of 256), while below a wave (water 1 k) the chained launches are as fast and hand a row tile over
         # without an L2 counter.  "auto" applies that rule; ANI_B200_MLP_FUSED=0 / 1 forces one of them.
         self.mlp_mode = os.environ.get("ANI_B200_MLP_FUSED", "auto")
+        # Where "auto" picks the data-flow launch and gradients are wanted, one launch of resident chains
+        # (csrc/mlp_resident.cuh) replaces it: every intermediate of a (row tile, member) chain stays in shared
+        # memory.  It exists in the 2 x fp16 build for hidden widths up to 256 (ani_b200_mlp_step_resident).
+        m = nets.model
+        self._resident_ok = (_lib.operand_format(self.variant).parts == 2
+                             and max(m.h1_max, m.h2_max, m.h3_max) <= 256)
+        self.mlp_resident = False
         self._num_sms = torch.cuda.get_device_properties(self.device).multi_processor_count
         self._side_stream: tp.Optional[torch.cuda.Stream] = None
         self._ev: tp.List[torch.cuda.Event] = []
@@ -599,9 +606,14 @@ class Engine:
                     graph.replay()
         # kernels launched by this library in one step (memsets excluded):
         # prepare 1 (+1 grid kernel for open single systems), AEV fwd 1, GEMM fwd 3,
-        # (zero + GEMM bwd 3 + AEV bwd 1), reduce 1
-        mlp = ((self.lib.ani_b200_mlp_step_windows(C.byref(self.nets.model), ws.rows_cap) + (1 if want_grad else 0))
-               if self._use_dataflow_mlp(hi - lo) else (3 + (4 if want_grad else 0)))
+        # (zero + GEMM bwd 3 + AEV bwd 1), reduce 1; the fused MLP: zero + one launch (resident chains) or + one per
+        # window (data flow)
+        if self._use_resident_mlp(hi - lo, want_grad):
+            mlp = 2
+        elif self._use_dataflow_mlp(hi - lo):
+            mlp = self.lib.ani_b200_mlp_step_windows(C.byref(self.nets.model), ws.rows_cap) + (1 if want_grad else 0)
+        else:
+            mlp = 3 + (4 if want_grad else 0)
         self.launches_per_step = 1 + (0 if (pbc or n_conf > 1) else 1) + 1 + mlp + (1 if want_grad else 0) + 1
         grad = ws.grad.view(n_conf, n_per_conf, 3) if want_grad else None
         virial = ws.virial.sum(0).view(3, 3) if want_virial else None
@@ -667,8 +679,15 @@ class Engine:
                 ptr(ws.species_i32), n, lo, hi, n_conf, n_per_conf, ptr(self.sae), ptr(ws.atomic),
                 ptr(ws.member_atomic), ws.energies_ptr, stream_handle)
 
-        self.mlp_fused = self._use_dataflow_mlp(hi - lo)
-        if not split and self.mlp_fused:
+        self.mlp_resident = not split and self._use_resident_mlp(hi - lo, want_grad)
+        self.mlp_fused = self.mlp_resident or self._use_dataflow_mlp(hi - lo)
+        if self.mlp_resident:
+            # the six GEMMs of the step as ONE launch of resident (row tile, member) chains (csrc/mlp_resident.cuh)
+            self._timed("mlp_forward_backward", lambda: L.ani_b200_mlp_step_resident(
+                C.byref(self.nets.model), ptr(ws.x), ptr(ws.dx), ws.rows_cap, ptr(ws.row_atom),
+                ptr(ws.layout_info), ptr(ws.aev_blocks), ptr(ws.act1), ptr(ws.act2), ptr(ws.e_member),
+                ptr(ws.status), st))
+        elif not split and self.mlp_fused:
             # the six GEMMs of the step as ONE persistent data-flow launch (csrc/gemm_tc.cuh)
             self._timed("mlp_forward_backward", lambda: L.ani_b200_mlp_step(
                 C.byref(self.nets.model), ptr(ws.x), ptr(ws.dx), ws.rows_cap, ptr(ws.row_atom),
@@ -789,6 +808,11 @@ class Engine:
             return self.mlp_mode == "1"
         units = (-(-owned // TILE) + 1) * self.nets.num_members     # per layer: row tiles x members (>= 1 column tile)
         return units >= self._num_sms
+
+    def _use_resident_mlp(self, owned: int, want_grad: bool) -> bool:
+        """One launch of resident chains (ani_b200_mlp_step_resident) where "auto" would pick the data-flow launch
+        for a step with gradients, and the build and the model have the kernel; see __init__."""
+        return self.mlp_mode == "auto" and want_grad and self._resident_ok and self._use_dataflow_mlp(owned)
 
     def note_composition(self, ws: Workspace) -> None:
         """Before a graph capture (the shape has already run eagerly): read the element mask of the last
