@@ -16,10 +16,28 @@
 // R is 8 K-blocks (256 columns) in the tiled-operand layout of common.cuh, so the wgmma descriptors of gemm_tc.cuh read
 // it unchanged.  Consumer warpgroup w reads and writes only rows 64w .. 64w+63 of R: a phase's output goes into R after
 // the warpgroup's last wgmma of that phase has retired, and a warpgroup barrier after fence.proxy.async makes it
-// visible to the next phase's wgmma.  The dCELU loads of phases 3 and 4 read back what the same thread stored in phases
-// 1 and 0 (tile_epilogue's thread -> (row, chunk) map is the same in every phase).  The only inputs are x (an earlier
-// launch) and the weights, so nothing waits on another CTA: the producer streams B (and x in phase 0) ahead across
-// phase and chain boundaries, limited only by the free ring slots.
+// visible to the next phase's wgmma.  The only inputs are x (an earlier launch) and the weights, so nothing waits on
+// another CTA: the producer streams B (and x in phase 0) ahead across phase and chain boundaries, limited only by the
+// free ring slots.
+//
+// Main loop: one wgmma per K-step, product and B slot, as wide as the slot's rows (m64n128k16, or n32 / n64 / n96 for
+// the remainder of the phase's columns), so A is read from shared memory once per 128 columns and no MMA runs on
+// padding.  The products keep the order a2b1, a1b2, a1b1, so every output element sees the same sums as with 64-column
+// slices.  Epilogue stores into R: stmatrix.x4 per (32-column group, row half, piece), matrix j = chunk j of the
+// group, each lane addressing one swizzled 16-byte row.
+//
+// act1 / act2 (read back for CELU' by phases 4 / 3) leave R by bulk copy.  Once the threads of a warpgroup have stored
+// their rows of phase 0 / 1, run fence.proxy.async.shared::cta and met at the warpgroup barrier, one of them (the
+// copier) issues cp.async.bulk.global.shared::cta for the warpgroup's 4 KB of every K-block and piece.  The fence
+// and the barrier order every thread's generic stores into R before the copier's async-proxy reads of R, as for wgmma.
+// The copier waits with cp.async.bulk.wait_group.read 0 before the barrier in front of the next epilogue (phases 1, 2),
+// so R is not overwritten while a copy still reads it.  Before the barrier in front of phase 3's epilogue it waits with
+// cp.async.bulk.wait_group 0: the copies of a1 and a2 are complete, and completion makes their writes visible to the
+// copier.  bar.sync then orders them before every later memory access of the warpgroup's other threads (the barrier
+// is a CTA-scope synchronisation in the PTX memory model, and causality order is transitive), so phases 3 and 4 read
+// the finished values.  They load with ld.global.cg: nothing of these lines was cached in this SM's L1 earlier in the
+// launch, and .cg leaves no room for a stale line either way.  Every copy of a chain is complete by its phase 3, so
+// none is in flight when the next chain's phase 0 overwrites R or when the CTA exits.
 //
 // Shared memory: R 128 KB + a ring of six 16 KB slots + 1 KB alignment = 230,400 B.  A K-block takes one slot for
 // the x block of phase 0 and one per 128 rows of B.
@@ -73,9 +91,71 @@ struct ResArgs {
 
 #if ANI_OPND_FP16X2
 __device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// 16-byte store into R by its shared-window address (a generic store would take the global-memory path)
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+// Four 8 x 8 matrices of 16-bit values into R: register j of lane l is row l / 4, columns 2 (l % 4) and 2 (l % 4) + 1
+// of matrix j (the layout of an 8-column chunk of the wgmma accumulator), and lanes 8j .. 8j + 7 give the shared-window
+// addresses of the eight 16-byte rows of matrix j.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+// bulk copy shared -> global, tracked by this thread's bulk async-groups
+__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// this thread's bulk copies have finished reading their shared-memory source
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// this thread's bulk copies are complete: their writes are visible to this thread
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// D[64 x N] += A[64 x 16] * B[N x 16]^T for the N = 32, 64, 96 or 128 B rows of one ring slot (fp32 accumulate, both
+// operands from shared memory).  The fragment is that of m64n64 products side by side: columns 0-63 in d0 (N = 32: its
+// first 16 registers), columns 64-127 in d1.
+#define ANI_RES_REGS16 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+#define ANI_RES_REGS32 ANI_RES_REGS16 ", %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define ANI_RES_REGS48 ANI_RES_REGS32 ", %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+#define ANI_RES_REGS64 ANI_RES_REGS48 ", %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define ANI_RES_F8(d, i) \
+  "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define ANI_RES_F16(d, i) ANI_RES_F8(d, i), ANI_RES_F8(d, i + 8)
+#define ANI_RES_F32(d) ANI_RES_F16(d, 0), ANI_RES_F16(d, 16)
+#define ANI_RES_WGMMA(N, REGS, DESCS, ...)                                                                   \
+  __device__ __forceinline__ void wgmma_res_n##N(float (&d0)[32], float (&d1)[32], uint64_t da, uint64_t db) { \
+    (void)d1;                                                                                                \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"                                            \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." ANI_WGMMA_AB " {" REGS "}, " DESCS        \
+                 ", p, 1, 1, 0, 0;\n\t}"                                                                     \
+                 : __VA_ARGS__                                                                               \
+                 : "l"(da), "l"(db));                                                                        \
+  }
+ANI_RES_WGMMA(32, ANI_RES_REGS16, "%16, %17", ANI_RES_F16(d0, 0))
+ANI_RES_WGMMA(64, ANI_RES_REGS32, "%32, %33", ANI_RES_F32(d0))
+ANI_RES_WGMMA(96, ANI_RES_REGS48, "%48, %49", ANI_RES_F32(d0), ANI_RES_F16(d1, 0))
+ANI_RES_WGMMA(128, ANI_RES_REGS64, "%64, %65", ANI_RES_F32(d0), ANI_RES_F32(d1))
+#undef ANI_RES_WGMMA
+#undef ANI_RES_F32
+#undef ANI_RES_F16
+#undef ANI_RES_F8
+#undef ANI_RES_REGS64
+#undef ANI_RES_REGS48
+#undef ANI_RES_REGS32
+#undef ANI_RES_REGS16
+
+// The three products of the 2 x fp16 split for one K-step and one ring slot of N = w columns (smallest terms first)
+__device__ __forceinline__ void res_mma_slot(float (&d0)[32], float (&d1)[32], const uint64_t (&da)[PARTS],
+                                             const uint64_t (&db)[PARTS], int w) {
+  switch (w) {
+#define ANI_RES_MMA3(N)                    \
+  case N:                                  \
+    wgmma_res_n##N(d0, d1, da[1], db[0]); \
+    wgmma_res_n##N(d0, d1, da[0], db[1]); \
+    wgmma_res_n##N(d0, d1, da[0], db[0]); \
+    break;
+    ANI_RES_MMA3(32) ANI_RES_MMA3(64) ANI_RES_MMA3(96)
+    default: ANI_RES_MMA3(128)
+#undef ANI_RES_MMA3
+  }
 }
 
 // chain c of the list: species in `order`, then row tile, then member.  false: past the end
@@ -125,10 +205,10 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
   const int r0 = 64 * wg + 16 * warp_in_wg + (lane >> 2);  // rows r0 and r0 + 8 of the tile
   const float acc_scale = sp.acc_scale[P];
   const float out_scale = ACT ? OPND_SCALE_VALUE : OPND_SCALE_GRAD;
-  // the global copy of a1 / a2: written by phases 0 / 1, read back for CELU' by phases 4 / 3
-  unsigned char* ct = nullptr;
-  if (P == 0 || P == 4) ct = a.act1 + ((size_t)rt * a.kb1 + (size_t)(m * sp.h1) / TK) * A_BLOCK_BYTES;
-  if (P == 1 || P == 3) ct = a.act2 + ((size_t)rt * a.kb2 + (size_t)(m * sp.h2) / TK) * A_BLOCK_BYTES;
+  // the global copy of a1 / a2 that phases 4 / 3 read back for CELU' (bulk-copied from R after phases 0 / 1)
+  const unsigned char* ct = nullptr;
+  if (P == 4) ct = a.act1 + ((size_t)rt * a.kb1 + (size_t)(m * sp.h1) / TK) * A_BLOCK_BYTES;
+  if (P == 3) ct = a.act2 + ((size_t)rt * a.kb2 + (size_t)(m * sp.h2) / TK) * A_BLOCK_BYTES;
   const float* bias = P <= 2 ? sp.bias[P] + (size_t)m * (P == 0 ? sp.h1 : P == 1 ? sp.h2 : sp.h3) : nullptr;
   const float* w4 = HEAD ? sp.w4 + (size_t)m * sp.h3 : nullptr;
   float e_acc[2] = {0.f, 0.f}, seed[2] = {0.f, 0.f};
@@ -141,12 +221,22 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
     }
   }
   const int ngroups = bn / 32;
-  // dCELU: the stored activation of the next (32-column group, row half) is loaded before the current one is computed
-  uint4 ybuf[2][PARTS];
-  auto load_y = [&](int g, int h, uint4 (&dst)[PARTS]) {
-    const unsigned char* b = ct + (size_t)g * A_BLOCK_BYTES + swz_off(r0 + 8 * h, q);
+  // stmatrix: lane l gives the address of row 8h + (l & 7) of this warp's 16 rows, chunk l >> 3 (piece 0, group 0)
+  uint32_t st_off[2];
 #pragma unroll
-    for (int p = 0; p < PARTS; ++p) dst[p] = *reinterpret_cast<const uint4*>(b + p * A_PART_BYTES);
+  for (int h = 0; h < 2; ++h) st_off[h] = res + swz_off(64 * wg + 16 * warp_in_wg + 8 * h + (lane & 7), lane >> 3);
+  // dCELU: the stored activation of the next (32-column group, row half) is loaded before the current one is computed.
+  // The thread loads the words of its own fragment, word q of chunk j of its row: columns 8j + 2q and 8j + 2q + 1.
+  // L2 only (.cg): the words were written there by the bulk copy, never through this SM's L1.
+  uint32_t ybuf[2][PARTS][4];
+  auto load_y = [&](int g, int h, uint32_t (&dst)[PARTS][4]) {
+    const int row = r0 + 8 * h;
+    const unsigned char* b = ct + (size_t)g * A_BLOCK_BYTES + 4 * q;
+#pragma unroll
+    for (int p = 0; p < PARTS; ++p)
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        dst[p][j] = __ldcg(reinterpret_cast<const unsigned int*>(b + p * A_PART_BYTES + swz_off(row, j)));
   };
   if (DCELU) load_y(0, 0, ybuf[0]);
   // One loop iteration per 32-column group, NOT unrolled: the body is compiled once per phase instead of eight times.
@@ -175,15 +265,6 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
         else if (g + 1 < ngroups)
           load_y(g + 1, 0, ybuf[0]);
       }
-      uint32_t yw[PARTS][4];
-      if (DCELU) {
-#pragma unroll
-        for (int p = 0; p < PARTS; ++p) {
-          const uint4 v = ybuf[h][p];
-          yw[p][0] = v.x, yw[p][1] = v.y, yw[p][2] = v.z, yw[p][3] = v.w;
-          quad_transpose(yw[p], lane);
-        }
-      }
       uint32_t w[PARTS][4];
       float o[4][2];
 #pragma unroll
@@ -195,7 +276,7 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
         if (DCELU) {
           uint32_t pw[PARTS];
 #pragma unroll
-          for (int p = 0; p < PARTS; ++p) pw[p] = yw[p][j];
+          for (int p = 0; p < PARTS; ++p) pw[p] = ybuf[h][p][j];
           y2 = join_pair(pw);
         }
 #pragma unroll
@@ -237,14 +318,9 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
             *reinterpret_cast<float2*>(dst) = make_float2(o[j][0], o[j][1]);
         }
       } else {
-        const uint32_t off = (uint32_t)g * A_BLOCK_BYTES + swz_off(row, q);
+        // matrix j of the stmatrix is chunk j of the group: whole 16-byte rows, swizzled by the lane addresses
 #pragma unroll
-        for (int p = 0; p < PARTS; ++p) {
-          quad_transpose(w[p], lane);
-          const uint4 v = make_uint4(w[p][0], w[p][1], w[p][2], w[p][3]);
-          st_shared_v4(res + off + p * A_PART_BYTES, v);
-          if (ACT) *reinterpret_cast<uint4*>(ct + off + p * A_PART_BYTES) = v;
-        }
+        for (int p = 0; p < PARTS; ++p) stmatrix_x4(st_off[h] + (uint32_t)g * A_BLOCK_BYTES + p * A_PART_BYTES, w[p]);
       }
     }
   }
@@ -295,11 +371,6 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
         const int nkb_all = p == 0 ? F.kbx : p == 5 ? F.members * sp.h1 / TK : nkb;
         const int kb_boff = p == 5 ? m * sp.h1 / TK : 0;
         const unsigned char* Bm = sp.B[p] + (p == 5 ? (size_t)0 : (size_t)m * n * nkb_all * (PARTS * ROW_BYTES));
-        // the stored activation the dCELU epilogue reads, on its way to L2 while the main loop runs
-        if (lane == 0 && (p == 3 || p == 4))
-          prefetch_l2(p == 4 ? F.act1 + ((size_t)rt * F.kb1 + (size_t)(m * sp.h1) / TK) * A_BLOCK_BYTES
-                             : F.act2 + ((size_t)rt * F.kb2 + (size_t)(m * sp.h2) / TK) * A_BLOCK_BYTES,
-                      (uint32_t)(n / TK) * A_BLOCK_BYTES);
         // phase 5 without the compact operand: lane -> (live block, piece) of a gathered 2 KB copy
         const bool gather = p == 5 && nblk >= 0 && !F.b_compact;
         for (int n0 = 0; n0 < n; n0 += TN_MAX) {
@@ -360,6 +431,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
   setmaxnreg_inc<CONS_REGS>();
   const int wg = (warp >> 2) - 1, warp_in_wg = warp & 3;
   const uint32_t res_u32 = smem_u32(res), res_a = res_u32 + wg * (64 / 8) * GROUP_BYTES;  // this warpgroup's rows of R
+  const bool copier = warp_in_wg == 0 && lane == 0;  // issues and waits for the warpgroup's bulk copies of a1 / a2
   uint32_t u = 0;    // ring slots consumed so far, in the producer's order
   float omax = 0.f;  // largest |scaled value| this thread handed to the half-precision split
   for (int r = 0; __shfl_sync(ANI_FULL_MASK, (int)res_chain(F, s_first, res_chain_id(r), s, rt, m), 0); ++r) {
@@ -372,9 +444,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
       for (int n0 = 0; n0 < n; n0 += TN_MAX) {
         const int bn = min(TN_MAX, n - n0);
         const int a_sl = p == 0 ? 1 : 0, nslot = a_sl + (bn + RES_HALF - 1) / RES_HALF;
-        // 64-column slices; a 32-column remainder is computed as a whole slice into columns nobody reads (rows of its
-        // slot that this K-block did not fill)
-        const int nsl = (bn + 63) / 64;
+        // one wgmma per B slot and product, as wide as the slot's rows: 128, or the 32-128 columns of the remainder
+        const int w0 = min(bn, RES_HALF), w1 = bn - w0;
         float acc[4][32];
 #pragma unroll
         for (int cc = 0; cc < 4; ++cc)
@@ -395,17 +466,14 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
             uint64_t da[PARTS];
 #pragma unroll
             for (int pp = 0; pp < PARTS; ++pp) da[pp] = make_desc(sa + pp * A_PART_BYTES + adv);
+            uint64_t db[PARTS];
 #pragma unroll
-            for (int cc = 0; cc < 4; ++cc) {
-              if (cc >= nsl) break;
-              uint64_t db[PARTS];
+            for (int pp = 0; pp < PARTS; ++pp) db[pp] = make_desc(sb0 + pp * A_PART_BYTES + adv);
+            res_mma_slot(acc[0], acc[1], da, db, w0);
+            if (w1 > 0) {
 #pragma unroll
-              for (int pp = 0; pp < PARTS; ++pp)
-                db[pp] = make_desc((cc < 2 ? sb0 : sb1) + pp * A_PART_BYTES + (cc & 1) * (64 / 8) * GROUP_BYTES + adv);
-              // smallest terms first
-              wgmma_n64(acc[cc], da[1], db[0]);
-              wgmma_n64(acc[cc], da[0], db[1]);
-              wgmma_n64(acc[cc], da[0], db[0]);
+              for (int pp = 0; pp < PARTS; ++pp) db[pp] = make_desc(sb1 + pp * A_PART_BYTES + adv);
+              res_mma_slot(acc[2], acc[3], da, db, w1);
             }
           }
           wgmma_commit();
@@ -419,6 +487,10 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
         wgmma_wait<0>();
         if (nkb > 0 && lane == 0)
           for (int j = 0; j < nslot; ++j) mbar_arrive(&empty[(prev + j) % RES_SLOTS]);
+        // the copies of a1 / a2 have read R before the epilogues of phases 1 / 2 overwrite it, and have landed in
+        // global memory before phase 3 reads act2 back (phase 4 reads act1, copied earlier)
+        if (copier && (p == 1 || p == 2)) bulk_wait_read();
+        if (copier && p == 3) bulk_wait();
         // every warp of the warpgroup is done reading R before any of them overwrites it
         if (p < 5) wg_bar(wg);
         switch (p) {
@@ -433,6 +505,20 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
         if (p < 5) {
           fence_proxy_async_shared();
           wg_bar(wg);
+        }
+        // a1 / a2 to act1 / act2 for the dCELU epilogues: this warpgroup's 64 rows of each K-block and piece are 4 KB,
+        // contiguous in R and in the tiled global operand
+        if (copier && p <= 1) {
+          unsigned char* ct = p == 0 ? F.act1 + ((size_t)rt * F.kb1 + (size_t)(m * sp.h1) / TK) * A_BLOCK_BYTES
+                                     : F.act2 + ((size_t)rt * F.kb2 + (size_t)(m * sp.h2) / TK) * A_BLOCK_BYTES;
+          const uint32_t off = wg * (64 / 8) * GROUP_BYTES;
+          for (int g = 0; g < bn / TK; ++g)
+#pragma unroll
+            for (int pp = 0; pp < PARTS; ++pp) {
+              const uint32_t o = g * A_BLOCK_BYTES + pp * A_PART_BYTES + off;
+              bulk_s2g(ct + o, res_u32 + o, (64 / 8) * GROUP_BYTES);
+            }
+          bulk_commit();
         }
       }
     }
