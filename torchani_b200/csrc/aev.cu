@@ -1537,7 +1537,11 @@ static int launch_aev_backward(const ani_aev_params* params, const ani_grid* gri
   // elements when the caller knows the composition (more elements at run time still work: those
   // pairs are read from global memory)
   const int E = (max_elements > 0 && max_elements < S) ? max_elements : S;
-  const int pair_cap = species_mask ? E * (E + 1) / 2 : NP;
+  // pair_sums reads the pairs beyond the table as float4 runs of the upstream row, which needs the angular block
+  // 16-byte aligned in every row: RL + ang_pad and ldx multiples of 4 (not so for, e.g., 7 elements x 15 shifts
+  // without ang_pad).  Otherwise the table holds every pair and global memory is never read there.
+  const bool ang_aligned = (RL + params->ang_pad) % 4 == 0 && ldx % 4 == 0 && ((uintptr_t)grad_aev & 15) == 0;
+  const int pair_cap = (species_mask && ang_aligned) ? E * (E + 1) / 2 : NP;
   const size_t wb = warp_smem_bytes(nbr_cap, ((RL + 3) & ~3) + 36 * pair_cap, true);
   const size_t smem = wb * AEV_WARPS;
   const int blocks = (hi - lo + AEV_WARPS - 1) / AEV_WARPS;
