@@ -252,8 +252,9 @@ int ani_b200_verlet_positions(int mode, const float* coords, const ani_grid* gri
 /*     conformer energies) so that no separate memset launches are needed.                          */
 /*     bucket_species (or NULL): i32[max_bins][8], per bucket the offset of its first atom of species >= s */
 /*     (buckets are species-sorted), consumed by ani_b200_aev_forward.                               */
-/*     scratch_i32: 3 n + max_bins + 4 + (ceil((hi-lo)/256) + 2) * ANI_MAX_SPECIES + 32 ints, ZERO at           */
-/*     allocation (two of them are the state of the device-wide barrier of the single-launch preparation).     */
+/*     scratch_i32: 3 n + max_bins + 4 + (max(1, ceil((hi-lo)/256)) + 2) * ANI_MAX_SPECIES + 32 ints (an empty     */
+/*     slice still takes one layout chunk), ZERO at allocation (two of them are the state of the device-wide      */
+/*     barrier of the single-launch preparation).                                                               */
 int ani_b200_prepare_step(const float* coords, const int32_t* species, int n_conf, int n_per_conf,
                           const float* cell, int pbc, int mode, float cutoff, int max_bins, ani_grid* grid,
                           int32_t* bin_start, int32_t* sorted_orig, int32_t* orig_to_sorted, float* spos,

@@ -1077,7 +1077,7 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
 //     atom walking its bucket through global memory (a chain of 2 x bucket-size dependent loads);
 //   * every CTA scans the chunk histograms itself (shared memory), so the row assignment follows
 //     without another barrier; CTA 0 writes the layout words, the tile table and the live AEV blocks.
-// Outputs are bit-identical to k_prep_fused (tests/test_gpu_api.py::test_prepare_cluster_matches_fused).
+// Outputs are bit-identical to k_prep_fused (tests/test_gpu_prepare.py::test_preparation_forms).
 // Used for periodic single systems up to PREP_CLUSTER_MAX_ATOMS atoms and PREP_CLUSTER_MAX_BINS buckets;
 // larger problems have enough work per phase for the whole device and keep the persistent-grid kernel.
 // ---------------------------------------------------------------------------------------
@@ -1611,7 +1611,7 @@ extern "C" int ani_b200_prepare_step(const float* coords, const int32_t* species
   A.zero_f64 = zero_f64_count > 0 ? zero_f64 : nullptr; A.zero_f64_count = zero_f64_count;
   A.status = status;
   A.bss = bucket_species;
-  {  // timing experiments: 16 words behind species_base (the scratch area has 64 spare ints)
+  {  // timing experiments: 12 int64 stamps behind species_base, inside the 32 spare ints of the documented scratch
     const char* te = getenv("ANI_B200_PREP_TRACE");
     A.trace = (te && atoi(te) != 0)
                   ? reinterpret_cast<unsigned long long*>((reinterpret_cast<uintptr_t>(A.species_base + ANI_MAX_SPECIES) + 7) & ~(uintptr_t)7)
