@@ -86,10 +86,11 @@ typedef struct ani_grid {
   float cell[9];   /* rows are lattice vectors (identity-like bounding box without PBC)  */
   float inv[9];    /* inverse: frac = (r - origin) @ inv                                  */
   float origin[3];
-  int32_t dims[3]; /* buckets per lattice direction                                       */
+  int32_t dims[3]; /* buckets per lattice direction (of one conformer's sub-grid, mode 2)  */
   int32_t pbc;     /* 1 = periodic in all three directions                                */
-  int32_t nbins;   /* real buckets; padding atoms live in bucket index nbins              */
-  int32_t mode;    /* 0 = one conformer on a grid, 1 = batch, bucket == conformer         */
+  int32_t nbins;   /* real buckets (all conformers); padding atoms live in bucket nbins   */
+  int32_t mode;    /* 0 = one conformer on a grid, 1 = batch, bucket == conformer,        */
+                   /* 2 = periodic batch: one sub-grid of the shared cell per conformer   */
   int32_t n_per_conf;
   int32_t n_real;  /* number of non-padding atoms (== bin_start[nbins])                  */
 } ani_grid;
@@ -111,6 +112,13 @@ const char* ani_b200_last_cuda_error(void);
 /*    coords  [n_conf*n_per_conf*3] f32, species [n_conf*n_per_conf] i32 (-1 = padding)    */
 /*    cell    device f32[9] (rows = lattice vectors) or NULL; pbc 0/1 (all directions)      */
 /*    mode 0 requires n_conf == 1; mode 1 requires pbc == 0.                                */
+/*    mode 2 (C conformers in one shared periodic cell) requires pbc == 1, a cell and        */
+/*    n_conf + 1 <= max_bins, else ANI_ERR_UNSUPPORTED (before any CUDA call).  Buckets are   */
+/*    conformer-major: bucket c * nb + local, nb = dims[0]*dims[1]*dims[2], nbins = C * nb;   */
+/*    dims come from the cell as in mode 0, capped so that nb <= (max_bins - 1) / n_conf, and  */
+/*    neighbour ranges never leave a conformer's sub-grid.  With max_bins = C * (max(64, A+2) */
+/*    - 1) + 1 a conformer's sub-grid, wrapped positions and in-bucket order are those of a   */
+/*    mode 0 call on that conformer alone (the engine sizes its workspaces so).               */
 /*    Outputs (all device):                                                                 */
 /*      grid            ani_grid                                                            */
 /*      bin_start       i32[max_bins+2]  exclusive scan of bucket populations               */
@@ -121,7 +129,7 @@ const char* ani_b200_last_cuda_error(void);
 /*    Scratch: scratch_i32[3*n + max_bins + 2].                                             */
 /*      bucket_ranges   f32[(max_bins-1)*27*8] or NULL: for every bucket the 27 neighbouring  */
 /*                      buckets as {first atom, end atom, image code, -} + image shift vector   */
-/*                      (mode 0 only; lets the AEV kernel skip the index / shift arithmetic)     */
+/*                      (modes 0 and 2; lets the AEV kernel skip the index / shift arithmetic)   */
 int ani_b200_build_cells(const float* coords, const int32_t* species, int n_conf, int n_per_conf,
                          const float* cell, int pbc, int mode, float cutoff, int max_bins,
                          ani_grid* grid, int32_t* bin_start, int32_t* sorted_orig,
@@ -183,7 +191,8 @@ int ani_b200_aev_forward(const ani_aev_params* params, const ani_grid* grid,
 /*    occupancy for few-element systems) -- pairs beyond it are read from global memory, the   */
 /*    result never depends on it.  virial (or NULL): f64[ANI_VIRIAL_SLOTS][9], zeroed by the     */
 /*    caller; the kernel adds partial sums of W_ab = sum_pairs (dE/dDelta)_a Delta_b, the "f dot r" */
-/*    virial of ase.py:164-168 (stress = sum over the slots / volume), row-major a, b.             */
+/*    virial of ase.py:164-168 (stress = sum over the slots / volume), row-major a, b.  Grid mode  */
+/*    2: f64[n_conf][ANI_VIRIAL_SLOTS][9], the pairs of a central atom go to its conformer's slots. */
 int ani_b200_aev_backward(const ani_aev_params* params, const ani_grid* grid, const float* spos,
                           const int32_t* sorted_orig, const int32_t* species_mask, int n, int lo,
                           int hi, const int32_t* row_of, const float* grad_aev, int ldx,
@@ -251,7 +260,9 @@ int ani_b200_verlet_positions(int mode, const float* coords, const ani_grid* gri
 /*     Also zero-fills zero_f32[0..count) (the force accumulator) and zero_f64[0..count) (the      */
 /*     conformer energies) so that no separate memset launches are needed.                          */
 /*     bucket_species (or NULL): i32[max_bins][8], per bucket the offset of its first atom of species >= s */
-/*     (buckets are species-sorted), consumed by ani_b200_aev_forward.                               */
+/*     (buckets are species-sorted), consumed by ani_b200_aev_forward.  bucket_ranges and bucket_species  */
+/*     are filled in grid modes 0 and 2 (ignored in mode 1).  Mode 2 runs the persistent-grid or the  */
+/*     five-launch form (the thread-block-cluster form is mode 0 only); same outputs.               */
 /*     scratch_i32: 3 n + max_bins + 4 + (max(1, ceil((hi-lo)/256)) + 2) * ANI_MAX_SPECIES + 32 ints (an empty     */
 /*     slice still takes one layout chunk), ZERO at allocation (two of them are the state of the device-wide      */
 /*     barrier of the single-launch preparation).                                                               */

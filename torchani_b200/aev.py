@@ -336,8 +336,6 @@ class AEVComputer(torch.nn.Module):
         assert elem_idxs.dim() == 2
         assert coords.shape == (elem_idxs.shape[0], elem_idxs.shape[1], 3)
         _validate_inputs(self.radial.cutoff, elem_idxs, coords, cell, pbc)
-        if pbc is not None and elem_idxs.shape[0] > 1:   # periodic batch: one conformer at a time
-            return torch.cat([self(elem_idxs[c:c + 1], coords[c:c + 1], cell, pbc) for c in range(elem_idxs.shape[0])])
         sup = None if isinstance(self.neighborlist, CellList) else \
             supercell_for_thin_cell(elem_idxs, coords, cell, pbc, self.radial.cutoff)
         if sup is not None:   # periodic cell thinner than the cutoff: AEVs of the original atoms of a supercell

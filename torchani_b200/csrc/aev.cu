@@ -68,9 +68,9 @@ struct ExplicitNbrs {
   const float4* d;
 };
 
-// bucket range + image code for offset (ox, oy, oz) around bucket (ix, iy, iz); false if it
-// does not exist (non-periodic boundary)
-__device__ __forceinline__ bool neighbour_bucket(const ani_grid& g, const int32_t* __restrict__ bin_start,
+// bucket range + image code for offset (ox, oy, oz) around bucket (ix, iy, iz) of the sub-grid that starts at
+// bucket `base` (bucket_coords); false if it does not exist (non-periodic boundary)
+__device__ __forceinline__ bool neighbour_bucket(const ani_grid& g, const int32_t* __restrict__ bin_start, int base,
                                                  int ix, int iy, int iz, int ox, int oy, int oz,
                                                  NeighbourRange& r) {
   int j[3] = {ix + ox, iy + oy, iz + oz};
@@ -87,7 +87,7 @@ __device__ __forceinline__ bool neighbour_bucket(const ani_grid& g, const int32_
     }
   }
   if (!g.pbc && (w[0] | w[1] | w[2])) return false;
-  int b = (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2];
+  int b = base + (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2];
   r.lo = bin_start[b];
   r.hi = bin_start[b + 1];
   r.code = (w[0] + 1) * 9 + (w[1] + 1) * 3 + (w[2] + 1);
@@ -397,7 +397,7 @@ __global__ void __launch_bounds__(AEV_WARPS * 32)
         s.nj[n] = j | (13 << ANI_IMG_SHIFT);
         s.nsp[n] = (unsigned char)__float_as_int(spos[j].w);
       }
-    } else if (g.mode != 0) {
+    } else if (g.mode == 1) {   // bucket == conformer
       scan_range(bin_start[b], bin_start[b + 1], 13, 0.f, 0.f, 0.f);
     } else if (ranges) {
       // precomputed table: lane o holds the record of neighbouring bucket o
@@ -415,12 +415,13 @@ __global__ void __launch_bounds__(AEV_WARPS * 32)
                    __shfl_sync(ANI_FULL_MASK, r1.z, o));
       }
     } else {
-      const int iz = b % g.dims[2], iy = (b / g.dims[2]) % g.dims[1], ix = b / (g.dims[2] * g.dims[1]);
+      int ix, iy, iz;
+      const int base = bucket_coords(g, b, ix, iy, iz);
       for (int ox = -1; ox <= 1; ++ox)
         for (int oy = -1; oy <= 1; ++oy)
           for (int oz = -1; oz <= 1; ++oz) {
             NeighbourRange r;
-            if (!neighbour_bucket(g, bin_start, ix, iy, iz, ox, oy, oz, r)) continue;
+            if (!neighbour_bucket(g, bin_start, base, ix, iy, iz, ox, oy, oz, r)) continue;
             const float3 sh = (r.code == 13) ? make_float3(0.f, 0.f, 0.f) : image_shift(g, r.code);
             scan_range(r.lo, r.hi, r.code, sh.x, sh.y, sh.z);
           }
@@ -627,7 +628,7 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
     if (tid < NRANGE) {
       int rlo = 0, rhi = 0, code = 13, nbk = cur;
       float4 sh = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (g.mode != 0) {
+      if (g.mode == 1) {   // bucket == conformer
         if (tid == 13) {
           rlo = bin_start[cur];
           rhi = bin_start[cur + 1];
@@ -641,9 +642,10 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
         nbk = __float_as_int(r0.w);
         sh = r1;
       } else {
-        const int iz = cur % g.dims[2], iy = (cur / g.dims[2]) % g.dims[1], ix = cur / (g.dims[2] * g.dims[1]);
+        int ix, iy, iz;
+        const int base = bucket_coords(g, cur, ix, iy, iz);
         NeighbourRange r;
-        if (neighbour_bucket(g, bin_start, ix, iy, iz, tid / 9 - 1, (tid / 3) % 3 - 1, tid % 3 - 1, r)) {
+        if (neighbour_bucket(g, bin_start, base, ix, iy, iz, tid / 9 - 1, (tid / 3) % 3 - 1, tid % 3 - 1, r)) {
           rlo = r.lo;
           rhi = r.hi;
           code = r.code;
@@ -1308,10 +1310,13 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
     }
   }
   if (VIRIAL && virial) {
+    // a periodic batch (mode 2) keeps one set of slots per conformer: the conformer of the central atom
+    const int conf = g.mode == 2 ? sorted_orig[i] / g.n_per_conf : 0;
+    double* slots = virial + (size_t)conf * ANI_VIRIAL_SLOTS * 9;
 #pragma unroll
     for (int k = 0; k < 9; ++k) {
       const float v = warp_sum(vir[k]);
-      if (lane == 0) atomicAdd(&virial[(blockIdx.x % ANI_VIRIAL_SLOTS) * 9 + k], (double)v);
+      if (lane == 0) atomicAdd(&slots[(blockIdx.x % ANI_VIRIAL_SLOTS) * 9 + k], (double)v);
     }
   }
   sx = warp_sum(sx);
@@ -1346,19 +1351,17 @@ __global__ void k_half_list(const ani_grid* __restrict__ grid, const int32_t* __
     const float c2 = cutoff * cutoff;
     long long out = FILL ? (long long)pair_start[i] : 0;
     const int b = sbin[i];
-    int ix = 0, iy = 0, iz = 0, span = 0;
-    if (g.mode == 0) {
-      iz = b % g.dims[2];
-      iy = (b / g.dims[2]) % g.dims[1];
-      ix = b / (g.dims[2] * g.dims[1]);
+    int ix = 0, iy = 0, iz = 0, span = 0, base = 0;
+    if (g.mode != 1) {
+      base = bucket_coords(g, b, ix, iy, iz);
       span = 1;
     }
     for (int ox = -span; ox <= span; ++ox)
       for (int oy = -span; oy <= span; ++oy)
         for (int oz = -span; oz <= span; ++oz) {
           NeighbourRange r;
-          if (g.mode == 0) {
-            if (!neighbour_bucket(g, bin_start, ix, iy, iz, ox, oy, oz, r)) continue;
+          if (g.mode != 1) {
+            if (!neighbour_bucket(g, bin_start, base, ix, iy, iz, ox, oy, oz, r)) continue;
           } else {
             r.lo = bin_start[b];
             r.hi = bin_start[b + 1];

@@ -10,6 +10,9 @@ namespace ani {
 // The grid of one call (executed by one thread).  mode 0 + pbc: buckets from the perpendicular
 // widths of the cell (>= 1 bucket per cutoff, neighbors.py:618-662 uses edge lengths; widths are
 // the safe choice for triclinic cells).  mode 0 without pbc: bounding box of the real atoms.
+// mode 2 (a periodic batch in one shared cell): every conformer gets the sub-grid a single system in
+// that cell would get from a 1 / n_conf share of the bucket capacity; dims are per conformer, nbins
+// counts the buckets of all of them (conformer-major: bucket c * nb + local).
 __device__ ani_grid compute_grid(int n_conf, int n_per_conf, const float* __restrict__ cell, int pbc, int mode,
                                  float cutoff, int max_bins, const float* box_min, const float* box_max,
                                  int32_t* __restrict__ status) {
@@ -73,14 +76,15 @@ __device__ ani_grid compute_grid(int n_conf, int n_per_conf, const float* __rest
       }
     }
     // respect the caller's bucket capacity (buckets may only get larger than the cutoff)
-    int cap = max_bins - 1;
+    const int n_sub = mode == 2 ? n_conf : 1;
+    int cap = (max_bins - 1) / n_sub;
     while ((long long)g.dims[0] * g.dims[1] * g.dims[2] > (long long)cap) {
       int big = 0;
       if (g.dims[1] > g.dims[big]) big = 1;
       if (g.dims[2] > g.dims[big]) big = 2;
       g.dims[big] = max(1, g.dims[big] - max(1, g.dims[big] / 8));
     }
-    g.nbins = g.dims[0] * g.dims[1] * g.dims[2];
+    g.nbins = g.dims[0] * g.dims[1] * g.dims[2] * n_sub;
   }
   return g;
 }
@@ -164,6 +168,7 @@ __device__ __forceinline__ void wrapped_position(const ani_grid& g, const float*
   pos.y = y - (k[0] * g.cell[1] + k[1] * g.cell[4] + k[2] * g.cell[7]);
   pos.z = z - (k[0] * g.cell[2] + k[1] * g.cell[5] + k[2] * g.cell[8]);
   bin = (idx[0] * g.dims[1] + idx[1]) * g.dims[2] + idx[2];
+  if (g.mode == 2) bin += (a / g.n_per_conf) * (g.dims[0] * g.dims[1] * g.dims[2]);  // the conformer's sub-grid
 }
 
 __global__ void k_bin_assign(const float* __restrict__ coords, const int32_t* __restrict__ species, int n,
@@ -280,8 +285,9 @@ __global__ void k_bucket_ranges(const ani_grid* __restrict__ grid, const int32_t
   const ani_grid g = *grid;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const int b = idx / 27, o = idx % 27;
-  if (b >= g.nbins || g.mode != 0) return;
-  const int iz = b % g.dims[2], iy = (b / g.dims[2]) % g.dims[1], ix = b / (g.dims[2] * g.dims[1]);
+  if (b >= g.nbins || g.mode == 1) return;
+  int ix, iy, iz;
+  const int base = bucket_coords(g, b, ix, iy, iz);   // neighbours stay inside the conformer's sub-grid
   int j[3] = {ix + o / 9 - 1, iy + (o / 3) % 3 - 1, iz + o % 3 - 1};
   int w[3];
   for (int d = 0; d < 3; ++d) {
@@ -298,7 +304,7 @@ __global__ void k_bucket_ranges(const ani_grid* __restrict__ grid, const int32_t
   int lo = 0, hi = 0;
   const int code = (w[0] + 1) * 9 + (w[1] + 1) * 3 + (w[2] + 1);
   if (exists) {
-    const int nb = (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2];
+    const int nb = base + (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2];
     lo = bin_start[nb];
     hi = bin_start[nb + 1];
   }
@@ -620,8 +626,9 @@ __global__ void __launch_bounds__(256) k_prep_scatter(const __grid_constant__ Pr
   if (!A.ranges) return;
   const ani_grid g = *A.grid;
   const int b = idx / 27, o = idx % 27;
-  if (b >= g.nbins || g.mode != 0) return;
-  const int iz = b % g.dims[2], iy = (b / g.dims[2]) % g.dims[1], ix = b / (g.dims[2] * g.dims[1]);
+  if (b >= g.nbins || g.mode == 1) return;
+  int ix, iy, iz;
+  const int base = bucket_coords(g, b, ix, iy, iz);
   int j[3] = {ix + o / 9 - 1, iy + (o / 3) % 3 - 1, iz + o % 3 - 1};
   int w[3];
   for (int d = 0; d < 3; ++d) {
@@ -638,12 +645,12 @@ __global__ void __launch_bounds__(256) k_prep_scatter(const __grid_constant__ Pr
   int lo = 0, hi = 0;
   const int code = (w[0] + 1) * 9 + (w[1] + 1) * 3 + (w[2] + 1);
   if (exists) {
-    const int nb = (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2];
+    const int nb = base + (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2];
     lo = A.bin_start[nb];
     hi = A.bin_start[nb + 1];
   }
   const float wx = (float)w[0], wy = (float)w[1], wz = (float)w[2];
-  const int nbk = exists ? (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2] : 0;
+  const int nbk = exists ? base + (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2] : 0;
   A.ranges[2 * (size_t)idx] = make_float4(__int_as_float(lo), __int_as_float(hi), __int_as_float(code), __int_as_float(nbk));
   A.ranges[2 * (size_t)idx + 1] = make_float4(wx * g.cell[0] + wy * g.cell[3] + wz * g.cell[6],
                                               wx * g.cell[1] + wy * g.cell[4] + wz * g.cell[7],
@@ -886,10 +893,11 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
     const long long t2 = A.ranges ? max((long long)n, (long long)sg.nbins * 27) : (long long)n;
     for (long long idx = gtid; idx < t2; idx += gstride) {
       if (idx < n) A.tmp_list[__ldcg(&A.bin_start[A.bin_of[idx]]) + A.slot[idx]] = (int)idx;
-      if (!A.ranges || sg.mode != 0) continue;
+      if (!A.ranges || sg.mode == 1) continue;
       const int b = (int)(idx / 27), o = (int)(idx % 27);
       if (b >= sg.nbins) continue;
-      const int iz = b % sg.dims[2], iy = (b / sg.dims[2]) % sg.dims[1], ix = b / (sg.dims[2] * sg.dims[1]);
+      int ix, iy, iz;
+      const int base = bucket_coords(sg, b, ix, iy, iz);
       int j[3] = {ix + o / 9 - 1, iy + (o / 3) % 3 - 1, iz + o % 3 - 1};
       int wv[3];
       for (int d = 0; d < 3; ++d) {
@@ -906,12 +914,12 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
       int lo = 0, hi = 0;
       const int code = (wv[0] + 1) * 9 + (wv[1] + 1) * 3 + (wv[2] + 1);
       if (exists) {
-        const int nb = (j[0] * sg.dims[1] + j[1]) * sg.dims[2] + j[2];
+        const int nb = base + (j[0] * sg.dims[1] + j[1]) * sg.dims[2] + j[2];
         lo = __ldcg(&A.bin_start[nb]);
         hi = __ldcg(&A.bin_start[nb + 1]);
       }
       const float wx = (float)wv[0], wy = (float)wv[1], wz = (float)wv[2];
-      const int nbk = exists ? (j[0] * sg.dims[1] + j[1]) * sg.dims[2] + j[2] : 0;
+      const int nbk = exists ? base + (j[0] * sg.dims[1] + j[1]) * sg.dims[2] + j[2] : 0;
       A.ranges[2 * (size_t)idx] =
           make_float4(__int_as_float(lo), __int_as_float(hi), __int_as_float(code), __int_as_float(nbk));
       A.ranges[2 * (size_t)idx + 1] = make_float4(wx * sg.cell[0] + wy * sg.cell[3] + wz * sg.cell[6],
@@ -1490,7 +1498,8 @@ extern "C" int ani_b200_build_cells(const float* coords, const int32_t* species,
   if (n_conf < 1 || n_per_conf < 1 || cutoff <= 0.f || max_bins < 2) return ANI_ERR_BAD_ARG;
   if (mode == 0 && n_conf != 1) return ANI_ERR_UNSUPPORTED;
   if (mode == 1 && (pbc || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
-  if (mode != 0 && mode != 1) return ANI_ERR_BAD_ARG;
+  if (mode == 2 && (!pbc || !cell || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
+  if (mode < 0 || mode > 2) return ANI_ERR_BAD_ARG;
   if (pbc && !cell) return ANI_ERR_BAD_ARG;
   const long long n_ll = (long long)n_conf * n_per_conf;
   if (n_ll >= (1ll << ANI_IMG_SHIFT)) return ANI_ERR_UNSUPPORTED;
@@ -1509,7 +1518,7 @@ extern "C" int ani_b200_build_cells(const float* coords, const int32_t* species,
   k_bin_scatter<<<nb, 256, 0, st>>>(n, bin_of, slot, bin_start, tmp_list);
   k_bin_finalize<<<nb, 256, 0, st>>>(coords, species, n, grid, bin_of, bin_start, tmp_list, sorted_orig,
                                      orig_to_sorted, reinterpret_cast<float4*>(spos), sbin);
-  if (bucket_ranges && mode == 0) {
+  if (bucket_ranges && mode != 1) {
     // nbins is only known on the device: cover the caller's bucket capacity, surplus threads exit
     const long long threads = (long long)(max_bins - 1) * 27;
     k_bucket_ranges<<<(int)((threads + 255) / 256), 256, 0, st>>>(grid, bin_start, reinterpret_cast<float4*>(bucket_ranges));
@@ -1575,7 +1584,8 @@ extern "C" int ani_b200_prepare_step(const float* coords, const int32_t* species
   if (n_conf < 1 || n_per_conf < 1 || cutoff <= 0.f || max_bins < 2) return ANI_ERR_BAD_ARG;
   if (mode == 0 && n_conf != 1) return ANI_ERR_UNSUPPORTED;
   if (mode == 1 && (pbc || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
-  if (mode != 0 && mode != 1) return ANI_ERR_BAD_ARG;
+  if (mode == 2 && (!pbc || !cell || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
+  if (mode < 0 || mode > 2) return ANI_ERR_BAD_ARG;
   if (pbc && !cell) return ANI_ERR_BAD_ARG;
   const long long n_ll = (long long)n_conf * n_per_conf;
   if (n_ll >= (1ll << ANI_IMG_SHIFT)) return ANI_ERR_UNSUPPORTED;
@@ -1591,7 +1601,7 @@ extern "C" int ani_b200_prepare_step(const float* coords, const int32_t* species
   A.cell = cell; A.pbc = pbc; A.mode = mode; A.cutoff = cutoff; A.max_bins = max_bins;
   A.grid = grid; A.bin_start = bin_start; A.sorted_orig = sorted_orig; A.orig_to_sorted = orig_to_sorted;
   A.spos = reinterpret_cast<float4*>(spos); A.sbin = sbin;
-  A.ranges = (bucket_ranges && mode == 0) ? reinterpret_cast<float4*>(bucket_ranges) : nullptr;
+  A.ranges = (bucket_ranges && mode != 1) ? reinterpret_cast<float4*>(bucket_ranges) : nullptr;
   A.lo = lo; A.hi = hi; A.S = num_species; A.rows_cap = rows_cap;
   A.row_of = row_of; A.row_atom = row_atom; A.tile_species = tile_species; A.layout_info = layout_info;
   A.n_shf_r = n_shf_r; A.angular_sub = angular_sub; A.out_dim = out_dim; A.ldx = ldx; A.ang_pad = ang_pad; A.blocks = aev_blocks;

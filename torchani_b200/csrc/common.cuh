@@ -107,6 +107,18 @@ __device__ __forceinline__ float3 image_shift(const ani_grid& g, int code) {
   return s;
 }
 
+// bucket b of a mode 0 / mode 2 grid -> its (ix, iy, iz) inside its sub-grid; returns the first bucket of that
+// sub-grid (0 in mode 0; c * dims[0] * dims[1] * dims[2] for conformer c of a periodic batch)
+__device__ __forceinline__ int bucket_coords(const ani_grid& g, int b, int& ix, int& iy, int& iz) {
+  const int nb = g.dims[0] * g.dims[1] * g.dims[2];
+  const int base = b - b % nb;
+  b -= base;
+  iz = b % g.dims[2];
+  iy = (b / g.dims[2]) % g.dims[1];
+  ix = b / (g.dims[2] * g.dims[1]);
+  return base;
+}
+
 // ---- "tiled operand" layout shared by the AEV kernel (producer) and the tensor-core GEMM ----
 // A matrix [rows][cols] is stored per 128-row tile and 32-column K-block as OPND_PARTS 16-bit
 // pieces: [p1 128 rows x 64 B | p2 128 x 64 B (| p3)], every 8-row group in SWIZZLE_64B order

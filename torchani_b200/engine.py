@@ -442,6 +442,33 @@ class Workspace:
         self.moved = torch.zeros(1, **i32)
         # partial sums of the virial W_ab = sum_pairs (dE/dDelta)_a Delta_b (ani_b200_aev_backward)
         self.virial = torch.zeros(_lib.ANI_VIRIAL_SLOTS, 9, dtype=torch.float64, device=device)
+        self.periodic = n_conf == 1
+        self._retired: tp.List[Tensor] = []
+
+    def make_periodic(self) -> None:
+        """Size the bucket buffers of a batch for a shared periodic cell (grid mode 2), once, on its first use with a
+        cell: every conformer gets the bucket capacity of a single-system workspace of its atoms, so that its sub-grid
+        is the grid a single system would get.  The buffers of the open batch (one bucket per conformer) stay alive
+        for the CUDA graphs captured with them."""
+        if self.periodic:
+            return
+        n, dev = self.n, self.grid.device
+        i32 = dict(dtype=torch.int32, device=dev)
+        self._retired += [self.bin_start, self.scratch]
+        self.max_bins = self.n_conf * (max(64, self.n_per_conf + 2) - 1) + 1
+        self.bin_start = torch.zeros(self.max_bins + 2, **i32)
+        self.scratch = torch.zeros(3 * n + self.max_bins + 2 + (n // 256 + 3) * 8 + 64, **i32)
+        self.bucket_ranges = torch.zeros((self.max_bins - 1) * 27 * 8, dtype=torch.float32, device=dev)
+        self.bucket_species = (torch.zeros(self.max_bins * 8, **i32)
+                               if os.environ.get("ANI_B200_AEV_BSS", "0") != "0" else None)
+        self.virial = torch.zeros(self.n_conf * _lib.ANI_VIRIAL_SLOTS, 9, dtype=torch.float64, device=dev)
+        self.periodic = True
+
+
+def _grid_mode(n_conf: int, pbc: bool) -> int:
+    """ani_grid::mode: 0 one system, 1 an open batch (one bucket per conformer), 2 a periodic batch in one shared cell
+    (one sub-grid per conformer)."""
+    return 0 if n_conf == 1 else (2 if pbc else 1)
 
 
 class StepResult(tp.NamedTuple):
@@ -449,7 +476,8 @@ class StepResult(tp.NamedTuple):
     atomic_energies: Tensor   # (C, A) float32: NN atomic energies (ensemble mean), 0 for padding
     member_atomic: Tensor     # (M, C, A) float32 per-member NN atomic energies
     grad: tp.Optional[Tensor]  # (C, A, 3) float32 dE/dcoords (forces = -grad) or None
-    virial: tp.Optional[Tensor] = None  # (3, 3) float64 sum_pairs (dE/dDelta)_a Delta_b (stress = virial / volume)
+    virial: tp.Optional[Tensor] = None  # (3, 3) float64 sum_pairs (dE/dDelta)_a Delta_b (stress = virial / volume);
+    #                                     (C, 3, 3) for a periodic batch
 
 
 class Engine:
@@ -553,9 +581,9 @@ class Engine:
             raise ValueError(f"inputs must live on {dev} (the engine has no CPU path)")
         if pbc and cell is None:
             raise ValueError("If pbc is not None, cell should be present")
-        if pbc and n_conf != 1:
-            raise NotImplementedError("periodic batches (C > 1 with one shared cell) are not supported yet")
         ws = self.workspace(n_conf, n_per_conf)
+        if pbc:
+            ws.make_periodic()
         # inputs -> persistent buffers (what the graph reads)
         ws.species_i32.copy_(species.reshape(-1))
         ws.coords.copy_(coords.reshape(-1, 3))
@@ -575,8 +603,14 @@ class Engine:
         rank, world = shard
         lo = (n * rank) // world
         hi = (n * (rank + 1)) // world
-        if want_virial and (not want_grad or reuse or n_conf != 1):
-            raise ValueError("the virial comes out of the force pass of a single system with a freshly built grid")
+        periodic_batch = bool(pbc) and n_conf > 1
+        if want_virial and (not want_grad or reuse or (n_conf != 1 and not periodic_batch)):
+            raise ValueError("the virial comes out of the force pass of a single system or a periodic batch with a "
+                             "freshly built grid")
+        if periodic_batch and not ws.periodic:
+            raise ValueError("the workspace of a periodic batch needs Workspace.make_periodic() first")
+        if periodic_batch and reuse:
+            raise ValueError("reuse=True (Verlet skin) is not supported for periodic batches")
         key = (n_conf, n_per_conf, bool(pbc), bool(want_grad), lo, hi, self.nets.active_key, bool(reuse), self.skin,
                bool(want_virial), self.mlp_mode)
         if reuse and not self.skin > 0:
@@ -616,7 +650,11 @@ class Engine:
             mlp = 3 + (4 if want_grad else 0)
         self.launches_per_step = 1 + (0 if (pbc or n_conf > 1) else 1) + 1 + mlp + (1 if want_grad else 0) + 1
         grad = ws.grad.view(n_conf, n_per_conf, 3) if want_grad else None
-        virial = ws.virial.sum(0).view(3, 3) if want_virial else None
+        virial = None
+        if want_virial:
+            virial = ws.virial.view(n_conf, -1, 9).sum(1).view(n_conf, 3, 3)
+            if n_conf == 1:
+                virial = virial[0]
         return StepResult(ws.energies, ws.atomic.view(n_conf, n_per_conf),
                           ws.member_atomic.view(-1, n_conf, n_per_conf), grad, virial)
 
@@ -628,7 +666,7 @@ class Engine:
         n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
         st = torch.cuda.current_stream(self.device).cuda_stream
         cell_ptr = ptr(ws.cell) if pbc else None
-        mode = 0 if n_conf == 1 else 1
+        mode = _grid_mode(n_conf, pbc)
         c = self.consts
         # bucket grid + species-grouped row layout + live AEV column blocks (+ zero-fill of the force
         # accumulator): one fused entry point, five launches -- or, with a Verlet skin and reuse=True,
@@ -750,9 +788,9 @@ class Engine:
         graph): an analysis call, not the MD loop."""
         dev = self.device
         n_conf, n_per_conf = species.shape
-        if pbc and n_conf != 1:
-            raise NotImplementedError("periodic batches: call once per conformer")
         ws = self.workspace(n_conf, n_per_conf)
+        if pbc:
+            ws.make_periodic()
         n, L, c = ws.n, self.lib, self.consts
         nets = self.nets
         M, ldx = nets.num_members, nets.ldx
@@ -771,7 +809,7 @@ class Engine:
                 ws.cell.copy_(cell.reshape(-1))
             check(L.ani_b200_prepare_step(
                 ptr(ws.coords), ptr(ws.species_i32), n_conf, n_per_conf, ptr(ws.cell) if pbc else None, int(bool(pbc)),
-                0 if n_conf == 1 else 1, c.rcr, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start), ptr(ws.sorted_orig),
+                _grid_mode(n_conf, pbc), c.rcr, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start), ptr(ws.sorted_orig),
                 ptr(ws.orig_to_sorted), ptr(ws.spos), ptr(ws.sbin), ptr(ws.bucket_ranges), 0, n, c.num_species,
                 ws.rows_cap, ptr(ws.row_of), ptr(ws.row_atom), ptr(ws.tile_species), ptr(ws.layout_info),
                 len(c.shf_r), len(c.shf_a) * len(c.shf_z), c.out_dim, ldx, self.nets.col_pad, ptr(ws.aev_blocks), None, 0,

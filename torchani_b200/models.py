@@ -207,11 +207,7 @@ class ANI(torch.nn.Module):
         self._check_inputs(species, coords, charge)
         elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
         _validate_inputs(self.cutoff, elem_idxs, coords, cell, pbc)
-        if pbc is not None and elem_idxs.shape[0] > 1:
-            # periodic batch (C conformers in one shared cell): one engine step per conformer
-            parts = [self((species[c:c + 1], coords[c:c + 1]), cell, pbc, charge, atomic, ensemble_values).energies
-                     for c in range(elem_idxs.shape[0])]
-            return SpeciesEnergies(elem_idxs, torch.cat(parts, dim=1 if ensemble_values else 0))
+        # (a periodic batch -- C conformers in one shared cell -- is one engine step: one sub-grid per conformer)
         # (with a cell-list neighbour list the reference raises "Cell is too small" instead, neighbors.py:402-403: so
         # does the engine; all_pairs / adaptive models take the supercell route)
         sup = None if isinstance(self.neighborlist, CellList) else \
@@ -304,10 +300,6 @@ class ANI(torch.nn.Module):
         self._check_inputs(species, coords, charge)
         elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
         _validate_inputs(self.cutoff, elem_idxs, coords, cell, pbc)
-        if pbc is not None and elem_idxs.shape[0] > 1:
-            parts = [self.members_forces((species[c:c + 1], coords[c:c + 1]), cell, pbc, charge)
-                     for c in range(elem_idxs.shape[0])]
-            return SpeciesForces(elem_idxs, torch.cat([p.energies for p in parts], 1), torch.cat([p.forces for p in parts], 1))
         cell = effective_periodic_cell(coords, cell, pbc, self.cutoff)
 
         def run():
@@ -383,8 +375,8 @@ class ANI(torch.nn.Module):
 
     def energies_forces_stress(self, species: Tensor, coords: Tensor, cell: Tensor,
                                pbc: tp.Optional[Tensor] = None) -> tp.Tuple[Tensor, Tensor, Tensor]:
-        """(energies f64 (1,), forces f32 (1, A, 3), stress f64 (3, 3) in Hartree/A^3) of one periodic
-        system.  The stress is the "f dot r" virial of ase.py:164-168 -- sum over the pairs of
+        """(energies f64 (C,), forces f32 (C, A, 3), stress f64 in Hartree/A^3) of periodic systems in one cell: (3, 3)
+        for one system, (C, 3, 3) for a batch of C conformers.  The stress is the "f dot r" virial of ase.py:164-168 -- sum over the pairs of
         (dE/dDelta)_a Delta_b, accumulated by the force kernel -- divided by the cell volume; it equals
         the strain derivative dE/d(scaling)/V of ase.py:170-173 and, unlike that one, does not need the
         atoms to be wrapped into the cell."""

@@ -2,7 +2,8 @@
 
 ``CellList`` / ``AllPairs`` / ``AdaptiveList`` all run the same bucket-grid kernels
 (``ani_b200_build_cells`` + ``ani_b200_half_neighbor_*``): one conformer is bucketed on a grid
-(periodic or bounding box), a batch uses one bucket per conformer.  The result has the
+(periodic or bounding box), an open batch uses one bucket per conformer, a periodic batch one
+sub-grid of the shared cell per conformer.  The result has the
 reference's format -- ``Neighbors(indices (2,P) int64 into the flattened atoms, distances (P,),
 diff_vectors (P,3) = x[idx0] - x[idx1] + shift)`` -- and carries autograd to ``coords`` the same
 way (neighbors.py:107-112).  Pair ORDER differs from the reference (it is not specified there
@@ -124,11 +125,12 @@ def supercell_for_thin_cell(species: Tensor, coords: Tensor, cell: tp.Optional[T
     """A periodic cell THINNER than the cutoff (the reference's `all_pairs` pairs every atom with several lattice
     images, neighbors.py:245-275; the bucket grid needs one bucket per cutoff): replicate the cell n_d = ceil(cutoff /
     width_d) times along every too-thin direction.  Returns None if the cell is wide enough, else
-    ``(species_rep (1, R*A), coords_rep (1, R*A, 3), cell_rep, R)`` with the original atoms first: every replica is
+    ``(species_rep (C, R*A), coords_rep (C, R*A, 3), cell_rep, R)``, every conformer replicated within its own row,
+    with the original atoms first: every replica is
     translation-equivalent, so AEVs / atomic energies of the original atoms are those of the first A atoms, the energy
     is 1/R of the supercell's, and dE/dx of an original atom is the SUM over its R copies of the supercell gradient
     (which autograd does by itself through the replication below).  One host sync (the cell widths)."""
-    if pbc is None or cell is None or species.shape[0] != 1:
+    if pbc is None or cell is None:
         return None
     c = cell.detach().to(torch.float64).cpu()
     inv = torch.linalg.inv(c)
@@ -141,7 +143,7 @@ def supercell_for_thin_cell(species: Tensor, coords: Tensor, cell: tp.Optional[T
                           dtype=coords.dtype, device=coords.device)
     offs = shifts @ cell.to(coords.dtype)                               # (R, 3); the first one is zero
     R = offs.shape[0]
-    coords_rep = (coords.unsqueeze(1) + offs.view(1, R, 1, 3)).reshape(1, -1, 3)
+    coords_rep = (coords.unsqueeze(1) + offs.view(1, R, 1, 3)).reshape(coords.shape[0], -1, 3)
     species_rep = species.repeat(1, R)
     cell_rep = cell * torch.tensor(reps, dtype=cell.dtype, device=cell.device).view(3, 1)
     return species_rep, coords_rep, cell_rep, R
@@ -153,12 +155,18 @@ class BucketGrid:
     def __init__(self, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor], pbc: bool, cutoff: float):
         dev = coords.device
         n_conf, n_per_conf = species.shape
-        if pbc and n_conf != 1:
-            raise NotImplementedError("periodic batches (C > 1 with one shared cell) are not supported yet")
         n = n_conf * n_per_conf
         self.n, self.n_conf, self.n_per_conf = n, n_conf, n_per_conf
         i32 = dict(dtype=torch.int32, device=dev)
-        self.max_bins = max(64, n + 2) if n_conf == 1 else n_conf + 2
+        # one conformer: its own grid; an open batch: one bucket per conformer; a periodic batch (mode 2): one sub-grid
+        # per conformer with the bucket capacity of a single system
+        self.mode = 0 if n_conf == 1 else (2 if pbc else 1)
+        if self.mode == 0:
+            self.max_bins = max(64, n + 2)
+        elif self.mode == 1:
+            self.max_bins = n_conf + 2
+        else:
+            self.max_bins = n_conf * (max(64, n_per_conf + 2) - 1) + 1
         self.grid = torch.zeros(C.sizeof(Grid) // 4, **i32)
         self.status = torch.zeros(1, **i32)
         self.bin_start = torch.zeros(self.max_bins + 2, **i32)
@@ -173,7 +181,7 @@ class BucketGrid:
         self.stream = torch.cuda.current_stream(dev).cuda_stream
         check(_lib.lib().ani_b200_build_cells(
             ptr(coords_f), ptr(self.species_i32), n_conf, n_per_conf, ptr(cell_f), int(pbc),
-            0 if n_conf == 1 else 1, float(cutoff), self.max_bins, ptr(self.grid), ptr(self.bin_start),
+            self.mode, float(cutoff), self.max_bins, ptr(self.grid), ptr(self.bin_start),
             ptr(self.sorted_orig), ptr(self.orig_to_sorted), ptr(self.spos), ptr(self.sbin), None, ptr(scratch),
             ptr(self.status), self.stream), "build_cells")
 
@@ -191,13 +199,8 @@ class BucketGrid:
 
 def _half_list(cutoff: float, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor],
                pbc: tp.Optional[Tensor]) -> Neighbors:
-    if pbc is not None and species.shape[0] > 1:
-        # periodic batch (C conformers in one shared cell, neighbors.py:187-212): one grid per conformer, the pair
-        # indices refer to the flattened (C * A) atoms
-        per = [_half_list(cutoff, species[c:c + 1], coords[c:c + 1], cell, pbc) for c in range(species.shape[0])]
-        a = species.shape[1]
-        return Neighbors(torch.cat([nb.indices + c * a for c, nb in enumerate(per)], 1),
-                         torch.cat([nb.distances for nb in per]), torch.cat([nb.diff_vectors for nb in per]))
+    # (a periodic batch, neighbors.py:187-212, is one grid with a sub-grid per conformer: the pair indices refer to the
+    # flattened (C * A) atoms, conformer after conformer)
     cell = effective_periodic_cell(coords, cell, pbc, cutoff)
     g = BucketGrid(species, coords, cell, pbc is not None, cutoff)
     L = _lib.lib()
@@ -235,7 +238,7 @@ def cell_list(cutoff: float, species: Tensor, coords: Tensor, cell: tp.Optional[
 
 def all_pairs(cutoff: float, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor] = None,
               pbc: tp.Optional[Tensor] = None) -> Neighbors:
-    """neighbors.py:187-212 (batches without PBC, one conformer with PBC).  Same pair set as the
+    """neighbors.py:187-212 (batches with or without PBC).  Same pair set as the
     reference's O(N^2) enumeration as long as the periodic cell is at least one cutoff wide."""
     _validate_inputs(cutoff, species, coords, cell, pbc, supports_batches=True)
     return _half_list(cutoff, species, coords, cell, pbc)
