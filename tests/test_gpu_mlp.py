@@ -206,10 +206,11 @@ def _pad32(v: int) -> int:
     return (v + 31) // 32 * 32
 
 
-def reference_weights(widths: str, M: int, ldx: int):
-    """float64 copies of the float32 weights, zero-padded to the kernel's widths (multiples of 32, ldx columns)."""
+def reference_weights(widths: str, M: int, ldx: int, w=None):
+    """float64 copies of the float32 weights (``w``, default the seeded weights of these widths), zero-padded to the
+    kernel's widths (multiples of 32, ldx columns)."""
     symbols, dims, in_dim = WIDTHS[widths]
-    w = weights(widths, M)
+    w = weights(widths, M) if w is None else w
     out = []
     for s in symbols:
         h = dims[s]

@@ -29,7 +29,7 @@ def engines():
 
 def gpu_aev(eng, species, coords, cell, pbc):
     """AEV forward only, returned in input order (C, A, D)."""
-    from torchani_b200._lib import check, lib, ptr
+    from torchani_b200._lib import check, ptr
     dev = eng.device
     res = eng.step(species.to(dev), coords.to(dev), None if cell is None else cell.to(dev), pbc is not None,
                    want_grad=False)
@@ -37,21 +37,34 @@ def gpu_aev(eng, species, coords, cell, pbc):
     n = species.numel()
     st = torch.cuda.current_stream().cuda_stream
     plain = torch.zeros(ws.rows_cap, eng.nets.ldx, device=dev)
-    check(lib().ani_b200_aev_forward(C.byref(eng.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos),
+    check(eng.lib.ani_b200_aev_forward(C.byref(eng.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos),
                                      ptr(ws.sbin), None, None, None, n, 0, n, ptr(ws.row_of), ptr(plain), eng.nets.ldx, 0,
                                      ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap, ptr(ws.status), st))
+    # the plain rows once more with the step's own arguments (range table, bucket species, element mask): the same
+    # kernel path and order of additions as the tiled operand the step wrote
+    same = torch.zeros(ws.rows_cap, eng.nets.ldx, device=dev)
+    check(eng.lib.ani_b200_aev_forward(C.byref(eng.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos),
+                                       ptr(ws.sbin), ptr(ws.bucket_ranges), ptr(ws.bucket_species),
+                                       ws.aev_blocks.data_ptr() + 4 * (ws.n_blocks + 1), n, 0, n, ptr(ws.row_of),
+                                       ptr(same), eng.nets.ldx, 0, ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap,
+                                       ptr(ws.status), st))
     torch.cuda.synchronize()
     eng.check_status(ws)
     D = eng.consts.out_dim
     n_real = int((species >= 0).sum())
     so = ws.sorted_orig[:n_real].long()
     rows = ws.row_of[:n_real].long()
-    # the engine's own AEV buffer holds the same numbers as 16-bit pieces (2 x fp16 of 64*x: 22 bits and an
-    # absolute floor of 2^-31; 3 x bf16: 24 bits)
+    # the engine's own AEV buffer holds the same numbers as 16-bit pieces: 2 x fp16 of 64*x, 22 bits and an absolute
+    # floor of 2^-31; 3 x bf16, 24 bits (the whole float32 significand: exact but for the bfloat16 subnormal range)
     from torchani_b200.engine import untile_a_operand
-    tiled = untile_a_operand(ws.x.reshape(-1), ws.rows_cap, eng.nets.ldx)
-    err = (tiled[rows, :D] - plain[rows, :D]).abs()
-    assert bool((err <= plain[rows, :D].abs() * 2.0 ** -21 + 2.0 ** -30).all()), "tiled and plain AEV outputs differ"
+    tiled = untile_a_operand(ws.x.reshape(-1), ws.rows_cap, eng.nets.ldx, variant=eng.variant)
+    cols = torch.arange(D, device=dev)   # the tiled operand's internal column order: ang_pad zeros after the radial block
+    cols = torch.where(cols < eng.nets.radial_len, cols, cols + eng.nets.col_pad) if eng.nets.col_pad else cols
+    rel, floor = (2.0 ** -24, 2.0 ** -120) if eng.variant == "bf16x3" else (2.0 ** -21, 2.0 ** -30)
+    err = (tiled[rows][:, cols] - same[rows, :D]).abs()
+    assert bool((err <= same[rows, :D].abs() * rel + floor).all()), \
+        f"tiled and plain AEV outputs differ by up to {float((err / same[rows, :D].abs().clamp(min=1e-30)).max()):.3e}"
+    assert bool(((same[rows, :D] - plain[rows, :D]).abs() <= plain[rows, :D].abs() * 2.0 ** -21 + 2.0 ** -30).all())
     aev = torch.zeros(n, D, device=dev)
     aev[so] = plain[rows, :D]
     return aev.view(*species.shape, D).cpu(), res

@@ -118,8 +118,8 @@ class HostCalculator:
             self._copies_out(False)
             virial = res.virial.cpu()
         self._have_grid = False
-        if int(self.h_status[0]):
-            self.engine.check_status(self.ws)
+        if int(self.h_status[0]) and self._check_or_switch():
+            return self.calculate_with_stress(positions)
         volume = abs(float(np.linalg.det(self.h_cell.numpy().reshape(3, 3).astype(np.float64))))
         return float(self.h_energy[0]), np.negative(self.h_grad.numpy()), virial.numpy() / volume
 
@@ -144,27 +144,33 @@ class HostCalculator:
             self._run(False)
         elif reuse and int(self.h_moved[0]):
             self._have_grid = False   # close to the limit: rebuild before the next step
-        if int(self.h_status[0]):   # came back with the results: raise what the reference raises
-            try:
-                eng.check_status(self.ws)
-            except _lib.OperandRangeError:
-                # the 2 x fp16 operand format ran out of range: rebuild on the 3 x bfloat16 build and redo the step
-                nets = self.model.neural_networks
-                if nets._variant == "bf16x3" or not _lib.available("bf16x3") or self.sharded is not None:
-                    raise
-                import warnings
-                warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this "
-                              "model to the 3 x bfloat16 build of the library")
-                nets.use_variant("bf16x3")
-                self.engine = self.model.engine(self.device)
-                self.engine.skin = self.skin
-                self.ws = self.engine.workspace(1, self.n)
-                self.ws.species_i32.copy_(self.elem_idxs.reshape(-1))
-                self._graphs, self._have_grid = {}, False
-                self._mode_calls = {False: 0, True: 0}
-                return self.calculate(positions)
+        if int(self.h_status[0]) and self._check_or_switch():   # came back with the results
+            return self.calculate(positions)
         # a fresh array: h_grad is the persistent pinned D2H buffer and is overwritten by the next call
         return float(self.h_energy[0]), np.negative(self.h_grad.numpy())
+
+    def _check_or_switch(self) -> bool:
+        """Raise what the reference raises for the status word of the last step.  If the 2 x fp16 operand format ran
+        out of range, rebuild on the 3 x bfloat16 build of the library instead and return True: the caller redoes the
+        step."""
+        try:
+            self.engine.check_status(self.ws)
+        except _lib.OperandRangeError:
+            nets = self.model.neural_networks
+            if nets._variant == "bf16x3" or not _lib.available("bf16x3") or self.sharded is not None:
+                raise
+            import warnings
+            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this "
+                          "model to the 3 x bfloat16 build of the library")
+            nets.use_variant("bf16x3")
+            self.engine = self.model.engine(self.device)
+            self.engine.skin = self.skin
+            self.ws = self.engine.workspace(1, self.n)
+            self.ws.species_i32.copy_(self.elem_idxs.reshape(-1))
+            self._graphs, self._have_grid = {}, False
+            self._mode_calls = {False: 0, True: 0}
+            return True
+        return False
 
     def _run(self, reuse: bool) -> None:
         """One step (H2D, kernels, D2H, synchronise); after a few eager uses of a mode its whole sequence

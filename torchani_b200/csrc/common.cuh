@@ -138,10 +138,10 @@ constexpr int OPND_PARTS = ANI_OPND_FP16X2 ? 2 : 3;
 constexpr int OPND_ROW_BYTES = 64;                               // 32 halves / bfloat16
 constexpr int OPND_PART_BYTES = ANI_TILE_ROWS * OPND_ROW_BYTES;  // 8 KB
 constexpr int OPND_BLOCK_BYTES = OPND_PARTS * OPND_PART_BYTES;   // 16 KB (24 KB for 3 x bf16)
-// operand scales (powers of two).  Values: AEVs and CELU activations (|v| < 1023 representable);
-// gradients dE/d(activation) (|g| < 16 representable).  Weights carry a per-tensor scale chosen by
-// the packer (ani_mlp_species::w_scale).  Out-of-range values become inf/NaN downstream and raise
-// ANI_STATUS_OPERAND_RANGE.
+// operand scales (powers of two).  Values: AEVs and CELU activations (|v| <= 65504 / 64 = 1023.5);
+// gradients dE/d(activation) (|g| <= 65504 / 4096 = 15.9921875).  Weights carry a per-tensor scale
+// chosen by the packer (ani_mlp_species::w_scale).  A producer that stores |s * v| > OPND_HALF_MAX
+// (or a NaN, in the GEMM epilogues) raises ANI_STATUS_OPERAND_RANGE.
 constexpr float OPND_SCALE_VALUE = ANI_OPND_FP16X2 ? 64.0f : 1.0f;
 constexpr float OPND_SCALE_GRAD = ANI_OPND_FP16X2 ? 4096.0f : 1.0f;
 constexpr float OPND_HALF_MAX = 65504.0f;

@@ -887,7 +887,7 @@ class Engine:
             if code & _lib.STATUS_OPERAND_RANGE:
                 raise _lib.OperandRangeError(
                     "an AEV, activation or gradient left the range of the half-precision GEMM operand pieces "
-                    "(inf/NaN input, or |value| >= 1023 / |gradient| >= 16); the 3 x bfloat16 build of the library "
+                    "(inf/NaN input, or |value| > 1023.5 / |gradient| > 65504 / 4096); the 3 x bfloat16 build of the library "
                     "(variant 'bf16x3') has no such limit -- models.ANI switches to it automatically")
 
     def grid_info(self, ws: Workspace) -> Grid:

@@ -119,7 +119,7 @@ class _MLPFunction(torch.autograd.Function):
               "mlp_forward_backward")
         if int(status.item()) & _lib.STATUS_OPERAND_RANGE:   # this module-level path synchronises anyway
             raise _lib.OperandRangeError("an AEV, activation or gradient left the range of the half-precision GEMM "
-                                         "operand pieces (inf/NaN input, or |value| >= 1023 / |gradient| >= 16)")
+                                         "operand pieces (inf/NaN input, or |value| > 1023.5 / |gradient| > 65504 / 4096)")
         em_sorted = e_member[:, rows] * real.view(1, -1)          # (M, n) in `order` order
         out = torch.zeros(M, n, dtype=torch.float32, device=dev)
         out[:, order] = em_sorted
