@@ -388,28 +388,29 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
                     (size_t)gpart * g_bns * ROW_BYTES;
           }
           for (int kb = 0; kb < nkb; ++kb) {
-            for (int j = 0; j < a_sl + nh; ++j)
-              mbar_wait(&empty[(u + j) % RES_SLOTS], (((u + j) / RES_SLOTS) & 1) ^ 1);
             const int kbi = p == 0 && nblk >= 0 ? s_blk[kb] : kb;
             const int kbb = kbi + kb_boff;
             // B K-block in global memory: [p1 bn x 64 B | p2 bn x 64 B]
             const unsigned char* bsrc = Bm + ((size_t)n0 * nkb_all + (size_t)kbb * bn) * (PARTS * ROW_BYTES);
-            if (lane == 0) {
-              if (p == 0) {
-                const int sl = u % RES_SLOTS;
-                mbar_arrive_expect_tx(&full[sl], A_BLOCK_BYTES);
-                bulk_g2s(ring + sl * RES_SLOT_BYTES, F.x + ((size_t)rt * F.kbx + kbi) * A_BLOCK_BYTES, A_BLOCK_BYTES,
-                         &full[sl]);
-              }
-              for (int h = 0; h < nh; ++h) {
-                const int sl = (u + a_sl + h) % RES_SLOTS;
-                const uint32_t rows = (uint32_t)min(RES_HALF, bn - h * RES_HALF);
-                mbar_arrive_expect_tx(&full[sl], PARTS * rows * ROW_BYTES);
-                if (!gather)
+            // each slot is filled as soon as it is free: the consumers release a K-block's slots at different times
+            for (int j = 0; j < a_sl + nh; ++j) {
+              const int sl = (u + j) % RES_SLOTS;
+              mbar_wait(&empty[sl], (((u + j) / RES_SLOTS) & 1) ^ 1);
+              if (lane == 0) {
+                if (j < a_sl) {
+                  mbar_arrive_expect_tx(&full[sl], A_BLOCK_BYTES);
+                  bulk_g2s(ring + sl * RES_SLOT_BYTES, F.x + ((size_t)rt * F.kbx + kbi) * A_BLOCK_BYTES, A_BLOCK_BYTES,
+                           &full[sl]);
+                } else {
+                  const int h = j - a_sl;
+                  const uint32_t rows = (uint32_t)min(RES_HALF, bn - h * RES_HALF);
+                  mbar_arrive_expect_tx(&full[sl], PARTS * rows * ROW_BYTES);
+                  if (!gather)
 #pragma unroll
-                  for (int pp = 0; pp < PARTS; ++pp)
-                    bulk_g2s(ring + sl * RES_SLOT_BYTES + pp * A_PART_BYTES,
-                             bsrc + ((size_t)pp * bn + h * RES_HALF) * ROW_BYTES, rows * ROW_BYTES, &full[sl]);
+                    for (int pp = 0; pp < PARTS; ++pp)
+                      bulk_g2s(ring + sl * RES_SLOT_BYTES + pp * A_PART_BYTES,
+                               bsrc + ((size_t)pp * bn + h * RES_HALF) * ROW_BYTES, rows * ROW_BYTES, &full[sl]);
+                }
               }
             }
             __syncwarp();
@@ -451,9 +452,20 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
         for (int cc = 0; cc < 4; ++cc)
 #pragma unroll
           for (int i = 0; i < 32; ++i) acc[cc][i] = 0.f;
-        uint32_t prev = 0;
+        // A K-block's products are two commit groups, one per B slot (the second only if w1 > 0).  Every slot goes back
+        // to the producer as soon as the last group that reads it has retired: B rows 0-127 after group 1, the A slot
+        // (phase 0) and B rows 128-255 after group 2.  One group stays queued behind the one retiring, so the tensor
+        // pipe keeps its overlap while the ring keeps as many slots in flight as it can (the weight feed is bound by
+        // L2 latency, DESIGN §4.1).  The two groups accumulate into different registers, so the sums are those of
+        // one interleaved group.
+        uint32_t prev = 0, held = 0;  // slots prev + j (bit j of held) still read by the previous K-block's last group
+        auto release = [&](uint32_t base, uint32_t mask) {
+          if (lane == 0)
+            for (int j = 0; j < 3; ++j)
+              if (mask >> j & 1) mbar_arrive(&empty[(base + j) % RES_SLOTS]);
+        };
         for (int kb = 0; kb < nkb; ++kb) {
-          for (int j = 0; j < nslot; ++j) mbar_wait(&full[(u + j) % RES_SLOTS], ((u + j) / RES_SLOTS) & 1);
+          for (int j = 0; j <= a_sl; ++j) mbar_wait(&full[(u + j) % RES_SLOTS], ((u + j) / RES_SLOTS) & 1);
           const uint32_t sa = p == 0 ? smem_u32(ring + (u % RES_SLOTS) * RES_SLOT_BYTES) + wg * (64 / 8) * GROUP_BYTES
                                      : res_a + kb * A_BLOCK_BYTES;
           // B rows 0-127 and 128-255
@@ -470,23 +482,36 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
 #pragma unroll
             for (int pp = 0; pp < PARTS; ++pp) db[pp] = make_desc(sb0 + pp * A_PART_BYTES + adv);
             res_mma_slot(acc[0], acc[1], da, db, w0);
-            if (w1 > 0) {
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          release(prev, held);
+          if (w1 > 0) {
+            mbar_wait(&full[(u + a_sl + 1) % RES_SLOTS], ((u + a_sl + 1) / RES_SLOTS) & 1);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < TK / 16; ++k) {
+              const uint32_t adv = 32u * k;
+              uint64_t da[PARTS];
+#pragma unroll
+              for (int pp = 0; pp < PARTS; ++pp) da[pp] = make_desc(sa + pp * A_PART_BYTES + adv);
+              uint64_t db[PARTS];
 #pragma unroll
               for (int pp = 0; pp < PARTS; ++pp) db[pp] = make_desc(sb1 + pp * A_PART_BYTES + adv);
               res_mma_slot(acc[2], acc[3], da, db, w1);
             }
+            wgmma_commit();
+            wgmma_wait<1>();
+            release(u, 1u << a_sl);
+            held = ((1u << nslot) - 1) & ~(1u << a_sl);
+          } else {
+            held = (1u << nslot) - 1;
           }
-          wgmma_commit();
-          // the previous K-block's products have retired: its slots go back to the producer
-          wgmma_wait<1>();
-          if (kb > 0 && lane == 0)
-            for (int j = 0; j < nslot; ++j) mbar_arrive(&empty[(prev + j) % RES_SLOTS]);
           prev = u;
           u += nslot;
         }
         wgmma_wait<0>();
-        if (nkb > 0 && lane == 0)
-          for (int j = 0; j < nslot; ++j) mbar_arrive(&empty[(prev + j) % RES_SLOTS]);
+        release(prev, held);
         // the copies of a1 / a2 have read R before the epilogues of phases 1 / 2 overwrite it, and have landed in
         // global memory before phase 3 reads act2 back (phase 4 reads act1, copied earlier)
         if (copier && (p == 1 || p == 2)) bulk_wait_read();
