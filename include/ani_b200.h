@@ -61,6 +61,7 @@ extern "C" {
 #define ANI_STATUS_INTERNAL 32      /* a device-side barrier / dependency wait timed out (never expected) */
 
 #define ANI_MAX_ANG 96 /* angular neighbours (<= Rca) one central atom may have */
+#define ANI_LATTICE_STRIDE 18 /* floats per conformer of the lattice table of grid mode 3: cell[9], inverse[9] */
 
 /* AEV constants; mirrors the CuaevComputer constructor (csrc/cuaev.cpp:247-278).       */
 typedef struct ani_aev_params {
@@ -90,7 +91,9 @@ typedef struct ani_grid {
   int32_t pbc;     /* 1 = periodic in all three directions                                */
   int32_t nbins;   /* real buckets (all conformers); padding atoms live in bucket nbins   */
   int32_t mode;    /* 0 = one conformer on a grid, 1 = batch, bucket == conformer,        */
-                   /* 2 = periodic batch: one sub-grid of the shared cell per conformer   */
+                   /* 2 = periodic batch: one sub-grid of the shared cell per conformer,  */
+                   /* 3 = periodic batch, one cell per conformer (cell / inv: conformer 0; */
+                   /*     every conformer's lattice is in the lattice table)              */
   int32_t n_per_conf;
   int32_t n_real;  /* number of non-padding atoms (== bin_start[nbins])                  */
 } ani_grid;
@@ -112,6 +115,7 @@ const char* ani_b200_last_cuda_error(void);
 /*    coords  [n_conf*n_per_conf*3] f32, species [n_conf*n_per_conf] i32 (-1 = padding)    */
 /*    cell    device f32[9] (rows = lattice vectors) or NULL; pbc 0/1 (all directions)      */
 /*    mode 0 requires n_conf == 1; mode 1 requires pbc == 0.                                */
+/*    mode 3 (one cell per conformer) is ANI_ERR_UNSUPPORTED here: ani_b200_prepare_step_cells. */
 /*    mode 2 (C conformers in one shared periodic cell) requires pbc == 1, a cell and        */
 /*    n_conf + 1 <= max_bins, else ANI_ERR_UNSUPPORTED (before any CUDA call).  Buckets are   */
 /*    conformer-major: bucket c * nb + local, nb = dims[0]*dims[1]*dims[2], nbins = C * nb;   */
@@ -200,6 +204,24 @@ int ani_b200_aev_backward(const ani_aev_params* params, const ani_grid* grid, co
                           const int32_t* nbr_list, int nbr_cap, float* grad_coords,
                           int32_t* status, int max_elements, double* virial, void* stream);
 
+/* 3d/4d. The AEV forward and backward of a grid-mode-3 preparation (one cell per conformer,              */
+/*    ani_b200_prepare_step_cells): the arguments of ani_b200_aev_forward / _backward plus the lattice      */
+/*    table that preparation wrote (device f32[n_conf][ANI_LATTICE_STRIDE], not NULL, else ANI_ERR_BAD_ARG). */
+/*    Image shifts are taken in the lattice of the central atom's conformer (its neighbours always lie in  */
+/*    that conformer).  A mode-3 grid must only be passed to these two entry points; the virial has the    */
+/*    per-conformer layout of mode 2.                                                                       */
+int ani_b200_aev_forward_cells(const ani_aev_params* params, const ani_grid* grid,
+                               const int32_t* bin_start, const float* spos, const int32_t* sbin,
+                               const float* bucket_ranges, const int32_t* bucket_species, const int32_t* species_mask,
+                               int n, int lo, int hi, const int32_t* row_of, float* aev, int ldx, int layout,
+                               int32_t* nbr_cnt, int32_t* nbr_list, int nbr_cap, int32_t* status,
+                               const float* lattice, void* stream);
+int ani_b200_aev_backward_cells(const ani_aev_params* params, const ani_grid* grid, const float* spos,
+                                const int32_t* sorted_orig, const int32_t* species_mask, int n, int lo,
+                                int hi, const int32_t* row_of, const float* grad_aev, int ldx,
+                                const int32_t* nbr_cnt, const int32_t* nbr_list, int nbr_cap, float* grad_coords,
+                                int32_t* status, int max_elements, double* virial, const float* lattice, void* stream);
+
 /* 4b. The same AEV kernels fed by an externally supplied HALF pair list (the reference's    */
 /*    Neighbors tuple; AEVComputer.compute_from_neighbors, aev/_computer.py:251-272 ->          */
 /*    cuaev::run_with_half_nbrlist, csrc/aev.cu:1128-1208,1779-1866).  ani_b200_pairs_to_rows     */
@@ -274,6 +296,28 @@ int ani_b200_prepare_step(const float* coords, const int32_t* species, int n_con
                           int n_shf_r, int angular_sub, int out_dim, int ldx, int ang_pad, int32_t* aev_blocks,
                           float* zero_f32, int zero_f32_count, double* zero_f64, int zero_f64_count,
                           int32_t* bucket_species, int32_t* scratch_i32, int32_t* status, void* stream);
+
+/* 3e. The same preparation in grid mode 3: a periodic batch with ONE CELL PER CONFORMER (the frames of an NPT      */
+/*     trajectory, a screened dataset).  Arguments of ani_b200_prepare_step with mode == 3 (else                     */
+/*     ANI_ERR_UNSUPPORTED), pbc == 1, n_conf + 1 <= max_bins, and                                                   */
+/*       cell     device f32[n_conf][9], rows of every 3x3 block are that conformer's lattice vectors              */
+/*       lattice  device f32[n_conf][ANI_LATTICE_STRIDE] (out, not NULL): per conformer {cell[9], inverse[9]}, the    */
+/*                inverse computed in double and rounded; read by ani_b200_aev_forward_cells / _backward_cells.    */
+/*     Buckets are conformer-major as in mode 2 (bucket c * nb + local) with sub-grid dims common to all            */
+/*     conformers: per axis the minimum over the conformers of floor(perpendicular width / (cutoff + 1e-5)),        */
+/*     capped so that nb <= (max_bins - 1) / n_conf.  Every atom is wrapped, and every image shift of the range     */
+/*     table is taken, in its own conformer's lattice.  A conformer whose cell is thinner than the cutoff raises    */
+/*     ANI_STATUS_CELL_TOO_SMALL.  With C equal cells every output equals that of mode 2 on the shared cell.       */
+/*     Runs the persistent-grid form or the five-launch form (+ one single-CTA setup launch); same outputs.        */
+int ani_b200_prepare_step_cells(const float* coords, const int32_t* species, int n_conf, int n_per_conf,
+                                const float* cell, int pbc, int mode, float cutoff, int max_bins, ani_grid* grid,
+                                int32_t* bin_start, int32_t* sorted_orig, int32_t* orig_to_sorted, float* spos,
+                                int32_t* sbin, float* bucket_ranges, int lo, int hi, int num_species, int rows_cap,
+                                int32_t* row_of, int32_t* row_atom, int32_t* tile_species, int32_t* layout_info,
+                                int n_shf_r, int angular_sub, int out_dim, int ldx, int ang_pad, int32_t* aev_blocks,
+                                float* zero_f32, int zero_f32_count, double* zero_f64, int zero_f64_count,
+                                int32_t* bucket_species, int32_t* scratch_i32, int32_t* status, float* lattice,
+                                void* stream);
 
 /* Timing experiments only: the first 4 CTAs of the next `launches` tensor-core GEMM launches    */
 /* write clock64 stamps [launch][cta 4][tile 8][role 3: producer, MMA, epilogue][4] into buf       */

@@ -21,6 +21,7 @@ ANI_MAX_MEMBERS = 16
 ANI_TILE_ROWS = 128
 ANI_MAX_ANG = 96
 ANI_VIRIAL_SLOTS = 64
+ANI_LATTICE_STRIDE = 18   # floats per conformer of the lattice table of grid mode 3: cell, inverse
 
 STATUS_NBR_OVERFLOW = 1
 STATUS_ANG_OVERFLOW = 2
@@ -86,7 +87,14 @@ _PROTOTYPES = {
     "ani_b200_aev_backward_rows": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _I, _I, _P, _P, _P]),
     "ani_b200_prepare_step": (C.c_int, [_P, _P, _I, _I, _P, _I, _I, C.c_float, _I, _P, _P, _P, _P, _P, _P, _P,
                                         _I, _I, _I, _I, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _I, _P, _P, _P, _P]),
-    "ani_b200_verlet_positions": (C.c_int, [_I, _P, _P, _P, _I, _F, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
+    "ani_b200_prepare_step_cells": (C.c_int, [_P, _P, _I, _I, _P, _I, _I, C.c_float, _I, _P, _P, _P, _P, _P, _P, _P,
+                                              _I, _I, _I, _I, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _I, _P,
+                                              _P, _P, _P, _P]),
+    "ani_b200_aev_forward_cells": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _I, _I, _P, _P, _I, _P,
+                                             _P, _P]),
+    "ani_b200_aev_backward_cells": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _P, _I, _P,
+                                              _P, _P]),
+    "ani_b200_verlet_positions":(C.c_int, [_I, _P, _P, _P, _I, _F, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
     "ani_b200_debug_gemm_trace": (C.c_int, [_P, _I]),
     "ani_b200_half_neighbor_count": (C.c_int, [_P, _P, _P, _P, _P, _I, _F, _P, _P]),
     "ani_b200_half_neighbor_fill": (C.c_int, [_P, _P, _P, _P, _P, _I, _F, _P, C.c_int64, _P, _P, _P, _P, _P, _P]),

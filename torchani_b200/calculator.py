@@ -26,11 +26,17 @@ HARTREE_TO_EV = 27.211386024367243  # units.py (CODATA 2014, as used by the refe
 class HostCalculator:
     """Energy + forces for a fixed set of atoms from host coordinates.
 
+    A BATCH of C systems of A atoms each (replicas, the frames of a trajectory, a screened dataset) is one step
+    too: ``atomic_numbers`` (C, A) (-1 pads a shorter system), ``cell`` one (3, 3) cell shared by all or one cell per
+    conformer (C, 3, 3); ``calculate`` then takes positions (C, A, 3) and returns energies (C,) and forces (C, A, 3)
+    with the same single H2D and D2H copy per step, inside the same captured graph.
+
     Args:
         model: a ``torchani_b200.models.ANI`` on a CUDA device
         atomic_numbers: (A,) or (1, A) integer array (atomic numbers, or element indices if the
-            model was built with ``periodic_table_index=False``)
-        cell: (3, 3) lattice vectors as rows, or None for a non-periodic system
+            model was built with ``periodic_table_index=False``), or (C, A) for a batch
+        cell: (3, 3) lattice vectors as rows, (C, 3, 3) one cell per conformer of a batch, or None for a non-periodic
+            system
         pbc: periodic in all three directions (partial periodicity is not supported)
         skin: > 0 switches on Verlet-skin reuse of the bucket grid (the counterpart of
             ``torchani.neighbors.VerletCellList``, neighbors.py:759-884): the grid is built for
@@ -46,13 +52,19 @@ class HostCalculator:
         if dev.type != "cuda":
             raise ValueError("HostCalculator needs a model on a CUDA device")
         self.model, self.device, self.pbc, self.shard = model, dev, bool(pbc), shard
-        z = torch.as_tensor(np.asarray(atomic_numbers)).reshape(1, -1).to(dev)
+        z = np.asarray(atomic_numbers)
+        self.n_conf = z.shape[0] if z.ndim == 2 else 1
+        self.batch = self.n_conf > 1
+        z = torch.as_tensor(z).reshape(self.n_conf, -1).to(dev)
         self.elem_idxs = model.species_converter(z, nop=not model.periodic_table_index)   # validated once
         self.n = z.shape[1]
         self.engine = model.engine(dev)
         self.skin = float(skin)
         if self.skin < 0:
             raise ValueError("skin must be >= 0")
+        if self.batch and (self.skin > 0 or sharded is not None):
+            raise ValueError("a batch of systems runs on one GPU with a freshly built grid: no skin, no sharding")
+        self.conformer_cells = False   # one cell per conformer of a batch (grid mode 3)
         if self.skin > 0:
             self.engine.skin = self.skin   # buckets for cutoff + skin (shared by every user of this engine)
         # multi-GPU (one process per GPU): `sharded` = parallel.ShardedEngine over this model's engine.  This rank
@@ -67,27 +79,26 @@ class HostCalculator:
                 raise ValueError("Verlet-skin reuse is not combined with multi-GPU sharding")
             self.shard = shard = (sharded.rank, sharded.world)
             self.ws = sharded.attach(1, self.n)
+            self.ws.species_i32.copy_(self.elem_idxs.reshape(-1))
         else:
-            self.ws = self.engine.workspace(1, self.n)
-        self.ws.species_i32.copy_(self.elem_idxs.reshape(-1))
+            self.ws = self._workspace()
         # pinned mirrors of the workspace's two transfer blocks (engine.Workspace.in_block / out_block): ONE H2D copy of
-        # [cell | coords] and ONE D2H copy of [energy | status | gradient] per step
+        # [cell(s) | coords] and ONE D2H copy of [energies | status | gradient] per step
+        C_ = self.n_conf
         self.h_in = torch.zeros(self.ws.in_block.numel(), dtype=torch.float32).pin_memory()
         self.h_out = torch.zeros(self.ws.out_block.numel(), dtype=torch.uint8).pin_memory()
-        self.h_coords = self.h_in[16:].view(self.n, 3)
+        shape = (C_, self.n, 3) if self.batch else (self.n, 3)
+        self.h_coords = self.h_in[self.ws.in_coords_off:].view(shape)
         self.h_cell = self.h_in[:9]
+        self.h_cells = self.h_in[:9 * C_].view(C_, 9)
         off = self.ws._out_grad_off
-        self.h_grad = self.h_out[off:].view(torch.float32).view(self.n, 3)
-        self.h_energy = self.h_out[:8].view(torch.float64)
-        self.h_status = self.h_out[8:12].view(torch.int32)
+        self.h_grad = self.h_out[off:].view(torch.float32).view(shape)
+        self.h_energy = self.h_out[:8 * C_].view(torch.float64)
+        self.h_status = self.h_out[8 * C_:8 * C_ + 4].view(torch.int32)
         self.h_moved = torch.zeros(1, dtype=torch.int32).pin_memory()
         self._have_grid = False       # a grid built with the skin exists and may be reused
         self.rebuilds = 0             # steps that built the grid
         self.redone = 0               # reuse steps that had to be recomputed (an atom left its skin/2 sphere)
-        if pbc and cell is None:
-            raise ValueError("If pbc is not None, cell should be present")
-        if cell is not None:
-            self.set_cell(cell)
         self.h2d_bytes = self.h_in.numel() * 4
         self.d2h_bytes = self.h_out.numel()
         self.graph_after = 3          # eager host-driven steps before copies + kernels are captured as one graph
@@ -95,9 +106,33 @@ class HostCalculator:
         self._graphs: tp.Dict[bool, torch.cuda.CUDAGraph] = {}   # reuse flag -> captured step
         self._mode_calls = {False: 0, True: 0}
         self._graph_version: tp.Any = None
+        if pbc and cell is None:
+            raise ValueError("If pbc is not None, cell should be present")
+        if cell is not None:
+            self.set_cell(cell)
+
+    def _workspace(self):
+        ws = self.engine.workspace(self.n_conf, self.n)
+        if self.batch and self.pbc:
+            ws.make_periodic()
+        ws.species_i32.copy_(self.elem_idxs.reshape(-1))
+        return ws
 
     def set_cell(self, cell) -> None:
-        self.h_cell.copy_(torch.as_tensor(np.asarray(cell, dtype=np.float32)).reshape(-1))
+        c = torch.as_tensor(np.asarray(cell, dtype=np.float32))
+        per = c.dim() == 3
+        if per and not self.batch:
+            c, per = c.reshape(3, 3), False   # (1, 3, 3): the cell of the one system
+        if per:
+            if c.shape != (self.n_conf, 3, 3):
+                raise ValueError(f"cell must be (3, 3) or ({self.n_conf}, 3, 3); got {tuple(c.shape)}")
+            self.h_cells.copy_(c.reshape(self.n_conf, 9))
+        else:
+            self.h_cell.copy_(c.reshape(-1))
+        if per != self.conformer_cells:   # another kind of cell: other kernels, other captured graphs
+            self.conformer_cells = per
+            self._graphs = {}
+            self._mode_calls = {False: 0, True: 0}
         self._have_grid = False   # a grid belongs to one cell
 
     def calculate_with_stress(self, positions, cell=None) -> tp.Tuple[float, np.ndarray, np.ndarray]:
@@ -108,30 +143,38 @@ class HostCalculator:
             raise ValueError("the stress needs a periodic cell")
         if cell is not None:
             self.set_cell(cell)
-        if isinstance(positions, Tensor):
-            self.h_coords.copy_(positions.reshape(self.n, 3))
-        else:
-            self.h_coords.numpy()[...] = np.asarray(positions, dtype=np.float32).reshape(self.n, 3)
+        self._set_positions(positions)
         with torch.cuda.device(self.device):
             self._copies_in(False)
-            res = self.engine.run(self.ws, True, want_grad=True, shard=self.shard, want_virial=True)
+            res = self.engine.run(self.ws, True, want_grad=True, shard=self.shard, want_virial=True,
+                                  conformer_cells=self.conformer_cells)
             self._copies_out(False)
-            virial = res.virial.cpu()
+            virial = res.virial.cpu().numpy()
         self._have_grid = False
         if int(self.h_status[0]) and self._check_or_switch():
             return self.calculate_with_stress(positions)
+        if self.batch:
+            cells = (self.h_cells.numpy().reshape(-1, 3, 3) if self.conformer_cells
+                     else self.h_cell.numpy().reshape(1, 3, 3))
+            volume = np.abs(np.linalg.det(cells.astype(np.float64))).reshape(-1, 1, 1)
+            return self.h_energy.numpy().copy(), np.negative(self.h_grad.numpy()), virial / volume
         volume = abs(float(np.linalg.det(self.h_cell.numpy().reshape(3, 3).astype(np.float64))))
-        return float(self.h_energy[0]), np.negative(self.h_grad.numpy()), virial.numpy() / volume
+        return float(self.h_energy[0]), np.negative(self.h_grad.numpy()), virial / volume
+
+    def _set_positions(self, positions) -> None:
+        shape = tuple(self.h_coords.shape)
+        if isinstance(positions, Tensor):
+            self.h_coords.copy_(positions.reshape(shape))
+        else:
+            self.h_coords.numpy()[...] = np.asarray(positions, dtype=np.float32).reshape(shape)
 
     def calculate(self, positions, cell=None) -> tp.Tuple[float, np.ndarray]:
         """positions: (A, 3) float array on the host (Angstrom).  Returns (energy [Hartree],
-        forces (A, 3) [Hartree/Angstrom]) -- multiply by HARTREE_TO_EV for ASE units."""
+        forces (A, 3) [Hartree/Angstrom]) -- multiply by HARTREE_TO_EV for ASE units.  A batch: positions (C, A, 3),
+        energies (C,) float64 and forces (C, A, 3); ``cell`` (3, 3) or (C, 3, 3) replaces the cell(s)."""
         if cell is not None:
             self.set_cell(cell)
-        if isinstance(positions, Tensor):
-            self.h_coords.copy_(positions.reshape(self.n, 3))
-        else:
-            self.h_coords.numpy()[...] = np.asarray(positions, dtype=np.float32).reshape(self.n, 3)
+        self._set_positions(positions)
         eng = self.engine
         self._calls += 1
         if self._graphs and self._graph_version != eng.nets.active_key:
@@ -147,6 +190,8 @@ class HostCalculator:
         if int(self.h_status[0]) and self._check_or_switch():   # came back with the results
             return self.calculate(positions)
         # a fresh array: h_grad is the persistent pinned D2H buffer and is overwritten by the next call
+        if self.batch:
+            return self.h_energy.numpy().copy(), np.negative(self.h_grad.numpy())
         return float(self.h_energy[0]), np.negative(self.h_grad.numpy())
 
     def _check_or_switch(self) -> bool:
@@ -165,8 +210,7 @@ class HostCalculator:
             nets.use_variant("bf16x3")
             self.engine = self.model.engine(self.device)
             self.engine.skin = self.skin
-            self.ws = self.engine.workspace(1, self.n)
-            self.ws.species_i32.copy_(self.elem_idxs.reshape(-1))
+            self.ws = self._workspace()
             self._graphs, self._have_grid = {}, False
             self._mode_calls = {False: 0, True: 0}
             return True
@@ -197,19 +241,19 @@ class HostCalculator:
             return
         if graph is None and eng.cuda_graph and not eng.profile and self._mode_calls[reuse] > self.graph_after:
             rank, world = self.shard
-            lo, hi = (self.n * rank) // world, (self.n * (rank + 1)) // world
+            lo, hi = (ws.n * rank) // world, (ws.n * (rank + 1)) // world   # (all atoms of a batch)
             eng.note_composition(ws)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 self._copies_in(reuse)
-                eng._launch(ws, self.pbc, True, lo, hi, reuse)
+                eng._launch(ws, self.pbc, True, lo, hi, reuse, conformer_cells=self.conformer_cells)
                 self._copies_out(reuse)
             self._graphs[reuse], self._graph_version = graph, eng.nets.active_key
         if graph is not None:
             graph.replay()
         else:
             self._copies_in(reuse)
-            eng.run(ws, self.pbc, want_grad=True, shard=self.shard, reuse=reuse)
+            eng.run(ws, self.pbc, want_grad=True, shard=self.shard, reuse=reuse, conformer_cells=self.conformer_cells)
             self._copies_out(reuse)
         torch.cuda.current_stream(self.device).synchronize()
         if not reuse:

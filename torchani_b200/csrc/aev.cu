@@ -320,7 +320,9 @@ __device__ __forceinline__ float transpose_reduce32(float (&acc)[32], int lane) 
 // ---------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------
-template <int NA, int NZ>
+// LAT (grid mode 3): image shifts in the lattice of the bucket's conformer (lattice table); the range table, when
+// given, already holds them
+template <int NA, int NZ, bool LAT = false>
 __global__ void __launch_bounds__(AEV_WARPS * 32)
     k_aev_forward(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
                   const int32_t* __restrict__ bin_start, const float4* __restrict__ spos,
@@ -328,7 +330,8 @@ __global__ void __launch_bounds__(AEV_WARPS * 32)
                   const int32_t* __restrict__ species_mask, const ExplicitNbrs ex, int lo, int hi,
                   const int32_t* __restrict__ row_of,
                   float* __restrict__ aev, int ldx, int layout, int32_t* __restrict__ nbr_cnt,
-                  int32_t* __restrict__ nbr_list, int cap, int32_t* __restrict__ status, size_t warp_bytes) {
+                  int32_t* __restrict__ nbr_list, int cap, int32_t* __restrict__ status, size_t warp_bytes,
+                  const float* __restrict__ lattice) {
   static_assert(NA * NZ == 32, "one lane per angular feature");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -422,7 +425,9 @@ __global__ void __launch_bounds__(AEV_WARPS * 32)
           for (int oz = -1; oz <= 1; ++oz) {
             NeighbourRange r;
             if (!neighbour_bucket(g, bin_start, base, ix, iy, iz, ox, oy, oz, r)) continue;
-            const float3 sh = (r.code == 13) ? make_float3(0.f, 0.f, 0.f) : image_shift(g, r.code);
+            const float3 sh = (r.code == 13) ? make_float3(0.f, 0.f, 0.f)
+                              : LAT ? image_shift(lattice, base / (g.dims[0] * g.dims[1] * g.dims[2]), r.code)
+                                    : image_shift(g, r.code);
             scan_range(r.lo, r.hi, r.code, sh.x, sh.y, sh.z);
           }
     }
@@ -570,7 +575,7 @@ struct CtaStage {
   unsigned long long tma_bar;                  // mbarrier of the TMA bulk copies that stage the bucket ranges
 };
 
-template <int NA, int NZ, bool TMA_STAGE = false>
+template <int NA, int NZ, bool TMA_STAGE = false, bool LAT = false>
 __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
     k_aev_forward_cta(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
                       const int32_t* __restrict__ bin_start, const float4* __restrict__ spos,
@@ -578,7 +583,7 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
                       const int32_t* __restrict__ species_mask, int lo, int hi, const int32_t* __restrict__ row_of,
                       float* __restrict__ aev, int ldx, int layout, int32_t* __restrict__ nbr_cnt,
                       int32_t* __restrict__ nbr_list, int cap, int32_t* __restrict__ status, size_t warp_bytes,
-                      int tma_stage, const int32_t* __restrict__ bss) {
+                      int tma_stage, const int32_t* __restrict__ bss, const float* __restrict__ lattice) {
   static_assert(NA * NZ == 32, "one lane per angular feature");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ CtaStage C;
@@ -650,7 +655,8 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
           rhi = r.hi;
           code = r.code;
           if (code != 13) {
-            const float3 v = image_shift(g, code);
+            const float3 v = LAT ? image_shift(lattice, base / (g.dims[0] * g.dims[1] * g.dims[2]), code)
+                                 : image_shift(g, code);
             sh = make_float4(v.x, v.y, v.z, 0.f);
           }
         }
@@ -1001,14 +1007,16 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
 // ---------------------------------------------------------------------------------------
 // backward
 // ---------------------------------------------------------------------------------------
-template <int NA, int NZ, bool VIRIAL = false>
+// LAT (grid mode 3): image shifts in the lattice of the central atom's conformer (lattice table)
+template <int NA, int NZ, bool VIRIAL = false, bool LAT = false>
 __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
     k_aev_backward(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
                    const float4* __restrict__ spos, const int32_t* __restrict__ sorted_orig, int lo, int hi,
                    const int32_t* __restrict__ row_of, const float* __restrict__ gaev, int ldx,
                    const int32_t* __restrict__ nbr_cnt, const int32_t* __restrict__ nbr_list, const ExplicitNbrs ex,
                    const int32_t* __restrict__ species_mask, int cap, float* __restrict__ grad_coords,
-                   int32_t* __restrict__ status, size_t warp_bytes, int pair_cap, double* __restrict__ virial) {
+                   int32_t* __restrict__ status, size_t warp_bytes, int pair_cap, double* __restrict__ virial,
+                   const float* __restrict__ lattice) {
   static_assert(NA * NZ == 32, "one lane per angular feature");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1059,6 +1067,7 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
   if (__float_as_int(pi.w) < 0) return;  // padding atom (explicit neighbour rows only)
   const int e0 = ex.start ? ex.start[i] : 0;
   const int cnt = ex.start ? min(ex.start[i + 1] - e0, cap) : nbr_cnt[i];
+  const int conf_i = LAT ? sorted_orig[i] / g.n_per_conf : 0;   // neighbours lie in the centre's conformer
   for (int n = lane; n < cnt; n += 32) {
     int j;
     float4 dR;
@@ -1071,7 +1080,7 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
       const int code = (unsigned)word >> ANI_IMG_SHIFT;
       const float4 p = spos[j];
       float3 sh = make_float3(0.f, 0.f, 0.f);
-      if (code != 13) sh = image_shift(g, code);
+      if (code != 13) sh = LAT ? image_shift(lattice, conf_i, code) : image_shift(g, code);
       const float dx = (p.x + sh.x) - pi.x, dy = (p.y + sh.y) - pi.y, dz = (p.z + sh.z) - pi.z;
       dR = make_float4(dx, dy, dz, sqrtf(dx * dx + dy * dy + dz * dz));
     }
@@ -1310,8 +1319,8 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
     }
   }
   if (VIRIAL && virial) {
-    // a periodic batch (mode 2) keeps one set of slots per conformer: the conformer of the central atom
-    const int conf = g.mode == 2 ? sorted_orig[i] / g.n_per_conf : 0;
+    // a periodic batch (modes 2, 3) keeps one set of slots per conformer: the conformer of the central atom
+    const int conf = LAT ? conf_i : g.mode == 2 ? sorted_orig[i] / g.n_per_conf : 0;
     double* slots = virial + (size_t)conf * ANI_VIRIAL_SLOTS * 9;
 #pragma unroll
     for (int k = 0; k < 9; ++k) {
@@ -1451,7 +1460,8 @@ static int launch_aev_forward(const ani_aev_params* params, const ani_grid* grid
                               const float* spos, const int32_t* sbin, const float* bucket_ranges,
                               const int32_t* bucket_species, const int32_t* species_mask, ExplicitNbrs ex, int n, int lo, int hi,
                               const int32_t* row_of, float* aev, int ldx, int layout, int32_t* nbr_cnt,
-                              int32_t* nbr_list, int nbr_cap, int32_t* status, void* stream) {
+                              int32_t* nbr_list, int nbr_cap, int32_t* status, void* stream,
+                              const float* lattice = nullptr) {
   int rc = check_params(params);
   if (rc != ANI_OK) return rc;
   if (!grid || !spos || !row_of || !aev || !status) return ANI_ERR_BAD_ARG;
@@ -1491,9 +1501,21 @@ static int launch_aev_forward(const ani_aev_params* params, const ani_grid* grid
       cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_f);
       k<<<blocks_f, AEV_FWD_WARPS * 32, smem_f, st>>>(*params, grid, bin_start, sp4, sbin, rng4, species_mask, lo, hi,
                                                       row_of, aev, ldx, layout, nbr_cnt, nbr_list, nbr_cap, status, wb,
-                                                      tma_stage, bucket_species);
+                                                      tma_stage, bucket_species, lattice);
     };
-    if (params->n_shf_a == 8) {
+    if (lattice) {   // grid mode 3
+      if (params->n_shf_a == 8) {
+        if (tma_stage)
+          go(k_aev_forward_cta<8, 4, true, true>);
+        else
+          go(k_aev_forward_cta<8, 4, false, true>);
+      } else {
+        if (tma_stage)
+          go(k_aev_forward_cta<4, 8, true, true>);
+        else
+          go(k_aev_forward_cta<4, 8, false, true>);
+      }
+    } else if (params->n_shf_a == 8) {
       if (tma_stage)
         go(k_aev_forward_cta<8, 4, true>);
       else
@@ -1507,16 +1529,21 @@ static int launch_aev_forward(const ani_aev_params* params, const ani_grid* grid
     ANI_CUDA_CHECK_LAUNCH();
     return ANI_OK;
   }
+  auto go = [&](auto k) {
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    k<<<blocks, AEV_WARPS * 32, smem, st>>>(*params, grid, bin_start, sp4, sbin, rng4, species_mask, ex, lo, hi, row_of,
+                                            aev, ldx, layout, nbr_cnt, nbr_list, nbr_cap, status, wb, lattice);
+  };
   if (params->n_shf_a == 8) {
-    auto k = k_aev_forward<8, 4>;
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k<<<blocks, AEV_WARPS * 32, smem, st>>>(*params, grid, bin_start, sp4, sbin, rng4, species_mask, ex, lo, hi, row_of,
-                                            aev, ldx, layout, nbr_cnt, nbr_list, nbr_cap, status, wb);
+    if (lattice)
+      go(k_aev_forward<8, 4, true>);
+    else
+      go(k_aev_forward<8, 4>);
   } else {
-    auto k = k_aev_forward<4, 8>;
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k<<<blocks, AEV_WARPS * 32, smem, st>>>(*params, grid, bin_start, sp4, sbin, rng4, species_mask, ex, lo, hi, row_of,
-                                            aev, ldx, layout, nbr_cnt, nbr_list, nbr_cap, status, wb);
+    if (lattice)
+      go(k_aev_forward<4, 8, true>);
+    else
+      go(k_aev_forward<4, 8>);
   }
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
@@ -1526,7 +1553,8 @@ static int launch_aev_backward(const ani_aev_params* params, const ani_grid* gri
                                const int32_t* sorted_orig, int n, int lo, int hi, const int32_t* row_of,
                                const float* grad_aev, int ldx, const int32_t* nbr_cnt, const int32_t* nbr_list,
                                ExplicitNbrs ex, const int32_t* species_mask, int nbr_cap, float* grad_coords,
-                               int32_t* status, void* stream, int max_elements = 0, double* virial = nullptr) {
+                               int32_t* status, void* stream, int max_elements = 0, double* virial = nullptr,
+                               const float* lattice = nullptr) {
   int rc = check_params(params);
   if (rc != ANI_OK) return rc;
   if (!grid || !spos || !sorted_orig || !row_of || !grad_aev || !grad_coords || !status) return ANI_ERR_BAD_ARG;
@@ -1554,9 +1582,21 @@ static int launch_aev_backward(const ani_aev_params* params, const ani_grid* gri
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k<<<blocks, AEV_WARPS * 32, smem, st>>>(*params, grid, sp4, sorted_orig, lo, hi, row_of, grad_aev, ldx, nbr_cnt,
                                             nbr_list, ex, species_mask, nbr_cap, grad_coords, status, wb, pair_cap,
-                                            virial);
+                                            virial, lattice);
   };
-  if (params->n_shf_a == 8) {
+  if (lattice) {   // grid mode 3
+    if (params->n_shf_a == 8) {
+      if (virial)
+        go(k_aev_backward<8, 4, true, true>);
+      else
+        go(k_aev_backward<8, 4, false, true>);
+    } else {
+      if (virial)
+        go(k_aev_backward<4, 8, true, true>);
+      else
+        go(k_aev_backward<4, 8, false, true>);
+    }
+  } else if (params->n_shf_a == 8) {
     if (virial)
       go(k_aev_backward<8, 4, true>);
     else
@@ -1666,6 +1706,34 @@ extern "C" int ani_b200_aev_backward(const ani_aev_params* params, const ani_gri
   return launch_aev_backward(params, grid, spos, sorted_orig, n, lo, hi, row_of, grad_aev, ldx, nbr_cnt, nbr_list,
                              ExplicitNbrs{nullptr, nullptr, nullptr}, species_mask, nbr_cap, grad_coords, status,
                              stream, max_elements, virial);
+}
+
+// grid mode 3 (ani_b200_prepare_step_cells): the same kernels, image shifts from the lattice table
+extern "C" int ani_b200_aev_forward_cells(const ani_aev_params* params, const ani_grid* grid, const int32_t* bin_start,
+                                          const float* spos, const int32_t* sbin, const float* bucket_ranges,
+                                          const int32_t* bucket_species, const int32_t* species_mask, int n, int lo,
+                                          int hi, const int32_t* row_of, float* aev, int ldx, int layout,
+                                          int32_t* nbr_cnt, int32_t* nbr_list, int nbr_cap, int32_t* status,
+                                          const float* lattice, void* stream) {
+  int rc = check_params(params);
+  if (rc != ANI_OK) return rc;
+  if (!bin_start || !sbin || !nbr_cnt || !nbr_list || !lattice) return ANI_ERR_BAD_ARG;
+  return launch_aev_forward(params, grid, bin_start, spos, sbin, bucket_ranges, bucket_ranges ? bucket_species : nullptr,
+                            species_mask, ExplicitNbrs{nullptr, nullptr, nullptr}, n, lo, hi, row_of, aev, ldx, layout, nbr_cnt,
+                            nbr_list, nbr_cap, status, stream, lattice);
+}
+
+extern "C" int ani_b200_aev_backward_cells(const ani_aev_params* params, const ani_grid* grid, const float* spos,
+                                           const int32_t* sorted_orig, const int32_t* species_mask, int n, int lo, int hi,
+                                           const int32_t* row_of, const float* grad_aev, int ldx, const int32_t* nbr_cnt,
+                                           const int32_t* nbr_list, int nbr_cap, float* grad_coords, int32_t* status,
+                                           int max_elements, double* virial, const float* lattice, void* stream) {
+  int rc = check_params(params);
+  if (rc != ANI_OK) return rc;
+  if (!nbr_cnt || !nbr_list || !lattice) return ANI_ERR_BAD_ARG;
+  return launch_aev_backward(params, grid, spos, sorted_orig, n, lo, hi, row_of, grad_aev, ldx, nbr_cnt, nbr_list,
+                             ExplicitNbrs{nullptr, nullptr, nullptr}, species_mask, nbr_cap, grad_coords, status,
+                             stream, max_elements, virial, lattice);
 }
 
 extern "C" int ani_b200_pairs_to_rows(const int64_t* idx0, const int64_t* idx1, const float* diff_vectors,

@@ -7,12 +7,47 @@
 
 namespace ani {
 
+// inverse of the 3x3 cell in double (host-quality), rows of `cell` are lattice vectors
+__device__ __forceinline__ void cell_inverse(const float* __restrict__ cell, double (&iv)[9]) {
+  double c[9];
+  for (int k = 0; k < 9; ++k) c[k] = (double)cell[k];
+  double det = c[0] * (c[4] * c[8] - c[5] * c[7]) - c[1] * (c[3] * c[8] - c[5] * c[6]) +
+               c[2] * (c[3] * c[7] - c[4] * c[6]);
+  double id = 1.0 / det;
+  iv[0] = (c[4] * c[8] - c[5] * c[7]) * id;
+  iv[1] = (c[2] * c[7] - c[1] * c[8]) * id;
+  iv[2] = (c[1] * c[5] - c[2] * c[4]) * id;
+  iv[3] = (c[5] * c[6] - c[3] * c[8]) * id;
+  iv[4] = (c[0] * c[8] - c[2] * c[6]) * id;
+  iv[5] = (c[2] * c[3] - c[0] * c[5]) * id;
+  iv[6] = (c[3] * c[7] - c[4] * c[6]) * id;
+  iv[7] = (c[1] * c[6] - c[0] * c[7]) * id;
+  iv[8] = (c[0] * c[4] - c[1] * c[3]) * id;
+}
+
+// buckets along lattice direction d: frac_d = r . inv[:, d]; planes frac_d = const are 1/|inv[:, d]| apart
+__device__ __forceinline__ int cell_buckets(const double (&iv)[9], int d, float bucket) {
+  double w = 1.0 / sqrt(iv[d] * iv[d] + iv[3 + d] * iv[3 + d] + iv[6 + d] * iv[6 + d]);
+  return (int)floor(w / (double)bucket);
+}
+
+// respect the caller's bucket capacity (buckets may only get larger than the cutoff)
+__device__ __forceinline__ void cap_dims(ani_grid& g, int cap) {
+  while ((long long)g.dims[0] * g.dims[1] * g.dims[2] > (long long)cap) {
+    int big = 0;
+    if (g.dims[1] > g.dims[big]) big = 1;
+    if (g.dims[2] > g.dims[big]) big = 2;
+    g.dims[big] = max(1, g.dims[big] - max(1, g.dims[big] / 8));
+  }
+}
+
 // The grid of one call (executed by one thread).  mode 0 + pbc: buckets from the perpendicular
 // widths of the cell (>= 1 bucket per cutoff, neighbors.py:618-662 uses edge lengths; widths are
 // the safe choice for triclinic cells).  mode 0 without pbc: bounding box of the real atoms.
 // mode 2 (a periodic batch in one shared cell): every conformer gets the sub-grid a single system in
 // that cell would get from a 1 / n_conf share of the bucket capacity; dims are per conformer, nbins
 // counts the buckets of all of them (conformer-major: bucket c * nb + local).
+// (mode 3, one cell per conformer, needs every conformer's cell: conformer_lattices below)
 __device__ ani_grid compute_grid(int n_conf, int n_per_conf, const float* __restrict__ cell, int pbc, int mode,
                                  float cutoff, int max_bins, const float* box_min, const float* box_max,
                                  int32_t* __restrict__ status) {
@@ -31,30 +66,14 @@ __device__ ani_grid compute_grid(int n_conf, int n_per_conf, const float* __rest
     g.inv[0] = g.inv[4] = g.inv[8] = 1.f;
   } else {
     if (pbc) {
-      // inverse of the 3x3 cell in double (host-quality), rows of `cell` are lattice vectors
-      double c[9];
-      for (int k = 0; k < 9; ++k) c[k] = (double)cell[k];
-      double det = c[0] * (c[4] * c[8] - c[5] * c[7]) - c[1] * (c[3] * c[8] - c[5] * c[6]) +
-                   c[2] * (c[3] * c[7] - c[4] * c[6]);
-      double id = 1.0 / det;
       double iv[9];
-      iv[0] = (c[4] * c[8] - c[5] * c[7]) * id;
-      iv[1] = (c[2] * c[7] - c[1] * c[8]) * id;
-      iv[2] = (c[1] * c[5] - c[2] * c[4]) * id;
-      iv[3] = (c[5] * c[6] - c[3] * c[8]) * id;
-      iv[4] = (c[0] * c[8] - c[2] * c[6]) * id;
-      iv[5] = (c[2] * c[3] - c[0] * c[5]) * id;
-      iv[6] = (c[3] * c[7] - c[4] * c[6]) * id;
-      iv[7] = (c[1] * c[6] - c[0] * c[7]) * id;
-      iv[8] = (c[0] * c[4] - c[1] * c[3]) * id;
+      cell_inverse(cell, iv);
       for (int k = 0; k < 9; ++k) {
         g.cell[k] = cell[k];
         g.inv[k] = (float)iv[k];
       }
       for (int d = 0; d < 3; ++d) {
-        // frac_d = r . inv[:, d]; planes frac_d = const are 1/|inv[:, d]| apart
-        double w = 1.0 / sqrt(iv[d] * iv[d] + iv[3 + d] * iv[3 + d] + iv[6 + d] * iv[6 + d]);
-        int nd = (int)floor(w / (double)bucket);
+        int nd = cell_buckets(iv, d, bucket);
         if (nd < 1) {
           atomicOr(status, ANI_STATUS_CELL_TOO_SMALL);
           nd = 1;
@@ -75,18 +94,84 @@ __device__ ani_grid compute_grid(int n_conf, int n_per_conf, const float* __rest
         g.dims[d] = nd < 1 ? 1 : nd;
       }
     }
-    // respect the caller's bucket capacity (buckets may only get larger than the cutoff)
     const int n_sub = mode == 2 ? n_conf : 1;
-    int cap = (max_bins - 1) / n_sub;
-    while ((long long)g.dims[0] * g.dims[1] * g.dims[2] > (long long)cap) {
-      int big = 0;
-      if (g.dims[1] > g.dims[big]) big = 1;
-      if (g.dims[2] > g.dims[big]) big = 2;
-      g.dims[big] = max(1, g.dims[big] - max(1, g.dims[big] / 8));
-    }
+    cap_dims(g, (max_bins - 1) / n_sub);
     g.nbins = g.dims[0] * g.dims[1] * g.dims[2] * n_sub;
   }
   return g;
+}
+
+// Grid mode 3 (a periodic batch with one cell per conformer), executed by ALL threads of one CTA: thread t inverts
+// the cells of conformers t, t + blockDim.x, ... (in double, as compute_grid) and writes their rows of the lattice
+// table {cell[9], inverse[9]}; the sub-grid dims common to all conformers are, per axis, the minimum over the
+// conformers of the buckets their own cell admits, capped like mode 2.  With C equal cells this is the mode 2 grid.
+// Thread 0 gets the grid (cell / inv: those of conformer 0).
+__device__ void conformer_lattices(int n_conf, int n_per_conf, const float* __restrict__ cells, float cutoff,
+                                   int max_bins, float* __restrict__ lattice, int32_t* __restrict__ status,
+                                   ani_grid& out) {
+  __shared__ int s_dims[3];
+  if (threadIdx.x < 3) s_dims[threadIdx.x] = 0x7fffffff;
+  __syncthreads();
+  const float bucket = cutoff + 1e-5f;
+  int nd_min[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff};
+  for (int c = threadIdx.x; c < n_conf; c += blockDim.x) {
+    const float* cell = cells + 9 * (size_t)c;
+    double iv[9];
+    cell_inverse(cell, iv);
+    float* L = lattice + (size_t)c * ANI_LATTICE_STRIDE;
+    for (int k = 0; k < 9; ++k) {
+      L[k] = cell[k];
+      L[9 + k] = (float)iv[k];
+    }
+    for (int d = 0; d < 3; ++d) {
+      int nd = cell_buckets(iv, d, bucket);
+      if (nd < 1) {
+        atomicOr(status, ANI_STATUS_CELL_TOO_SMALL);
+        nd = 1;
+      }
+      nd_min[d] = min(nd_min[d], nd);
+    }
+  }
+  for (int d = 0; d < 3; ++d) atomicMin(&s_dims[d], nd_min[d]);
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  ani_grid g;
+  for (int k = 0; k < 9; ++k) {
+    g.cell[k] = lattice[k];   // written by this thread above
+    g.inv[k] = lattice[9 + k];
+  }
+  g.origin[0] = g.origin[1] = g.origin[2] = 0.f;
+  for (int d = 0; d < 3; ++d) g.dims[d] = s_dims[d];
+  g.pbc = 1;
+  g.mode = 3;
+  g.n_per_conf = n_per_conf;
+  g.n_real = 0;
+  cap_dims(g, (max_bins - 1) / n_conf);
+  g.nbins = g.dims[0] * g.dims[1] * g.dims[2] * n_conf;
+  out = g;
+}
+
+// the cell (and its inverse) of conformer `conf`: with LAT (grid mode 3) its row of the lattice table, written in
+// the same launch by another CTA (hence the L2 loads), else the grid's own
+template <bool LAT>
+__device__ __forceinline__ void cell_of(const ani_grid& g, const float* __restrict__ lattice, int conf, float (&cl)[9]) {
+#pragma unroll
+  for (int k = 0; k < 9; ++k) cl[k] = LAT ? __ldcg(lattice + (size_t)conf * ANI_LATTICE_STRIDE + k) : g.cell[k];
+}
+
+template <bool LAT>
+__device__ __forceinline__ void inv_of(const ani_grid& g, const float* __restrict__ lattice, int conf, float (&inv)[9]) {
+#pragma unroll
+  for (int k = 0; k < 9; ++k) inv[k] = LAT ? __ldcg(lattice + (size_t)conf * ANI_LATTICE_STRIDE + 9 + k) : g.inv[k];
+}
+
+// one CTA: the lattice table and the grid of a mode 3 preparation in the five-launch form
+__global__ void k_lattice_setup(int n_conf, int n_per_conf, const float* __restrict__ cells, float cutoff,
+                                int max_bins, float* __restrict__ lattice, ani_grid* __restrict__ grid,
+                                int32_t* __restrict__ status) {
+  ani_grid g;
+  conformer_lattices(n_conf, n_per_conf, cells, cutoff, max_bins, lattice, status, g);
+  if (threadIdx.x == 0) *grid = g;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -137,19 +222,24 @@ __global__ void k_grid_setup(const float* __restrict__ coords, const int32_t* __
   *grid = compute_grid(n_conf, n_per_conf, cell, pbc, mode, cutoff, max_bins, mn, mx, status);
 }
 
+// LAT (grid mode 3): wrap with the lattice of the atom's own conformer, from the lattice table
+template <bool LAT = false>
 __device__ __forceinline__ void wrapped_position(const ani_grid& g, const float* __restrict__ coords, int a,
-                                                 float3& pos, int& bin) {
+                                                 float3& pos, int& bin, const float* __restrict__ lattice = nullptr) {
   float x = coords[3 * a], y = coords[3 * a + 1], z = coords[3 * a + 2];
-  if (g.mode == 1) {
+  if (!LAT && g.mode == 1) {
     pos = make_float3(x, y, z);
     bin = a / g.n_per_conf;
     return;
   }
+  float cl[9], inv[9];
+  cell_of<LAT>(g, lattice, LAT ? a / g.n_per_conf : 0, cl);
+  inv_of<LAT>(g, lattice, LAT ? a / g.n_per_conf : 0, inv);
   float rx = x - g.origin[0], ry = y - g.origin[1], rz = z - g.origin[2];
   float f[3];
-  f[0] = rx * g.inv[0] + ry * g.inv[3] + rz * g.inv[6];
-  f[1] = rx * g.inv[1] + ry * g.inv[4] + rz * g.inv[7];
-  f[2] = rx * g.inv[2] + ry * g.inv[5] + rz * g.inv[8];
+  f[0] = rx * inv[0] + ry * inv[3] + rz * inv[6];
+  f[1] = rx * inv[1] + ry * inv[4] + rz * inv[7];
+  f[2] = rx * inv[2] + ry * inv[5] + rz * inv[8];
   int idx[3];
   float k[3] = {0.f, 0.f, 0.f};
 #pragma unroll
@@ -164,11 +254,11 @@ __device__ __forceinline__ void wrapped_position(const ani_grid& g, const float*
   // Subtract whole lattice vectors from the input position instead of rebuilding it from the
   // fractional coordinates: atoms already inside the cell keep their exact float32 position
   // (the reference's frac @ cell round trip costs ~1e-7 * |cell| of absolute accuracy).
-  pos.x = x - (k[0] * g.cell[0] + k[1] * g.cell[3] + k[2] * g.cell[6]);
-  pos.y = y - (k[0] * g.cell[1] + k[1] * g.cell[4] + k[2] * g.cell[7]);
-  pos.z = z - (k[0] * g.cell[2] + k[1] * g.cell[5] + k[2] * g.cell[8]);
+  pos.x = x - (k[0] * cl[0] + k[1] * cl[3] + k[2] * cl[6]);
+  pos.y = y - (k[0] * cl[1] + k[1] * cl[4] + k[2] * cl[7]);
+  pos.z = z - (k[0] * cl[2] + k[1] * cl[5] + k[2] * cl[8]);
   bin = (idx[0] * g.dims[1] + idx[1]) * g.dims[2] + idx[2];
-  if (g.mode == 2) bin += (a / g.n_per_conf) * (g.dims[0] * g.dims[1] * g.dims[2]);  // the conformer's sub-grid
+  if (LAT || g.mode == 2) bin += (a / g.n_per_conf) * (g.dims[0] * g.dims[1] * g.dims[2]);  // the conformer's sub-grid
 }
 
 __global__ void k_bin_assign(const float* __restrict__ coords, const int32_t* __restrict__ species, int n,
@@ -521,6 +611,7 @@ struct PrepArgs {
   int32_t* status;
   int32_t* bss;  // [nbins][8] or nullptr: offset inside bucket b of its first atom of species >= s (buckets are species-sorted)
   unsigned long long* trace;  // timing experiments (ANI_B200_PREP_TRACE=1): %globaltimer at the phase boundaries of k_prep_cluster
+  float* lattice;  // grid mode 3: [n_conf][ANI_LATTICE_STRIDE] {cell, inverse} per conformer (written by the preparation)
 };
 
 // per-bucket species offsets: bss[b][s] = atoms of bucket b with species < s (s = 0..7; bss[b][0] = 0).  With the
@@ -547,6 +638,8 @@ __device__ __forceinline__ void bucket_species_offsets(const PrepArgs& A, int b)
   dst[1] = make_int4(off[4], off[5], off[6], off[7]);
 }
 
+// LAT: grid mode 3 (the grid and the lattice table come from k_lattice_setup, A.inline_setup == 0)
+template <bool LAT = false>
 __global__ void __launch_bounds__(256) k_prep_assign(const __grid_constant__ PrepArgs A) {
   __shared__ ani_grid sg;
   __shared__ bool s_last;
@@ -570,7 +663,7 @@ __global__ void __launch_bounds__(256) k_prep_assign(const __grid_constant__ Pre
       bin = sg.nbins;  // padding atoms: trash bucket, never a neighbour, never a centre
     } else {
       float3 p;
-      wrapped_position(sg, A.coords, a, p, bin);
+      wrapped_position<LAT>(sg, A.coords, a, p, bin, A.lattice);
     }
     A.bin_of[a] = bin;
     A.slot[a] = atomicAdd(&A.bin_count[bin], 1);
@@ -619,6 +712,7 @@ __global__ void __launch_bounds__(256) k_prep_assign(const __grid_constant__ Pre
   }
 }
 
+template <bool LAT = false>
 __global__ void __launch_bounds__(256) k_prep_scatter(const __grid_constant__ PrepArgs A) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx < A.n) A.tmp_list[A.bin_start[A.bin_of[idx]] + A.slot[idx]] = idx;
@@ -651,12 +745,15 @@ __global__ void __launch_bounds__(256) k_prep_scatter(const __grid_constant__ Pr
   }
   const float wx = (float)w[0], wy = (float)w[1], wz = (float)w[2];
   const int nbk = exists ? base + (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2] : 0;
+  float cl[9];   // the image shift in the lattice of the bucket's conformer
+  cell_of<LAT>(g, A.lattice, LAT ? base / (g.dims[0] * g.dims[1] * g.dims[2]) : 0, cl);
   A.ranges[2 * (size_t)idx] = make_float4(__int_as_float(lo), __int_as_float(hi), __int_as_float(code), __int_as_float(nbk));
-  A.ranges[2 * (size_t)idx + 1] = make_float4(wx * g.cell[0] + wy * g.cell[3] + wz * g.cell[6],
-                                              wx * g.cell[1] + wy * g.cell[4] + wz * g.cell[7],
-                                              wx * g.cell[2] + wy * g.cell[5] + wz * g.cell[8], 0.f);
+  A.ranges[2 * (size_t)idx + 1] = make_float4(wx * cl[0] + wy * cl[3] + wz * cl[6],
+                                              wx * cl[1] + wy * cl[4] + wz * cl[7],
+                                              wx * cl[2] + wy * cl[5] + wz * cl[8], 0.f);
 }
 
+template <bool LAT = false>
 __global__ void __launch_bounds__(256) k_prep_finalize(const __grid_constant__ PrepArgs A) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   const ani_grid g = *A.grid;
@@ -686,7 +783,7 @@ __global__ void __launch_bounds__(256) k_prep_finalize(const __grid_constant__ P
     sp = A.species[a];
     if (sp >= 0) {
       int bb;
-      wrapped_position(g, A.coords, a, p, bb);
+      wrapped_position<LAT>(g, A.coords, a, p, bb, A.lattice);
     }
     A.spos[i] = make_float4(p.x, p.y, p.z, __int_as_float(sp));
     // species histogram of the owned slice, per 256-atom chunk of the SORTED order
@@ -813,6 +910,9 @@ __device__ __forceinline__ void grid_barrier(int32_t* bar, int32_t* status) {
   __syncthreads();
 }
 
+// LAT: grid mode 3 -- block 0 builds the lattice table and the grid in phase 0, the other blocks read the grid after
+// the first barrier
+template <bool LAT = false>
 __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ PrepArgs A, int32_t* bar, int zeroed) {
   __shared__ ani_grid sg;
   __shared__ int s_warp[8];
@@ -825,7 +925,12 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
   const int gstride = gridDim.x * blockDim.x, gtid = blockIdx.x * blockDim.x + tid;
   const int n = A.n, S = A.S;
   // ---- phase 0: the grid (every block computes its own copy) + zero-fill of the counters
-  if (tid == 0) {
+  if (LAT) {
+    if (blockIdx.x == 0) {
+      conformer_lattices(A.n_conf, A.n_per_conf, A.cell, A.cutoff, A.max_bins, A.lattice, A.status, sg);
+      if (tid == 0) *A.grid = sg;
+    }
+  } else if (tid == 0) {
     if (A.inline_setup) {
       const float none[3] = {0.f, 0.f, 0.f};
       sg = compute_grid(A.n_conf, A.n_per_conf, A.cell, A.pbc, A.mode, A.cutoff, A.max_bins, none, none, A.status);
@@ -836,6 +941,11 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
   }
   for (int k = gtid; k < zeroed; k += gstride) A.bin_count[k] = 0;
   grid_barrier(bar, A.status);
+  if (LAT && blockIdx.x != 0) {
+    if (tid < (int)(sizeof(ani_grid) / 4))
+      reinterpret_cast<int*>(&sg)[tid] = __ldcg(reinterpret_cast<const int*>(A.grid) + tid);
+    __syncthreads();
+  }
   // ---- phase 1: bucket of every atom, slot inside the bucket by atomics
   for (int a = gtid; a < n; a += gstride) {
     int bin;
@@ -843,7 +953,7 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
       bin = sg.nbins;  // padding atoms: trash bucket, never a neighbour, never a centre
     } else {
       float3 p;
-      wrapped_position(sg, A.coords, a, p, bin);
+      wrapped_position<LAT>(sg, A.coords, a, p, bin, A.lattice);
     }
     A.bin_of[a] = bin;
     A.slot[a] = atomicAdd(&A.bin_count[bin], 1);
@@ -920,11 +1030,13 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
       }
       const float wx = (float)wv[0], wy = (float)wv[1], wz = (float)wv[2];
       const int nbk = exists ? base + (j[0] * sg.dims[1] + j[1]) * sg.dims[2] + j[2] : 0;
+      float cl[9];   // the image shift in the lattice of the bucket's conformer
+      cell_of<LAT>(sg, A.lattice, LAT ? base / (sg.dims[0] * sg.dims[1] * sg.dims[2]) : 0, cl);
       A.ranges[2 * (size_t)idx] =
           make_float4(__int_as_float(lo), __int_as_float(hi), __int_as_float(code), __int_as_float(nbk));
-      A.ranges[2 * (size_t)idx + 1] = make_float4(wx * sg.cell[0] + wy * sg.cell[3] + wz * sg.cell[6],
-                                                  wx * sg.cell[1] + wy * sg.cell[4] + wz * sg.cell[7],
-                                                  wx * sg.cell[2] + wy * sg.cell[5] + wz * sg.cell[8], 0.f);
+      A.ranges[2 * (size_t)idx + 1] = make_float4(wx * cl[0] + wy * cl[3] + wz * cl[6],
+                                                  wx * cl[1] + wy * cl[4] + wz * cl[7],
+                                                  wx * cl[2] + wy * cl[5] + wz * cl[8], 0.f);
     }
   }
   grid_barrier(bar, A.status);
@@ -958,7 +1070,7 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
         sp = spa;
         if (sp >= 0) {
           int bb;
-          wrapped_position(sg, A.coords, a, p, bb);
+          wrapped_position<LAT>(sg, A.coords, a, p, bb, A.lattice);
         }
         A.spos[i] = make_float4(p.x, p.y, p.z, __int_as_float(sp));
         if (sp >= 0 && i >= A.lo && i < hi_real)
@@ -1499,6 +1611,7 @@ extern "C" int ani_b200_build_cells(const float* coords, const int32_t* species,
   if (mode == 0 && n_conf != 1) return ANI_ERR_UNSUPPORTED;
   if (mode == 1 && (pbc || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
   if (mode == 2 && (!pbc || !cell || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
+  if (mode == 3) return ANI_ERR_UNSUPPORTED;   // one cell per conformer: ani_b200_prepare_step_cells only
   if (mode < 0 || mode > 2) return ANI_ERR_BAD_ARG;
   if (pbc && !cell) return ANI_ERR_BAD_ARG;
   const long long n_ll = (long long)n_conf * n_per_conf;
@@ -1568,16 +1681,15 @@ extern "C" int ani_b200_verlet_positions(int mode, const float* coords, const an
   return ANI_OK;
 }
 
-extern "C" int ani_b200_prepare_step(const float* coords, const int32_t* species, int n_conf, int n_per_conf,
-                                     const float* cell, int pbc, int mode, float cutoff, int max_bins,
-                                     ani_grid* grid, int32_t* bin_start, int32_t* sorted_orig,
-                                     int32_t* orig_to_sorted, float* spos, int32_t* sbin, float* bucket_ranges,
-                                     int lo, int hi, int num_species, int rows_cap, int32_t* row_of,
-                                     int32_t* row_atom, int32_t* tile_species, int32_t* layout_info, int n_shf_r,
-                                     int angular_sub, int out_dim, int ldx, int ang_pad, int32_t* aev_blocks,
-                                     float* zero_f32,
-                                     int zero_f32_count, double* zero_f64, int zero_f64_count,
-                                     int32_t* bucket_species, int32_t* scratch_i32, int32_t* status, void* stream) {
+// ani_b200_prepare_step and ani_b200_prepare_step_cells (lattice: the table of grid mode 3, NULL otherwise)
+static int prepare_step(const float* coords, const int32_t* species, int n_conf, int n_per_conf, const float* cell,
+                        int pbc, int mode, float cutoff, int max_bins, ani_grid* grid, int32_t* bin_start,
+                        int32_t* sorted_orig, int32_t* orig_to_sorted, float* spos, int32_t* sbin, float* bucket_ranges,
+                        int lo, int hi, int num_species, int rows_cap, int32_t* row_of, int32_t* row_atom,
+                        int32_t* tile_species, int32_t* layout_info, int n_shf_r, int angular_sub, int out_dim, int ldx,
+                        int ang_pad, int32_t* aev_blocks, float* zero_f32, int zero_f32_count, double* zero_f64,
+                        int zero_f64_count, int32_t* bucket_species, int32_t* scratch_i32, int32_t* status,
+                        float* lattice, void* stream) {
   if (!coords || !species || !grid || !bin_start || !sorted_orig || !orig_to_sorted || !spos || !sbin ||
       !row_of || !row_atom || !tile_species || !layout_info || !aev_blocks || !scratch_i32 || !status)
     return ANI_ERR_BAD_ARG;
@@ -1585,7 +1697,8 @@ extern "C" int ani_b200_prepare_step(const float* coords, const int32_t* species
   if (mode == 0 && n_conf != 1) return ANI_ERR_UNSUPPORTED;
   if (mode == 1 && (pbc || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
   if (mode == 2 && (!pbc || !cell || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
-  if (mode < 0 || mode > 2) return ANI_ERR_BAD_ARG;
+  if (mode == 3 && (!pbc || !cell || !lattice || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
+  if (mode < 0 || mode > 3) return ANI_ERR_BAD_ARG;
   if (pbc && !cell) return ANI_ERR_BAD_ARG;
   const long long n_ll = (long long)n_conf * n_per_conf;
   if (n_ll >= (1ll << ANI_IMG_SHIFT)) return ANI_ERR_UNSUPPORTED;
@@ -1627,9 +1740,12 @@ extern "C" int ani_b200_prepare_step(const float* coords, const int32_t* species
                   ? reinterpret_cast<unsigned long long*>((reinterpret_cast<uintptr_t>(A.species_base + ANI_MAX_SPECIES) + 7) & ~(uintptr_t)7)
                   : nullptr;
   }
-  A.inline_setup = (mode == 1 || pbc) ? 1 : 0;
+  A.lattice = lattice;
+  const bool lat = mode == 3;
+  // (mode 3: the grid comes from k_lattice_setup / block 0 of the persistent grid)
+  A.inline_setup = ((mode == 1 || pbc) && !lat) ? 1 : 0;
   const size_t zeroed = (size_t)(max_bins + 1) + 2 + (size_t)(A.n_chunks + 1) * ANI_MAX_SPECIES;
-  if (!A.inline_setup)
+  if (!A.inline_setup && !lat)
     k_grid_setup<<<1, 1024, 0, st>>>(coords, species, n, n_conf, n_per_conf, cell, pbc, mode, cutoff, max_bins,
                                      grid, status);
   const int nb = (n + 255) / 256;
@@ -1696,17 +1812,63 @@ extern "C" int ani_b200_prepare_step(const float* coords, const int32_t* species
     // 2 blocks of 256 threads per SM at most (the kernel allows far more)
     int32_t* bar = grid_bar;
     const int blocks = min(2 * num_sms, max(1, nb));
-    k_prep_fused<<<blocks, 256, 0, st>>>(A, bar, (int)zeroed);
+    if (lat)
+      k_prep_fused<true><<<blocks, 256, 0, st>>>(A, bar, (int)zeroed);
+    else
+      k_prep_fused<<<blocks, 256, 0, st>>>(A, bar, (int)zeroed);
   } else {
     cudaMemsetAsync(A.bin_count, 0, sizeof(int32_t) * zeroed, st);
-    k_prep_assign<<<nb, 256, 0, st>>>(A);
     const long long t2 = A.ranges ? max((long long)n, (long long)(max_bins - 1) * 27) : (long long)n;
-    k_prep_scatter<<<(int)((t2 + 255) / 256), 256, 0, st>>>(A);
-    k_prep_finalize<<<nb, 256, 0, st>>>(A);
+    if (lat) {
+      k_lattice_setup<<<1, 256, 0, st>>>(n_conf, n_per_conf, cell, cutoff, max_bins, lattice, grid, status);
+      k_prep_assign<true><<<nb, 256, 0, st>>>(A);
+      k_prep_scatter<true><<<(int)((t2 + 255) / 256), 256, 0, st>>>(A);
+      k_prep_finalize<true><<<nb, 256, 0, st>>>(A);
+    } else {
+      k_prep_assign<<<nb, 256, 0, st>>>(A);
+      k_prep_scatter<<<(int)((t2 + 255) / 256), 256, 0, st>>>(A);
+      k_prep_finalize<<<nb, 256, 0, st>>>(A);
+    }
     k_prep_layout<<<1, 1024, 0, st>>>(A);
     k_layout_assign<<<A.n_chunks, LAYOUT_CHUNK, 0, st>>>(A.spos, grid, lo, hi, num_species, A.chunk_hist, A.species_base,
                                                         row_of, row_atom);
   }
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
+}
+
+extern "C" int ani_b200_prepare_step(const float* coords, const int32_t* species, int n_conf, int n_per_conf,
+                                     const float* cell, int pbc, int mode, float cutoff, int max_bins,
+                                     ani_grid* grid, int32_t* bin_start, int32_t* sorted_orig,
+                                     int32_t* orig_to_sorted, float* spos, int32_t* sbin, float* bucket_ranges,
+                                     int lo, int hi, int num_species, int rows_cap, int32_t* row_of,
+                                     int32_t* row_atom, int32_t* tile_species, int32_t* layout_info, int n_shf_r,
+                                     int angular_sub, int out_dim, int ldx, int ang_pad, int32_t* aev_blocks,
+                                     float* zero_f32,
+                                     int zero_f32_count, double* zero_f64, int zero_f64_count,
+                                     int32_t* bucket_species, int32_t* scratch_i32, int32_t* status, void* stream) {
+  return prepare_step(coords, species, n_conf, n_per_conf, cell, pbc, mode, cutoff, max_bins, grid, bin_start,
+                           sorted_orig, orig_to_sorted, spos, sbin, bucket_ranges, lo, hi, num_species, rows_cap, row_of,
+                           row_atom, tile_species, layout_info, n_shf_r, angular_sub, out_dim, ldx, ang_pad, aev_blocks,
+                           zero_f32, zero_f32_count, zero_f64, zero_f64_count, bucket_species, scratch_i32, status,
+                           nullptr, stream);
+}
+
+extern "C" int ani_b200_prepare_step_cells(const float* coords, const int32_t* species, int n_conf, int n_per_conf,
+                                           const float* cell, int pbc, int mode, float cutoff, int max_bins,
+                                           ani_grid* grid, int32_t* bin_start, int32_t* sorted_orig,
+                                           int32_t* orig_to_sorted, float* spos, int32_t* sbin, float* bucket_ranges,
+                                           int lo, int hi, int num_species, int rows_cap, int32_t* row_of,
+                                           int32_t* row_atom, int32_t* tile_species, int32_t* layout_info, int n_shf_r,
+                                           int angular_sub, int out_dim, int ldx, int ang_pad, int32_t* aev_blocks,
+                                           float* zero_f32, int zero_f32_count, double* zero_f64, int zero_f64_count,
+                                           int32_t* bucket_species, int32_t* scratch_i32, int32_t* status,
+                                           float* lattice, void* stream) {
+  if (!lattice) return ANI_ERR_BAD_ARG;
+  if (mode != 3) return ANI_ERR_UNSUPPORTED;
+  return prepare_step(coords, species, n_conf, n_per_conf, cell, pbc, mode, cutoff, max_bins, grid, bin_start,
+                           sorted_orig, orig_to_sorted, spos, sbin, bucket_ranges, lo, hi, num_species, rows_cap, row_of,
+                           row_atom, tile_species, layout_info, n_shf_r, angular_sub, out_dim, ldx, ang_pad, aev_blocks,
+                           zero_f32, zero_f32_count, zero_f64, zero_f64_count, bucket_species, scratch_i32, status,
+                           lattice, stream);
 }

@@ -107,7 +107,19 @@ __device__ __forceinline__ float3 image_shift(const ani_grid& g, int code) {
   return s;
 }
 
-// bucket b of a mode 0 / mode 2 grid -> its (ix, iy, iz) inside its sub-grid; returns the first bucket of that
+// grid mode 3 (one cell per conformer): the same shift in the lattice of conformer `conf`, from its row of the
+// lattice table (ANI_LATTICE_STRIDE floats: cell, inverse)
+__device__ __forceinline__ float3 image_shift(const float* __restrict__ lattice, int conf, int code) {
+  const float* c = lattice + (size_t)conf * ANI_LATTICE_STRIDE;
+  float wx = (float)(code / 9 - 1), wy = (float)((code / 3) % 3 - 1), wz = (float)(code % 3 - 1);
+  float3 s;
+  s.x = wx * c[0] + wy * c[3] + wz * c[6];
+  s.y = wx * c[1] + wy * c[4] + wz * c[7];
+  s.z = wx * c[2] + wy * c[5] + wz * c[8];
+  return s;
+}
+
+// bucket b of a mode 0 / mode 2 / mode 3 grid -> its (ix, iy, iz) inside its sub-grid; returns the first bucket of that
 // sub-grid (0 in mode 0; c * dims[0] * dims[1] * dims[2] for conformer c of a periodic batch)
 __device__ __forceinline__ int bucket_coords(const ani_grid& g, int b, int& ix, int& iy, int& iz) {
   const int nb = g.dims[0] * g.dims[1] * g.dims[2];

@@ -384,9 +384,10 @@ class Workspace:
         self.grid = torch.zeros(C.sizeof(Grid) // 4, **i32)
         # What a host-driven loop moves per step lives in TWO contiguous blocks, so that calculator.HostCalculator needs one
         # H2D and one D2H copy (each copy is a node of the captured graph with its own DMA set-up latency):
-        #   in_block  f32: [cell 9 | pad to 16 | coords 3 n]
+        #   in_block  f32: [cell 9 x n_conf (one per conformer, or the shared one first) | pad to 16 | coords 3 n]
         #   out_block u8 : [energies f64 x n_conf | status i32 | pad to 16 B | grad f32 x 3 n]
-        self.in_block = torch.zeros(16 + 3 * n, **f32)
+        self.in_coords_off = (9 * n_conf + 15) // 16 * 16
+        self.in_block = torch.zeros(self.in_coords_off + 3 * n, **f32)
         self._out_grad_off = (8 * n_conf + 4 + 15) // 16 * 16
         self.out_block = torch.zeros(self._out_grad_off + 12 * n, dtype=torch.uint8, device=device)
         self.status = self.out_block[8 * n_conf: 8 * n_conf + 4].view(torch.int32)
@@ -420,8 +421,9 @@ class Workspace:
         self.e_member = torch.zeros(num_members, self.rows_cap, **f32)
         self.mlp_sync = torch.zeros(6 * (self.rows_cap // TILE) * _lib.ANI_MAX_MEMBERS + 8, **i32)   # ani_b200_mlp_step counters
         self.species_i32 = torch.zeros(n, **i32)
-        self.coords = self.in_block[16:].view(n, 3)
+        self.coords = self.in_block[self.in_coords_off:].view(n, 3)
         self.cell = self.in_block[:9]
+        self.cells = self.in_block[:9 * n_conf].view(n_conf, 9)   # grid mode 3: one cell per conformer
         self.grad = self.out_block[self._out_grad_off:].view(torch.float32).view(n, 3)
         self.atomic = torch.zeros(n, **f32)
         self.member_atomic = torch.zeros(num_members, n, **f32)
@@ -443,10 +445,11 @@ class Workspace:
         # partial sums of the virial W_ab = sum_pairs (dE/dDelta)_a Delta_b (ani_b200_aev_backward)
         self.virial = torch.zeros(_lib.ANI_VIRIAL_SLOTS, 9, dtype=torch.float64, device=device)
         self.periodic = n_conf == 1
+        self.lattice: tp.Optional[Tensor] = None
         self._retired: tp.List[Tensor] = []
 
     def make_periodic(self) -> None:
-        """Size the bucket buffers of a batch for a shared periodic cell (grid mode 2), once, on its first use with a
+        """Size the bucket buffers of a batch for periodic cells (grid modes 2 and 3), once, on its first use with a
         cell: every conformer gets the bucket capacity of a single-system workspace of its atoms, so that its sub-grid
         is the grid a single system would get.  The buffers of the open batch (one bucket per conformer) stay alive
         for the CUDA graphs captured with them."""
@@ -462,13 +465,26 @@ class Workspace:
         self.bucket_species = (torch.zeros(self.max_bins * 8, **i32)
                                if os.environ.get("ANI_B200_AEV_BSS", "0") != "0" else None)
         self.virial = torch.zeros(self.n_conf * _lib.ANI_VIRIAL_SLOTS, 9, dtype=torch.float64, device=dev)
+        # grid mode 3: per conformer {cell, inverse}, written by the preparation of every step
+        self.lattice = torch.zeros(self.n_conf, _lib.ANI_LATTICE_STRIDE, dtype=torch.float32, device=dev)
         self.periodic = True
 
 
-def _grid_mode(n_conf: int, pbc: bool) -> int:
+def _grid_mode(n_conf: int, pbc: bool, conformer_cells: bool = False) -> int:
     """ani_grid::mode: 0 one system, 1 an open batch (one bucket per conformer), 2 a periodic batch in one shared cell
-    (one sub-grid per conformer)."""
+    (one sub-grid per conformer), 3 a periodic batch with one cell per conformer."""
+    if conformer_cells and n_conf > 1:
+        return 3
     return 0 if n_conf == 1 else (2 if pbc else 1)
+
+
+def conformer_cells(cell: tp.Optional[Tensor], n_conf: int) -> bool:
+    """True if ``cell`` is one cell per conformer, (C, 3, 3) (grid mode 3); False for one shared (3, 3) cell or None."""
+    if cell is None or cell.dim() == 2:
+        return False
+    if cell.shape != (n_conf, 3, 3):
+        raise ValueError(f"cell must be (3, 3) or one cell per conformer, ({n_conf}, 3, 3); got {tuple(cell.shape)}")
+    return True
 
 
 class StepResult(tp.NamedTuple):
@@ -581,29 +597,38 @@ class Engine:
             raise ValueError(f"inputs must live on {dev} (the engine has no CPU path)")
         if pbc and cell is None:
             raise ValueError("If pbc is not None, cell should be present")
+        per_conf = bool(pbc) and conformer_cells(cell, n_conf)
+        if per_conf and n_conf == 1:
+            cell, per_conf = cell[0], False   # one conformer: its cell is the shared cell
         ws = self.workspace(n_conf, n_per_conf)
         if pbc:
             ws.make_periodic()
         # inputs -> persistent buffers (what the graph reads)
         ws.species_i32.copy_(species.reshape(-1))
         ws.coords.copy_(coords.reshape(-1, 3))
-        if pbc:
+        if per_conf:
+            ws.cells.copy_(cell.reshape(n_conf, 9))
+        elif pbc:
             ws.cell.copy_(cell.reshape(-1))
-        res = self.run(ws, bool(pbc), want_grad, shard, want_virial=want_virial)
+        res = self.run(ws, bool(pbc), want_grad, shard, want_virial=want_virial, conformer_cells=per_conf)
         if check:   # one 4-byte D2H read: cell too small / neighbour overflow / operand range raise here
             self.check_status(ws)
         return res
 
     def run(self, ws: Workspace, pbc: bool, want_grad: bool = True, shard: tp.Tuple[int, int] = (0, 1),
-            reuse: bool = False, want_virial: bool = False) -> StepResult:
+            reuse: bool = False, want_virial: bool = False, conformer_cells: bool = False) -> StepResult:
         """One step on inputs that are ALREADY in the workspace buffers (``ws.species_i32``,
-        ``ws.coords``, ``ws.cell``) -- the entry point of host-driven loops that copy straight into
-        them (calculator.HostCalculator).  The results alias workspace buffers."""
+        ``ws.coords``, ``ws.cell`` -- or, with ``conformer_cells``, one cell per conformer in ``ws.cells``) -- the
+        entry point of host-driven loops that copy straight into them (calculator.HostCalculator).  The results alias
+        workspace buffers."""
         n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
         rank, world = shard
         lo = (n * rank) // world
         hi = (n * (rank + 1)) // world
         periodic_batch = bool(pbc) and n_conf > 1
+        conformer_cells = bool(conformer_cells)
+        if conformer_cells and not periodic_batch:
+            raise ValueError("one cell per conformer needs a periodic batch (C > 1, pbc)")
         if want_virial and (not want_grad or reuse or (n_conf != 1 and not periodic_batch)):
             raise ValueError("the virial comes out of the force pass of a single system or a periodic batch with a "
                              "freshly built grid")
@@ -612,12 +637,12 @@ class Engine:
         if periodic_batch and reuse:
             raise ValueError("reuse=True (Verlet skin) is not supported for periodic batches")
         key = (n_conf, n_per_conf, bool(pbc), bool(want_grad), lo, hi, self.nets.active_key, bool(reuse), self.skin,
-               bool(want_virial), self.mlp_mode)
+               bool(want_virial), self.mlp_mode, conformer_cells)
         if reuse and not self.skin > 0:
             raise ValueError("reuse=True needs Engine.skin > 0 and a previous step that built the grid")
         with torch.cuda.device(self.device):   # the C-ABI launches on the CURRENT device's stream
             if not self.cuda_graph or self.profile:
-                self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial)
+                self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells)
             else:
                 graph = self._graphs.get(key)
                 if graph is not None:
@@ -628,12 +653,12 @@ class Engine:
                     if len(self._graph_seen) > 4 * self.max_graphs:
                         self._graph_seen.clear()
                     self._graph_seen[key] = self._graph_seen.get(key, 0) + 1
-                    self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial)
+                    self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells)
                 else:
                     self.note_composition(ws)
                     graph = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(graph):
-                        self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial)
+                        self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells)
                     while len(self._graphs) >= self.max_graphs:   # evict the least recently used capture
                         self._graphs.pop(next(iter(self._graphs)))
                     self._graphs[key] = graph
@@ -659,15 +684,22 @@ class Engine:
                           ws.member_atomic.view(-1, n_conf, n_per_conf), grad, virial)
 
     def _launch(self, ws: Workspace, pbc: bool, want_grad: bool, lo: int, hi: int, reuse: bool = False,
-                want_virial: bool = False) -> None:
+                want_virial: bool = False, conformer_cells: bool = False) -> None:
         """Enqueue the kernels of one step on the current stream (graph-capturable: no allocation,
         no synchronisation, only this library's launches and two memsets)."""
         L = self.lib
         n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
         st = torch.cuda.current_stream(self.device).cuda_stream
         cell_ptr = ptr(ws.cell) if pbc else None
-        mode = _grid_mode(n_conf, pbc)
+        mode = _grid_mode(n_conf, pbc, conformer_cells)
         c = self.consts
+        # grid mode 3 (one cell per conformer): the same kernels through the entry points that take the lattice table
+        # the preparation writes; the cells are read from the workspace by the preparation (inside a captured graph)
+        prepare, aev_forward, aev_backward = L.ani_b200_prepare_step, L.ani_b200_aev_forward, L.ani_b200_aev_backward
+        lat: tp.Tuple[tp.Any, ...] = ()
+        if mode == 3:
+            prepare, aev_forward = L.ani_b200_prepare_step_cells, L.ani_b200_aev_forward_cells
+            aev_backward, lat, cell_ptr = L.ani_b200_aev_backward_cells, (ptr(ws.lattice),), ptr(ws.cells)
         # bucket grid + species-grouped row layout + live AEV column blocks (+ zero-fill of the force
         # accumulator): one fused entry point, five launches -- or, with a Verlet skin and reuse=True,
         # one launch that only refreshes the positions inside the grid of an earlier step
@@ -677,7 +709,7 @@ class Engine:
                 ptr(ws.ref_shift), ptr(ws.moved), ws.grad_ptr if want_grad else None, 3 * n if want_grad else 0,
                 ptr(ws.aev_blocks), self.nets.ldx, st))
         else:
-            self._timed("prepare_step", lambda: L.ani_b200_prepare_step(
+            self._timed("prepare_step", lambda: prepare(
                 ptr(ws.coords), ptr(ws.species_i32), n_conf, n_per_conf, cell_ptr, int(bool(pbc)), mode,
                 c.rcr + self.skin, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start), ptr(ws.sorted_orig),
                 ptr(ws.orig_to_sorted), ptr(ws.spos), ptr(ws.sbin), ptr(ws.bucket_ranges),
@@ -685,7 +717,7 @@ class Engine:
                 ptr(ws.layout_info), len(c.shf_r), len(c.shf_a) * len(c.shf_z), c.out_dim, self.nets.ldx,
                 self.nets.col_pad, ptr(ws.aev_blocks), ws.grad_ptr if want_grad else None, 3 * n if want_grad else 0,
                 ptr(ws.virial) if want_virial else None, ws.virial.numel() if want_virial else 0,
-                ptr(ws.bucket_species), ptr(ws.scratch), ptr(ws.status), st))
+                ptr(ws.bucket_species), ptr(ws.scratch), ptr(ws.status), *lat, st))
             if self.skin > 0:
                 check(L.ani_b200_verlet_positions(
                     0, ptr(ws.coords), ptr(ws.grid), ptr(ws.sorted_orig), n, self.skin, ptr(ws.spos),
@@ -704,12 +736,12 @@ class Engine:
             check(L.ani_b200_zero_live_blocks(C.byref(self.nets.model), ptr(ws.dx), ptr(ws.layout_info),
                                               ptr(ws.aev_blocks), side.cuda_stream), "zero_live_blocks")
             self._ev[1].record(side)
-        self._timed("aev_forward", lambda: L.ani_b200_aev_forward(
+        self._timed("aev_forward", lambda: aev_forward(
             C.byref(self.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sbin),
             ptr(ws.bucket_ranges), ptr(ws.bucket_species) if not reuse else None,
             ws.aev_blocks.data_ptr() + 4 * (ws.n_blocks + 1), n, lo, hi,
             ptr(ws.row_of), ptr(ws.x), self.nets.ldx, 1, ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap,
-            ptr(ws.status), st))
+            ptr(ws.status), *lat, st))
 
         def reduce_on(stream_handle):
             return L.ani_b200_reduce_energies(
@@ -762,11 +794,11 @@ class Engine:
             check(reduce_on(side2.cuda_stream), "reduce_energies")
             self._ev[3].record(side2)
         if want_grad:
-            self._timed("aev_backward", lambda: L.ani_b200_aev_backward(
+            self._timed("aev_backward", lambda: aev_backward(
                 C.byref(self.params), ptr(ws.grid), ptr(ws.spos), ptr(ws.sorted_orig),
                 ws.aev_blocks.data_ptr() + 4 * (ws.n_blocks + 1), n, lo, hi,
                 ptr(ws.row_of), ptr(ws.dx), self.nets.ldx, ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap,
-                ws.grad_ptr, ptr(ws.status), ws.max_elements, ptr(ws.virial) if want_virial else None, st))
+                ws.grad_ptr, ptr(ws.status), ws.max_elements, ptr(ws.virial) if want_virial else None, *lat, st))
         if overlap or split:
             main.wait_event(self._ev[3])
         else:
@@ -788,10 +820,19 @@ class Engine:
         graph): an analysis call, not the MD loop."""
         dev = self.device
         n_conf, n_per_conf = species.shape
+        per_conf = bool(pbc) and conformer_cells(cell, n_conf)
+        if per_conf and n_conf == 1:
+            cell, per_conf = cell[0], False
         ws = self.workspace(n_conf, n_per_conf)
         if pbc:
             ws.make_periodic()
         n, L, c = ws.n, self.lib, self.consts
+        prepare, aev_forward, aev_backward = L.ani_b200_prepare_step, L.ani_b200_aev_forward, L.ani_b200_aev_backward
+        lat: tp.Tuple[tp.Any, ...] = ()
+        cell_ptr = ptr(ws.cell) if pbc else None
+        if per_conf:   # grid mode 3, see _launch
+            prepare, aev_forward = L.ani_b200_prepare_step_cells, L.ani_b200_aev_forward_cells
+            aev_backward, lat, cell_ptr = L.ani_b200_aev_backward_cells, (ptr(ws.lattice),), ptr(ws.cells)
         nets = self.nets
         M, ldx = nets.num_members, nets.ldx
         active = list(nets.active)
@@ -805,31 +846,34 @@ class Engine:
             st = torch.cuda.current_stream(dev).cuda_stream
             ws.species_i32.copy_(species.reshape(-1))
             ws.coords.copy_(coords.reshape(-1, 3))
-            if pbc:
+            if per_conf:
+                ws.cells.copy_(cell.reshape(n_conf, 9))
+            elif pbc:
                 ws.cell.copy_(cell.reshape(-1))
-            check(L.ani_b200_prepare_step(
-                ptr(ws.coords), ptr(ws.species_i32), n_conf, n_per_conf, ptr(ws.cell) if pbc else None, int(bool(pbc)),
-                _grid_mode(n_conf, pbc), c.rcr, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start), ptr(ws.sorted_orig),
+            check(prepare(
+                ptr(ws.coords), ptr(ws.species_i32), n_conf, n_per_conf, cell_ptr, int(bool(pbc)),
+                _grid_mode(n_conf, pbc, per_conf), c.rcr, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start),
+                ptr(ws.sorted_orig),
                 ptr(ws.orig_to_sorted), ptr(ws.spos), ptr(ws.sbin), ptr(ws.bucket_ranges), 0, n, c.num_species,
                 ws.rows_cap, ptr(ws.row_of), ptr(ws.row_atom), ptr(ws.tile_species), ptr(ws.layout_info),
                 len(c.shf_r), len(c.shf_a) * len(c.shf_z), c.out_dim, ldx, self.nets.col_pad, ptr(ws.aev_blocks), None, 0,
                 None, 0,
-                ptr(ws.bucket_species), ptr(ws.scratch), ptr(ws.status), st), "prepare_step")
+                ptr(ws.bucket_species), ptr(ws.scratch), ptr(ws.status), *lat, st), "prepare_step")
             mask_ptr = ws.aev_blocks.data_ptr() + 4 * (ws.n_blocks + 1)
-            check(L.ani_b200_aev_forward(
+            check(aev_forward(
                 C.byref(self.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sbin),
                 ptr(ws.bucket_ranges), ptr(ws.bucket_species), mask_ptr, n, 0, n, ptr(ws.row_of), ptr(ws.x), ldx, 1,
                 ptr(ws.nbr_cnt),
-                ptr(ws.nbr_list), ws.nbr_cap, ptr(ws.status), st), "aev_forward")
+                ptr(ws.nbr_list), ws.nbr_cap, ptr(ws.status), *lat, st), "aev_forward")
             check(L.ani_b200_mlp_step(
                 C.byref(model), ptr(ws.x), ptr(ws.dx_members), ws.rows_cap, ptr(ws.row_atom), ptr(ws.layout_info),
                 ptr(ws.aev_blocks), ptr(ws.act1), ptr(ws.act2), ptr(ws.act3), ptr(ws.e_member), 2, ptr(ws.mlp_sync),
                 ptr(ws.status), st), "mlp_step")
             for k, m in enumerate(active):
-                check(L.ani_b200_aev_backward(
+                check(aev_backward(
                     C.byref(self.params), ptr(ws.grid), ptr(ws.spos), ptr(ws.sorted_orig), mask_ptr, n, 0, n,
                     ptr(ws.row_of), ws.dx_members[m].data_ptr(), ldx, ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap,
-                    grads[k].data_ptr(), ptr(ws.status), 0, None, st), "aev_backward")
+                    grads[k].data_ptr(), ptr(ws.status), 0, None, *lat, st), "aev_backward")
             check(L.ani_b200_reduce_energies(
                 C.byref(model), ptr(ws.e_member), ws.rows_cap, ptr(ws.row_of), ptr(ws.orig_to_sorted),
                 ptr(ws.species_i32), n, 0, n, n_conf, n_per_conf, None, ptr(ws.atomic), ptr(ws.member_atomic),

@@ -114,6 +114,11 @@ class _FusedEnergy(torch.autograd.Function):
         return out, None, None, None, None, None
 
 
+def _per_conformer(cell: tp.Optional[Tensor]) -> bool:
+    """One cell per conformer, (C, 3, 3): a periodic batch in grid mode 3."""
+    return cell is not None and cell.dim() == 3
+
+
 class ANI(torch.nn.Module):
     r"""ANI-style neural network interatomic potential (interface of arch.py:90-381)."""
 
@@ -206,11 +211,13 @@ class ANI(torch.nn.Module):
         species, coords = species_coordinates
         self._check_inputs(species, coords, charge)
         elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
-        _validate_inputs(self.cutoff, elem_idxs, coords, cell, pbc)
-        # (a periodic batch -- C conformers in one shared cell -- is one engine step: one sub-grid per conformer)
+        _validate_inputs(self.cutoff, elem_idxs, coords, cell, pbc, conformer_cells=True)
+        # (a periodic batch -- C conformers in one shared cell, or one (C, 3, 3) cell per conformer -- is one engine
+        # step: one sub-grid per conformer)
         # (with a cell-list neighbour list the reference raises "Cell is too small" instead, neighbors.py:402-403: so
-        # does the engine; all_pairs / adaptive models take the supercell route)
-        sup = None if isinstance(self.neighborlist, CellList) else \
+        # does the engine; all_pairs / adaptive models take the supercell route -- for a shared cell only: a thin cell
+        # of one conformer of a (C, 3, 3) batch raises too)
+        sup = None if (isinstance(self.neighborlist, CellList) or _per_conformer(cell)) else \
             supercell_for_thin_cell(species, coords, cell, pbc, self.cutoff)
         if sup is not None:
             # periodic cell thinner than the cutoff (neighbors.py:245-275): evaluate a supercell of R translation-
@@ -299,7 +306,7 @@ class ANI(torch.nn.Module):
         species, coords = species_coordinates
         self._check_inputs(species, coords, charge)
         elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
-        _validate_inputs(self.cutoff, elem_idxs, coords, cell, pbc)
+        _validate_inputs(self.cutoff, elem_idxs, coords, cell, pbc, conformer_cells=True)
         cell = effective_periodic_cell(coords, cell, pbc, self.cutoff)
 
         def run():
@@ -360,6 +367,8 @@ class ANI(torch.nn.Module):
         ``forward`` loses ~3e-3 Ha at |E| ~ 2.5e4 Ha, see BASELINE.md)."""
         species, coords = species_coordinates
         elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
+        if _per_conformer(cell):
+            _validate_inputs(self.cutoff, elem_idxs, coords, cell, pbc, conformer_cells=True)
         cell = effective_periodic_cell(coords, cell, pbc, self.cutoff)
         return self._guarded(lambda: self.engine(coords.device).step(
             elem_idxs, coords.detach(), cell, pbc is not None, want_grad=False, check=True).energies.clone())
@@ -368,6 +377,8 @@ class ANI(torch.nn.Module):
                             pbc: tp.Optional[Tensor] = None) -> tp.Tuple[Tensor, Tensor]:
         """grad.py:263-290 without the autograd round trip: (energies f64 (C,), forces f32 (C,A,3))."""
         elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
+        if _per_conformer(cell):
+            _validate_inputs(self.cutoff, elem_idxs, coords, cell, pbc, conformer_cells=True)
         cell = effective_periodic_cell(coords, cell, pbc, self.cutoff)
         res = self._guarded(lambda: self.engine(coords.device).step(
             elem_idxs, coords.detach(), cell, pbc is not None, want_grad=True, check=True))
@@ -379,11 +390,19 @@ class ANI(torch.nn.Module):
         for one system, (C, 3, 3) for a batch of C conformers.  The stress is the "f dot r" virial of ase.py:164-168 -- sum over the pairs of
         (dE/dDelta)_a Delta_b, accumulated by the force kernel -- divided by the cell volume; it equals
         the strain derivative dE/d(scaling)/V of ase.py:170-173 and, unlike that one, does not need the
-        atoms to be wrapped into the cell."""
+        atoms to be wrapped into the cell.  With one cell per conformer, ``cell`` (C, 3, 3), conformer c's stress is
+        its virial over the volume of its own cell."""
         elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
+        if _per_conformer(cell):   # (periodic in all directions whether or not pbc is given)
+            full = torch.ones(3, dtype=torch.bool, device=coords.device) if pbc is None else pbc
+            _validate_inputs(self.cutoff, elem_idxs, coords, cell, full, conformer_cells=True)
         res = self._guarded(lambda: self.engine(coords.device).step(
             elem_idxs, coords.detach(), cell, True, want_grad=True, want_virial=True, check=True))
         volume = torch.det(cell.detach().double()).abs()
+        if _per_conformer(cell):
+            volume = volume.view(-1, 1, 1)
+            if res.virial.dim() == 2:   # a batch of one conformer
+                return res.energies.clone(), -res.grad, res.virial.unsqueeze(0) / volume
         return res.energies.clone(), -res.grad, res.virial / volume
 
     # -- state dicts of the reference (arch.py:278-290) ------------------------------------

@@ -71,12 +71,23 @@ def narrow_down(cutoff: float, elem_idxs: Tensor, coords: Tensor, neighbor_idxs:
 
 
 def _validate_inputs(cutoff: float, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor],
-                     pbc: tp.Optional[Tensor], supports_batches: bool = True) -> None:
+                     pbc: tp.Optional[Tensor], supports_batches: bool = True, conformer_cells: bool = False) -> None:
     # neighbors.py:918-949
     if cutoff <= 0.0:
         raise ValueError("Cutoff must be a strictly positive float")
     if species.dim() != 2 or coords.shape != (species.shape[0], species.shape[1], 3):
         raise ValueError("species must be (C, A) and coords (C, A, 3)")
+    if cell is not None and cell.dim() != 2:
+        # one cell per conformer (C, 3, 3) is a models.ANI input (grid mode 3); the neighbour lists and the
+        # AEVComputer take one (3, 3) cell
+        if not conformer_cells:
+            raise ValueError("one cell per conformer, (C, 3, 3), is supported by models.ANI only; neighbour lists "
+                             "and AEVComputer take one (3, 3) cell")
+        if cell.shape != (species.shape[0], 3, 3):
+            raise ValueError(f"cell must be (3, 3) or one cell per conformer, ({species.shape[0]}, 3, 3); "
+                             f"got {tuple(cell.shape)}")
+        if pbc is not None and not bool(pbc.all()):
+            raise ValueError("one cell per conformer needs PBC in all three directions")
     if not supports_batches and coords.shape[0] != 1:
         raise ValueError("This neighborlist doesn't support batches")
     if pbc is not None:
