@@ -324,6 +324,13 @@ int ani_b200_prepare_step_cells(const float* coords, const int32_t* species, int
 /* (device memory, launches*384 int64).  NULL switches it off.  No reference counterpart.           */
 int ani_b200_debug_gemm_trace(long long* buf, int launches);
 
+/* Timing experiments only: the CTA-staged AEV forward kernel writes per-phase clock64 cycles and    */
+/* %globaltimer / clock64 stamps, 16 int64 per record, into buf (device memory): one record per atom */
+/* (index - lo).  NULL switches it off.                                                              */
+/* ANI_ERR_UNSUPPORTED unless the library was built with -DANI_AEV_FWD_TRACE=1 (build variant      */
+/* "aevtrace").  No reference counterpart.                                                            */
+int ani_b200_debug_aev_trace(long long* buf);
+
 /* 5. Reference-format half neighbour list (neighbors.py:13-18) from the bucket grid.       */
 /*    Two calls: count (fills pair_start i32[n+1], exclusive scan, total in pair_start[n]),  */
 /*    then fill with capacity `cap` pairs.  indices are flat INPUT indices, idx0 < idx1       */

@@ -96,6 +96,7 @@ _PROTOTYPES = {
                                               _P, _P]),
     "ani_b200_verlet_positions":(C.c_int, [_I, _P, _P, _P, _I, _F, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
     "ani_b200_debug_gemm_trace": (C.c_int, [_P, _I]),
+    "ani_b200_debug_aev_trace": (C.c_int, [_P]),
     "ani_b200_half_neighbor_count": (C.c_int, [_P, _P, _P, _P, _P, _I, _F, _P, _P]),
     "ani_b200_half_neighbor_fill": (C.c_int, [_P, _P, _P, _P, _P, _I, _F, _P, C.c_int64, _P, _P, _P, _P, _P, _P]),
     "ani_b200_mlp_forward_backward": (C.c_int, [_P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P]),

@@ -49,6 +49,8 @@ VARIANTS = {
     "fwd7": ["-DANI_AEV_FWD_MIN_CTAS=7", "-DANI_AEV_CAND_CAP=640"],
     "fwd8w": ["-DANI_AEV_FWD_WARPS=8", "-DANI_AEV_FWD_MIN_CTAS=3"],
     "fwd6w": ["-DANI_AEV_FWD_WARPS=6", "-DANI_AEV_FWD_MIN_CTAS=4"],
+    # phase trace of the CTA-staged AEV forward (tools/aev_forward_trace.py)
+    "aevtrace": ["-DANI_AEV_FWD_TRACE=1"],
 }
 
 

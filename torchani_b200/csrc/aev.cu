@@ -302,18 +302,27 @@ __device__ __forceinline__ void triangle_decode(int q, int& a, int& b) {
   a = q - b * (b - 1) / 2;
 }
 
-// sum acc[f] over the 32 lanes; lane l returns the total of feature l (31 shuffles)
-__device__ __forceinline__ float transpose_reduce32(float (&acc)[32], int lane) {
+// one level of transpose_reduce32: lanes l and l ^ HALF swap halves of acc[0, 2 HALF) and each keeps a sum
+template <int HALF>
+__device__ __forceinline__ void transpose_level(float (&acc)[32], int lane) {
+  const bool up = (lane & HALF) != 0;
 #pragma unroll
-  for (int half = 16; half >= 1; half >>= 1) {
-    const bool up = (lane & half) != 0;
-#pragma unroll
-    for (int i = 0; i < half; ++i) {
-      float send = up ? acc[i] : acc[i + half];
-      float keep = up ? acc[i + half] : acc[i];
-      acc[i] = keep + __shfl_xor_sync(ANI_FULL_MASK, send, half);
-    }
+  for (int i = 0; i < HALF; ++i) {
+    float send = up ? acc[i] : acc[i + HALF];
+    float keep = up ? acc[i + HALF] : acc[i];
+    acc[i] = keep + __shfl_xor_sync(ANI_FULL_MASK, send, HALF);
   }
+}
+
+// sum acc[f] over the 32 lanes; lane l returns the total of feature l (31 shuffles).  The levels are template
+// instances so that every index into acc is a constant: written as a loop over `half`, nvcc kept it rolled, which put
+// the 32 accumulators on the stack and cost a local-memory store and load around every shuffle.
+__device__ __forceinline__ float transpose_reduce32(float (&acc)[32], int lane) {
+  transpose_level<16>(acc, lane);
+  transpose_level<8>(acc, lane);
+  transpose_level<4>(acc, lane);
+  transpose_level<2>(acc, lane);
+  transpose_level<1>(acc, lane);
   return acc[0];
 }
 
@@ -575,6 +584,62 @@ struct CtaStage {
   unsigned long long tma_bar;                  // mbarrier of the TMA bulk copies that stage the bucket ranges
 };
 
+// ---- opt-in phase trace (build variant "aevtrace": -DANI_AEV_FWD_TRACE=1; tools/aev_forward_trace.py) --------------
+// One record of 16 int64 per atom (index i - lo), written by its warp: clock64 cycles spent in each phase (the staging
+// phases include the CTA barriers that close them), %globaltimer and clock64 at the warp's start and end, the SM.
+// Absent from the default build.
+#ifndef ANI_AEV_FWD_TRACE
+#define ANI_AEV_FWD_TRACE 0
+#endif
+enum AevTracePhase { TR_RANGES, TR_COUNT, TR_PLACE, TR_COMPACT, TR_LIST, TR_RADIAL, TR_ANGULAR, TR_PHASES };
+#if ANI_AEV_FWD_TRACE
+__device__ long long* g_aev_fwd_trace;
+struct AevTrace {
+  long long acc[TR_PHASES];
+  long long t, gt0, ck0;
+  __device__ __forceinline__ static long long clk() {
+    long long v;
+    asm volatile("mov.u64 %0, %%clock64;" : "=l"(v));
+    return v;
+  }
+  __device__ __forceinline__ static long long gtime() {
+    long long v;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(v));
+    return v;
+  }
+  __device__ __forceinline__ void start() {
+#pragma unroll
+    for (int k = 0; k < TR_PHASES; ++k) acc[k] = 0;
+    gt0 = gtime();
+    ck0 = t = clk();
+  }
+  __device__ __forceinline__ void mark(int ph) {
+    const long long c = clk();
+    acc[ph] += c - t;
+    t = c;
+  }
+  __device__ __forceinline__ void write(size_t rec, int lane) {
+    if (lane != 0 || !g_aev_fwd_trace) return;
+    long long* r = g_aev_fwd_trace + rec * 16;
+#pragma unroll
+    for (int k = 0; k < TR_PHASES; ++k) r[k] = acc[k];
+    unsigned sm;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    r[8] = gt0;
+    r[9] = gtime();
+    r[10] = ck0;
+    r[11] = clk();
+    r[12] = sm;
+  }
+};
+#else
+struct AevTrace {
+  __device__ __forceinline__ void start() {}
+  __device__ __forceinline__ void mark(int) {}
+  __device__ __forceinline__ void write(size_t, int) {}
+};
+#endif
+
 template <int NA, int NZ, bool TMA_STAGE = false, bool LAT = false>
 __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
     k_aev_forward_cta(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
@@ -588,6 +653,8 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ CtaStage C;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  AevTrace tr;
+  tr.start();
   const ani_grid g = *grid;
   hi = min(hi, g.n_real);
   const int i = lo + blockIdx.x * AEV_FWD_WARPS + warp;
@@ -700,6 +767,7 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
       __syncwarp();
     }
     if (!use_bss) __syncthreads();
+    tr.mark(TR_RANGES);
     const int T = C.r_off[NRANGE];
     // first bucket of the CTA, neighbourhood fits: one TMA bulk copy per non-empty range (contiguous float4 runs of
     // the bucket-sorted position array), all completing on one mbarrier
@@ -780,6 +848,7 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
       __syncwarp();
     }
     if (!use_bss) __syncthreads();
+    tr.mark(TR_COUNT);
     const bool mine = has && myb == cur;
     for (int F0 = 0; F0 < T; F0 += CAND_CAP) {
       // (c) place the candidates whose species-major position falls into this window
@@ -811,6 +880,7 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
         }
       }
       __syncthreads();
+      tr.mark(TR_PLACE);
       // (d) the warps of this bucket compact their neighbours out of the window
       if (mine) {
         if (F0 == 0) {
@@ -858,6 +928,7 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
         }
       }
       __syncthreads();  // before the next window / phase overwrites the staging area
+      tr.mark(TR_COMPACT);
     }
   }
   if (!has) return;
@@ -904,6 +975,7 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
     rf[n] = make_float2(cr * R, cutoff_value(R, P.rcr, P.cutoff_kind));
   }
   __syncwarp();
+  tr.mark(TR_LIST);
 
   // element pairs / elements that do not occur anywhere in the system are never read by the MLP:
   // skip them (species_mask[1] != 0: the composition changed since the last call -> write them once)
@@ -930,6 +1002,7 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
       if (h == 0 && m < nR) store_feature(sp * nR + m, 0.25f * acc);
     }
   }
+  tr.mark(TR_RADIAL);
 
   // ---- 3. angular block
   const int n_ang = cnt_a;
@@ -1002,6 +1075,8 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
     }
   }
   if (ANI_OPND_FP16X2 && !(vmax <= OPND_HALF_MAX)) atomicOr(status, ANI_STATUS_OPERAND_RANGE);
+  tr.mark(TR_ANGULAR);
+  tr.write((size_t)(i - lo), lane);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1674,6 +1749,17 @@ __global__ void k_full_list_rows(const float* __restrict__ coords, const int32_t
     ++cnt;
   }
   if (!FILL) counts[i] = cnt;
+}
+
+// phase trace of k_aev_forward_cta: only the "aevtrace" build variant records it
+extern "C" int ani_b200_debug_aev_trace(long long* buf) {
+#if ANI_AEV_FWD_TRACE
+  if (cudaMemcpyToSymbol(g_aev_fwd_trace, &buf, sizeof(buf)) != cudaSuccess) return ANI_ERR_CUDA;
+  return ANI_OK;
+#else
+  (void)buf;
+  return ANI_ERR_UNSUPPORTED;
+#endif
 }
 
 }  // namespace ani
