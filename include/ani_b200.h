@@ -25,6 +25,8 @@
  *   ani_b200_reduce_energies    nn/_containers.py:418-421,633-636, sae.py:54-64
  *   ani_b200_verlet_positions   neighbors.py:759-884 (VerletCellList: reuse of a list built with a skin)
  *   ani_b200_aev_backward(..., virial, ...)   ase.py:164-168 (the "f dot r" virial of the stress)
+ *   ani_b200_aev_backward_members  arch.py:403-436 (members_forces: one autograd pass per member)
+ *   ani_b200_ensemble_qbc       arch.py:439-485,543-576 (energies_qbcs, force_magnitudes, force_qbc)
  *   ani_b200_operand_format     (no counterpart: format of the tensor-core GEMM operands of this build)
  */
 #ifndef ANI_B200_H
@@ -221,6 +223,49 @@ int ani_b200_aev_backward_cells(const ani_aev_params* params, const ani_grid* gr
                                 int hi, const int32_t* row_of, const float* grad_aev, int ldx,
                                 const int32_t* nbr_cnt, const int32_t* nbr_list, int nbr_cap, float* grad_coords,
                                 int32_t* status, int max_elements, double* virial, const float* lattice, void* stream);
+
+/* 4e. AEV backward of EVERY active ensemble member in one launch (members_forces, arch.py:403-436; the force       */
+/*    disagreement of query-by-committee active learning).  grad_slabs holds one dE_m/dAEV slab per member m,        */
+/*    slab m at grad_slabs + m * slab_stride floats, each in the row layout of ani_b200_aev_backward's grad_aev (the   */
+/*    want_backward == 2 output of ani_b200_mlp_step, or ani_b200_mlp_step_resident_members).  members: HOST array    */
+/*    of n_members (1..ANI_MAX_MEMBERS) member indices, read at launch; output k (the member order of the caller,     */
+/*    e.g. the active order) contracts slab members[k] and is accumulated (+=, float atomics) into                    */
+/*    grad_members + k * 3 n, f32[n_members][n][3] in flat INPUT order (zeroed by the caller, e.g. as the zero_f32 of */
+/*    the preparation).  Only the columns ani_b200_aev_backward reads are read: the radial block and the angular     */
+/*    blocks of element pairs present in species_mask, i.e. the live column blocks the MLP writes.  A warp builds its */
+/*    atom's neighbour geometry once and loops over the members, their rows double-buffered in shared memory          */
+/*    (shared memory does not depend on n_members).  max_elements as in ani_b200_aev_backward.  No virial, no         */
+/*    explicit neighbour rows.  Status: ANI_STATUS_ANG_OVERFLOW as ani_b200_aev_backward.  The _cells form takes the   */
+/*    lattice table of grid mode 3 (not NULL).                                                                       */
+int ani_b200_aev_backward_members(const ani_aev_params* params, const ani_grid* grid, const float* spos,
+                                  const int32_t* sorted_orig, const int32_t* species_mask, int n, int lo, int hi,
+                                  const int32_t* row_of, const float* grad_slabs, int ldx, long long slab_stride,
+                                  const int32_t* members, int n_members, const int32_t* nbr_cnt,
+                                  const int32_t* nbr_list, int nbr_cap, float* grad_members, int32_t* status,
+                                  int max_elements, void* stream);
+int ani_b200_aev_backward_members_cells(const ani_aev_params* params, const ani_grid* grid, const float* spos,
+                                        const int32_t* sorted_orig, const int32_t* species_mask, int n, int lo, int hi,
+                                        const int32_t* row_of, const float* grad_slabs, int ldx, long long slab_stride,
+                                        const int32_t* members, int n_members, const int32_t* nbr_cnt,
+                                        const int32_t* nbr_list, int nbr_cap, float* grad_members, int32_t* status,
+                                        int max_elements, const float* lattice, void* stream);
+
+/* 4f. Query-by-committee statistics of an ensemble step (arch.py:439-485, 543-576), from                         */
+/*      grad_members     f32[n_members][n][3]  dE_m/dcoords (ani_b200_aev_backward_members), n = n_conf * n_per_conf */
+/*      members          HOST i32[n_members]  member index of every output k (as given to the backward)             */
+/*      member_atomic    f32[M][n]  the member_atomic_out of ani_b200_reduce_energies (indexed by member index)     */
+/*      species          i32[n]  element index, -1 padding;  sae f64[num_species] or NULL                          */
+/*    writes (plain stores, nothing accumulated, no zero-fill needed):                                               */
+/*      grad             f32[n][3]  mean over the outputs of grad_members (the ensemble's dE/dcoords)               */
+/*      atom_stats       f32[3][n]  per atom: mean_k |F_k|, (std_k |F_k| + 1e-8) / (mean + 1e-8) (unbiased std),       */
+/*                                  (max_k |F_k| - min_k |F_k| + 1e-8) / (mean + 1e-8); one member: 0 and 1.          */
+/*                                  Padding atoms follow the same formulas (their forces are 0)                     */
+/*      member_energies  f64[n_members][n_conf]  sum over the conformer's real atoms of member_atomic + sae          */
+/*      qbc              f64[n_conf]  std_k(E_k) (unbiased; 0 for one member) / sqrt(real atoms of the conformer)    */
+/*    Two launches; raises no status bits.                                                                           */
+int ani_b200_ensemble_qbc(const float* grad_members, const int32_t* members, int n_members, const float* member_atomic,
+                          const int32_t* species, const double* sae, int n_conf, int n_per_conf, float* grad,
+                          float* atom_stats, double* member_energies, double* qbc, void* stream);
 
 /* 4b. The same AEV kernels fed by an externally supplied HALF pair list (the reference's    */
 /*    Neighbors tuple; AEVComputer.compute_from_neighbors, aev/_computer.py:251-272 ->          */
@@ -455,6 +500,20 @@ int ani_b200_mlp_step(const ani_mlp_model* model, const void* x, float* dx, int 
 int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void* x, float* dx, int rows_cap,
                                const int32_t* row_atom, const int32_t* layout_info, const int32_t* aev_blocks,
                                void* act1, void* act2, float* e_member, int32_t* status, void* stream);
+
+/*    The same launch with one dE/dAEV slab per member (the query-by-committee step, ani_b200_aev_backward_members):   */
+/*    the arguments of ani_b200_mlp_step_resident plus slab_stride (floats, >= rows_cap * ldx).  Only the chains of    */
+/*    the ACTIVE members (member_scale[m] != 0) run.  Active member m's slab, dx + m * slab_stride, f32[rows_cap][ldx], */
+/*    receives d(member_scale[m] * e_m)/dAEV by plain stores in the rows of the row tiles of the layout (padding rows  */
+/*    get zeros) and the live column blocks of aev_blocks (every column without a block list); no other column or row, */
+/*    and no slab of an inactive member, is written.  No zero-fill is needed: ani_b200_aev_backward_members reads     */
+/*    only the live blocks of active members' real rows.  e_member rows of inactive members are set to 0.  Same limits  */
+/*    as ani_b200_mlp_step_resident (ANI_ERR_UNSUPPORTED in the 3 x bf16 build and above hidden width 256; there,     */
+/*    ani_b200_mlp_step(..., want_backward = 2) provides the slabs); ANI_ERR_BAD_ARG without an active member.       */
+int ani_b200_mlp_step_resident_members(const ani_mlp_model* model, const void* x, float* dx, long long slab_stride,
+                                       int rows_cap, const int32_t* row_atom, const int32_t* layout_info,
+                                       const int32_t* aev_blocks, void* act1, void* act2, float* e_member,
+                                       int32_t* status, void* stream);
 
 /* 7. Scatter per-member atomic energies back to input order and reduce per conformer.      */
 /*      atomic_out f32[n] (mean over active members, 0 for padding; flat input order)         */

@@ -94,6 +94,11 @@ _PROTOTYPES = {
                                              _P, _P]),
     "ani_b200_aev_backward_cells": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _P, _I, _P,
                                               _P, _P]),
+    "ani_b200_aev_backward_members": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _I, C.c_longlong, _P, _I, _P,
+                                                _P, _I, _P, _P, _I, _P]),
+    "ani_b200_aev_backward_members_cells": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _I, C.c_longlong, _P, _I,
+                                                      _P, _P, _I, _P, _P, _I, _P, _P]),
+    "ani_b200_ensemble_qbc": (C.c_int, [_P, _P, _I, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
     "ani_b200_verlet_positions":(C.c_int, [_I, _P, _P, _P, _I, _F, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
     "ani_b200_debug_gemm_trace": (C.c_int, [_P, _I]),
     "ani_b200_debug_aev_trace": (C.c_int, [_P]),
@@ -103,6 +108,7 @@ _PROTOTYPES = {
     "ani_b200_mlp_step_windows": (C.c_int, [_P, _I]),
     "ani_b200_mlp_step": (C.c_int, [_P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P]),
     "ani_b200_mlp_step_resident": (C.c_int, [_P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "ani_b200_mlp_step_resident_members": (C.c_int, [_P, _P, _P, C.c_longlong, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
     "ani_b200_mlp_forward": (C.c_int, [_P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P]),
     "ani_b200_zero_live_blocks": (C.c_int, [_P, _P, _P, _P, _P]),
     "ani_b200_mlp_backward": (C.c_int, [_P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _P, _P]),

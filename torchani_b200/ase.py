@@ -43,7 +43,13 @@ class Calculator(AseCalculator):
 
     implemented_properties = ["energy", "free_energy", "forces", "stress"]
 
-    def __init__(self, model, overwrite: bool = False, stress_kind: StressKind = "scaling", skin: float = 0.0):
+    def __init__(self, model, overwrite: bool = False, stress_kind: StressKind = "scaling", skin: float = 0.0,
+                 qbc: bool = False):
+        """``qbc=True``: every calculation also reports the ensemble's disagreement (query-by-committee active
+        learning; HostCalculator.calculate_with_qbc): ``results["energy_qbc"]`` (eV), ``"force_magnitudes"`` (eV/A,
+        per atom), ``"force_relative_stdev"`` and ``"force_relative_range"`` (per atom, dimensionless).  A calculation
+        that also asks for the virial stress (``"scaling"`` / ``"fdotr"``) runs the stress step and then the QBC step on
+        the same positions: the results carry both, at the cost of a second evaluation."""
         super().__init__()
         self.model = model
         buf = next(model.buffers())
@@ -55,6 +61,10 @@ class Calculator(AseCalculator):
         self.overwrite = overwrite
         self.stress_kind = stress_kind
         self.skin = skin
+        self.qbc = bool(qbc)
+        if self.qbc:
+            self.implemented_properties = list(Calculator.implemented_properties) + [
+                "energy_qbc", "force_magnitudes", "force_relative_stdev", "force_relative_range"]
         self._host: tp.Optional[HostCalculator] = None
         self._host_key: tp.Any = None
 
@@ -97,6 +107,12 @@ class Calculator(AseCalculator):
                 raise ValueError("the stress needs a periodic cell")
             e, f, stress = host.calculate_with_stress(positions)
             self.results["stress"] = stress * ha
+            if self.qbc:
+                _, _, q = host.calculate_with_qbc(positions)
+                self._store_qbc(q, ha)
+        elif self.qbc:
+            e, f, q = host.calculate_with_qbc(positions)
+            self._store_qbc(q, ha)
         else:
             e, f = host.calculate(positions)
         self.results["energy"] = e * ha
@@ -104,3 +120,9 @@ class Calculator(AseCalculator):
         self.results["forces"] = f.astype(np.float64) * ha
         if needs_stress and self.stress_kind == "numerical":
             self.results["stress"] = self.calculate_numerical_stress(self.atoms)
+
+    def _store_qbc(self, q, ha: float) -> None:
+        self.results["energy_qbc"] = q.energy_qbc * ha
+        self.results["force_magnitudes"] = q.force_magnitudes.astype(np.float64) * ha
+        self.results["force_relative_stdev"] = q.force_relative_stdev.astype(np.float64)
+        self.results["force_relative_range"] = q.force_relative_range.astype(np.float64)

@@ -23,6 +23,15 @@ from .models import ANI
 HARTREE_TO_EV = 27.211386024367243  # units.py (CODATA 2014, as used by the reference's ASE interface)
 
 
+class QBC(tp.NamedTuple):
+    """Ensemble disagreement of one ``HostCalculator.calculate_with_qbc`` call (arch.py:439-576 of the reference).
+    Shapes are those of a single system; a batch adds a leading conformer axis."""
+    energy_qbc: tp.Any                  # float (Hartree), or (C,) float64: std_m(E_m) / sqrt(real atoms)
+    force_magnitudes: np.ndarray        # (A,) / (C, A) float32 [Hartree/A]: mean over the members of |F_m|
+    force_relative_stdev: np.ndarray    # (A,) / (C, A): (std_m |F_m| + 1e-8) / (mean + 1e-8), unbiased std
+    force_relative_range: np.ndarray    # (A,) / (C, A): (max_m |F_m| - min_m |F_m| + 1e-8) / (mean + 1e-8)
+
+
 class HostCalculator:
     """Energy + forces for a fixed set of atoms from host coordinates.
 
@@ -86,7 +95,9 @@ class HostCalculator:
         # [cell(s) | coords] and ONE D2H copy of [energies | status | gradient] per step
         C_ = self.n_conf
         self.h_in = torch.zeros(self.ws.in_block.numel(), dtype=torch.float32).pin_memory()
-        self.h_out = torch.zeros(self.ws.out_block.numel(), dtype=torch.uint8).pin_memory()
+        # (out_full: out_block followed by what the query-by-committee step adds; calculate copies out_block only)
+        self.h_out_full = torch.zeros(self.ws.out_full.numel(), dtype=torch.uint8).pin_memory()
+        self.h_out = self.h_out_full[:self.ws.out_block.numel()]
         shape = (C_, self.n, 3) if self.batch else (self.n, 3)
         self.h_coords = self.h_in[self.ws.in_coords_off:].view(shape)
         self.h_cell = self.h_in[:9]
@@ -95,6 +106,10 @@ class HostCalculator:
         self.h_grad = self.h_out[off:].view(torch.float32).view(shape)
         self.h_energy = self.h_out[:8 * C_].view(torch.float64)
         self.h_status = self.h_out[8 * C_:8 * C_ + 4].view(torch.int32)
+        q0, s0 = self.ws._out_qbc_off, self.ws._out_stats_off
+        M = self.engine.nets.num_members
+        self.h_energy_qbc = self.h_out_full[q0 + 8 * M * C_:q0 + 8 * (M + 1) * C_].view(torch.float64)
+        self.h_atom_stats = self.h_out_full[s0:].view(torch.float32).view((3,) + shape[:-1])
         self.h_moved = torch.zeros(1, dtype=torch.int32).pin_memory()
         self._have_grid = False       # a grid built with the skin exists and may be reused
         self.rebuilds = 0             # steps that built the grid
@@ -103,7 +118,7 @@ class HostCalculator:
         self.d2h_bytes = self.h_out.numel()
         self.graph_after = 3          # eager host-driven steps before copies + kernels are captured as one graph
         self._calls = 0
-        self._graphs: tp.Dict[bool, torch.cuda.CUDAGraph] = {}   # reuse flag -> captured step
+        self._graphs: tp.Dict[tp.Any, torch.cuda.CUDAGraph] = {}   # reuse flag (or ("qbc", reuse)) -> captured step
         self._mode_calls = {False: 0, True: 0}
         self._graph_version: tp.Any = None
         if pbc and cell is None:
@@ -194,6 +209,37 @@ class HostCalculator:
             return self.h_energy.numpy().copy(), np.negative(self.h_grad.numpy())
         return float(self.h_energy[0]), np.negative(self.h_grad.numpy())
 
+    def calculate_with_qbc(self, positions, cell=None) -> tp.Tuple[tp.Any, np.ndarray, QBC]:
+        """``calculate`` plus the ensemble's disagreement, for query-by-committee active learning: (energy [Hartree],
+        forces [Hartree/A], ``QBC``).  One step evaluates every active member's forces (one AEV-backward launch for
+        all of them) and the statistics on the device; like ``calculate`` it is one H2D and one D2H copy per call and,
+        after a few calls, its own captured CUDA graph.  Energy and forces are the ensemble mean, as from
+        ``calculate``.  Works with ``skin > 0`` and with batches; not with multi-GPU sharding."""
+        if self.sharded is not None or tuple(self.shard) != (0, 1):
+            raise ValueError("calculate_with_qbc runs on one GPU: no sharding")
+        if cell is not None:
+            self.set_cell(cell)
+        self._set_positions(positions)
+        eng = self.engine
+        self._calls += 1
+        if self._graphs and self._graph_version != eng.nets.active_key:
+            self._graphs = {}   # the active ensemble members changed: the captured launches are stale
+        reuse = self.skin > 0 and self._have_grid
+        self._run(reuse, members=True)
+        if reuse and (int(self.h_moved[0]) & 1):
+            self.redone += 1   # an atom left its skin/2 sphere: rebuild, redo
+            self._run(False, members=True)
+        elif reuse and int(self.h_moved[0]):
+            self._have_grid = False
+        if int(self.h_status[0]) and self._check_or_switch():
+            return self.calculate_with_qbc(positions)
+        stats = self.h_atom_stats.numpy().copy()
+        eq = self.h_energy_qbc.numpy().copy() if self.batch else float(self.h_energy_qbc[0])
+        qbc = QBC(eq, stats[0], stats[1], stats[2])
+        if self.batch:
+            return self.h_energy.numpy().copy(), np.negative(self.h_grad.numpy()), qbc
+        return float(self.h_energy[0]), np.negative(self.h_grad.numpy()), qbc
+
     def _check_or_switch(self) -> bool:
         """Raise what the reference raises for the status word of the last step.  If the 2 x fp16 operand format ran
         out of range, rebuild on the 3 x bfloat16 build of the library instead and return True: the caller redoes the
@@ -216,11 +262,40 @@ class HostCalculator:
             return True
         return False
 
-    def _run(self, reuse: bool) -> None:
+    def _run(self, reuse: bool, members: bool = False) -> None:
         """One step (H2D, kernels, D2H, synchronise); after a few eager uses of a mode its whole sequence
-        is captured into one CUDA graph."""
+        is captured into one CUDA graph.  ``members``: the query-by-committee step (Engine.run(..., members=True))."""
         with torch.cuda.device(self.device):   # the C-ABI launches on the current device's stream
-            self._run_on_device(reuse)
+            if members:
+                self._run_members(reuse)
+            else:
+                self._run_on_device(reuse)
+
+    def _run_members(self, reuse: bool) -> None:
+        ws, eng = self.ws, self.engine
+        key = ("qbc", reuse)
+        self._mode_calls[key] = self._mode_calls.get(key, 0) + 1
+        if not reuse:
+            self.rebuilds += 1
+        eng.members_buffers(ws)
+        graph = self._graphs.get(key)
+        if graph is None and eng.cuda_graph and not eng.profile and self._mode_calls[key] > self.graph_after:
+            eng.note_composition(ws)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                self._copies_in(reuse)
+                eng._launch(ws, self.pbc, True, 0, ws.n, reuse, conformer_cells=self.conformer_cells, members=True)
+                self._copies_out(reuse, members=True)
+            self._graphs[key], self._graph_version = graph, eng.nets.active_key
+        if graph is not None:
+            graph.replay()
+        else:
+            self._copies_in(reuse)
+            eng.run(ws, self.pbc, want_grad=True, reuse=reuse, conformer_cells=self.conformer_cells, members=True)
+            self._copies_out(reuse, members=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        if not reuse:
+            self._have_grid = self.skin > 0
 
     def _run_on_device(self, reuse: bool) -> None:
         ws, eng = self.ws, self.engine
@@ -264,8 +339,11 @@ class HostCalculator:
             self.ws.moved.zero_()
         self.ws.in_block.copy_(self.h_in, non_blocking=True)
 
-    def _copies_out(self, reuse: bool = False) -> None:
-        self.h_out.copy_(self.ws.out_block, non_blocking=True)
+    def _copies_out(self, reuse: bool = False, members: bool = False) -> None:
+        if members:
+            self.h_out_full.copy_(self.ws.out_full, non_blocking=True)
+        else:
+            self.h_out.copy_(self.ws.out_block, non_blocking=True)
         if reuse:
             self.h_moved.copy_(self.ws.moved, non_blocking=True)
 

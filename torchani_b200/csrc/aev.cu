@@ -55,6 +55,11 @@ constexpr int AEV_WARPS = 4;  // warps (= central atoms) per CTA
 #ifndef ANI_AEV_BWD_MIN_CTAS
 #define ANI_AEV_BWD_MIN_CTAS 7  // register budget of the backward kernel: 7 CTAs (28 warps) per SM
 #endif
+// the member loop of k_aev_backward_members keeps more state live: its ANI-2x form (8 x 4 angular terms) spills at 7
+// and 6 CTAs per SM (72, 80 registers), not at 5 (96); the 4 x 8 form needs one CTA fewer (128)
+#ifndef ANI_AEV_BWD_MEMBERS_MIN_CTAS
+#define ANI_AEV_BWD_MEMBERS_MIN_CTAS 5
+#endif
 
 struct NeighbourRange {
   int lo, hi, code;
@@ -1415,6 +1420,312 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
 }
 
 // ---------------------------------------------------------------------------------------
+// backward of every ensemble member in one launch (query-by-committee statistics)
+// ---------------------------------------------------------------------------------------
+// Active members of an ani_b200_aev_backward_members call: output k contracts slab idx[k]
+struct MemberSlabs {
+  int count;
+  int idx[ANI_MAX_MEMBERS];
+  long long stride;  // floats between the dE/dAEV slabs of consecutive members
+};
+
+// k_aev_backward with the per-member work in a loop.  A warp rebuilds its atom's neighbour geometry (distances,
+// cutoffs, image shifts, the angular list) once; then, for k = 0 .. count - 1, it contracts member idx[k]'s dE/dAEV row
+// and scatters into grad_members[k].  The rows are staged in two shared-memory buffers with cp.async: member k + 1's
+// row is in flight while member k is contracted, so shared memory per warp does not depend on the number of members.
+// The arithmetic of one member is that of k_aev_backward (same order within an atom): only the order of the float
+// atomics differs.  No explicit neighbour rows and no virial.
+template <int NA, int NZ, bool LAT = false>
+__global__ void __launch_bounds__(AEV_WARPS * 32, NA == 8 ? ANI_AEV_BWD_MEMBERS_MIN_CTAS : ANI_AEV_BWD_MEMBERS_MIN_CTAS - 1)
+    k_aev_backward_members(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
+                           const float4* __restrict__ spos, const int32_t* __restrict__ sorted_orig, int lo, int hi,
+                           const int32_t* __restrict__ row_of, const float* __restrict__ slabs, int ldx,
+                           const int32_t* __restrict__ nbr_cnt, const int32_t* __restrict__ nbr_list,
+                           const int32_t* __restrict__ species_mask, int cap, float* __restrict__ grad_members,
+                           long long grad_stride, int32_t* __restrict__ status, size_t warp_bytes, int pair_cap,
+                           int gbuf_floats, const float* __restrict__ lattice, const __grid_constant__ MemberSlabs ms) {
+  static_assert(NA * NZ == 32, "one lane per angular feature");
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const ani_grid g = *grid;
+  hi = min(hi, g.n_real);
+  const int i = lo + blockIdx.x * AEV_WARPS + warp;
+  if (i >= hi) return;
+  const WarpSmem s = carve(smem_raw + warp * warp_bytes, cap, true);
+  const int S = P.num_species;
+  const int nR = P.n_shf_r;
+  const int RL = S * nR;
+  constexpr int GSTRIDE = 36;
+  const unsigned present = (species_mask ? (unsigned)species_mask[0] : 0xffffffffu) & ((1u << S) - 1u);
+  const int n_present = __popc(present);
+  // [buffer 0 | buffer 1] of {g_rad [RL], g_ang [pair_cap][36]}, then dfc(R; Rcr) per neighbour
+  float* ndfc = s.rad + 2 * gbuf_floats;
+  const size_t row = (size_t)row_of[i] * ldx;
+
+  auto copy_async4 = [](float* dst_smem, const float* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src)
+                 : "memory");
+  };
+  // member k's row -> buffer k & 1 (one commit group per member; an empty group past the last member)
+  auto stage = [&](int k) {
+    if (k < ms.count) {
+      const float* gaev = slabs + (size_t)ms.idx[k] * ms.stride + row;
+      float* g_rad = s.rad + (k & 1) * gbuf_floats;
+      float* g_ang = g_rad + ((RL + 3) & ~3);
+      for (int t = lane; t < RL; t += 32) copy_async4(g_rad + t, gaev + t);
+      int c1 = 0;
+      for (unsigned m1 = present; m1; m1 &= m1 - 1, ++c1) {
+        const int s1 = __ffs(m1) - 1;
+        const int base = s1 * (2 * S - s1 + 1) / 2 - s1;
+        int c2 = c1;
+        for (unsigned m2 = m1; m2; m2 &= m2 - 1, ++c2) {
+          const int pp = base + __ffs(m2) - 1;
+          const int cp = c1 * (2 * n_present - c1 + 1) / 2 + (c2 - c1);
+          if (cp < pair_cap) copy_async4(g_ang + cp * GSTRIDE + lane, gaev + RL + P.ang_pad + pp * 32 + lane);
+        }
+      }
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  stage(0);
+
+  // ---- geometry of the stored neighbours, once for all members
+  const float4 pi = spos[i];
+  const int cnt = nbr_cnt[i];
+  const int conf_i = LAT ? sorted_orig[i] / g.n_per_conf : 0;
+  for (int n = lane; n < cnt; n += 32) {
+    const int word = nbr_list[(size_t)i * cap + n];
+    const int j = word & ANI_IDX_MASK;
+    const int code = (unsigned)word >> ANI_IMG_SHIFT;
+    const float4 p = spos[j];
+    float3 sh = make_float3(0.f, 0.f, 0.f);
+    if (code != 13) sh = LAT ? image_shift(lattice, conf_i, code) : image_shift(g, code);
+    const float dx = (p.x + sh.x) - pi.x, dy = (p.y + sh.y) - pi.y, dz = (p.z + sh.z) - pi.z;
+    const float4 dR = make_float4(dx, dy, dz, sqrtf(dx * dx + dy * dy + dz * dz));
+    s.nd[n] = dR;
+    s.nj[n] = j;
+    s.nsp[n] = (unsigned char)__float_as_int(p.w);
+    float fc, dfc;
+    cutoff_value_grad(dR.w, P.rcr, P.cutoff_kind, fc, dfc);
+    s.nfc[n] = fc;
+    ndfc[n] = dfc;
+  }
+  __syncwarp();
+  const int n_ang = compact_angular_list(P, s, cnt, lane, status);
+  const int oi = sorted_orig[i];
+
+  for (int k = 0; k < ms.count; ++k) {
+    stage(k + 1);
+    asm volatile("cp.async.wait_group 1;" ::: "memory");  // member k's row has landed
+    __syncwarp();
+    const float* g_rad = s.rad + (k & 1) * gbuf_floats;
+    const float* g_ang = g_rad + ((RL + 3) & ~3);
+    const float* gaev = slabs + (size_t)ms.idx[k] * ms.stride + row;
+    float* gout = grad_members + (size_t)k * grad_stride;
+
+    // ---- radial
+    for (int n = lane; n < cnt; n += 32) {
+      const float4 d = s.nd[n];
+      const float fc = s.nfc[n], dfc = ndfc[n];
+      const float* __restrict__ gr = g_rad + s.nsp[n] * nR;
+      float acc = 0.f;
+#pragma unroll 4
+      for (int m = 0; m < nR; ++m) {
+        const float x = d.w - P.shf_r[m];
+        const float G = 0.25f * fast_exp(-P.eta_r * x * x);
+        acc = fmaf(gr[m] * G, fmaf(-2.0f * P.eta_r * x, fc, dfc), acc);
+      }
+      const float sc = d.w > 1e-10f ? acc * fast_rcp(d.w) : 0.f;
+      s.fgrad[3 * n + 0] = sc * d.x;
+      s.fgrad[3 * n + 1] = sc * d.y;
+      s.fgrad[3 * n + 2] = sc * d.z;
+    }
+    __syncwarp();
+
+    // ---- angular (as in k_aev_backward)
+    if (n_ang >= 2) {
+      // (the angular constants are read from the kernel parameters, constant-bank operands, not held in registers)
+      auto pair_sums = [&](const float4& dj, const float4& dk, int sj, int sk, float& cosT, float& inv_rr, float& S0,
+                           float& S1, float& S2) {
+        const float dot = dj.x * dk.x + dj.y * dk.y + dj.z * dk.z;
+        inv_rr = fast_rcp(fmaxf(dj.w * dk.w, 1e-10f));
+        cosT = dot * inv_rr;
+        const float c = 0.95f * cosT;
+        const float sn = fast_sqrt(fmaxf(1.0f - c * c, 0.f));
+        const float c_over_s = c * fast_rcp(sn);
+        const float rbar = 0.5f * (dj.w + dk.w);
+        const int cj = __popc(present & ((1u << sj) - 1u)), ck = __popc(present & ((1u << sk) - 1u));
+        const int clo = min(cj, ck), chi = max(cj, ck);
+        const int cp = clo * (2 * n_present - clo + 1) / 2 + (chi - clo);
+        const float4* __restrict__ gp =
+            cp < pair_cap ? reinterpret_cast<const float4*>(g_ang + cp * GSTRIDE)
+                          : reinterpret_cast<const float4*>(gaev + RL + P.ang_pad + pair_index(sj, sk, S) * 32);
+        float tz[NZ], uz[NZ];
+#pragma unroll
+        for (int z = 0; z < NZ; ++z) tz[z] = uz[z] = 0.f;
+#pragma unroll
+        for (int a = 0; a < NA; ++a) {
+          const float d = rbar - P.shf_a[a];
+          const float f2 = fast_exp(-P.eta_a * d * d);
+          const float f2p = -2.0f * P.eta_a * d * f2;
+#pragma unroll
+          for (int q = 0; q < NZ / 4; ++q) {
+            const float4 gv = gp[a * (NZ / 4) + q];
+            tz[4 * q + 0] = fmaf(gv.x, f2, tz[4 * q + 0]);
+            tz[4 * q + 1] = fmaf(gv.y, f2, tz[4 * q + 1]);
+            tz[4 * q + 2] = fmaf(gv.z, f2, tz[4 * q + 2]);
+            tz[4 * q + 3] = fmaf(gv.w, f2, tz[4 * q + 3]);
+            uz[4 * q + 0] = fmaf(gv.x, f2p, uz[4 * q + 0]);
+            uz[4 * q + 1] = fmaf(gv.y, f2p, uz[4 * q + 1]);
+            uz[4 * q + 2] = fmaf(gv.z, f2p, uz[4 * q + 2]);
+            uz[4 * q + 3] = fmaf(gv.w, f2p, uz[4 * q + 3]);
+          }
+        }
+        S0 = S1 = S2 = 0.f;
+#pragma unroll
+        for (int z = 0; z < NZ; ++z) {
+          const float base = fmaxf(0.5f * (1.0f + c * P.cos_z[z] + sn * P.sin_z[z]), 0.f);
+          const float lg = fast_log2(base);
+          const float f1 = fast_exp2(P.zeta * lg);
+          const float pw1 = fast_exp2((P.zeta - 1.0f) * lg);
+          const float f1p = P.zeta * pw1 * (0.475f * (P.cos_z[z] - c_over_s * P.sin_z[z]));
+          S0 = fmaf(f1, tz[z], S0);
+          S1 = fmaf(f1p, tz[z], S1);
+          S2 = fmaf(f1, uz[z], S2);
+        }
+      };
+      int lpr = 1;
+      while (lpr * 2 * n_ang <= 32) lpr *= 2;
+      const int sub = lane % lpr;
+      if (n_ang <= 32) {
+        // rotation over unordered pairs, see k_aev_backward
+        const int j = lane / lpr;
+        const bool jvalid = j < n_ang;
+        const int half_n = n_ang >> 1;
+        const bool even = (n_ang & 1) == 0;
+        float gx = 0.f, gy = 0.f, gz = 0.f;
+        int nj_ = 0, sj = 0;
+        float4 dj = make_float4(0.f, 0.f, 0.f, 1.f);
+        float fcj = 0.f, dfcj = 0.f, inv_rj = 0.f;
+        if (jvalid) {
+          nj_ = s.aidx[j];
+          dj = s.nd[nj_];
+          fcj = s.afc[j];
+          dfcj = s.afcd[j];
+          sj = s.nsp[nj_];
+          inv_rj = dj.w > 1e-10f ? fast_rcp(dj.w) : 0.f;
+        }
+        const int steps = (half_n + lpr - 1) / lpr;
+        for (int it = 0; it < steps; ++it) {
+          const int t = 1 + it * lpr + sub;
+          const bool active = jvalid && t <= half_n && !(even && t == half_n && j >= half_n);
+          float px = 0.f, py = 0.f, pz = 0.f;
+          if (active) {
+            int kk = j + t;
+            if (kk >= n_ang) kk -= n_ang;
+            const int nk_ = s.aidx[kk];
+            const float4 dk = s.nd[nk_];
+            const float fck = s.afc[kk], dfck = s.afcd[kk];
+            const float inv_rk = dk.w > 1e-10f ? fast_rcp(dk.w) : 0.f;
+            float cosT, inv_rr, S0, S1, S2;
+            pair_sums(dj, dk, sj, (int)s.nsp[nk_], cosT, inv_rr, S0, S1, S2);
+            const float W = fcj * fck;
+            const float dEdcos = 2.0f * W * S1;
+            const float dEdRj = S2 * W + 2.0f * S0 * dfcj * fck;
+            const float dEdRk = S2 * W + 2.0f * S0 * fcj * dfck;
+            const float coefj = (dEdRj - dEdcos * cosT * inv_rj) * inv_rj;
+            const float coefk = (dEdRk - dEdcos * cosT * inv_rk) * inv_rk;
+            const float coefx = dEdcos * inv_rr;
+            gx += coefj * dj.x + coefx * dk.x;
+            gy += coefj * dj.y + coefx * dk.y;
+            gz += coefj * dj.z + coefx * dk.z;
+            px = coefk * dk.x + coefx * dj.x;
+            py = coefk * dk.y + coefx * dj.y;
+            pz = coefk * dk.z + coefx * dj.z;
+          }
+          int src_row = j - t;
+          if (src_row < 0) src_row += n_ang;
+          const int src_lane = jvalid ? src_row * lpr + sub : lane;
+          const float rx = __shfl_sync(ANI_FULL_MASK, px, src_lane);
+          const float ry = __shfl_sync(ANI_FULL_MASK, py, src_lane);
+          const float rz = __shfl_sync(ANI_FULL_MASK, pz, src_lane);
+          if (jvalid) {
+            gx += rx;
+            gy += ry;
+            gz += rz;
+          }
+        }
+        for (int o = lpr / 2; o > 0; o >>= 1) {
+          gx += __shfl_xor_sync(ANI_FULL_MASK, gx, o);
+          gy += __shfl_xor_sync(ANI_FULL_MASK, gy, o);
+          gz += __shfl_xor_sync(ANI_FULL_MASK, gz, o);
+        }
+        if (jvalid && sub == 0) {
+          s.fgrad[3 * nj_ + 0] += gx;
+          s.fgrad[3 * nj_ + 1] += gy;
+          s.fgrad[3 * nj_ + 2] += gz;
+        }
+      } else {
+        // more rows than lanes: ordered pairs (j, k), several passes of 32 rows
+        for (int row0 = 0; row0 < n_ang; row0 += 32) {
+          const int j = row0 + lane;
+          float gx = 0.f, gy = 0.f, gz = 0.f;
+          if (j < n_ang) {
+            const int nj_ = s.aidx[j];
+            const float4 dj = s.nd[nj_];
+            const float fcj = s.afc[j], dfcj = s.afcd[j];
+            const int sj = s.nsp[nj_];
+            const float inv_rj = dj.w > 1e-10f ? fast_rcp(dj.w) : 0.f;
+            for (int kk = 0; kk < n_ang; ++kk) {
+              if (kk == j) continue;
+              const int nk_ = s.aidx[kk];
+              const float4 dk = s.nd[nk_];
+              const float fck = s.afc[kk];
+              float cosT, inv_rr, S0, S1, S2;
+              pair_sums(dj, dk, sj, (int)s.nsp[nk_], cosT, inv_rr, S0, S1, S2);
+              const float W = fcj * fck;
+              const float dEdRj = S2 * W + 2.0f * S0 * dfcj * fck;
+              const float dEdcos = 2.0f * W * S1;
+              const float coefj = (dEdRj - dEdcos * cosT * inv_rj) * inv_rj;
+              const float coefk = dEdcos * inv_rr;
+              gx += coefj * dj.x + coefk * dk.x;
+              gy += coefj * dj.y + coefk * dk.y;
+              gz += coefj * dj.z + coefk * dk.z;
+            }
+            s.fgrad[3 * nj_ + 0] += gx;
+            s.fgrad[3 * nj_ + 1] += gy;
+            s.fgrad[3 * nj_ + 2] += gz;
+          }
+        }
+      }
+    }
+    __syncwarp();
+
+    // ---- scatter into member k's gradient: neighbour j gets +dE_i/dr_j, the centre minus the sum
+    float sx = 0.f, sy = 0.f, sz_ = 0.f;
+    for (int n = lane; n < cnt; n += 32) {
+      const float fx = s.fgrad[3 * n], fy = s.fgrad[3 * n + 1], fz = s.fgrad[3 * n + 2];
+      const int oj = sorted_orig[s.nj[n]];
+      atomicAdd(&gout[3 * (size_t)oj + 0], fx);
+      atomicAdd(&gout[3 * (size_t)oj + 1], fy);
+      atomicAdd(&gout[3 * (size_t)oj + 2], fz);
+      sx += fx;
+      sy += fy;
+      sz_ += fz;
+    }
+    sx = warp_sum(sx);
+    sy = warp_sum(sy);
+    sz_ = warp_sum(sz_);
+    if (lane == 0) {
+      atomicAdd(&gout[3 * (size_t)oi + 0], -sx);
+      atomicAdd(&gout[3 * (size_t)oi + 1], -sy);
+      atomicAdd(&gout[3 * (size_t)oi + 2], -sz_);
+    }
+    __syncwarp();  // fgrad and buffer k & 1 are rewritten by the next member
+  }
+}
+
+// ---------------------------------------------------------------------------------------
 // reference-format half neighbour list (API parity path; one thread per atom)
 // ---------------------------------------------------------------------------------------
 template <bool FILL>
@@ -1686,6 +1997,64 @@ static int launch_aev_backward(const ani_aev_params* params, const ani_grid* gri
   return ANI_OK;
 }
 
+static int launch_aev_backward_members(const ani_aev_params* params, const ani_grid* grid, const float* spos,
+                                       const int32_t* sorted_orig, const int32_t* species_mask, int n, int lo, int hi,
+                                       const int32_t* row_of, const float* slabs, int ldx, long long slab_stride,
+                                       const int32_t* members, int n_members, const int32_t* nbr_cnt,
+                                       const int32_t* nbr_list, int nbr_cap, float* grad_members, int32_t* status,
+                                       int max_elements, const float* lattice, void* stream) {
+  int rc = check_params(params);
+  if (rc != ANI_OK) return rc;
+  if (!grid || !spos || !sorted_orig || !row_of || !slabs || !grad_members || !status || !nbr_cnt || !nbr_list)
+    return ANI_ERR_BAD_ARG;
+  if (lo < 0 || hi > n || lo > hi) return ANI_ERR_BAD_ARG;
+  if (nbr_cap < 32 || nbr_cap > 256 || nbr_cap % 32) return ANI_ERR_BAD_ARG;
+  if (n_members < 1 || n_members > ANI_MAX_MEMBERS || !members || slab_stride < (long long)ldx) return ANI_ERR_BAD_ARG;
+  MemberSlabs ms;
+  ms.count = n_members;
+  ms.stride = slab_stride;
+  for (int k = 0; k < ANI_MAX_MEMBERS; ++k) ms.idx[k] = 0;
+  for (int k = 0; k < n_members; ++k) {
+    if (members[k] < 0 || members[k] >= ANI_MAX_MEMBERS) return ANI_ERR_BAD_ARG;
+    ms.idx[k] = members[k];
+  }
+  if (hi == lo) return ANI_OK;
+  const int S = params->num_species;
+  const int RL = S * params->n_shf_r;
+  const int NP = S * (S + 1) / 2;
+  // the shared-memory gradient table as in launch_aev_backward; two of them (double-buffered rows), plus dfc per
+  // neighbour
+  const int E = (max_elements > 0 && max_elements < S) ? max_elements : S;
+  const bool ang_aligned = (RL + params->ang_pad) % 4 == 0 && ldx % 4 == 0 && ((uintptr_t)slabs & 15) == 0 &&
+                           slab_stride % 4 == 0;
+  const int pair_cap = (species_mask && ang_aligned) ? E * (E + 1) / 2 : NP;
+  const int gbuf = ((RL + 3) & ~3) + 36 * pair_cap;
+  const size_t wb = warp_smem_bytes(nbr_cap, 2 * gbuf + nbr_cap, true);
+  const size_t smem = wb * AEV_WARPS;
+  const int blocks = (hi - lo + AEV_WARPS - 1) / AEV_WARPS;
+  cudaStream_t st = (cudaStream_t)stream;
+  const float4* sp4 = reinterpret_cast<const float4*>(spos);
+  auto go = [&](auto k) {
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    k<<<blocks, AEV_WARPS * 32, smem, st>>>(*params, grid, sp4, sorted_orig, lo, hi, row_of, slabs, ldx, nbr_cnt,
+                                            nbr_list, species_mask, nbr_cap, grad_members, 3LL * n, status, wb,
+                                            pair_cap, gbuf, lattice, ms);
+  };
+  if (params->n_shf_a == 8) {
+    if (lattice)
+      go(k_aev_backward_members<8, 4, true>);
+    else
+      go(k_aev_backward_members<8, 4>);
+  } else {
+    if (lattice)
+      go(k_aev_backward_members<4, 8, true>);
+    else
+      go(k_aev_backward_members<4, 8>);
+  }
+  ANI_CUDA_CHECK_LAUNCH();
+  return ANI_OK;
+}
+
 // ---- half pair list -> per-atom rows (both directions) ------------------------------------
 __global__ void k_pairs_count(const int64_t* __restrict__ idx0, const int64_t* __restrict__ idx1, long long P,
                               int32_t* __restrict__ counts) {
@@ -1820,6 +2189,31 @@ extern "C" int ani_b200_aev_backward_cells(const ani_aev_params* params, const a
   return launch_aev_backward(params, grid, spos, sorted_orig, n, lo, hi, row_of, grad_aev, ldx, nbr_cnt, nbr_list,
                              ExplicitNbrs{nullptr, nullptr, nullptr}, species_mask, nbr_cap, grad_coords, status,
                              stream, max_elements, virial, lattice);
+}
+
+extern "C" int ani_b200_aev_backward_members(const ani_aev_params* params, const ani_grid* grid, const float* spos,
+                                             const int32_t* sorted_orig, const int32_t* species_mask, int n, int lo,
+                                             int hi, const int32_t* row_of, const float* grad_slabs, int ldx,
+                                             long long slab_stride, const int32_t* members, int n_members,
+                                             const int32_t* nbr_cnt, const int32_t* nbr_list, int nbr_cap,
+                                             float* grad_members, int32_t* status, int max_elements, void* stream) {
+  return launch_aev_backward_members(params, grid, spos, sorted_orig, species_mask, n, lo, hi, row_of, grad_slabs, ldx,
+                                     slab_stride, members, n_members, nbr_cnt, nbr_list, nbr_cap, grad_members, status,
+                                     max_elements, nullptr, stream);
+}
+
+extern "C" int ani_b200_aev_backward_members_cells(const ani_aev_params* params, const ani_grid* grid,
+                                                   const float* spos, const int32_t* sorted_orig,
+                                                   const int32_t* species_mask, int n, int lo, int hi,
+                                                   const int32_t* row_of, const float* grad_slabs, int ldx,
+                                                   long long slab_stride, const int32_t* members, int n_members,
+                                                   const int32_t* nbr_cnt, const int32_t* nbr_list, int nbr_cap,
+                                                   float* grad_members, int32_t* status, int max_elements,
+                                                   const float* lattice, void* stream) {
+  if (!lattice) return ANI_ERR_BAD_ARG;
+  return launch_aev_backward_members(params, grid, spos, sorted_orig, species_mask, n, lo, hi, row_of, grad_slabs, ldx,
+                                     slab_stride, members, n_members, nbr_cnt, nbr_list, nbr_cap, grad_members, status,
+                                     max_elements, lattice, stream);
 }
 
 extern "C" int ani_b200_pairs_to_rows(const int64_t* idx0, const int64_t* idx1, const float* diff_vectors,

@@ -596,16 +596,14 @@ extern "C" int ani_b200_mlp_step(const ani_mlp_model* model, const void* x, floa
 }
 
 // ---- the whole MLP of a step as ONE launch of resident chains (mlp_resident.cuh) ----------------------------------
-extern "C" int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void* x, float* dx, int rows_cap,
-                                          const int32_t* row_atom, const int32_t* layout_info,
-                                          const int32_t* aev_blocks, void* act1, void* act2, float* e_member,
-                                          int32_t* status, void* stream) {
+#if ANI_OPND_FP16X2
+// the kernel arguments of both resident entry points (~2 KB, built in place, passed by value as __grid_constant__)
+static int resident_args(const ani_mlp_model* model, const void* x, float* dx, int rows_cap, const int32_t* row_atom,
+                         const int32_t* layout_info, const int32_t* aev_blocks, void* act1, void* act2,
+                         float* e_member, int32_t* status, tc::ResArgs& F) {
   if (!x || !dx || !e_member || !row_atom || !layout_info || !act1 || !act2) return ANI_ERR_BAD_ARG;
   const int rc = check_model(model, rows_cap);
   if (rc != ANI_OK) return rc;
-#if !ANI_OPND_FP16X2
-  return ANI_ERR_UNSUPPORTED;  // 3 x bf16 K-blocks are 24 KB: R would need 192 KB
-#else
   const int S = model->num_species, M = model->num_members, ldx = model->ldx;
   for (int s = 0; s < S; ++s) {
     const ani_mlp_species& p = model->sp[s];
@@ -613,7 +611,6 @@ extern "C" int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void
       return ANI_ERR_UNSUPPORTED;
   }
   if (ldx / 32 > tc::MAX_BLOCKS) return ANI_ERR_UNSUPPORTED;
-  static tc::ResArgs F;   // ~2 KB: built in place, passed by value (__grid_constant__)
   const float sv = OPND_SCALE_VALUE, sg = OPND_SCALE_GRAD;
   const bool compact = use_b1_compact(model, aev_blocks);
   F.x = static_cast<const unsigned char*>(x);
@@ -668,15 +665,75 @@ extern "C" int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void
       F.order[j] = F.order[j - 1];
       F.order[j - 1] = t;
     }
+  F.slab_stride = 0;
+  F.n_chain_members = M;
+  for (int m = 0; m < ANI_MAX_MEMBERS; ++m) F.member_of[m] = m;
+  return ANI_OK;
+}
+#endif
+
+extern "C" int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void* x, float* dx, int rows_cap,
+                                          const int32_t* row_atom, const int32_t* layout_info,
+                                          const int32_t* aev_blocks, void* act1, void* act2, float* e_member,
+                                          int32_t* status, void* stream) {
+#if !ANI_OPND_FP16X2
+  if (!x || !dx || !e_member || !row_atom || !layout_info || !act1 || !act2) return ANI_ERR_BAD_ARG;
+  const int rc = check_model(model, rows_cap);
+  if (rc != ANI_OK) return rc;
+  return ANI_ERR_UNSUPPORTED;  // 3 x bf16 K-blocks are 24 KB: R would need 192 KB
+#else
+  static tc::ResArgs F;   // ~2 KB: built in place, passed by value (__grid_constant__)
+  const int rc = resident_args(model, x, dx, rows_cap, row_atom, layout_info, aev_blocks, act1, act2, e_member, status, F);
+  if (rc != ANI_OK) return rc;
   static const bool attr = []() {
-    return cudaFuncSetAttribute(tc::k_mlp_resident, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::RES_SMEM_BYTES) ==
-           cudaSuccess;
+    return cudaFuncSetAttribute(tc::k_mlp_resident<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                tc::RES_SMEM_BYTES) == cudaSuccess;
   }();
   (void)attr;
   cudaStream_t st = (cudaStream_t)stream;
   // zero the live blocks of dx (the members' REDs accumulate into it) and gather the compact W1^T operands
-  launch_zero_compact(model, M > 1 ? dx : nullptr, layout_info, aev_blocks, st);
-  tc::k_mlp_resident<<<num_sms(), tc::THREADS, tc::RES_SMEM_BYTES, st>>>(F);
+  launch_zero_compact(model, model->num_members > 1 ? dx : nullptr, layout_info, aev_blocks, st);
+  tc::k_mlp_resident<false><<<num_sms(), tc::THREADS, tc::RES_SMEM_BYTES, st>>>(F);
+  ANI_CUDA_CHECK_LAUNCH();
+  return ANI_OK;
+#endif
+}
+
+// ---- the same launch with one dE/dAEV slab per member (query-by-committee step) ------------------------------------
+extern "C" int ani_b200_mlp_step_resident_members(const ani_mlp_model* model, const void* x, float* dx,
+                                                  long long slab_stride, int rows_cap, const int32_t* row_atom,
+                                                  const int32_t* layout_info, const int32_t* aev_blocks, void* act1,
+                                                  void* act2, float* e_member, int32_t* status, void* stream) {
+#if !ANI_OPND_FP16X2
+  if (!x || !dx || !e_member || !row_atom || !layout_info || !act1 || !act2) return ANI_ERR_BAD_ARG;
+  const int rc = check_model(model, rows_cap);
+  if (rc != ANI_OK) return rc;
+  return ANI_ERR_UNSUPPORTED;
+#else
+  static tc::ResArgs F;
+  const int rc = resident_args(model, x, dx, rows_cap, row_atom, layout_info, aev_blocks, act1, act2, e_member, status, F);
+  if (rc != ANI_OK) return rc;
+  if (slab_stride < (long long)rows_cap * model->ldx) return ANI_ERR_BAD_ARG;
+  // chains of the active members only (member_scale != 0); the e_member rows of the others are zeroed, so that the
+  // energy reduction's weighted sum never meets what an earlier step left there
+  cudaStream_t st = (cudaStream_t)stream;
+  F.slab_stride = slab_stride;
+  F.n_chain_members = 0;
+  for (int m = 0; m < model->num_members; ++m) {
+    if (model->member_scale[m] != 0.f)
+      F.member_of[F.n_chain_members++] = m;
+    else
+      cudaMemsetAsync(e_member + (size_t)m * rows_cap, 0, sizeof(float) * (size_t)rows_cap, st);
+  }
+  if (F.n_chain_members == 0) return ANI_ERR_BAD_ARG;
+  static const bool attr = []() {
+    return cudaFuncSetAttribute(tc::k_mlp_resident<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                tc::RES_SMEM_BYTES) == cudaSuccess;
+  }();
+  (void)attr;
+  // gather the compact W1^T operands; the slabs take plain stores and need no zero-fill
+  launch_zero_compact(model, nullptr, layout_info, aev_blocks, st);
+  tc::k_mlp_resident<true><<<num_sms(), tc::THREADS, tc::RES_SMEM_BYTES, st>>>(F);
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
 #endif

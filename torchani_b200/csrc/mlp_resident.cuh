@@ -87,6 +87,11 @@ struct ResArgs {
   int order[ANI_MAX_SPECIES];          // species by decreasing chain length: the longest chains start first
   float member_scale[ANI_MAX_MEMBERS];
   ResSpecies sp[ANI_MAX_SPECIES];
+  // per-member slabs (k_mlp_resident<true>): the chains of a row tile are those of the n_chain_members members
+  // member_of[0..), and phase 5 stores member m's dE/dAEV into dx + m * slab_stride instead of reducing into dx
+  long long slab_stride;
+  int n_chain_members;
+  int member_of[ANI_MAX_MEMBERS];
 };
 
 #if ANI_OPND_FP16X2
@@ -158,15 +163,18 @@ __device__ __forceinline__ void res_mma_slot(float (&d0)[32], float (&d1)[32], c
   }
 }
 
-// chain c of the list: species in `order`, then row tile, then member.  false: past the end
+// chain c of the list: species in `order`, then row tile, then member (SLABS: the members of member_of only).
+// false: past the end
+template <bool SLABS>
 __device__ __forceinline__ bool res_chain(const ResArgs& a, const int* first, int c, int& s, int& rt, int& m) {
+  const int cm = SLABS ? a.n_chain_members : a.members;
   for (int i = 0; i < a.num_species; ++i) {
     const int t = a.order[i];
-    const int n = (first[t + 1] - first[t]) * a.members;
+    const int n = (first[t + 1] - first[t]) * cm;
     if (c < n) {
       s = t;
-      rt = first[t] + c / a.members;
-      m = c % a.members;
+      rt = first[t] + c / cm;
+      m = SLABS ? a.member_of[c % cm] : c % cm;
       return true;
     }
     c -= n;
@@ -195,7 +203,7 @@ __device__ __forceinline__ void res_phase(const ResArgs& a, const ResSpecies& sp
 
 // ---- epilogue of one consumer warpgroup and phase P: 64 rows x bn columns from the accumulator registers ----
 // Same register -> (row, column) map as tile_epilogue (gemm_tc.cuh).
-template <int P>
+template <int P, bool SLABS>
 __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies& sp, int rt, int m, int n0, int bn,
                                              float (&acc)[4][32], uint32_t res, const int* blk, int nblk, int wg,
                                              int lane, int warp_in_wg, float& omax) {
@@ -306,13 +314,13 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
         }
       }
       if (PLAIN) {
-        float* dst_row = a.dx + (size_t)(rt * TM + row) * a.ldx;
+        float* dst_row = a.dx + (SLABS ? (size_t)m * (size_t)a.slab_stride : (size_t)0) + (size_t)(rt * TM + row) * a.ldx;
         // live column blocks map back to their place: group g of the tile is live block n0 / 32 + g
         const int col0 = nblk >= 0 ? blk[n0 / 32 + g] * 32 : n0 + g * 32;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           float* dst = dst_row + col0 + 8 * j + 2 * q;
-          if (a.members > 1)
+          if (!SLABS && a.members > 1)
             red_add_v2(dst, o[j][0], o[j][1]);
           else
             *reinterpret_cast<float2*>(dst) = make_float2(o[j][0], o[j][1]);
@@ -336,6 +344,10 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
 }
 
 // ---- the kernel: one persistent CTA per SM, chains res_chain_id(0), res_chain_id(1), ... ----
+// SLABS = false: every member's chains, phase 5 reduces the members into dx (ani_b200_mlp_step_resident).
+// SLABS = true: the chains of F.member_of only, phase 5 stores each member's rows into its own slab
+// (ani_b200_mlp_step_resident_members).
+template <bool SLABS>
 __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_constant__ ResArgs F) {
   extern __shared__ unsigned char smem_raw[];
   // 1024-byte aligned (swizzle groups are 8 rows x 64 B): R, then the ring
@@ -362,7 +374,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
     if (warp != PROD_WARP) return;
     // ================================ producer (TMA) ================================
     uint32_t u = 0;  // ring slots handed out so far: slot u % RES_SLOTS, use u / RES_SLOTS of that slot
-    for (int r = 0; res_chain(F, s_first, res_chain_id(r), s, rt, m); ++r) {
+    for (int r = 0; res_chain<SLABS>(F, s_first, res_chain_id(r), s, rt, m); ++r) {
       const ResSpecies& sp = F.sp[s];
       for (int p = 0; p < RES_PHASES; ++p) {
         int nkb, n;
@@ -435,7 +447,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
   const bool copier = warp_in_wg == 0 && lane == 0;  // issues and waits for the warpgroup's bulk copies of a1 / a2
   uint32_t u = 0;    // ring slots consumed so far, in the producer's order
   float omax = 0.f;  // largest |scaled value| this thread handed to the half-precision split
-  for (int r = 0; __shfl_sync(ANI_FULL_MASK, (int)res_chain(F, s_first, res_chain_id(r), s, rt, m), 0); ++r) {
+  for (int r = 0; __shfl_sync(ANI_FULL_MASK, (int)res_chain<SLABS>(F, s_first, res_chain_id(r), s, rt, m), 0); ++r) {
     const ResSpecies& sp = F.sp[s];
 #pragma unroll 1
     for (int p = 0; p < RES_PHASES; ++p) {
@@ -519,12 +531,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
         // every warp of the warpgroup is done reading R before any of them overwrites it
         if (p < 5) wg_bar(wg);
         switch (p) {
-          case 0: res_epilogue<0>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          case 1: res_epilogue<1>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          case 2: res_epilogue<2>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          case 3: res_epilogue<3>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          case 4: res_epilogue<4>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          default: res_epilogue<5>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 0: res_epilogue<0, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 1: res_epilogue<1, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 2: res_epilogue<2, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 3: res_epilogue<3, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 4: res_epilogue<4, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          default: res_epilogue<5, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
         }
         // this warpgroup's rows of the phase's output, visible to the next phase's wgmma
         if (p < 5) {

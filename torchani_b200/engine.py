@@ -386,10 +386,26 @@ class Workspace:
         # H2D and one D2H copy (each copy is a node of the captured graph with its own DMA set-up latency):
         #   in_block  f32: [cell 9 x n_conf (one per conformer, or the shared one first) | pad to 16 | coords 3 n]
         #   out_block u8 : [energies f64 x n_conf | status i32 | pad to 16 B | grad f32 x 3 n]
+        # followed, in the same allocation (out_full), by what the query-by-committee step adds (Engine.run(...,
+        # members=True)), so that it too needs one D2H copy while the ordinary step still copies out_block only:
+        #   [member energies f64 x M x n_conf | qbc f64 x n_conf | pad to 16 B | atom stats f32 x 3 n]
         self.in_coords_off = (9 * n_conf + 15) // 16 * 16
         self.in_block = torch.zeros(self.in_coords_off + 3 * n, **f32)
         self._out_grad_off = (8 * n_conf + 4 + 15) // 16 * 16
-        self.out_block = torch.zeros(self._out_grad_off + 12 * n, dtype=torch.uint8, device=device)
+        out_len = self._out_grad_off + 12 * n
+        self._out_qbc_off = (out_len + 15) // 16 * 16
+        self._out_stats_off = (self._out_qbc_off + 8 * (num_members + 1) * n_conf + 15) // 16 * 16
+        self.out_full = torch.zeros(self._out_stats_off + 12 * n, dtype=torch.uint8, device=device)
+        self.out_block = self.out_full[:out_len]
+        self.member_energies = self.out_full[self._out_qbc_off:self._out_qbc_off + 8 * num_members * n_conf].view(
+            torch.float64).view(num_members, n_conf)
+        self.qbc = self.out_full[self._out_qbc_off + 8 * num_members * n_conf:
+                                 self._out_qbc_off + 8 * (num_members + 1) * n_conf].view(torch.float64)
+        self.atom_stats = self.out_full[self._out_stats_off:].view(torch.float32).view(3, n)
+        # per-member dE/dAEV slabs f32[M][rows_cap][ldx] and dE_m/dcoords f32[M][n][3] of the query-by-committee step:
+        # allocated on its first use (Engine.members_buffers; at 10 k atoms the slabs of 8 members take ~340 MB)
+        self.dx_members: tp.Optional[Tensor] = None
+        self.grad_members: tp.Optional[Tensor] = None
         self.status = self.out_block[8 * n_conf: 8 * n_conf + 4].view(torch.int32)
         self.bin_start = torch.zeros(self.max_bins + 2, **i32)
         self.sorted_orig = torch.zeros(n, **i32)
@@ -494,6 +510,16 @@ class StepResult(tp.NamedTuple):
     grad: tp.Optional[Tensor]  # (C, A, 3) float32 dE/dcoords (forces = -grad) or None
     virial: tp.Optional[Tensor] = None  # (3, 3) float64 sum_pairs (dE/dDelta)_a Delta_b (stress = virial / volume);
     #                                     (C, 3, 3) for a periodic batch
+
+
+class MembersResult(tp.NamedTuple):
+    """What the query-by-committee step (``Engine.run(..., members=True)``) adds; member k is ``nets.active[k]``."""
+    energies: Tensor           # (M_active, C) float64: member energies incl. self energies
+    grad: Tensor               # (M_active, C, A, 3) float32: dE_m/dcoords
+    qbc: Tensor                # (C,) float64: std_m(E_m) / sqrt(real atoms), arch.py:439-485
+    force_magnitudes: Tensor   # (C, A) float32: mean_m |F_m|, arch.py:510-540
+    force_relative_stdev: Tensor   # (C, A) float32: (std_m |F_m| + 1e-8) / (mean + 1e-8), arch.py:543-576
+    force_relative_range: Tensor   # (C, A) float32: (max_m |F_m| - min_m |F_m| + 1e-8) / (mean + 1e-8)
 
 
 class Engine:
@@ -616,12 +642,20 @@ class Engine:
         return res
 
     def run(self, ws: Workspace, pbc: bool, want_grad: bool = True, shard: tp.Tuple[int, int] = (0, 1),
-            reuse: bool = False, want_virial: bool = False, conformer_cells: bool = False) -> StepResult:
+            reuse: bool = False, want_virial: bool = False, conformer_cells: bool = False,
+            members: bool = False) -> StepResult:
         """One step on inputs that are ALREADY in the workspace buffers (``ws.species_i32``,
         ``ws.coords``, ``ws.cell`` -- or, with ``conformer_cells``, one cell per conformer in ``ws.cells``) -- the
         entry point of host-driven loops that copy straight into them (calculator.HostCalculator).  The results alias
-        workspace buffers."""
+        workspace buffers.
+
+        ``members=True``: the query-by-committee step (``_launch_members``).  Besides the ordinary results (the
+        gradient is the mean of the members' gradients) it leaves every active member's energy and gradient and the
+        force / energy disagreement statistics in the workspace (``members_result``).  One GPU only."""
         n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
+        members = bool(members)
+        if members and (tuple(shard) != (0, 1) or not want_grad or want_virial):
+            raise ValueError("the query-by-committee step runs unsharded, with forces and without the virial")
         rank, world = shard
         lo = (n * rank) // world
         hi = (n * (rank + 1)) // world
@@ -637,12 +671,14 @@ class Engine:
         if periodic_batch and reuse:
             raise ValueError("reuse=True (Verlet skin) is not supported for periodic batches")
         key = (n_conf, n_per_conf, bool(pbc), bool(want_grad), lo, hi, self.nets.active_key, bool(reuse), self.skin,
-               bool(want_virial), self.mlp_mode, conformer_cells)
+               bool(want_virial), self.mlp_mode, conformer_cells, members)
         if reuse and not self.skin > 0:
             raise ValueError("reuse=True needs Engine.skin > 0 and a previous step that built the grid")
+        if members:
+            self.members_buffers(ws)
         with torch.cuda.device(self.device):   # the C-ABI launches on the CURRENT device's stream
             if not self.cuda_graph or self.profile:
-                self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells)
+                self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells, members)
             else:
                 graph = self._graphs.get(key)
                 if graph is not None:
@@ -653,12 +689,12 @@ class Engine:
                     if len(self._graph_seen) > 4 * self.max_graphs:
                         self._graph_seen.clear()
                     self._graph_seen[key] = self._graph_seen.get(key, 0) + 1
-                    self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells)
+                    self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells, members)
                 else:
                     self.note_composition(ws)
                     graph = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(graph):
-                        self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells)
+                        self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells, members)
                     while len(self._graphs) >= self.max_graphs:   # evict the least recently used capture
                         self._graphs.pop(next(iter(self._graphs)))
                     self._graphs[key] = graph
@@ -667,7 +703,12 @@ class Engine:
         # prepare 1 (+1 grid kernel for open single systems), AEV fwd 1, GEMM fwd 3,
         # (zero + GEMM bwd 3 + AEV bwd 1), reduce 1; the fused MLP: zero + one launch (resident chains) or + one per
         # window (data flow)
-        if self._use_resident_mlp(hi - lo, want_grad):
+        if members:
+            # the resident launch (+ its operand gather) or one data-flow launch per window (want_backward=2), then the
+            # members' AEV backward and the two statistics launches
+            mlp = (2 if self._use_resident_mlp(n, True) else
+                   self.lib.ani_b200_mlp_step_windows(C.byref(self.nets.model), ws.rows_cap)) + 2
+        elif self._use_resident_mlp(hi - lo, want_grad):
             mlp = 2
         elif self._use_dataflow_mlp(hi - lo):
             mlp = self.lib.ani_b200_mlp_step_windows(C.byref(self.nets.model), ws.rows_cap) + (1 if want_grad else 0)
@@ -684,9 +725,12 @@ class Engine:
                           ws.member_atomic.view(-1, n_conf, n_per_conf), grad, virial)
 
     def _launch(self, ws: Workspace, pbc: bool, want_grad: bool, lo: int, hi: int, reuse: bool = False,
-                want_virial: bool = False, conformer_cells: bool = False) -> None:
+                want_virial: bool = False, conformer_cells: bool = False, members: bool = False) -> None:
         """Enqueue the kernels of one step on the current stream (graph-capturable: no allocation,
         no synchronisation, only this library's launches and two memsets)."""
+        if members:
+            self._launch_members(ws, pbc, reuse, conformer_cells)
+            return
         L = self.lib
         n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
         st = torch.cuda.current_stream(self.device).cuda_stream
@@ -811,78 +855,123 @@ class Engine:
                 return 0
             self._timed("allreduce", reduce_all)
 
+    def members_buffers(self, ws: Workspace) -> None:
+        """Allocate the per-member slabs and gradients of the query-by-committee step (once per workspace, before any
+        capture of the step)."""
+        M = self.nets.num_members
+        if ws.dx_members is None:
+            ws.dx_members = torch.zeros(M, ws.rows_cap, self.nets.ldx, dtype=torch.float32, device=self.device)
+        if ws.grad_members is None:
+            ws.grad_members = torch.zeros(M, ws.n, 3, dtype=torch.float32, device=self.device)
+
+    def _launch_members(self, ws: Workspace, pbc: bool, reuse: bool, conformer_cells: bool) -> None:
+        """The query-by-committee step (graph-capturable like _launch): preparation (or the Verlet refresh) that zeroes
+        the members' gradients, AEV forward, ONE MLP launch whose layer-1 backward writes a dE_m/dAEV slab per active
+        member with unit weight (the resident chains of ani_b200_mlp_step_resident_members where the ordinary step
+        would run ani_b200_mlp_step_resident, else ani_b200_mlp_step with want_backward=2), ONE AEV backward over every
+        active member's slab
+        (ani_b200_aev_backward_members), the energy reduction (ensemble mean, per-member atomic energies) and the
+        statistics kernel, which also writes the ensemble-mean gradient into ``ws.grad``."""
+        L = self.lib
+        n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        c, nets = self.consts, self.nets
+        active = list(nets.active)
+        Ma = len(active)
+        idx = (C.c_int32 * Ma)(*active)
+        mode = _grid_mode(n_conf, pbc, conformer_cells)
+        prepare, aev_forward, backward = L.ani_b200_prepare_step, L.ani_b200_aev_forward, L.ani_b200_aev_backward_members
+        lat: tp.Tuple[tp.Any, ...] = ()
+        cell_ptr = ptr(ws.cell) if pbc else None
+        if mode == 3:   # one cell per conformer, see _launch
+            prepare, aev_forward = L.ani_b200_prepare_step_cells, L.ani_b200_aev_forward_cells
+            backward, lat, cell_ptr = L.ani_b200_aev_backward_members_cells, (ptr(ws.lattice),), ptr(ws.cells)
+        gm, zero_count = ptr(ws.grad_members), 3 * n * Ma
+        if reuse:
+            check(L.ani_b200_verlet_positions(
+                1, ptr(ws.coords), ptr(ws.grid), ptr(ws.sorted_orig), n, self.skin, ptr(ws.spos), ptr(ws.ref_pos),
+                ptr(ws.ref_shift), ptr(ws.moved), gm, zero_count, ptr(ws.aev_blocks), nets.ldx, st), "verlet_positions")
+        else:
+            check(prepare(
+                ptr(ws.coords), ptr(ws.species_i32), n_conf, n_per_conf, cell_ptr, int(bool(pbc)), mode,
+                c.rcr + self.skin, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start), ptr(ws.sorted_orig),
+                ptr(ws.orig_to_sorted), ptr(ws.spos), ptr(ws.sbin), ptr(ws.bucket_ranges), 0, n, c.num_species,
+                ws.rows_cap, ptr(ws.row_of), ptr(ws.row_atom), ptr(ws.tile_species), ptr(ws.layout_info),
+                len(c.shf_r), len(c.shf_a) * len(c.shf_z), c.out_dim, nets.ldx, nets.col_pad, ptr(ws.aev_blocks),
+                gm, zero_count, None, 0, ptr(ws.bucket_species), ptr(ws.scratch), ptr(ws.status), *lat, st),
+                "prepare_step")
+            if self.skin > 0:
+                check(L.ani_b200_verlet_positions(
+                    0, ptr(ws.coords), ptr(ws.grid), ptr(ws.sorted_orig), n, self.skin, ptr(ws.spos),
+                    ptr(ws.ref_pos), ptr(ws.ref_shift), ptr(ws.moved), None, 0, None, nets.ldx, st),
+                    "verlet_positions")
+        mask_ptr = ws.aev_blocks.data_ptr() + 4 * (ws.n_blocks + 1)
+        check(aev_forward(
+            C.byref(self.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sbin),
+            ptr(ws.bucket_ranges), ptr(ws.bucket_species) if not reuse else None, mask_ptr, n, 0, n,
+            ptr(ws.row_of), ptr(ws.x), nets.ldx, 1, ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap,
+            ptr(ws.status), *lat, st), "aev_forward")
+        unit = _lib.MLPModel.from_buffer_copy(nets.model)     # every active member with weight 1 (not 1 / M)
+        for m in range(_lib.ANI_MAX_MEMBERS):
+            unit.member_scale[m] = 1.0 if m in active else 0.0
+        self.mlp_resident = self._use_resident_mlp(n, True)
+        if self.mlp_resident:
+            check(L.ani_b200_mlp_step_resident_members(
+                C.byref(unit), ptr(ws.x), ptr(ws.dx_members), ws.rows_cap * nets.ldx, ws.rows_cap, ptr(ws.row_atom),
+                ptr(ws.layout_info), ptr(ws.aev_blocks), ptr(ws.act1), ptr(ws.act2), ptr(ws.e_member), ptr(ws.status),
+                st), "mlp_step_resident_members")
+        else:
+            check(L.ani_b200_mlp_step(
+                C.byref(unit), ptr(ws.x), ptr(ws.dx_members), ws.rows_cap, ptr(ws.row_atom), ptr(ws.layout_info),
+                ptr(ws.aev_blocks), ptr(ws.act1), ptr(ws.act2), ptr(ws.act3), ptr(ws.e_member), 2, ptr(ws.mlp_sync),
+                ptr(ws.status), st), "mlp_step")
+        check(backward(
+            C.byref(self.params), ptr(ws.grid), ptr(ws.spos), ptr(ws.sorted_orig), mask_ptr, n, 0, n,
+            ptr(ws.row_of), ptr(ws.dx_members), nets.ldx, ws.rows_cap * nets.ldx, idx, Ma, ptr(ws.nbr_cnt),
+            ptr(ws.nbr_list), ws.nbr_cap, gm, ptr(ws.status), ws.max_elements, *lat, st), "aev_backward_members")
+        check(L.ani_b200_reduce_energies(
+            C.byref(nets.model), ptr(ws.e_member), ws.rows_cap, ptr(ws.row_of), ptr(ws.orig_to_sorted),
+            ptr(ws.species_i32), n, 0, n, n_conf, n_per_conf, ptr(self.sae), ptr(ws.atomic), ptr(ws.member_atomic),
+            ws.energies_ptr, st), "reduce_energies")
+        check(L.ani_b200_ensemble_qbc(
+            gm, idx, Ma, ptr(ws.member_atomic), ptr(ws.species_i32), ptr(self.sae), n_conf, n_per_conf,
+            ptr(ws.grad), ptr(ws.atom_stats), ptr(ws.member_energies), ptr(ws.qbc), st), "ensemble_qbc")
+
+    def members_result(self, ws: Workspace) -> MembersResult:
+        """Views of the query-by-committee outputs of the last ``run(..., members=True)`` on ``ws``."""
+        Ma, C_, A = len(self.nets.active), ws.n_conf, ws.n_per_conf
+        assert ws.grad_members is not None, "no query-by-committee step has run on this workspace"
+        st = ws.atom_stats.view(3, C_, A)
+        return MembersResult(ws.member_energies[:Ma], ws.grad_members[:Ma].view(Ma, C_, A, 3), ws.qbc, st[0], st[1],
+                             st[2])
+
     def step_members(self, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor] = None, pbc: bool = False
                      ) -> tp.Tuple[Tensor, Tensor]:
         """Energies (M_active, C) float64 and dE_m/dcoords (M_active, C, A, 3) float32 of every ACTIVE ensemble member
-        in ONE pass (arch.py:403-436 differentiates every member by autograd; round 1 ran the engine once per member):
-        one preparation, one AEV forward, one MLP launch whose layer-1 backward writes a per-member dE_m/dAEV slab
-        (``ani_b200_mlp_step(want_backward=2)``), then the AEV backward once per member on its slab.  Eager (no
-        graph): an analysis call, not the MD loop."""
-        dev = self.device
+        (arch.py:403-436 differentiates every member by autograd): the query-by-committee step,
+        ``run(..., members=True)`` -- one MLP launch writes a dE_m/dAEV slab per member and ONE AEV backward contracts
+        all of them -- captured into a CUDA graph like the ordinary step."""
         n_conf, n_per_conf = species.shape
+        if coords.shape != (n_conf, n_per_conf, 3):
+            raise ValueError("coords must have shape (C, A, 3)")
+        if pbc and cell is None:
+            raise ValueError("If pbc is not None, cell should be present")
         per_conf = bool(pbc) and conformer_cells(cell, n_conf)
         if per_conf and n_conf == 1:
             cell, per_conf = cell[0], False
         ws = self.workspace(n_conf, n_per_conf)
         if pbc:
             ws.make_periodic()
-        n, L, c = ws.n, self.lib, self.consts
-        prepare, aev_forward, aev_backward = L.ani_b200_prepare_step, L.ani_b200_aev_forward, L.ani_b200_aev_backward
-        lat: tp.Tuple[tp.Any, ...] = ()
-        cell_ptr = ptr(ws.cell) if pbc else None
-        if per_conf:   # grid mode 3, see _launch
-            prepare, aev_forward = L.ani_b200_prepare_step_cells, L.ani_b200_aev_forward_cells
-            aev_backward, lat, cell_ptr = L.ani_b200_aev_backward_cells, (ptr(ws.lattice),), ptr(ws.cells)
-        nets = self.nets
-        M, ldx = nets.num_members, nets.ldx
-        active = list(nets.active)
-        if getattr(ws, "dx_members", None) is None:
-            ws.dx_members = torch.zeros(M, ws.rows_cap, ldx, dtype=torch.float32, device=dev)
-        model = _lib.MLPModel.from_buffer_copy(nets.model)     # every active member with weight 1 (not 1 / M)
-        for m in range(_lib.ANI_MAX_MEMBERS):
-            model.member_scale[m] = 1.0 if m in active else 0.0
-        grads = torch.zeros(len(active), n, 3, dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            st = torch.cuda.current_stream(dev).cuda_stream
+        with torch.cuda.device(self.device):
             ws.species_i32.copy_(species.reshape(-1))
             ws.coords.copy_(coords.reshape(-1, 3))
             if per_conf:
                 ws.cells.copy_(cell.reshape(n_conf, 9))
             elif pbc:
                 ws.cell.copy_(cell.reshape(-1))
-            check(prepare(
-                ptr(ws.coords), ptr(ws.species_i32), n_conf, n_per_conf, cell_ptr, int(bool(pbc)),
-                _grid_mode(n_conf, pbc, per_conf), c.rcr, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start),
-                ptr(ws.sorted_orig),
-                ptr(ws.orig_to_sorted), ptr(ws.spos), ptr(ws.sbin), ptr(ws.bucket_ranges), 0, n, c.num_species,
-                ws.rows_cap, ptr(ws.row_of), ptr(ws.row_atom), ptr(ws.tile_species), ptr(ws.layout_info),
-                len(c.shf_r), len(c.shf_a) * len(c.shf_z), c.out_dim, ldx, self.nets.col_pad, ptr(ws.aev_blocks), None, 0,
-                None, 0,
-                ptr(ws.bucket_species), ptr(ws.scratch), ptr(ws.status), *lat, st), "prepare_step")
-            mask_ptr = ws.aev_blocks.data_ptr() + 4 * (ws.n_blocks + 1)
-            check(aev_forward(
-                C.byref(self.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sbin),
-                ptr(ws.bucket_ranges), ptr(ws.bucket_species), mask_ptr, n, 0, n, ptr(ws.row_of), ptr(ws.x), ldx, 1,
-                ptr(ws.nbr_cnt),
-                ptr(ws.nbr_list), ws.nbr_cap, ptr(ws.status), *lat, st), "aev_forward")
-            check(L.ani_b200_mlp_step(
-                C.byref(model), ptr(ws.x), ptr(ws.dx_members), ws.rows_cap, ptr(ws.row_atom), ptr(ws.layout_info),
-                ptr(ws.aev_blocks), ptr(ws.act1), ptr(ws.act2), ptr(ws.act3), ptr(ws.e_member), 2, ptr(ws.mlp_sync),
-                ptr(ws.status), st), "mlp_step")
-            for k, m in enumerate(active):
-                check(aev_backward(
-                    C.byref(self.params), ptr(ws.grid), ptr(ws.spos), ptr(ws.sorted_orig), mask_ptr, n, 0, n,
-                    ptr(ws.row_of), ws.dx_members[m].data_ptr(), ldx, ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap,
-                    grads[k].data_ptr(), ptr(ws.status), 0, None, *lat, st), "aev_backward")
-            check(L.ani_b200_reduce_energies(
-                C.byref(model), ptr(ws.e_member), ws.rows_cap, ptr(ws.row_of), ptr(ws.orig_to_sorted),
-                ptr(ws.species_i32), n, 0, n, n_conf, n_per_conf, None, ptr(ws.atomic), ptr(ws.member_atomic),
-                ptr(ws.energies), st), "reduce_energies")
-        e_m = ws.member_atomic.view(M, n_conf, n_per_conf)[active].double().sum(-1)          # (M_active, C)
-        if self.sae is not None:
-            sp = species.clamp(min=0)
-            e_m = e_m + self.sae[sp].masked_fill(species < 0, 0.0).sum(-1).unsqueeze(0)
-        return e_m, grads.view(len(active), n_conf, n_per_conf, 3)
+        self.run(ws, bool(pbc), True, members=True, conformer_cells=per_conf)
+        r = self.members_result(ws)
+        return r.energies.clone(), r.grad.clone()
 
     def _use_dataflow_mlp(self, owned: int) -> bool:
         """One data-flow launch (True) or six chained launches (False) for `owned` atoms; see __init__."""

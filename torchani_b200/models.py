@@ -301,8 +301,8 @@ class ANI(torch.nn.Module):
                        pbc: tp.Optional[Tensor] = None, charge: int = 0) -> SpeciesForces:
         """Energies (M, C) and forces (M, C, A, 3) of every active ensemble member (arch.py:403-436).
         The reference differentiates each member's energy by autograd; here ONE pass of the engine
-        (``Engine.step_members``): the layer-1 backward GEMM writes one dE_m/dAEV slab per member instead of their
-        sum, and the force kernel runs once per slab."""
+        (``Engine.step_members``, the query-by-committee step): the MLP launch writes one dE_m/dAEV slab per member
+        instead of their sum, and ONE force-kernel launch contracts all of them, inside a captured CUDA graph."""
         species, coords = species_coordinates
         self._check_inputs(species, coords, charge)
         elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
