@@ -1087,67 +1087,58 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
 // ---------------------------------------------------------------------------------------
 // backward
 // ---------------------------------------------------------------------------------------
-// LAT (grid mode 3): image shifts in the lattice of the central atom's conformer (lattice table)
-template <int NA, int NZ, bool VIRIAL = false, bool LAT = false>
-__global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
-    k_aev_backward(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
-                   const float4* __restrict__ spos, const int32_t* __restrict__ sorted_orig, int lo, int hi,
-                   const int32_t* __restrict__ row_of, const float* __restrict__ gaev, int ldx,
-                   const int32_t* __restrict__ nbr_cnt, const int32_t* __restrict__ nbr_list, const ExplicitNbrs ex,
-                   const int32_t* __restrict__ species_mask, int cap, float* __restrict__ grad_coords,
-                   int32_t* __restrict__ status, size_t warp_bytes, int pair_cap, double* __restrict__ virial,
-                   const float* __restrict__ lattice) {
-  static_assert(NA * NZ == 32, "one lane per angular feature");
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const ani_grid g = *grid;
-  hi = min(hi, g.n_real);
-  const int i = lo + blockIdx.x * AEV_WARPS + warp;
-  if (i >= hi) return;
-  const WarpSmem s = carve(smem_raw + warp * warp_bytes, cap, true);
+// The per-atom pieces of the backward pass.  k_aev_backward (one dE/dAEV row) and k_aev_backward_members (one row per
+// ensemble member) are both sequences of these, so one member's arithmetic is that of the single-row kernel.
+//
+// The upstream gradient row lives in shared memory as the table {g_rad [RL], g_ang [pair_cap][GSTRIDE]}: g_ang is
+// COMPACT, row = pair index among the elements present in the system (c1 <= c2 ranks), `pair_cap` rows; pairs beyond
+// it (more elements than the launch was sized for) are read from the row in global memory.
+constexpr int GSTRIDE = 36;  // floats per species-pair row: 16-byte aligned, rows 4 banks apart
+
+template <class T>
+__device__ __forceinline__ T* grad_table_ang(T* table, int RL) { return table + ((RL + 3) & ~3); }
+
+__device__ __forceinline__ int compact_pair_row(int c1, int c2, int n_present) {
+  return c1 * (2 * n_present - c1 + 1) / 2 + (c2 - c1);
+}
+
+__device__ __forceinline__ void copy_async4(float* dst_smem, const float* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src)
+               : "memory");
+}
+
+// Issue the cp.async copies of the upstream row `grow` into `table`; the caller commits the group.  Element pairs that
+// do not occur in the system are never looked up (and never written by the MLP backward): walk the set bits of the
+// element mask, (s1, s2 >= s1) pairs of present elements only.
+__device__ __forceinline__ void stage_grad_row(const ani_aev_params& P, float* table, const float* grow,
+                                               unsigned present, int n_present, int pair_cap) {
+  const int lane = threadIdx.x & 31;
   const int S = P.num_species;
-  const int nR = P.n_shf_r;
-  const int RL = S * nR;
-  constexpr int GSTRIDE = 36;  // floats per species-pair row: 16-byte aligned, rows 4 banks apart
-  const unsigned present = (species_mask ? (unsigned)species_mask[0] : 0xffffffffu) & ((1u << S) - 1u);
-  const int n_present = __popc(present);
-  float* g_rad = s.rad;
-  float* g_ang = s.rad + ((RL + 3) & ~3);
-
-  // ---- 1. upstream gradient row -> shared memory ([pair][32 features]); element pairs that do
-  //         not occur in the system are never looked up (and never written by the MLP backward)
-  //         cp.async: the copies are all in flight while the neighbour geometry below is rebuilt
-  auto copy_async4 = [](float* dst_smem, const float* src) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src)
-                 : "memory");
-  };
-  const size_t row = (size_t)row_of[i] * ldx;
-  for (int t = lane; t < RL; t += 32) copy_async4(g_rad + t, gaev + row + t);
-  {
-    // walk the set bits of the element mask: (s1, s2 >= s1) pairs of present elements only.  The
-    // shared-memory table is COMPACT: row = pair index among the present elements (c1 <= c2 ranks),
-    // `pair_cap` rows; pairs beyond it (more elements than the launch was sized for) are read from
-    // global memory by pair_sums
-    int c1 = 0;
-    for (unsigned m1 = present; m1; m1 &= m1 - 1, ++c1) {
-      const int s1 = __ffs(m1) - 1;
-      const int base = s1 * (2 * S - s1 + 1) / 2 - s1;  // pair_index(s1, s2) = base + s2
-      int c2 = c1;
-      for (unsigned m2 = m1; m2; m2 &= m2 - 1, ++c2) {
-        const int pp = base + __ffs(m2) - 1;
-        const int cp = c1 * (2 * n_present - c1 + 1) / 2 + (c2 - c1);
-        if (cp < pair_cap) copy_async4(g_ang + cp * GSTRIDE + lane, gaev + row + RL + P.ang_pad + pp * 32 + lane);
-      }
+  const int RL = S * P.n_shf_r;
+  float* g_ang = grad_table_ang(table, RL);
+  for (int t = lane; t < RL; t += 32) copy_async4(table + t, grow + t);
+  int c1 = 0;
+  for (unsigned m1 = present; m1; m1 &= m1 - 1, ++c1) {
+    const int s1 = __ffs(m1) - 1;
+    const int base = s1 * (2 * S - s1 + 1) / 2 - s1;  // pair_index(s1, s2) = base + s2
+    int c2 = c1;
+    for (unsigned m2 = m1; m2; m2 &= m2 - 1, ++c2) {
+      const int pp = base + __ffs(m2) - 1;
+      const int cp = compact_pair_row(c1, c2, n_present);
+      if (cp < pair_cap) copy_async4(g_ang + cp * GSTRIDE + lane, grow + RL + P.ang_pad + pp * 32 + lane);
     }
-    asm volatile("cp.async.commit_group;" ::: "memory");
   }
+}
 
-  // ---- 2. geometry of the stored neighbours
-  const float4 pi = spos[i];
-  if (__float_as_int(pi.w) < 0) return;  // padding atom (explicit neighbour rows only)
-  const int e0 = ex.start ? ex.start[i] : 0;
-  const int cnt = ex.start ? min(ex.start[i + 1] - e0, cap) : nbr_cnt[i];
-  const int conf_i = LAT ? sorted_orig[i] / g.n_per_conf : 0;   // neighbours lie in the centre's conformer
+// Geometry of atom i's neighbours, from the stored neighbour words or from the explicit rows `ex`: nd, nj, nsp, nfc,
+// and the radial cutoff's derivative (once per neighbour, not once per (neighbour, shift) lane) into dfc[n * dfc_stride].
+template <bool LAT>
+__device__ __forceinline__ void backward_geometry(const ani_aev_params& P, const ani_grid& g, const WarpSmem& s,
+                                                  const float4* __restrict__ spos, float4 pi, int i, int cnt,
+                                                  const ExplicitNbrs& ex, int e0, const int32_t* __restrict__ nbr_list,
+                                                  int cap, const float* __restrict__ lattice, int conf_i,
+                                                  float* dfc_out, int dfc_stride) {
+  const int lane = threadIdx.x & 31;
   for (int n = lane; n < cnt; n += 32) {
     int j;
     float4 dR;
@@ -1167,21 +1158,23 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
     s.nd[n] = dR;
     s.nj[n] = j;
     s.nsp[n] = (unsigned char)__float_as_int(spos[j].w);
-    // radial cutoff and its derivative once per neighbour (not once per (neighbour, shift) lane)
     float fc, dfc;
     cutoff_value_grad(dR.w, P.rcr, P.cutoff_kind, fc, dfc);
     s.nfc[n] = fc;
-    s.fgrad[3 * n] = dfc;  // parked here until the radial loop overwrites fgrad[3n..3n+2]
+    dfc_out[n * dfc_stride] = dfc;
   }
-  asm volatile("cp.async.wait_all;" ::: "memory");  // the upstream gradient row has landed
-  __syncwarp();
+}
 
-  // ---- 3. radial: dE/dR_n = sum_m g[s_n, m] * (G' fc + G fc'), then along the unit vector.
-  //         Lane = neighbour, serial over the shifts: no cross-lane reduction at all.
+// Radial: dE/dR_n = sum_m g[s_n, m] * (G' fc + G fc'), then along the unit vector, into fgrad[3n .. 3n+2].  Lane =
+// neighbour, serial over the shifts: no cross-lane reduction at all.
+__device__ __forceinline__ void radial_backward(const ani_aev_params& P, const WarpSmem& s, int cnt,
+                                                const float* table, const float* dfc_in, int dfc_stride) {
+  const int lane = threadIdx.x & 31;
+  const int nR = P.n_shf_r;
   for (int n = lane; n < cnt; n += 32) {
     const float4 d = s.nd[n];
-    const float fc = s.nfc[n], dfc = s.fgrad[3 * n];
-    const float* __restrict__ gr = g_rad + s.nsp[n] * nR;
+    const float fc = s.nfc[n], dfc = dfc_in[n * dfc_stride];
+    const float* __restrict__ gr = table + s.nsp[n] * nR;
     float acc = 0.f;
 #pragma unroll 4
     for (int m = 0; m < nR; ++m) {
@@ -1194,12 +1187,24 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
     s.fgrad[3 * n + 1] = sc * d.y;
     s.fgrad[3 * n + 2] = sc * d.z;
   }
-  __syncwarp();
+}
 
-  // ---- 4. angular.  Lanes own rows j of the species-sorted angular list.
-  const int n_ang = compact_angular_list(P, s, cnt, lane, status);
-  if (n_ang >= 2) {
-    float shfA[NA], cz[NZ], sz[NZ];
+// Angular: adds dE/dr_j of the n_ang neighbours of the angular list to fgrad.  Lanes own rows j of the list.
+// CONSTS_IN_REGS: the angular constants (shf_a, cos_z, sin_z) are copied into registers; otherwise they are read from
+// the kernel parameters as constant-bank operands, which keeps the member loop of k_aev_backward_members within its
+// register budget.  SHAPE_IN_REGS: likewise for the element count and the radial width that
+// address pairs beyond the table.  Both are register-allocation choices of the calling kernel; they change no result.
+template <int NA, int NZ, bool CONSTS_IN_REGS, bool SHAPE_IN_REGS>
+__device__ __forceinline__ void angular_backward(const ani_aev_params& P, const WarpSmem& s, int n_ang,
+                                                 const float* table, const float* grow, unsigned present, int n_present,
+                                                 int pair_cap) {
+  const int lane = threadIdx.x & 31;
+  if (n_ang < 2) return;
+  const int S_reg = P.num_species;
+  const int RL_reg = S_reg * P.n_shf_r;
+  const float* g_ang = grad_table_ang(table, RL_reg);
+  float shfA[NA], cz[NZ], sz[NZ];
+  if (CONSTS_IN_REGS) {
 #pragma unroll
     for (int a = 0; a < NA; ++a) shfA[a] = P.shf_a[a];
 #pragma unroll
@@ -1207,177 +1212,181 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
       cz[z] = P.cos_z[z];
       sz[z] = P.sin_z[z];
     }
-    // The three sums every pair needs (symmetric in j <-> k):
-    //   S0 = sum g f1 f2,  S1 = sum g f1' f2 (d/dcos),  S2 = sum g f1 f2' (d/dRbar)
-    auto pair_sums = [&](const float4& dj, const float4& dk, int sj, int sk, float& cosT, float& inv_rr, float& S0,
-                         float& S1, float& S2) {
-      const float dot = dj.x * dk.x + dj.y * dk.y + dj.z * dk.z;
-      inv_rr = fast_rcp(fmaxf(dj.w * dk.w, 1e-10f));
-      cosT = dot * inv_rr;
-      const float c = 0.95f * cosT;
-      const float sn = fast_sqrt(fmaxf(1.0f - c * c, 0.f));
-      const float c_over_s = c * fast_rcp(sn);
-      const float rbar = 0.5f * (dj.w + dk.w);
-      // t_z = sum_a g[a,z] f2[a],  u_z = sum_a g[a,z] f2'[a]: the 32 upstream values of this pair are
-      // one 16-byte-aligned row -> 8 vector loads
-      // compact table row of the element pair (ranks among the present elements) or, beyond the
-      // table, the upstream row in global memory
-      const int cj = __popc(present & ((1u << sj) - 1u)), ck = __popc(present & ((1u << sk) - 1u));
-      const int clo = min(cj, ck), chi = max(cj, ck);
-      const int cp = clo * (2 * n_present - clo + 1) / 2 + (chi - clo);
-      const float4* __restrict__ gp =
-          cp < pair_cap ? reinterpret_cast<const float4*>(g_ang + cp * GSTRIDE)
-                        : reinterpret_cast<const float4*>(gaev + row + RL + P.ang_pad + pair_index(sj, sk, S) * 32);
-      float tz[NZ], uz[NZ];
+  }
+  // The three sums every pair needs (symmetric in j <-> k):
+  //   S0 = sum g f1 f2,  S1 = sum g f1' f2 (d/dcos),  S2 = sum g f1 f2' (d/dRbar)
+  auto pair_sums = [&](const float4& dj, const float4& dk, int sj, int sk, float& cosT, float& inv_rr, float& S0,
+                       float& S1, float& S2) {
+    const float dot = dj.x * dk.x + dj.y * dk.y + dj.z * dk.z;
+    inv_rr = fast_rcp(fmaxf(dj.w * dk.w, 1e-10f));
+    cosT = dot * inv_rr;
+    const float c = 0.95f * cosT;
+    const float sn = fast_sqrt(fmaxf(1.0f - c * c, 0.f));
+    const float c_over_s = c * fast_rcp(sn);
+    const float rbar = 0.5f * (dj.w + dk.w);
+    // t_z = sum_a g[a,z] f2[a],  u_z = sum_a g[a,z] f2'[a]: the 32 upstream values of this pair are
+    // one 16-byte-aligned row -> 8 vector loads, from the compact table or, beyond it, from the row in global memory
+    const int cj = __popc(present & ((1u << sj) - 1u)), ck = __popc(present & ((1u << sk) - 1u));
+    const int cp = compact_pair_row(min(cj, ck), max(cj, ck), n_present);
+    const float4* __restrict__ gp =
+        cp < pair_cap ? reinterpret_cast<const float4*>(g_ang + cp * GSTRIDE)
+                      : reinterpret_cast<const float4*>(grow + (SHAPE_IN_REGS ? RL_reg : P.num_species * P.n_shf_r) + P.ang_pad +
+                                                         pair_index(sj, sk, SHAPE_IN_REGS ? S_reg : P.num_species) * 32);
+    float tz[NZ], uz[NZ];
 #pragma unroll
-      for (int z = 0; z < NZ; ++z) tz[z] = uz[z] = 0.f;
+    for (int z = 0; z < NZ; ++z) tz[z] = uz[z] = 0.f;
 #pragma unroll
-      for (int a = 0; a < NA; ++a) {
-        const float d = rbar - shfA[a];
-        const float f2 = fast_exp(-P.eta_a * d * d);
-        const float f2p = -2.0f * P.eta_a * d * f2;
+    for (int a = 0; a < NA; ++a) {
+      const float d = rbar - (CONSTS_IN_REGS ? shfA[a] : P.shf_a[a]);
+      const float f2 = fast_exp(-P.eta_a * d * d);
+      const float f2p = -2.0f * P.eta_a * d * f2;
 #pragma unroll
-        for (int q = 0; q < NZ / 4; ++q) {
-          const float4 gv = gp[a * (NZ / 4) + q];
-          tz[4 * q + 0] = fmaf(gv.x, f2, tz[4 * q + 0]);
-          tz[4 * q + 1] = fmaf(gv.y, f2, tz[4 * q + 1]);
-          tz[4 * q + 2] = fmaf(gv.z, f2, tz[4 * q + 2]);
-          tz[4 * q + 3] = fmaf(gv.w, f2, tz[4 * q + 3]);
-          uz[4 * q + 0] = fmaf(gv.x, f2p, uz[4 * q + 0]);
-          uz[4 * q + 1] = fmaf(gv.y, f2p, uz[4 * q + 1]);
-          uz[4 * q + 2] = fmaf(gv.z, f2p, uz[4 * q + 2]);
-          uz[4 * q + 3] = fmaf(gv.w, f2p, uz[4 * q + 3]);
-        }
+      for (int q = 0; q < NZ / 4; ++q) {
+        const float4 gv = gp[a * (NZ / 4) + q];
+        tz[4 * q + 0] = fmaf(gv.x, f2, tz[4 * q + 0]);
+        tz[4 * q + 1] = fmaf(gv.y, f2, tz[4 * q + 1]);
+        tz[4 * q + 2] = fmaf(gv.z, f2, tz[4 * q + 2]);
+        tz[4 * q + 3] = fmaf(gv.w, f2, tz[4 * q + 3]);
+        uz[4 * q + 0] = fmaf(gv.x, f2p, uz[4 * q + 0]);
+        uz[4 * q + 1] = fmaf(gv.y, f2p, uz[4 * q + 1]);
+        uz[4 * q + 2] = fmaf(gv.z, f2p, uz[4 * q + 2]);
+        uz[4 * q + 3] = fmaf(gv.w, f2p, uz[4 * q + 3]);
       }
-      S0 = S1 = S2 = 0.f;
+    }
+    S0 = S1 = S2 = 0.f;
 #pragma unroll
-      for (int z = 0; z < NZ; ++z) {
-        const float base = fmaxf(0.5f * (1.0f + c * cz[z] + sn * sz[z]), 0.f);
-        const float lg = fast_log2(base);
-        const float f1 = fast_exp2(P.zeta * lg);
-        const float pw1 = fast_exp2((P.zeta - 1.0f) * lg);
-        const float f1p = P.zeta * pw1 * (0.475f * (cz[z] - c_over_s * sz[z]));
-        S0 = fmaf(f1, tz[z], S0);
-        S1 = fmaf(f1p, tz[z], S1);
-        S2 = fmaf(f1, uz[z], S2);
+    for (int z = 0; z < NZ; ++z) {
+      const float cosz = CONSTS_IN_REGS ? cz[z] : P.cos_z[z], sinz = CONSTS_IN_REGS ? sz[z] : P.sin_z[z];
+      const float base = fmaxf(0.5f * (1.0f + c * cosz + sn * sinz), 0.f);
+      const float lg = fast_log2(base);
+      const float f1 = fast_exp2(P.zeta * lg);
+      const float pw1 = fast_exp2((P.zeta - 1.0f) * lg);
+      const float f1p = P.zeta * pw1 * (0.475f * (cosz - c_over_s * sinz));
+      S0 = fmaf(f1, tz[z], S0);
+      S1 = fmaf(f1p, tz[z], S1);
+      S2 = fmaf(f1, uz[z], S2);
+    }
+  };
+  int lpr = 1;
+  while (lpr * 2 * n_ang <= 32) lpr *= 2;
+  const int sub = lane % lpr;
+  if (n_ang <= 32) {
+    // Rotation over UNORDERED pairs: in step t row j evaluates the pair (j, (j + t) mod n) once,
+    // keeps its own share and hands the partner's share to the lane that owns row k with one
+    // shuffle (every row receives from row j - t at the same step).  t runs to n/2; for even n
+    // the last step would see every pair from both ends, so only rows j < n/2 take part in it.
+    // The lpr lanes of a row split the steps.  Half the transcendental work of ordered pairs.
+    const int j = lane / lpr;
+    const bool jvalid = j < n_ang;
+    const int half_n = n_ang >> 1;
+    const bool even = (n_ang & 1) == 0;
+    float gx = 0.f, gy = 0.f, gz = 0.f;
+    int nj_ = 0, sj = 0;
+    float4 dj = make_float4(0.f, 0.f, 0.f, 1.f);
+    float fcj = 0.f, dfcj = 0.f, inv_rj = 0.f;
+    if (jvalid) {
+      nj_ = s.aidx[j];
+      dj = s.nd[nj_];
+      fcj = s.afc[j];
+      dfcj = s.afcd[j];
+      sj = s.nsp[nj_];
+      inv_rj = dj.w > 1e-10f ? fast_rcp(dj.w) : 0.f;
+    }
+    const int steps = (half_n + lpr - 1) / lpr;
+    for (int it = 0; it < steps; ++it) {
+      const int t = 1 + it * lpr + sub;
+      const bool active = jvalid && t <= half_n && !(even && t == half_n && j >= half_n);
+      float px = 0.f, py = 0.f, pz = 0.f;
+      if (active) {
+        int k = j + t;
+        if (k >= n_ang) k -= n_ang;
+        const int nk_ = s.aidx[k];
+        const float4 dk = s.nd[nk_];
+        const float fck = s.afc[k], dfck = s.afcd[k];
+        const float inv_rk = dk.w > 1e-10f ? fast_rcp(dk.w) : 0.f;
+        float cosT, inv_rr, S0, S1, S2;
+        pair_sums(dj, dk, sj, (int)s.nsp[nk_], cosT, inv_rr, S0, S1, S2);
+        // feature = 2 f1 f2 fcj fck (once per unordered pair): its derivative with respect to
+        // r_j is this lane's share, the one with respect to r_k goes to the partner row
+        const float W = fcj * fck;
+        const float dEdcos = 2.0f * W * S1;
+        const float dEdRj = S2 * W + 2.0f * S0 * dfcj * fck;
+        const float dEdRk = S2 * W + 2.0f * S0 * fcj * dfck;
+        const float coefj = (dEdRj - dEdcos * cosT * inv_rj) * inv_rj;
+        const float coefk = (dEdRk - dEdcos * cosT * inv_rk) * inv_rk;
+        const float coefx = dEdcos * inv_rr;
+        gx += coefj * dj.x + coefx * dk.x;
+        gy += coefj * dj.y + coefx * dk.y;
+        gz += coefj * dj.z + coefx * dk.z;
+        px = coefk * dk.x + coefx * dj.x;
+        py = coefk * dk.y + coefx * dj.y;
+        pz = coefk * dk.z + coefx * dj.z;
       }
-    };
-    int lpr = 1;
-    while (lpr * 2 * n_ang <= 32) lpr *= 2;
-    const int sub = lane % lpr;
-    if (n_ang <= 32) {
-      // Rotation over UNORDERED pairs: in step t row j evaluates the pair (j, (j + t) mod n) once,
-      // keeps its own share and hands the partner's share to the lane that owns row k with one
-      // shuffle (every row receives from row j - t at the same step).  t runs to n/2; for even n
-      // the last step would see every pair from both ends, so only rows j < n/2 take part in it.
-      // The lpr lanes of a row split the steps.  Half the transcendental work of ordered pairs.
-      const int j = lane / lpr;
-      const bool jvalid = j < n_ang;
-      const int half_n = n_ang >> 1;
-      const bool even = (n_ang & 1) == 0;
+      int src_row = j - t;
+      if (src_row < 0) src_row += n_ang;
+      const int src_lane = jvalid ? src_row * lpr + sub : lane;
+      const float rx = __shfl_sync(ANI_FULL_MASK, px, src_lane);
+      const float ry = __shfl_sync(ANI_FULL_MASK, py, src_lane);
+      const float rz = __shfl_sync(ANI_FULL_MASK, pz, src_lane);
+      if (jvalid) {  // inactive sources sent zeros
+        gx += rx;
+        gy += ry;
+        gz += rz;
+      }
+    }
+    for (int o = lpr / 2; o > 0; o >>= 1) {
+      gx += __shfl_xor_sync(ANI_FULL_MASK, gx, o);
+      gy += __shfl_xor_sync(ANI_FULL_MASK, gy, o);
+      gz += __shfl_xor_sync(ANI_FULL_MASK, gz, o);
+    }
+    if (jvalid && sub == 0) {
+      s.fgrad[3 * nj_ + 0] += gx;
+      s.fgrad[3 * nj_ + 1] += gy;
+      s.fgrad[3 * nj_ + 2] += gz;
+    }
+  } else {
+    // more rows than lanes: ordered pairs (j, k), several passes of 32 rows
+    for (int row0 = 0; row0 < n_ang; row0 += 32) {
+      const int j = row0 + lane;
       float gx = 0.f, gy = 0.f, gz = 0.f;
-      int nj_ = 0, sj = 0;
-      float4 dj = make_float4(0.f, 0.f, 0.f, 1.f);
-      float fcj = 0.f, dfcj = 0.f, inv_rj = 0.f;
-      if (jvalid) {
-        nj_ = s.aidx[j];
-        dj = s.nd[nj_];
-        fcj = s.afc[j];
-        dfcj = s.afcd[j];
-        sj = s.nsp[nj_];
-        inv_rj = dj.w > 1e-10f ? fast_rcp(dj.w) : 0.f;
-      }
-      const int steps = (half_n + lpr - 1) / lpr;
-      for (int it = 0; it < steps; ++it) {
-        const int t = 1 + it * lpr + sub;
-        const bool active = jvalid && t <= half_n && !(even && t == half_n && j >= half_n);
-        float px = 0.f, py = 0.f, pz = 0.f;
-        if (active) {
-          int k = j + t;
-          if (k >= n_ang) k -= n_ang;
+      if (j < n_ang) {
+        const int nj_ = s.aidx[j];
+        const float4 dj = s.nd[nj_];
+        const float fcj = s.afc[j], dfcj = s.afcd[j];
+        const int sj = s.nsp[nj_];
+        const float inv_rj = dj.w > 1e-10f ? fast_rcp(dj.w) : 0.f;
+        for (int k = 0; k < n_ang; ++k) {
+          if (k == j) continue;
           const int nk_ = s.aidx[k];
           const float4 dk = s.nd[nk_];
-          const float fck = s.afc[k], dfck = s.afcd[k];
-          const float inv_rk = dk.w > 1e-10f ? fast_rcp(dk.w) : 0.f;
+          const float fck = s.afc[k];
           float cosT, inv_rr, S0, S1, S2;
           pair_sums(dj, dk, sj, (int)s.nsp[nk_], cosT, inv_rr, S0, S1, S2);
-          // feature = 2 f1 f2 fcj fck (once per unordered pair): its derivative with respect to
-          // r_j is this lane's share, the one with respect to r_k goes to the partner row
           const float W = fcj * fck;
+          const float dEdRj = S2 * W + 2.0f * S0 * dfcj * fck;  // 2*(0.5*S2*W + S0*fcj'*fck)
           const float dEdcos = 2.0f * W * S1;
-          const float dEdRj = S2 * W + 2.0f * S0 * dfcj * fck;
-          const float dEdRk = S2 * W + 2.0f * S0 * fcj * dfck;
           const float coefj = (dEdRj - dEdcos * cosT * inv_rj) * inv_rj;
-          const float coefk = (dEdRk - dEdcos * cosT * inv_rk) * inv_rk;
-          const float coefx = dEdcos * inv_rr;
-          gx += coefj * dj.x + coefx * dk.x;
-          gy += coefj * dj.y + coefx * dk.y;
-          gz += coefj * dj.z + coefx * dk.z;
-          px = coefk * dk.x + coefx * dj.x;
-          py = coefk * dk.y + coefx * dj.y;
-          pz = coefk * dk.z + coefx * dj.z;
+          const float coefk = dEdcos * inv_rr;
+          gx += coefj * dj.x + coefk * dk.x;
+          gy += coefj * dj.y + coefk * dk.y;
+          gz += coefj * dj.z + coefk * dk.z;
         }
-        int src_row = j - t;
-        if (src_row < 0) src_row += n_ang;
-        const int src_lane = jvalid ? src_row * lpr + sub : lane;
-        const float rx = __shfl_sync(ANI_FULL_MASK, px, src_lane);
-        const float ry = __shfl_sync(ANI_FULL_MASK, py, src_lane);
-        const float rz = __shfl_sync(ANI_FULL_MASK, pz, src_lane);
-        if (jvalid) {  // inactive sources sent zeros
-          gx += rx;
-          gy += ry;
-          gz += rz;
-        }
-      }
-      for (int o = lpr / 2; o > 0; o >>= 1) {
-        gx += __shfl_xor_sync(ANI_FULL_MASK, gx, o);
-        gy += __shfl_xor_sync(ANI_FULL_MASK, gy, o);
-        gz += __shfl_xor_sync(ANI_FULL_MASK, gz, o);
-      }
-      if (jvalid && sub == 0) {
         s.fgrad[3 * nj_ + 0] += gx;
         s.fgrad[3 * nj_ + 1] += gy;
         s.fgrad[3 * nj_ + 2] += gz;
       }
-    } else {
-      // more rows than lanes: ordered pairs (j, k), several passes of 32 rows
-      for (int row0 = 0; row0 < n_ang; row0 += 32) {
-        const int j = row0 + lane;
-        float gx = 0.f, gy = 0.f, gz = 0.f;
-        if (j < n_ang) {
-          const int nj_ = s.aidx[j];
-          const float4 dj = s.nd[nj_];
-          const float fcj = s.afc[j], dfcj = s.afcd[j];
-          const int sj = s.nsp[nj_];
-          const float inv_rj = dj.w > 1e-10f ? fast_rcp(dj.w) : 0.f;
-          for (int k = 0; k < n_ang; ++k) {
-            if (k == j) continue;
-            const int nk_ = s.aidx[k];
-            const float4 dk = s.nd[nk_];
-            const float fck = s.afc[k];
-            float cosT, inv_rr, S0, S1, S2;
-            pair_sums(dj, dk, sj, (int)s.nsp[nk_], cosT, inv_rr, S0, S1, S2);
-            const float W = fcj * fck;
-            const float dEdRj = S2 * W + 2.0f * S0 * dfcj * fck;  // 2*(0.5*S2*W + S0*fcj'*fck)
-            const float dEdcos = 2.0f * W * S1;
-            const float coefj = (dEdRj - dEdcos * cosT * inv_rj) * inv_rj;
-            const float coefk = dEdcos * inv_rr;
-            gx += coefj * dj.x + coefk * dk.x;
-            gy += coefj * dj.y + coefk * dk.y;
-            gz += coefj * dj.z + coefk * dk.z;
-          }
-          s.fgrad[3 * nj_ + 0] += gx;
-          s.fgrad[3 * nj_ + 1] += gy;
-          s.fgrad[3 * nj_ + 2] += gz;
-        }
-      }
     }
   }
-  __syncwarp();
+}
 
-  // ---- 5. scatter: neighbour j gets +dE_i/dr_j, the centre gets minus the sum
-  //         VIRIAL: W_ab += (dE_i/dDelta_in)_a (Delta_in)_b, the "f dot r" virial of ase.py:164-168
-  //         (dE/dDelta^T @ Delta over the pairs); ANI_VIRIAL_SLOTS partial sums keep the atomics apart
+// Scatter into `grad`: neighbour j gets +dE_i/dr_j, the centre atom i minus the sum.
+// VIRIAL: W_ab += (dE_i/dDelta_in)_a (Delta_in)_b, the "f dot r" virial of ase.py:164-168 (dE/dDelta^T @ Delta over
+// the pairs); ANI_VIRIAL_SLOTS partial sums keep the atomics apart.
+template <bool VIRIAL, bool LAT>
+__device__ __forceinline__ void scatter_backward(const ani_grid& g, const WarpSmem& s, int cnt,
+                                                 const int32_t* __restrict__ sorted_orig, int i, int conf_i,
+                                                 float* __restrict__ grad, double* __restrict__ virial) {
+  const int lane = threadIdx.x & 31;
   float sx = 0.f, sy = 0.f, sz_ = 0.f;
   float vir[9];
 #pragma unroll
@@ -1385,9 +1394,9 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
   for (int n = lane; n < cnt; n += 32) {
     const float fx = s.fgrad[3 * n], fy = s.fgrad[3 * n + 1], fz = s.fgrad[3 * n + 2];
     const int oj = sorted_orig[s.nj[n]];
-    atomicAdd(&grad_coords[3 * (size_t)oj + 0], fx);
-    atomicAdd(&grad_coords[3 * (size_t)oj + 1], fy);
-    atomicAdd(&grad_coords[3 * (size_t)oj + 2], fz);
+    atomicAdd(&grad[3 * (size_t)oj + 0], fx);
+    atomicAdd(&grad[3 * (size_t)oj + 1], fy);
+    atomicAdd(&grad[3 * (size_t)oj + 2], fz);
     sx += fx;
     sy += fy;
     sz_ += fz;
@@ -1413,10 +1422,53 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
   sz_ = warp_sum(sz_);
   if (lane == 0) {
     const int oi = sorted_orig[i];
-    atomicAdd(&grad_coords[3 * (size_t)oi + 0], -sx);
-    atomicAdd(&grad_coords[3 * (size_t)oi + 1], -sy);
-    atomicAdd(&grad_coords[3 * (size_t)oi + 2], -sz_);
+    atomicAdd(&grad[3 * (size_t)oi + 0], -sx);
+    atomicAdd(&grad[3 * (size_t)oi + 1], -sy);
+    atomicAdd(&grad[3 * (size_t)oi + 2], -sz_);
   }
+}
+
+// Backward (forces) of one dE/dAEV row per atom: the row's cp.async copies are in flight while the neighbour geometry
+// is rebuilt; radial; angular list; angular; scatter.  LAT (grid mode 3): image shifts in the lattice of the central
+// atom's conformer (lattice table)
+template <int NA, int NZ, bool VIRIAL = false, bool LAT = false>
+__global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
+    k_aev_backward(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
+                   const float4* __restrict__ spos, const int32_t* __restrict__ sorted_orig, int lo, int hi,
+                   const int32_t* __restrict__ row_of, const float* __restrict__ gaev, int ldx,
+                   const int32_t* __restrict__ nbr_cnt, const int32_t* __restrict__ nbr_list, const ExplicitNbrs ex,
+                   const int32_t* __restrict__ species_mask, int cap, float* __restrict__ grad_coords,
+                   int32_t* __restrict__ status, size_t warp_bytes, int pair_cap, double* __restrict__ virial,
+                   const float* __restrict__ lattice) {
+  static_assert(NA * NZ == 32, "one lane per angular feature");
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const ani_grid g = *grid;
+  hi = min(hi, g.n_real);
+  const int i = lo + blockIdx.x * AEV_WARPS + warp;
+  if (i >= hi) return;
+  const WarpSmem s = carve(smem_raw + warp * warp_bytes, cap, true);
+  const unsigned present = (species_mask ? (unsigned)species_mask[0] : 0xffffffffu) & ((1u << P.num_species) - 1u);
+  const int n_present = __popc(present);
+  const float* grow = gaev + (size_t)row_of[i] * ldx;
+  stage_grad_row(P, s.rad, grow, present, n_present, pair_cap);
+  asm volatile("cp.async.commit_group;" ::: "memory");
+
+  const float4 pi = spos[i];
+  if (__float_as_int(pi.w) < 0) return;  // padding atom (explicit neighbour rows only)
+  const int e0 = ex.start ? ex.start[i] : 0;
+  const int cnt = ex.start ? min(ex.start[i + 1] - e0, cap) : nbr_cnt[i];
+  const int conf_i = LAT ? sorted_orig[i] / g.n_per_conf : 0;   // neighbours lie in the centre's conformer
+  // dfc is parked in fgrad[3n] until the radial pass overwrites fgrad[3n .. 3n+2]
+  backward_geometry<LAT>(P, g, s, spos, pi, i, cnt, ex, e0, nbr_list, cap, lattice, conf_i, s.fgrad, 3);
+  asm volatile("cp.async.wait_all;" ::: "memory");  // the upstream gradient row has landed
+  __syncwarp();
+  radial_backward(P, s, cnt, s.rad, s.fgrad, 3);
+  __syncwarp();
+  const int n_ang = compact_angular_list(P, s, cnt, lane, status);
+  angular_backward<NA, NZ, true, VIRIAL>(P, s, n_ang, s.rad, grow, present, n_present, pair_cap);
+  __syncwarp();
+  scatter_backward<VIRIAL, LAT>(g, s, cnt, sorted_orig, i, conf_i, grad_coords, virial);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1429,12 +1481,13 @@ struct MemberSlabs {
   long long stride;  // floats between the dE/dAEV slabs of consecutive members
 };
 
-// k_aev_backward with the per-member work in a loop.  A warp rebuilds its atom's neighbour geometry (distances,
-// cutoffs, image shifts, the angular list) once; then, for k = 0 .. count - 1, it contracts member idx[k]'s dE/dAEV row
-// and scatters into grad_members[k].  The rows are staged in two shared-memory buffers with cp.async: member k + 1's
-// row is in flight while member k is contracted, so shared memory per warp does not depend on the number of members.
-// The arithmetic of one member is that of k_aev_backward (same order within an atom): only the order of the float
-// atomics differs.  No explicit neighbour rows and no virial.
+// The pieces of k_aev_backward with the per-member ones in a loop.  A warp rebuilds its atom's neighbour geometry
+// (backward_geometry, compact_angular_list) once; then, for k = 0 .. count - 1, it contracts member idx[k]'s dE/dAEV
+// row (radial_backward, angular_backward) and scatters into grad_members[k] (scatter_backward).  The rows are staged in two
+// shared-memory tables with stage_grad_row: member k + 1's row is in flight while member k is contracted, so shared
+// memory per warp does not depend on the number of members; dfc has its own array after them (fgrad is rewritten per
+// member).  The arithmetic of one member is that of k_aev_backward (same order within an atom): only the order of the
+// float atomics differs.  No explicit neighbour rows and no virial.
 template <int NA, int NZ, bool LAT = false>
 __global__ void __launch_bounds__(AEV_WARPS * 32, NA == 8 ? ANI_AEV_BWD_MEMBERS_MIN_CTAS : ANI_AEV_BWD_MEMBERS_MIN_CTAS - 1)
     k_aev_backward_members(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
@@ -1452,276 +1505,38 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, NA == 8 ? ANI_AEV_BWD_MEMBERS_
   const int i = lo + blockIdx.x * AEV_WARPS + warp;
   if (i >= hi) return;
   const WarpSmem s = carve(smem_raw + warp * warp_bytes, cap, true);
-  const int S = P.num_species;
-  const int nR = P.n_shf_r;
-  const int RL = S * nR;
-  constexpr int GSTRIDE = 36;
-  const unsigned present = (species_mask ? (unsigned)species_mask[0] : 0xffffffffu) & ((1u << S) - 1u);
+  const unsigned present = (species_mask ? (unsigned)species_mask[0] : 0xffffffffu) & ((1u << P.num_species) - 1u);
   const int n_present = __popc(present);
-  // [buffer 0 | buffer 1] of {g_rad [RL], g_ang [pair_cap][36]}, then dfc(R; Rcr) per neighbour
+  // [table 0 | table 1] of gbuf_floats each, then dfc(R; Rcr) per neighbour
   float* ndfc = s.rad + 2 * gbuf_floats;
   const size_t row = (size_t)row_of[i] * ldx;
-
-  auto copy_async4 = [](float* dst_smem, const float* src) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src)
-                 : "memory");
-  };
-  // member k's row -> buffer k & 1 (one commit group per member; an empty group past the last member)
+  auto member_row = [&](int k) { return slabs + (size_t)ms.idx[k] * ms.stride + row; };
+  // member k's row -> table k & 1 (one commit group per member; an empty group past the last member)
   auto stage = [&](int k) {
-    if (k < ms.count) {
-      const float* gaev = slabs + (size_t)ms.idx[k] * ms.stride + row;
-      float* g_rad = s.rad + (k & 1) * gbuf_floats;
-      float* g_ang = g_rad + ((RL + 3) & ~3);
-      for (int t = lane; t < RL; t += 32) copy_async4(g_rad + t, gaev + t);
-      int c1 = 0;
-      for (unsigned m1 = present; m1; m1 &= m1 - 1, ++c1) {
-        const int s1 = __ffs(m1) - 1;
-        const int base = s1 * (2 * S - s1 + 1) / 2 - s1;
-        int c2 = c1;
-        for (unsigned m2 = m1; m2; m2 &= m2 - 1, ++c2) {
-          const int pp = base + __ffs(m2) - 1;
-          const int cp = c1 * (2 * n_present - c1 + 1) / 2 + (c2 - c1);
-          if (cp < pair_cap) copy_async4(g_ang + cp * GSTRIDE + lane, gaev + RL + P.ang_pad + pp * 32 + lane);
-        }
-      }
-    }
+    if (k < ms.count) stage_grad_row(P, s.rad + (k & 1) * gbuf_floats, member_row(k), present, n_present, pair_cap);
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
   stage(0);
 
-  // ---- geometry of the stored neighbours, once for all members
-  const float4 pi = spos[i];
   const int cnt = nbr_cnt[i];
   const int conf_i = LAT ? sorted_orig[i] / g.n_per_conf : 0;
-  for (int n = lane; n < cnt; n += 32) {
-    const int word = nbr_list[(size_t)i * cap + n];
-    const int j = word & ANI_IDX_MASK;
-    const int code = (unsigned)word >> ANI_IMG_SHIFT;
-    const float4 p = spos[j];
-    float3 sh = make_float3(0.f, 0.f, 0.f);
-    if (code != 13) sh = LAT ? image_shift(lattice, conf_i, code) : image_shift(g, code);
-    const float dx = (p.x + sh.x) - pi.x, dy = (p.y + sh.y) - pi.y, dz = (p.z + sh.z) - pi.z;
-    const float4 dR = make_float4(dx, dy, dz, sqrtf(dx * dx + dy * dy + dz * dz));
-    s.nd[n] = dR;
-    s.nj[n] = j;
-    s.nsp[n] = (unsigned char)__float_as_int(p.w);
-    float fc, dfc;
-    cutoff_value_grad(dR.w, P.rcr, P.cutoff_kind, fc, dfc);
-    s.nfc[n] = fc;
-    ndfc[n] = dfc;
-  }
+  backward_geometry<LAT>(P, g, s, spos, spos[i], i, cnt, ExplicitNbrs{nullptr, nullptr, nullptr}, 0, nbr_list, cap,
+                         lattice, conf_i, ndfc, 1);
   __syncwarp();
   const int n_ang = compact_angular_list(P, s, cnt, lane, status);
-  const int oi = sorted_orig[i];
 
   for (int k = 0; k < ms.count; ++k) {
     stage(k + 1);
     asm volatile("cp.async.wait_group 1;" ::: "memory");  // member k's row has landed
     __syncwarp();
-    const float* g_rad = s.rad + (k & 1) * gbuf_floats;
-    const float* g_ang = g_rad + ((RL + 3) & ~3);
-    const float* gaev = slabs + (size_t)ms.idx[k] * ms.stride + row;
-    float* gout = grad_members + (size_t)k * grad_stride;
-
-    // ---- radial
-    for (int n = lane; n < cnt; n += 32) {
-      const float4 d = s.nd[n];
-      const float fc = s.nfc[n], dfc = ndfc[n];
-      const float* __restrict__ gr = g_rad + s.nsp[n] * nR;
-      float acc = 0.f;
-#pragma unroll 4
-      for (int m = 0; m < nR; ++m) {
-        const float x = d.w - P.shf_r[m];
-        const float G = 0.25f * fast_exp(-P.eta_r * x * x);
-        acc = fmaf(gr[m] * G, fmaf(-2.0f * P.eta_r * x, fc, dfc), acc);
-      }
-      const float sc = d.w > 1e-10f ? acc * fast_rcp(d.w) : 0.f;
-      s.fgrad[3 * n + 0] = sc * d.x;
-      s.fgrad[3 * n + 1] = sc * d.y;
-      s.fgrad[3 * n + 2] = sc * d.z;
-    }
+    const float* table = s.rad + (k & 1) * gbuf_floats;
+    radial_backward(P, s, cnt, table, ndfc, 1);
     __syncwarp();
-
-    // ---- angular (as in k_aev_backward)
-    if (n_ang >= 2) {
-      // (the angular constants are read from the kernel parameters, constant-bank operands, not held in registers)
-      auto pair_sums = [&](const float4& dj, const float4& dk, int sj, int sk, float& cosT, float& inv_rr, float& S0,
-                           float& S1, float& S2) {
-        const float dot = dj.x * dk.x + dj.y * dk.y + dj.z * dk.z;
-        inv_rr = fast_rcp(fmaxf(dj.w * dk.w, 1e-10f));
-        cosT = dot * inv_rr;
-        const float c = 0.95f * cosT;
-        const float sn = fast_sqrt(fmaxf(1.0f - c * c, 0.f));
-        const float c_over_s = c * fast_rcp(sn);
-        const float rbar = 0.5f * (dj.w + dk.w);
-        const int cj = __popc(present & ((1u << sj) - 1u)), ck = __popc(present & ((1u << sk) - 1u));
-        const int clo = min(cj, ck), chi = max(cj, ck);
-        const int cp = clo * (2 * n_present - clo + 1) / 2 + (chi - clo);
-        const float4* __restrict__ gp =
-            cp < pair_cap ? reinterpret_cast<const float4*>(g_ang + cp * GSTRIDE)
-                          : reinterpret_cast<const float4*>(gaev + RL + P.ang_pad + pair_index(sj, sk, S) * 32);
-        float tz[NZ], uz[NZ];
-#pragma unroll
-        for (int z = 0; z < NZ; ++z) tz[z] = uz[z] = 0.f;
-#pragma unroll
-        for (int a = 0; a < NA; ++a) {
-          const float d = rbar - P.shf_a[a];
-          const float f2 = fast_exp(-P.eta_a * d * d);
-          const float f2p = -2.0f * P.eta_a * d * f2;
-#pragma unroll
-          for (int q = 0; q < NZ / 4; ++q) {
-            const float4 gv = gp[a * (NZ / 4) + q];
-            tz[4 * q + 0] = fmaf(gv.x, f2, tz[4 * q + 0]);
-            tz[4 * q + 1] = fmaf(gv.y, f2, tz[4 * q + 1]);
-            tz[4 * q + 2] = fmaf(gv.z, f2, tz[4 * q + 2]);
-            tz[4 * q + 3] = fmaf(gv.w, f2, tz[4 * q + 3]);
-            uz[4 * q + 0] = fmaf(gv.x, f2p, uz[4 * q + 0]);
-            uz[4 * q + 1] = fmaf(gv.y, f2p, uz[4 * q + 1]);
-            uz[4 * q + 2] = fmaf(gv.z, f2p, uz[4 * q + 2]);
-            uz[4 * q + 3] = fmaf(gv.w, f2p, uz[4 * q + 3]);
-          }
-        }
-        S0 = S1 = S2 = 0.f;
-#pragma unroll
-        for (int z = 0; z < NZ; ++z) {
-          const float base = fmaxf(0.5f * (1.0f + c * P.cos_z[z] + sn * P.sin_z[z]), 0.f);
-          const float lg = fast_log2(base);
-          const float f1 = fast_exp2(P.zeta * lg);
-          const float pw1 = fast_exp2((P.zeta - 1.0f) * lg);
-          const float f1p = P.zeta * pw1 * (0.475f * (P.cos_z[z] - c_over_s * P.sin_z[z]));
-          S0 = fmaf(f1, tz[z], S0);
-          S1 = fmaf(f1p, tz[z], S1);
-          S2 = fmaf(f1, uz[z], S2);
-        }
-      };
-      int lpr = 1;
-      while (lpr * 2 * n_ang <= 32) lpr *= 2;
-      const int sub = lane % lpr;
-      if (n_ang <= 32) {
-        // rotation over unordered pairs, see k_aev_backward
-        const int j = lane / lpr;
-        const bool jvalid = j < n_ang;
-        const int half_n = n_ang >> 1;
-        const bool even = (n_ang & 1) == 0;
-        float gx = 0.f, gy = 0.f, gz = 0.f;
-        int nj_ = 0, sj = 0;
-        float4 dj = make_float4(0.f, 0.f, 0.f, 1.f);
-        float fcj = 0.f, dfcj = 0.f, inv_rj = 0.f;
-        if (jvalid) {
-          nj_ = s.aidx[j];
-          dj = s.nd[nj_];
-          fcj = s.afc[j];
-          dfcj = s.afcd[j];
-          sj = s.nsp[nj_];
-          inv_rj = dj.w > 1e-10f ? fast_rcp(dj.w) : 0.f;
-        }
-        const int steps = (half_n + lpr - 1) / lpr;
-        for (int it = 0; it < steps; ++it) {
-          const int t = 1 + it * lpr + sub;
-          const bool active = jvalid && t <= half_n && !(even && t == half_n && j >= half_n);
-          float px = 0.f, py = 0.f, pz = 0.f;
-          if (active) {
-            int kk = j + t;
-            if (kk >= n_ang) kk -= n_ang;
-            const int nk_ = s.aidx[kk];
-            const float4 dk = s.nd[nk_];
-            const float fck = s.afc[kk], dfck = s.afcd[kk];
-            const float inv_rk = dk.w > 1e-10f ? fast_rcp(dk.w) : 0.f;
-            float cosT, inv_rr, S0, S1, S2;
-            pair_sums(dj, dk, sj, (int)s.nsp[nk_], cosT, inv_rr, S0, S1, S2);
-            const float W = fcj * fck;
-            const float dEdcos = 2.0f * W * S1;
-            const float dEdRj = S2 * W + 2.0f * S0 * dfcj * fck;
-            const float dEdRk = S2 * W + 2.0f * S0 * fcj * dfck;
-            const float coefj = (dEdRj - dEdcos * cosT * inv_rj) * inv_rj;
-            const float coefk = (dEdRk - dEdcos * cosT * inv_rk) * inv_rk;
-            const float coefx = dEdcos * inv_rr;
-            gx += coefj * dj.x + coefx * dk.x;
-            gy += coefj * dj.y + coefx * dk.y;
-            gz += coefj * dj.z + coefx * dk.z;
-            px = coefk * dk.x + coefx * dj.x;
-            py = coefk * dk.y + coefx * dj.y;
-            pz = coefk * dk.z + coefx * dj.z;
-          }
-          int src_row = j - t;
-          if (src_row < 0) src_row += n_ang;
-          const int src_lane = jvalid ? src_row * lpr + sub : lane;
-          const float rx = __shfl_sync(ANI_FULL_MASK, px, src_lane);
-          const float ry = __shfl_sync(ANI_FULL_MASK, py, src_lane);
-          const float rz = __shfl_sync(ANI_FULL_MASK, pz, src_lane);
-          if (jvalid) {
-            gx += rx;
-            gy += ry;
-            gz += rz;
-          }
-        }
-        for (int o = lpr / 2; o > 0; o >>= 1) {
-          gx += __shfl_xor_sync(ANI_FULL_MASK, gx, o);
-          gy += __shfl_xor_sync(ANI_FULL_MASK, gy, o);
-          gz += __shfl_xor_sync(ANI_FULL_MASK, gz, o);
-        }
-        if (jvalid && sub == 0) {
-          s.fgrad[3 * nj_ + 0] += gx;
-          s.fgrad[3 * nj_ + 1] += gy;
-          s.fgrad[3 * nj_ + 2] += gz;
-        }
-      } else {
-        // more rows than lanes: ordered pairs (j, k), several passes of 32 rows
-        for (int row0 = 0; row0 < n_ang; row0 += 32) {
-          const int j = row0 + lane;
-          float gx = 0.f, gy = 0.f, gz = 0.f;
-          if (j < n_ang) {
-            const int nj_ = s.aidx[j];
-            const float4 dj = s.nd[nj_];
-            const float fcj = s.afc[j], dfcj = s.afcd[j];
-            const int sj = s.nsp[nj_];
-            const float inv_rj = dj.w > 1e-10f ? fast_rcp(dj.w) : 0.f;
-            for (int kk = 0; kk < n_ang; ++kk) {
-              if (kk == j) continue;
-              const int nk_ = s.aidx[kk];
-              const float4 dk = s.nd[nk_];
-              const float fck = s.afc[kk];
-              float cosT, inv_rr, S0, S1, S2;
-              pair_sums(dj, dk, sj, (int)s.nsp[nk_], cosT, inv_rr, S0, S1, S2);
-              const float W = fcj * fck;
-              const float dEdRj = S2 * W + 2.0f * S0 * dfcj * fck;
-              const float dEdcos = 2.0f * W * S1;
-              const float coefj = (dEdRj - dEdcos * cosT * inv_rj) * inv_rj;
-              const float coefk = dEdcos * inv_rr;
-              gx += coefj * dj.x + coefk * dk.x;
-              gy += coefj * dj.y + coefk * dk.y;
-              gz += coefj * dj.z + coefk * dk.z;
-            }
-            s.fgrad[3 * nj_ + 0] += gx;
-            s.fgrad[3 * nj_ + 1] += gy;
-            s.fgrad[3 * nj_ + 2] += gz;
-          }
-        }
-      }
-    }
+    angular_backward<NA, NZ, false, true>(P, s, n_ang, table, member_row(k), present, n_present, pair_cap);
     __syncwarp();
-
-    // ---- scatter into member k's gradient: neighbour j gets +dE_i/dr_j, the centre minus the sum
-    float sx = 0.f, sy = 0.f, sz_ = 0.f;
-    for (int n = lane; n < cnt; n += 32) {
-      const float fx = s.fgrad[3 * n], fy = s.fgrad[3 * n + 1], fz = s.fgrad[3 * n + 2];
-      const int oj = sorted_orig[s.nj[n]];
-      atomicAdd(&gout[3 * (size_t)oj + 0], fx);
-      atomicAdd(&gout[3 * (size_t)oj + 1], fy);
-      atomicAdd(&gout[3 * (size_t)oj + 2], fz);
-      sx += fx;
-      sy += fy;
-      sz_ += fz;
-    }
-    sx = warp_sum(sx);
-    sy = warp_sum(sy);
-    sz_ = warp_sum(sz_);
-    if (lane == 0) {
-      atomicAdd(&gout[3 * (size_t)oi + 0], -sx);
-      atomicAdd(&gout[3 * (size_t)oi + 1], -sy);
-      atomicAdd(&gout[3 * (size_t)oi + 2], -sz_);
-    }
-    __syncwarp();  // fgrad and buffer k & 1 are rewritten by the next member
+    scatter_backward<false, LAT>(g, s, cnt, sorted_orig, i, conf_i, grad_members + (size_t)k * grad_stride,
+                                 nullptr);
+    __syncwarp();  // fgrad and table k & 1 are rewritten by the next member
   }
 }
 
@@ -1935,31 +1750,65 @@ static int launch_aev_forward(const ani_aev_params* params, const ani_grid* grid
   return ANI_OK;
 }
 
+// ---- backward launchers -------------------------------------------------------------------
+static int check_backward_args(const ani_aev_params* params, const ani_grid* grid, const float* spos,
+                               const int32_t* sorted_orig, int n, int lo, int hi, const int32_t* row_of,
+                               const float* grad_aev, const float* grad_out, const int32_t* status, int nbr_cap) {
+  int rc = check_params(params);
+  if (rc != ANI_OK) return rc;
+  if (!grid || !spos || !sorted_orig || !row_of || !grad_aev || !grad_out || !status) return ANI_ERR_BAD_ARG;
+  if (lo < 0 || hi > n || lo > hi) return ANI_ERR_BAD_ARG;
+  if (nbr_cap < 32 || nbr_cap > 256 || nbr_cap % 32) return ANI_ERR_BAD_ARG;
+  return ANI_OK;
+}
+
+// The shared-memory gradient table {g_rad, g_ang [pair_cap][GSTRIDE]} of the backward kernels.  Its rows are every
+// element pair, or the pairs of `max_elements` elements when the caller knows the composition (more elements at run
+// time still work: those pairs are read from global memory).  pair_sums reads the pairs beyond the table as float4 runs
+// of the upstream row, which needs the angular block 16-byte aligned in every row: RL + ang_pad, ldx and the stride
+// between slabs multiples of 4 (not so for, e.g., 7 elements x 15 shifts without ang_pad).  Otherwise the table holds
+// every pair and global memory is never read there.
+struct GradTable {
+  int pair_cap;
+  int floats;
+};
+static GradTable grad_table(const ani_aev_params* params, const int32_t* species_mask, int max_elements,
+                            const float* grad_aev, int ldx, long long slab_stride) {
+  const int S = params->num_species;
+  const int RL = S * params->n_shf_r;
+  const int E = (max_elements > 0 && max_elements < S) ? max_elements : S;
+  const bool ang_aligned = (RL + params->ang_pad) % 4 == 0 && ldx % 4 == 0 && ((uintptr_t)grad_aev & 15) == 0 &&
+                           slab_stride % 4 == 0;
+  const int pair_cap = (species_mask && ang_aligned) ? E * (E + 1) / 2 : S * (S + 1) / 2;
+  return GradTable{pair_cap, ((RL + 3) & ~3) + GSTRIDE * pair_cap};
+}
+
+// the template instance of a backward kernel for the angular shape (ShfA x ShfZ) and grid mode 3 (lattice table)
+template <int NA_, bool LAT_>
+struct BackwardShape {
+  static constexpr int NA = NA_, NZ = 32 / NA_;
+  static constexpr bool LAT = LAT_;
+};
+template <class F>
+static void dispatch_backward(const ani_aev_params* params, bool lattice, F&& f) {
+  if (params->n_shf_a == 8)
+    lattice ? f(BackwardShape<8, true>{}) : f(BackwardShape<8, false>{});
+  else
+    lattice ? f(BackwardShape<4, true>{}) : f(BackwardShape<4, false>{});
+}
+
 static int launch_aev_backward(const ani_aev_params* params, const ani_grid* grid, const float* spos,
                                const int32_t* sorted_orig, int n, int lo, int hi, const int32_t* row_of,
                                const float* grad_aev, int ldx, const int32_t* nbr_cnt, const int32_t* nbr_list,
                                ExplicitNbrs ex, const int32_t* species_mask, int nbr_cap, float* grad_coords,
                                int32_t* status, void* stream, int max_elements = 0, double* virial = nullptr,
                                const float* lattice = nullptr) {
-  int rc = check_params(params);
+  int rc = check_backward_args(params, grid, spos, sorted_orig, n, lo, hi, row_of, grad_aev, grad_coords, status,
+                               nbr_cap);
   if (rc != ANI_OK) return rc;
-  if (!grid || !spos || !sorted_orig || !row_of || !grad_aev || !grad_coords || !status) return ANI_ERR_BAD_ARG;
-  if (lo < 0 || hi > n || lo > hi) return ANI_ERR_BAD_ARG;
-  if (nbr_cap < 32 || nbr_cap > 256 || nbr_cap % 32) return ANI_ERR_BAD_ARG;
   if (hi == lo) return ANI_OK;
-  const int S = params->num_species;
-  const int RL = S * params->n_shf_r;
-  const int NP = S * (S + 1) / 2;
-  // rows of the shared-memory gradient table: every element pair, or the pairs of `max_elements`
-  // elements when the caller knows the composition (more elements at run time still work: those
-  // pairs are read from global memory)
-  const int E = (max_elements > 0 && max_elements < S) ? max_elements : S;
-  // pair_sums reads the pairs beyond the table as float4 runs of the upstream row, which needs the angular block
-  // 16-byte aligned in every row: RL + ang_pad and ldx multiples of 4 (not so for, e.g., 7 elements x 15 shifts
-  // without ang_pad).  Otherwise the table holds every pair and global memory is never read there.
-  const bool ang_aligned = (RL + params->ang_pad) % 4 == 0 && ldx % 4 == 0 && ((uintptr_t)grad_aev & 15) == 0;
-  const int pair_cap = (species_mask && ang_aligned) ? E * (E + 1) / 2 : NP;
-  const size_t wb = warp_smem_bytes(nbr_cap, ((RL + 3) & ~3) + 36 * pair_cap, true);
+  const GradTable t = grad_table(params, species_mask, max_elements, grad_aev, ldx, ldx);
+  const size_t wb = warp_smem_bytes(nbr_cap, t.floats, true);
   const size_t smem = wb * AEV_WARPS;
   const int blocks = (hi - lo + AEV_WARPS - 1) / AEV_WARPS;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1967,32 +1816,16 @@ static int launch_aev_backward(const ani_aev_params* params, const ani_grid* gri
   auto go = [&](auto k) {
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k<<<blocks, AEV_WARPS * 32, smem, st>>>(*params, grid, sp4, sorted_orig, lo, hi, row_of, grad_aev, ldx, nbr_cnt,
-                                            nbr_list, ex, species_mask, nbr_cap, grad_coords, status, wb, pair_cap,
+                                            nbr_list, ex, species_mask, nbr_cap, grad_coords, status, wb, t.pair_cap,
                                             virial, lattice);
   };
-  if (lattice) {   // grid mode 3
-    if (params->n_shf_a == 8) {
-      if (virial)
-        go(k_aev_backward<8, 4, true, true>);
-      else
-        go(k_aev_backward<8, 4, false, true>);
-    } else {
-      if (virial)
-        go(k_aev_backward<4, 8, true, true>);
-      else
-        go(k_aev_backward<4, 8, false, true>);
-    }
-  } else if (params->n_shf_a == 8) {
+  dispatch_backward(params, lattice, [&](auto sh) {
+    using Sh = decltype(sh);
     if (virial)
-      go(k_aev_backward<8, 4, true>);
+      go(k_aev_backward<Sh::NA, Sh::NZ, true, Sh::LAT>);
     else
-      go(k_aev_backward<8, 4, false>);
-  } else {
-    if (virial)
-      go(k_aev_backward<4, 8, true>);
-    else
-      go(k_aev_backward<4, 8, false>);
-  }
+      go(k_aev_backward<Sh::NA, Sh::NZ, false, Sh::LAT>);
+  });
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
 }
@@ -2003,12 +1836,10 @@ static int launch_aev_backward_members(const ani_aev_params* params, const ani_g
                                        const int32_t* members, int n_members, const int32_t* nbr_cnt,
                                        const int32_t* nbr_list, int nbr_cap, float* grad_members, int32_t* status,
                                        int max_elements, const float* lattice, void* stream) {
-  int rc = check_params(params);
+  int rc = check_backward_args(params, grid, spos, sorted_orig, n, lo, hi, row_of, slabs, grad_members, status,
+                               nbr_cap);
   if (rc != ANI_OK) return rc;
-  if (!grid || !spos || !sorted_orig || !row_of || !slabs || !grad_members || !status || !nbr_cnt || !nbr_list)
-    return ANI_ERR_BAD_ARG;
-  if (lo < 0 || hi > n || lo > hi) return ANI_ERR_BAD_ARG;
-  if (nbr_cap < 32 || nbr_cap > 256 || nbr_cap % 32) return ANI_ERR_BAD_ARG;
+  if (!nbr_cnt || !nbr_list) return ANI_ERR_BAD_ARG;
   if (n_members < 1 || n_members > ANI_MAX_MEMBERS || !members || slab_stride < (long long)ldx) return ANI_ERR_BAD_ARG;
   MemberSlabs ms;
   ms.count = n_members;
@@ -2019,38 +1850,21 @@ static int launch_aev_backward_members(const ani_aev_params* params, const ani_g
     ms.idx[k] = members[k];
   }
   if (hi == lo) return ANI_OK;
-  const int S = params->num_species;
-  const int RL = S * params->n_shf_r;
-  const int NP = S * (S + 1) / 2;
-  // the shared-memory gradient table as in launch_aev_backward; two of them (double-buffered rows), plus dfc per
-  // neighbour
-  const int E = (max_elements > 0 && max_elements < S) ? max_elements : S;
-  const bool ang_aligned = (RL + params->ang_pad) % 4 == 0 && ldx % 4 == 0 && ((uintptr_t)slabs & 15) == 0 &&
-                           slab_stride % 4 == 0;
-  const int pair_cap = (species_mask && ang_aligned) ? E * (E + 1) / 2 : NP;
-  const int gbuf = ((RL + 3) & ~3) + 36 * pair_cap;
-  const size_t wb = warp_smem_bytes(nbr_cap, 2 * gbuf + nbr_cap, true);
+  // two gradient tables (double-buffered rows), plus dfc per neighbour
+  const GradTable t = grad_table(params, species_mask, max_elements, slabs, ldx, slab_stride);
+  const size_t wb = warp_smem_bytes(nbr_cap, 2 * t.floats + nbr_cap, true);
   const size_t smem = wb * AEV_WARPS;
   const int blocks = (hi - lo + AEV_WARPS - 1) / AEV_WARPS;
   cudaStream_t st = (cudaStream_t)stream;
   const float4* sp4 = reinterpret_cast<const float4*>(spos);
-  auto go = [&](auto k) {
+  dispatch_backward(params, lattice, [&](auto sh) {
+    using Sh = decltype(sh);
+    auto k = k_aev_backward_members<Sh::NA, Sh::NZ, Sh::LAT>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k<<<blocks, AEV_WARPS * 32, smem, st>>>(*params, grid, sp4, sorted_orig, lo, hi, row_of, slabs, ldx, nbr_cnt,
                                             nbr_list, species_mask, nbr_cap, grad_members, 3LL * n, status, wb,
-                                            pair_cap, gbuf, lattice, ms);
-  };
-  if (params->n_shf_a == 8) {
-    if (lattice)
-      go(k_aev_backward_members<8, 4, true>);
-    else
-      go(k_aev_backward_members<8, 4>);
-  } else {
-    if (lattice)
-      go(k_aev_backward_members<4, 8, true>);
-    else
-      go(k_aev_backward_members<4, 8>);
-  }
+                                            t.pair_cap, t.floats, lattice, ms);
+  });
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
 }

@@ -605,6 +605,29 @@ class Engine:
             self._ws[key] = ws
         return ws
 
+    def _stage_inputs(self, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor], pbc: bool
+                      ) -> tp.Tuple[Workspace, bool]:
+        """Copy a step's inputs into the persistent buffers of its workspace (what a captured graph reads).  Returns the
+        workspace and whether it holds one cell per conformer."""
+        n_conf, n_per_conf = species.shape
+        if coords.shape != (n_conf, n_per_conf, 3):
+            raise ValueError("coords must have shape (C, A, 3)")
+        if pbc and cell is None:
+            raise ValueError("If pbc is not None, cell should be present")
+        per_conf = bool(pbc) and conformer_cells(cell, n_conf)
+        if per_conf and n_conf == 1:
+            cell, per_conf = cell[0], False   # one conformer: its cell is the shared cell
+        ws = self.workspace(n_conf, n_per_conf)
+        if pbc:
+            ws.make_periodic()
+        ws.species_i32.copy_(species.reshape(-1))
+        ws.coords.copy_(coords.reshape(-1, 3))
+        if per_conf:
+            ws.cells.copy_(cell.reshape(n_conf, 9))
+        elif pbc:
+            ws.cell.copy_(cell.reshape(-1))
+        return ws, per_conf
+
     # -- one step --------------------------------------------------------------------------
     def step(self, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor] = None, pbc: bool = False,
              want_grad: bool = True, shard: tp.Tuple[int, int] = (0, 1), want_virial: bool = False,
@@ -616,26 +639,9 @@ class Engine:
         The launch sequence of a given problem shape is captured into a CUDA graph on its fourth
         use and replayed afterwards (``cuda_graph=False`` at construction disables this)."""
         dev = self.device
-        n_conf, n_per_conf = species.shape
-        if coords.shape != (n_conf, n_per_conf, 3):
-            raise ValueError("coords must have shape (C, A, 3)")
         if species.device != dev or coords.device != dev:
             raise ValueError(f"inputs must live on {dev} (the engine has no CPU path)")
-        if pbc and cell is None:
-            raise ValueError("If pbc is not None, cell should be present")
-        per_conf = bool(pbc) and conformer_cells(cell, n_conf)
-        if per_conf and n_conf == 1:
-            cell, per_conf = cell[0], False   # one conformer: its cell is the shared cell
-        ws = self.workspace(n_conf, n_per_conf)
-        if pbc:
-            ws.make_periodic()
-        # inputs -> persistent buffers (what the graph reads)
-        ws.species_i32.copy_(species.reshape(-1))
-        ws.coords.copy_(coords.reshape(-1, 3))
-        if per_conf:
-            ws.cells.copy_(cell.reshape(n_conf, 9))
-        elif pbc:
-            ws.cell.copy_(cell.reshape(-1))
+        ws, per_conf = self._stage_inputs(species, coords, cell, pbc)
         res = self.run(ws, bool(pbc), want_grad, shard, want_virial=want_virial, conformer_cells=per_conf)
         if check:   # one 4-byte D2H read: cell too small / neighbour overflow / operand range raise here
             self.check_status(ws)
@@ -724,6 +730,57 @@ class Engine:
         return StepResult(ws.energies, ws.atomic.view(n_conf, n_per_conf),
                           ws.member_atomic.view(-1, n_conf, n_per_conf), grad, virial)
 
+    def _prepare(self, ws: Workspace, pbc: bool, conformer_cells: bool, lo: int, hi: int, reuse: bool,
+                 zero_ptr: tp.Optional[int], zero_count: int, virial: tp.Optional[Tensor],
+                 run: tp.Callable[[str, tp.Callable[[], int]], None], refresh_stage: str = "prepare_step"
+                 ) -> tp.Tuple[tp.Any, ...]:
+        """Enqueue the step's preparation: bucket grid + species-grouped row layout + live AEV column blocks, and the
+        zero-fill of the ``zero_count`` floats at ``zero_ptr`` (the force accumulator) and of ``virial`` -- one fused
+        entry point -- or, with a Verlet skin and reuse=True, one launch that only refreshes the positions inside the
+        grid of an earlier step (stage ``refresh_stage``).  ``run(name, fn)`` launches the stage.  Returns the extra arguments of the AEV entry
+        points: in grid mode 3 (one cell per conformer) the same kernels run through the ``_cells`` entry points, which
+        take the lattice table the preparation writes (the cells are read from the workspace by the preparation,
+        inside a captured graph)."""
+        L, c = self.lib, self.consts
+        n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        mode = _grid_mode(n_conf, pbc, conformer_cells)
+        prepare, cell_ptr, lat = L.ani_b200_prepare_step, ptr(ws.cell) if pbc else None, ()
+        if mode == 3:
+            prepare, cell_ptr, lat = L.ani_b200_prepare_step_cells, ptr(ws.cells), (ptr(ws.lattice),)
+        if reuse:
+            run(refresh_stage, lambda: L.ani_b200_verlet_positions(
+                1, ptr(ws.coords), ptr(ws.grid), ptr(ws.sorted_orig), n, self.skin, ptr(ws.spos), ptr(ws.ref_pos),
+                ptr(ws.ref_shift), ptr(ws.moved), zero_ptr, zero_count, ptr(ws.aev_blocks), self.nets.ldx, st))
+        else:
+            run("prepare_step", lambda: prepare(
+                ptr(ws.coords), ptr(ws.species_i32), n_conf, n_per_conf, cell_ptr, int(bool(pbc)), mode,
+                c.rcr + self.skin, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start), ptr(ws.sorted_orig),
+                ptr(ws.orig_to_sorted), ptr(ws.spos), ptr(ws.sbin), ptr(ws.bucket_ranges),
+                lo, hi, c.num_species, ws.rows_cap, ptr(ws.row_of), ptr(ws.row_atom), ptr(ws.tile_species),
+                ptr(ws.layout_info), len(c.shf_r), len(c.shf_a) * len(c.shf_z), c.out_dim, self.nets.ldx,
+                self.nets.col_pad, ptr(ws.aev_blocks), zero_ptr, zero_count,
+                ptr(virial) if virial is not None else None, virial.numel() if virial is not None else 0,
+                ptr(ws.bucket_species), ptr(ws.scratch), ptr(ws.status), *lat, st))
+            if self.skin > 0:
+                check(L.ani_b200_verlet_positions(
+                    0, ptr(ws.coords), ptr(ws.grid), ptr(ws.sorted_orig), n, self.skin, ptr(ws.spos),
+                    ptr(ws.ref_pos), ptr(ws.ref_shift), ptr(ws.moved), None, 0, None, self.nets.ldx, st),
+                    "verlet_positions")
+        return lat
+
+    def _aev_forward(self, ws: Workspace, lo: int, hi: int, reuse: bool, lat: tp.Tuple[tp.Any, ...],
+                     run: tp.Callable[[str, tp.Callable[[], int]], None]) -> None:
+        """Enqueue the AEV forward of atoms [lo, hi) into ``ws.x`` (``lat`` as returned by ``_prepare``)."""
+        L = self.lib
+        aev_forward = L.ani_b200_aev_forward_cells if lat else L.ani_b200_aev_forward
+        run("aev_forward", lambda: aev_forward(
+            C.byref(self.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sbin),
+            ptr(ws.bucket_ranges), ptr(ws.bucket_species) if not reuse else None,
+            ws.aev_blocks.data_ptr() + 4 * (ws.n_blocks + 1), ws.n, lo, hi,
+            ptr(ws.row_of), ptr(ws.x), self.nets.ldx, 1, ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap,
+            ptr(ws.status), *lat, torch.cuda.current_stream(self.device).cuda_stream))
+
     def _launch(self, ws: Workspace, pbc: bool, want_grad: bool, lo: int, hi: int, reuse: bool = False,
                 want_virial: bool = False, conformer_cells: bool = False, members: bool = False) -> None:
         """Enqueue the kernels of one step on the current stream (graph-capturable: no allocation,
@@ -734,39 +791,9 @@ class Engine:
         L = self.lib
         n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
         st = torch.cuda.current_stream(self.device).cuda_stream
-        cell_ptr = ptr(ws.cell) if pbc else None
-        mode = _grid_mode(n_conf, pbc, conformer_cells)
-        c = self.consts
-        # grid mode 3 (one cell per conformer): the same kernels through the entry points that take the lattice table
-        # the preparation writes; the cells are read from the workspace by the preparation (inside a captured graph)
-        prepare, aev_forward, aev_backward = L.ani_b200_prepare_step, L.ani_b200_aev_forward, L.ani_b200_aev_backward
-        lat: tp.Tuple[tp.Any, ...] = ()
-        if mode == 3:
-            prepare, aev_forward = L.ani_b200_prepare_step_cells, L.ani_b200_aev_forward_cells
-            aev_backward, lat, cell_ptr = L.ani_b200_aev_backward_cells, (ptr(ws.lattice),), ptr(ws.cells)
-        # bucket grid + species-grouped row layout + live AEV column blocks (+ zero-fill of the force
-        # accumulator): one fused entry point, five launches -- or, with a Verlet skin and reuse=True,
-        # one launch that only refreshes the positions inside the grid of an earlier step
-        if reuse:
-            self._timed("prepare_step", lambda: L.ani_b200_verlet_positions(
-                1, ptr(ws.coords), ptr(ws.grid), ptr(ws.sorted_orig), n, self.skin, ptr(ws.spos), ptr(ws.ref_pos),
-                ptr(ws.ref_shift), ptr(ws.moved), ws.grad_ptr if want_grad else None, 3 * n if want_grad else 0,
-                ptr(ws.aev_blocks), self.nets.ldx, st))
-        else:
-            self._timed("prepare_step", lambda: prepare(
-                ptr(ws.coords), ptr(ws.species_i32), n_conf, n_per_conf, cell_ptr, int(bool(pbc)), mode,
-                c.rcr + self.skin, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start), ptr(ws.sorted_orig),
-                ptr(ws.orig_to_sorted), ptr(ws.spos), ptr(ws.sbin), ptr(ws.bucket_ranges),
-                lo, hi, c.num_species, ws.rows_cap, ptr(ws.row_of), ptr(ws.row_atom), ptr(ws.tile_species),
-                ptr(ws.layout_info), len(c.shf_r), len(c.shf_a) * len(c.shf_z), c.out_dim, self.nets.ldx,
-                self.nets.col_pad, ptr(ws.aev_blocks), ws.grad_ptr if want_grad else None, 3 * n if want_grad else 0,
-                ptr(ws.virial) if want_virial else None, ws.virial.numel() if want_virial else 0,
-                ptr(ws.bucket_species), ptr(ws.scratch), ptr(ws.status), *lat, st))
-            if self.skin > 0:
-                check(L.ani_b200_verlet_positions(
-                    0, ptr(ws.coords), ptr(ws.grid), ptr(ws.sorted_orig), n, self.skin, ptr(ws.spos),
-                    ptr(ws.ref_pos), ptr(ws.ref_shift), ptr(ws.moved), None, 0, None, self.nets.ldx, st),
-                    "verlet_positions")
+        lat = self._prepare(ws, pbc, conformer_cells, lo, hi, reuse, ws.grad_ptr if want_grad else None,
+                            3 * n if want_grad else 0, ws.virial if want_virial else None, self._timed)
+        aev_backward = L.ani_b200_aev_backward_cells if lat else L.ani_b200_aev_backward
         # Two small kernels leave the critical path on a side stream (forked and joined with events, so
         # the whole thing still captures into one CUDA graph): the zero-fill of dE/dAEV runs beside the
         # AEV forward / forward GEMMs, the energy reduction beside the backward GEMMs / AEV backward.
@@ -780,12 +807,7 @@ class Engine:
             check(L.ani_b200_zero_live_blocks(C.byref(self.nets.model), ptr(ws.dx), ptr(ws.layout_info),
                                               ptr(ws.aev_blocks), side.cuda_stream), "zero_live_blocks")
             self._ev[1].record(side)
-        self._timed("aev_forward", lambda: aev_forward(
-            C.byref(self.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sbin),
-            ptr(ws.bucket_ranges), ptr(ws.bucket_species) if not reuse else None,
-            ws.aev_blocks.data_ptr() + 4 * (ws.n_blocks + 1), n, lo, hi,
-            ptr(ws.row_of), ptr(ws.x), self.nets.ldx, 1, ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap,
-            ptr(ws.status), *lat, st))
+        self._aev_forward(ws, lo, hi, reuse, lat, self._timed)
 
         def reduce_on(stream_handle):
             return L.ani_b200_reduce_energies(
@@ -875,42 +897,18 @@ class Engine:
         L = self.lib
         n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
         st = torch.cuda.current_stream(self.device).cuda_stream
-        c, nets = self.consts, self.nets
+        nets = self.nets
         active = list(nets.active)
         Ma = len(active)
         idx = (C.c_int32 * Ma)(*active)
-        mode = _grid_mode(n_conf, pbc, conformer_cells)
-        prepare, aev_forward, backward = L.ani_b200_prepare_step, L.ani_b200_aev_forward, L.ani_b200_aev_backward_members
-        lat: tp.Tuple[tp.Any, ...] = ()
-        cell_ptr = ptr(ws.cell) if pbc else None
-        if mode == 3:   # one cell per conformer, see _launch
-            prepare, aev_forward = L.ani_b200_prepare_step_cells, L.ani_b200_aev_forward_cells
-            backward, lat, cell_ptr = L.ani_b200_aev_backward_members_cells, (ptr(ws.lattice),), ptr(ws.cells)
-        gm, zero_count = ptr(ws.grad_members), 3 * n * Ma
-        if reuse:
-            check(L.ani_b200_verlet_positions(
-                1, ptr(ws.coords), ptr(ws.grid), ptr(ws.sorted_orig), n, self.skin, ptr(ws.spos), ptr(ws.ref_pos),
-                ptr(ws.ref_shift), ptr(ws.moved), gm, zero_count, ptr(ws.aev_blocks), nets.ldx, st), "verlet_positions")
-        else:
-            check(prepare(
-                ptr(ws.coords), ptr(ws.species_i32), n_conf, n_per_conf, cell_ptr, int(bool(pbc)), mode,
-                c.rcr + self.skin, ws.max_bins, ptr(ws.grid), ptr(ws.bin_start), ptr(ws.sorted_orig),
-                ptr(ws.orig_to_sorted), ptr(ws.spos), ptr(ws.sbin), ptr(ws.bucket_ranges), 0, n, c.num_species,
-                ws.rows_cap, ptr(ws.row_of), ptr(ws.row_atom), ptr(ws.tile_species), ptr(ws.layout_info),
-                len(c.shf_r), len(c.shf_a) * len(c.shf_z), c.out_dim, nets.ldx, nets.col_pad, ptr(ws.aev_blocks),
-                gm, zero_count, None, 0, ptr(ws.bucket_species), ptr(ws.scratch), ptr(ws.status), *lat, st),
-                "prepare_step")
-            if self.skin > 0:
-                check(L.ani_b200_verlet_positions(
-                    0, ptr(ws.coords), ptr(ws.grid), ptr(ws.sorted_orig), n, self.skin, ptr(ws.spos),
-                    ptr(ws.ref_pos), ptr(ws.ref_shift), ptr(ws.moved), None, 0, None, nets.ldx, st),
-                    "verlet_positions")
+        gm = ptr(ws.grad_members)
+
+        def run(name: str, fn: tp.Callable[[], int]) -> None:   # no profile events in this step
+            check(fn(), name)
+        lat = self._prepare(ws, pbc, conformer_cells, 0, n, reuse, gm, 3 * n * Ma, None, run, "verlet_positions")
+        self._aev_forward(ws, 0, n, reuse, lat, run)
+        backward = L.ani_b200_aev_backward_members_cells if lat else L.ani_b200_aev_backward_members
         mask_ptr = ws.aev_blocks.data_ptr() + 4 * (ws.n_blocks + 1)
-        check(aev_forward(
-            C.byref(self.params), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sbin),
-            ptr(ws.bucket_ranges), ptr(ws.bucket_species) if not reuse else None, mask_ptr, n, 0, n,
-            ptr(ws.row_of), ptr(ws.x), nets.ldx, 1, ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap,
-            ptr(ws.status), *lat, st), "aev_forward")
         unit = _lib.MLPModel.from_buffer_copy(nets.model)     # every active member with weight 1 (not 1 / M)
         for m in range(_lib.ANI_MAX_MEMBERS):
             unit.member_scale[m] = 1.0 if m in active else 0.0
@@ -951,24 +949,8 @@ class Engine:
         (arch.py:403-436 differentiates every member by autograd): the query-by-committee step,
         ``run(..., members=True)`` -- one MLP launch writes a dE_m/dAEV slab per member and ONE AEV backward contracts
         all of them -- captured into a CUDA graph like the ordinary step."""
-        n_conf, n_per_conf = species.shape
-        if coords.shape != (n_conf, n_per_conf, 3):
-            raise ValueError("coords must have shape (C, A, 3)")
-        if pbc and cell is None:
-            raise ValueError("If pbc is not None, cell should be present")
-        per_conf = bool(pbc) and conformer_cells(cell, n_conf)
-        if per_conf and n_conf == 1:
-            cell, per_conf = cell[0], False
-        ws = self.workspace(n_conf, n_per_conf)
-        if pbc:
-            ws.make_periodic()
         with torch.cuda.device(self.device):
-            ws.species_i32.copy_(species.reshape(-1))
-            ws.coords.copy_(coords.reshape(-1, 3))
-            if per_conf:
-                ws.cells.copy_(cell.reshape(n_conf, 9))
-            elif pbc:
-                ws.cell.copy_(cell.reshape(-1))
+            ws, per_conf = self._stage_inputs(species, coords, cell, pbc)
         self.run(ws, bool(pbc), True, members=True, conformer_cells=per_conf)
         r = self.members_result(ws)
         return r.energies.clone(), r.grad.clone()
