@@ -27,6 +27,9 @@
  *   ani_b200_aev_backward(..., virial, ...)   ase.py:164-168 (the "f dot r" virial of the stress)
  *   ani_b200_aev_backward_members  arch.py:403-436 (members_forces: one autograd pass per member)
  *   ani_b200_ensemble_qbc       arch.py:439-485,543-576 (energies_qbcs, force_magnitudes, force_qbc)
+ *   ani_b200_pair_potential     potentials/core.py:106-207, potentials/xtb.py:57-77, potentials/zbl.py:68-81
+ *                               (RepulsionXTB / RepulsionZBL over the step's own neighbour list); _pairs: over a
+ *                               caller-supplied half list, with ghost weights
  *   ani_b200_operand_format     (no counterpart: format of the tensor-core GEMM operands of this build)
  */
 #ifndef ANI_B200_H
@@ -266,6 +269,59 @@ int ani_b200_aev_backward_members_cells(const ani_aev_params* params, const ani_
 int ani_b200_ensemble_qbc(const float* grad_members, const int32_t* members, int n_members, const float* member_atomic,
                           const int32_t* species, const double* sae, int n_conf, int n_per_conf, float* grad,
                           float* atom_stats, double* member_energies, double* qbc, void* stream);
+
+/* 4g. Pair potentials over the neighbour list of the step (potentials/core.py:106-207: BasePairPotential;           */
+/*    potentials/xtb.py:57-77 RepulsionXTB; potentials/zbl.py:68-81 RepulsionZBL).  With d = max(R, 1e-7) * to_bohr:    */
+/*      kind 0 (xTB)  E = a[s][t] / d * exp(-b[s][t] * d^c[s][t])      a = y_ab, b = sqrt_alpha_ab, c = k_rep_ab          */
+/*      kind 1 (ZBL)  E = a[s][t] / d * sum_q screen_coeff[q] exp(-screen_exp[q] * b[s][t] * d)                          */
+/*                    a = Z_s Z_t, b = (Z_s^p + Z_t^p) / k                                                              */
+/*    times the envelope fc(R; cutoff): cutoff_fn 0 = cosine, 1 = smooth(2, 1e-10), 2 = none (then `cutoff` is not      */
+/*    read and no pair is screened out).  Pairs with R > cutoff contribute nothing.  The tables are symmetric.          */
+typedef struct ani_pair_params {
+  int32_t kind, cutoff_fn, num_species, pad_;
+  float cutoff;  /* Angstrom */
+  float to_bohr; /* Angstrom -> Bohr */
+  float a[ANI_MAX_SPECIES][ANI_MAX_SPECIES];
+  float b[ANI_MAX_SPECIES][ANI_MAX_SPECIES];
+  float c[ANI_MAX_SPECIES][ANI_MAX_SPECIES];
+  float screen_coeff[4], screen_exp[4];
+} ani_pair_params;
+
+/*    ani_b200_pair_potential evaluates one potential for the sorted atoms lo..hi-1 over the neighbour words             */
+/*    ani_b200_aev_forward left in nbr_cnt / nbr_list (so cutoff <= Rcr of that forward: the list holds nothing beyond)   */
+/*    and ADDS, per owned atom i with e_i = 1/2 sum_j E fc (the atomic split of potentials/core.py:196-200):             */
+/*      atomic        f32[n]  += e_i                     (flat input order; or NULL)                                    */
+/*      energies      f64[n_conf] += sum of e_i           (or NULL)                                                      */
+/*      grad_coords   f32[n][3] += dE/dr_i = sum_j d[E fc]/dR (-Delta_ij / R)   (or NULL)                                */
+/*      virial        += 1/2 (dE/dDelta_ij)_a (Delta_ij)_b per listed pair, buffers and slot rule of                     */
+/*                    ani_b200_aev_backward (or NULL)                                                                   */
+/*      member_atomic f32[M][n] row members[k] += e_i and grad_members f32[n_members][n][3] slab k += dE/dr_i for        */
+/*                    k < n_members (either may be NULL; members: HOST i32[n_members], read at launch): the reference    */
+/*                    adds a pair potential to every ensemble member (arch.py:365-378)                                   */
+/*    by plain read-modify-write -- every element has one writer, the atom's owner -- so the call must be ordered on    */
+/*    the stream after the kernels that produce those buffers (ani_b200_aev_backward[_members],                          */
+/*    ani_b200_reduce_energies) and before their consumers (ani_b200_ensemble_qbc, the all-reduce).  energies and the    */
+/*    virial take float64 atomics.  The per-rank results of a sharded run add up to the full answer.  One launch; no     */
+/*    status bits.  The _cells form is for grid mode 3 and takes its lattice table (not NULL).                          */
+int ani_b200_pair_potential(const ani_pair_params* params, const ani_grid* grid, const float* spos,
+                            const int32_t* sorted_orig, int n, int lo, int hi, int n_conf, int n_per_conf,
+                            const int32_t* nbr_cnt, const int32_t* nbr_list, int nbr_cap, float* atomic,
+                            double* energies, float* grad_coords, double* virial, float* member_atomic,
+                            float* grad_members, const int32_t* members, int n_members, void* stream);
+int ani_b200_pair_potential_cells(const ani_pair_params* params, const ani_grid* grid, const float* spos,
+                                  const int32_t* sorted_orig, int n, int lo, int hi, int n_conf, int n_per_conf,
+                                  const int32_t* nbr_cnt, const int32_t* nbr_list, int nbr_cap, float* atomic,
+                                  double* energies, float* grad_coords, double* virial, float* member_atomic,
+                                  float* grad_members, const int32_t* members, int n_members, const float* lattice,
+                                  void* stream);
+/*    The same potential over a caller-supplied HALF pair list (the reference's Neighbors tuple: flat input indices,    */
+/*    diff_vectors = x[idx0] - x[idx1] + shift): species i32[n_conf * n_per_conf] (-1 padding), ghost_flags u8 per atom  */
+/*    or NULL -- a pair that touches a ghost atom counts half (potentials/core.py:170-177).  ADDS (float atomics; any    */
+/*    of them may be NULL) atomic f32[n], energies f64[n_conf] and grad_coords f32[n][3] = dE/dcoords.                   */
+int ani_b200_pair_potential_pairs(const ani_pair_params* params, const int32_t* species, const int64_t* idx0,
+                                  const int64_t* idx1, const float* distances, const float* diff_vectors,
+                                  const uint8_t* ghost_flags, int64_t num_pairs, int n_conf, int n_per_conf,
+                                  float* atomic, double* energies, float* grad_coords, void* stream);
 
 /* 4b. The same AEV kernels fed by an externally supplied HALF pair list (the reference's    */
 /*    Neighbors tuple; AEVComputer.compute_from_neighbors, aev/_computer.py:251-272 ->          */

@@ -68,9 +68,20 @@ class MLPModel(C.Structure):
     ]
 
 
+class PairParams(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32), ("cutoff_fn", C.c_int32), ("num_species", C.c_int32), ("pad_", C.c_int32),
+        ("cutoff", C.c_float), ("to_bohr", C.c_float),
+        ("a", C.c_float * ANI_MAX_SPECIES * ANI_MAX_SPECIES), ("b", C.c_float * ANI_MAX_SPECIES * ANI_MAX_SPECIES),
+        ("c", C.c_float * ANI_MAX_SPECIES * ANI_MAX_SPECIES),
+        ("screen_coeff", C.c_float * 4), ("screen_exp", C.c_float * 4),
+    ]
+
+
 _P = C.c_void_p
 _I = C.c_int
 _F = C.c_float
+_PAIR_ARGS = [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I]
 
 _PROTOTYPES = {
     "ani_b200_abi_version": (C.c_int, []),
@@ -99,6 +110,9 @@ _PROTOTYPES = {
     "ani_b200_aev_backward_members_cells": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _I, C.c_longlong, _P, _I,
                                                       _P, _P, _I, _P, _P, _I, _P, _P]),
     "ani_b200_ensemble_qbc": (C.c_int, [_P, _P, _I, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
+    "ani_b200_pair_potential": (C.c_int, _PAIR_ARGS + [_P]),
+    "ani_b200_pair_potential_cells": (C.c_int, _PAIR_ARGS + [_P, _P]),
+    "ani_b200_pair_potential_pairs": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int64, _I, _I, _P, _P, _P, _P]),
     "ani_b200_verlet_positions":(C.c_int, [_I, _P, _P, _P, _I, _F, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
     "ani_b200_debug_gemm_trace": (C.c_int, [_P, _I]),
     "ani_b200_debug_aev_trace": (C.c_int, [_P]),

@@ -1,0 +1,294 @@
+// Pair potentials (short-range repulsion) evaluated over the neighbour list of the step.
+//
+// The AEV forward leaves, for every processed atom, the neighbours within Rcr as words (sorted index | image code
+// << 26), BOTH directions of every pair.  A pair potential with a cutoff <= Rcr therefore needs no neighbour search of
+// its own: the warp that owns atom i walks i's words, rebuilds Delta_ij = r_j + shift - r_i exactly as the AEV backward
+// does (image_shift of common.cuh, in the lattice of the central atom's conformer in grid mode 3) and sums
+//   e_i      = 1/2 sum_j E(R_ij) fc(R_ij)                 (potentials/core.py:196-200, the atomic split)
+//   dE/dr_i  = sum_j d[E fc]/dR (-Delta_ij / R_ij)        (the whole gradient on i: the list is full)
+//   W_ab    += 1/2 sum_j (d[E fc]/dR Delta_a / R) Delta_b (the "f dot r" virial of ase.py:164-168)
+// No scatter and no atomics on the forces, a fixed summation order (lane-strided partial sums, butterfly reduction),
+// and central-atom shards need nothing new: an atom's gradient comes from the rank that owns it, a pair's energy is
+// split between the owners of its two ends.
+//
+// Functional forms (potentials/xtb.py:57-77, potentials/zbl.py:68-81), d = max(R, 1e-7) * to_bohr:
+//   xTB  E = y_ab / d * exp(-sqrt_alpha_ab * d^k_ab)
+//   ZBL  E = Z_a Z_b / d * sum_q c_q exp(-x_q * d * (Z_a^p + Z_b^p) / k)
+// Arithmetic: expf / sqrtf / powf and true divisions (the repulsion is of order 1 Ha at 0.4 A, so the approximate MUFU
+// forms of the AEV kernels would cost the 1e-5 relative bar on atomic energies); d^1.5 is d * sqrt(d).
+#include "common.cuh"
+
+namespace ani {
+
+constexpr int PAIR_WARPS = 8;
+
+// Active members of a query-by-committee step: output k of grad_members belongs to member idx[k] of member_atomic
+struct PairMembers {
+  int count;
+  int idx[ANI_MAX_MEMBERS];
+};
+
+// E(R) fc(R) and its derivative with respect to R (Angstrom) for the element pair (a, b)
+__device__ __forceinline__ void pair_energy(const ani_pair_params& P, int a, int b, float R, float& e, float& de) {
+  const float d = fmaxf(R, 1e-7f) * P.to_bohr;   // potentials/core.py:137-139
+  float E, dE;                                   // dE: dE/dd
+  if (P.kind == 0) {
+    const float y = P.a[a][b], sa = P.b[a][b], k = P.c[a][b];
+    const float dk = (k == 1.5f) ? d * sqrtf(d) : (k == 1.0f) ? d : powf(d, k);
+    E = y / d * expf(-sa * dk);
+    dE = -E * (1.0f + sa * k * dk) / d;
+  } else {
+    const float zz = P.a[a][b], s = P.b[a][b];
+    float sum = 0.f, dsum = 0.f;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float t = P.screen_coeff[q] * expf(-P.screen_exp[q] * s * d);
+      sum += t;
+      dsum = fmaf(-P.screen_exp[q] * s, t, dsum);
+    }
+    E = zz / d * sum;
+    dE = (zz * dsum - E) / d;
+  }
+  dE = (R >= 1e-7f) ? dE * P.to_bohr : 0.f;      // the clamp has no slope below its floor
+  float f = 1.f, df = 0.f;
+  if (P.cutoff_fn != 2) cutoff_value_grad(R, P.cutoff, P.cutoff_fn, f, df);
+  e = E * f;
+  de = fmaf(dE, f, E * df);
+}
+
+// One warp per sorted atom i in lo..hi-1.  Everything is ADDED to what the step has produced so far, by plain
+// read-modify-write: every output element of an atom has exactly one writer (the warp that owns the atom), and the
+// launch is ordered on the stream after the kernels that accumulate into the same buffers (the AEV backward's atomics
+// into grad, the energy reduction's stores into atomic / member_atomic / energies).  The conformer energies and the
+// virial slots have many contributors and take float64 atomics, one per CTA and conformer / one per warp.
+template <bool LAT, bool VIRIAL>
+__global__ void __launch_bounds__(PAIR_WARPS * 32)
+    k_pair_potential(const __grid_constant__ ani_pair_params P, const ani_grid* __restrict__ grid,
+                     const float4* __restrict__ spos, const int32_t* __restrict__ sorted_orig, int n, int lo, int hi,
+                     int n_per_conf, const int32_t* __restrict__ nbr_cnt, const int32_t* __restrict__ nbr_list, int cap,
+                     const float* __restrict__ lattice, float* __restrict__ atomic, double* __restrict__ energies,
+                     float* __restrict__ grad, double* __restrict__ virial, float* __restrict__ member_atomic,
+                     float* __restrict__ grad_members, const __grid_constant__ PairMembers ms) {
+  __shared__ float s_e[PAIR_WARPS];
+  __shared__ int s_conf[PAIR_WARPS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const ani_grid g = *grid;
+  hi = min(hi, g.n_real);
+  const int i = lo + blockIdx.x * PAIR_WARPS + warp;
+  int conf_out = -1;
+  float e_out = 0.f;
+  if (i < hi) {
+    const float4 pi = spos[i];
+    const int si = __float_as_int(pi.w);
+    const int oi = sorted_orig[i];
+    const int conf_i = oi / n_per_conf;   // the neighbours of an atom lie in its conformer
+    const int cnt = min(nbr_cnt[i], cap);
+    float e = 0.f, gx = 0.f, gy = 0.f, gz = 0.f;
+    float vir[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) vir[k] = 0.f;
+    for (int t = lane; t < cnt && si >= 0; t += 32) {
+      const int word = nbr_list[(size_t)i * cap + t];
+      const int j = word & ANI_IDX_MASK;
+      const int code = (unsigned)word >> ANI_IMG_SHIFT;
+      const float4 p = spos[j];
+      float3 sh = make_float3(0.f, 0.f, 0.f);
+      if (code != 13) sh = LAT ? image_shift(lattice, conf_i, code) : image_shift(g, code);
+      const float dx = (p.x + sh.x) - pi.x, dy = (p.y + sh.y) - pi.y, dz = (p.z + sh.z) - pi.z;
+      const float R = sqrtf(dx * dx + dy * dy + dz * dz);
+      if (P.cutoff_fn != 2 && R > P.cutoff) continue;
+      float ep, de;
+      pair_energy(P, si, __float_as_int(p.w), R, ep, de);
+      e = fmaf(0.5f, ep, e);
+      const float sc = R >= 1e-7f ? de / R : 0.f;   // dE/dDelta = sc * Delta
+      const float fx = sc * dx, fy = sc * dy, fz = sc * dz;
+      gx -= fx;
+      gy -= fy;
+      gz -= fz;
+      if (VIRIAL) {
+        vir[0] = fmaf(fx, dx, vir[0]); vir[1] = fmaf(fx, dy, vir[1]); vir[2] = fmaf(fx, dz, vir[2]);
+        vir[3] = fmaf(fy, dx, vir[3]); vir[4] = fmaf(fy, dy, vir[4]); vir[5] = fmaf(fy, dz, vir[5]);
+        vir[6] = fmaf(fz, dx, vir[6]); vir[7] = fmaf(fz, dy, vir[7]); vir[8] = fmaf(fz, dz, vir[8]);
+      }
+    }
+    e = warp_sum(e);
+    gx = warp_sum(gx);
+    gy = warp_sum(gy);
+    gz = warp_sum(gz);
+    if (VIRIAL) {
+      // slot rule of the AEV backward: one set of slots per conformer of a periodic batch (grid modes 2, 3)
+      double* slots = virial + (size_t)(g.mode >= 2 ? conf_i : 0) * ANI_VIRIAL_SLOTS * 9;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) {
+        const float v = warp_sum(vir[k]);
+        if (lane == 0) atomicAdd(&slots[(blockIdx.x % ANI_VIRIAL_SLOTS) * 9 + k], 0.5 * (double)v);
+      }
+    }
+    if (lane == 0 && si >= 0) {
+      conf_out = conf_i;
+      e_out = e;
+      if (atomic) atomic[oi] += e;
+      if (grad) {
+        grad[3 * (size_t)oi + 0] += gx;
+        grad[3 * (size_t)oi + 1] += gy;
+        grad[3 * (size_t)oi + 2] += gz;
+      }
+      // the reference adds a pair potential to every member of the ensemble (arch.py:365-378)
+      for (int k = 0; k < ms.count; ++k) {
+        if (member_atomic) member_atomic[(size_t)ms.idx[k] * n + oi] += e;
+        if (grad_members) {
+          float* gm = grad_members + ((size_t)k * n + oi) * 3;
+          gm[0] += gx;
+          gm[1] += gy;
+          gm[2] += gz;
+        }
+      }
+    }
+  }
+  if (!energies) return;
+  if (lane == 0) {
+    s_e[warp] = e_out;
+    s_conf[warp] = conf_out;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {   // sorted atoms are conformer-major in a batch: runs of equal conformers, one atomic each
+    int c = -1;
+    double acc = 0.0;
+    for (int w = 0; w < PAIR_WARPS; ++w) {
+      if (s_conf[w] < 0) continue;
+      if (s_conf[w] != c) {
+        if (c >= 0) atomicAdd(&energies[c], acc);
+        c = s_conf[w];
+        acc = 0.0;
+      }
+      acc += (double)s_e[w];
+    }
+    if (c >= 0) atomicAdd(&energies[c], acc);
+  }
+}
+
+// The same potential over a caller-supplied HALF pair list (the reference's Neighbors tuple; diff = x[idx0] - x[idx1] +
+// shift): one thread per pair, float atomics (not the hot path).  Pairs that touch a ghost atom count half
+// (potentials/core.py:170-177); pairs beyond the cutoff and pairs with a padding atom contribute nothing.
+__global__ void k_pair_potential_pairs(const __grid_constant__ ani_pair_params P, const int32_t* __restrict__ species,
+                                       const int64_t* __restrict__ idx0, const int64_t* __restrict__ idx1,
+                                       const float* __restrict__ distances, const float* __restrict__ diff,
+                                       const uint8_t* __restrict__ ghost, long long num_pairs, int n_per_conf,
+                                       float* __restrict__ atomic, double* __restrict__ energies,
+                                       float* __restrict__ grad) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= num_pairs) return;
+  const long long i0 = idx0[p], i1 = idx1[p];
+  const int s0 = species[i0], s1 = species[i1];
+  const float R = distances[p];
+  if (s0 < 0 || s1 < 0 || (P.cutoff_fn != 2 && R > P.cutoff)) return;
+  float e, de;
+  pair_energy(P, s0, s1, R, e, de);
+  if (ghost && (ghost[i0] | ghost[i1])) {
+    e *= 0.5f;
+    de *= 0.5f;
+  }
+  if (atomic) {
+    atomicAdd(&atomic[i0], 0.5f * e);
+    atomicAdd(&atomic[i1], 0.5f * e);
+  }
+  if (energies) atomicAdd(&energies[i0 / n_per_conf], (double)e);
+  if (grad) {
+    const float sc = R >= 1e-7f ? de / R : 0.f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const float f = sc * diff[3 * p + k];
+      atomicAdd(&grad[3 * i0 + k], f);
+      atomicAdd(&grad[3 * i1 + k], -f);
+    }
+  }
+}
+
+static int check_pair_params(const ani_pair_params* p) {
+  if (!p) return ANI_ERR_BAD_ARG;
+  if (p->kind < 0 || p->kind > 1 || p->cutoff_fn < 0 || p->cutoff_fn > 2) return ANI_ERR_BAD_ARG;
+  if (p->num_species < 1 || p->num_species > ANI_MAX_SPECIES) return ANI_ERR_BAD_ARG;
+  if (!(p->to_bohr > 0.f)) return ANI_ERR_BAD_ARG;
+  if (p->cutoff_fn != 2 && !(p->cutoff > 0.f && p->cutoff < 1e30f)) return ANI_ERR_BAD_ARG;
+  return ANI_OK;
+}
+
+static int launch_pair_potential(const ani_pair_params* params, const ani_grid* grid, const float* spos,
+                                 const int32_t* sorted_orig, int n, int lo, int hi, int n_conf, int n_per_conf,
+                                 const int32_t* nbr_cnt, const int32_t* nbr_list, int nbr_cap, float* atomic,
+                                 double* energies, float* grad_coords, double* virial, float* member_atomic,
+                                 float* grad_members, const int32_t* members, int n_members, const float* lattice,
+                                 bool want_lattice, void* stream) {
+  const int rc = check_pair_params(params);
+  if (rc != ANI_OK) return rc;
+  if (!grid || !spos || !sorted_orig || !nbr_cnt || !nbr_list) return ANI_ERR_BAD_ARG;
+  if (want_lattice && !lattice) return ANI_ERR_BAD_ARG;
+  if (n_conf < 1 || n_per_conf < 1 || n != n_conf * n_per_conf || nbr_cap < 1) return ANI_ERR_BAD_ARG;
+  if (lo < 0 || hi > n || lo > hi) return ANI_ERR_BAD_ARG;
+  if (n_members < 0 || n_members > ANI_MAX_MEMBERS || (n_members > 0 && !members)) return ANI_ERR_BAD_ARG;
+  if ((member_atomic || grad_members) && n_members == 0) return ANI_ERR_BAD_ARG;
+  PairMembers ms;
+  ms.count = n_members;
+  for (int k = 0; k < ANI_MAX_MEMBERS; ++k) {
+    ms.idx[k] = k < n_members ? members[k] : 0;
+    if (ms.idx[k] < 0 || ms.idx[k] >= ANI_MAX_MEMBERS) return ANI_ERR_BAD_ARG;
+  }
+  if (hi == lo) return ANI_OK;
+  const int blocks = (hi - lo + PAIR_WARPS - 1) / PAIR_WARPS;
+  auto launch = [&](auto kernel) {
+    kernel<<<blocks, PAIR_WARPS * 32, 0, (cudaStream_t)stream>>>(
+        *params, grid, reinterpret_cast<const float4*>(spos), sorted_orig, n, lo, hi, n_per_conf, nbr_cnt, nbr_list,
+        nbr_cap, lattice, atomic, energies, grad_coords, virial, member_atomic, grad_members, ms);
+  };
+  if (want_lattice) {
+    virial ? launch(k_pair_potential<true, true>) : launch(k_pair_potential<true, false>);
+  } else {
+    virial ? launch(k_pair_potential<false, true>) : launch(k_pair_potential<false, false>);
+  }
+  ANI_CUDA_CHECK_LAUNCH();
+  return ANI_OK;
+}
+
+}  // namespace ani
+
+extern "C" int ani_b200_pair_potential(const ani_pair_params* params, const ani_grid* grid, const float* spos,
+                                       const int32_t* sorted_orig, int n, int lo, int hi, int n_conf, int n_per_conf,
+                                       const int32_t* nbr_cnt, const int32_t* nbr_list, int nbr_cap, float* atomic,
+                                       double* energies, float* grad_coords, double* virial, float* member_atomic,
+                                       float* grad_members, const int32_t* members, int n_members, void* stream) {
+  return ani::launch_pair_potential(params, grid, spos, sorted_orig, n, lo, hi, n_conf, n_per_conf, nbr_cnt, nbr_list,
+                                    nbr_cap, atomic, energies, grad_coords, virial, member_atomic, grad_members,
+                                    members, n_members, nullptr, false, stream);
+}
+
+extern "C" int ani_b200_pair_potential_cells(const ani_pair_params* params, const ani_grid* grid, const float* spos,
+                                             const int32_t* sorted_orig, int n, int lo, int hi, int n_conf,
+                                             int n_per_conf, const int32_t* nbr_cnt, const int32_t* nbr_list,
+                                             int nbr_cap, float* atomic, double* energies, float* grad_coords,
+                                             double* virial, float* member_atomic, float* grad_members,
+                                             const int32_t* members, int n_members, const float* lattice,
+                                             void* stream) {
+  return ani::launch_pair_potential(params, grid, spos, sorted_orig, n, lo, hi, n_conf, n_per_conf, nbr_cnt, nbr_list,
+                                    nbr_cap, atomic, energies, grad_coords, virial, member_atomic, grad_members,
+                                    members, n_members, lattice, true, stream);
+}
+
+extern "C" int ani_b200_pair_potential_pairs(const ani_pair_params* params, const int32_t* species,
+                                             const int64_t* idx0, const int64_t* idx1, const float* distances,
+                                             const float* diff_vectors, const uint8_t* ghost_flags, int64_t num_pairs,
+                                             int n_conf, int n_per_conf, float* atomic, double* energies,
+                                             float* grad_coords, void* stream) {
+  const int rc = ani::check_pair_params(params);
+  if (rc != ANI_OK) return rc;
+  if (num_pairs < 0 || n_conf < 1 || n_per_conf < 1) return ANI_ERR_BAD_ARG;
+  if (num_pairs == 0) return ANI_OK;
+  if (!species || !idx0 || !idx1 || !distances) return ANI_ERR_BAD_ARG;
+  if (grad_coords && !diff_vectors) return ANI_ERR_BAD_ARG;
+  const long long blocks = (num_pairs + 255) / 256;
+  if (blocks > 0x7fffffffLL) return ANI_ERR_BAD_ARG;
+  ani::k_pair_potential_pairs<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+      *params, species, idx0, idx1, distances, diff_vectors, ghost_flags, num_pairs, n_per_conf, atomic, energies,
+      grad_coords);
+  ANI_CUDA_CHECK_LAUNCH();
+  return ANI_OK;
+}

@@ -20,7 +20,7 @@ import torch
 from torch import Tensor
 
 from . import _lib
-from ._lib import AEVParams, Grid, MLPModel, check, ptr
+from ._lib import AEVParams, Grid, MLPModel, PairParams, check, ptr
 
 TILE = _lib.ANI_TILE_ROWS
 
@@ -503,6 +503,14 @@ def conformer_cells(cell: tp.Optional[Tensor], n_conf: int) -> bool:
     return True
 
 
+def check_pair_cutoff(cutoff: float, rcr: float) -> None:
+    """A pair potential runs in the fused step over the neighbour words of the AEV forward, which hold nothing beyond
+    the radial cutoff: its own cutoff may not be larger (there is no second neighbour search)."""
+    if not _f32(cutoff) <= _f32(rcr):
+        raise ValueError(f"a pair potential of the fused step needs cutoff <= the radial AEV cutoff ({rcr} A), got "
+                         f"{cutoff}: it is evaluated over the AEV's neighbour list, which holds nothing beyond it")
+
+
 class StepResult(tp.NamedTuple):
     energies: Tensor          # (C,) float64: NN energy + self energies of the owned atoms
     atomic_energies: Tensor   # (C, A) float32: NN atomic energies (ensemble mean), 0 for padding
@@ -527,12 +535,20 @@ class Engine:
     bucket-sorted atoms this engine owns (multi-GPU sharding, see parallel.py)."""
 
     def __init__(self, consts: AEVConstants, nets: PackedNetworks, sae: tp.Optional[tp.Sequence[float]] = None,
-                 nbr_cap: int = 128, cuda_graph: bool = True):
+                 nbr_cap: int = 128, cuda_graph: bool = True, pairs: tp.Sequence[PairParams] = ()):
+        """``pairs``: the ``ani_pair_params`` of the model's pair potentials (potentials.PairPotential.params()); each
+        adds one launch to the step (``_pair_potentials``), a model without any issues exactly the launches it
+        issued before."""
         if nets.in_dim != consts.out_dim:
             raise ValueError("network input width != AEV length")
         if nets.num_species != consts.num_species:
             raise ValueError("network / AEV species mismatch")
         self.consts, self.nets = consts, nets
+        for p in pairs:
+            check_pair_cutoff(math.inf if p.cutoff_fn == 2 else p.cutoff, consts.rcr)
+            if p.num_species != consts.num_species:
+                raise ValueError("pair potential / AEV species mismatch")
+        self.pairs = list(pairs)
         self.device = nets.device
         self.params = consts.to_struct()
         # internal column order of the tiled AEV operand / dE/dAEV rows: must be the one the layer-1 weights were packed in
@@ -720,7 +736,8 @@ class Engine:
             mlp = self.lib.ani_b200_mlp_step_windows(C.byref(self.nets.model), ws.rows_cap) + (1 if want_grad else 0)
         else:
             mlp = 3 + (4 if want_grad else 0)
-        self.launches_per_step = 1 + (0 if (pbc or n_conf > 1) else 1) + 1 + mlp + (1 if want_grad else 0) + 1
+        self.launches_per_step = (1 + (0 if (pbc or n_conf > 1) else 1) + 1 + mlp + (1 if want_grad else 0) + 1
+                                  + len(self.pairs))
         grad = ws.grad.view(n_conf, n_per_conf, 3) if want_grad else None
         virial = None
         if want_virial:
@@ -869,6 +886,9 @@ class Engine:
             main.wait_event(self._ev[3])
         else:
             self._timed("reduce_energies", lambda: reduce_on(st))
+        if self.pairs:
+            self._pair_potentials(ws, lo, hi, lat, ws.grad_ptr if want_grad else None,
+                                  ptr(ws.virial) if want_virial else None, None, self._timed)
         if ws.reducer is not None:
             # multi-GPU: sum the partial forces / energies of all ranks over NVLink peer memory (one launch,
             # part of the captured graph); without forces only the energies matter but the buffer is small
@@ -876,6 +896,26 @@ class Engine:
                 ws.reducer.launch(ws.grad, ws.energies)
                 return 0
             self._timed("allreduce", reduce_all)
+
+    def _pair_potentials(self, ws: Workspace, lo: int, hi: int, lat: tp.Tuple[tp.Any, ...], grad_ptr: tp.Optional[int],
+                         virial_ptr: tp.Optional[int], grad_members_ptr: tp.Optional[int],
+                         run: tp.Callable[[str, tp.Callable[[], int]], None]) -> None:
+        """Enqueue the model's pair potentials for atoms [lo, hi): one launch each over the neighbour words the AEV
+        forward left in the workspace, adding to the atomic / conformer energies, to every active member's atomic
+        energies (the reference adds a pair potential to every member, arch.py:365-378), to the gradient and the
+        virial and -- the query-by-committee step -- to every member's gradient.  The kernel adds by plain
+        read-modify-write, so it goes on the main stream after the AEV backward and the energy reduction and before
+        the statistics / the all-reduce."""
+        L = self.lib
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        active = list(self.nets.active)
+        idx = (C.c_int32 * len(active))(*active)
+        fn = L.ani_b200_pair_potential_cells if lat else L.ani_b200_pair_potential
+        for p in self.pairs:
+            run("pair_potential", lambda p=p: fn(
+                C.byref(p), ptr(ws.grid), ptr(ws.spos), ptr(ws.sorted_orig), ws.n, lo, hi, ws.n_conf, ws.n_per_conf,
+                ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap, ptr(ws.atomic), ws.energies_ptr, grad_ptr, virial_ptr,
+                ptr(ws.member_atomic), grad_members_ptr, idx, len(active), *lat, st))
 
     def members_buffers(self, ws: Workspace) -> None:
         """Allocate the per-member slabs and gradients of the query-by-committee step (once per workspace, before any
@@ -931,6 +971,8 @@ class Engine:
             C.byref(nets.model), ptr(ws.e_member), ws.rows_cap, ptr(ws.row_of), ptr(ws.orig_to_sorted),
             ptr(ws.species_i32), n, 0, n, n_conf, n_per_conf, ptr(self.sae), ptr(ws.atomic), ptr(ws.member_atomic),
             ws.energies_ptr, st), "reduce_energies")
+        if self.pairs:   # before the statistics: they read the members' atomic energies and gradients
+            self._pair_potentials(ws, 0, n, lat, None, None, gm, run)
         check(L.ani_b200_ensemble_qbc(
             gm, idx, Ma, ptr(ws.member_atomic), ptr(ws.species_i32), ptr(self.sae), n_conf, n_per_conf,
             ptr(ws.grad), ptr(ws.atom_stats), ptr(ws.member_energies), ptr(ws.qbc), st), "ensemble_qbc")

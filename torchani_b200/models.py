@@ -21,11 +21,13 @@ from torch import Tensor
 
 from . import _lib
 from .aev import AEVComputer
-from .engine import Engine, StepResult
+from .engine import Engine, StepResult, check_pair_cutoff
 from .neighbors import (CellList, Neighbors, NeighborlistArg, _validate_inputs, discard_outside_cutoff,
                         effective_periodic_cell, narrow_down, supercell_for_thin_cell)
 from .nn import (ANINetworks, ATOMIC_NUMBER, AtomicContainer, AtomicNetwork, Ensemble, SpeciesConverter,
                  SpeciesEnergies)
+from .potentials import PairPotential
+from . import potentials as _potentials
 
 SYMBOLS_1X = ("H", "C", "N", "O")
 SYMBOLS_2X = ("H", "C", "N", "O", "S", "F", "Cl")
@@ -123,7 +125,11 @@ class ANI(torch.nn.Module):
     r"""ANI-style neural network interatomic potential (interface of arch.py:90-381)."""
 
     def __init__(self, symbols: tp.Sequence[str], aev_computer: AEVComputer, neural_networks: AtomicContainer,
-                 energy_shifter: SelfEnergy, periodic_table_index: bool = True):
+                 energy_shifter: SelfEnergy, periodic_table_index: bool = True,
+                 potentials: tp.Optional[tp.Mapping[str, PairPotential]] = None):
+        """``potentials``: pair potentials evaluated next to the networks (arch.py:116-127), e.g.
+        ``{"repulsion_xtb": RepulsionXTB(...)}``.  They run inside the fused step over the AEV's own neighbour list,
+        so each needs ``cutoff <=`` the radial AEV cutoff."""
         super().__init__()
         self.register_buffer("atomic_numbers", torch.tensor([ATOMIC_NUMBER[e] for e in symbols], dtype=torch.long))
         assert len(energy_shifter.self_energies) == len(symbols)
@@ -136,6 +142,15 @@ class ANI(torch.nn.Module):
         self.energy_shifter = energy_shifter
         self.species_converter = SpeciesConverter(symbols)
         self.cutoff = aev_computer.radial.cutoff
+        for name, pot in (potentials or {}).items():
+            if name == "nnp" or not isinstance(pot, PairPotential):
+                raise ValueError(f"potential {name!r}: expected a torchani_b200.potentials.PairPotential under a name "
+                                 "other than 'nnp' (the networks)")
+            if tuple(pot.symbols) != tuple(symbols):
+                raise ValueError(f"potential {name!r} was built for other symbols")
+            check_pair_cutoff(pot.cutoff, self.cutoff)
+        # (the networks are the "nnp" potential of the reference and come first; they stay direct attributes here)
+        self.potentials = torch.nn.ModuleDict(dict(potentials or {}))
         self.periodic_table_index = periodic_table_index
         self._engine: tp.Optional[Engine] = None
         self._engine_key: tp.Any = None
@@ -156,7 +171,18 @@ class ANI(torch.nn.Module):
         if not isinstance(nets, Ensemble):
             raise ValueError("Only ensembles can be indexed")
         return ANI(self.symbols, copy.deepcopy(self.aev_computer), copy.deepcopy(nets[idx]),
-                   copy.deepcopy(self.energy_shifter), self.periodic_table_index)
+                   copy.deepcopy(self.energy_shifter), self.periodic_table_index,
+                   {k: copy.deepcopy(p) for k, p in self.potentials.items()})
+
+    def set_enabled(self, key: str, val: bool = True) -> None:
+        """arch.py:136-142: switch the energy shifter or a pair potential on or off."""
+        if key == "energy_shifter":
+            self.energy_shifter._enabled = val
+        else:
+            self.potentials[key]._enabled = val
+
+    def _enabled_potentials(self) -> tp.List[PairPotential]:
+        return [p for p in self.potentials.values() if p._enabled]
 
     def to_infer_model(self, use_mnp: bool = False) -> "ANI":
         return self
@@ -174,12 +200,15 @@ class ANI(torch.nn.Module):
         self.neural_networks._radial_len = c.num_species * len(c.shf_r)
         nets = self.neural_networks.packed(device)
         shifter = self.energy_shifter
-        # the engine bakes the self energies in: key it on their values (edits, `_enabled` toggles)
+        # the engine bakes the self energies and the pair-potential tables in: key it on their values (edits,
+        # `_enabled` toggles)
+        pairs = [p.params() for p in self._enabled_potentials()]
         key = (str(device), id(nets), bool(shifter._enabled), shifter.self_energies._version,
-               shifter.self_energies.data_ptr())
+               shifter.self_energies.data_ptr(), tuple(bytes(p) for p in pairs))
         if self._engine is None or self._engine_key != key:
             sae = self.energy_shifter.self_energies.tolist() if self.energy_shifter._enabled else None
-            self._engine = Engine(self.aev_computer.constants, nets, sae, nbr_cap=self.aev_computer.nbr_cap)
+            self._engine = Engine(self.aev_computer.constants, nets, sae, nbr_cap=self.aev_computer.nbr_cap,
+                                  pairs=pairs)
             self._engine_key = key
         return self._engine
 
@@ -258,6 +287,10 @@ class ANI(torch.nn.Module):
         neighbors = discard_outside_cutoff(neighbors, self.cutoff)
         aevs = self.aev_computer.compute_from_neighbors(elem_idxs, coords, neighbors)
         energies = self.neural_networks(elem_idxs, aevs, atomic, ensemble_values)
+        for pot in self._enabled_potentials():   # (C,) / (C, A): broadcast over the members, arch.py:365-378
+            energies = energies + pot.compute_from_neighbors(
+                elem_idxs, coords, discard_outside_cutoff(neighbors, pot.cutoff), charge, atomic,
+                ensemble_values).to(energies.dtype)
         if self.energy_shifter._enabled:
             energies = energies + self.energy_shifter(elem_idxs, atomic=atomic).to(energies.dtype)
         return energies
@@ -281,6 +314,9 @@ class ANI(torch.nn.Module):
         potentials/nnp.py:20-32).  Ghost atoms contribute as neighbours only: their energies are masked out, and
         ``torch.autograd.grad`` of the result gives dE/dx for local and ghost coordinates alike."""
         self._check_inputs(species, coords, 0)
+        if self._enabled_potentials():
+            raise NotImplementedError("pair potentials are not evaluated over a full neighbour list with ghost atoms; "
+                                      "disable them (set_enabled) or use compute_from_external_neighbors")
         elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
         aevs = self.aev_computer.compute_from_full_neighborlist(elem_idxs, coords, ilist_unique, jlist, numneigh)
         local = torch.zeros_like(elem_idxs, dtype=torch.bool).view(-1)
@@ -410,6 +446,10 @@ class ANI(torch.nn.Module):
         for old in list(state_dict.keys()):
             new = old.replace("potentials.nnp.aev_computer.", "aev_computer.")
             new = new.replace("potentials.nnp.neural_networks.", "neural_networks.")
+            if new.startswith(prefix + "potentials.1."):   # legacy numbered potentials, arch.py:278-290
+                new = new.replace("potentials.1.", "potentials.repulsion_xtb.", 1)
+            elif new.startswith(prefix + "potentials.2."):
+                new = new.replace("potentials.2.", "", 1)
             new = new.replace("radial_terms", "radial").replace("angular_terms", "angular")
             new = new.replace(".EtaR", ".eta").replace(".ShfR", ".shifts").replace(".EtaA", ".eta")
             new = new.replace(".Zeta", ".zeta").replace(".ShfA", ".shifts").replace(".ShfZ", ".sections")
@@ -529,7 +569,17 @@ def from_torchani(ref_model, device=None) -> ANI:
     nets = networks_from_torchani(netr)
     sae = SelfEnergy(symbols, ref_model.energy_shifter.self_energies.double().tolist())
     sae._enabled = bool(ref_model.energy_shifter._enabled)
-    model = ANI(symbols, aevc, nets, sae, ref_model.periodic_table_index)
+    # every other potential of the reference model is converted or refused, never dropped
+    extra = {}
+    for name, pot in ref_model.potentials.items():
+        if name == "nnp":
+            continue
+        try:
+            extra[name] = _potentials.from_torchani(pot)
+        except ValueError as exc:
+            raise ValueError(f"cannot convert potential {name!r} of the reference model: {exc}; a converted model "
+                             "without it would compute other energies and forces") from None
+    model = ANI(symbols, aevc, nets, sae, ref_model.periodic_table_index, extra)
     model.requires_grad_(False)
     if device is None:
         device = ref_model.energy_shifter.self_energies.device
@@ -549,4 +599,37 @@ def accelerate_torchani_(ref_model):
     nnp.aev_computer = aevc
     nnp.neural_networks = nets
     ref_model.neighborlist = aevc.neighborlist
+    # RepulsionXTB / RepulsionZBL members run through the CUDA pair-list kernel; any other potential stays as it is
+    for name, pot in list(ref_model.potentials.items()):
+        if name != "nnp" and type(pot).__name__ in ("RepulsionXTB", "RepulsionZBL"):
+            ref_model.potentials[name] = _DropInPairPotential(_potentials.from_torchani(pot).to(dev))
     return ref_model
+
+
+class _DropInPairPotential(torch.nn.Module):
+    """A CUDA pair potential in a reference model's ``potentials``: the reference's call convention
+    (``compute_from_neighbors(...) -> EnergiesScalars``-like object with ``.energies``) around ``PairPotential``."""
+
+    class _Energies(tp.NamedTuple):
+        energies: Tensor
+        scalars: tp.Optional[Tensor] = None
+
+    def __init__(self, potential: PairPotential):
+        super().__init__()
+        self.potential = potential
+        self.cutoff = potential.cutoff
+
+    @property
+    def _enabled(self) -> bool:
+        return self.potential._enabled
+
+    @_enabled.setter
+    def _enabled(self, val: bool) -> None:
+        self.potential._enabled = val
+
+    def compute_from_neighbors(self, elem_idxs: Tensor, coords: Tensor, neighbors, charge: int = 0,
+                               atomic: bool = False, ensemble_values: bool = False,
+                               ghost_flags: tp.Optional[Tensor] = None):
+        return self._Energies(self.potential.compute_from_neighbors(
+            elem_idxs, coords, Neighbors(neighbors.indices, neighbors.distances, neighbors.diff_vectors), charge,
+            atomic, ensemble_values, ghost_flags))

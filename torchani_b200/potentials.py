@@ -1,0 +1,254 @@
+"""Pair potentials with the interface of ``torchani.potentials`` (potentials/core.py:106-207): the short-range
+repulsion terms ``RepulsionXTB`` (potentials/xtb.py) and ``RepulsionZBL`` (potentials/zbl.py).
+
+Inside a model (``models.ANI(..., potentials={...})``) a pair potential is evaluated by the fused step over the
+neighbour list the AEV kernel has just built (``ani_b200_pair_potential``), which is why its cutoff may not exceed the
+radial AEV cutoff.  On its own a module evaluates a half pair list (``compute_from_neighbors``, ``forward``) through
+``ani_b200_pair_potential_pairs``.  CUDA float32 only; there is no CPU path.
+
+The reference's per-element xTB ``alpha`` / ``yeff`` defaults are not shipped: pass them, or convert a reference
+module (``from_torchani``), which reads its buffers.
+"""
+from __future__ import annotations
+
+import math
+import typing as tp
+
+import torch
+from torch import Tensor
+
+from . import _lib
+from ._lib import PairParams, check, ptr
+from .neighbors import Neighbors, all_pairs
+from .nn import ATOMIC_NUMBER
+
+ANGSTROM_TO_BOHR = 1.8897261258369282   # units.py:41
+_CUTOFF_FNS = {"cosine": 0, "smooth": 1, "dummy": 2}
+
+
+def _cutoff_fn_name(cutoff_fn: tp.Any) -> str:
+    """'cosine' / 'smooth' from a name or a reference cutoff module (cutoffs.py: CutoffCosine, CutoffSmooth with
+    order 2 and eps 1e-10, CutoffDummy)."""
+    if isinstance(cutoff_fn, str):
+        name = cutoff_fn
+    else:
+        name = {"CutoffCosine": "cosine", "CutoffSmooth": "smooth", "CutoffDummy": "dummy"}.get(
+            type(cutoff_fn).__name__, type(cutoff_fn).__name__)
+        if name == "smooth" and (getattr(cutoff_fn, "order", 2) != 2 or getattr(cutoff_fn, "eps", 1e-10) != 1e-10):
+            raise ValueError("only the smooth cutoff with order=2, eps=1e-10 is supported by the CUDA kernels")
+    if name not in ("cosine", "smooth", "dummy"):
+        raise ValueError(f"cutoff function {name!r} is not supported by the CUDA kernels")
+    return name
+
+
+class _PairEnergy(torch.autograd.Function):
+    """coords -> (energies (C,) float64, atomic energies (C, A)) over a half pair list; dE/dcoords is produced by the
+    forward launch (gradients reach ``coords`` only, as in ``AEVComputer.compute_from_neighbors``)."""
+
+    @staticmethod
+    def forward(ctx, coords: Tensor, elem_idxs: Tensor, neighbors: Neighbors, ghost_flags: tp.Optional[Tensor],
+                params: PairParams):
+        n_conf, n_per_conf = elem_idxs.shape
+        dev = coords.device
+        species = elem_idxs.reshape(-1).to(torch.int32).contiguous()
+        idx = neighbors.indices.to(torch.int64).contiguous()
+        dist = neighbors.distances.detach().to(torch.float32).contiguous()
+        diff = neighbors.diff_vectors.detach().to(torch.float32).contiguous()
+        ghost = None if ghost_flags is None else ghost_flags.reshape(-1).to(torch.uint8).contiguous()
+        want_grad = bool(coords.requires_grad)
+        atomic = torch.zeros(n_conf, n_per_conf, dtype=torch.float32, device=dev)
+        energies = torch.zeros(n_conf, dtype=torch.float64, device=dev)
+        grad = torch.zeros(n_conf, n_per_conf, 3, dtype=torch.float32, device=dev) if want_grad else None
+        with torch.cuda.device(dev):
+            check(_lib.lib().ani_b200_pair_potential_pairs(
+                _lib.C.byref(params), ptr(species), idx[0].data_ptr(), idx[1].data_ptr(), ptr(dist), ptr(diff),
+                ptr(ghost), idx.shape[1], n_conf, n_per_conf, ptr(atomic), ptr(energies), ptr(grad),
+                torch.cuda.current_stream(dev).cuda_stream), "pair_potential_pairs")
+        ctx.want_grad = want_grad
+        if want_grad:
+            ctx.save_for_backward(grad)
+        return energies, atomic
+
+    @staticmethod
+    def backward(ctx, g_energy, g_atomic):
+        if not ctx.want_grad:
+            raise RuntimeError("energies were computed without forces (coords.requires_grad was False)")
+        (grad,) = ctx.saved_tensors
+        out = torch.zeros_like(grad)
+        if g_energy is not None:
+            out = out + grad * g_energy.to(grad.dtype).view(-1, 1, 1)
+        if g_atomic is not None and bool((g_atomic != 0).any()):
+            if not bool((g_atomic == g_atomic[:, :1]).all()):
+                raise NotImplementedError("per-atom upstream gradients that differ inside a conformer are not supported")
+            out = out + grad * g_atomic[:, :1].to(grad.dtype).unsqueeze(-1)
+        return out, None, None, None, None
+
+
+class PairPotential(torch.nn.Module):
+    """Base of the pair potentials (potentials/core.py:106-207, ``BasePairPotential``).  Subclasses fill the
+    element-pair tables of ``ani_pair_params`` in ``_fill``."""
+
+    kind = -1
+
+    def __init__(self, symbols: tp.Sequence[str], *, cutoff: float = math.inf, cutoff_fn: tp.Any = "smooth"):
+        super().__init__()
+        if not 1 <= len(symbols) <= _lib.ANI_MAX_SPECIES:
+            raise ValueError(f"the CUDA kernels support 1..{_lib.ANI_MAX_SPECIES} elements")
+        self.symbols = tuple(symbols)
+        self.register_buffer("atomic_numbers", torch.tensor([ATOMIC_NUMBER[s] for s in symbols], dtype=torch.long),
+                             persistent=False)
+        self.cutoff = float(cutoff)
+        if not self.cutoff > 0:
+            raise ValueError("cutoff must be positive")
+        # potentials/core.py:132-135: without a cutoff there is no envelope
+        self.cutoff_fn = "dummy" if self.cutoff == math.inf else _cutoff_fn_name(cutoff_fn)
+        if self.cutoff != math.inf and self.cutoff_fn == "dummy":
+            raise ValueError("a finite cutoff needs the cosine or the smooth envelope")
+        self._enabled = True
+
+    def _fill(self, p: PairParams) -> None:
+        raise NotImplementedError
+
+    def params(self) -> PairParams:
+        """The ``ani_pair_params`` of this potential (built from its current buffers)."""
+        p = PairParams()
+        p.kind, p.cutoff_fn, p.num_species = self.kind, _CUTOFF_FNS[self.cutoff_fn], len(self.symbols)
+        p.cutoff = self.cutoff if self.cutoff != math.inf else 0.0
+        p.to_bohr = ANGSTROM_TO_BOHR
+        self._fill(p)
+        return p
+
+    def _table(self, dst, values: Tensor) -> None:
+        v = values.detach().to("cpu", torch.float64)
+        if not bool(torch.isfinite(v).all()):
+            raise ValueError("pair-potential parameters contain inf/NaN")
+        for a in range(v.shape[0]):
+            for b in range(v.shape[1]):
+                dst[a][b] = float(v[a, b])
+
+    def compute_from_neighbors(self, elem_idxs: Tensor, coords: Tensor, neighbors: Neighbors, charge: int = 0,
+                               atomic: bool = False, ensemble_values: bool = False,
+                               ghost_flags: tp.Optional[Tensor] = None) -> Tensor:
+        """Energies ``(C,)`` or ``(C, A)`` of the given half pair list (potentials/core.py:181-207; pairs beyond the
+        cutoff are ignored, pairs that touch a ghost atom count half; ``ensemble_values`` is disregarded as in the
+        reference)."""
+        assert elem_idxs.dim() == 2 and coords.shape == (elem_idxs.shape[0], elem_idxs.shape[1], 3)
+        if coords.device.type != "cuda":
+            raise ValueError("torchani_b200 runs on CUDA tensors only (there is no CPU path)")
+        if ghost_flags is not None and ghost_flags.numel() != elem_idxs.numel():
+            raise ValueError("ghost_flags and species should have the same number of elements")
+        energies, atomic_e = _PairEnergy.apply(coords, elem_idxs, neighbors, ghost_flags, self.params())
+        return atomic_e.to(coords.dtype) if atomic else energies.to(coords.dtype)
+
+    def forward(self, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor] = None,
+                pbc: tp.Optional[Tensor] = None, atomic: bool = False, ensemble_values: bool = False,
+                atomic_nums_input: bool = True) -> Tensor:
+        """potentials/core.py:37-67: the energies of this potential alone, with a neighbour list of its own."""
+        if self.cutoff == math.inf:
+            raise ValueError("forward() needs a finite cutoff (the neighbour list is a bucket grid); "
+                             "use compute_from_neighbors with a list of your own")
+        elem_idxs = species
+        if atomic_nums_input:
+            conv = torch.full((int(self.atomic_numbers.max()) + 2,), -1, dtype=torch.long, device=species.device)
+            conv[self.atomic_numbers.to(species.device)] = torch.arange(len(self.symbols), device=species.device)
+            elem_idxs = conv[species]
+        neighbors = all_pairs(self.cutoff, elem_idxs, coords, cell, pbc)
+        return self.compute_from_neighbors(elem_idxs, coords, neighbors, 0, atomic, ensemble_values)
+
+
+class RepulsionXTB(PairPotential):
+    r"""xTB repulsion (potentials/xtb.py:16-77): ``E = y_ab / d * exp(-sqrt_alpha_ab * d^k_ab)``, d in Bohr, ``k_ab =
+    krep`` except H-H (``krep_hydrogen``).  ``alpha`` and ``yeff`` (one value per symbol) are required."""
+
+    kind = 0
+
+    def __init__(self, symbols: tp.Sequence[str], krep_hydrogen: float = 1.0, krep: float = 1.5,
+                 alpha: tp.Sequence[float] = (), yeff: tp.Sequence[float] = (), *, cutoff: float = math.inf,
+                 cutoff_fn: tp.Any = "smooth"):
+        super().__init__(symbols, cutoff=cutoff, cutoff_fn=cutoff_fn)
+        for name, seq in (("alpha", alpha), ("yeff", yeff)):
+            if not len(seq):
+                raise ValueError(
+                    f"RepulsionXTB needs `{name}` (one value per symbol): the reference's per-element xTB parameter "
+                    "table is not shipped with torchani_b200; pass the values or convert a reference module "
+                    "(potentials.from_torchani / models.from_torchani), which reads its buffers")
+            if len(seq) != len(symbols):
+                raise ValueError(f"`{name}` needs one value per symbol")
+        k_rep_ab = torch.full((len(symbols), len(symbols)), float(krep))
+        if "H" in self.symbols:
+            h = self.symbols.index("H")
+            k_rep_ab[h, h] = float(krep_hydrogen)
+        _yeff = torch.tensor(list(yeff), dtype=torch.float32)
+        _alpha = torch.tensor(list(alpha), dtype=torch.float32)
+        self.register_buffer("y_ab", torch.outer(_yeff, _yeff))
+        self.register_buffer("sqrt_alpha_ab", torch.outer(_alpha, _alpha).sqrt())
+        self.register_buffer("k_rep_ab", k_rep_ab)
+
+    def _fill(self, p: PairParams) -> None:
+        self._table(p.a, self.y_ab)
+        self._table(p.b, self.sqrt_alpha_ab)
+        self._table(p.c, self.k_rep_ab)
+
+
+class RepulsionZBL(PairPotential):
+    r"""Ziegler-Biersack-Littmark screened nuclear repulsion (potentials/zbl.py:14-81):
+    ``E = Z_a Z_b / d * sum_q c_q exp(-x_q * d * (Z_a^p + Z_b^p) / k)``, d in Bohr.  The defaults are the published
+    universal screening function (the coefficient set LAMMPS uses, which sums to 1); effective Z = atomic number."""
+
+    kind = 1
+
+    def __init__(self, symbols: tp.Sequence[str], k: float = 0.8853,
+                 screen_coeffs: tp.Sequence[float] = (0.18175, 0.50986, 0.28022, 0.02817),
+                 screen_exponents: tp.Sequence[float] = (3.19980, 0.94229, 0.40290, 0.20162),
+                 eff_exponent: float = 0.23, eff_atomic_nums: tp.Sequence[float] = (), *, cutoff: float = math.inf,
+                 cutoff_fn: tp.Any = "smooth"):
+        super().__init__(symbols, cutoff=cutoff, cutoff_fn=cutoff_fn)
+        if len(screen_exponents) != len(screen_coeffs):
+            raise ValueError("screen_exponents and screen_coeffs must have the same len")
+        if len(screen_coeffs) != 4:
+            raise ValueError("the CUDA kernel evaluates exactly four screening terms")
+        if not math.isclose(sum(screen_coeffs), 1.0, abs_tol=1e-6):   # (float32 buffers of a converted module)
+            raise ValueError("Screen coeffs must sum to 1")
+        if not len(eff_atomic_nums):
+            eff_atomic_nums = [float(ATOMIC_NUMBER[s]) for s in symbols]
+        if len(eff_atomic_nums) != len(symbols):
+            raise ValueError("`eff_atomic_nums` needs one value per symbol")
+        self.register_buffer("_eff_atomic_nums", torch.tensor(list(eff_atomic_nums), dtype=torch.float32),
+                             persistent=False)
+        self.register_buffer("_coeffs", torch.tensor(list(screen_coeffs), dtype=torch.float32).view(1, -1),
+                             persistent=False)
+        self.register_buffer("_exponents", torch.tensor(list(screen_exponents), dtype=torch.float32).view(1, -1),
+                             persistent=False)
+        self._k = float(k)
+        self._kz = float(eff_exponent)
+
+    def _fill(self, p: PairParams) -> None:
+        z = self._eff_atomic_nums.detach().to("cpu", torch.float64)
+        self._table(p.a, torch.outer(z, z))
+        zp = z ** self._kz
+        self._table(p.b, (zp.view(-1, 1) + zp.view(1, -1)) / self._k)
+        for q in range(4):
+            p.screen_coeff[q] = float(self._coeffs.view(-1)[q])
+            p.screen_exp[q] = float(self._exponents.view(-1)[q])
+
+
+def from_torchani(ref_pot) -> PairPotential:
+    """A reference ``RepulsionXTB`` / ``RepulsionZBL`` module -> the CUDA module with the same parameters (read from the
+    module's buffers).  Any other potential raises ``ValueError``."""
+    name = type(ref_pot).__name__
+    symbols = tuple(ref_pot.symbols)
+    cutoff_fn = ref_pot.cutoff_fn
+    if name == "RepulsionXTB":
+        out: PairPotential = RepulsionXTB(symbols, alpha=[1.0] * len(symbols), yeff=[1.0] * len(symbols),
+                                          cutoff=ref_pot.cutoff, cutoff_fn=cutoff_fn)
+        for key in ("y_ab", "sqrt_alpha_ab", "k_rep_ab"):
+            getattr(out, key).copy_(getattr(ref_pot, key).detach().to("cpu", torch.float32))
+    elif name == "RepulsionZBL":
+        out = RepulsionZBL(symbols, k=ref_pot._k, screen_coeffs=ref_pot._coeffs.view(-1).tolist(),
+                           screen_exponents=ref_pot._exponents.view(-1).tolist(), eff_exponent=ref_pot._kz,
+                           eff_atomic_nums=ref_pot._eff_atomic_nums.tolist(), cutoff=ref_pot.cutoff,
+                           cutoff_fn=cutoff_fn)
+    else:
+        raise ValueError(f"potential {name} has no CUDA counterpart (RepulsionXTB and RepulsionZBL do)")
+    out._enabled = bool(ref_pot._enabled)
+    return out
