@@ -261,123 +261,39 @@ __device__ __forceinline__ void wrapped_position(const ani_grid& g, const float*
   if (LAT || g.mode == 2) bin += (a / g.n_per_conf) * (g.dims[0] * g.dims[1] * g.dims[2]);  // the conformer's sub-grid
 }
 
-__global__ void k_bin_assign(const float* __restrict__ coords, const int32_t* __restrict__ species, int n,
-                             const ani_grid* __restrict__ grid, int32_t* __restrict__ bin_of,
-                             int32_t* __restrict__ slot, int32_t* __restrict__ bin_count) {
-  int a = blockIdx.x * blockDim.x + threadIdx.x;
-  if (a >= n) return;
-  const ani_grid g = *grid;
+// ---------------------------------------------------------------------------------------
+// The phases of the preparation, written once.  Every preparation form (the three-call public API, the five-launch
+// sequence, the persistent grid, the cluster) is a sequence of these pieces.  Where the forms read an array
+// differently (plain loads, L2 loads of data another CTA wrote in the same launch, a CTA's shared-memory copy), the
+// caller passes the read as a functor.
+// ---------------------------------------------------------------------------------------
+constexpr int LAYOUT_CHUNK = 256;   // atoms per chunk of the species histograms and the row assignment
+
+// bucket of atom a and its slot inside the bucket (arrival order, by atomics)
+template <bool LAT = false>
+__device__ __forceinline__ void assign_bucket(const ani_grid& g, const float* __restrict__ coords,
+                                              const int32_t* __restrict__ species, int a, int32_t* __restrict__ bin_of,
+                                              int32_t* __restrict__ slot, int32_t* __restrict__ bin_count,
+                                              const float* __restrict__ lattice = nullptr) {
   int bin;
   if (species[a] < 0) {
     bin = g.nbins;  // padding atoms: trash bucket, never a neighbour, never a centre
   } else {
     float3 p;
-    wrapped_position(g, coords, a, p, bin);
+    wrapped_position<LAT>(g, coords, a, p, bin, lattice);
   }
   bin_of[a] = bin;
   slot[a] = atomicAdd(&bin_count[bin], 1);
 }
 
-// exclusive scan of cnt[0..m-1] -> start[0..m] by one block (m = nbins + 1, read from grid)
-__global__ void k_bin_scan(const int32_t* __restrict__ cnt, ani_grid* grid, int32_t* __restrict__ start) {
-  __shared__ int s_warp[32];
-  __shared__ int s_carry;
-  const int m = grid->nbins + 1;
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
-  for (int base = 0; base < m; base += blockDim.x) {
-    int i = base + tid;
-    int v = (i < m) ? cnt[i] : 0;
-    int x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int y = __shfl_up_sync(ANI_FULL_MASK, x, o);
-      if (lane >= o) x += y;
-    }
-    if (lane == 31) s_warp[w] = x;
-    __syncthreads();
-    if (w == 0) {
-      int t = (lane < (blockDim.x >> 5)) ? s_warp[lane] : 0;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        int y = __shfl_up_sync(ANI_FULL_MASK, t, o);
-        if (lane >= o) t += y;
-      }
-      s_warp[lane] = t;  // inclusive over warps
-    }
-    __syncthreads();
-    int warp_off = (w == 0) ? 0 : s_warp[w - 1];
-    int incl = x + warp_off + s_carry;
-    if (i < m) start[i] = incl - v;
-    __syncthreads();
-    if (tid == blockDim.x - 1) s_carry = incl;
-    __syncthreads();
-  }
-  if (tid == 0) {
-    start[m] = s_carry;
-    grid->n_real = start[m - 1];  // everything before the trash bucket
-  }
-}
-
-__global__ void k_bin_scatter(int n, const int32_t* __restrict__ bin_of, const int32_t* __restrict__ slot,
-                              const int32_t* __restrict__ bin_start, int32_t* __restrict__ tmp_list) {
-  int a = blockIdx.x * blockDim.x + threadIdx.x;
-  if (a >= n) return;
-  tmp_list[bin_start[bin_of[a]] + slot[a]] = a;
-}
-
-// the atomics above give an arbitrary order inside a bucket; rank by (species, input index) to make
-// the sorted order (and with it every later summation order) deterministic and species-grouped
-__global__ void k_bin_finalize(const float* __restrict__ coords, const int32_t* __restrict__ species, int n,
-                               const ani_grid* __restrict__ grid, const int32_t* __restrict__ bin_of,
-                               const int32_t* __restrict__ bin_start, const int32_t* __restrict__ tmp_list,
-                               int32_t* __restrict__ sorted_orig, int32_t* __restrict__ orig_to_sorted,
-                               float4* __restrict__ spos, int32_t* __restrict__ sbin) {
-  int a = blockIdx.x * blockDim.x + threadIdx.x;
-  if (a >= n) return;
-  const ani_grid g = *grid;
-  int b = bin_of[a];
-  int lo = bin_start[b], hi = bin_start[b + 1];
-  // order inside a bucket: by species, then by input index (deterministic; the AEV kernel relies on
-  // every bucket being species-sorted)
-  const int spa = species[a];
-  int rank = 0;
-  if (spa < 0) {
-    // trash bucket (padding atoms of a conformer batch, possibly thousands): all of one "species", so the rank is
-    // the number of smaller indices -- independent loads, no dependent species gather per entry
-    for (int e = lo; e < hi; ++e) rank += tmp_list[e] < a;
-  } else {
-    for (int e = lo; e < hi; ++e) {
-      const int t = tmp_list[e];
-      const int spt = species[t];
-      rank += (spt < spa) || (spt == spa && t < a);
-    }
-  }
-  int i = lo + rank;
-  sorted_orig[i] = a;
-  orig_to_sorted[a] = i;
-  sbin[i] = b;
-  float3 p = make_float3(0.f, 0.f, 0.f);
-  int sp = species[a];
-  if (sp >= 0) {
-    int bb;
-    wrapped_position(g, coords, a, p, bb);
-  }
-  spos[i] = make_float4(p.x, p.y, p.z, __int_as_float(sp));
-}
-
-// Per-bucket table of the 27 neighbouring buckets: {first atom, end atom, image code, exists} and
-// the image shift vector.  The AEV kernel then reads 27 records instead of redoing the index
-// wrapping and shift arithmetic for every central atom.
-__global__ void k_bucket_ranges(const ani_grid* __restrict__ grid, const int32_t* __restrict__ bin_start,
-                                float4* __restrict__ ranges) {
-  const ani_grid g = *grid;
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  const int b = idx / 27, o = idx % 27;
-  if (b >= g.nbins || g.mode == 1) return;
+// Record o (0..26) of bucket b's table of neighbouring buckets: r0 = {first atom, end atom, image code, neighbour
+// bucket}, r1 = the image shift in the lattice of the bucket's conformer.  Neighbours stay inside the conformer's
+// sub-grid; outside a non-periodic box the neighbour does not exist (empty range, bucket 0).  start(k) reads bin_start[k].
+template <bool LAT, class Start>
+__device__ __forceinline__ void neighbour_record(const ani_grid& g, const float* __restrict__ lattice, int b, int o,
+                                                 Start start, float4& r0, float4& r1) {
   int ix, iy, iz;
-  const int base = bucket_coords(g, b, ix, iy, iz);   // neighbours stay inside the conformer's sub-grid
+  const int base = bucket_coords(g, b, ix, iy, iz);
   int j[3] = {ix + o / 9 - 1, iy + (o / 3) % 3 - 1, iz + o % 3 - 1};
   int w[3];
   for (int d = 0; d < 3; ++d) {
@@ -393,16 +309,155 @@ __global__ void k_bucket_ranges(const ani_grid* __restrict__ grid, const int32_t
   const bool exists = g.pbc || !(w[0] | w[1] | w[2]);
   int lo = 0, hi = 0;
   const int code = (w[0] + 1) * 9 + (w[1] + 1) * 3 + (w[2] + 1);
+  const int nbk = exists ? base + (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2] : 0;
   if (exists) {
-    const int nb = base + (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2];
-    lo = bin_start[nb];
-    hi = bin_start[nb + 1];
+    lo = start(nbk);
+    hi = start(nbk + 1);
   }
   const float wx = (float)w[0], wy = (float)w[1], wz = (float)w[2];
-  ranges[2 * (size_t)idx] = make_float4(__int_as_float(lo), __int_as_float(hi), __int_as_float(code), 0.f);
-  ranges[2 * (size_t)idx + 1] = make_float4(wx * g.cell[0] + wy * g.cell[3] + wz * g.cell[6],
-                                            wx * g.cell[1] + wy * g.cell[4] + wz * g.cell[7],
-                                            wx * g.cell[2] + wy * g.cell[5] + wz * g.cell[8], 0.f);
+  float cl[9];
+  cell_of<LAT>(g, lattice, LAT ? base / (g.dims[0] * g.dims[1] * g.dims[2]) : 0, cl);
+  r0 = make_float4(__int_as_float(lo), __int_as_float(hi), __int_as_float(code), __int_as_float(nbk));
+  r1 = make_float4(wx * cl[0] + wy * cl[3] + wz * cl[6], wx * cl[1] + wy * cl[4] + wz * cl[7],
+                   wx * cl[2] + wy * cl[5] + wz * cl[8], 0.f);
+}
+
+// Exclusive scan of the bucket counts by one block of WARPS warps (the whole block calls it): store(i, start) for
+// i < m, where load(i) reads count i.  Returns the total to every thread.
+template <int WARPS, class Load, class Store>
+__device__ __forceinline__ int scan_bucket_counts(int m, Load load, Store store) {
+  __shared__ int s_warp[WARPS];
+  __shared__ int s_carry;
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  if (tid == 0) s_carry = 0;
+  __syncthreads();
+  for (int base = 0; base < m; base += blockDim.x) {
+    const int i = base + tid;
+    const int v = (i < m) ? load(i) : 0;
+    int x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(ANI_FULL_MASK, x, o);
+      if (lane >= o) x += y;
+    }
+    if (lane == 31) s_warp[w] = x;
+    __syncthreads();
+    if (w == 0) {
+      int t = (lane < WARPS) ? s_warp[lane] : 0;
+#pragma unroll
+      for (int o = 1; o < WARPS; o <<= 1) {
+        const int y = __shfl_up_sync(ANI_FULL_MASK, t, o);
+        if (lane >= o) t += y;
+      }
+      if (lane < WARPS) s_warp[lane] = t;  // inclusive over warps
+    }
+    __syncthreads();
+    const int incl = x + ((w == 0) ? 0 : s_warp[w - 1]) + s_carry;
+    if (i < m) store(i, incl - v);
+    __syncthreads();
+    if (tid == blockDim.x - 1) s_carry = incl;
+    __syncthreads();
+  }
+  return s_carry;
+}
+
+// The atomics above give an arbitrary order inside a bucket; rank by (species, input index) to make the sorted order
+// (and with it every later summation order) deterministic and every bucket species-sorted, as the AEV kernels require.
+// The rank of real atom a (species spa) among the bucket's members member(lo .. hi - 1).
+template <class Member>
+__device__ __forceinline__ int species_index_rank(const int32_t* __restrict__ species, int lo, int hi, int a, int spa,
+                                                  Member member) {
+  int rank = 0;
+  for (int e = lo; e < hi; ++e) {
+    const int t = member(e);
+    const int spt = species[t];
+    rank += (spt < spa) || (spt == spa && t < a);
+  }
+  return rank;
+}
+
+// Atom a (species sp) of bucket b at sorted position i: the sorted arrays, and with a chunk histogram the count of
+// a real atom in its 256-atom chunk of the owned sorted slice [lo, hi_real)
+template <bool LAT = false>
+__device__ __forceinline__ void place_atom(const ani_grid& g, const float* __restrict__ coords,
+                                           const float* __restrict__ lattice, int a, int sp, int b, int i,
+                                           int32_t* __restrict__ sorted_orig, int32_t* __restrict__ orig_to_sorted,
+                                           int32_t* __restrict__ sbin, float4* __restrict__ spos,
+                                           int32_t* __restrict__ chunk_hist = nullptr, int lo = 0, int hi_real = 0) {
+  sorted_orig[i] = a;
+  orig_to_sorted[a] = i;
+  sbin[i] = b;
+  float3 p = make_float3(0.f, 0.f, 0.f);
+  if (sp >= 0) {
+    int bb;
+    wrapped_position<LAT>(g, coords, a, p, bb, lattice);
+  }
+  spos[i] = make_float4(p.x, p.y, p.z, __int_as_float(sp));
+  if (chunk_hist && sp >= 0 && i >= lo && i < hi_real)
+    atomicAdd(&chunk_hist[((i - lo) / LAYOUT_CHUNK) * ANI_MAX_SPECIES + sp], 1);
+}
+
+__global__ void k_bin_assign(const float* __restrict__ coords, const int32_t* __restrict__ species, int n,
+                             const ani_grid* __restrict__ grid, int32_t* __restrict__ bin_of,
+                             int32_t* __restrict__ slot, int32_t* __restrict__ bin_count) {
+  int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= n) return;
+  const ani_grid g = *grid;
+  assign_bucket(g, coords, species, a, bin_of, slot, bin_count);
+}
+
+// exclusive scan of cnt[0..m-1] -> start[0..m] by one block of 1024 threads (m = nbins + 1, read from grid)
+__global__ void k_bin_scan(const int32_t* __restrict__ cnt, ani_grid* grid, int32_t* __restrict__ start) {
+  const int m = grid->nbins + 1;
+  const int total = scan_bucket_counts<32>(m, [&](int i) { return cnt[i]; }, [&](int i, int v) { start[i] = v; });
+  if (threadIdx.x == 0) {
+    start[m] = total;
+    grid->n_real = start[m - 1];  // everything before the trash bucket
+  }
+}
+
+__global__ void k_bin_scatter(int n, const int32_t* __restrict__ bin_of, const int32_t* __restrict__ slot,
+                              const int32_t* __restrict__ bin_start, int32_t* __restrict__ tmp_list) {
+  int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= n) return;
+  tmp_list[bin_start[bin_of[a]] + slot[a]] = a;
+}
+
+__global__ void k_bin_finalize(const float* __restrict__ coords, const int32_t* __restrict__ species, int n,
+                               const ani_grid* __restrict__ grid, const int32_t* __restrict__ bin_of,
+                               const int32_t* __restrict__ bin_start, const int32_t* __restrict__ tmp_list,
+                               int32_t* __restrict__ sorted_orig, int32_t* __restrict__ orig_to_sorted,
+                               float4* __restrict__ spos, int32_t* __restrict__ sbin) {
+  int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= n) return;
+  const ani_grid g = *grid;
+  int b = bin_of[a];
+  int lo = bin_start[b], hi = bin_start[b + 1];
+  const int spa = species[a];
+  int rank = 0;
+  if (spa < 0) {
+    // trash bucket (padding atoms of a conformer batch, possibly thousands): all of one "species", so the rank is
+    // the number of smaller indices -- independent loads, no dependent species gather per entry
+    for (int e = lo; e < hi; ++e) rank += tmp_list[e] < a;
+  } else {
+    rank = species_index_rank(species, lo, hi, a, spa, [&](int e) { return tmp_list[e]; });
+  }
+  place_atom(g, coords, nullptr, a, spa, b, lo + rank, sorted_orig, orig_to_sorted, sbin, spos);
+}
+
+// Per-bucket table of the 27 neighbouring buckets (neighbour_record, with .w = 0 in this form).  The AEV kernel then
+// reads 27 records instead of redoing the index wrapping and shift arithmetic for every central atom.
+__global__ void k_bucket_ranges(const ani_grid* __restrict__ grid, const int32_t* __restrict__ bin_start,
+                                float4* __restrict__ ranges) {
+  const ani_grid g = *grid;
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  const int b = idx / 27, o = idx % 27;
+  if (b >= g.nbins || g.mode == 1) return;
+  float4 r0, r1;
+  neighbour_record<false>(g, nullptr, b, o, [&](int k) { return bin_start[k]; }, r0, r1);
+  r0.w = 0.f;
+  ranges[2 * (size_t)idx] = r0;
+  ranges[2 * (size_t)idx + 1] = r1;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -412,7 +467,94 @@ __global__ void k_bucket_ranges(const ani_grid* __restrict__ grid, const int32_t
 //      emit the tile table
 //   3. per-chunk: assign rows (ballot ranks inside the chunk)
 // ---------------------------------------------------------------------------------------
-constexpr int LAYOUT_CHUNK = 256;
+
+// Exclusive scan over the chunks of chunk_hist[c][s], per species, in place (the whole block calls it): s_tot[s] =
+// the total of species s.  The histogram is staged through shared memory in slabs so that the serial scan does not
+// pay a global-memory round trip per chunk; load(k) reads chunk_hist[k].
+template <class Load>
+__device__ __forceinline__ void scan_chunk_hist(int n_chunks, int S, int32_t* __restrict__ chunk_hist, Load load,
+                                                int* s_tot) {
+  __shared__ int s_slab[128 * ANI_MAX_SPECIES];
+  const int tid = threadIdx.x;
+  int run = 0;
+  for (int c0 = 0; c0 < n_chunks; c0 += 128) {
+    const int nc = min(128, n_chunks - c0);
+    for (int k = tid; k < nc * ANI_MAX_SPECIES; k += blockDim.x) s_slab[k] = load(c0 * ANI_MAX_SPECIES + k);
+    __syncthreads();
+    if (tid < S) {
+      for (int c = 0; c < nc; ++c) {
+        const int v = s_slab[c * ANI_MAX_SPECIES + tid];
+        s_slab[c * ANI_MAX_SPECIES + tid] = run;
+        run += v;
+      }
+    }
+    __syncthreads();
+    for (int k = tid; k < nc * ANI_MAX_SPECIES; k += blockDim.x) chunk_hist[c0 * ANI_MAX_SPECIES + k] = s_slab[k];
+    __syncthreads();
+  }
+  if (tid < S) s_tot[tid] = run;
+  __syncthreads();
+}
+
+// From the species totals s_tot: the first row s_base[s] of every species, each species block padded to whole row
+// tiles (s_base[S] = all rows), and the tables that are given (the whole block calls it):
+//   species_base[s] = s_base[s];
+//   layout_info = {row tiles, rows, owned atoms, 0, [4 + s] first row tile of species s, [4 + S..] total row tiles};
+//   tile_species[t] = species of row tile t, -1 for tiles of padding rows only and beyond the layout.
+__device__ __forceinline__ void species_rows(int S, int rows_cap, const int* s_tot, int* s_base,
+                                             int32_t* __restrict__ species_base, int32_t* __restrict__ layout_info,
+                                             int32_t* __restrict__ tile_species) {
+  if (threadIdx.x == 0) {
+    int row = 0, owned = 0;
+    for (int s = 0; s < S; ++s) {
+      s_base[s] = row;
+      if (species_base) species_base[s] = row;
+      owned += s_tot[s];
+      row += (s_tot[s] + ANI_TILE_ROWS - 1) / ANI_TILE_ROWS * ANI_TILE_ROWS;
+    }
+    s_base[S] = row;
+    if (layout_info) {
+      layout_info[0] = row / ANI_TILE_ROWS;
+      layout_info[1] = row;
+      layout_info[2] = owned;
+      layout_info[3] = 0;
+      for (int s = 0; s <= ANI_MAX_SPECIES; ++s) layout_info[4 + s] = (s <= S ? s_base[s] : row) / ANI_TILE_ROWS;
+    }
+  }
+  __syncthreads();
+  if (!tile_species) return;
+  const int n_tiles_cap = rows_cap / ANI_TILE_ROWS;
+  for (int t = threadIdx.x; t < n_tiles_cap; t += blockDim.x) {
+    const int r = t * ANI_TILE_ROWS;
+    int sp = -1;
+    for (int s = 0; s < S; ++s)
+      if (r >= s_base[s] && r < s_base[s + 1] && r < s_base[s] + s_tot[s]) sp = s;
+    tile_species[t] = sp;
+  }
+}
+
+// Rows of one 256-atom chunk of the owned sorted slice, whose thread k holds sorted atom i of species sp (-1: none):
+// row0(sp) is the first row of the chunk's atoms of species sp, ballots rank the atoms of a species inside the chunk.
+// The whole block calls it, with one or more chunks of 8 warps each; s_wcnt holds one row per warp of the block.
+template <class Row0>
+__device__ __forceinline__ void assign_chunk_rows(int i, int sp, int S, int (*s_wcnt)[ANI_MAX_SPECIES], Row0 row0,
+                                                  int32_t* __restrict__ row_of, int32_t* __restrict__ row_atom) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int my_rank = 0;
+  for (int s = 0; s < S; ++s) {
+    const unsigned m = __ballot_sync(ANI_FULL_MASK, sp == s);
+    if (sp == s) my_rank = __popc(m & ((1u << lane) - 1u));
+    if (lane == 0) s_wcnt[w][s] = __popc(m);
+  }
+  __syncthreads();
+  if (sp >= 0) {
+    int off = 0;
+    for (int ww = w - w % (LAYOUT_CHUNK / 32); ww < w; ++ww) off += s_wcnt[ww][sp];   // from the chunk's first warp
+    const int row = row0(sp) + off + my_rank;
+    row_of[i] = row;
+    row_atom[row] = i;
+  }
+}
 
 __global__ void k_layout_count(const float4* __restrict__ spos, const ani_grid* __restrict__ grid, int lo,
                                int hi, int S, int32_t* __restrict__ chunk_hist) {
@@ -437,54 +579,9 @@ __global__ void k_layout_scan(int n_chunks, int S, int rows_cap, int32_t* __rest
   // chunk_hist[c][s] -> exclusive prefix over chunks (in place); species_base[s] = first row
   __shared__ int s_tot[ANI_MAX_SPECIES];
   __shared__ int s_base[ANI_MAX_SPECIES + 1];
-  const int tid = threadIdx.x;
-  // exclusive scan over chunks, per species; the histogram is staged through shared memory in
-  // slabs so that the serial scan does not pay a global-memory round trip per chunk
-  __shared__ int s_slab[128 * ANI_MAX_SPECIES];
-  int run = 0;
-  for (int c0 = 0; c0 < n_chunks; c0 += 128) {
-    const int nc = min(128, n_chunks - c0);
-    for (int k = tid; k < nc * ANI_MAX_SPECIES; k += blockDim.x) s_slab[k] = chunk_hist[c0 * ANI_MAX_SPECIES + k];
-    __syncthreads();
-    if (tid < S) {
-      for (int c = 0; c < nc; ++c) {
-        const int v = s_slab[c * ANI_MAX_SPECIES + tid];
-        s_slab[c * ANI_MAX_SPECIES + tid] = run;
-        run += v;
-      }
-    }
-    __syncthreads();
-    for (int k = tid; k < nc * ANI_MAX_SPECIES; k += blockDim.x) chunk_hist[c0 * ANI_MAX_SPECIES + k] = s_slab[k];
-    __syncthreads();
-  }
-  if (tid < S) s_tot[tid] = run;
-  __syncthreads();
-  if (tid == 0) {
-    int row = 0, owned = 0;
-    for (int s = 0; s < S; ++s) {
-      s_base[s] = row;
-      species_base[s] = row;
-      owned += s_tot[s];
-      row += (s_tot[s] + ANI_TILE_ROWS - 1) / ANI_TILE_ROWS * ANI_TILE_ROWS;
-    }
-    s_base[S] = row;
-    layout_info[0] = row / ANI_TILE_ROWS;
-    layout_info[1] = row;
-    layout_info[2] = owned;
-    layout_info[3] = 0;
-    // [4 + s] = first row tile of species s, [4 + S] = total row tiles (tile lists of the GEMMs)
-    for (int s = 0; s <= S; ++s) layout_info[4 + s] = s_base[s] / ANI_TILE_ROWS;
-    for (int s = S + 1; s <= ANI_MAX_SPECIES; ++s) layout_info[4 + s] = row / ANI_TILE_ROWS;
-  }
-  __syncthreads();
-  const int n_tiles_cap = rows_cap / ANI_TILE_ROWS;
-  for (int t = tid; t < n_tiles_cap; t += blockDim.x) {
-    int r = t * ANI_TILE_ROWS, sp = -1;
-    for (int s = 0; s < S; ++s)
-      if (r >= s_base[s] && r < s_base[s + 1] && r < s_base[s] + s_tot[s]) sp = s;
-    tile_species[t] = sp;
-  }
-  for (int r = tid; r < rows_cap; r += blockDim.x) row_atom[r] = -1;
+  scan_chunk_hist(n_chunks, S, chunk_hist, [&](int k) { return chunk_hist[k]; }, s_tot);
+  species_rows(S, rows_cap, s_tot, s_base, species_base, layout_info, tile_species);
+  for (int r = threadIdx.x; r < rows_cap; r += blockDim.x) row_atom[r] = -1;
 }
 
 __global__ void k_layout_assign(const float4* __restrict__ spos, const ani_grid* __restrict__ grid, int lo,
@@ -494,23 +591,11 @@ __global__ void k_layout_assign(const float4* __restrict__ spos, const ani_grid*
   __shared__ int s_wcnt[LAYOUT_CHUNK / 32][ANI_MAX_SPECIES];
   const int n_real = grid->n_real;
   hi = min(hi, n_real);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   int i = lo + blockIdx.x * LAYOUT_CHUNK + threadIdx.x;
   int sp = (i < hi) ? __float_as_int(spos[i].w) : -1;
-  int my_rank = 0;
-  for (int s = 0; s < S; ++s) {
-    unsigned m = __ballot_sync(ANI_FULL_MASK, sp == s);
-    if (sp == s) my_rank = __popc(m & ((1u << lane) - 1u));
-    if (lane == 0) s_wcnt[w][s] = __popc(m);
-  }
-  __syncthreads();
-  if (sp >= 0) {
-    int off = 0;
-    for (int ww = 0; ww < w; ++ww) off += s_wcnt[ww][sp];
-    int row = species_base[sp] + chunk_hist[blockIdx.x * ANI_MAX_SPECIES + sp] + off + my_rank;
-    row_of[i] = row;
-    row_atom[row] = i;
-  }
+  assign_chunk_rows(i, sp, S, s_wcnt,
+                    [&](int s) { return species_base[s] + chunk_hist[blockIdx.x * ANI_MAX_SPECIES + s]; }, row_of,
+                    row_atom);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -535,6 +620,36 @@ __device__ __forceinline__ bool aev_column_live(int c, unsigned mask, int S, int
   return ((mask >> s1) & 1u) && ((mask >> (s1 + rem)) & 1u);
 }
 
+// Is any column of 32-column block b live?  One thread walks the block: radial columns one by one, angular columns
+// pair block by pair block.
+__device__ __forceinline__ bool aev_block_live(int b, unsigned mask, int S, int n_shf_r, int angular_sub, int out_dim,
+                                               int pad) {
+  bool active = false;
+  for (int c = b * 32; c < b * 32 + 32 && !active; ++c) active = aev_column_live(c, mask, S, n_shf_r, angular_sub, out_dim, pad);
+  return active;
+}
+
+// One warp (the whole warp calls it) compacts the live blocks among the nblk blocks (live(b)) into blocks[1 ..], their
+// count into blocks[0], and behind the list the element-presence mask and a "changed since the previous call" flag,
+// read by the AEV kernel: dead element pairs are skipped, but zero-filled once whenever the composition changes.
+template <class Live>
+__device__ __forceinline__ void compact_live_blocks(int nblk, unsigned mask, int32_t* __restrict__ blocks, Live live) {
+  const int lane = threadIdx.x & 31;
+  int count = 0;
+  for (int b0 = 0; b0 < nblk; b0 += 32) {
+    const int b = b0 + lane;
+    const bool active = b < nblk && live(b);
+    const unsigned m = __ballot_sync(ANI_FULL_MASK, active);
+    if (active) blocks[1 + count + __popc(m & ((1u << lane) - 1u))] = b;
+    count += __popc(m);
+  }
+  if (lane == 0) {
+    blocks[0] = count;
+    blocks[nblk + 2] = (blocks[nblk + 1] != (int)mask);
+    blocks[nblk + 1] = (int)mask;
+  }
+}
+
 __global__ void k_species_present(const float4* __restrict__ spos, const ani_grid* __restrict__ grid, int n,
                                   int32_t* __restrict__ present) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -549,28 +664,8 @@ __global__ void k_active_blocks(const int32_t* __restrict__ present, int S, int 
                                 int out_dim, int ldx, int ang_pad, int32_t* __restrict__ blocks) {
   // one warp; lane b tests the 32 columns of block b (32 blocks per round), a ballot compacts
   const unsigned mask = (unsigned)*present;
-  const int RL = S * n_shf_r;
-  const int lane = threadIdx.x;
-  int count = 0;
-  for (int b0 = 0; b0 < ldx / 32; b0 += 32) {
-    const int b = b0 + lane;
-    bool active = false;
-    if (b < ldx / 32) {
-      // radial columns one by one, angular columns pair block by pair block
-      for (int c = b * 32; c < b * 32 + 32 && !active; ++c)
-        active = aev_column_live(c, mask, S, n_shf_r, angular_sub, out_dim, ang_pad);
-    }
-    const unsigned live = __ballot_sync(ANI_FULL_MASK, active);
-    if (active) blocks[1 + count + __popc(live & ((1u << lane) - 1u))] = b;
-    count += __popc(live);
-  }
-  if (lane == 0) {
-    blocks[0] = count;
-    // element-presence bits + "changed since the previous call" flag, read by the AEV kernel: dead
-    // element pairs are skipped, but zero-filled once whenever the composition changes
-    blocks[ldx / 32 + 2] = (blocks[ldx / 32 + 1] != (int)mask);
-    blocks[ldx / 32 + 1] = (int)mask;
-  }
+  compact_live_blocks(ldx / 32, mask, blocks,
+                      [&](int b) { return aev_block_live(b, mask, S, n_shf_r, angular_sub, out_dim, ang_pad); });
 }
 
 
@@ -643,8 +738,6 @@ template <bool LAT = false>
 __global__ void __launch_bounds__(256) k_prep_assign(const __grid_constant__ PrepArgs A) {
   __shared__ ani_grid sg;
   __shared__ bool s_last;
-  __shared__ int s_warp[8];
-  __shared__ int s_carry;
   const int tid = threadIdx.x;
   if (tid == 0) {
     if (A.inline_setup) {
@@ -657,17 +750,7 @@ __global__ void __launch_bounds__(256) k_prep_assign(const __grid_constant__ Pre
   }
   __syncthreads();
   const int a = blockIdx.x * blockDim.x + tid;
-  if (a < A.n) {
-    int bin;
-    if (A.species[a] < 0) {
-      bin = sg.nbins;  // padding atoms: trash bucket, never a neighbour, never a centre
-    } else {
-      float3 p;
-      wrapped_position<LAT>(sg, A.coords, a, p, bin, A.lattice);
-    }
-    A.bin_of[a] = bin;
-    A.slot[a] = atomicAdd(&A.bin_count[bin], 1);
-  }
+  if (a < A.n) assign_bucket<LAT>(sg, A.coords, A.species, a, A.bin_of, A.slot, A.bin_count, A.lattice);
   // the last block to get here scans the bucket counts (exclusive) -> bin_start
   __threadfence();
   __syncthreads();
@@ -676,39 +759,11 @@ __global__ void __launch_bounds__(256) k_prep_assign(const __grid_constant__ Pre
   if (!s_last) return;
   __threadfence();
   const int m = sg.nbins + 1;
-  const int lane = tid & 31, w = tid >> 5;
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
-  for (int base = 0; base < m; base += blockDim.x) {
-    const int i = base + tid;
-    const int v = (i < m) ? __ldcg(&A.bin_count[i]) : 0;
-    int x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(ANI_FULL_MASK, x, o);
-      if (lane >= o) x += y;
-    }
-    if (lane == 31) s_warp[w] = x;
-    __syncthreads();
-    if (w == 0) {
-      int t = (lane < 8) ? s_warp[lane] : 0;
-#pragma unroll
-      for (int o = 1; o < 8; o <<= 1) {
-        const int y = __shfl_up_sync(ANI_FULL_MASK, t, o);
-        if (lane >= o) t += y;
-      }
-      if (lane < 8) s_warp[lane] = t;  // inclusive over warps
-    }
-    __syncthreads();
-    const int incl = x + ((w == 0) ? 0 : s_warp[w - 1]) + s_carry;
-    if (i < m) A.bin_start[i] = incl - v;
-    __syncthreads();
-    if (tid == blockDim.x - 1) s_carry = incl;
-    __syncthreads();
-  }
+  const int total = scan_bucket_counts<8>(m, [&](int i) { return __ldcg(&A.bin_count[i]); },
+                                          [&](int i, int v) { A.bin_start[i] = v; });
   if (tid == 0) {
-    A.bin_start[m] = s_carry;
-    A.grid->n_real = s_carry - __ldcg(&A.bin_count[m - 1]);  // everything before the trash bucket
+    A.bin_start[m] = total;
+    A.grid->n_real = total - __ldcg(&A.bin_count[m - 1]);  // everything before the trash bucket
   }
 }
 
@@ -721,75 +776,31 @@ __global__ void __launch_bounds__(256) k_prep_scatter(const __grid_constant__ Pr
   const ani_grid g = *A.grid;
   const int b = idx / 27, o = idx % 27;
   if (b >= g.nbins || g.mode == 1) return;
-  int ix, iy, iz;
-  const int base = bucket_coords(g, b, ix, iy, iz);
-  int j[3] = {ix + o / 9 - 1, iy + (o / 3) % 3 - 1, iz + o % 3 - 1};
-  int w[3];
-  for (int d = 0; d < 3; ++d) {
-    w[d] = 0;
-    if (j[d] < 0) {
-      w[d] = -1;
-      j[d] += g.dims[d];
-    } else if (j[d] >= g.dims[d]) {
-      w[d] = 1;
-      j[d] -= g.dims[d];
-    }
-  }
-  const bool exists = g.pbc || !(w[0] | w[1] | w[2]);
-  int lo = 0, hi = 0;
-  const int code = (w[0] + 1) * 9 + (w[1] + 1) * 3 + (w[2] + 1);
-  if (exists) {
-    const int nb = base + (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2];
-    lo = A.bin_start[nb];
-    hi = A.bin_start[nb + 1];
-  }
-  const float wx = (float)w[0], wy = (float)w[1], wz = (float)w[2];
-  const int nbk = exists ? base + (j[0] * g.dims[1] + j[1]) * g.dims[2] + j[2] : 0;
-  float cl[9];   // the image shift in the lattice of the bucket's conformer
-  cell_of<LAT>(g, A.lattice, LAT ? base / (g.dims[0] * g.dims[1] * g.dims[2]) : 0, cl);
-  A.ranges[2 * (size_t)idx] = make_float4(__int_as_float(lo), __int_as_float(hi), __int_as_float(code), __int_as_float(nbk));
-  A.ranges[2 * (size_t)idx + 1] = make_float4(wx * cl[0] + wy * cl[3] + wz * cl[6],
-                                              wx * cl[1] + wy * cl[4] + wz * cl[7],
-                                              wx * cl[2] + wy * cl[5] + wz * cl[8], 0.f);
+  neighbour_record<LAT>(g, A.lattice, b, o, [&](int k) { return A.bin_start[k]; }, A.ranges[2 * (size_t)idx],
+                        A.ranges[2 * (size_t)idx + 1]);
 }
 
 template <bool LAT = false>
 __global__ void __launch_bounds__(256) k_prep_finalize(const __grid_constant__ PrepArgs A) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   const ani_grid g = *A.grid;
-  int sp = -1, i = -1;
+  int sp = -1;
   if (a < A.n) {
     const int b = A.bin_of[a];
     const int lo = A.bin_start[b], hi = A.bin_start[b + 1];
-    // rank by (species, input index): deterministic order, every bucket species-sorted
     const int spa = A.species[a];
-    int rank = 0;
+    int rank;
     if (spa < 0) {
       // padding atoms (trash bucket) are never neighbours nor centres: any order will do -- their arrival slot,
       // instead of ranking thousands of padded entries of a conformer batch against each other
       rank = A.slot[a];
     } else {
-      for (int e = lo; e < hi; ++e) {
-        const int t = A.tmp_list[e];
-        const int spt = A.species[t];
-        rank += (spt < spa) || (spt == spa && t < a);
-      }
+      rank = species_index_rank(A.species, lo, hi, a, spa, [&](int e) { return A.tmp_list[e]; });
     }
-    i = lo + rank;
-    A.sorted_orig[i] = a;
-    A.orig_to_sorted[a] = i;
-    A.sbin[i] = b;
-    float3 p = make_float3(0.f, 0.f, 0.f);
-    sp = A.species[a];
-    if (sp >= 0) {
-      int bb;
-      wrapped_position<LAT>(g, A.coords, a, p, bb, A.lattice);
-    }
-    A.spos[i] = make_float4(p.x, p.y, p.z, __int_as_float(sp));
-    // species histogram of the owned slice, per 256-atom chunk of the SORTED order
-    const int hi_real = min(A.hi, g.n_real);
-    if (sp >= 0 && i >= A.lo && i < hi_real)
-      atomicAdd(&A.chunk_hist[((i - A.lo) / LAYOUT_CHUNK) * ANI_MAX_SPECIES + sp], 1);
+    sp = A.species[a];   // read again: reusing spa here makes ptxas spill the grid fields around the rank loop
+    // with the species histogram of the owned slice, per 256-atom chunk of the SORTED order
+    place_atom<LAT>(g, A.coords, A.lattice, a, sp, b, lo + rank, A.sorted_orig, A.orig_to_sorted, A.sbin, A.spos,
+                    A.chunk_hist, A.lo, min(A.hi, g.n_real));
   }
   unsigned mask = 0;
   for (int s = 0; s < ANI_MAX_SPECIES; ++s)
@@ -804,75 +815,17 @@ __global__ void __launch_bounds__(256) k_prep_finalize(const __grid_constant__ P
 __global__ void __launch_bounds__(1024) k_prep_layout(const __grid_constant__ PrepArgs A) {
   __shared__ int s_tot[ANI_MAX_SPECIES];
   __shared__ int s_base[ANI_MAX_SPECIES + 1];
-  __shared__ int s_slab[128 * ANI_MAX_SPECIES];
   const int tid = threadIdx.x, S = A.S;
   // ---- live AEV column blocks (warp 31; independent of the scan below)
   if (tid >= 992) {
     const unsigned mask = (unsigned)*A.present;
-    const int RL = S * A.n_shf_r;
-    const int lane = tid & 31;
-    int count = 0;
-    for (int b0 = 0; b0 < A.ldx / 32; b0 += 32) {
-      const int b = b0 + lane;
-      bool active = false;
-      if (b < A.ldx / 32) {
-        for (int c = b * 32; c < b * 32 + 32 && !active; ++c)
-          active = aev_column_live(c, mask, S, A.n_shf_r, A.angular_sub, A.out_dim, A.ang_pad);
-      }
-      const unsigned live = __ballot_sync(ANI_FULL_MASK, active);
-      if (active) A.blocks[1 + count + __popc(live & ((1u << lane) - 1u))] = b;
-      count += __popc(live);
-    }
-    if (lane == 0) {
-      A.blocks[0] = count;
-      A.blocks[A.ldx / 32 + 2] = (A.blocks[A.ldx / 32 + 1] != (int)mask);
-      A.blocks[A.ldx / 32 + 1] = (int)mask;
-    }
+    compact_live_blocks(A.ldx / 32, mask, A.blocks, [&](int b) {
+      return aev_block_live(b, mask, S, A.n_shf_r, A.angular_sub, A.out_dim, A.ang_pad);
+    });
   }
-  // ---- exclusive scan of the chunk histograms per species (in place)
-  int run = 0;
-  for (int c0 = 0; c0 < A.n_chunks; c0 += 128) {
-    const int nc = min(128, A.n_chunks - c0);
-    for (int k = tid; k < nc * ANI_MAX_SPECIES; k += blockDim.x) s_slab[k] = A.chunk_hist[c0 * ANI_MAX_SPECIES + k];
-    __syncthreads();
-    if (tid < S) {
-      for (int c = 0; c < nc; ++c) {
-        const int v = s_slab[c * ANI_MAX_SPECIES + tid];
-        s_slab[c * ANI_MAX_SPECIES + tid] = run;
-        run += v;
-      }
-    }
-    __syncthreads();
-    for (int k = tid; k < nc * ANI_MAX_SPECIES; k += blockDim.x) A.chunk_hist[c0 * ANI_MAX_SPECIES + k] = s_slab[k];
-    __syncthreads();
-  }
-  if (tid < S) s_tot[tid] = run;
-  __syncthreads();
-  if (tid == 0) {
-    int row = 0, owned = 0;
-    for (int s = 0; s < S; ++s) {
-      s_base[s] = row;
-      A.species_base[s] = row;
-      owned += s_tot[s];
-      row += (s_tot[s] + ANI_TILE_ROWS - 1) / ANI_TILE_ROWS * ANI_TILE_ROWS;
-    }
-    s_base[S] = row;
-    A.layout_info[0] = row / ANI_TILE_ROWS;
-    A.layout_info[1] = row;
-    A.layout_info[2] = owned;
-    A.layout_info[3] = 0;
-    for (int s = 0; s <= S; ++s) A.layout_info[4 + s] = s_base[s] / ANI_TILE_ROWS;
-    for (int s = S + 1; s <= ANI_MAX_SPECIES; ++s) A.layout_info[4 + s] = row / ANI_TILE_ROWS;
-  }
-  __syncthreads();
-  const int n_tiles_cap = A.rows_cap / ANI_TILE_ROWS;
-  for (int t = tid; t < n_tiles_cap; t += blockDim.x) {
-    const int r = t * ANI_TILE_ROWS;
-    int sp = -1;
-    for (int s = 0; s < S; ++s)
-      if (r >= s_base[s] && r < s_base[s + 1] && r < s_base[s] + s_tot[s]) sp = s;
-    A.tile_species[t] = sp;
-  }
+  // ---- exclusive scan of the chunk histograms per species (in place), row bases, tile table
+  scan_chunk_hist(A.n_chunks, S, A.chunk_hist, [&](int k) { return A.chunk_hist[k]; }, s_tot);
+  species_rows(S, A.rows_cap, s_tot, s_base, A.species_base, A.layout_info, A.tile_species);
   for (int r = tid; r < A.rows_cap; r += blockDim.x) A.row_atom[r] = -1;
   if (A.zero_f64)
     for (int k = tid; k < A.zero_f64_count; k += blockDim.x) A.zero_f64[k] = 0.0;
@@ -915,11 +868,8 @@ __device__ __forceinline__ void grid_barrier(int32_t* bar, int32_t* status) {
 template <bool LAT = false>
 __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ PrepArgs A, int32_t* bar, int zeroed) {
   __shared__ ani_grid sg;
-  __shared__ int s_warp[8];
-  __shared__ int s_carry;
   __shared__ int s_tot[ANI_MAX_SPECIES];
   __shared__ int s_base[ANI_MAX_SPECIES + 1];
-  __shared__ int s_slab[128 * ANI_MAX_SPECIES];
   __shared__ int s_wcnt[LAYOUT_CHUNK / 32][ANI_MAX_SPECIES];
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int gstride = gridDim.x * blockDim.x, gtid = blockIdx.x * blockDim.x + tid;
@@ -947,96 +897,31 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
     __syncthreads();
   }
   // ---- phase 1: bucket of every atom, slot inside the bucket by atomics
-  for (int a = gtid; a < n; a += gstride) {
-    int bin;
-    if (A.species[a] < 0) {
-      bin = sg.nbins;  // padding atoms: trash bucket, never a neighbour, never a centre
-    } else {
-      float3 p;
-      wrapped_position<LAT>(sg, A.coords, a, p, bin, A.lattice);
-    }
-    A.bin_of[a] = bin;
-    A.slot[a] = atomicAdd(&A.bin_count[bin], 1);
-  }
+  for (int a = gtid; a < n; a += gstride)
+    assign_bucket<LAT>(sg, A.coords, A.species, a, A.bin_of, A.slot, A.bin_count, A.lattice);
   grid_barrier(bar, A.status);
   // ---- phase 1b: block 0 scans the bucket counts (exclusive) -> bin_start, n_real
   if (blockIdx.x == 0) {
     const int m = sg.nbins + 1;
-    if (tid == 0) s_carry = 0;
-    __syncthreads();
-    for (int base = 0; base < m; base += blockDim.x) {
-      const int i = base + tid;
-      const int v = (i < m) ? __ldcg(&A.bin_count[i]) : 0;
-      int x = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(ANI_FULL_MASK, x, o);
-        if (lane >= o) x += y;
-      }
-      if (lane == 31) s_warp[w] = x;
-      __syncthreads();
-      if (w == 0) {
-        int t = (lane < 8) ? s_warp[lane] : 0;
-#pragma unroll
-        for (int o = 1; o < 8; o <<= 1) {
-          const int y = __shfl_up_sync(ANI_FULL_MASK, t, o);
-          if (lane >= o) t += y;
-        }
-        if (lane < 8) s_warp[lane] = t;
-      }
-      __syncthreads();
-      const int incl = x + ((w == 0) ? 0 : s_warp[w - 1]) + s_carry;
-      if (i < m) A.bin_start[i] = incl - v;
-      __syncthreads();
-      if (tid == blockDim.x - 1) s_carry = incl;
-      __syncthreads();
-    }
+    const int total = scan_bucket_counts<8>(m, [&](int i) { return __ldcg(&A.bin_count[i]); },
+                                            [&](int i, int v) { A.bin_start[i] = v; });
     if (tid == 0) {
-      A.bin_start[m] = s_carry;
-      A.grid->n_real = s_carry - __ldcg(&A.bin_count[m - 1]);  // everything before the trash bucket
+      A.bin_start[m] = total;
+      A.grid->n_real = total - __ldcg(&A.bin_count[m - 1]);  // everything before the trash bucket
     }
   }
   grid_barrier(bar, A.status);
   const int n_real = __ldcg(&A.grid->n_real);
+  auto start = [&](int k) { return __ldcg(&A.bin_start[k]); };
   // ---- phase 2: scatter into buckets + per-bucket table of the 27 neighbouring buckets
   {
     const long long t2 = A.ranges ? max((long long)n, (long long)sg.nbins * 27) : (long long)n;
     for (long long idx = gtid; idx < t2; idx += gstride) {
-      if (idx < n) A.tmp_list[__ldcg(&A.bin_start[A.bin_of[idx]]) + A.slot[idx]] = (int)idx;
+      if (idx < n) A.tmp_list[start(A.bin_of[idx]) + A.slot[idx]] = (int)idx;
       if (!A.ranges || sg.mode == 1) continue;
       const int b = (int)(idx / 27), o = (int)(idx % 27);
       if (b >= sg.nbins) continue;
-      int ix, iy, iz;
-      const int base = bucket_coords(sg, b, ix, iy, iz);
-      int j[3] = {ix + o / 9 - 1, iy + (o / 3) % 3 - 1, iz + o % 3 - 1};
-      int wv[3];
-      for (int d = 0; d < 3; ++d) {
-        wv[d] = 0;
-        if (j[d] < 0) {
-          wv[d] = -1;
-          j[d] += sg.dims[d];
-        } else if (j[d] >= sg.dims[d]) {
-          wv[d] = 1;
-          j[d] -= sg.dims[d];
-        }
-      }
-      const bool exists = sg.pbc || !(wv[0] | wv[1] | wv[2]);
-      int lo = 0, hi = 0;
-      const int code = (wv[0] + 1) * 9 + (wv[1] + 1) * 3 + (wv[2] + 1);
-      if (exists) {
-        const int nb = base + (j[0] * sg.dims[1] + j[1]) * sg.dims[2] + j[2];
-        lo = __ldcg(&A.bin_start[nb]);
-        hi = __ldcg(&A.bin_start[nb + 1]);
-      }
-      const float wx = (float)wv[0], wy = (float)wv[1], wz = (float)wv[2];
-      const int nbk = exists ? base + (j[0] * sg.dims[1] + j[1]) * sg.dims[2] + j[2] : 0;
-      float cl[9];   // the image shift in the lattice of the bucket's conformer
-      cell_of<LAT>(sg, A.lattice, LAT ? base / (sg.dims[0] * sg.dims[1] * sg.dims[2]) : 0, cl);
-      A.ranges[2 * (size_t)idx] =
-          make_float4(__int_as_float(lo), __int_as_float(hi), __int_as_float(code), __int_as_float(nbk));
-      A.ranges[2 * (size_t)idx + 1] = make_float4(wx * cl[0] + wy * cl[3] + wz * cl[6],
-                                                  wx * cl[1] + wy * cl[4] + wz * cl[7],
-                                                  wx * cl[2] + wy * cl[5] + wz * cl[8], 0.f);
+      neighbour_record<LAT>(sg, A.lattice, b, o, start, A.ranges[2 * (size_t)idx], A.ranges[2 * (size_t)idx + 1]);
     }
   }
   grid_barrier(bar, A.status);
@@ -1050,31 +935,13 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
       int sp = -1;
       if (a < n) {
         const int b = A.bin_of[a];
-        const int lo = __ldcg(&A.bin_start[b]), hi = __ldcg(&A.bin_start[b + 1]);
-        const int spa = A.species[a];
-        int rank = 0;
-        if (spa < 0) {
-          rank = A.slot[a];   // padding atoms: arrival order (see k_prep_finalize)
-        } else {
-          for (int e = lo; e < hi; ++e) {
-            const int t = __ldcg(&A.tmp_list[e]);
-            const int spt = A.species[t];
-            rank += (spt < spa) || (spt == spa && t < a);
-          }
-        }
-        const int i = lo + rank;
-        A.sorted_orig[i] = a;
-        A.orig_to_sorted[a] = i;
-        A.sbin[i] = b;
-        float3 p = make_float3(0.f, 0.f, 0.f);
-        sp = spa;
-        if (sp >= 0) {
-          int bb;
-          wrapped_position<LAT>(sg, A.coords, a, p, bb, A.lattice);
-        }
-        A.spos[i] = make_float4(p.x, p.y, p.z, __int_as_float(sp));
-        if (sp >= 0 && i >= A.lo && i < hi_real)
-          atomicAdd(&A.chunk_hist[((i - A.lo) / LAYOUT_CHUNK) * ANI_MAX_SPECIES + sp], 1);
+        const int lo = start(b), hi = start(b + 1);
+        sp = A.species[a];
+        const int rank = sp < 0 ? A.slot[a]   // padding atoms: arrival order (see k_prep_finalize)
+                                : species_index_rank(A.species, lo, hi, a, sp,
+                                                     [&](int e) { return __ldcg(&A.tmp_list[e]); });
+        place_atom<LAT>(sg, A.coords, A.lattice, a, sp, b, lo + rank, A.sorted_orig, A.orig_to_sorted, A.sbin, A.spos,
+                        A.chunk_hist, A.lo, hi_real);
       }
       for (int s = 0; s < ANI_MAX_SPECIES; ++s)
         if (__any_sync(ANI_FULL_MASK, sp == s)) mask |= 1u << s;
@@ -1092,68 +959,12 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
   if (blockIdx.x == 0) {
     if (w == 7) {
       const unsigned mask = (unsigned)__ldcg(A.present);
-      const int RL = S * A.n_shf_r;
-      int count = 0;
-      for (int b0 = 0; b0 < A.ldx / 32; b0 += 32) {
-        const int b = b0 + lane;
-        bool active = false;
-        if (b < A.ldx / 32) {
-          for (int c = b * 32; c < b * 32 + 32 && !active; ++c)
-            active = aev_column_live(c, mask, S, A.n_shf_r, A.angular_sub, A.out_dim, A.ang_pad);
-        }
-        const unsigned live = __ballot_sync(ANI_FULL_MASK, active);
-        if (active) A.blocks[1 + count + __popc(live & ((1u << lane) - 1u))] = b;
-        count += __popc(live);
-      }
-      if (lane == 0) {
-        A.blocks[0] = count;
-        A.blocks[A.ldx / 32 + 2] = (A.blocks[A.ldx / 32 + 1] != (int)mask);
-        A.blocks[A.ldx / 32 + 1] = (int)mask;
-      }
+      compact_live_blocks(A.ldx / 32, mask, A.blocks, [&](int b) {
+        return aev_block_live(b, mask, S, A.n_shf_r, A.angular_sub, A.out_dim, A.ang_pad);
+      });
     }
-    int run = 0;
-    for (int c0 = 0; c0 < A.n_chunks; c0 += 128) {
-      const int nc = min(128, A.n_chunks - c0);
-      for (int k = tid; k < nc * ANI_MAX_SPECIES; k += blockDim.x) s_slab[k] = __ldcg(&A.chunk_hist[c0 * ANI_MAX_SPECIES + k]);
-      __syncthreads();
-      if (tid < S) {
-        for (int c = 0; c < nc; ++c) {
-          const int v = s_slab[c * ANI_MAX_SPECIES + tid];
-          s_slab[c * ANI_MAX_SPECIES + tid] = run;
-          run += v;
-        }
-      }
-      __syncthreads();
-      for (int k = tid; k < nc * ANI_MAX_SPECIES; k += blockDim.x) A.chunk_hist[c0 * ANI_MAX_SPECIES + k] = s_slab[k];
-      __syncthreads();
-    }
-    if (tid < S) s_tot[tid] = run;
-    __syncthreads();
-    if (tid == 0) {
-      int row = 0, owned = 0;
-      for (int s = 0; s < S; ++s) {
-        s_base[s] = row;
-        A.species_base[s] = row;
-        owned += s_tot[s];
-        row += (s_tot[s] + ANI_TILE_ROWS - 1) / ANI_TILE_ROWS * ANI_TILE_ROWS;
-      }
-      s_base[S] = row;
-      A.layout_info[0] = row / ANI_TILE_ROWS;
-      A.layout_info[1] = row;
-      A.layout_info[2] = owned;
-      A.layout_info[3] = 0;
-      for (int s = 0; s <= S; ++s) A.layout_info[4 + s] = s_base[s] / ANI_TILE_ROWS;
-      for (int s = S + 1; s <= ANI_MAX_SPECIES; ++s) A.layout_info[4 + s] = row / ANI_TILE_ROWS;
-    }
-    __syncthreads();
-    const int n_tiles_cap = A.rows_cap / ANI_TILE_ROWS;
-    for (int t = tid; t < n_tiles_cap; t += blockDim.x) {
-      const int r = t * ANI_TILE_ROWS;
-      int sp = -1;
-      for (int s = 0; s < S; ++s)
-        if (r >= s_base[s] && r < s_base[s + 1] && r < s_base[s] + s_tot[s]) sp = s;
-      A.tile_species[t] = sp;
-    }
+    scan_chunk_hist(A.n_chunks, S, A.chunk_hist, [&](int k) { return __ldcg(&A.chunk_hist[k]); }, s_tot);
+    species_rows(S, A.rows_cap, s_tot, s_base, A.species_base, A.layout_info, A.tile_species);
     if (A.zero_f64)
       for (int k = tid; k < A.zero_f64_count; k += blockDim.x) A.zero_f64[k] = 0.0;
   }
@@ -1164,20 +975,9 @@ __global__ void __launch_bounds__(256) k_prep_fused(const __grid_constant__ Prep
     for (int c = blockIdx.x; c < A.n_chunks; c += gridDim.x) {
       const int i = A.lo + c * LAYOUT_CHUNK + tid;
       const int sp = (i < hi_real) ? __float_as_int(__ldcg(&A.spos[i]).w) : -1;
-      int my_rank = 0;
-      for (int s = 0; s < S; ++s) {
-        const unsigned m = __ballot_sync(ANI_FULL_MASK, sp == s);
-        if (sp == s) my_rank = __popc(m & ((1u << lane) - 1u));
-        if (lane == 0) s_wcnt[w][s] = __popc(m);
-      }
-      __syncthreads();
-      if (sp >= 0) {
-        int off = 0;
-        for (int ww = 0; ww < w; ++ww) off += s_wcnt[ww][sp];
-        const int row = __ldcg(&A.species_base[sp]) + __ldcg(&A.chunk_hist[c * ANI_MAX_SPECIES + sp]) + off + my_rank;
-        A.row_of[i] = row;
-        A.row_atom[row] = i;
-      }
+      assign_chunk_rows(i, sp, S, s_wcnt, [&](int s) {
+        return __ldcg(&A.species_base[s]) + __ldcg(&A.chunk_hist[c * ANI_MAX_SPECIES + s]);
+      }, A.row_of, A.row_atom);
       __syncthreads();
     }
   }
@@ -1218,8 +1018,6 @@ __global__ void __launch_bounds__(PREP_CLUSTER_THREADS, 1)
   extern __shared__ int s_start[];   // [nbins + 2]: this CTA's copy of bin_start
   __shared__ ani_grid sg;
   __shared__ int s_live[MAX_AEV_BLOCKS];
-  __shared__ int s_warp[32];
-  __shared__ int s_carry;
   __shared__ int s_hist[PREP_CLUSTER_MAX_CHUNKS * ANI_MAX_SPECIES];   // exclusive scan over the chunks, per species
   __shared__ int s_tot[ANI_MAX_SPECIES];
   __shared__ int s_base[ANI_MAX_SPECIES + 1];
@@ -1254,17 +1052,7 @@ __global__ void __launch_bounds__(PREP_CLUSTER_THREADS, 1)
   prep_cluster_barrier();
   stamp(2);
   // ---- phase 1: bucket of every atom, slot inside the bucket by atomics
-  for (int a = gtid; a < n; a += gstride) {
-    int bin;
-    if (A.species[a] < 0) {
-      bin = nbins;  // padding atoms: trash bucket, never a neighbour, never a centre
-    } else {
-      float3 p;
-      wrapped_position(sg, A.coords, a, p, bin);
-    }
-    A.bin_of[a] = bin;
-    A.slot[a] = atomicAdd(&A.bin_count[bin], 1);
-  }
+  for (int a = gtid; a < n; a += gstride) assign_bucket(sg, A.coords, A.species, a, A.bin_of, A.slot, A.bin_count);
   // (independent of everything else, in the shadow of the atomics' round trip) the force accumulator, the row table and
   // the conformer energies start from zero / -1; the row table is written again two cluster barriers further down
   if (A.zero_f32)
@@ -1278,42 +1066,15 @@ __global__ void __launch_bounds__(PREP_CLUSTER_THREADS, 1)
   // ---- phase 1b: EVERY CTA scans the bucket counts (exclusive) into its shared-memory bin_start
   {
     const int m = nbins + 1;
-    if (tid == 0) s_carry = 0;
-    __syncthreads();
-    for (int base = 0; base < m; base += PREP_CLUSTER_THREADS) {
-      const int i = base + tid;
-      const int v = (i < m) ? __ldcg(&A.bin_count[i]) : 0;
-      int x = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(ANI_FULL_MASK, x, o);
-        if (lane >= o) x += y;
-      }
-      if (lane == 31) s_warp[w] = x;
-      __syncthreads();
-      if (w == 0) {
-        int t = s_warp[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const int y = __shfl_up_sync(ANI_FULL_MASK, t, o);
-          if (lane >= o) t += y;
-        }
-        s_warp[lane] = t;  // inclusive over warps
-      }
-      __syncthreads();
-      const int incl = x + ((w == 0) ? 0 : s_warp[w - 1]) + s_carry;
-      if (i < m) {
-        s_start[i] = incl - v;
-        if (blockIdx.x == 0) A.bin_start[i] = incl - v;
-      }
-      __syncthreads();
-      if (tid == PREP_CLUSTER_THREADS - 1) s_carry = incl;
-      __syncthreads();
-    }
+    const int total = scan_bucket_counts<PREP_CLUSTER_THREADS / 32>(m, [&](int i) { return __ldcg(&A.bin_count[i]); },
+                                                                    [&](int i, int v) {
+                                                                      s_start[i] = v;
+                                                                      if (blockIdx.x == 0) A.bin_start[i] = v;
+                                                                    });
     if (tid == 0) {
-      s_start[m] = s_carry;
+      s_start[m] = total;
       if (blockIdx.x == 0) {
-        A.bin_start[m] = s_carry;
+        A.bin_start[m] = total;
         A.grid->n_real = s_start[nbins];  // everything before the trash bucket
       }
     }
@@ -1329,33 +1090,8 @@ __global__ void __launch_bounds__(PREP_CLUSTER_THREADS, 1)
       if (!A.ranges || sg.mode != 0) continue;
       const int b = idx / 27, o = idx % 27;
       if (b >= nbins) continue;
-      const int iz = b % sg.dims[2], iy = (b / sg.dims[2]) % sg.dims[1], ix = b / (sg.dims[2] * sg.dims[1]);
-      int j[3] = {ix + o / 9 - 1, iy + (o / 3) % 3 - 1, iz + o % 3 - 1};
-      int wv[3];
-      for (int d = 0; d < 3; ++d) {
-        wv[d] = 0;
-        if (j[d] < 0) {
-          wv[d] = -1;
-          j[d] += sg.dims[d];
-        } else if (j[d] >= sg.dims[d]) {
-          wv[d] = 1;
-          j[d] -= sg.dims[d];
-        }
-      }
-      const bool exists = sg.pbc || !(wv[0] | wv[1] | wv[2]);
-      int lo = 0, hi = 0;
-      const int code = (wv[0] + 1) * 9 + (wv[1] + 1) * 3 + (wv[2] + 1);
-      const int nbk = exists ? (j[0] * sg.dims[1] + j[1]) * sg.dims[2] + j[2] : 0;
-      if (exists) {
-        lo = s_start[nbk];
-        hi = s_start[nbk + 1];
-      }
-      const float wx = (float)wv[0], wy = (float)wv[1], wz = (float)wv[2];
-      A.ranges[2 * (size_t)idx] =
-          make_float4(__int_as_float(lo), __int_as_float(hi), __int_as_float(code), __int_as_float(nbk));
-      A.ranges[2 * (size_t)idx + 1] = make_float4(wx * sg.cell[0] + wy * sg.cell[3] + wz * sg.cell[6],
-                                                  wx * sg.cell[1] + wy * sg.cell[4] + wz * sg.cell[7],
-                                                  wx * sg.cell[2] + wy * sg.cell[5] + wz * sg.cell[8], 0.f);
+      neighbour_record<false>(sg, nullptr, b, o, [&](int k) { return s_start[k]; }, A.ranges[2 * (size_t)idx],
+                              A.ranges[2 * (size_t)idx + 1]);
     }
   }
   stamp(6);
@@ -1408,20 +1144,9 @@ __global__ void __launch_bounds__(PREP_CLUSTER_THREADS, 1)
 #pragma unroll
         for (int k = 0; k < ANI_MAX_SPECIES; ++k)
           if (__any_sync(ANI_FULL_MASK, valid && spa == k)) present |= 1u << k;
-        if (valid) {
-          const int i = lo + rank;
-          A.sorted_orig[i] = a;
-          A.orig_to_sorted[a] = i;
-          A.sbin[i] = b;
-          float3 p = make_float3(0.f, 0.f, 0.f);
-          if (spa >= 0) {
-            int bb;
-            wrapped_position(sg, A.coords, a, p, bb);
-          }
-          A.spos[i] = make_float4(p.x, p.y, p.z, __int_as_float(spa));
-          if (spa >= 0 && i >= A.lo && i < hi_real)
-            atomicAdd(&A.chunk_hist[((i - A.lo) / LAYOUT_CHUNK) * ANI_MAX_SPECIES + spa], 1);
-        }
+        if (valid)
+          place_atom(sg, A.coords, nullptr, a, spa, b, lo + rank, A.sorted_orig, A.orig_to_sorted, A.sbin, A.spos,
+                     A.chunk_hist, A.lo, hi_real);
       }
       if (A.bss && b < nbins && lane == 0) {
         int4* dst = reinterpret_cast<int4*>(A.bss + (size_t)b * ANI_MAX_SPECIES);
@@ -1455,33 +1180,9 @@ __global__ void __launch_bounds__(PREP_CLUSTER_THREADS, 1)
       if (lane == 0) s_tot[w] = run;
     }
     __syncthreads();
-    if (tid == 0) {
-      int row = 0, owned = 0;
-      for (int s = 0; s < S; ++s) {
-        s_base[s] = row;
-        owned += s_tot[s];
-        row += (s_tot[s] + ANI_TILE_ROWS - 1) / ANI_TILE_ROWS * ANI_TILE_ROWS;
-      }
-      s_base[S] = row;
-      if (blockIdx.x == 0) {
-        A.layout_info[0] = row / ANI_TILE_ROWS;
-        A.layout_info[1] = row;
-        A.layout_info[2] = owned;
-        A.layout_info[3] = 0;
-        for (int s = 0; s <= S; ++s) A.layout_info[4 + s] = s_base[s] / ANI_TILE_ROWS;
-        for (int s = S + 1; s <= ANI_MAX_SPECIES; ++s) A.layout_info[4 + s] = row / ANI_TILE_ROWS;
-      }
-    }
-    __syncthreads();
-    if (blockIdx.x == 0) {
-      const int n_tiles_cap = A.rows_cap / ANI_TILE_ROWS;
-      for (int t = tid; t < n_tiles_cap; t += PREP_CLUSTER_THREADS) {
-        const int r = t * ANI_TILE_ROWS;
-        int sp = -1;
-        for (int s = 0; s < S; ++s)
-          if (r >= s_base[s] && r < s_base[s + 1] && r < s_base[s] + s_tot[s]) sp = s;
-        A.tile_species[t] = sp;
-      }
+    const bool cta0 = blockIdx.x == 0;
+    species_rows(S, A.rows_cap, s_tot, s_base, nullptr, cta0 ? A.layout_info : nullptr, cta0 ? A.tile_species : nullptr);
+    if (cta0) {
       // live 32-column AEV blocks: warp w tests the 32 columns of block w (+32, ...) -- one column per lane -- instead
       // of one lane walking a whole block (the serial walk was 5 us of this kernel's critical path)
       const unsigned mask = (unsigned)__ldcg(A.present);
@@ -1492,21 +1193,7 @@ __global__ void __launch_bounds__(PREP_CLUSTER_THREADS, 1)
         if (lane == 0) s_live[b] = live;
       }
       __syncthreads();
-      if (w == 0) {
-        int count = 0;
-        for (int b0 = 0; b0 < nblk; b0 += 32) {
-          const int b = b0 + lane;
-          const bool live = b < nblk && s_live[b];
-          const unsigned m = __ballot_sync(ANI_FULL_MASK, live);
-          if (live) A.blocks[1 + count + __popc(m & ((1u << lane) - 1u))] = b;
-          count += __popc(m);
-        }
-        if (lane == 0) {
-          A.blocks[0] = count;
-          A.blocks[nblk + 2] = (A.blocks[nblk + 1] != (int)mask);
-          A.blocks[nblk + 1] = (int)mask;
-        }
-      }
+      if (w == 0) compact_live_blocks(nblk, mask, A.blocks, [&](int b) { return s_live[b] != 0; });
     }
   }
   stamp(10);
@@ -1514,25 +1201,12 @@ __global__ void __launch_bounds__(PREP_CLUSTER_THREADS, 1)
   {
     const int hi_real = min(A.hi, n_real);
     constexpr int SUBS = PREP_CLUSTER_THREADS / LAYOUT_CHUNK;   // 4
-    const int sub = tid / LAYOUT_CHUNK, wl = w % (LAYOUT_CHUNK / 32);
     for (int c0 = blockIdx.x * SUBS; c0 < A.n_chunks; c0 += gridDim.x * SUBS) {
-      const int c = c0 + sub;
+      const int c = c0 + tid / LAYOUT_CHUNK;
       const int i = A.lo + c * LAYOUT_CHUNK + (tid % LAYOUT_CHUNK);
       const int sp = (c < A.n_chunks && i < hi_real) ? __float_as_int(__ldcg(&A.spos[i]).w) : -1;
-      int my_rank = 0;
-      for (int s = 0; s < S; ++s) {
-        const unsigned m = __ballot_sync(ANI_FULL_MASK, sp == s);
-        if (sp == s) my_rank = __popc(m & ((1u << lane) - 1u));
-        if (lane == 0) s_wcnt[w][s] = __popc(m);
-      }
-      __syncthreads();
-      if (sp >= 0) {
-        int off = 0;
-        for (int ww = 0; ww < wl; ++ww) off += s_wcnt[sub * (LAYOUT_CHUNK / 32) + ww][sp];
-        const int row = s_base[sp] + s_hist[c * ANI_MAX_SPECIES + sp] + off + my_rank;
-        A.row_of[i] = row;
-        A.row_atom[row] = i;
-      }
+      assign_chunk_rows(i, sp, S, s_wcnt, [&](int s) { return s_base[s] + s_hist[c * ANI_MAX_SPECIES + s]; },
+                        A.row_of, A.row_atom);
       __syncthreads();
     }
   }
@@ -1599,6 +1273,23 @@ extern "C" int ani_b200_active_aev_blocks(const float* spos, const ani_grid* gri
   return ANI_OK;
 }
 
+// The checks of the grid inputs, common to ani_b200_build_cells and the preparation; n = n_conf * n_per_conf.  Grid
+// mode 3 needs the lattice table, which only ani_b200_prepare_step_cells has (lattice == NULL: unsupported).
+static int check_grid_args(int n_conf, int n_per_conf, const float* cell, int pbc, int mode, float cutoff, int max_bins,
+                           const float* lattice, int& n) {
+  if (n_conf < 1 || n_per_conf < 1 || cutoff <= 0.f || max_bins < 2) return ANI_ERR_BAD_ARG;
+  if (mode == 0 && n_conf != 1) return ANI_ERR_UNSUPPORTED;
+  if (mode == 1 && (pbc || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
+  if (mode == 2 && (!pbc || !cell || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
+  if (mode == 3 && (!pbc || !cell || !lattice || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
+  if (mode < 0 || mode > 3) return ANI_ERR_BAD_ARG;
+  if (pbc && !cell) return ANI_ERR_BAD_ARG;
+  const long long n_ll = (long long)n_conf * n_per_conf;
+  if (n_ll >= (1ll << ANI_IMG_SHIFT)) return ANI_ERR_UNSUPPORTED;
+  n = (int)n_ll;
+  return ANI_OK;
+}
+
 extern "C" int ani_b200_build_cells(const float* coords, const int32_t* species, int n_conf, int n_per_conf,
                                     const float* cell, int pbc, int mode, float cutoff, int max_bins,
                                     ani_grid* grid, int32_t* bin_start, int32_t* sorted_orig,
@@ -1607,16 +1298,8 @@ extern "C" int ani_b200_build_cells(const float* coords, const int32_t* species,
   if (!coords || !species || !grid || !bin_start || !sorted_orig || !orig_to_sorted || !spos || !sbin ||
       !scratch_i32 || !status)
     return ANI_ERR_BAD_ARG;
-  if (n_conf < 1 || n_per_conf < 1 || cutoff <= 0.f || max_bins < 2) return ANI_ERR_BAD_ARG;
-  if (mode == 0 && n_conf != 1) return ANI_ERR_UNSUPPORTED;
-  if (mode == 1 && (pbc || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
-  if (mode == 2 && (!pbc || !cell || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
-  if (mode == 3) return ANI_ERR_UNSUPPORTED;   // one cell per conformer: ani_b200_prepare_step_cells only
-  if (mode < 0 || mode > 2) return ANI_ERR_BAD_ARG;
-  if (pbc && !cell) return ANI_ERR_BAD_ARG;
-  const long long n_ll = (long long)n_conf * n_per_conf;
-  if (n_ll >= (1ll << ANI_IMG_SHIFT)) return ANI_ERR_UNSUPPORTED;
-  const int n = (int)n_ll;
+  int n;
+  if (const int err = check_grid_args(n_conf, n_per_conf, cell, pbc, mode, cutoff, max_bins, nullptr, n)) return err;
   cudaStream_t st = (cudaStream_t)stream;
   int32_t* bin_of = scratch_i32;
   int32_t* slot = scratch_i32 + n;
@@ -1693,16 +1376,8 @@ static int prepare_step(const float* coords, const int32_t* species, int n_conf,
   if (!coords || !species || !grid || !bin_start || !sorted_orig || !orig_to_sorted || !spos || !sbin ||
       !row_of || !row_atom || !tile_species || !layout_info || !aev_blocks || !scratch_i32 || !status)
     return ANI_ERR_BAD_ARG;
-  if (n_conf < 1 || n_per_conf < 1 || cutoff <= 0.f || max_bins < 2) return ANI_ERR_BAD_ARG;
-  if (mode == 0 && n_conf != 1) return ANI_ERR_UNSUPPORTED;
-  if (mode == 1 && (pbc || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
-  if (mode == 2 && (!pbc || !cell || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
-  if (mode == 3 && (!pbc || !cell || !lattice || n_conf + 1 > max_bins)) return ANI_ERR_UNSUPPORTED;
-  if (mode < 0 || mode > 3) return ANI_ERR_BAD_ARG;
-  if (pbc && !cell) return ANI_ERR_BAD_ARG;
-  const long long n_ll = (long long)n_conf * n_per_conf;
-  if (n_ll >= (1ll << ANI_IMG_SHIFT)) return ANI_ERR_UNSUPPORTED;
-  const int n = (int)n_ll;
+  int n;
+  if (const int err = check_grid_args(n_conf, n_per_conf, cell, pbc, mode, cutoff, max_bins, lattice, n)) return err;
   if (num_species < 1 || num_species > ANI_MAX_SPECIES || lo < 0 || hi > n || lo > hi) return ANI_ERR_BAD_ARG;
   if (rows_cap % ANI_TILE_ROWS != 0) return ANI_ERR_BAD_ARG;
   if ((long long)rows_cap < (long long)(hi - lo) + (long long)num_species * (ANI_TILE_ROWS - 1)) return ANI_ERR_BAD_ARG;
