@@ -427,12 +427,11 @@ def check_forward(gpu: Gpu, ref: Ref, group: str, rows: tp.Optional[torch.Tensor
     lv = live.to(DEV)
     pr = pm[gpu.rows][:, :D]
     assert torch.equal(pr[:, lv], plain[gpu.rows][:, :D][:, lv])
-    # dead element-pair blocks are never written; dead radial blocks: never written by the bucket-grid kernel,
-    # zero-filled by the warp-per-atom search (ANI_B200_AEV_LEGACY=1)
+    # dead element blocks, radial and element-pair, are never written (both forward kernels share the feature code)
     dead_ang = ~lv & (torch.arange(D, device=DEV) >= spec.radial_len)
     dead_rad = ~lv & (torch.arange(D, device=DEV) < spec.radial_len)
     assert bool((pr[:, dead_ang] == SENTINEL).all())
-    assert bool(((pr[:, dead_rad] == SENTINEL) | (pr[:, dead_rad] == 0)).all())
+    assert bool((pr[:, dead_rad] == SENTINEL).all())
     # live 32-column blocks of the internal order (aev_column_live)
     ws = gpu.ws
     blocks = ws.aev_blocks[1:1 + int(ws.aev_blocks[0])].tolist()

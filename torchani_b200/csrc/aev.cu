@@ -1,15 +1,17 @@
 // Fused neighbour search + AEV forward, and AEV backward (forces), one warp per central atom.
 //
 // Forward (replaces neighbors.py:64-113,968-1002 + aev/_computer.py:274-350; the reference's
-// GPU path is csrc/aev.cu K1-K9).  Two kernels:
+// GPU path is csrc/aev.cu K1-K9).  One per-atom feature tail (atom_features), two ways to fill it with the
+// neighbours in species-major order:
 //   * k_aev_forward_cta (the bucket-grid path): the AEV_FWD_WARPS consecutive atoms of a CTA share the
 //     27-bucket neighbourhood, staged once per CTA in shared memory in species-major order; a warp
 //     compacts its neighbours with one ballot per 32 candidates and gets the neighbour list and the
-//     angular sub-list grouped by species for free; radial sums in registers, per species pair
-//     every lane evaluates whole triples (32 angular features in registers) + one warp
-//     transpose-reduce.  No atomics in the forward pass.
+//     angular sub-list grouped by species for free.
 //   * k_aev_forward (explicit neighbour rows handed in by the caller, and ANI_B200_AEV_LEGACY=1): every
-//     warp walks its own candidate ranges in global memory and counting-sorts the neighbours by species.
+//     warp gathers its own neighbours (the rows, or its candidate ranges in global memory) and regroups
+//     them by species (group_by_species).
+// The tail: radial sums in registers, per species pair every lane evaluates whole triples (32 angular
+// features in registers) + one warp transpose-reduce.  No atomics in the forward pass.
 //
 // Backward (csrc/aev.cu K10/K11): recomputes the geometry from the stored neighbour words, copies the
 // live blocks of the upstream gradient row with cp.async into a compact per-composition table, and
@@ -73,6 +75,10 @@ struct ExplicitNbrs {
   const float4* d;
 };
 
+// r^2 of a neighbour vector, written out: both forward kernels must round it the same way (nvcc's own contraction of
+// dx * dx + dy * dy + dz * dz depends on the surrounding code)
+__device__ __forceinline__ float norm2(float dx, float dy, float dz) { return fmaf(dz, dz, fmaf(dx, dx, dy * dy)); }
+
 // bucket range + image code for offset (ox, oy, oz) around bucket (ix, iy, iz) of the sub-grid that starts at
 // bucket `base` (bucket_coords); false if it does not exist (non-periodic boundary)
 __device__ __forceinline__ bool neighbour_bucket(const ani_grid& g, const int32_t* __restrict__ bin_start, int base,
@@ -101,7 +107,7 @@ __device__ __forceinline__ bool neighbour_bucket(const ani_grid& g, const int32_
 
 // per-warp shared memory carve-up (byte offsets), shared by forward and backward
 struct WarpSmem {
-  float4* nd;            // [cap] dx, dy, dz, R   (neighbour - centre)
+  float4* nd;            // [cap] dx, dy, dz, R   (neighbour - centre; the forward gathers r^2 into .w)
   float* nfc;            // [cap] forward: fc(R; Rcr).  backward: unused
   int32_t* nj;           // [cap] neighbour word
   float* fgrad;          // [cap*3] backward only
@@ -110,8 +116,7 @@ struct WarpSmem {
   float* afc;            // [ANI_MAX_ANG] fc(R; Rca)
   float* afcd;           // [ANI_MAX_ANG] d fc / dR (backward)
   int32_t* seg;          // [ANI_MAX_SPECIES + 1] species segments of aidx
-  int32_t* seg_all;      // [ANI_MAX_SPECIES + 1] species segments of ord (forward)
-  unsigned char* ord;    // [cap] all neighbours, species-sorted (forward)
+  int32_t* seg_all;      // [ANI_MAX_SPECIES + 1] species segments of nd (forward)
   float* rad;            // forward: [2*RL] accumulators; backward: g_rad [RL] + g_ang [pairs][36]
 };
 
@@ -123,7 +128,8 @@ __host__ __device__ inline size_t warp_smem_bytes(int cap, int rad_floats, bool 
   b = (b + 15) / 16 * 16;
   b += (size_t)ANI_MAX_ANG * 4 * 2;          // afc, afcd
   b += 2 * 16 * 4;                           // seg, seg_all (padded)
-  b += ((size_t)cap + 15) / 16 * 16;         // ord
+  b += ((size_t)cap + 15) / 16 * 16;         // unused; the launch shapes, occupancies and TMA staging capacity
+                                             // of the kernels were tuned with these bytes in place
   b += (size_t)rad_floats * 4;
   return (b + 15) / 16 * 16;
 }
@@ -152,84 +158,14 @@ __device__ __forceinline__ WarpSmem carve(unsigned char* base, int cap, bool bac
   p += 16 * 4;
   s.seg_all = reinterpret_cast<int32_t*>(p);
   p += 16 * 4;
-  s.ord = p;
   p += ((size_t)cap + 15) / 16 * 16;
   s.rad = reinterpret_cast<float*>(p);
   return s;
 }
 
-// Counting sort (by species) of the neighbours within Rca.  Fills aidx/afc(/afcd)/seg, returns
-// the number of angular neighbours (clamped to ANI_MAX_ANG).
-template <bool WITH_GRAD>
-__device__ __forceinline__ int build_angular_list(const ani_aev_params& P, const WarpSmem& s, int cnt, int lane,
-                                                  int32_t* status) {
-  const int S = P.num_species;
-  int seg_cnt[ANI_MAX_SPECIES];
-#pragma unroll
-  for (int k = 0; k < ANI_MAX_SPECIES; ++k) seg_cnt[k] = 0;
-  for (int base = 0; base < cnt; base += 32) {
-    int n = base + lane;
-    int sp = -1;
-    if (n < cnt && s.nd[n].w <= P.rca) sp = s.nsp[n];
-#pragma unroll
-    for (int k = 0; k < ANI_MAX_SPECIES; ++k) {
-      unsigned m = __ballot_sync(ANI_FULL_MASK, sp == k);
-      seg_cnt[k] += __popc(m);
-    }
-  }
-  int seg_start[ANI_MAX_SPECIES + 1];
-  seg_start[0] = 0;
-#pragma unroll
-  for (int k = 0; k < ANI_MAX_SPECIES; ++k) seg_start[k + 1] = seg_start[k] + seg_cnt[k];
-  int total = seg_start[ANI_MAX_SPECIES];
-  if (total > ANI_MAX_ANG) {
-    if (lane == 0) atomicOr(status, ANI_STATUS_ANG_OVERFLOW);
-    total = ANI_MAX_ANG;
-  }
-  if (lane == 0) {
-#pragma unroll
-    for (int k = 0; k <= ANI_MAX_SPECIES; ++k)
-      if (k <= S) s.seg[k] = min(seg_start[k], ANI_MAX_ANG);
-  }
-  int run[ANI_MAX_SPECIES];
-#pragma unroll
-  for (int k = 0; k < ANI_MAX_SPECIES; ++k) run[k] = 0;
-  const unsigned lt = (1u << lane) - 1u;
-  for (int base = 0; base < cnt; base += 32) {
-    int n = base + lane;
-    int sp = -1;
-    float R = 0.f;
-    if (n < cnt) {
-      R = s.nd[n].w;
-      if (R <= P.rca) sp = s.nsp[n];
-    }
-    int pos = -1;
-#pragma unroll
-    for (int k = 0; k < ANI_MAX_SPECIES; ++k) {
-      unsigned m = __ballot_sync(ANI_FULL_MASK, sp == k);
-      if (sp == k) pos = seg_start[k] + run[k] + __popc(m & lt);
-      run[k] += __popc(m);
-    }
-    if (pos >= 0 && pos < ANI_MAX_ANG) {
-      s.aidx[pos] = (unsigned char)n;
-      if (WITH_GRAD) {
-        float f, df;
-        cutoff_value_grad(R, P.rca, P.cutoff_kind, f, df);
-        s.afc[pos] = f;
-        s.afcd[pos] = df;
-      } else {
-        s.afc[pos] = cutoff_value(R, P.rca, P.cutoff_kind);
-      }
-    }
-  }
-  __syncwarp();
-  return total;
-}
-
 // Order-preserving compaction of the neighbours within Rca (backward pass): the pair rotation there looks the
-// species of both partners up per pair and needs neither species segments nor a species-sorted list, so the counting
-// sort of build_angular_list (2 passes x 8 ballots per 32 neighbours; 8.6 % of the kernel's stall samples in round 1)
-// is replaced by one ballot per 32 neighbours.  Fills aidx/afc/afcd, returns the count (clamped to ANI_MAX_ANG).
+// species of both partners up per pair and needs neither species segments nor a species-sorted list: one ballot per
+// 32 neighbours, no counting sort.  Fills aidx/afc/afcd, returns the count (clamped to ANI_MAX_ANG).
 __device__ __forceinline__ int compact_angular_list(const ani_aev_params& P, const WarpSmem& s, int cnt, int lane,
                                                     int32_t* status) {
   const unsigned lt = (1u << lane) - 1u;
@@ -255,56 +191,6 @@ __device__ __forceinline__ int compact_angular_list(const ani_aev_params& P, con
   }
   __syncwarp();
   return total;
-}
-
-// Counting sort (by species) of ALL neighbours: ord[] = neighbour indices grouped by species,
-// seg_all[] = segment starts.  The radial block then accumulates one species segment at a time in
-// registers (no shared-memory read-modify-write chain).
-__device__ __forceinline__ void build_species_order(const ani_aev_params& P, const WarpSmem& s, int cnt, int lane) {
-  const int S = P.num_species;
-  int seg_cnt[ANI_MAX_SPECIES];
-#pragma unroll
-  for (int k = 0; k < ANI_MAX_SPECIES; ++k) seg_cnt[k] = 0;
-  for (int base = 0; base < cnt; base += 32) {
-    const int n = base + lane;
-    const int sp = n < cnt ? (int)s.nsp[n] : -1;
-#pragma unroll
-    for (int k = 0; k < ANI_MAX_SPECIES; ++k) seg_cnt[k] += __popc(__ballot_sync(ANI_FULL_MASK, sp == k));
-  }
-  int seg_start[ANI_MAX_SPECIES + 1];
-  seg_start[0] = 0;
-#pragma unroll
-  for (int k = 0; k < ANI_MAX_SPECIES; ++k) seg_start[k + 1] = seg_start[k] + seg_cnt[k];
-  if (lane == 0) {
-#pragma unroll
-    for (int k = 0; k <= ANI_MAX_SPECIES; ++k)
-      if (k <= S) s.seg_all[k] = seg_start[k];
-  }
-  int run[ANI_MAX_SPECIES];
-#pragma unroll
-  for (int k = 0; k < ANI_MAX_SPECIES; ++k) run[k] = 0;
-  const unsigned lt = (1u << lane) - 1u;
-  for (int base = 0; base < cnt; base += 32) {
-    const int n = base + lane;
-    const int sp = n < cnt ? (int)s.nsp[n] : -1;
-    int pos = -1;
-#pragma unroll
-    for (int k = 0; k < ANI_MAX_SPECIES; ++k) {
-      const unsigned m = __ballot_sync(ANI_FULL_MASK, sp == k);
-      if (sp == k) pos = seg_start[k] + run[k] + __popc(m & lt);
-      run[k] += __popc(m);
-    }
-    if (pos >= 0) s.ord[pos] = (unsigned char)n;
-  }
-  __syncwarp();
-}
-
-// q-th unordered pair (a < b) of a triangle
-__device__ __forceinline__ void triangle_decode(int q, int& a, int& b) {
-  b = (int)((1.0f + sqrtf(1.0f + 8.0f * (float)q)) * 0.5f);
-  while (b * (b - 1) / 2 > q) --b;
-  while ((b + 1) * b / 2 <= q) ++b;
-  a = q - b * (b - 1) / 2;
 }
 
 // one level of transpose_reduce32: lanes l and l ^ HALF swap halves of acc[0, 2 HALF) and each keeps a sum
@@ -334,233 +220,6 @@ __device__ __forceinline__ float transpose_reduce32(float (&acc)[32], int lane) 
 // ---------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------
-// LAT (grid mode 3): image shifts in the lattice of the bucket's conformer (lattice table); the range table, when
-// given, already holds them
-template <int NA, int NZ, bool LAT = false>
-__global__ void __launch_bounds__(AEV_WARPS * 32)
-    k_aev_forward(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
-                  const int32_t* __restrict__ bin_start, const float4* __restrict__ spos,
-                  const int32_t* __restrict__ sbin, const float4* __restrict__ ranges,
-                  const int32_t* __restrict__ species_mask, const ExplicitNbrs ex, int lo, int hi,
-                  const int32_t* __restrict__ row_of,
-                  float* __restrict__ aev, int ldx, int layout, int32_t* __restrict__ nbr_cnt,
-                  int32_t* __restrict__ nbr_list, int cap, int32_t* __restrict__ status, size_t warp_bytes,
-                  const float* __restrict__ lattice) {
-  static_assert(NA * NZ == 32, "one lane per angular feature");
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const ani_grid g = *grid;
-  hi = min(hi, g.n_real);
-  const int i = lo + blockIdx.x * AEV_WARPS + warp;
-  if (i >= hi) return;
-  const WarpSmem s = carve(smem_raw + warp * warp_bytes, cap, false);
-  // output: plain row-major rows, or the tiled operand layout (16-bit pieces) the GEMM consumes
-  const int out_row = row_of[i];
-  const int kblocks = ldx >> 5;
-  float vmax = 0.f;  // largest scaled feature this lane wrote (operand range check, fp16 pieces)
-  auto store_feature = [&](int col, float v) {
-    if (layout == 0) {
-      aev[(size_t)out_row * ldx + col] = v;
-    } else {
-      unsigned char* dst = reinterpret_cast<unsigned char*>(aev) + opnd_offset(out_row, col, kblocks);
-      unsigned short pc[OPND_PARTS];
-      v *= OPND_SCALE_VALUE;
-      vmax = fmaxf(vmax, v);  // AEV features are >= 0
-      opnd_split(v, pc);
-#pragma unroll
-      for (int k = 0; k < OPND_PARTS; ++k) *reinterpret_cast<unsigned short*>(dst + k * OPND_PART_BYTES) = pc[k];
-    }
-  };
-  const int S = P.num_species;
-  const int nR = P.n_shf_r;
-  const int RL = S * nR;
-
-  // ---- 1. neighbours within Rcr -> shared memory
-  const float4 pi = spos[i];
-  if (__float_as_int(pi.w) < 0) return;  // padding atom (only reachable with explicit neighbour rows)
-  const float rcr2 = P.rcr * P.rcr;
-  const unsigned lt = (1u << lane) - 1u;
-  int cnt = 0;
-  {
-    const int b = ex.start ? 0 : sbin[i];
-    // one candidate range: compact the atoms within Rcr into shared memory
-    auto scan_range = [&](int rlo, int rhi, int code, float shx, float shy, float shz) {
-      for (int base = rlo; base < rhi; base += 32) {
-        const int c = base + lane;
-        const bool valid = c < rhi;
-        const float4 p = valid ? spos[c] : pi;
-        const float dx = (p.x + shx) - pi.x, dy = (p.y + shy) - pi.y, dz = (p.z + shz) - pi.z;
-        const float r2 = dx * dx + dy * dy + dz * dz;
-        const bool keep = valid && r2 <= rcr2 && !(c == i && code == 13);
-        const unsigned m = __ballot_sync(ANI_FULL_MASK, keep);
-        if (keep) {
-          const int pos = cnt + __popc(m & lt);
-          if (pos < cap) {
-            s.nd[pos] = make_float4(dx, dy, dz, sqrtf(r2));
-            s.nj[pos] = c | (code << ANI_IMG_SHIFT);
-            s.nsp[pos] = (unsigned char)__float_as_int(p.w);
-          }
-        }
-        cnt += __popc(m);
-      }
-    };
-    if (ex.start) {
-      // neighbours handed in by the caller (already screened to Rcr): copy the row
-      const int e0 = ex.start[i];
-      cnt = ex.start[i + 1] - e0;
-      for (int n = lane; n < min(cnt, cap); n += 32) {
-        const int j = ex.j[e0 + n];
-        s.nd[n] = ex.d[e0 + n];
-        s.nj[n] = j | (13 << ANI_IMG_SHIFT);
-        s.nsp[n] = (unsigned char)__float_as_int(spos[j].w);
-      }
-    } else if (g.mode == 1) {   // bucket == conformer
-      scan_range(bin_start[b], bin_start[b + 1], 13, 0.f, 0.f, 0.f);
-    } else if (ranges) {
-      // precomputed table: lane o holds the record of neighbouring bucket o
-      float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f), r1 = r0;
-      if (lane < 27) {
-        r0 = ranges[2 * ((size_t)b * 27 + lane)];
-        r1 = ranges[2 * ((size_t)b * 27 + lane) + 1];
-      }
-      for (int o = 0; o < 27; ++o) {
-        const int rlo = __float_as_int(__shfl_sync(ANI_FULL_MASK, r0.x, o));
-        const int rhi = __float_as_int(__shfl_sync(ANI_FULL_MASK, r0.y, o));
-        if (rhi <= rlo) continue;
-        const int code = __float_as_int(__shfl_sync(ANI_FULL_MASK, r0.z, o));
-        scan_range(rlo, rhi, code, __shfl_sync(ANI_FULL_MASK, r1.x, o), __shfl_sync(ANI_FULL_MASK, r1.y, o),
-                   __shfl_sync(ANI_FULL_MASK, r1.z, o));
-      }
-    } else {
-      int ix, iy, iz;
-      const int base = bucket_coords(g, b, ix, iy, iz);
-      for (int ox = -1; ox <= 1; ++ox)
-        for (int oy = -1; oy <= 1; ++oy)
-          for (int oz = -1; oz <= 1; ++oz) {
-            NeighbourRange r;
-            if (!neighbour_bucket(g, bin_start, base, ix, iy, iz, ox, oy, oz, r)) continue;
-            const float3 sh = (r.code == 13) ? make_float3(0.f, 0.f, 0.f)
-                              : LAT ? image_shift(lattice, base / (g.dims[0] * g.dims[1] * g.dims[2]), r.code)
-                                    : image_shift(g, r.code);
-            scan_range(r.lo, r.hi, r.code, sh.x, sh.y, sh.z);
-          }
-    }
-  }
-  if (cnt > cap) {
-    if (lane == 0) atomicOr(status, ANI_STATUS_NBR_OVERFLOW);
-    cnt = cap;
-  }
-  __syncwarp();
-  if (lane == 0 && nbr_cnt) nbr_cnt[i] = cnt;
-  for (int n = lane; n < cnt; n += 32) {
-    if (nbr_list) nbr_list[(size_t)i * cap + n] = s.nj[n];
-    s.nfc[n] = cutoff_value(s.nd[n].w, P.rcr, P.cutoff_kind);
-  }
-  __syncwarp();
-
-  // ---- 2. radial block: lane = (shift m, neighbour parity h).  The neighbours are grouped by
-  //         species first, so each (species, shift) sum lives in a register and goes straight to
-  //         the output: no shared-memory accumulators, no atomics
-  build_species_order(P, s, cnt, lane);
-  {
-    const int lpn = (nR <= 16) ? 16 : 32;
-    const int halves = 32 / lpn;
-    const int m = lane % lpn, h = lane / lpn;
-    const float shf = P.shf_r[m < nR ? m : 0];
-    for (int sp = 0; sp < S; ++sp) {
-      const int k1 = s.seg_all[sp + 1];
-      float acc = 0.f;
-      for (int k = s.seg_all[sp] + h; k < k1; k += halves) {
-        const int n = s.ord[k];
-        const float d = s.nd[n].w - shf;
-        acc = fmaf(fast_exp(-P.eta_r * d * d), s.nfc[n], acc);
-      }
-      if (halves == 2) acc += __shfl_xor_sync(ANI_FULL_MASK, acc, 16);
-      if (h == 0 && m < nR) store_feature(sp * nR + m, 0.25f * acc);
-    }
-  }
-
-  // ---- 3. angular block
-  const int n_ang = build_angular_list<false>(P, s, cnt, lane, status);
-  (void)n_ang;
-  float shfA[NA], cz[NZ], sz[NZ];
-#pragma unroll
-  for (int a = 0; a < NA; ++a) shfA[a] = P.shf_a[a];
-#pragma unroll
-  for (int z = 0; z < NZ; ++z) {
-    cz[z] = P.cos_z[z];
-    sz[z] = P.sin_z[z];
-  }
-  // element pairs that do not occur anywhere in the system are never read by the MLP: skip them
-  // (species_mask[1] != 0: the composition changed since the last call -> zero-fill them once)
-  const unsigned present = (species_mask && !species_mask[1]) ? (unsigned)species_mask[0] : 0xffffffffu;
-  int p = 0;
-  for (int s1 = 0; s1 < S; ++s1) {
-    if (!((present >> s1) & 1u)) {
-      p += S - s1;
-      continue;
-    }
-    const int a0 = s.seg[s1], na = s.seg[s1 + 1] - a0;
-    for (int s2 = s1; s2 < S; ++s2, ++p) {
-      if (!((present >> s2) & 1u)) continue;
-      const int b0 = s.seg[s2], nb = s.seg[s2 + 1] - b0;
-      const int count = (s1 == s2) ? na * (na - 1) / 2 : na * nb;
-      float out = 0.f;
-      if (count > 0) {
-        float acc[32];
-#pragma unroll
-        for (int f = 0; f < 32; ++f) acc[f] = 0.f;
-        for (int q = lane; q < count; q += 32) {
-          int ja, jb;
-          if (s1 == s2) {
-            triangle_decode(q, ja, jb);
-            ja += a0;
-            jb += a0;
-          } else {
-            ja = a0 + q / nb;
-            jb = b0 + q % nb;
-          }
-          const float4 dj = s.nd[s.aidx[ja]], dk = s.nd[s.aidx[jb]];
-          const float w2 = 2.0f * s.afc[ja] * s.afc[jb];
-          const float dot = dj.x * dk.x + dj.y * dk.y + dj.z * dk.z;
-          const float c = 0.95f * dot * fast_rcp(fmaxf(dj.w * dk.w, 1e-10f));
-          const float sn = fast_sqrt(fmaxf(1.0f - c * c, 0.f));
-          const float rbar = 0.5f * (dj.w + dk.w);
-          float f1[NZ];
-#pragma unroll
-          for (int z = 0; z < NZ; ++z) {
-            const float base = fmaxf(0.5f * (1.0f + c * cz[z] + sn * sz[z]), 0.f);
-            f1[z] = fast_exp2(P.zeta * fast_log2(base));  // base^zeta; base = 0 -> ex2(-inf) = 0
-          }
-#pragma unroll
-          for (int a = 0; a < NA; ++a) {
-            const float d = rbar - shfA[a];
-            const float f2 = fast_exp(-P.eta_a * d * d) * w2;
-#pragma unroll
-            for (int z = 0; z < NZ; ++z) acc[a * NZ + z] += f1[z] * f2;
-          }
-        }
-        out = transpose_reduce32(acc, lane);
-      }
-      store_feature(RL + (layout ? P.ang_pad : 0) + p * 32 + lane, out);
-    }
-  }
-  if (ANI_OPND_FP16X2 && !(vmax <= OPND_HALF_MAX)) atomicOr(status, ANI_STATUS_OPERAND_RANGE);
-}
-
-// ---------------------------------------------------------------------------------------
-// forward, CTA-staged neighbourhood (the bucket-grid path)
-//
-// The AEV_WARPS consecutive (bucket-sorted) atoms of a CTA almost always share one bucket, so the
-// candidates of its 27 neighbouring buckets are staged ONCE per CTA in shared memory -- shifted by
-// their lattice image and ordered species-major (the buckets are species-sorted, so the place of
-// every candidate follows from a 27 x S table of counts) -- instead of every warp walking the 27
-// ranges in global memory.  A warp then compacts its neighbours with one ballot per 32 candidates,
-// species segment by species segment: the neighbour list and the angular sub-list come out
-// grouped by species, which the two counting sorts of k_aev_forward used to establish.
-// CTAs that straddle a bucket boundary run one staging phase per distinct bucket; neighbourhoods
-// larger than CAND_CAP candidates are staged in windows of the species-major order.
-// ---------------------------------------------------------------------------------------
 #ifndef ANI_AEV_CAND_CAP
 #define ANI_AEV_CAND_CAP 768
 #endif
@@ -574,20 +233,6 @@ constexpr int CAND_CAP = ANI_AEV_CAND_CAP;
 constexpr int AEV_FWD_WARPS = ANI_AEV_FWD_WARPS;  // atoms (= warps) per CTA of the staged forward kernel
 constexpr int NRANGE = 27;
 constexpr int T2O_CAP = 1024;
-
-struct CtaStage {
-  float4 cand[CAND_CAP];  // shifted position; .w = neighbour word (sorted index | image code << 26)
-  float4 r_shift[NRANGE];
-  int r_lo[NRANGE], r_code[NRANGE];
-  int r_len[NRANGE];                           // candidates of every range
-  int r_off[NRANGE + 1];                       // exclusive prefix of the range lengths
-  int cnt[ANI_MAX_SPECIES][NRANGE];            // candidates per (species, range)
-  int off[ANI_MAX_SPECIES * NRANGE + 1];       // exclusive prefix of cnt in species-major order
-  int adj[ANI_MAX_SPECIES][NRANGE];            // off[s][o] - (candidates of lower species in range o)
-  int wbin[AEV_FWD_WARPS];
-  unsigned char t2o[T2O_CAP];                  // range of the t-th candidate (range-major numbering)
-  unsigned long long tma_bar;                  // mbarrier of the TMA bulk copies that stage the bucket ranges
-};
 
 // ---- opt-in phase trace (build variant "aevtrace": -DANI_AEV_FWD_TRACE=1; tools/aev_forward_trace.py) --------------
 // One record of 16 int64 per atom (index i - lo), written by its warp: clock64 cycles spent in each phase (the staging
@@ -645,6 +290,400 @@ struct AevTrace {
 };
 #endif
 
+// Candidate range o (0 .. 26; o = 9 (ox + 1) + 3 (oy + 1) + (oz + 1)) of bucket b: atoms lo .. hi - 1 of the
+// bucket-sorted arrays, their image code and shift, and (range table only) the id of the neighbouring bucket, which
+// addresses its per-bucket species offsets.  Mode 1 (bucket == conformer) has range 13 alone.  The range table, when
+// given, holds the records; otherwise they are computed, the shift from the grid or, with LAT (grid mode 3), from the
+// lattice of the bucket's conformer.  A range that does not exist (non-periodic boundary) is empty with code 13.
+struct RangeRecord {
+  int lo, hi, code, bucket;
+  float3 shift;
+};
+
+template <bool LAT>
+__device__ __forceinline__ RangeRecord bucket_range(const ani_grid& g, const int32_t* __restrict__ bin_start,
+                                                   const float4* __restrict__ ranges, const float* __restrict__ lattice,
+                                                   int b, int o) {
+  RangeRecord r{0, 0, 13, b, make_float3(0.f, 0.f, 0.f)};
+  if (g.mode == 1) {
+    if (o == 13) {
+      r.lo = bin_start[b];
+      r.hi = bin_start[b + 1];
+    }
+  } else if (ranges) {
+    const float4 r0 = ranges[2 * ((size_t)b * NRANGE + o)];
+    const float4 r1 = ranges[2 * ((size_t)b * NRANGE + o) + 1];
+    r.lo = __float_as_int(r0.x);
+    r.hi = __float_as_int(r0.y);
+    r.code = __float_as_int(r0.z);
+    r.bucket = __float_as_int(r0.w);
+    r.shift = make_float3(r1.x, r1.y, r1.z);
+  } else {
+    int ix, iy, iz;
+    const int base = bucket_coords(g, b, ix, iy, iz);
+    NeighbourRange n;
+    if (neighbour_bucket(g, bin_start, base, ix, iy, iz, o / 9 - 1, (o / 3) % 3 - 1, o % 3 - 1, n)) {
+      r.lo = n.lo;
+      r.hi = n.hi;
+      r.code = n.code;
+      if (n.code != 13)
+        r.shift = LAT ? image_shift(lattice, base / (g.dims[0] * g.dims[1] * g.dims[2]), n.code)
+                      : image_shift(g, n.code);
+    }
+  }
+  return r;
+}
+
+// A lane's stores into one AEV row: plain row-major (layout 0), or the tiled operand layout (16-bit pieces) the GEMM
+// consumes.  vmax is the largest scaled feature the lane wrote, for the operand range check of the fp16 pieces.
+struct FeatureWriter {
+  float* aev;
+  int row, ldx, kblocks, layout;
+  float vmax;
+  __device__ __forceinline__ void operator()(int col, float v) {
+    if (layout == 0) {
+      aev[(size_t)row * ldx + col] = v;
+    } else {
+      unsigned char* dst = reinterpret_cast<unsigned char*>(aev) + opnd_offset(row, col, kblocks);
+      unsigned short pc[OPND_PARTS];
+      v *= OPND_SCALE_VALUE;
+      vmax = fmaxf(vmax, v);  // AEV features are >= 0
+      opnd_split(v, pc);
+#pragma unroll
+      for (int k = 0; k < OPND_PARTS; ++k) *reinterpret_cast<unsigned short*>(dst + k * OPND_PART_BYTES) = pc[k];
+    }
+  }
+};
+
+// The features of atom i from its neighbourhood in the warp's shared memory: the per-atom tail of both forward
+// kernels.  Input: nd[n] = (dx, dy, dz, r^2) of the neighbours within Rcr in species-major order, nj[n] their
+// words, seg_all the species segments of that list, aidx the angular sub-list (r^2 <= Rca^2, indices into nd) and
+// seg its species segments; cnt and cnt_a unclamped (an overflow sets its status bit).  Writes nbr_cnt / nbr_list
+// (when given) and the AEV row of atom i.
+template <int NA, int NZ>
+__device__ __forceinline__ void atom_features(const ani_aev_params& P, const WarpSmem& s, int i, int cnt, int cnt_a,
+                                              const int32_t* __restrict__ species_mask,
+                                              const int32_t* __restrict__ row_of, float* __restrict__ aev, int ldx,
+                                              int layout, int32_t* __restrict__ nbr_cnt,
+                                              int32_t* __restrict__ nbr_list, int cap, int32_t* __restrict__ status,
+                                              AevTrace& tr) {
+  const int lane = threadIdx.x & 31;
+  const int S = P.num_species;
+  const int nR = P.n_shf_r;
+  const int RL = S * nR;
+  if (cnt > cap) {
+    if (lane == 0) atomicOr(status, ANI_STATUS_NBR_OVERFLOW);
+    cnt = cap;
+  }
+  if (cnt_a > ANI_MAX_ANG) {
+    if (lane == 0) atomicOr(status, ANI_STATUS_ANG_OVERFLOW);
+    cnt_a = ANI_MAX_ANG;
+  }
+  __syncwarp();
+
+  FeatureWriter store{aev, row_of[i], ldx, ldx >> 5, layout, 0.f};
+
+  if (lane == 0 && nbr_cnt) nbr_cnt[i] = cnt;
+  // per neighbour: (c R, fc(R)) with c = sqrt(eta_r log2 e), so that a Gaussian factor is
+  // ex2(-(c R - c ShfR)^2); the neighbour words go to the list the backward kernel reads
+  const float cr = sqrtf(P.eta_r * 1.4426950408889634f);
+  if (nbr_list)
+    for (int n = lane; n < cnt; n += 32) nbr_list[(size_t)i * cap + n] = s.nj[n];
+  __syncwarp();
+  // [cap] float2 over nfc and nj (adjacent, 8-byte aligned; the words were just copied out)
+  float2* rf = reinterpret_cast<float2*>(s.nfc);
+  for (int n = lane; n < cnt; n += 32) {
+    const float R = sqrtf(s.nd[n].w);
+    s.nd[n].w = R;
+    rf[n] = make_float2(cr * R, cutoff_value(R, P.rcr, P.cutoff_kind));
+  }
+  __syncwarp();
+  tr.mark(TR_LIST);
+
+  // element pairs / elements that do not occur anywhere in the system are never read by the MLP:
+  // skip them (species_mask[1] != 0: the composition changed since the last call -> write them once)
+  const unsigned present = (species_mask && !species_mask[1]) ? (unsigned)species_mask[0] : 0xffffffffu;
+
+  // ---- radial block: lane = (shift m, neighbour parity h); one species segment at a time, the
+  //      (species, shift) sum lives in a register: no shared-memory accumulators, no atomics
+  {
+    const int lpn = (nR <= 16) ? 16 : 32;
+    const int halves = 32 / lpn;
+    const int m = lane % lpn, h = lane / lpn;
+    const float cshf = cr * P.shf_r[m < nR ? m : 0];
+    for (int sp = 0; sp < S; ++sp) {
+      if (!((present >> sp) & 1u)) continue;
+      const int k1 = s.seg_all[sp + 1];
+      float acc = 0.f;
+#pragma unroll 2
+      for (int k = s.seg_all[sp] + h; k < k1; k += halves) {
+        const float2 v = rf[k];
+        const float d = v.x - cshf;
+        acc = fmaf(fast_exp2(-d * d), v.y, acc);
+      }
+      if (halves == 2) acc += __shfl_xor_sync(ANI_FULL_MASK, acc, 16);
+      if (h == 0 && m < nR) store(sp * nR + m, 0.25f * acc);
+    }
+  }
+  tr.mark(TR_RADIAL);
+
+  // ---- angular block
+  const int n_ang = cnt_a;
+  for (int q = lane; q < n_ang; q += 32) s.afc[q] = cutoff_value(s.nd[s.aidx[q]].w, P.rca, P.cutoff_kind);
+  __syncwarp();
+  // f2[a] * w = ex2(-(ca rbar - ca ShfA)^2 + lg2 w),  f1[z] = (0.5 + c (cz/2) + s (sz/2))^zeta
+  const float ca = sqrtf(P.eta_a * 1.4426950408889634f);
+  float cshfA[NA], hcz[NZ], hsz[NZ];
+#pragma unroll
+  for (int a = 0; a < NA; ++a) cshfA[a] = ca * P.shf_a[a];
+#pragma unroll
+  for (int z = 0; z < NZ; ++z) {
+    hcz[z] = 0.5f * P.cos_z[z];
+    hsz[z] = 0.5f * P.sin_z[z];
+  }
+  // walk the set bits of the element mask: pairs (s1, s2 >= s1) of present elements only
+  for (unsigned m1 = present & ((1u << S) - 1u); m1; m1 &= m1 - 1) {
+    const int s1 = __ffs(m1) - 1;
+    const int a0 = s.seg[s1], na = s.seg[s1 + 1] - a0;
+    const int pbase = s1 * (2 * S - s1 + 1) / 2 - s1;  // pair_index(s1, s2) = pbase + s2
+    for (unsigned m2 = m1; m2; m2 &= m2 - 1) {
+      const int s2 = __ffs(m2) - 1;
+      const int p = pbase + s2;
+      const int b0 = s.seg[s2], nb = s.seg[s2 + 1] - b0;
+      const int count = (s1 == s2) ? na * (na - 1) / 2 : na * nb;
+      float out = 0.f;
+      if (count > 0) {
+        float acc[32];
+#pragma unroll
+        for (int f = 0; f < 32; ++f) acc[f] = 0.f;
+        const float inv_nb = 1.0f / (float)nb;
+        for (int q = lane; q < count; q += 32) {
+          int ja, jb;
+          if (s1 == s2) {
+            // q-th pair (a < b) of the triangle: b = floor((1 + sqrt(1 + 8 q)) / 2), one fix-up each way
+            int bb = (int)(0.5f + 0.5f * fast_sqrt(1.0f + 8.0f * (float)q));
+            if (bb * (bb - 1) / 2 > q) --bb;
+            if ((bb + 1) * bb / 2 <= q) ++bb;
+            ja = a0 + q - bb * (bb - 1) / 2;
+            jb = a0 + bb;
+          } else {
+            // q / nb for q < 2^13, nb <= 96: the float quotient of (q + 0.5) is never within rounding of an integer
+            const int qa = (int)(((float)q + 0.5f) * inv_nb);
+            ja = a0 + qa;
+            jb = b0 + q - qa * nb;
+          }
+          const float4 dj = s.nd[s.aidx[ja]], dk = s.nd[s.aidx[jb]];
+          const float lw = fast_log2(2.0f * s.afc[ja] * s.afc[jb]);  // -inf at the cutoff: every term 0
+          const float dot = dj.x * dk.x + dj.y * dk.y + dj.z * dk.z;
+          const float c = 0.95f * dot * fast_rcp(fmaxf(dj.w * dk.w, 1e-10f));
+          const float sn = fast_sqrt(fmaxf(1.0f - c * c, 0.f));
+          const float rbar = ca * 0.5f * (dj.w + dk.w);
+          float f1[NZ];
+#pragma unroll
+          for (int z = 0; z < NZ; ++z) {
+            const float base = fmaxf(fmaf(sn, hsz[z], fmaf(c, hcz[z], 0.5f)), 0.f);
+            f1[z] = fast_exp2(P.zeta * fast_log2(base));  // base^zeta; base = 0 -> ex2(-inf) = 0
+          }
+#pragma unroll
+          for (int a = 0; a < NA; ++a) {
+            const float d = rbar - cshfA[a];
+            const float f2 = fast_exp2(fmaf(-d, d, lw));
+#pragma unroll
+            for (int z = 0; z < NZ; ++z) acc[a * NZ + z] = fmaf(f1[z], f2, acc[a * NZ + z]);
+          }
+        }
+        out = transpose_reduce32(acc, lane);
+      }
+      store(RL + (layout ? P.ang_pad : 0) + p * 32 + lane, out);
+    }
+  }
+  if (ANI_OPND_FP16X2 && !(store.vmax <= OPND_HALF_MAX)) atomicOr(status, ANI_STATUS_OPERAND_RANGE);
+  tr.mark(TR_ANGULAR);
+}
+
+// Stable regroup of a warp's first cnt neighbour rows (nd with r^2 in .w, nj, species nsp) into species-major order,
+// then the angular sub-list with one ballot per 32 regrouped neighbours: the input of atom_features as the CTA
+// kernel's compaction leaves it.  Each lane holds its rows in registers while they move (cnt <= nbr_cap <= 256); the
+// running place of every species is kept in seg until the angular segments overwrite it.  Returns the number of
+// angular neighbours (unclamped).
+__device__ __forceinline__ int group_by_species(const ani_aev_params& P, const WarpSmem& s, int cnt) {
+  constexpr int PER = 256 / 32;
+  const int lane = threadIdx.x & 31;
+  const unsigned lt = (1u << lane) - 1u;
+  int spv[PER];
+  int seg_start[ANI_MAX_SPECIES + 1];
+#pragma unroll
+  for (int e = 0; e <= ANI_MAX_SPECIES; ++e) seg_start[e] = 0;
+#pragma unroll
+  for (int k = 0; k < PER; ++k) {
+    const int n = k * 32 + lane;
+    spv[k] = n < cnt ? (int)s.nsp[n] : -1;
+    if (k * 32 < cnt) {
+#pragma unroll
+      for (int e = 0; e < ANI_MAX_SPECIES; ++e) seg_start[e + 1] += __popc(__ballot_sync(ANI_FULL_MASK, spv[k] == e));
+    }
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int e = 0; e < ANI_MAX_SPECIES; ++e) {
+      seg_start[e + 1] += seg_start[e];
+      s.seg[e] = seg_start[e];
+      if (e <= P.num_species) s.seg_all[e] = seg_start[e];
+    }
+    if (P.num_species == ANI_MAX_SPECIES) s.seg_all[ANI_MAX_SPECIES] = seg_start[ANI_MAX_SPECIES];
+  }
+  __syncwarp();
+  float4 d[PER];
+  int w[PER], dst[PER];
+#pragma unroll
+  for (int k = 0; k < PER; ++k) {
+    dst[k] = -1;
+    if (k * 32 < cnt) {
+      const int e = spv[k];
+      const bool placed = e >= 0 && e < ANI_MAX_SPECIES;
+      const unsigned peers = __match_any_sync(ANI_FULL_MASK, e);  // the lanes of this species, in lane order
+      if (placed) {
+        dst[k] = s.seg[e] + __popc(peers & lt);
+        d[k] = s.nd[k * 32 + lane];
+        w[k] = s.nj[k * 32 + lane];
+      }
+      __syncwarp();
+      if (placed && !(peers & lt)) s.seg[e] += __popc(peers);
+      __syncwarp();
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < PER; ++k)
+    if (dst[k] >= 0) {
+      s.nd[dst[k]] = d[k];
+      s.nj[dst[k]] = w[k];
+    }
+  __syncwarp();
+  // the angular sub-list: one ballot per 32 neighbours of the regrouped list; lane e < S counts the angular neighbours
+  // before the end of species segment e, the boundary seg[e + 1]
+  const float rca2 = P.rca * P.rca;
+  const int end = s.seg_all[P.num_species];
+  const int seg_end = lane < P.num_species ? s.seg_all[lane + 1] : 0;
+  int cnt_a = 0, below = 0;
+  for (int base = 0; base < end; base += 32) {
+    const int n = base + lane;
+    const bool keep_a = n < end && s.nd[n].w <= rca2;
+    const unsigned ma = __ballot_sync(ANI_FULL_MASK, keep_a);
+    const int pa = cnt_a + __popc(ma & lt);
+    if (keep_a && pa < ANI_MAX_ANG) s.aidx[pa] = (unsigned char)n;
+    cnt_a += __popc(ma);
+    const int before = seg_end - base;
+    below += __popc(ma & (before >= 32 ? 0xffffffffu : before <= 0 ? 0u : (1u << before) - 1u));
+  }
+  if (lane < P.num_species) s.seg[lane + 1] = min(below, ANI_MAX_ANG);
+  if (lane == 0) s.seg[0] = 0;
+  __syncwarp();
+  return cnt_a;
+}
+
+// Warp-per-atom forward (explicit neighbour rows, and the bucket grid with ANI_B200_AEV_LEGACY=1): every warp gathers
+// its own neighbours -- the caller's rows, or its bucket's 27 candidate ranges walked in global memory in range order
+// -- regroups them by species and evaluates the shared tail.  On the bucket grid the neighbours come out in the order
+// of k_aev_forward_cta (species, range, position), so both kernels give the same bits unless nbr_cap overflows.
+// LAT (grid mode 3): image shifts in the lattice of the bucket's conformer (lattice table); the range table, when
+// given, already holds them
+template <int NA, int NZ, bool LAT = false>
+__global__ void __launch_bounds__(AEV_WARPS * 32)
+    k_aev_forward(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
+                  const int32_t* __restrict__ bin_start, const float4* __restrict__ spos,
+                  const int32_t* __restrict__ sbin, const float4* __restrict__ ranges,
+                  const int32_t* __restrict__ species_mask, const ExplicitNbrs ex, int lo, int hi,
+                  const int32_t* __restrict__ row_of,
+                  float* __restrict__ aev, int ldx, int layout, int32_t* __restrict__ nbr_cnt,
+                  int32_t* __restrict__ nbr_list, int cap, int32_t* __restrict__ status, size_t warp_bytes,
+                  const float* __restrict__ lattice) {
+  static_assert(NA * NZ == 32, "one lane per angular feature");
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  AevTrace tr;  // (the phase trace records k_aev_forward_cta only: nothing is written)
+  tr.start();
+  const ani_grid g = *grid;
+  hi = min(hi, g.n_real);
+  const int i = lo + blockIdx.x * AEV_WARPS + warp;
+  if (i >= hi) return;
+  const WarpSmem s = carve(smem_raw + warp * warp_bytes, cap, false);
+  const float4 pi = spos[i];
+  if (__float_as_int(pi.w) < 0) return;  // padding atom (only reachable with explicit neighbour rows)
+  int cnt = 0;
+  if (ex.start) {
+    // neighbours handed in by the caller (already screened to Rcr): copy the row
+    const int e0 = ex.start[i];
+    cnt = ex.start[i + 1] - e0;
+    for (int n = lane; n < min(cnt, cap); n += 32) {
+      const int j = ex.j[e0 + n];
+      const float4 d = ex.d[e0 + n];
+      s.nd[n] = make_float4(d.x, d.y, d.z, norm2(d.x, d.y, d.z));
+      s.nj[n] = j | (13 << ANI_IMG_SHIFT);
+      s.nsp[n] = (unsigned char)__float_as_int(spos[j].w);
+    }
+  } else {
+    // lane o holds the record of candidate range o; the warp compacts the atoms within Rcr range after range
+    const float rcr2 = P.rcr * P.rcr;
+    const unsigned lt = (1u << lane) - 1u;
+    RangeRecord r{};
+    if (lane < NRANGE) r = bucket_range<LAT>(g, bin_start, ranges, lattice, sbin[i], lane);
+    for (int o = 0; o < NRANGE; ++o) {
+      const int rlo = __shfl_sync(ANI_FULL_MASK, r.lo, o), rhi = __shfl_sync(ANI_FULL_MASK, r.hi, o);
+      if (rhi <= rlo) continue;
+      const int code = __shfl_sync(ANI_FULL_MASK, r.code, o);
+      const float shx = __shfl_sync(ANI_FULL_MASK, r.shift.x, o), shy = __shfl_sync(ANI_FULL_MASK, r.shift.y, o),
+                  shz = __shfl_sync(ANI_FULL_MASK, r.shift.z, o);
+      for (int base = rlo; base < rhi; base += 32) {
+        const int c = base + lane;
+        const bool valid = c < rhi;
+        const float4 p = valid ? spos[c] : pi;
+        const float dx = (p.x + shx) - pi.x, dy = (p.y + shy) - pi.y, dz = (p.z + shz) - pi.z;
+        const float r2 = norm2(dx, dy, dz);
+        const bool keep = valid && r2 <= rcr2 && !(c == i && code == 13);
+        const unsigned m = __ballot_sync(ANI_FULL_MASK, keep);
+        const int pos = cnt + __popc(m & lt);
+        if (keep && pos < cap) {
+          s.nd[pos] = make_float4(dx, dy, dz, r2);
+          s.nj[pos] = c | (code << ANI_IMG_SHIFT);
+          s.nsp[pos] = (unsigned char)__float_as_int(p.w);
+        }
+        cnt += __popc(m);
+      }
+    }
+  }
+  __syncwarp();
+  const int cnt_a = group_by_species(P, s, min(cnt, cap));
+  atom_features<NA, NZ>(P, s, i, cnt, cnt_a, species_mask, row_of, aev, ldx, layout, nbr_cnt, nbr_list, cap, status,
+                        tr);
+}
+
+// ---------------------------------------------------------------------------------------
+// forward, CTA-staged neighbourhood (the bucket-grid path)
+//
+// The AEV_WARPS consecutive (bucket-sorted) atoms of a CTA almost always share one bucket, so the
+// candidates of its 27 neighbouring buckets are staged ONCE per CTA in shared memory -- shifted by
+// their lattice image and ordered species-major (the buckets are species-sorted, so the place of
+// every candidate follows from a 27 x S table of counts) -- instead of every warp walking the 27
+// ranges in global memory.  A warp then compacts its neighbours with one ballot per 32 candidates,
+// species segment by species segment: the neighbour list and the angular sub-list come out
+// grouped by species, ready for atom_features.
+// CTAs that straddle a bucket boundary run one staging phase per distinct bucket; neighbourhoods
+// larger than CAND_CAP candidates are staged in windows of the species-major order.
+// ---------------------------------------------------------------------------------------
+struct CtaStage {
+  float4 cand[CAND_CAP];  // shifted position; .w = neighbour word (sorted index | image code << 26)
+  float4 r_shift[NRANGE];
+  int r_lo[NRANGE], r_code[NRANGE];
+  int r_len[NRANGE];                           // candidates of every range
+  int r_off[NRANGE + 1];                       // exclusive prefix of the range lengths
+  int cnt[ANI_MAX_SPECIES][NRANGE];            // candidates per (species, range)
+  int off[ANI_MAX_SPECIES * NRANGE + 1];       // exclusive prefix of cnt in species-major order
+  int adj[ANI_MAX_SPECIES][NRANGE];            // off[s][o] - (candidates of lower species in range o)
+  int wbin[AEV_FWD_WARPS];
+  unsigned char t2o[T2O_CAP];                  // range of the t-th candidate (range-major numbering)
+  unsigned long long tma_bar;                  // mbarrier of the TMA bulk copies that stage the bucket ranges
+};
+
 template <int NA, int NZ, bool TMA_STAGE = false, bool LAT = false>
 __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
     k_aev_forward_cta(const __grid_constant__ ani_aev_params P, const ani_grid* __restrict__ grid,
@@ -666,8 +705,6 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
   const bool has = i < hi;  // warps without an atom still help with the staging
   const WarpSmem s = carve(smem_raw + warp * warp_bytes, cap, false);
   const int S = P.num_species;
-  const int nR = P.n_shf_r;
-  const int RL = S * nR;
   float4 pi = make_float4(0.f, 0.f, 0.f, 0.f);
   int myb = 0x7fffffff;
   if (has) {
@@ -703,47 +740,18 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
     __syncthreads();  // every warp has chosen `cur`; the tables of the previous phase may be rewritten
     // (a) the 27 candidate ranges of bucket `cur`
     if (tid < NRANGE) {
-      int rlo = 0, rhi = 0, code = 13, nbk = cur;
-      float4 sh = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (g.mode == 1) {   // bucket == conformer
-        if (tid == 13) {
-          rlo = bin_start[cur];
-          rhi = bin_start[cur + 1];
-        }
-      } else if (ranges) {
-        const float4 r0 = ranges[2 * ((size_t)cur * NRANGE + tid)];
-        const float4 r1 = ranges[2 * ((size_t)cur * NRANGE + tid) + 1];
-        rlo = __float_as_int(r0.x);
-        rhi = __float_as_int(r0.y);
-        code = __float_as_int(r0.z);
-        nbk = __float_as_int(r0.w);
-        sh = r1;
-      } else {
-        int ix, iy, iz;
-        const int base = bucket_coords(g, cur, ix, iy, iz);
-        NeighbourRange r;
-        if (neighbour_bucket(g, bin_start, base, ix, iy, iz, tid / 9 - 1, (tid / 3) % 3 - 1, tid % 3 - 1, r)) {
-          rlo = r.lo;
-          rhi = r.hi;
-          code = r.code;
-          if (code != 13) {
-            const float3 v = LAT ? image_shift(lattice, base / (g.dims[0] * g.dims[1] * g.dims[2]), code)
-                                 : image_shift(g, code);
-            sh = make_float4(v.x, v.y, v.z, 0.f);
-          }
-        }
-      }
-      C.r_lo[tid] = rlo;
-      C.r_code[tid] = code;
-      C.r_shift[tid] = sh;
-      const int len = max(rhi - rlo, 0);
+      const RangeRecord r = bucket_range<LAT>(g, bin_start, ranges, lattice, cur, tid);
+      C.r_lo[tid] = r.lo;
+      C.r_code[tid] = r.code;
+      C.r_shift[tid] = make_float4(r.shift.x, r.shift.y, r.shift.z, 0.f);
+      const int len = max(r.hi - r.lo, 0);
       C.r_len[tid] = len;
       if (use_bss) {
         // candidates per (species, range) straight from the per-bucket species offsets of the preparation kernel
         // (buckets are species-sorted): no counting pass over the candidates, no shared-memory atomics
         int off8[ANI_MAX_SPECIES + 1];
         if (len > 0) {
-          const int4 q0 = reinterpret_cast<const int4*>(bss)[2 * (size_t)nbk], q1 = reinterpret_cast<const int4*>(bss)[2 * (size_t)nbk + 1];
+          const int4 q0 = reinterpret_cast<const int4*>(bss)[2 * (size_t)r.bucket], q1 = reinterpret_cast<const int4*>(bss)[2 * (size_t)r.bucket + 1];
           off8[0] = q0.x; off8[1] = q0.y; off8[2] = q0.z; off8[3] = q0.w;
           off8[4] = q1.x; off8[5] = q1.y; off8[6] = q1.z; off8[7] = q1.w;
           off8[ANI_MAX_SPECIES] = len;
@@ -904,7 +912,7 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
             const float4 p = C.cand[valid ? idx - F0 : 0];
             const int word = __float_as_int(p.w);
             const float dx = p.x - pi.x, dy = p.y - pi.y, dz = p.z - pi.z;
-            const float r2 = dx * dx + dy * dy + dz * dz;
+            const float r2 = norm2(dx, dy, dz);
             const bool keep = valid && r2 <= rcr2 && word != (i | (13 << ANI_IMG_SHIFT));
             const unsigned m = __ballot_sync(ANI_FULL_MASK, keep);
             const int pos = cnt + __popc(m & lt);
@@ -937,150 +945,8 @@ __global__ void __launch_bounds__(AEV_FWD_WARPS * 32, ANI_AEV_FWD_MIN_CTAS)
     }
   }
   if (!has) return;
-  if (cnt > cap) {
-    if (lane == 0) atomicOr(status, ANI_STATUS_NBR_OVERFLOW);
-    cnt = cap;
-  }
-  if (cnt_a > ANI_MAX_ANG) {
-    if (lane == 0) atomicOr(status, ANI_STATUS_ANG_OVERFLOW);
-    cnt_a = ANI_MAX_ANG;
-  }
-  __syncwarp();
-
-  // output: plain row-major rows, or the tiled operand layout (16-bit pieces) the GEMM consumes
-  const int out_row = row_of[i];
-  const int kblocks = ldx >> 5;
-  float vmax = 0.f;
-  auto store_feature = [&](int col, float v) {
-    if (layout == 0) {
-      aev[(size_t)out_row * ldx + col] = v;
-    } else {
-      unsigned char* dst = reinterpret_cast<unsigned char*>(aev) + opnd_offset(out_row, col, kblocks);
-      unsigned short pc[OPND_PARTS];
-      v *= OPND_SCALE_VALUE;
-      vmax = fmaxf(vmax, v);
-      opnd_split(v, pc);
-#pragma unroll
-      for (int k = 0; k < OPND_PARTS; ++k) *reinterpret_cast<unsigned short*>(dst + k * OPND_PART_BYTES) = pc[k];
-    }
-  };
-
-  if (lane == 0 && nbr_cnt) nbr_cnt[i] = cnt;
-  // per neighbour: (c R, fc(R)) with c = sqrt(eta_r log2 e), so that a Gaussian factor is
-  // ex2(-(c R - c ShfR)^2); the neighbour words go to the list the backward kernel reads
-  const float cr = sqrtf(P.eta_r * 1.4426950408889634f);
-  if (nbr_list)
-    for (int n = lane; n < cnt; n += 32) nbr_list[(size_t)i * cap + n] = s.nj[n];
-  __syncwarp();
-  // [cap] float2 over nfc and nj (adjacent, 8-byte aligned; the words were just copied out)
-  float2* rf = reinterpret_cast<float2*>(s.nfc);
-  for (int n = lane; n < cnt; n += 32) {
-    const float R = sqrtf(s.nd[n].w);
-    s.nd[n].w = R;
-    rf[n] = make_float2(cr * R, cutoff_value(R, P.rcr, P.cutoff_kind));
-  }
-  __syncwarp();
-  tr.mark(TR_LIST);
-
-  // element pairs / elements that do not occur anywhere in the system are never read by the MLP:
-  // skip them (species_mask[1] != 0: the composition changed since the last call -> write them once)
-  const unsigned present = (species_mask && !species_mask[1]) ? (unsigned)species_mask[0] : 0xffffffffu;
-
-  // ---- 2. radial block: lane = (shift m, neighbour parity h); one species segment at a time, the
-  //         (species, shift) sum lives in a register: no shared-memory accumulators, no atomics
-  {
-    const int lpn = (nR <= 16) ? 16 : 32;
-    const int halves = 32 / lpn;
-    const int m = lane % lpn, h = lane / lpn;
-    const float cshf = cr * P.shf_r[m < nR ? m : 0];
-    for (int sp = 0; sp < S; ++sp) {
-      if (!((present >> sp) & 1u)) continue;
-      const int k1 = s.seg_all[sp + 1];
-      float acc = 0.f;
-#pragma unroll 2
-      for (int k = s.seg_all[sp] + h; k < k1; k += halves) {
-        const float2 v = rf[k];
-        const float d = v.x - cshf;
-        acc = fmaf(fast_exp2(-d * d), v.y, acc);
-      }
-      if (halves == 2) acc += __shfl_xor_sync(ANI_FULL_MASK, acc, 16);
-      if (h == 0 && m < nR) store_feature(sp * nR + m, 0.25f * acc);
-    }
-  }
-  tr.mark(TR_RADIAL);
-
-  // ---- 3. angular block
-  const int n_ang = cnt_a;
-  for (int q = lane; q < n_ang; q += 32) s.afc[q] = cutoff_value(s.nd[s.aidx[q]].w, P.rca, P.cutoff_kind);
-  __syncwarp();
-  // f2[a] * w = ex2(-(ca rbar - ca ShfA)^2 + lg2 w),  f1[z] = (0.5 + c (cz/2) + s (sz/2))^zeta
-  const float ca = sqrtf(P.eta_a * 1.4426950408889634f);
-  float cshfA[NA], hcz[NZ], hsz[NZ];
-#pragma unroll
-  for (int a = 0; a < NA; ++a) cshfA[a] = ca * P.shf_a[a];
-#pragma unroll
-  for (int z = 0; z < NZ; ++z) {
-    hcz[z] = 0.5f * P.cos_z[z];
-    hsz[z] = 0.5f * P.sin_z[z];
-  }
-  // walk the set bits of the element mask: pairs (s1, s2 >= s1) of present elements only
-  for (unsigned m1 = present & ((1u << S) - 1u); m1; m1 &= m1 - 1) {
-    const int s1 = __ffs(m1) - 1;
-    const int a0 = s.seg[s1], na = s.seg[s1 + 1] - a0;
-    const int pbase = s1 * (2 * S - s1 + 1) / 2 - s1;  // pair_index(s1, s2) = pbase + s2
-    for (unsigned m2 = m1; m2; m2 &= m2 - 1) {
-      const int s2 = __ffs(m2) - 1;
-      const int p = pbase + s2;
-      const int b0 = s.seg[s2], nb = s.seg[s2 + 1] - b0;
-      const int count = (s1 == s2) ? na * (na - 1) / 2 : na * nb;
-      float out = 0.f;
-      if (count > 0) {
-        float acc[32];
-#pragma unroll
-        for (int f = 0; f < 32; ++f) acc[f] = 0.f;
-        const float inv_nb = 1.0f / (float)nb;
-        for (int q = lane; q < count; q += 32) {
-          int ja, jb;
-          if (s1 == s2) {
-            // q-th pair (a < b) of the triangle: b = floor((1 + sqrt(1 + 8 q)) / 2), one fix-up each way
-            int bb = (int)(0.5f + 0.5f * fast_sqrt(1.0f + 8.0f * (float)q));
-            if (bb * (bb - 1) / 2 > q) --bb;
-            if ((bb + 1) * bb / 2 <= q) ++bb;
-            ja = a0 + q - bb * (bb - 1) / 2;
-            jb = a0 + bb;
-          } else {
-            // q / nb for q < 2^13, nb <= 96: the float quotient of (q + 0.5) is never within rounding of an integer
-            const int qa = (int)(((float)q + 0.5f) * inv_nb);
-            ja = a0 + qa;
-            jb = b0 + q - qa * nb;
-          }
-          const float4 dj = s.nd[s.aidx[ja]], dk = s.nd[s.aidx[jb]];
-          const float lw = fast_log2(2.0f * s.afc[ja] * s.afc[jb]);  // -inf at the cutoff: every term 0
-          const float dot = dj.x * dk.x + dj.y * dk.y + dj.z * dk.z;
-          const float c = 0.95f * dot * fast_rcp(fmaxf(dj.w * dk.w, 1e-10f));
-          const float sn = fast_sqrt(fmaxf(1.0f - c * c, 0.f));
-          const float rbar = ca * 0.5f * (dj.w + dk.w);
-          float f1[NZ];
-#pragma unroll
-          for (int z = 0; z < NZ; ++z) {
-            const float base = fmaxf(fmaf(sn, hsz[z], fmaf(c, hcz[z], 0.5f)), 0.f);
-            f1[z] = fast_exp2(P.zeta * fast_log2(base));  // base^zeta; base = 0 -> ex2(-inf) = 0
-          }
-#pragma unroll
-          for (int a = 0; a < NA; ++a) {
-            const float d = rbar - cshfA[a];
-            const float f2 = fast_exp2(fmaf(-d, d, lw));
-#pragma unroll
-            for (int z = 0; z < NZ; ++z) acc[a * NZ + z] = fmaf(f1[z], f2, acc[a * NZ + z]);
-          }
-        }
-        out = transpose_reduce32(acc, lane);
-      }
-      store_feature(RL + (layout ? P.ang_pad : 0) + p * 32 + lane, out);
-    }
-  }
-  if (ANI_OPND_FP16X2 && !(vmax <= OPND_HALF_MAX)) atomicOr(status, ANI_STATUS_OPERAND_RANGE);
-  tr.mark(TR_ANGULAR);
+  atom_features<NA, NZ>(P, s, i, cnt, cnt_a, species_mask, row_of, aev, ldx, layout, nbr_cnt, nbr_list, cap, status,
+                        tr);
   tr.write((size_t)(i - lo), lane);
 }
 
@@ -1656,6 +1522,20 @@ static int check_params(const ani_aev_params* p) {
   return ANI_OK;
 }
 
+// the template instance of an AEV kernel for the angular shape (ShfA x ShfZ) and grid mode 3 (lattice table)
+template <int NA_, bool LAT_>
+struct AevShape {
+  static constexpr int NA = NA_, NZ = 32 / NA_;
+  static constexpr bool LAT = LAT_;
+};
+template <class F>
+static void dispatch_shape(const ani_aev_params* params, bool lattice, F&& f) {
+  if (params->n_shf_a == 8)
+    lattice ? f(AevShape<8, true>{}) : f(AevShape<8, false>{});
+  else
+    lattice ? f(AevShape<4, true>{}) : f(AevShape<4, false>{});
+}
+
 // ---- launchers shared by the bucket-grid and the explicit-pair-list entry points -----------
 static int launch_aev_forward(const ani_aev_params* params, const ani_grid* grid, const int32_t* bin_start,
                               const float* spos, const int32_t* sbin, const float* bucket_ranges,
@@ -1674,10 +1554,7 @@ static int launch_aev_forward(const ani_aev_params* params, const ani_grid* grid
   if (layout != 0 && layout != 1) return ANI_ERR_BAD_ARG;
   if (layout == 1 && ldx % 32) return ANI_ERR_BAD_ARG;
   if (hi == lo) return ANI_OK;
-  const int RL = params->num_species * params->n_shf_r;
   const size_t wb = warp_smem_bytes(nbr_cap, 0, false);
-  const size_t smem = wb * AEV_WARPS;
-  const int blocks = (hi - lo + AEV_WARPS - 1) / AEV_WARPS;
   cudaStream_t st = (cudaStream_t)stream;
   const float4* sp4 = reinterpret_cast<const float4*>(spos);
   const float4* rng4 = reinterpret_cast<const float4*>(bucket_ranges);
@@ -1695,57 +1572,25 @@ static int launch_aev_forward(const ani_aev_params* params, const ani_grid* grid
     const char* e = getenv("ANI_B200_AEV_TMA");
     return e && atoi(e) != 0 ? 1 : 0;
   }();
-  if (!ex.start && !legacy) {
-    const size_t smem_f = wb * AEV_FWD_WARPS;
-    const int blocks_f = (hi - lo + AEV_FWD_WARPS - 1) / AEV_FWD_WARPS;
-    auto go = [&](auto k) {
-      cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_f);
-      k<<<blocks_f, AEV_FWD_WARPS * 32, smem_f, st>>>(*params, grid, bin_start, sp4, sbin, rng4, species_mask, lo, hi,
-                                                      row_of, aev, ldx, layout, nbr_cnt, nbr_list, nbr_cap, status, wb,
-                                                      tma_stage, bucket_species, lattice);
-    };
-    if (lattice) {   // grid mode 3
-      if (params->n_shf_a == 8) {
-        if (tma_stage)
-          go(k_aev_forward_cta<8, 4, true, true>);
-        else
-          go(k_aev_forward_cta<8, 4, false, true>);
-      } else {
-        if (tma_stage)
-          go(k_aev_forward_cta<4, 8, true, true>);
-        else
-          go(k_aev_forward_cta<4, 8, false, true>);
-      }
-    } else if (params->n_shf_a == 8) {
-      if (tma_stage)
-        go(k_aev_forward_cta<8, 4, true>);
-      else
-        go(k_aev_forward_cta<8, 4, false>);
-    } else {
-      if (tma_stage)
-        go(k_aev_forward_cta<4, 8, true>);
-      else
-        go(k_aev_forward_cta<4, 8, false>);
-    }
-    ANI_CUDA_CHECK_LAUNCH();
-    return ANI_OK;
-  }
-  auto go = [&](auto k) {
+  const bool staged = !ex.start && !legacy;
+  const int warps = staged ? AEV_FWD_WARPS : AEV_WARPS;
+  const size_t smem = wb * warps;
+  const int blocks = (hi - lo + warps - 1) / warps;
+  auto go = [&](auto k, auto... args) {
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k<<<blocks, AEV_WARPS * 32, smem, st>>>(*params, grid, bin_start, sp4, sbin, rng4, species_mask, ex, lo, hi, row_of,
-                                            aev, ldx, layout, nbr_cnt, nbr_list, nbr_cap, status, wb, lattice);
+    k<<<blocks, warps * 32, smem, st>>>(args...);
   };
-  if (params->n_shf_a == 8) {
-    if (lattice)
-      go(k_aev_forward<8, 4, true>);
-    else
-      go(k_aev_forward<8, 4>);
-  } else {
-    if (lattice)
-      go(k_aev_forward<4, 8, true>);
-    else
-      go(k_aev_forward<4, 8>);
-  }
+  dispatch_shape(params, lattice != nullptr, [&](auto sh) {
+    using Sh = decltype(sh);
+    if (staged) {
+      auto k = tma_stage ? k_aev_forward_cta<Sh::NA, Sh::NZ, true, Sh::LAT> : k_aev_forward_cta<Sh::NA, Sh::NZ, false, Sh::LAT>;
+      go(k, *params, grid, bin_start, sp4, sbin, rng4, species_mask, lo, hi, row_of, aev, ldx, layout, nbr_cnt,
+         nbr_list, nbr_cap, status, wb, tma_stage, bucket_species, lattice);
+    } else {
+      go(k_aev_forward<Sh::NA, Sh::NZ, Sh::LAT>, *params, grid, bin_start, sp4, sbin, rng4, species_mask, ex, lo, hi,
+         row_of, aev, ldx, layout, nbr_cnt, nbr_list, nbr_cap, status, wb, lattice);
+    }
+  });
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
 }
@@ -1783,20 +1628,6 @@ static GradTable grad_table(const ani_aev_params* params, const int32_t* species
   return GradTable{pair_cap, ((RL + 3) & ~3) + GSTRIDE * pair_cap};
 }
 
-// the template instance of a backward kernel for the angular shape (ShfA x ShfZ) and grid mode 3 (lattice table)
-template <int NA_, bool LAT_>
-struct BackwardShape {
-  static constexpr int NA = NA_, NZ = 32 / NA_;
-  static constexpr bool LAT = LAT_;
-};
-template <class F>
-static void dispatch_backward(const ani_aev_params* params, bool lattice, F&& f) {
-  if (params->n_shf_a == 8)
-    lattice ? f(BackwardShape<8, true>{}) : f(BackwardShape<8, false>{});
-  else
-    lattice ? f(BackwardShape<4, true>{}) : f(BackwardShape<4, false>{});
-}
-
 static int launch_aev_backward(const ani_aev_params* params, const ani_grid* grid, const float* spos,
                                const int32_t* sorted_orig, int n, int lo, int hi, const int32_t* row_of,
                                const float* grad_aev, int ldx, const int32_t* nbr_cnt, const int32_t* nbr_list,
@@ -1819,7 +1650,7 @@ static int launch_aev_backward(const ani_aev_params* params, const ani_grid* gri
                                             nbr_list, ex, species_mask, nbr_cap, grad_coords, status, wb, t.pair_cap,
                                             virial, lattice);
   };
-  dispatch_backward(params, lattice, [&](auto sh) {
+  dispatch_shape(params, lattice, [&](auto sh) {
     using Sh = decltype(sh);
     if (virial)
       go(k_aev_backward<Sh::NA, Sh::NZ, true, Sh::LAT>);
@@ -1857,7 +1688,7 @@ static int launch_aev_backward_members(const ani_aev_params* params, const ani_g
   const int blocks = (hi - lo + AEV_WARPS - 1) / AEV_WARPS;
   cudaStream_t st = (cudaStream_t)stream;
   const float4* sp4 = reinterpret_cast<const float4*>(spos);
-  dispatch_backward(params, lattice, [&](auto sh) {
+  dispatch_shape(params, lattice, [&](auto sh) {
     using Sh = decltype(sh);
     auto k = k_aev_backward_members<Sh::NA, Sh::NZ, Sh::LAT>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
