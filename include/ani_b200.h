@@ -30,6 +30,8 @@
  *   ani_b200_pair_potential     potentials/core.py:106-207, potentials/xtb.py:57-77, potentials/zbl.py:68-81
  *                               (RepulsionXTB / RepulsionZBL over the step's own neighbour list); _pairs: over a
  *                               caller-supplied half list, with ghost weights
+ *   ani_b200_dispersion_d3      potentials/dftd3.py:102-311 (TwoBodyDispersionD3, D3(BJ) two-body dispersion with its
+ *                               own neighbour search); _pairs: over a caller-supplied half list, with ghost weights
  *   ani_b200_operand_format     (no counterpart: format of the tensor-core GEMM operands of this build)
  */
 #ifndef ANI_B200_H
@@ -322,6 +324,60 @@ int ani_b200_pair_potential_pairs(const ani_pair_params* params, const int32_t* 
                                   const int64_t* idx1, const float* distances, const float* diff_vectors,
                                   const uint8_t* ghost_flags, int64_t num_pairs, int n_conf, int n_per_conf,
                                   float* atomic, double* energies, float* grad_coords, void* stream);
+
+/* 4h. D3(BJ) two-body dispersion (potentials/dftd3.py:140-311, TwoBodyDispersionD3) with its own neighbour search    */
+/*    over the step's bucket grid (its cutoff, 8 A in the reference's models, is beyond Rcr).  With d = R * to_bohr:       */
+/*      CN_i  = sum_j 1 / (1 + exp(-k1 (k2 (rcov[s_i] + rcov[s_j]) / d - 1)))     (every pair within the cutoff)          */
+/*      C6_ij = (sum_pq C6ref_pq L_pq + 1e-35) / (sum_pq L_pq + 1e-35),  over the pq with C6ref_pq > 0,              */
+/*              L_pq = exp(-k3 ((CN_i - CNa_pq)^2 + (CN_j - CNb_pq)^2))  (the largest L is factored out of both sums and */
+/*              the 1e-35; no positive C6ref: C6 = 1, dC6/dCN = 0)                                                        */
+/*      E_ij  = -(s6 C6 / (d^6 + damp6) + s8 c8_scale C6 / (d^8 + damp8)) fc(R; cutoff)                                  */
+/*    damp6/8[s][t] = (a1 R0_st + a2)^6/8 (Bohr^6/8), c8_scale[s][t] = 3 sqrt_charge_st; cutoff_fn as ani_pair_params.   */
+/*    a1, a2 are informational (damp6/8 are what the kernels read).  Tables: device f32[S][S][25][4], per element pair   */
+/*    (s, t) and reference pair (p, q) = 5 p + q the values {C6ref, CNa, CNb, 0} (precalc_coeff6, precalc_coordnums_a/b). */
+typedef struct ani_d3_params {
+  int32_t cutoff_fn, num_species;
+  float cutoff;  /* Angstrom */
+  float to_bohr; /* Angstrom -> Bohr */
+  float s6, s8, a1, a2;
+  float k1, k2, k3, pad_;
+  float rcov[ANI_MAX_SPECIES]; /* Bohr */
+  float damp6[ANI_MAX_SPECIES][ANI_MAX_SPECIES];
+  float damp8[ANI_MAX_SPECIES][ANI_MAX_SPECIES];
+  float c8_scale[ANI_MAX_SPECIES][ANI_MAX_SPECIES];
+} ani_d3_params;
+
+/*    ani_b200_dispersion_d3 evaluates the term for the grid of ani_b200_prepare_step (bin_start, spos, sorted_orig of     */
+/*    that preparation; cutoff_fn 0 or 1, a finite cutoff).  Per lattice direction the search reaches                     */
+/*    ceil((cutoff + skin) / bucket width) buckets; a neighbour inside the cutoff at two images counts twice.  Periodic   */
+/*    widths must be >= cutoff + skin, else ANI_STATUS_CELL_TOO_SMALL is OR-ed into status and nothing else is written.   */
+/*    Three launches: cn (f32[n], scratch) of every real atom, then dedcn (f32[n], scratch) of every real atom together   */
+/*    with the energies / direct gradient / direct virial of the owned atoms lo..hi-1, then (only if grad_coords,         */
+/*    grad_members or virial is given) the coordination-number chain of the gradient and virial of the owned atoms.      */
+/*    Outputs, add-only contract and member rules are those of ani_b200_pair_potential (4g): plain read-modify-write of    */
+/*    atomic, grad_coords, member_atomic, grad_members by the atom's owner; float64 atomics into energies and the virial  */
+/*    slots.  The per-rank results of a sharded run add up to the full answer (cn and dedcn are computed on every rank).  */
+/*    The _cells form is for grid mode 3 and takes its lattice table (not NULL).                                          */
+int ani_b200_dispersion_d3(const ani_d3_params* params, const float* tables, const ani_grid* grid,
+                           const int32_t* bin_start, const float* spos, const int32_t* sorted_orig, int n, int lo,
+                           int hi, int n_conf, int n_per_conf, float skin, float* cn, float* dedcn, float* atomic,
+                           double* energies, float* grad_coords, double* virial, float* member_atomic,
+                           float* grad_members, const int32_t* members, int n_members, int32_t* status, void* stream);
+int ani_b200_dispersion_d3_cells(const ani_d3_params* params, const float* tables, const ani_grid* grid,
+                                 const int32_t* bin_start, const float* spos, const int32_t* sorted_orig, int n, int lo,
+                                 int hi, int n_conf, int n_per_conf, float skin, float* cn, float* dedcn, float* atomic,
+                                 double* energies, float* grad_coords, double* virial, float* member_atomic,
+                                 float* grad_members, const int32_t* members, int n_members, int32_t* status,
+                                 const float* lattice, void* stream);
+/*    The same term over a caller-supplied HALF pair list (conventions of ani_b200_pair_potential_pairs; cutoff_fn 2 =   */
+/*    no envelope and no cutoff).  A pair that touches a ghost atom counts half in the energy and fully in the           */
+/*    coordination numbers.  cn, dedcn: f32[n] scratch (zeroed here; dedcn may be NULL without grad_coords).  Three       */
+/*    launches (two without grad_coords), float atomics; not the hot path.                                              */
+int ani_b200_dispersion_d3_pairs(const ani_d3_params* params, const float* tables, const int32_t* species,
+                                 const int64_t* idx0, const int64_t* idx1, const float* distances,
+                                 const float* diff_vectors, const uint8_t* ghost_flags, int64_t num_pairs, int n_conf,
+                                 int n_per_conf, float* cn, float* dedcn, float* atomic, double* energies,
+                                 float* grad_coords, void* stream);
 
 /* 4b. The same AEV kernels fed by an externally supplied HALF pair list (the reference's    */
 /*    Neighbors tuple; AEVComputer.compute_from_neighbors, aev/_computer.py:251-272 ->          */

@@ -78,9 +78,22 @@ class PairParams(C.Structure):
     ]
 
 
+class D3Params(C.Structure):
+    _fields_ = [
+        ("cutoff_fn", C.c_int32), ("num_species", C.c_int32), ("cutoff", C.c_float), ("to_bohr", C.c_float),
+        ("s6", C.c_float), ("s8", C.c_float), ("a1", C.c_float), ("a2", C.c_float),
+        ("k1", C.c_float), ("k2", C.c_float), ("k3", C.c_float), ("pad_", C.c_float),
+        ("rcov", C.c_float * ANI_MAX_SPECIES),
+        ("damp6", C.c_float * ANI_MAX_SPECIES * ANI_MAX_SPECIES),
+        ("damp8", C.c_float * ANI_MAX_SPECIES * ANI_MAX_SPECIES),
+        ("c8_scale", C.c_float * ANI_MAX_SPECIES * ANI_MAX_SPECIES),
+    ]
+
+
 _P = C.c_void_p
 _I = C.c_int
 _F = C.c_float
+_D3_ARGS = [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P]
 _PAIR_ARGS = [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I]
 
 _PROTOTYPES = {
@@ -113,6 +126,10 @@ _PROTOTYPES = {
     "ani_b200_pair_potential": (C.c_int, _PAIR_ARGS + [_P]),
     "ani_b200_pair_potential_cells": (C.c_int, _PAIR_ARGS + [_P, _P]),
     "ani_b200_pair_potential_pairs": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int64, _I, _I, _P, _P, _P, _P]),
+    "ani_b200_dispersion_d3": (C.c_int, _D3_ARGS + [_P]),
+    "ani_b200_dispersion_d3_cells": (C.c_int, _D3_ARGS + [_P, _P]),
+    "ani_b200_dispersion_d3_pairs": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _I, _I, _P, _P, _P, _P, _P,
+                                               _P]),
     "ani_b200_verlet_positions":(C.c_int, [_I, _P, _P, _P, _I, _F, _P, _P, _P, _P, _P, _I, _P, _I, _P]),
     "ani_b200_debug_gemm_trace": (C.c_int, [_P, _I]),
     "ani_b200_debug_aev_trace": (C.c_int, [_P]),

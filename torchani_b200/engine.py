@@ -20,7 +20,7 @@ import torch
 from torch import Tensor
 
 from . import _lib
-from ._lib import AEVParams, Grid, MLPModel, PairParams, check, ptr
+from ._lib import AEVParams, D3Params, Grid, MLPModel, PairParams, check, ptr
 
 TILE = _lib.ANI_TILE_ROWS
 
@@ -535,10 +535,13 @@ class Engine:
     bucket-sorted atoms this engine owns (multi-GPU sharding, see parallel.py)."""
 
     def __init__(self, consts: AEVConstants, nets: PackedNetworks, sae: tp.Optional[tp.Sequence[float]] = None,
-                 nbr_cap: int = 128, cuda_graph: bool = True, pairs: tp.Sequence[PairParams] = ()):
+                 nbr_cap: int = 128, cuda_graph: bool = True, pairs: tp.Sequence[PairParams] = (),
+                 dispersion: tp.Optional[tp.Tuple[D3Params, Tensor]] = None):
         """``pairs``: the ``ani_pair_params`` of the model's pair potentials (potentials.PairPotential.params()); each
         adds one launch to the step (``_pair_potentials``), a model without any issues exactly the launches it
-        issued before."""
+        issued before.  ``dispersion``: the ``ani_d3_params`` and device tables of a D3 term
+        (potentials.TwoBodyDispersionD3.params() / .tables(device)), or None; it adds three launches to a step with
+        forces and two to one without (``_dispersion``)."""
         if nets.in_dim != consts.out_dim:
             raise ValueError("network input width != AEV length")
         if nets.num_species != consts.num_species:
@@ -549,6 +552,15 @@ class Engine:
             if p.num_species != consts.num_species:
                 raise ValueError("pair potential / AEV species mismatch")
         self.pairs = list(pairs)
+        if dispersion is not None:
+            d3p, d3t = dispersion
+            if d3p.cutoff_fn == 2 or not d3p.cutoff > 0:
+                raise ValueError("D3 in the fused step needs a finite cutoff (its neighbour search runs on the grid)")
+            if d3p.num_species != consts.num_species:
+                raise ValueError("D3 / AEV species mismatch")
+            if d3t.device != nets.device or d3t.dtype != torch.float32 or d3t.numel() != d3p.num_species ** 2 * 100:
+                raise ValueError("D3 tables must be float32 (S, S, 25, 4) on the engine's device")
+        self.dispersion = dispersion
         self.device = nets.device
         self.params = consts.to_struct()
         # internal column order of the tiled AEV operand / dE/dAEV rows: must be the one the layer-1 weights were packed in
@@ -618,6 +630,9 @@ class Engine:
         if ws is None:
             ws = Workspace(n_conf, n_per_conf, self.consts.num_species, self.nets.ldx, self.nets.ld,
                            self.nets.num_members, self.nbr_cap, self.device, variant=self.variant)
+            if self.dispersion is not None:   # coordination numbers and dE/dCN of every atom (D3 scratch)
+                ws.d3_cn = torch.zeros(ws.n, dtype=torch.float32, device=self.device)
+                ws.d3_dedcn = torch.zeros(ws.n, dtype=torch.float32, device=self.device)
             self._ws[key] = ws
         return ws
 
@@ -738,6 +753,8 @@ class Engine:
             mlp = 3 + (4 if want_grad else 0)
         self.launches_per_step = (1 + (0 if (pbc or n_conf > 1) else 1) + 1 + mlp + (1 if want_grad else 0) + 1
                                   + len(self.pairs))
+        if self.dispersion is not None:   # CN, energies + dE/dCN, and the chain where forces are wanted
+            self.launches_per_step += 3 if (want_grad or members) else 2
         grad = ws.grad.view(n_conf, n_per_conf, 3) if want_grad else None
         virial = None
         if want_virial:
@@ -889,6 +906,9 @@ class Engine:
         if self.pairs:
             self._pair_potentials(ws, lo, hi, lat, ws.grad_ptr if want_grad else None,
                                   ptr(ws.virial) if want_virial else None, None, self._timed)
+        if self.dispersion is not None:
+            self._dispersion(ws, lo, hi, lat, ws.grad_ptr if want_grad else None,
+                             ptr(ws.virial) if want_virial else None, None, self._timed)
         if ws.reducer is not None:
             # multi-GPU: sum the partial forces / energies of all ranks over NVLink peer memory (one launch,
             # part of the captured graph); without forces only the energies matter but the buffer is small
@@ -916,6 +936,23 @@ class Engine:
                 C.byref(p), ptr(ws.grid), ptr(ws.spos), ptr(ws.sorted_orig), ws.n, lo, hi, ws.n_conf, ws.n_per_conf,
                 ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap, ptr(ws.atomic), ws.energies_ptr, grad_ptr, virial_ptr,
                 ptr(ws.member_atomic), grad_members_ptr, idx, len(active), *lat, st))
+
+    def _dispersion(self, ws: Workspace, lo: int, hi: int, lat: tp.Tuple[tp.Any, ...], grad_ptr: tp.Optional[int],
+                    virial_ptr: tp.Optional[int], grad_members_ptr: tp.Optional[int],
+                    run: tp.Callable[[str, tp.Callable[[], int]], None]) -> None:
+        """Enqueue the D3 term for atoms [lo, hi) (ani_b200_dispersion_d3: its own neighbour search over the step's
+        bucket grid, reach cutoff + ``skin``) with the outputs and the ordering rules of ``_pair_potentials``.  A cell
+        thinner than the D3 cutoff + skin raises ANI_STATUS_CELL_TOO_SMALL (``check_status``)."""
+        L = self.lib
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        active = list(self.nets.active)
+        idx = (C.c_int32 * len(active))(*active)
+        fn = L.ani_b200_dispersion_d3_cells if lat else L.ani_b200_dispersion_d3
+        params, tables = self.dispersion
+        run("dispersion_d3", lambda: fn(
+            C.byref(params), ptr(tables), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sorted_orig), ws.n, lo,
+            hi, ws.n_conf, ws.n_per_conf, self.skin, ptr(ws.d3_cn), ptr(ws.d3_dedcn), ptr(ws.atomic), ws.energies_ptr,
+            grad_ptr, virial_ptr, ptr(ws.member_atomic), grad_members_ptr, idx, len(active), ptr(ws.status), *lat, st))
 
     def members_buffers(self, ws: Workspace) -> None:
         """Allocate the per-member slabs and gradients of the query-by-committee step (once per workspace, before any
@@ -973,6 +1010,8 @@ class Engine:
             ws.energies_ptr, st), "reduce_energies")
         if self.pairs:   # before the statistics: they read the members' atomic energies and gradients
             self._pair_potentials(ws, 0, n, lat, None, None, gm, run)
+        if self.dispersion is not None:
+            self._dispersion(ws, 0, n, lat, None, None, gm, run)
         check(L.ani_b200_ensemble_qbc(
             gm, idx, Ma, ptr(ws.member_atomic), ptr(ws.species_i32), ptr(self.sae), n_conf, n_per_conf,
             ptr(ws.grad), ptr(ws.atom_stats), ptr(ws.member_energies), ptr(ws.qbc), st), "ensemble_qbc")

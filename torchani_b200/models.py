@@ -14,6 +14,7 @@ an existing ``torchani.arch.ANI`` instance (weights, AEV constants, self energie
 """
 from __future__ import annotations
 
+import math
 import typing as tp
 
 import torch
@@ -26,7 +27,7 @@ from .neighbors import (CellList, Neighbors, NeighborlistArg, _validate_inputs, 
                         effective_periodic_cell, narrow_down, supercell_for_thin_cell)
 from .nn import (ANINetworks, ATOMIC_NUMBER, AtomicContainer, AtomicNetwork, Ensemble, SpeciesConverter,
                  SpeciesEnergies)
-from .potentials import PairPotential
+from .potentials import PairPotential, TwoBodyDispersionD3
 from . import potentials as _potentials
 
 SYMBOLS_1X = ("H", "C", "N", "O")
@@ -128,8 +129,10 @@ class ANI(torch.nn.Module):
                  energy_shifter: SelfEnergy, periodic_table_index: bool = True,
                  potentials: tp.Optional[tp.Mapping[str, PairPotential]] = None):
         """``potentials``: pair potentials evaluated next to the networks (arch.py:116-127), e.g.
-        ``{"repulsion_xtb": RepulsionXTB(...)}``.  They run inside the fused step over the AEV's own neighbour list,
-        so each needs ``cutoff <=`` the radial AEV cutoff."""
+        ``{"repulsion_xtb": RepulsionXTB(...)}``.  The repulsion terms run inside the fused step over the AEV's own
+        neighbour list, so each needs ``cutoff <=`` the radial AEV cutoff; a ``TwoBodyDispersionD3`` (at most one, any
+        name, a finite cutoff) runs its own neighbour search over the step's bucket grid.  ``self.cutoff`` is the
+        largest cutoff of the networks and the potentials (arch.py:125)."""
         super().__init__()
         self.register_buffer("atomic_numbers", torch.tensor([ATOMIC_NUMBER[e] for e in symbols], dtype=torch.long))
         assert len(energy_shifter.self_energies) == len(symbols)
@@ -142,13 +145,23 @@ class ANI(torch.nn.Module):
         self.energy_shifter = energy_shifter
         self.species_converter = SpeciesConverter(symbols)
         self.cutoff = aev_computer.radial.cutoff
+        n_d3 = 0
         for name, pot in (potentials or {}).items():
             if name == "nnp" or not isinstance(pot, PairPotential):
                 raise ValueError(f"potential {name!r}: expected a torchani_b200.potentials.PairPotential under a name "
                                  "other than 'nnp' (the networks)")
             if tuple(pot.symbols) != tuple(symbols):
                 raise ValueError(f"potential {name!r} was built for other symbols")
-            check_pair_cutoff(pot.cutoff, self.cutoff)
+            if isinstance(pot, TwoBodyDispersionD3):
+                n_d3 += 1
+                if pot.cutoff == math.inf:
+                    raise ValueError(f"potential {name!r}: D3 in a model needs a finite cutoff (its neighbour search "
+                                     "runs on the step's bucket grid)")
+            else:
+                check_pair_cutoff(pot.cutoff, self.cutoff)
+        if n_d3 > 1:
+            raise ValueError("a model takes at most one TwoBodyDispersionD3")
+        self.cutoff = max([self.cutoff] + [float(p.cutoff) for p in (potentials or {}).values()])
         # (the networks are the "nnp" potential of the reference and come first; they stay direct attributes here)
         self.potentials = torch.nn.ModuleDict(dict(potentials or {}))
         self.periodic_table_index = periodic_table_index
@@ -184,6 +197,10 @@ class ANI(torch.nn.Module):
     def _enabled_potentials(self) -> tp.List[PairPotential]:
         return [p for p in self.potentials.values() if p._enabled]
 
+    def _enabled_dispersion(self) -> tp.Optional[TwoBodyDispersionD3]:
+        d3 = [p for p in self._enabled_potentials() if isinstance(p, TwoBodyDispersionD3)]
+        return d3[0] if d3 else None
+
     def to_infer_model(self, use_mnp: bool = False) -> "ANI":
         return self
 
@@ -202,13 +219,18 @@ class ANI(torch.nn.Module):
         shifter = self.energy_shifter
         # the engine bakes the self energies and the pair-potential tables in: key it on their values (edits,
         # `_enabled` toggles)
-        pairs = [p.params() for p in self._enabled_potentials()]
+        pairs = [p.params() for p in self._enabled_potentials() if not isinstance(p, TwoBodyDispersionD3)]
+        d3 = self._enabled_dispersion()
+        disp = None if d3 is None else (d3.params(), d3.tables(device))
         key = (str(device), id(nets), bool(shifter._enabled), shifter.self_energies._version,
                shifter.self_energies.data_ptr(), tuple(bytes(p) for p in pairs))
+        if disp is not None:   # (the device tables are rebuilt when the reference tables change: key on them too)
+            key = key + (bytes(disp[0]), disp[1].data_ptr())
         if self._engine is None or self._engine_key != key:
             sae = self.energy_shifter.self_energies.tolist() if self.energy_shifter._enabled else None
+            kw = {} if disp is None else {"dispersion": disp}
             self._engine = Engine(self.aev_computer.constants, nets, sae, nbr_cap=self.aev_computer.nbr_cap,
-                                  pairs=pairs)
+                                  pairs=pairs, **kw)
             self._engine_key = key
         return self._engine
 
@@ -285,7 +307,9 @@ class ANI(torch.nn.Module):
         every potential of the reference).  Shape: (C,), (C, A), (M, C) or (M, C, A)."""
         self._check_inputs(elem_idxs, coords, charge)
         neighbors = discard_outside_cutoff(neighbors, self.cutoff)
-        aevs = self.aev_computer.compute_from_neighbors(elem_idxs, coords, neighbors)
+        rcr = self.aev_computer.radial.cutoff
+        aevs = self.aev_computer.compute_from_neighbors(
+            elem_idxs, coords, neighbors if self.cutoff <= rcr else discard_outside_cutoff(neighbors, rcr))
         energies = self.neural_networks(elem_idxs, aevs, atomic, ensemble_values)
         for pot in self._enabled_potentials():   # (C,) / (C, A): broadcast over the members, arch.py:365-378
             energies = energies + pot.compute_from_neighbors(
@@ -446,7 +470,9 @@ class ANI(torch.nn.Module):
         for old in list(state_dict.keys()):
             new = old.replace("potentials.nnp.aev_computer.", "aev_computer.")
             new = new.replace("potentials.nnp.neural_networks.", "neural_networks.")
-            if new.startswith(prefix + "potentials.1."):   # legacy numbered potentials, arch.py:278-290
+            if new.startswith(prefix + "potentials.0."):   # legacy numbered potentials, arch.py:278-290
+                new = new.replace("potentials.0.", "potentials.dispersion_d3.", 1)
+            elif new.startswith(prefix + "potentials.1."):
                 new = new.replace("potentials.1.", "potentials.repulsion_xtb.", 1)
             elif new.startswith(prefix + "potentials.2."):
                 new = new.replace("potentials.2.", "", 1)
@@ -599,9 +625,10 @@ def accelerate_torchani_(ref_model):
     nnp.aev_computer = aevc
     nnp.neural_networks = nets
     ref_model.neighborlist = aevc.neighborlist
-    # RepulsionXTB / RepulsionZBL members run through the CUDA pair-list kernel; any other potential stays as it is
+    # RepulsionXTB / RepulsionZBL / TwoBodyDispersionD3 members run through the CUDA pair-list kernels; any other
+    # potential stays as it is
     for name, pot in list(ref_model.potentials.items()):
-        if name != "nnp" and type(pot).__name__ in ("RepulsionXTB", "RepulsionZBL"):
+        if name != "nnp" and type(pot).__name__ in ("RepulsionXTB", "RepulsionZBL", "TwoBodyDispersionD3"):
             ref_model.potentials[name] = _DropInPairPotential(_potentials.from_torchani(pot).to(dev))
     return ref_model
 

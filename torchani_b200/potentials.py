@@ -1,13 +1,18 @@
 """Pair potentials with the interface of ``torchani.potentials`` (potentials/core.py:106-207): the short-range
-repulsion terms ``RepulsionXTB`` (potentials/xtb.py) and ``RepulsionZBL`` (potentials/zbl.py).
+repulsion terms ``RepulsionXTB`` (potentials/xtb.py) and ``RepulsionZBL`` (potentials/zbl.py), and the D3(BJ)
+two-body dispersion ``TwoBodyDispersionD3`` (potentials/dftd3.py).
 
 Inside a model (``models.ANI(..., potentials={...})``) a pair potential is evaluated by the fused step over the
 neighbour list the AEV kernel has just built (``ani_b200_pair_potential``), which is why its cutoff may not exceed the
 radial AEV cutoff.  On its own a module evaluates a half pair list (``compute_from_neighbors``, ``forward``) through
 ``ani_b200_pair_potential_pairs``.  CUDA float32 only; there is no CPU path.
 
-The reference's per-element xTB ``alpha`` / ``yeff`` defaults are not shipped: pass them, or convert a reference
-module (``from_torchani``), which reads its buffers.
+D3 has a cutoff beyond Rcr (8 A in the reference's models) and coordination numbers that make it many-body: inside a
+model it runs its own neighbour search over the step's bucket grid (``ani_b200_dispersion_d3``, three launches).
+
+The reference's per-element xTB ``alpha`` / ``yeff`` defaults and its D3 tables (C6 references, covalent radii,
+empirical charges) are not shipped: pass them, or convert a reference module (``from_torchani``), which reads its
+buffers.
 """
 from __future__ import annotations
 
@@ -18,7 +23,7 @@ import torch
 from torch import Tensor
 
 from . import _lib
-from ._lib import PairParams, check, ptr
+from ._lib import D3Params, PairParams, check, ptr
 from .neighbors import Neighbors, all_pairs
 from .nn import ATOMIC_NUMBER
 
@@ -232,9 +237,174 @@ class RepulsionZBL(PairPotential):
             p.screen_exp[q] = float(self._exponents.view(-1)[q])
 
 
+class _D3Energy(torch.autograd.Function):
+    """coords -> (energies (C,) float64, atomic energies (C, A)) of D3 over a half pair list; dE/dcoords (direct part
+    and coordination-number chain) is produced by the forward launches, as in ``_PairEnergy``."""
+
+    @staticmethod
+    def forward(ctx, coords: Tensor, elem_idxs: Tensor, neighbors: Neighbors, ghost_flags: tp.Optional[Tensor],
+                params: D3Params, tables: Tensor):
+        n_conf, n_per_conf = elem_idxs.shape
+        dev = coords.device
+        species = elem_idxs.reshape(-1).to(torch.int32).contiguous()
+        idx = neighbors.indices.to(torch.int64).contiguous()
+        dist = neighbors.distances.detach().to(torch.float32).contiguous()
+        diff = neighbors.diff_vectors.detach().to(torch.float32).contiguous()
+        ghost = None if ghost_flags is None else ghost_flags.reshape(-1).to(torch.uint8).contiguous()
+        want_grad = bool(coords.requires_grad)
+        n = n_conf * n_per_conf
+        cn = torch.empty(n, dtype=torch.float32, device=dev)
+        dedcn = torch.empty(n, dtype=torch.float32, device=dev) if want_grad else None
+        atomic = torch.zeros(n_conf, n_per_conf, dtype=torch.float32, device=dev)
+        energies = torch.zeros(n_conf, dtype=torch.float64, device=dev)
+        grad = torch.zeros(n_conf, n_per_conf, 3, dtype=torch.float32, device=dev) if want_grad else None
+        with torch.cuda.device(dev):
+            check(_lib.lib().ani_b200_dispersion_d3_pairs(
+                _lib.C.byref(params), ptr(tables), ptr(species), idx[0].data_ptr(), idx[1].data_ptr(), ptr(dist),
+                ptr(diff), ptr(ghost), idx.shape[1], n_conf, n_per_conf, ptr(cn), ptr(dedcn), ptr(atomic),
+                ptr(energies), ptr(grad), torch.cuda.current_stream(dev).cuda_stream), "dispersion_d3_pairs")
+        ctx.want_grad = want_grad
+        if want_grad:
+            ctx.save_for_backward(grad)
+        return energies, atomic
+
+    @staticmethod
+    def backward(ctx, g_energy, g_atomic):
+        return _PairEnergy.backward(ctx, g_energy, g_atomic) + (None,)
+
+
+class _BeckeJohnsonDamp(torch.nn.Module):
+    """Holds the damping radii of D3(BJ) under the reference's state-dict key ``_damp_fn.cutoff_radii``
+    (potentials/dftd3.py:45-110): ``cutoff_radii = sqrt(3 outer(sqrt_q, sqrt_q))`` in Bohr, and ``_a1``, ``_a2``."""
+
+    def __init__(self, a1: float, a2: float, sqrt_empirical_charge: Tensor):
+        super().__init__()
+        self.register_buffer("cutoff_radii", torch.sqrt(3 * torch.outer(sqrt_empirical_charge, sqrt_empirical_charge)))
+        self._a1 = float(a1)
+        self._a2 = float(a2)
+
+
+class TwoBodyDispersionD3(PairPotential):
+    r"""DFT-D3 two-body dispersion with Becke-Johnson damping (potentials/dftd3.py:113-311): coordination numbers,
+    C6 interpolated between the tabulated references, ``C8 = 3 C6 sqrt_q_a sqrt_q_b``, and
+    ``E = -(s6 C6 / (d^6 + (a1 R0 + a2)^6) + s8 C8 / (d^8 + (a1 R0 + a2)^8))`` per pair, times the envelope.
+
+    ``sqrt_empirical_charge`` and ``covalent_radii`` (Angstrom) are one value per symbol; ``coeff6``,
+    ``coordnums_a``, ``coordnums_b`` are the reference's ``precalc_*`` tables for these symbols, shape ``(S, S, 5,
+    5)``, -1 where a reference is missing.  None of them is shipped: pass them, or convert a reference module
+    (``potentials.from_torchani``), or pass the buffers of a reference state dict (the keys are the reference's,
+    ``load_state_dict`` accepts its legacy ``_damp_fn_6`` / ``_damp_fn_8`` keys)."""
+
+    kind = 2
+
+    def __init__(self, symbols: tp.Sequence[str], s6: float, s8: float, damp_a1: float, damp_a2: float,
+                 sqrt_empirical_charge: tp.Sequence[float] = (), covalent_radii: tp.Sequence[float] = (), *,
+                 coeff6: tp.Optional[tp.Any] = None, coordnums_a: tp.Optional[tp.Any] = None,
+                 coordnums_b: tp.Optional[tp.Any] = None, cutoff_fn: tp.Any = "smooth", cutoff: float = math.inf):
+        super().__init__(symbols, cutoff=cutoff, cutoff_fn=cutoff_fn)
+        S = len(symbols)
+        named = {"sqrt_empirical_charge": sqrt_empirical_charge, "covalent_radii": covalent_radii,
+                 "coeff6": coeff6, "coordnums_a": coordnums_a, "coordnums_b": coordnums_b}
+        for name, val in named.items():
+            if val is None or (not isinstance(val, Tensor) and not len(val)):
+                raise ValueError(
+                    f"TwoBodyDispersionD3 needs `{name}`: the reference's D3 tables (c6.h5, atomic constants) are not "
+                    "shipped with torchani_b200; pass them (e.g. the precalc_* buffers of a reference state dict, "
+                    "then load_state_dict), or convert a reference module with potentials.from_torchani")
+        sq = torch.as_tensor(sqrt_empirical_charge, dtype=torch.float32).reshape(-1)
+        rc = torch.as_tensor(covalent_radii, dtype=torch.float32).reshape(-1)
+        if sq.numel() != S or rc.numel() != S:
+            raise ValueError("sqrt_empirical_charge and covalent_radii need one value per symbol")
+        tabs = [torch.as_tensor(t, dtype=torch.float32) for t in (coeff6, coordnums_a, coordnums_b)]
+        for t in tabs:
+            if t.shape != (S, S, 5, 5):
+                raise ValueError(f"the D3 reference tables must have shape ({S}, {S}, 5, 5), got {tuple(t.shape)}")
+        self._damp_fn = _BeckeJohnsonDamp(damp_a1, damp_a2, sq)
+        self._s6 = float(s6)
+        self._s8 = float(s8)
+        self._k1, self._k2, self._k3 = 16, 4 / 3, 4      # dftd3.py:171-174
+        self.register_buffer("precalc_coeff6", tabs[0].clone())
+        self.register_buffer("precalc_coordnums_a", tabs[1].clone())
+        self.register_buffer("precalc_coordnums_b", tabs[2].clone())
+        self.register_buffer("sqrt_charge_ab", torch.outer(sq, sq))
+        self.register_buffer("covalent_radii", rc * ANGSTROM_TO_BOHR)   # Bohr, dftd3.py:162-163
+        self._device_tables: tp.Dict[str, tp.Tuple[tp.Any, Tensor]] = {}
+
+    def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs) -> None:
+        # dftd3.py:127-138: older files hold `_damp_fn_6` (dropped) and `_damp_fn_8` (= `_damp_fn`)
+        for k in list(state_dict.keys()):
+            if not k.startswith(prefix):
+                continue
+            if "damp_fn_6" in k:
+                state_dict.pop(k)
+            elif "damp_fn_8" in k:
+                state_dict[k.replace("damp_fn_8", "damp_fn")] = state_dict.pop(k)
+        super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
+
+    def _versions(self) -> tp.Tuple[tp.Any, ...]:
+        bufs = (self.precalc_coeff6, self.precalc_coordnums_a, self.precalc_coordnums_b)
+        return tuple((b._version, b.data_ptr()) for b in bufs)
+
+    def params(self) -> D3Params:
+        """The ``ani_d3_params`` of this term (built from its current buffers)."""
+        p = D3Params()
+        S = len(self.symbols)
+        p.cutoff_fn, p.num_species = _CUTOFF_FNS[self.cutoff_fn], S
+        p.cutoff = self.cutoff if self.cutoff != math.inf else 0.0
+        p.to_bohr = ANGSTROM_TO_BOHR
+        p.s6, p.s8, p.a1, p.a2 = self._s6, self._s8, self._damp_fn._a1, self._damp_fn._a2
+        p.k1, p.k2, p.k3 = float(self._k1), float(self._k2), float(self._k3)
+        rcov = self.covalent_radii.detach().to("cpu", torch.float64)
+        r0 = self._damp_fn.cutoff_radii.detach().to("cpu", torch.float64)
+        q = self.sqrt_charge_ab.detach().to("cpu", torch.float64)
+        for t in (rcov, r0, q):
+            if not bool(torch.isfinite(t).all()):
+                raise ValueError("D3 parameters contain inf/NaN")
+        damp = self._damp_fn._a1 * r0 + self._damp_fn._a2
+        for a in range(S):
+            p.rcov[a] = float(rcov[a])
+            for b in range(S):
+                p.damp6[a][b] = float(damp[a, b] ** 6)
+                p.damp8[a][b] = float(damp[a, b] ** 8)
+                p.c8_scale[a][b] = float(3.0 * q[a, b])
+        return p
+
+    def tables(self, device: torch.device) -> Tensor:
+        """The reference tables as the kernels read them: f32 (S, S, 25, 4) = {C6ref, CNa, CNb, 0} on ``device``
+        (cached while the buffers are unchanged)."""
+        key = str(device)
+        hit = self._device_tables.get(key)
+        if hit is not None and hit[0] == self._versions():
+            return hit[1]
+        S = len(self.symbols)
+        t = torch.zeros(S, S, 25, 4, dtype=torch.float32)
+        for k, buf in enumerate((self.precalc_coeff6, self.precalc_coordnums_a, self.precalc_coordnums_b)):
+            t[..., k] = buf.detach().to("cpu", torch.float32).reshape(S, S, 25)
+        if not bool(torch.isfinite(t).all()):
+            raise ValueError("D3 reference tables contain inf/NaN")
+        t = t.to(device)
+        self._device_tables[key] = (self._versions(), t)
+        return t
+
+    def compute_from_neighbors(self, elem_idxs: Tensor, coords: Tensor, neighbors: Neighbors, charge: int = 0,
+                               atomic: bool = False, ensemble_values: bool = False,
+                               ghost_flags: tp.Optional[Tensor] = None) -> Tensor:
+        """Energies ``(C,)`` or ``(C, A)`` of the given half pair list (potentials/core.py:181-207 over
+        dftd3.py:221-246): pairs beyond the cutoff are ignored, coordination numbers count every listed pair, pair
+        energies that touch a ghost atom count half."""
+        assert elem_idxs.dim() == 2 and coords.shape == (elem_idxs.shape[0], elem_idxs.shape[1], 3)
+        if coords.device.type != "cuda":
+            raise ValueError("torchani_b200 runs on CUDA tensors only (there is no CPU path)")
+        if ghost_flags is not None and ghost_flags.numel() != elem_idxs.numel():
+            raise ValueError("ghost_flags and species should have the same number of elements")
+        energies, atomic_e = _D3Energy.apply(coords, elem_idxs, neighbors, ghost_flags, self.params(),
+                                             self.tables(coords.device))
+        return atomic_e.to(coords.dtype) if atomic else energies.to(coords.dtype)
+
+
 def from_torchani(ref_pot) -> PairPotential:
-    """A reference ``RepulsionXTB`` / ``RepulsionZBL`` module -> the CUDA module with the same parameters (read from the
-    module's buffers).  Any other potential raises ``ValueError``."""
+    """A reference ``RepulsionXTB`` / ``RepulsionZBL`` / ``TwoBodyDispersionD3`` module -> the CUDA module with the
+    same parameters (read from the module's buffers).  Any other potential raises ``ValueError``."""
     name = type(ref_pot).__name__
     symbols = tuple(ref_pot.symbols)
     cutoff_fn = ref_pot.cutoff_fn
@@ -248,7 +418,23 @@ def from_torchani(ref_pot) -> PairPotential:
                            screen_exponents=ref_pot._exponents.view(-1).tolist(), eff_exponent=ref_pot._kz,
                            eff_atomic_nums=ref_pot._eff_atomic_nums.tolist(), cutoff=ref_pot.cutoff,
                            cutoff_fn=cutoff_fn)
+    elif name == "TwoBodyDispersionD3":
+        S = len(symbols)
+        damp = ref_pot._damp_fn
+        # (sqrt_charge_ab = outer(sqrt_q, sqrt_q); the diagonal gives sqrt_q back.  The buffers are then copied as they
+        # are, so nothing is recomputed from them)
+        sq = ref_pot.sqrt_charge_ab.detach().double().diagonal().sqrt().tolist()
+        out = TwoBodyDispersionD3(symbols, float(ref_pot._s6), float(ref_pot._s8), float(damp._a1), float(damp._a2),
+                                  sq, [1.0] * S, coeff6=ref_pot.precalc_coeff6.detach().cpu(),
+                                  coordnums_a=ref_pot.precalc_coordnums_a.detach().cpu(),
+                                  coordnums_b=ref_pot.precalc_coordnums_b.detach().cpu(), cutoff=ref_pot.cutoff,
+                                  cutoff_fn=cutoff_fn)
+        for key in ("sqrt_charge_ab", "covalent_radii"):
+            getattr(out, key).copy_(getattr(ref_pot, key).detach().to("cpu", torch.float32))
+        out._damp_fn.cutoff_radii.copy_(damp.cutoff_radii.detach().to("cpu", torch.float32))
+        out._k1, out._k2, out._k3 = ref_pot._k1, ref_pot._k2, ref_pot._k3
     else:
-        raise ValueError(f"potential {name} has no CUDA counterpart (RepulsionXTB and RepulsionZBL do)")
+        raise ValueError(f"potential {name} has no CUDA counterpart (RepulsionXTB, RepulsionZBL and "
+                         "TwoBodyDispersionD3 do)")
     out._enabled = bool(ref_pot._enabled)
     return out
