@@ -501,7 +501,11 @@ int ani_b200_half_neighbor_fill(const ani_grid* grid, const int32_t* bin_start, 
                                 float* distances, float* diff_vectors, int32_t* status, void* stream);
 
 /* 6. Ensemble MLP forward + backward-to-input on the species-grouped AEV matrix.           */
-/*    Layer widths: in -> h1 -> h2 -> h3 -> 1, CELU(alpha) after the three hidden layers.    */
+/*    Layer widths: in -> h1 -> h2 -> h3 -> 1, the activation after the three hidden layers: */
+/*    ani_mlp_model::activation = ANI_ACT_CELU: CELU(celu_alpha), every layer with biases;    */
+/*                                ANI_ACT_GELU: GELU (exact erf form), no biases (the packer  */
+/*                                passes zeros in b1..b4, which the GELU kernels never read). */
+/*    Any other value: ANI_ERR_BAD_ARG from every entry point of this section.                */
 /*    "Tiled operand" layout (both GEMM operands; fp32 accuracy on the tensor cores from 16-bit    */
 /*    pieces, see ani_b200_operand_format): every value x of an operand with power-of-two scale s   */
 /*    is stored as P pieces with s*x = p1 + ... + pP, each rounded to nearest:                       */
@@ -518,7 +522,10 @@ int ani_b200_half_neighbor_fill(const ani_grid* grid, const int32_t* bin_start, 
 /*    of row r sits at chunk position c ^ ((r >> 1) & 3)), i.e. exactly the shared-memory image    */
 /*    a K-major UMMA descriptor expects: one K-block of one tile is a contiguous byte range        */
 /*    that a single cp.async.bulk (TMA) moves into shared memory.  Hidden widths that are not       */
-/*    multiples of 32 are zero-padded by the packer (zero weights and biases: CELU(0) = 0).         */
+/*    multiples of 32 are zero-padded by the packer (zero weights and biases: CELU(0) = GELU(0) = 0; */
+/*    GELU'(0) = 1/2 in the padded columns meets the zero rows of the transposed weights).         */
+#define ANI_ACT_CELU 0
+#define ANI_ACT_GELU 1
 typedef struct ani_mlp_species {
   int32_t h1, h2, h3, pad_;
   float w_scale[4];  /* [0..2]: power-of-two scale the packer multiplied W1, W2, W3 by (fp16 pieces) */
@@ -537,8 +544,9 @@ typedef struct ani_mlp_species {
 
 typedef struct ani_mlp_model {
   int32_t num_species, num_members, in_dim, ldx;
-  int32_t h1_max, h2_max, h3_max, pad_;
-  float celu_alpha;
+  int32_t h1_max, h2_max, h3_max;
+  int32_t activation;                  /* ANI_ACT_CELU or ANI_ACT_GELU                          */
+  float celu_alpha;                    /* ANI_ACT_CELU only                                     */
   float member_scale[ANI_MAX_MEMBERS]; /* d(output)/d(member energy): 1/M_active or 0       */
   ani_mlp_species sp[ANI_MAX_SPECIES];
   /* optional device scratch, sum over the species of ldx * (M * h1 / 32) * 2 * P * 32 bytes (the size of the t_b1   */
@@ -565,6 +573,11 @@ int ani_b200_pack_b_operand(const float* src, int n, int k, int ld_src, int tran
 /*                 With a block list, layer 1 skips the dead K-blocks and dE/dAEV is written     */
 /*                 only for the live column blocks (the others keep their previous content).     */
 /*    act1/2/3     tiled operands, 2*P*rows_cap*M*h{1,2,3}_max bytes (activations, then gradients) */
+/*                 GELU model: act1 / act2 are twice that size.  The first half is the activation   */
+/*                 operand as above; the second, the derivative operand of the same shape directly  */
+/*                 behind it, receives GELU'(z) of every element from the forward (want_backward    */
+/*                 != 0 only; at the value scale), which the backward multiplies by: GELU cannot be */
+/*                 recovered from its output as CELU' is.                                           */
 /*    e_member     f32[M][rows_cap]     per-member atomic energies                               */
 /*    status       i32[1] device word, ANI_STATUS_OPERAND_RANGE is OR-ed in (may be NULL)        */
 int ani_b200_mlp_forward_backward(const ani_mlp_model* model, const void* x, float* dx, int rows_cap,
@@ -607,8 +620,9 @@ int ani_b200_mlp_step(const ani_mlp_model* model, const void* x, float* dx, int 
 /*    The same step with gradients (want_backward == 1) as one launch that keeps every intermediate of a      */
 /*    (row tile, member) chain in shared memory (csrc/mlp_resident.cuh): act1 / act2 receive the activations   */
 /*    a1 / a2 (tiled, scaled like the forward's), e_member and dx as above; no act3, no gradient pieces in     */
-/*    global memory, no counters.  ANI_ERR_UNSUPPORTED in the 3 x bf16 build and for models with a hidden      */
-/*    width above 256.                                                                                         */
+/*    global memory, no counters.  GELU model: act1 / act2 receive d1 = GELU'(z1) / d2 = GELU'(z2) instead of   */
+/*    a1 / a2 (same tiled layout and scale, same size as for CELU: no derivative operand behind them).         */
+/*    ANI_ERR_UNSUPPORTED in the 3 x bf16 build and for models with a hidden width above 256.                  */
 int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void* x, float* dx, int rows_cap,
                                const int32_t* row_atom, const int32_t* layout_info, const int32_t* aev_blocks,
                                void* act1, void* act2, float* e_member, int32_t* status, void* stream);

@@ -21,6 +21,8 @@ ANI_MAX_MEMBERS = 16
 ANI_TILE_ROWS = 128
 ANI_MAX_ANG = 96
 ANI_VIRIAL_SLOTS = 64
+ACT_CELU = 0                # ani_mlp_model::activation
+ACT_GELU = 1
 ANI_LATTICE_STRIDE = 18   # floats per conformer of the lattice table of grid mode 3: cell, inverse
 
 STATUS_NBR_OVERFLOW = 1
@@ -61,7 +63,7 @@ class MLPSpecies(C.Structure):
 class MLPModel(C.Structure):
     _fields_ = [
         ("num_species", C.c_int32), ("num_members", C.c_int32), ("in_dim", C.c_int32), ("ldx", C.c_int32),
-        ("h1_max", C.c_int32), ("h2_max", C.c_int32), ("h3_max", C.c_int32), ("pad_", C.c_int32),
+        ("h1_max", C.c_int32), ("h2_max", C.c_int32), ("h3_max", C.c_int32), ("activation", C.c_int32),
         ("celu_alpha", C.c_float), ("member_scale", C.c_float * ANI_MAX_MEMBERS),
         ("sp", MLPSpecies * ANI_MAX_SPECIES),
         ("b1_compact", C.c_void_p),

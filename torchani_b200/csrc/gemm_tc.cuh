@@ -24,6 +24,8 @@
 //               wgmma.m64n64k16 per 64-column slice from the shared-memory ring into a
 //               register accumulator of up to 64 x 256, then runs the epilogue straight from registers:
 //               bias + CELU | * CELU'(stored activation) | final layer + gradient seed | plain
+//               (GELU models, ACT_GELU: GELU without bias, storing GELU' beside the activation | * stored GELU' |
+//               GELU head)
 // Ring: STAGES slots of (A block + B block of up to 256 rows); the producer runs ahead across units, so
 // the loads of the next unit overlap the epilogue of the current one.
 //
@@ -68,6 +70,12 @@ constexpr int CHAIN_MAX_D = 8;
 constexpr long long SPIN_LIMIT = 6000000000LL;  // ~3 s of clock64 ticks
 
 enum { EPI_BIAS_CELU = 0, EPI_MUL_DCELU = 1, EPI_PLAIN = 2, EPI_HEAD = 3 };
+// The hidden-layer activation (ani_mlp_model::activation), a compile-time parameter of the epilogues and kernels:
+//   ACT_CELU  CELU(alpha) after bias: EPI_MUL_DCELU recovers CELU' from the stored activation itself.
+//   ACT_GELU  exact-erf GELU, no biases.  GELU is not invertible, so the forward epilogues of layers 1 and 2 also store
+//             d = GELU'(z) into the DERIVATIVE OPERAND, the same-shaped tiled operand directly behind C (d_offset),
+//             and EPI_MUL_DCELU multiplies by that d.  |d| <= 1.13: stored at the value scale, no range check.
+enum { ACT_CELU = ANI_ACT_CELU, ACT_GELU = ANI_ACT_GELU };
 
 struct Species {
   const unsigned char* Bt;  // tiled B operand
@@ -240,6 +248,21 @@ __device__ __forceinline__ float celu(float x, const CeluConst& c) {
 }
 __device__ __forceinline__ float dcelu_from_out(float y, const CeluConst& c) {
   return y > 0.f ? 1.0f : fmaf(y, c.inv_alpha, 1.0f);
+}
+// GELU(x) = x Phi(x) (torch's approximate="none") and GELU'(x) = Phi(x) + x phi(x), from one erf and one exp.
+// Phi = (1 + erf(x / sqrt 2)) / 2 cancels in the negative tail: its absolute error stays ~3e-8 there (2^-25 |x| in
+// GELU), below what the 16-bit operand pieces keep of the values around it.
+__device__ __forceinline__ void gelu_and_grad(float x, float& a, float& d) {
+  const float cdf = fmaf(0.5f, erff(x * 0.70710678118654752f), 0.5f);
+  float e;  // exp(-x^2 / 2) = 2^(-x^2 log2(e) / 2)
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * x * -0.72134752044448170f));
+  a = x * cdf;
+  d = fmaf(x * 0.39894228040143268f, e, cdf);
+}
+// byte offset of the derivative operand of a GELU model behind a tiled activation operand of c_kblocks 32-column
+// blocks per row (include/ani_b200.h section 6)
+__device__ __forceinline__ size_t d_offset(int rows_cap, int c_kblocks) {
+  return (size_t)(rows_cap / TM) * c_kblocks * A_BLOCK_BYTES;
 }
 // running max of |v| in which a NaN sticks (fmaxf drops it): an inf/NaN operand piece turns the products into NaN,
 // and that must raise ANI_STATUS_OPERAND_RANGE like any other value out of range
@@ -478,7 +501,7 @@ __device__ __forceinline__ void wait_inputs(const StepArgs& F, const TileMap* tm
 // ---- epilogue of one consumer warpgroup: 64 rows x bn columns straight from the accumulator registers ----
 // Register i of 64-column slice c holds row 16 * warp + lane / 4 + 8 * ((i >> 1) & 1), column
 // 64 c + 8 (i >> 2) + 2 (lane & 3) + (i & 1).
-template <int EPI>
+template <int EPI, int ACT>
 __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& tm, const Tile& tl, float (&acc)[4][32],
                                               int wg, int lane, int warp_in_wg, float& omax) {
   const Species& sp = args.sp[tl.s];
@@ -486,10 +509,15 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
   const int q = lane & 3;
   const int r0 = 64 * wg + 16 * warp_in_wg + (lane >> 2);  // rows r0 and r0 + 8 of the tile
   const float acc_scale = sp.acc_scale;
+  constexpr bool GELU = ACT == ACT_GELU;
   const bool tiled_out = EPI != EPI_PLAIN && (EPI != EPI_HEAD || args.want_backward);
   unsigned char* ct = reinterpret_cast<unsigned char*>(args.C) +
                       ((size_t)tl.rt * args.c_kblocks + (size_t)(tl.mem * sp.c_moff + tl.n0) / TK) * A_BLOCK_BYTES;
-  const float* bias = EPI == EPI_BIAS_CELU || EPI == EPI_HEAD ? sp.bias + (size_t)tl.mem * sp.bias_mstride + tl.n0 : nullptr;
+  // GELU: where d = GELU'(z) of these columns is stored (EPI_BIAS_CELU, only for a backward) and read (EPI_MUL_DCELU)
+  unsigned char* dt = GELU ? ct + d_offset(args.rows_cap, args.c_kblocks) : nullptr;
+  const bool store_d = GELU && EPI == EPI_BIAS_CELU && args.want_backward;
+  const float* bias = !GELU && (EPI == EPI_BIAS_CELU || EPI == EPI_HEAD) ? sp.bias + (size_t)tl.mem * sp.bias_mstride + tl.n0
+                                                                         : nullptr;
   const float* w4 = EPI == EPI_HEAD ? sp.w4 + (size_t)tl.mem * sp.N : nullptr;
   float e_acc[2] = {0.f, 0.f}, seed[2] = {0.f, 0.f};
   bool row_valid[2] = {false, false};
@@ -501,12 +529,13 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
     }
   }
   const int ngroups = tl.bn / 32;
-  // EPI_MUL_DCELU: the stored activation of the next (32-column group, row half) is loaded before the current one is
-  // computed and stored in its place.  (Loads may not pass stores into the same buffer, so without this every step
-  // would wait for a full global round trip.)  [step parity][piece]: chunk q of every piece of the row
+  // EPI_MUL_DCELU: the stored activation (GELU: the stored derivative) of the next (32-column group, row half) is loaded
+  // before the current one is computed and stored in its place.  (Loads may not pass stores into the same buffer, so
+  // without this every step would wait for a full global round trip.)  [step parity][piece]: chunk q of every piece
+  // of the row
   uint4 ybuf[2][PARTS];
   auto load_y = [&](int g, int h, uint4 (&dst)[PARTS]) {
-    const unsigned char* blk = ct + (size_t)g * A_BLOCK_BYTES + swz_off(r0 + 8 * h, q);
+    const unsigned char* blk = (GELU ? dt : ct) + (size_t)g * A_BLOCK_BYTES + swz_off(r0 + 8 * h, q);
 #pragma unroll
     for (int p = 0; p < PARTS; ++p) dst[p] = *reinterpret_cast<const uint4*>(blk + p * A_PART_BYTES);
   };
@@ -534,13 +563,13 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
           quad_transpose(yw[p], lane);
         }
       }
-      uint32_t w[PARTS][4];
-      float o[4][2];
+      uint32_t w[PARTS][4], dw[PARTS][4];
+      float o[4][2], od[2];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int col = 32 * g + 8 * j + 2 * q;  // column inside the tile
         float2 b2 = make_float2(0.f, 0.f), w2 = make_float2(0.f, 0.f), y2 = make_float2(0.f, 0.f);
-        if (EPI == EPI_BIAS_CELU || EPI == EPI_HEAD) b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
+        if (!GELU && (EPI == EPI_BIAS_CELU || EPI == EPI_HEAD)) b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
         if (EPI == EPI_HEAD) w2 = __ldg(reinterpret_cast<const float2*>(w4 + col));
         if (EPI == EPI_MUL_DCELU) {
           uint32_t pw[PARTS];
@@ -552,7 +581,18 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
         for (int e = 0; e < 2; ++e) {
           float v = acc[c][ib + 4 * j + 2 * h + e] * acc_scale;
           const float bb = e ? b2.y : b2.x, ww = e ? w2.y : w2.x, yy = e ? y2.y : y2.x;
-          if (EPI == EPI_BIAS_CELU) {
+          if (GELU && EPI == EPI_BIAS_CELU) {
+            float d;
+            gelu_and_grad(v, v, d);
+            od[e] = d * args.out_scale;
+          } else if (GELU && EPI == EPI_MUL_DCELU) {
+            v *= yy * args.y_inv_scale;
+          } else if (GELU && EPI == EPI_HEAD) {
+            float a, d;
+            gelu_and_grad(v, a, d);
+            e_acc[h] = fmaf(a, ww, e_acc[h]);
+            v = seed[h] * ww * d;
+          } else if (EPI == EPI_BIAS_CELU) {
             v = celu(v + bb, cc);
           } else if (EPI == EPI_MUL_DCELU) {
             v *= dcelu_from_out(yy * args.y_inv_scale, cc);
@@ -572,6 +612,12 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
           split_pair(o[j][0], o[j][1], pw);
 #pragma unroll
           for (int p = 0; p < PARTS; ++p) w[p][j] = pw[p];
+        }
+        if (store_d) {
+          uint32_t pw[PARTS];
+          split_pair(od[0], od[1], pw);
+#pragma unroll
+          for (int p = 0; p < PARTS; ++p) dw[p][j] = pw[p];
         }
       }
       if (EPI == EPI_PLAIN) {
@@ -593,6 +639,14 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
           quad_transpose(w[p], lane);
           *reinterpret_cast<uint4*>(blk + p * A_PART_BYTES) = make_uint4(w[p][0], w[p][1], w[p][2], w[p][3]);
         }
+        if (store_d) {
+          unsigned char* dblk = dt + (size_t)g * A_BLOCK_BYTES + swz_off(row, q);
+#pragma unroll
+          for (int p = 0; p < PARTS; ++p) {
+            quad_transpose(dw[p], lane);
+            *reinterpret_cast<uint4*>(dblk + p * A_PART_BYTES) = make_uint4(dw[p][0], dw[p][1], dw[p][2], dw[p][3]);
+          }
+        }
       }
     }
   }
@@ -609,6 +663,8 @@ __device__ __forceinline__ void tile_epilogue(const Args& args, const TileMap& t
 }
 
 // ---- the kernel -----------------------------------------------------------------------------
+// ACT: the activation of the model (ACT_CELU / ACT_GELU), one instance each
+template <int ACT>
 __global__ void __launch_bounds__(THREADS, 1) k_gemm_wg(const __grid_constant__ StepArgs F) {
   extern __shared__ unsigned char smem_raw[];
   // 1024-byte aligned ring (swizzle groups are 8 rows x 64 B)
@@ -656,10 +712,11 @@ __global__ void __launch_bounds__(THREADS, 1) k_gemm_wg(const __grid_constant__ 
           stamp(tloc, 0, 0);
           wait_inputs(F, tms, un.p, tl);
           if (F.sync) fence_proxy_async_all();
-          // the stored activation the dCELU epilogue reads: contiguous 32-column blocks of this tile, on their way to L2
-          // while the main loop runs
+          // the stored activation (GELU: derivative) the dCELU epilogue reads: contiguous 32-column blocks of this tile,
+          // on their way to L2 while the main loop runs
           if (F.epi[un.p] == EPI_MUL_DCELU)
             prefetch_l2(static_cast<const unsigned char*>(args.C) +
+                            (ACT == ACT_GELU ? d_offset(args.rows_cap, args.c_kblocks) : (size_t)0) +
                             ((size_t)tl.rt * args.c_kblocks + (size_t)(tl.mem * sp.c_moff + tl.n0) / TK) * A_BLOCK_BYTES,
                         (uint32_t)(tl.bn / TK) * A_BLOCK_BYTES);
         }
@@ -812,10 +869,10 @@ __global__ void __launch_bounds__(THREADS, 1) k_gemm_wg(const __grid_constant__ 
       wg_bar(wg);
     }
     switch (F.epi[un.p]) {
-      case EPI_BIAS_CELU: tile_epilogue<EPI_BIAS_CELU>(args, tm, tl, acc, wg, lane, warp_in_wg, omax); break;
-      case EPI_MUL_DCELU: tile_epilogue<EPI_MUL_DCELU>(args, tm, tl, acc, wg, lane, warp_in_wg, omax); break;
-      case EPI_HEAD: tile_epilogue<EPI_HEAD>(args, tm, tl, acc, wg, lane, warp_in_wg, omax); break;
-      default: tile_epilogue<EPI_PLAIN>(args, tm, tl, acc, wg, lane, warp_in_wg, omax); break;
+      case EPI_BIAS_CELU: tile_epilogue<EPI_BIAS_CELU, ACT>(args, tm, tl, acc, wg, lane, warp_in_wg, omax); break;
+      case EPI_MUL_DCELU: tile_epilogue<EPI_MUL_DCELU, ACT>(args, tm, tl, acc, wg, lane, warp_in_wg, omax); break;
+      case EPI_HEAD: tile_epilogue<EPI_HEAD, ACT>(args, tm, tl, acc, wg, lane, warp_in_wg, omax); break;
+      default: tile_epilogue<EPI_PLAIN, ACT>(args, tm, tl, acc, wg, lane, warp_in_wg, omax); break;
     }
     // one release per warpgroup and unit: its 64 rows of the tile are stored
     if (F.sync && un.p + 1 < F.n_phases) {

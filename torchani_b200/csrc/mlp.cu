@@ -9,6 +9,8 @@
 // concatenated along N (the AEV is read once, not 8x as in BmmLinear's expand()).
 // Backward-to-input runs the same kernel on the transposed weights; CELU'(x) is recovered
 // from the stored activation y as (y > 0 ? 1 : (y + alpha) / alpha)  (csrc/mnp.cpp:206-209).
+// GELU models (no biases) store GELU'(x) itself in the forward: the derivative operand behind act1 / act2, or, in the
+// resident launch, act1 / act2 themselves (gemm_tc.cuh, mlp_resident.cuh).
 //
 // Arithmetic: wgmma tensor cores on fp32-accurate 16-bit operand pieces (2 x fp16 with power-of-two
 // operand scales, or 3 x bf16; gemm_tc.cuh / common.cuh).
@@ -183,7 +185,8 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    cudaFuncSetAttribute(tc::k_gemm_wg, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES);
+    cudaFuncSetAttribute(tc::k_gemm_wg<tc::ACT_CELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES);
+    cudaFuncSetAttribute(tc::k_gemm_wg<tc::ACT_GELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES);
   }
   return n;
 }
@@ -193,8 +196,13 @@ static int num_sms() {
 // scheduled while the previous kernel of the stream drains (its CTAs occupy a whole SM each, so a
 // new CTA starts as soon as one of them exits), run their prologue (barriers, tile map) and block in
 // griddepcontrol.wait until the previous grid has completed and flushed.
+// the instance of the GEMM kernel for the model's activation (checked by check_model)
+static void (*gemm_kernel(const ani_mlp_model* model))(tc::StepArgs) {
+  return model->activation == ANI_ACT_GELU ? tc::k_gemm_wg<tc::ACT_GELU> : tc::k_gemm_wg<tc::ACT_CELU>;
+}
+
 template <int EPI>
-static void launch_gemm_tc(const tc::Args& a, cudaStream_t st, bool dependent = false) {
+static void launch_gemm_tc(const ani_mlp_model* model, const tc::Args& a, cudaStream_t st, bool dependent = false) {
   static tc::StepArgs F;   // ~4 KB: built in place, passed by value (__grid_constant__)
   F.n_phases = 1;
   F.epi[0] = EPI;
@@ -219,7 +227,7 @@ static void launch_gemm_tc(const tc::Args& a, cudaStream_t st, bool dependent = 
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = dependent && pdl ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, tc::k_gemm_wg, F);
+  cudaLaunchKernelEx(&cfg, gemm_kernel(model), F);
 }
 
 extern "C" int ani_b200_pack_b_operand(const float* src, int n, int k, int ld_src, int transpose, float scale,
@@ -241,6 +249,7 @@ static int check_model(const ani_mlp_model* model, int rows_cap) {
   if (!model) return ANI_ERR_BAD_ARG;
   const int S = model->num_species, M = model->num_members;
   if (S < 1 || S > ANI_MAX_SPECIES || M < 1 || M > ANI_MAX_MEMBERS) return ANI_ERR_BAD_ARG;
+  if (model->activation != ANI_ACT_CELU && model->activation != ANI_ACT_GELU) return ANI_ERR_BAD_ARG;
   if (rows_cap < ANI_TILE_ROWS || rows_cap % ANI_TILE_ROWS) return ANI_ERR_BAD_ARG;
   const int ldx = model->ldx;
   if (ldx % 32 || ldx < model->in_dim) return ANI_ERR_BAD_ARG;
@@ -362,7 +371,7 @@ extern "C" int ani_b200_mlp_forward(const ani_mlp_model* model, const void* x, i
                             1.0f / (sv * wsc(p, 0))};
   }
   ta.kblocks = aev_blocks;  // dead AEV column blocks contribute exact zeros: skip them
-  launch_gemm_tc<tc::EPI_BIAS_CELU>(ta, st);
+  launch_gemm_tc<tc::EPI_BIAS_CELU>(model, ta, st);
   ta.kblocks = nullptr;
   ta.A = static_cast<const unsigned char*>(act1); ta.a_kblocks = kb1; ta.C = act2; ta.c_kblocks = kb2; ta.members = M;
   for (int s = 0; s < S; ++s) {
@@ -370,7 +379,7 @@ extern "C" int ani_b200_mlp_forward(const ani_mlp_model* model, const void* x, i
     ta.sp[s] = tc::Species{static_cast<const unsigned char*>(p.t_f2), p.b2, p.h1, p.h2, p.h1, p.h2, p.h2, nullptr, nullptr, 0, 0,
                             1.0f / (sv * wsc(p, 1))};
   }
-  launch_gemm_tc<tc::EPI_BIAS_CELU>(ta, st, true);
+  launch_gemm_tc<tc::EPI_BIAS_CELU>(model, ta, st, true);
   ta.A = static_cast<const unsigned char*>(act2); ta.a_kblocks = kb2; ta.C = act3; ta.c_kblocks = kb3; ta.members = M;
   for (int s = 0; s < S; ++s) {
     const ani_mlp_species& p = model->sp[s];
@@ -381,7 +390,7 @@ extern "C" int ani_b200_mlp_forward(const ani_mlp_model* model, const void* x, i
   // G3 = scale_m * w4 * celu'(a3) directly, e_member the per-member atomic energies
   ta.out_scale = sg;  // act3 receives the gradient seed
   ta.allow_narrow = 0;  // the fused final layer needs all of h3 in one accumulator
-  launch_gemm_tc<tc::EPI_HEAD>(ta, st, true);
+  launch_gemm_tc<tc::EPI_HEAD>(model, ta, st, true);
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
 }
@@ -415,14 +424,14 @@ extern "C" int ani_b200_mlp_backward(const ani_mlp_model* model, float* dx, int 
                             1.0f / (sg * wsc(p, 2))};
   }
   // (after a cross-stream join -- the caller zeroed dx elsewhere -- the first launch is a plain one)
-  launch_gemm_tc<tc::EPI_MUL_DCELU>(ta, st, !dx_zeroed);
+  launch_gemm_tc<tc::EPI_MUL_DCELU>(model, ta, st, !dx_zeroed);
   ta.A = static_cast<const unsigned char*>(act2); ta.a_kblocks = kb2; ta.C = act1; ta.c_kblocks = kb1; ta.members = M;
   for (int s = 0; s < S; ++s) {
     const ani_mlp_species& p = model->sp[s];
     ta.sp[s] = tc::Species{static_cast<const unsigned char*>(p.t_b2), nullptr, p.h2, p.h1, p.h2, p.h1, 0, nullptr, nullptr, 0, 0,
                             1.0f / (sg * wsc(p, 1))};
   }
-  launch_gemm_tc<tc::EPI_MUL_DCELU>(ta, st, true);
+  launch_gemm_tc<tc::EPI_MUL_DCELU>(model, ta, st, true);
   // dX = sum_m G1_m x W1_m: split-K over the members (one work unit per (row tile, member), so
   // all SMs are busy even when there are fewer row tiles than SMs); the partial tiles are
   // accumulated with vector REDs into the zeroed live column blocks of dx
@@ -441,7 +450,7 @@ extern "C" int ani_b200_mlp_backward(const ani_mlp_model* model, float* dx, int 
   }
   // (ani_b200_zero_live_blocks, if the caller ran it for this step, has also gathered the compact operands)
   if (!dx_zeroed) launch_zero_compact(model, ta.c_accumulate ? dx : nullptr, layout_info, aev_blocks, st);
-  launch_gemm_tc<tc::EPI_PLAIN>(ta, st, true);
+  launch_gemm_tc<tc::EPI_PLAIN>(model, ta, st, true);
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
 }
@@ -588,7 +597,7 @@ extern "C" int ani_b200_mlp_step(const ani_mlp_model* model, const void* x, floa
       F.ph[p].win_idx = c;
       F.ph[p].win_cnt = chunks;
     }
-    tc::k_gemm_wg<<<num_sms(), tc::THREADS, tc::SMEM_BYTES, st>>>(F);
+    gemm_kernel(model)<<<num_sms(), tc::THREADS, tc::SMEM_BYTES, st>>>(F);
     F.trace = nullptr;   // (the role timeline records the first window)
   }
   ANI_CUDA_CHECK_LAUNCH();
@@ -670,6 +679,22 @@ static int resident_args(const ani_mlp_model* model, const void* x, float* dx, i
   for (int m = 0; m < ANI_MAX_MEMBERS; ++m) F.member_of[m] = m;
   return ANI_OK;
 }
+
+// the instance of the resident kernel for the model's activation (checked by check_model), with its shared-memory limit
+template <bool SLABS>
+static void (*resident_kernel(const ani_mlp_model* model))(tc::ResArgs) {
+  static const bool attr = []() {
+    bool ok = true;
+    ok &= cudaFuncSetAttribute(tc::k_mlp_resident<tc::ACT_CELU, SLABS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               tc::RES_SMEM_BYTES) == cudaSuccess;
+    ok &= cudaFuncSetAttribute(tc::k_mlp_resident<tc::ACT_GELU, SLABS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               tc::RES_SMEM_BYTES) == cudaSuccess;
+    return ok;
+  }();
+  (void)attr;
+  return model->activation == ANI_ACT_GELU ? tc::k_mlp_resident<tc::ACT_GELU, SLABS>
+                                           : tc::k_mlp_resident<tc::ACT_CELU, SLABS>;
+}
 #endif
 
 extern "C" int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void* x, float* dx, int rows_cap,
@@ -685,15 +710,10 @@ extern "C" int ani_b200_mlp_step_resident(const ani_mlp_model* model, const void
   static tc::ResArgs F;   // ~2 KB: built in place, passed by value (__grid_constant__)
   const int rc = resident_args(model, x, dx, rows_cap, row_atom, layout_info, aev_blocks, act1, act2, e_member, status, F);
   if (rc != ANI_OK) return rc;
-  static const bool attr = []() {
-    return cudaFuncSetAttribute(tc::k_mlp_resident<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                tc::RES_SMEM_BYTES) == cudaSuccess;
-  }();
-  (void)attr;
   cudaStream_t st = (cudaStream_t)stream;
   // zero the live blocks of dx (the members' REDs accumulate into it) and gather the compact W1^T operands
   launch_zero_compact(model, model->num_members > 1 ? dx : nullptr, layout_info, aev_blocks, st);
-  tc::k_mlp_resident<false><<<num_sms(), tc::THREADS, tc::RES_SMEM_BYTES, st>>>(F);
+  resident_kernel<false>(model)<<<num_sms(), tc::THREADS, tc::RES_SMEM_BYTES, st>>>(F);
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
 #endif
@@ -726,14 +746,9 @@ extern "C" int ani_b200_mlp_step_resident_members(const ani_mlp_model* model, co
       cudaMemsetAsync(e_member + (size_t)m * rows_cap, 0, sizeof(float) * (size_t)rows_cap, st);
   }
   if (F.n_chain_members == 0) return ANI_ERR_BAD_ARG;
-  static const bool attr = []() {
-    return cudaFuncSetAttribute(tc::k_mlp_resident<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                tc::RES_SMEM_BYTES) == cudaSuccess;
-  }();
-  (void)attr;
   // gather the compact W1^T operands; the slabs take plain stores and need no zero-fill
   launch_zero_compact(model, nullptr, layout_info, aev_blocks, st);
-  tc::k_mlp_resident<true><<<num_sms(), tc::THREADS, tc::RES_SMEM_BYTES, st>>>(F);
+  resident_kernel<true>(model)<<<num_sms(), tc::THREADS, tc::RES_SMEM_BYTES, st>>>(F);
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
 #endif

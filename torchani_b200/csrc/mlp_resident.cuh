@@ -39,6 +39,11 @@
 // launch, and .cg leaves no room for a stale line either way.  Every copy of a chain is complete by its phase 3, so
 // none is in flight when the next chain's phase 0 overwrites R or when the CTA exits.
 //
+// GELU models (ACT_GELU): phases 0 / 1 store a = GELU(z) into R and d = GELU'(z) into act1 / act2, each thread the
+// words it computed with plain stores (exactly the words its load_y reads back in phases 4 / 3, so program order alone
+// makes them visible); nothing reads a1 / a2 after the forward phases, and there are no bulk copies.  Phases 3 / 4
+// multiply by d, the head computes GELU and GELU' from registers, and no bias is loaded.
+//
 // Shared memory: R 128 KB + a ring of six 16 KB slots + 1 KB alignment = 230,400 B.  A K-block takes one slot for
 // the x block of phase 0 and one per 128 rows of B.
 // The 3 x bf16 build would need 192 KB for R and does not compile this kernel.
@@ -203,21 +208,22 @@ __device__ __forceinline__ void res_phase(const ResArgs& a, const ResSpecies& sp
 
 // ---- epilogue of one consumer warpgroup and phase P: 64 rows x bn columns from the accumulator registers ----
 // Same register -> (row, column) map as tile_epilogue (gemm_tc.cuh).
-template <int P, bool SLABS>
+template <int P, int ACT, bool SLABS>
 __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies& sp, int rt, int m, int n0, int bn,
                                              float (&acc)[4][32], uint32_t res, const int* blk, int nblk, int wg,
                                              int lane, int warp_in_wg, float& omax) {
-  constexpr bool ACT = P <= 1, HEAD = P == 2, DCELU = P == 3 || P == 4, PLAIN = P == 5;
+  constexpr bool ACTV = P <= 1, HEAD = P == 2, DCELU = P == 3 || P == 4, PLAIN = P == 5, GELU = ACT == ACT_GELU;
   const CeluConst cc{a.alpha, 1.0f / a.alpha, 1.4426950408889634f / a.alpha};
   const int q = lane & 3;
   const int r0 = 64 * wg + 16 * warp_in_wg + (lane >> 2);  // rows r0 and r0 + 8 of the tile
   const float acc_scale = sp.acc_scale[P];
-  const float out_scale = ACT ? OPND_SCALE_VALUE : OPND_SCALE_GRAD;
-  // the global copy of a1 / a2 that phases 4 / 3 read back for CELU' (bulk-copied from R after phases 0 / 1)
-  const unsigned char* ct = nullptr;
-  if (P == 4) ct = a.act1 + ((size_t)rt * a.kb1 + (size_t)(m * sp.h1) / TK) * A_BLOCK_BYTES;
-  if (P == 3) ct = a.act2 + ((size_t)rt * a.kb2 + (size_t)(m * sp.h2) / TK) * A_BLOCK_BYTES;
-  const float* bias = P <= 2 ? sp.bias[P] + (size_t)m * (P == 0 ? sp.h1 : P == 1 ? sp.h2 : sp.h3) : nullptr;
+  const float out_scale = ACTV ? OPND_SCALE_VALUE : OPND_SCALE_GRAD;
+  // the global copy of a1 / a2 that phases 4 / 3 read back for CELU' (bulk-copied from R after phases 0 / 1), or
+  // GELU: d1 / d2, stored there by phases 0 / 1
+  unsigned char* ct = nullptr;
+  if (P == 4 || (GELU && P == 0)) ct = a.act1 + ((size_t)rt * a.kb1 + (size_t)(m * sp.h1) / TK) * A_BLOCK_BYTES;
+  if (P == 3 || (GELU && P == 1)) ct = a.act2 + ((size_t)rt * a.kb2 + (size_t)(m * sp.h2) / TK) * A_BLOCK_BYTES;
+  const float* bias = !GELU && P <= 2 ? sp.bias[P] + (size_t)m * (P == 0 ? sp.h1 : P == 1 ? sp.h2 : sp.h3) : nullptr;
   const float* w4 = HEAD ? sp.w4 + (size_t)m * sp.h3 : nullptr;
   float e_acc[2] = {0.f, 0.f}, seed[2] = {0.f, 0.f};
   bool row_valid[2] = {false, false};
@@ -274,12 +280,12 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
           load_y(g + 1, 0, ybuf[0]);
       }
       uint32_t w[PARTS][4];
-      float o[4][2];
+      float o[4][2], od[2];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int col = 32 * g + 8 * j + 2 * q;  // column inside the tile
         float2 b2 = make_float2(0.f, 0.f), w2 = make_float2(0.f, 0.f), y2 = make_float2(0.f, 0.f);
-        if (P <= 2) b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
+        if (!GELU && P <= 2) b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
         if (HEAD) w2 = __ldg(reinterpret_cast<const float2*>(w4 + col));
         if (DCELU) {
           uint32_t pw[PARTS];
@@ -291,7 +297,18 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
         for (int e = 0; e < 2; ++e) {
           float v = ag[4 * j + 2 * h + e] * acc_scale;
           const float bb = e ? b2.y : b2.x, ww = e ? w2.y : w2.x, yy = e ? y2.y : y2.x;
-          if (ACT) {
+          if (GELU && ACTV) {
+            float d;
+            gelu_and_grad(v, v, d);
+            od[e] = d * OPND_SCALE_VALUE;
+          } else if (GELU && DCELU) {
+            v *= yy * (1.0f / OPND_SCALE_VALUE);
+          } else if (GELU && HEAD) {
+            float av, d;
+            gelu_and_grad(v, av, d);
+            e_acc[h] = fmaf(av, ww, e_acc[h]);
+            v = seed[h] * ww * d;
+          } else if (ACTV) {
             v = celu(v + bb, cc);
           } else if (DCELU) {
             v *= dcelu_from_out(yy * (1.0f / OPND_SCALE_VALUE), cc);
@@ -311,6 +328,13 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
           split_pair(o[j][0], o[j][1], pw);
 #pragma unroll
           for (int p = 0; p < PARTS; ++p) w[p][j] = pw[p];
+        }
+        if (GELU && ACTV) {  // word q of chunk j of the row: the word load_y reads back
+          uint32_t pw[PARTS];
+          split_pair(od[0], od[1], pw);
+          unsigned char* b = ct + (size_t)g * A_BLOCK_BYTES + 4 * q + swz_off(row, j);
+#pragma unroll
+          for (int p = 0; p < PARTS; ++p) *reinterpret_cast<uint32_t*>(b + p * A_PART_BYTES) = pw[p];
         }
       }
       if (PLAIN) {
@@ -344,10 +368,11 @@ __device__ __forceinline__ void res_epilogue(const ResArgs& a, const ResSpecies&
 }
 
 // ---- the kernel: one persistent CTA per SM, chains res_chain_id(0), res_chain_id(1), ... ----
+// ACT: the activation of the model (ACT_CELU / ACT_GELU).
 // SLABS = false: every member's chains, phase 5 reduces the members into dx (ani_b200_mlp_step_resident).
 // SLABS = true: the chains of F.member_of only, phase 5 stores each member's rows into its own slab
 // (ani_b200_mlp_step_resident_members).
-template <bool SLABS>
+template <int ACT, bool SLABS>
 __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_constant__ ResArgs F) {
   extern __shared__ unsigned char smem_raw[];
   // 1024-byte aligned (swizzle groups are 8 rows x 64 B): R, then the ring
@@ -526,17 +551,17 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
         release(prev, held);
         // the copies of a1 / a2 have read R before the epilogues of phases 1 / 2 overwrite it, and have landed in
         // global memory before phase 3 reads act2 back (phase 4 reads act1, copied earlier)
-        if (copier && (p == 1 || p == 2)) bulk_wait_read();
-        if (copier && p == 3) bulk_wait();
+        if (ACT == ACT_CELU && copier && (p == 1 || p == 2)) bulk_wait_read();
+        if (ACT == ACT_CELU && copier && p == 3) bulk_wait();
         // every warp of the warpgroup is done reading R before any of them overwrites it
         if (p < 5) wg_bar(wg);
         switch (p) {
-          case 0: res_epilogue<0, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          case 1: res_epilogue<1, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          case 2: res_epilogue<2, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          case 3: res_epilogue<3, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          case 4: res_epilogue<4, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
-          default: res_epilogue<5, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 0: res_epilogue<0, ACT, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 1: res_epilogue<1, ACT, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 2: res_epilogue<2, ACT, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 3: res_epilogue<3, ACT, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          case 4: res_epilogue<4, ACT, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
+          default: res_epilogue<5, ACT, SLABS>(F, sp, rt, m, n0, bn, acc, res_u32, s_blk, nblk, wg, lane, warp_in_wg, omax); break;
         }
         // this warpgroup's rows of the phase's output, visible to the next phase's wgmma
         if (p < 5) {
@@ -545,7 +570,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
         }
         // a1 / a2 to act1 / act2 for the dCELU epilogues: this warpgroup's 64 rows of each K-block and piece are 4 KB,
         // contiguous in R and in the tiled global operand
-        if (copier && p <= 1) {
+        if (ACT == ACT_CELU && copier && p <= 1) {
           unsigned char* ct = p == 0 ? F.act1 + ((size_t)rt * F.kb1 + (size_t)(m * sp.h1) / TK) * A_BLOCK_BYTES
                                      : F.act2 + ((size_t)rt * F.kb2 + (size_t)(m * sp.h2) / TK) * A_BLOCK_BYTES;
           const uint32_t off = wg * (64 / 8) * GROUP_BYTES;

@@ -201,11 +201,13 @@ class PackedNetworks:
 
     ``weights[member][species_index] = [(W [out,in], b [out]) x 4]`` in ``torch.nn.Linear``
     layout (nn/_core.py:117-149).  All members must share the layer widths of a species.
+    ``activation``: ``_lib.ACT_CELU`` (CELU(celu_alpha), every ``b`` given) or ``_lib.ACT_GELU`` (GELU, every ``b``
+    None: bias-free networks, the kernel model gets zeros it never reads).
     """
 
-    def __init__(self, weights: tp.Sequence[tp.Sequence[tp.Sequence[tp.Tuple[Tensor, Tensor]]]],
+    def __init__(self, weights: tp.Sequence[tp.Sequence[tp.Sequence[tp.Tuple[Tensor, tp.Optional[Tensor]]]]],
                  in_dim: int, device: torch.device, celu_alpha: float = 0.1, variant: tp.Optional[str] = None,
-                 radial_len: int = 0):
+                 radial_len: int = 0, activation: int = _lib.ACT_CELU):
         """``radial_len`` (number of radial AEV columns, S * len(ShfR)) > 0 and not a multiple of 32: the angular block
         of the layer-1 operands starts at the next 32-column boundary (``col_pad`` zero columns in between) if that
         still fits the padded width -- every element pair then fills exactly one 32-column GEMM block, and the
@@ -224,12 +226,16 @@ class PackedNetworks:
         if in_dim + self.col_pad > self.ldx or os.environ.get("ANI_B200_ALIGN_ANGULAR", "1") == "0":
             self.col_pad = 0
         self.celu_alpha = celu_alpha
+        if activation not in (_lib.ACT_CELU, _lib.ACT_GELU):
+            raise ValueError(f"unknown activation {activation!r} (engine: _lib.ACT_CELU or _lib.ACT_GELU)")
+        self.activation = activation
         self.dims: tp.List[tp.Tuple[int, int, int]] = []
         self._keep: tp.List[Tensor] = []
         self.model = MLPModel()
         mdl = self.model
         mdl.num_species, mdl.num_members, mdl.in_dim, mdl.ldx = S, M, in_dim, self.ldx
         mdl.celu_alpha = celu_alpha
+        mdl.activation = activation
         # Weights are gathered on the HOST into one flat float32 buffer (zero-padded to 32-column blocks),
         # uploaded with a single copy and re-laid out into the tiled B operands by this library's own
         # ani_b200_pack_b_operand kernel: no ATen kernel touches them (one launch per operand kind).
@@ -263,7 +269,10 @@ class PackedNetworks:
                 raise ValueError("first layer width does not match the AEV length")
             self.dims.append((h1, h2, h3))
             W = [[weights[m][s][k][0].detach().to("cpu", torch.float32) for m in range(M)] for k in range(4)]
-            Bv = [[weights[m][s][k][1].detach().to("cpu", torch.float32) for m in range(M)] for k in range(4)]
+            if any((weights[m][s][k][1] is None) != (activation == _lib.ACT_GELU) for m in range(M) for k in range(4)):
+                raise ValueError("CELU networks need biases in every layer, GELU networks have none")
+            Bv = [[torch.zeros(W[k][m].shape[0]) if weights[m][s][k][1] is None
+                   else weights[m][s][k][1].detach().to("cpu", torch.float32) for m in range(M)] for k in range(4)]
             for m in range(M):
                 if tuple(W[0][m].shape) != (h1, in_dim) or tuple(W[1][m].shape) != (h2, h1) \
                         or tuple(W[2][m].shape) != (h3, h2) or tuple(W[3][m].shape) != (1, h3):
@@ -361,6 +370,14 @@ class PackedNetworks:
     def ld(self) -> tp.Tuple[int, int, int]:
         M = self.num_members
         return M * self.model.h1_max, M * self.model.h2_max, M * self.model.h3_max
+
+    @property
+    def act_cols(self) -> tp.Tuple[int, int, int]:
+        """Columns of the act1 / act2 / act3 buffers: ``ld``, with room for the derivative operand of a GELU model
+        directly behind the activation operands act1 / act2 (include/ani_b200.h section 6)."""
+        ld1, ld2, ld3 = self.ld
+        k = 2 if self.activation == _lib.ACT_GELU else 1
+        return k * ld1, k * ld2, ld3
 
     def flops_per_atom(self, species_index: int, backward: bool = True) -> float:
         h1, h2, h3 = self.dims[species_index]
@@ -628,7 +645,7 @@ class Engine:
         key = (n_conf, n_per_conf)
         ws = self._ws.get(key)
         if ws is None:
-            ws = Workspace(n_conf, n_per_conf, self.consts.num_species, self.nets.ldx, self.nets.ld,
+            ws = Workspace(n_conf, n_per_conf, self.consts.num_species, self.nets.ldx, self.nets.act_cols,
                            self.nets.num_members, self.nbr_cap, self.device, variant=self.variant)
             if self.dispersion is not None:   # coordination numbers and dE/dCN of every atom (D3 scratch)
                 ws.d3_cn = torch.zeros(ws.n, dtype=torch.float32, device=self.device)

@@ -546,22 +546,26 @@ def aev_computer_from_torchani(aevr, neighborlist: NeighborlistArg = "cell_list"
 
 def networks_from_torchani(netr) -> AtomicContainer:
     """``torchani.nn.Ensemble`` / ``ANINetworks`` / ``BmmEnsemble`` (nn/_containers.py:319-660,
-    nn/_infer.py:61-216) -> the CUDA container with the same weights and active members."""
+    nn/_infer.py:61-216) -> the CUDA container with the same weights, activation and active members: CELU networks
+    with biases (ANI-1x / 2x) or GELU networks without (ANI-2xr / 2dr, ``simple_ani``)."""
     first = next(iter(netr.atomics.values())) if hasattr(netr, "atomics") else None
     # (BmmEnsemble does not carry atomic_numbers: the keys of `atomics` are the symbols everywhere)
     symbols = tuple(netr.atomics.keys()) if first is not None else tuple(netr.members[0].atomics.keys())
     per_member: tp.List[tp.Dict[str, tp.List[tp.Tuple[Tensor, tp.Optional[Tensor]]]]] = []
     if hasattr(netr, "members"):
+        activation = netr.members[0].atomics[symbols[0]].activation
         for rm in netr.members:
             per_member.append({s: [(l.weight, l.bias) for l in list(rm.atomics[s].layers) + [rm.atomics[s].final_layer]]
                                for s in symbols})
     elif first is not None and hasattr(first, "_num_batched_networks"):
-        # BmmAtomicNetwork: weights stacked as (members, in, out), biases (members, 1, out)
+        # BmmAtomicNetwork: weights stacked as (members, in, out), biases (members, 1, out); _beta == 0: no bias
+        activation = first.activation
         for m in range(int(first._num_batched_networks)):
             per_member.append({s: [(l.weight[m].t(), l.bias[m, 0] if l._beta else None)
                                    for l in list(netr.atomics[s].layers) + [netr.atomics[s].final_layer]]
                                for s in symbols})
     else:
+        activation = first.activation
         per_member.append({s: [(l.weight, l.bias) for l in list(netr.atomics[s].layers) + [netr.atomics[s].final_layer]]
                            for s in symbols})
     members = []
@@ -569,13 +573,15 @@ def networks_from_torchani(netr) -> AtomicContainer:
         mods = {}
         for s in symbols:
             dims = [layers[s][0][0].shape[1]] + [w.shape[0] for w, _ in layers[s]]
-            an = AtomicNetwork(dims)
+            biases = {b is not None for _, b in layers[s]}
+            if len(biases) != 1:
+                raise ValueError("networks with biases in some layers only are not supported")
+            an = AtomicNetwork(dims, activation, bias=biases.pop())   # raises for unsupported kinds
             with torch.no_grad():
                 for (w_dst, b_dst), (w, b) in zip(an.linear_pairs(), layers[s]):
-                    if b is None:
-                        raise ValueError("bias-free networks are not supported")
                     w_dst.copy_(w)
-                    b_dst.copy_(b)
+                    if b_dst is not None:
+                        b_dst.copy_(b)
             mods[s] = an
         members.append(ANINetworks(mods))
     nets: AtomicContainer = Ensemble(members) if len(members) > 1 else members[0]

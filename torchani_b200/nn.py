@@ -37,27 +37,52 @@ class TightCELU(torch.nn.Module):
         return torch.nn.functional.celu(x, alpha=0.1)
 
 
+def activation_kind(activation: tp.Union[str, torch.nn.Module]) -> int:
+    """The kernels' code of an activation: ``_lib.ACT_CELU`` for "celu" / a ``TightCELU`` (this package's or the
+    reference's), ``_lib.ACT_GELU`` for "gelu" / ``torch.nn.GELU(approximate="none")``; ValueError otherwise."""
+    if isinstance(activation, str):
+        kinds = {"celu": _lib.ACT_CELU, "gelu": _lib.ACT_GELU}
+        if activation not in kinds:
+            raise ValueError(f"activation {activation!r}: the MLP kernels implement 'celu' (CELU(alpha=0.1)) and "
+                             "'gelu' (exact-erf GELU) only")
+        return kinds[activation]
+    if type(activation).__name__ == "TightCELU":
+        return _lib.ACT_CELU
+    if type(activation) is torch.nn.GELU:
+        if activation.approximate != "none":
+            raise ValueError(f"GELU(approximate={activation.approximate!r}): the MLP kernels implement the exact-erf "
+                             "GELU (approximate='none') only")
+        return _lib.ACT_GELU
+    raise ValueError(f"activation {activation!r}: the MLP kernels implement TightCELU (CELU(alpha=0.1)) and "
+                     "torch.nn.GELU(approximate='none') only")
+
+
 class AtomicNetwork(torch.nn.Module):
     """Parameter holder with the module tree of nn/_core.py:117-160.  The CUDA kernels support
-    3 hidden layers + scalar output, CELU(0.1), with biases (the ANI-1x/2x/1ccx nets)."""
+    3 hidden layers + scalar output, in two kinds: CELU(0.1) with biases (the ANI-1x/2x/1ccx nets) and exact-erf
+    GELU without biases (ANI-2xr / ANI-2dr and the models ``simple_ani`` assembles)."""
 
     def __init__(self, layer_dims: tp.Sequence[int], activation: tp.Union[str, torch.nn.Module] = "celu",
                  bias: bool = True) -> None:
         super().__init__()
         if any(d <= 0 for d in layer_dims):
             raise ValueError("Layer dims must be strict positive integers")
-        if not (activation == "celu" or isinstance(activation, TightCELU)):
-            raise ValueError("the MLP kernels implement CELU(alpha=0.1) only")
-        if not bias:
-            raise ValueError("the MLP kernels expect biases")
+        kind = activation_kind(activation)
+        if kind == _lib.ACT_CELU and not bias:
+            raise ValueError("CELU networks without biases are not supported: the MLP kernels run CELU networks "
+                             "with biases and GELU networks without")
+        if kind == _lib.ACT_GELU and bias:
+            raise ValueError("GELU networks with biases are not supported: the MLP kernels run GELU networks "
+                             "without biases (bias=False) and CELU networks with")
         dims = tuple(layer_dims)
         self.layers = torch.nn.ModuleList(
-            [torch.nn.Linear(i, o, bias=True) for i, o in zip(dims[:-2], dims[1:-1])])
-        self.final_layer = torch.nn.Linear(dims[-2], dims[-1], bias=True)
-        self.activation = TightCELU()
-        self.has_biases = True
+            [torch.nn.Linear(i, o, bias=bias) for i, o in zip(dims[:-2], dims[1:-1])])
+        self.final_layer = torch.nn.Linear(dims[-2], dims[-1], bias=bias)
+        self.activation = TightCELU() if kind == _lib.ACT_CELU else torch.nn.GELU()
+        self.has_biases = bias
+        self.activation_kind = kind
 
-    def linear_pairs(self) -> tp.List[tp.Tuple[Tensor, Tensor]]:
+    def linear_pairs(self) -> tp.List[tp.Tuple[Tensor, tp.Optional[Tensor]]]:
         return [(l.weight, l.bias) for l in list(self.layers) + [self.final_layer]]
 
     def forward(self, features: Tensor) -> Tensor:
@@ -109,8 +134,7 @@ class _MLPFunction(torch.autograd.Function):
             xp[:, :D].index_add_(0, rows, src)
         x_tiled = tile_a_operand(xp, variant=nets.variant)                    # the GEMM consumes the tiled form
         x = torch.zeros(rows_cap, ldx, dtype=torch.float32, device=dev)   # dE/dAEV comes back as plain rows
-        ld = nets.ld
-        act1, act2, act3 = (operand_buffer(rows_cap, w, dev, nets.variant) for w in ld)
+        act1, act2, act3 = (operand_buffer(rows_cap, w, dev, nets.variant) for w in nets.act_cols)
         status = torch.zeros(1, dtype=torch.int32, device=dev)
         e_member = torch.zeros(M, rows_cap, dtype=torch.float32, device=dev)
         check(L.ani_b200_mlp_forward_backward(C.byref(nets.model), ptr(x_tiled), ptr(x), rows_cap,
@@ -236,7 +260,8 @@ class AtomicContainer(torch.nn.Module):
             weights = [[m.atomics[s].linear_pairs() for s in m.atomics] for m in members]
             in_dim = members[0].in_dim
             self._packed = PackedNetworks(weights, in_dim, device, variant=self._variant,
-                                          radial_len=getattr(self, "_radial_len", 0))
+                                          radial_len=getattr(self, "_radial_len", 0),
+                                          activation=members[0].activation_kind)
             self._packed.set_active_members(self.active_members_idxs)
             self._packed_key = key
         return self._packed
@@ -281,6 +306,10 @@ class ANINetworks(AtomicContainer):
         first = next(iter(self.atomics.values()))
         self.out_dim: int = first.final_layer.out_features
         self.in_dim: int = first.layers[0].in_features
+        if len({m.activation_kind for m in self.atomics.values()}) != 1:
+            raise ValueError("all networks of a container must share one activation (the MLP kernels run one per "
+                             "model)")
+        self.activation_kind: int = first.activation_kind
 
     def __getitem__(self, idx: str) -> AtomicNetwork:
         return self.atomics[idx]
@@ -299,19 +328,37 @@ class ANINetworks(AtomicContainer):
     # -- constructors (nn/_containers.py:423-570) ------------------------------------------
     @classmethod
     def build(cls, symbols: tp.Sequence[str], in_dim: int, dims: tp.Dict[str, tp.Tuple[int, ...]],
-              out_dim: int = 1, default_dims: tp.Tuple[int, ...] = ()):
-        return cls({s: AtomicNetwork((in_dim,) + tuple(dims.get(s, default_dims)) + (out_dim,)) for s in symbols})
+              out_dim: int = 1, activation: tp.Union[str, torch.nn.Module] = "gelu", bias: bool = False,
+              default_dims: tp.Tuple[int, ...] = ()):
+        return cls({s: AtomicNetwork((in_dim,) + tuple(dims.get(s, default_dims)) + (out_dim,), activation, bias)
+                    for s in symbols})
 
     @classmethod
-    def like_2x(cls, symbols: tp.Sequence[str] = ("H", "C", "N", "O", "S", "F", "Cl"), in_dim: int = 1008):
+    def like_2x(cls, symbols: tp.Sequence[str] = ("H", "C", "N", "O", "S", "F", "Cl"), in_dim: int = 1008,
+                out_dim: int = 1, activation: tp.Union[str, torch.nn.Module] = "celu", bias: bool = True):
         dims = {"H": (256, 192, 160), "C": (224, 192, 160), "N": (192, 160, 128), "O": (192, 160, 128),
                 "S": (160, 128, 96), "F": (160, 128, 96), "Cl": (160, 128, 96)}
-        return cls.build(symbols, in_dim, dims, default_dims=(160, 128, 96))
+        return cls.build(symbols, in_dim, dims, out_dim, activation, bias, default_dims=(160, 128, 96))
 
     @classmethod
-    def like_1x(cls, symbols: tp.Sequence[str] = ("H", "C", "N", "O"), in_dim: int = 384):
+    def like_dr(cls, symbols: tp.Sequence[str] = ("H", "C", "N", "O", "S", "F", "Cl"), in_dim: int = 1008,
+                out_dim: int = 1, activation: tp.Union[str, torch.nn.Module] = "gelu", bias: bool = False):
+        """The networks of ANI-2dr (nn/_containers.py:447-478): GELU, no biases by default."""
+        dims = {"H": (256, 192, 160), "C": (256, 192, 160), "N": (192, 160, 128), "O": (192, 160, 128),
+                "S": (160, 128, 96), "F": (160, 128, 96), "Cl": (160, 128, 96)}
+        return cls.build(symbols, in_dim, dims, out_dim, activation, bias, default_dims=(160, 128, 96))
+
+    @classmethod
+    def default(cls, symbols: tp.Sequence[str], in_dim: int, out_dim: int = 1,
+                activation: tp.Union[str, torch.nn.Module] = "gelu", bias: bool = False):
+        """The networks ``simple_ani`` assembles (nn/_containers.py:531-540): ANI-2x widths, GELU, no biases."""
+        return cls.like_2x(symbols, in_dim, out_dim, activation, bias)
+
+    @classmethod
+    def like_1x(cls, symbols: tp.Sequence[str] = ("H", "C", "N", "O"), in_dim: int = 384, out_dim: int = 1,
+                activation: tp.Union[str, torch.nn.Module] = "celu", bias: bool = True):
         dims = {"H": (160, 128, 96), "C": (144, 112, 96), "N": (128, 112, 96), "O": (128, 112, 96)}
-        return cls.build(symbols, in_dim, dims, default_dims=(128, 112, 96))
+        return cls.build(symbols, in_dim, dims, out_dim, activation, bias, default_dims=(128, 112, 96))
 
 
 class ANIModel(ANINetworks):
@@ -337,6 +384,9 @@ class Ensemble(AtomicContainer):
         self.num_species = modules[0].num_species
         if any(m.num_species != self.num_species for m in modules):
             raise ValueError("All modules must support the same number of elements")
+        if any(m.activation_kind != modules[0].activation_kind for m in modules):
+            raise ValueError("all members of an ensemble must share one activation (the MLP kernels run one per "
+                             "model)")
         self.register_buffer("atomic_numbers", modules[0].atomic_numbers, persistent=False)
 
     def __len__(self) -> int:
