@@ -811,57 +811,69 @@ __global__ void __launch_bounds__(THREADS, 1) k_gemm_wg(const __grid_constant__ 
     const int nsl = __shfl_sync(ANI_FULL_MASK, (bn + 63) / 64, 0);
     if (wg == 0 && leader) stamp(tloc, 1, 0);
     float acc[4][32];
+    // NSL = nsl at compile time: a K-block's products are then one branch-free commit group (a run-time slice count
+    // inside the group split it into one wgmma group per branch, so wgmma.wait_group 1 waited for all of them).  Only
+    // the NSL slices the epilogue reads are zeroed: zeros in the others would be copied into them at every exit.
+    auto main_loop = [&](auto nsl_) {
+      constexpr int NSL = decltype(nsl_)::value;
 #pragma unroll
-    for (int c = 0; c < 4; ++c)
+      for (int c = 0; c < NSL; ++c)
 #pragma unroll
-      for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
-    uint32_t prev = 0;
-    for (int kb = 0; kb < nkb; ++kb) {
-      mbar_wait(&full[stage], phase);
-      if (wg == 0 && leader && kb == 0) stamp(tloc, 1, 1);
-      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + wg * (64 / 8) * GROUP_BYTES;  // this warpgroup's rows
-      const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES) + A_BLOCK_BYTES;
-      wgmma_fence();
+        for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+      uint32_t prev = 0;
+#pragma unroll 1
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        if (wg == 0 && leader && kb == 0) stamp(tloc, 1, 1);
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + wg * (64 / 8) * GROUP_BYTES;  // this warpgroup's rows
+        const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES) + A_BLOCK_BYTES;
+        wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < TK / 16; ++k) {
-        const uint32_t adv = 32u * k;  // 16 pieces = 32 B along the swizzle row
-        uint64_t da[PARTS];
+        for (int k = 0; k < TK / 16; ++k) {
+          const uint32_t adv = 32u * k;  // 16 pieces = 32 B along the swizzle row
+          uint64_t da[PARTS];
 #pragma unroll
-        for (int p = 0; p < PARTS; ++p) da[p] = make_desc(sa + p * A_PART_BYTES + adv);
+          for (int p = 0; p < PARTS; ++p) da[p] = make_desc(sa + p * A_PART_BYTES + adv);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          if (c >= nsl) break;
-          uint64_t db[PARTS];
+          for (int c = 0; c < NSL; ++c) {
+            uint64_t db[PARTS];
 #pragma unroll
-          for (int p = 0; p < PARTS; ++p) db[p] = make_desc(sb + p * b_bytes + c * (64 / 8) * GROUP_BYTES + adv);
-          auto mma = [&](int pa, int pb) { wgmma_n64(acc[c], da[pa], db[pb]); };
-          // smallest terms first
+            for (int p = 0; p < PARTS; ++p) db[p] = make_desc(sb + p * b_bytes + c * (64 / 8) * GROUP_BYTES + adv);
+            auto mma = [&](int pa, int pb) { wgmma_n64(acc[c], da[pa], db[pb]); };
+            // smallest terms first
 #if ANI_OPND_FP16X2
-          mma(1, 0);
-          mma(0, 1);
-          mma(0, 0);
+            mma(1, 0);
+            mma(0, 1);
+            mma(0, 0);
 #else
-          mma(2, 0);
-          mma(0, 2);
-          mma(1, 1);
-          mma(1, 0);
-          mma(0, 1);
-          mma(0, 0);
+            mma(2, 0);
+            mma(0, 2);
+            mma(1, 1);
+            mma(1, 0);
+            mma(0, 1);
+            mma(0, 0);
 #endif
+          }
+        }
+        wgmma_commit();
+        // the previous K-block's products have retired: its slot goes back to the producer
+        wgmma_wait<1>();
+        if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
         }
       }
-      wgmma_commit();
-      // the previous K-block's products have retired: its slot goes back to the producer
-      wgmma_wait<1>();
-      if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
-      prev = stage;
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
+      wgmma_wait<0>();
+      if (nkb > 0 && lane == 0) mbar_arrive(&empty[prev]);
+    };
+    switch (nsl) {
+      case 1: main_loop(std::integral_constant<int, 1>{}); break;
+      case 2: main_loop(std::integral_constant<int, 2>{}); break;
+      case 3: main_loop(std::integral_constant<int, 3>{}); break;
+      default: main_loop(std::integral_constant<int, 4>{}); break;
     }
-    wgmma_wait<0>();
-    if (nkb > 0 && lane == 0) mbar_arrive(&empty[prev]);
     if (wg == 0 && leader) stamp(tloc, 1, 2);
     // the stored activation of EPI_MUL_DCELU was written by other CTAs: acquire its counters in this warpgroup too
     if (F.sync && F.epi[un.p] == EPI_MUL_DCELU) {

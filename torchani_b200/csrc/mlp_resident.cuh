@@ -130,14 +130,17 @@ __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_g
   "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
 #define ANI_RES_F16(d, i) ANI_RES_F8(d, i), ANI_RES_F8(d, i + 8)
 #define ANI_RES_F32(d) ANI_RES_F16(d, 0), ANI_RES_F16(d, 16)
-#define ANI_RES_WGMMA(N, REGS, DESCS, ...)                                                                   \
-  __device__ __forceinline__ void wgmma_res_n##N(float (&d0)[32], float (&d1)[32], uint64_t da, uint64_t db) { \
-    (void)d1;                                                                                                \
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"                                            \
-                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." ANI_WGMMA_AB " {" REGS "}, " DESCS        \
-                 ", p, 1, 1, 0, 0;\n\t}"                                                                     \
-                 : __VA_ARGS__                                                                               \
-                 : "l"(da), "l"(db));                                                                        \
+template <int N>
+__device__ __forceinline__ void wgmma_res(float (&d0)[32], float (&d1)[32], uint64_t da, uint64_t db);
+#define ANI_RES_WGMMA(N, REGS, DESCS, ...)                                                                       \
+  template <>                                                                                                    \
+  __device__ __forceinline__ void wgmma_res<N>(float (&d0)[32], float (&d1)[32], uint64_t da, uint64_t db) {     \
+    (void)d1;                                                                                                    \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"                                                \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." ANI_WGMMA_AB " {" REGS "}, " DESCS            \
+                 ", p, 1, 1, 0, 0;\n\t}"                                                                         \
+                 : __VA_ARGS__                                                                                   \
+                 : "l"(da), "l"(db));                                                                            \
   }
 ANI_RES_WGMMA(32, ANI_RES_REGS16, "%16, %17", ANI_RES_F16(d0, 0))
 ANI_RES_WGMMA(64, ANI_RES_REGS32, "%32, %33", ANI_RES_F32(d0))
@@ -152,21 +155,30 @@ ANI_RES_WGMMA(128, ANI_RES_REGS64, "%64, %65", ANI_RES_F32(d0), ANI_RES_F32(d1))
 #undef ANI_RES_REGS32
 #undef ANI_RES_REGS16
 
-// The three products of the 2 x fp16 split for one K-step and one ring slot of N = w columns (smallest terms first)
-__device__ __forceinline__ void res_mma_slot(float (&d0)[32], float (&d1)[32], const uint64_t (&da)[PARTS],
-                                             const uint64_t (&db)[PARTS], int w) {
-  switch (w) {
-#define ANI_RES_MMA3(N)                    \
-  case N:                                  \
-    wgmma_res_n##N(d0, d1, da[1], db[0]); \
-    wgmma_res_n##N(d0, d1, da[0], db[1]); \
-    wgmma_res_n##N(d0, d1, da[0], db[0]); \
-    break;
-    ANI_RES_MMA3(32) ANI_RES_MMA3(64) ANI_RES_MMA3(96)
-    default: ANI_RES_MMA3(128)
-#undef ANI_RES_MMA3
+// One commit group: the three products of the 2 x fp16 split (smallest terms first) of every K-step of one K-block, A
+// at sa and the N B rows of one ring slot at sb.  N is a compile-time width because ptxas closes every branch inside a
+// group with its own wgmma group boundary: a run-time width there split the group into one group per K-step, so
+// wgmma.wait_group 1 waited for all of them, and ptxas injected a warpgroup.arrive (C7519) before every run.
+template <int N>
+__device__ __forceinline__ void res_mma_group(float (&d0)[32], float (&d1)[32], uint32_t sa, uint32_t sb) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < TK / 16; ++k) {
+    const uint32_t adv = 32u * k;  // 16 pieces = 32 B along the swizzle row
+    uint64_t da[PARTS], db[PARTS];
+#pragma unroll
+    for (int pp = 0; pp < PARTS; ++pp) {
+      da[pp] = make_desc(sa + pp * A_PART_BYTES + adv);
+      db[pp] = make_desc(sb + pp * A_PART_BYTES + adv);
+    }
+    wgmma_res<N>(d0, d1, da[1], db[0]);
+    wgmma_res<N>(d0, d1, da[0], db[1]);
+    wgmma_res<N>(d0, d1, da[0], db[0]);
   }
+  wgmma_commit();
 }
+template <int N>
+using ResWidth = std::integral_constant<int, N>;
 
 // chain c of the list: species in `order`, then row tile, then member (SLABS: the members of member_of only).
 // false: past the end
@@ -482,73 +494,68 @@ __global__ void __launch_bounds__(THREADS, 1) k_mlp_resident(const __grid_consta
       for (int n0 = 0; n0 < n; n0 += TN_MAX) {
         const int bn = min(TN_MAX, n - n0);
         const int a_sl = p == 0 ? 1 : 0, nslot = a_sl + (bn + RES_HALF - 1) / RES_HALF;
-        // one wgmma per B slot and product, as wide as the slot's rows: 128, or the 32-128 columns of the remainder
-        const int w0 = min(bn, RES_HALF), w1 = bn - w0;
         float acc[4][32];
-#pragma unroll
-        for (int cc = 0; cc < 4; ++cc)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) acc[cc][i] = 0.f;
-        // A K-block's products are two commit groups, one per B slot (the second only if w1 > 0).  Every slot goes back
+        // A K-block's products are two commit groups, one per B slot (the second only if W1 > 0).  Every slot goes back
         // to the producer as soon as the last group that reads it has retired: B rows 0-127 after group 1, the A slot
         // (phase 0) and B rows 128-255 after group 2.  One group stays queued behind the one retiring, so the tensor
         // pipe keeps its overlap while the ring keeps as many slots in flight as it can (the weight feed is bound by
         // L2 latency, DESIGN §4.1).  The two groups accumulate into different registers, so the sums are those of
         // one interleaved group.
-        uint32_t prev = 0, held = 0;  // slots prev + j (bit j of held) still read by the previous K-block's last group
         auto release = [&](uint32_t base, uint32_t mask) {
           if (lane == 0)
             for (int j = 0; j < 3; ++j)
               if (mask >> j & 1) mbar_arrive(&empty[(base + j) % RES_SLOTS]);
         };
-        for (int kb = 0; kb < nkb; ++kb) {
-          for (int j = 0; j <= a_sl; ++j) mbar_wait(&full[(u + j) % RES_SLOTS], ((u + j) / RES_SLOTS) & 1);
-          const uint32_t sa = p == 0 ? smem_u32(ring + (u % RES_SLOTS) * RES_SLOT_BYTES) + wg * (64 / 8) * GROUP_BYTES
-                                     : res_a + kb * A_BLOCK_BYTES;
-          // B rows 0-127 and 128-255
-          const uint32_t sb0 = smem_u32(ring + ((u + a_sl) % RES_SLOTS) * RES_SLOT_BYTES);
-          const uint32_t sb1 = smem_u32(ring + ((u + a_sl + 1) % RES_SLOTS) * RES_SLOT_BYTES);
-          wgmma_fence();
+        // W0 / W1: the B rows of the K-block's two slots, as wide as each wgmma of the slot (the 32-128 columns of the
+        // remainder, so no MMA runs on padding)
+        auto main_loop = [&](auto w0_, auto w1_) {
+          constexpr int W0 = decltype(w0_)::value, W1 = decltype(w1_)::value;
+          // zero only the W0 + W1 columns the instance accumulates and the epilogue reads (w columns of a 64-column
+          // slice are its registers 0 .. w / 2 - 1): the others stay dead, where zeros would be copied into every one
+          // of them at the exit of every instance
+          auto zero = [&](float (&d)[32], int w) {
 #pragma unroll
-          for (int k = 0; k < TK / 16; ++k) {
-            const uint32_t adv = 32u * k;  // 16 pieces = 32 B along the swizzle row
-            uint64_t da[PARTS];
-#pragma unroll
-            for (int pp = 0; pp < PARTS; ++pp) da[pp] = make_desc(sa + pp * A_PART_BYTES + adv);
-            uint64_t db[PARTS];
-#pragma unroll
-            for (int pp = 0; pp < PARTS; ++pp) db[pp] = make_desc(sb0 + pp * A_PART_BYTES + adv);
-            res_mma_slot(acc[0], acc[1], da, db, w0);
-          }
-          wgmma_commit();
-          wgmma_wait<1>();
-          release(prev, held);
-          if (w1 > 0) {
-            mbar_wait(&full[(u + a_sl + 1) % RES_SLOTS], ((u + a_sl + 1) / RES_SLOTS) & 1);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < TK / 16; ++k) {
-              const uint32_t adv = 32u * k;
-              uint64_t da[PARTS];
-#pragma unroll
-              for (int pp = 0; pp < PARTS; ++pp) da[pp] = make_desc(sa + pp * A_PART_BYTES + adv);
-              uint64_t db[PARTS];
-#pragma unroll
-              for (int pp = 0; pp < PARTS; ++pp) db[pp] = make_desc(sb1 + pp * A_PART_BYTES + adv);
-              res_mma_slot(acc[2], acc[3], da, db, w1);
-            }
-            wgmma_commit();
+            for (int i = 0; i < 32; ++i)
+              if (i < w / 2) d[i] = 0.f;
+          };
+          zero(acc[0], min(W0, 64));
+          zero(acc[1], W0 - 64);
+          zero(acc[2], min(W1, 64));
+          zero(acc[3], W1 - 64);
+          uint32_t prev = 0, held = 0;  // slots prev + j (bit j of held) still read by the previous K-block's last group
+#pragma unroll 1
+          for (int kb = 0; kb < nkb; ++kb) {
+            for (int j = 0; j <= a_sl; ++j) mbar_wait(&full[(u + j) % RES_SLOTS], ((u + j) / RES_SLOTS) & 1);
+            const uint32_t sa = p == 0 ? smem_u32(ring + (u % RES_SLOTS) * RES_SLOT_BYTES) + wg * (64 / 8) * GROUP_BYTES
+                                       : res_a + kb * A_BLOCK_BYTES;
+            res_mma_group<W0>(acc[0], acc[1], sa, smem_u32(ring + ((u + a_sl) % RES_SLOTS) * RES_SLOT_BYTES));
             wgmma_wait<1>();
-            release(u, 1u << a_sl);
-            held = ((1u << nslot) - 1) & ~(1u << a_sl);
-          } else {
-            held = (1u << nslot) - 1;
+            release(prev, held);
+            if constexpr (W1 > 0) {
+              mbar_wait(&full[(u + a_sl + 1) % RES_SLOTS], ((u + a_sl + 1) / RES_SLOTS) & 1);
+              res_mma_group<W1>(acc[2], acc[3], sa, smem_u32(ring + ((u + a_sl + 1) % RES_SLOTS) * RES_SLOT_BYTES));
+              wgmma_wait<1>();
+              release(u, 1u << a_sl);
+              held = ((1u << nslot) - 1) & ~(1u << a_sl);
+            } else {
+              held = (1u << nslot) - 1;
+            }
+            prev = u;
+            u += nslot;
           }
-          prev = u;
-          u += nslot;
+          wgmma_wait<0>();
+          release(prev, held);
+        };
+        switch (bn / 32) {  // W0 = min(bn, 128), W1 = bn - W0
+          case 1: main_loop(ResWidth<32>{}, ResWidth<0>{}); break;
+          case 2: main_loop(ResWidth<64>{}, ResWidth<0>{}); break;
+          case 3: main_loop(ResWidth<96>{}, ResWidth<0>{}); break;
+          case 4: main_loop(ResWidth<128>{}, ResWidth<0>{}); break;
+          case 5: main_loop(ResWidth<128>{}, ResWidth<32>{}); break;
+          case 6: main_loop(ResWidth<128>{}, ResWidth<64>{}); break;
+          case 7: main_loop(ResWidth<128>{}, ResWidth<96>{}); break;
+          default: main_loop(ResWidth<128>{}, ResWidth<128>{}); break;
         }
-        wgmma_wait<0>();
-        release(prev, held);
         // the copies of a1 / a2 have read R before the epilogues of phases 1 / 2 overwrite it, and have landed in
         // global memory before phase 3 reads act2 back (phase 4 reads act1, copied earlier)
         if (ACT == ACT_CELU && copier && (p == 1 || p == 2)) bulk_wait_read();
