@@ -69,6 +69,59 @@ def test_argument_validation_without_gpu():
     with pytest.raises(_lib.ANIB200Error):
         _lib.check(-2, "x")
 
+    # member lists of the step terms: the arguments are valid except where a case says otherwise.  The pointers are
+    # host dummies, so every call below must return before it touches CUDA; the pair and AEV-members calls with an
+    # empty atom range (lo == hi) and a valid list return OK there, which shows the other cases fail on their lists.
+    buf = (C.c_char * 4096)()
+    h = C.cast(buf, C.c_void_p)
+    ok_list = (C.c_int32 * 3)(0, 3, 7)
+    lists = {"count above 16": (ok_list, 17), "index out of range": ((C.c_int32 * 2)(0, 16), 2),
+             "negative index": ((C.c_int32 * 2)(-1, 0), 2), "null list": (None, 3)}
+    pp = _lib.PairParams()
+    pp.kind, pp.cutoff_fn, pp.num_species, pp.cutoff, pp.to_bohr = 0, 1, 7, 5.1, 1.8897
+    dp = _lib.D3Params()
+    dp.cutoff_fn, dp.num_species, dp.cutoff, dp.to_bohr = 1, 7, 8.0, 1.8897
+    ap = _lib.AEVParams()
+    ap.num_species, ap.n_shf_r, ap.n_shf_a, ap.n_shf_z, ap.cutoff_kind = 7, 16, 8, 4, 0
+    ap.rcr, ap.rca, ap.zeta = 5.1, 3.5, 14.1
+
+    def pair(members, n_members, lo=0, hi=4, member_atomic=h, grad_members=h):
+        return L.ani_b200_pair_potential(C.byref(pp), h, h, h, 4, lo, hi, 1, 4, h, h, 32, h, h, h, h, member_atomic,
+                                         grad_members, members, n_members, None)
+
+    def d3(members, n_members, member_atomic=h, grad_members=h, cells=False, lattice=h):
+        args = (C.byref(dp), h, h, h, h, h, 4, 0, 4, 1, 4, 1.0, h, h, h, h, h, h, member_atomic, grad_members, members,
+                n_members, h)
+        if cells:
+            return L.ani_b200_dispersion_d3_cells(*args, lattice, None)
+        return L.ani_b200_dispersion_d3(*args, None)
+
+    def aev_members(members, n_members, lo=0, hi=4):
+        return L.ani_b200_aev_backward_members(C.byref(ap), h, h, h, h, 4, lo, hi, h, h, 1008, 1008, members,
+                                               n_members, h, h, 64, h, h, 0, None)
+
+    def qbc(members, n_members):
+        return L.ani_b200_ensemble_qbc(h, members, n_members, h, h, None, 1, 4, h, h, h, h, None)
+
+    assert pair(ok_list, 3, hi=0) == 0
+    assert aev_members(ok_list, 3, hi=0) == 0
+    for case, (members, n_members) in lists.items():
+        assert pair(members, n_members) == -1, case
+        assert d3(members, n_members) == -1, case
+        assert d3(members, n_members, cells=True) == -1, case
+        assert aev_members(members, n_members) == -1, case
+        assert qbc(members, n_members) == -1, case
+    # member outputs with no members
+    assert pair(None, 0, grad_members=None) == -1
+    assert pair(None, 0, member_atomic=None) == -1
+    assert d3(None, 0, grad_members=None) == -1
+    assert d3(None, 0, member_atomic=None, cells=True) == -1
+    # zero members where the call needs one
+    assert aev_members(ok_list, 0) == -1
+    assert qbc(ok_list, 0) == -1
+    # the _cells form of D3 without its lattice table
+    assert d3(ok_list, 3, cells=True, lattice=None) == -1
+
 
 def test_product_package_does_not_import_the_oracle():
     """The oracle is test infrastructure: nothing under torchani_b200/ may reference it."""

@@ -21,6 +21,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "terms.cuh"
 
 namespace ani {
 
@@ -1341,9 +1342,7 @@ __global__ void __launch_bounds__(AEV_WARPS * 32, ANI_AEV_BWD_MIN_CTAS)
 // backward of every ensemble member in one launch (query-by-committee statistics)
 // ---------------------------------------------------------------------------------------
 // Active members of an ani_b200_aev_backward_members call: output k contracts slab idx[k]
-struct MemberSlabs {
-  int count;
-  int idx[ANI_MAX_MEMBERS];
+struct MemberSlabs : ActiveMembers {
   long long stride;  // floats between the dE/dAEV slabs of consecutive members
 };
 
@@ -1671,15 +1670,11 @@ static int launch_aev_backward_members(const ani_aev_params* params, const ani_g
                                nbr_cap);
   if (rc != ANI_OK) return rc;
   if (!nbr_cnt || !nbr_list) return ANI_ERR_BAD_ARG;
-  if (n_members < 1 || n_members > ANI_MAX_MEMBERS || !members || slab_stride < (long long)ldx) return ANI_ERR_BAD_ARG;
+  if (n_members < 1 || slab_stride < (long long)ldx) return ANI_ERR_BAD_ARG;
   MemberSlabs ms;
-  ms.count = n_members;
+  rc = active_members(members, n_members, ms);
+  if (rc != ANI_OK) return rc;
   ms.stride = slab_stride;
-  for (int k = 0; k < ANI_MAX_MEMBERS; ++k) ms.idx[k] = 0;
-  for (int k = 0; k < n_members; ++k) {
-    if (members[k] < 0 || members[k] >= ANI_MAX_MEMBERS) return ANI_ERR_BAD_ARG;
-    ms.idx[k] = members[k];
-  }
   if (hi == lo) return ANI_OK;
   // two gradient tables (double-buffered rows), plus dfc per neighbour
   const GradTable t = grad_table(params, species_mask, max_elements, slabs, ldx, slab_stride);

@@ -37,18 +37,13 @@
 // passes 1-2 run over all atoms on every rank.  Passes 2 and 3 search again instead of reading a list written by
 // pass 1 (DESIGN section 4.6): no capacity, no overflow mode.
 // Arithmetic: expf and true divisions, as csrc/pair.cu.
-#include "common.cuh"
+#include "terms.cuh"
 
 namespace ani {
 
 constexpr int D3_WARPS = 8;
 constexpr int D3_REFS = 25;   // 5 x 5 reference pairs per element pair
 constexpr float D3_LN_EPS = -80.5904782547916f;   // ln(1e-35), the eps of dftd3.py:177
-
-struct D3Members {
-  int count;
-  int idx[ANI_MAX_MEMBERS];
-};
 
 // largest bucket b with bin_start[b] <= i: the bucket of sorted atom i (empty buckets share their start with the next)
 __device__ __forceinline__ int bucket_of(const int32_t* __restrict__ bin_start, int nbins, int i) {
@@ -232,21 +227,6 @@ __device__ __forceinline__ void d3_energy(const ani_d3_params& P, int a, int b, 
   de_dc6 = per_c6 * f;
 }
 
-__device__ __forceinline__ void add_outer(float (&vir)[9], float fx, float fy, float fz, float dx, float dy, float dz) {
-  vir[0] = fmaf(fx, dx, vir[0]); vir[1] = fmaf(fx, dy, vir[1]); vir[2] = fmaf(fx, dz, vir[2]);
-  vir[3] = fmaf(fy, dx, vir[3]); vir[4] = fmaf(fy, dy, vir[4]); vir[5] = fmaf(fy, dz, vir[5]);
-  vir[6] = fmaf(fz, dx, vir[6]); vir[7] = fmaf(fz, dy, vir[7]); vir[8] = fmaf(fz, dz, vir[8]);
-}
-
-struct D3Out {
-  float* atomic;
-  double* energies;
-  float* grad;
-  double* virial;
-  float* member_atomic;
-  float* grad_members;
-};
-
 // PASS 1: cn of every real atom.  PASS 2: dedcn of every real atom, energies + direct gradient / virial of the owned
 // atoms.  PASS 3: chain gradient / virial of the owned atoms.  One warp per sorted atom, first = lo (pass 3) or 0.
 template <int PASS, bool LAT, bool VIRIAL>
@@ -255,10 +235,8 @@ __global__ void __launch_bounds__(D3_WARPS * 32)
                     const ani_grid* __restrict__ grid, const int32_t* __restrict__ bin_start,
                     const float4* __restrict__ spos, const int32_t* __restrict__ sorted_orig, int n, int first, int lo,
                     int hi, int n_per_conf, float skin, const float* __restrict__ lattice, float* __restrict__ cn,
-                    float* __restrict__ dedcn, const __grid_constant__ D3Out out, const __grid_constant__ D3Members ms,
-                    int32_t* __restrict__ status) {
-  __shared__ float s_e[D3_WARPS];
-  __shared__ int s_conf[D3_WARPS];
+                    float* __restrict__ dedcn, const __grid_constant__ TermOut out,
+                    const __grid_constant__ ActiveMembers ms, int32_t* __restrict__ status) {
   __shared__ D3Hit s_q[D3_WARPS][D3_QUEUE];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const ani_grid g = *grid;
@@ -318,63 +296,12 @@ __global__ void __launch_bounds__(D3_WARPS * 32)
         if (lane == 0) (PASS == 1 ? cn : dedcn)[i] = acc;
       }
       if (PASS >= 2 && owned && si >= 0) {
-        gx = warp_sum(gx);
-        gy = warp_sum(gy);
-        gz = warp_sum(gz);
-        if (PASS == 2) e = warp_sum(e);
-        if (VIRIAL) {
-          double* slots = out.virial + (size_t)(g.mode >= 2 ? conf_i : 0) * ANI_VIRIAL_SLOTS * 9;
-#pragma unroll
-          for (int k = 0; k < 9; ++k) {
-            const float v = warp_sum(vir[k]);
-            if (lane == 0) atomicAdd(&slots[(blockIdx.x % ANI_VIRIAL_SLOTS) * 9 + k], 0.5 * (double)v);
-          }
-        }
-        if (lane == 0) {
-          if (PASS == 2) {
-            conf_out = conf_i;
-            e_out = e;
-            if (out.atomic) out.atomic[oi] += e;
-          }
-          if (out.grad) {
-            out.grad[3 * (size_t)oi + 0] += gx;
-            out.grad[3 * (size_t)oi + 1] += gy;
-            out.grad[3 * (size_t)oi + 2] += gz;
-          }
-          // the reference adds its potentials to every member of the ensemble (arch.py:365-378)
-          for (int k = 0; k < ms.count; ++k) {
-            if (PASS == 2 && out.member_atomic) out.member_atomic[(size_t)ms.idx[k] * n + oi] += e;
-            if (out.grad_members) {
-              float* gm = out.grad_members + ((size_t)k * n + oi) * 3;
-              gm[0] += gx;
-              gm[1] += gy;
-              gm[2] += gz;
-            }
-          }
-        }
+        e_out = add_atom_term<PASS == 2, VIRIAL>(out, ms, n, g.mode, oi, conf_i, e, gx, gy, gz, vir);
+        conf_out = conf_i;
       }
     }
   }
-  if (PASS != 2 || !out.energies) return;
-  if (lane == 0) {
-    s_e[warp] = e_out;
-    s_conf[warp] = conf_out;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {   // sorted atoms are conformer-major in a batch: runs of equal conformers, one atomic each
-    int c = -1;
-    double acc = 0.0;
-    for (int w = 0; w < D3_WARPS; ++w) {
-      if (s_conf[w] < 0) continue;
-      if (s_conf[w] != c) {
-        if (c >= 0) atomicAdd(&out.energies[c], acc);
-        c = s_conf[w];
-        acc = 0.0;
-      }
-      acc += (double)s_e[w];
-    }
-    if (c >= 0) atomicAdd(&out.energies[c], acc);
-  }
+  if (PASS == 2) add_conformer_energies<D3_WARPS>(out.energies, e_out, conf_out);
 }
 
 // ---- a caller's HALF pair list (not the hot path): one thread per pair, float atomics ----
@@ -416,11 +343,7 @@ __global__ void k_dispersion_d3_pairs(const __grid_constant__ ani_d3_params P, c
       de_dr *= 0.5f;
       de_dc6 *= 0.5f;
     }
-    if (atomic) {
-      atomicAdd(&atomic[i0], 0.5f * e);
-      atomicAdd(&atomic[i1], 0.5f * e);
-    }
-    if (energies) atomicAdd(&energies[i0 / n_per_conf], (double)e);
+    add_pair_energy(atomic, energies, i0, i1, n_per_conf, e);
     if (!grad) return;
     atomicAdd(&dedcn[i0], de_dc6 * dc60);
     atomicAdd(&dedcn[i1], de_dc6 * dc61);
@@ -430,21 +353,11 @@ __global__ void k_dispersion_d3_pairs(const __grid_constant__ ani_d3_params P, c
     d3_count(P, s0, s1, R, c, dc);
     sc = (dedcn[i0] + dedcn[i1]) * dc / R;
   }
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {   // dR/dx0 = diff / R
-    const float f = sc * diff[3 * p + k];
-    atomicAdd(&grad[3 * i0 + k], f);
-    atomicAdd(&grad[3 * i1 + k], -f);
-  }
+  add_pair_grad(grad, diff, p, i0, i1, sc);   // dR/dx0 = diff / R
 }
 
 static int check_d3_params(const ani_d3_params* p, const float* tables) {
-  if (!p || !tables) return ANI_ERR_BAD_ARG;
-  if (p->cutoff_fn < 0 || p->cutoff_fn > 2) return ANI_ERR_BAD_ARG;
-  if (p->num_species < 1 || p->num_species > ANI_MAX_SPECIES) return ANI_ERR_BAD_ARG;
-  if (!(p->to_bohr > 0.f)) return ANI_ERR_BAD_ARG;
-  if (p->cutoff_fn != 2 && !(p->cutoff > 0.f && p->cutoff < 1e30f)) return ANI_ERR_BAD_ARG;
-  return ANI_OK;
+  return tables ? check_term_params(p) : ANI_ERR_BAD_ARG;
 }
 
 static int launch_dispersion_d3(const ani_d3_params* params, const float* tables, const ani_grid* grid,
@@ -453,23 +366,16 @@ static int launch_dispersion_d3(const ani_d3_params* params, const float* tables
                                 float* atomic, double* energies, float* grad_coords, double* virial,
                                 float* member_atomic, float* grad_members, const int32_t* members, int n_members,
                                 int32_t* status, const float* lattice, bool want_lattice, void* stream) {
-  const int rc = check_d3_params(params, tables);
+  int rc = check_d3_params(params, tables);
   if (rc != ANI_OK) return rc;
   // the fused step searches its own neighbours: it needs a finite cutoff
   if (params->cutoff_fn == 2) return ANI_ERR_BAD_ARG;
-  if (!grid || !bin_start || !spos || !sorted_orig || !cn || !dedcn) return ANI_ERR_BAD_ARG;
-  if (want_lattice && !lattice) return ANI_ERR_BAD_ARG;
-  if (n_conf < 1 || n_per_conf < 1 || n != n_conf * n_per_conf || !(skin >= 0.f)) return ANI_ERR_BAD_ARG;
-  if (lo < 0 || hi > n || lo > hi) return ANI_ERR_BAD_ARG;
-  if (n_members < 0 || n_members > ANI_MAX_MEMBERS || (n_members > 0 && !members)) return ANI_ERR_BAD_ARG;
-  if ((member_atomic || grad_members) && n_members == 0) return ANI_ERR_BAD_ARG;
-  D3Members ms;
-  ms.count = n_members;
-  for (int k = 0; k < ANI_MAX_MEMBERS; ++k) {
-    ms.idx[k] = k < n_members ? members[k] : 0;
-    if (ms.idx[k] < 0 || ms.idx[k] >= ANI_MAX_MEMBERS) return ANI_ERR_BAD_ARG;
-  }
-  D3Out out{atomic, energies, grad_coords, virial, member_atomic, grad_members};
+  ActiveMembers ms;
+  rc = check_step_term_args(grid, spos, sorted_orig, n, lo, hi, n_conf, n_per_conf, lattice, want_lattice,
+                            member_atomic, grad_members, members, n_members, ms);
+  if (rc != ANI_OK) return rc;
+  if (!bin_start || !cn || !dedcn || !(skin >= 0.f)) return ANI_ERR_BAD_ARG;
+  const TermOut out{atomic, energies, grad_coords, virial, member_atomic, grad_members};
   const bool want_grad = grad_coords || grad_members || virial;
   const float4* tab = reinterpret_cast<const float4*>(tables);
   const float4* sp = reinterpret_cast<const float4*>(spos);

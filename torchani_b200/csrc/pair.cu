@@ -16,17 +16,11 @@
 //   ZBL  E = Z_a Z_b / d * sum_q c_q exp(-x_q * d * (Z_a^p + Z_b^p) / k)
 // Arithmetic: expf / sqrtf / powf and true divisions (the repulsion is of order 1 Ha at 0.4 A, so the approximate MUFU
 // forms of the AEV kernels would cost the 1e-5 relative bar on atomic energies); d^1.5 is d * sqrt(d).
-#include "common.cuh"
+#include "terms.cuh"
 
 namespace ani {
 
 constexpr int PAIR_WARPS = 8;
-
-// Active members of a query-by-committee step: output k of grad_members belongs to member idx[k] of member_atomic
-struct PairMembers {
-  int count;
-  int idx[ANI_MAX_MEMBERS];
-};
 
 // E(R) fc(R) and its derivative with respect to R (Angstrom) for the element pair (a, b)
 __device__ __forceinline__ void pair_energy(const ani_pair_params& P, int a, int b, float R, float& e, float& de) {
@@ -56,21 +50,16 @@ __device__ __forceinline__ void pair_energy(const ani_pair_params& P, int a, int
   de = fmaf(dE, f, E * df);
 }
 
-// One warp per sorted atom i in lo..hi-1.  Everything is ADDED to what the step has produced so far, by plain
-// read-modify-write: every output element of an atom has exactly one writer (the warp that owns the atom), and the
-// launch is ordered on the stream after the kernels that accumulate into the same buffers (the AEV backward's atomics
-// into grad, the energy reduction's stores into atomic / member_atomic / energies).  The conformer energies and the
-// virial slots have many contributors and take float64 atomics, one per CTA and conformer / one per warp.
+// One warp per sorted atom i in lo..hi-1.  Everything is ADDED to what the step has produced so far (the AEV
+// backward's atomics into grad, the energy reduction's stores into atomic / member_atomic / energies), by
+// add_atom_term and add_conformer_energies of terms.cuh.
 template <bool LAT, bool VIRIAL>
 __global__ void __launch_bounds__(PAIR_WARPS * 32)
     k_pair_potential(const __grid_constant__ ani_pair_params P, const ani_grid* __restrict__ grid,
                      const float4* __restrict__ spos, const int32_t* __restrict__ sorted_orig, int n, int lo, int hi,
                      int n_per_conf, const int32_t* __restrict__ nbr_cnt, const int32_t* __restrict__ nbr_list, int cap,
-                     const float* __restrict__ lattice, float* __restrict__ atomic, double* __restrict__ energies,
-                     float* __restrict__ grad, double* __restrict__ virial, float* __restrict__ member_atomic,
-                     float* __restrict__ grad_members, const __grid_constant__ PairMembers ms) {
-  __shared__ float s_e[PAIR_WARPS];
-  __shared__ int s_conf[PAIR_WARPS];
+                     const float* __restrict__ lattice, const __grid_constant__ TermOut out,
+                     const __grid_constant__ ActiveMembers ms) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const ani_grid g = *grid;
   hi = min(hi, g.n_real);
@@ -105,66 +94,14 @@ __global__ void __launch_bounds__(PAIR_WARPS * 32)
       gx -= fx;
       gy -= fy;
       gz -= fz;
-      if (VIRIAL) {
-        vir[0] = fmaf(fx, dx, vir[0]); vir[1] = fmaf(fx, dy, vir[1]); vir[2] = fmaf(fx, dz, vir[2]);
-        vir[3] = fmaf(fy, dx, vir[3]); vir[4] = fmaf(fy, dy, vir[4]); vir[5] = fmaf(fy, dz, vir[5]);
-        vir[6] = fmaf(fz, dx, vir[6]); vir[7] = fmaf(fz, dy, vir[7]); vir[8] = fmaf(fz, dz, vir[8]);
-      }
+      if (VIRIAL) add_outer(vir, fx, fy, fz, dx, dy, dz);
     }
-    e = warp_sum(e);
-    gx = warp_sum(gx);
-    gy = warp_sum(gy);
-    gz = warp_sum(gz);
-    if (VIRIAL) {
-      // slot rule of the AEV backward: one set of slots per conformer of a periodic batch (grid modes 2, 3)
-      double* slots = virial + (size_t)(g.mode >= 2 ? conf_i : 0) * ANI_VIRIAL_SLOTS * 9;
-#pragma unroll
-      for (int k = 0; k < 9; ++k) {
-        const float v = warp_sum(vir[k]);
-        if (lane == 0) atomicAdd(&slots[(blockIdx.x % ANI_VIRIAL_SLOTS) * 9 + k], 0.5 * (double)v);
-      }
-    }
-    if (lane == 0 && si >= 0) {
+    if (si >= 0) {
+      e_out = add_atom_term<true, VIRIAL>(out, ms, n, g.mode, oi, conf_i, e, gx, gy, gz, vir);
       conf_out = conf_i;
-      e_out = e;
-      if (atomic) atomic[oi] += e;
-      if (grad) {
-        grad[3 * (size_t)oi + 0] += gx;
-        grad[3 * (size_t)oi + 1] += gy;
-        grad[3 * (size_t)oi + 2] += gz;
-      }
-      // the reference adds a pair potential to every member of the ensemble (arch.py:365-378)
-      for (int k = 0; k < ms.count; ++k) {
-        if (member_atomic) member_atomic[(size_t)ms.idx[k] * n + oi] += e;
-        if (grad_members) {
-          float* gm = grad_members + ((size_t)k * n + oi) * 3;
-          gm[0] += gx;
-          gm[1] += gy;
-          gm[2] += gz;
-        }
-      }
     }
   }
-  if (!energies) return;
-  if (lane == 0) {
-    s_e[warp] = e_out;
-    s_conf[warp] = conf_out;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {   // sorted atoms are conformer-major in a batch: runs of equal conformers, one atomic each
-    int c = -1;
-    double acc = 0.0;
-    for (int w = 0; w < PAIR_WARPS; ++w) {
-      if (s_conf[w] < 0) continue;
-      if (s_conf[w] != c) {
-        if (c >= 0) atomicAdd(&energies[c], acc);
-        c = s_conf[w];
-        acc = 0.0;
-      }
-      acc += (double)s_e[w];
-    }
-    if (c >= 0) atomicAdd(&energies[c], acc);
-  }
+  add_conformer_energies<PAIR_WARPS>(out.energies, e_out, conf_out);
 }
 
 // The same potential over a caller-supplied HALF pair list (the reference's Neighbors tuple; diff = x[idx0] - x[idx1] +
@@ -188,29 +125,14 @@ __global__ void k_pair_potential_pairs(const __grid_constant__ ani_pair_params P
     e *= 0.5f;
     de *= 0.5f;
   }
-  if (atomic) {
-    atomicAdd(&atomic[i0], 0.5f * e);
-    atomicAdd(&atomic[i1], 0.5f * e);
-  }
-  if (energies) atomicAdd(&energies[i0 / n_per_conf], (double)e);
-  if (grad) {
-    const float sc = R >= 1e-7f ? de / R : 0.f;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      const float f = sc * diff[3 * p + k];
-      atomicAdd(&grad[3 * i0 + k], f);
-      atomicAdd(&grad[3 * i1 + k], -f);
-    }
-  }
+  add_pair_energy(atomic, energies, i0, i1, n_per_conf, e);
+  if (grad) add_pair_grad(grad, diff, p, i0, i1, R >= 1e-7f ? de / R : 0.f);
 }
 
 static int check_pair_params(const ani_pair_params* p) {
-  if (!p) return ANI_ERR_BAD_ARG;
-  if (p->kind < 0 || p->kind > 1 || p->cutoff_fn < 0 || p->cutoff_fn > 2) return ANI_ERR_BAD_ARG;
-  if (p->num_species < 1 || p->num_species > ANI_MAX_SPECIES) return ANI_ERR_BAD_ARG;
-  if (!(p->to_bohr > 0.f)) return ANI_ERR_BAD_ARG;
-  if (p->cutoff_fn != 2 && !(p->cutoff > 0.f && p->cutoff < 1e30f)) return ANI_ERR_BAD_ARG;
-  return ANI_OK;
+  const int rc = check_term_params(p);
+  if (rc != ANI_OK) return rc;
+  return p->kind == 0 || p->kind == 1 ? ANI_OK : ANI_ERR_BAD_ARG;
 }
 
 static int launch_pair_potential(const ani_pair_params* params, const ani_grid* grid, const float* spos,
@@ -219,26 +141,20 @@ static int launch_pair_potential(const ani_pair_params* params, const ani_grid* 
                                  double* energies, float* grad_coords, double* virial, float* member_atomic,
                                  float* grad_members, const int32_t* members, int n_members, const float* lattice,
                                  bool want_lattice, void* stream) {
-  const int rc = check_pair_params(params);
+  int rc = check_pair_params(params);
   if (rc != ANI_OK) return rc;
-  if (!grid || !spos || !sorted_orig || !nbr_cnt || !nbr_list) return ANI_ERR_BAD_ARG;
-  if (want_lattice && !lattice) return ANI_ERR_BAD_ARG;
-  if (n_conf < 1 || n_per_conf < 1 || n != n_conf * n_per_conf || nbr_cap < 1) return ANI_ERR_BAD_ARG;
-  if (lo < 0 || hi > n || lo > hi) return ANI_ERR_BAD_ARG;
-  if (n_members < 0 || n_members > ANI_MAX_MEMBERS || (n_members > 0 && !members)) return ANI_ERR_BAD_ARG;
-  if ((member_atomic || grad_members) && n_members == 0) return ANI_ERR_BAD_ARG;
-  PairMembers ms;
-  ms.count = n_members;
-  for (int k = 0; k < ANI_MAX_MEMBERS; ++k) {
-    ms.idx[k] = k < n_members ? members[k] : 0;
-    if (ms.idx[k] < 0 || ms.idx[k] >= ANI_MAX_MEMBERS) return ANI_ERR_BAD_ARG;
-  }
+  ActiveMembers ms;
+  rc = check_step_term_args(grid, spos, sorted_orig, n, lo, hi, n_conf, n_per_conf, lattice, want_lattice,
+                            member_atomic, grad_members, members, n_members, ms);
+  if (rc != ANI_OK) return rc;
+  if (!nbr_cnt || !nbr_list || nbr_cap < 1) return ANI_ERR_BAD_ARG;
   if (hi == lo) return ANI_OK;
   const int blocks = (hi - lo + PAIR_WARPS - 1) / PAIR_WARPS;
+  const TermOut out{atomic, energies, grad_coords, virial, member_atomic, grad_members};
   auto launch = [&](auto kernel) {
     kernel<<<blocks, PAIR_WARPS * 32, 0, (cudaStream_t)stream>>>(
         *params, grid, reinterpret_cast<const float4*>(spos), sorted_orig, n, lo, hi, n_per_conf, nbr_cnt, nbr_list,
-        nbr_cap, lattice, atomic, energies, grad_coords, virial, member_atomic, grad_members, ms);
+        nbr_cap, lattice, out, ms);
   };
   if (want_lattice) {
     virial ? launch(k_pair_potential<true, true>) : launch(k_pair_potential<true, false>);

@@ -3,7 +3,7 @@
 // gradient, per atom the mean, relative stdev and relative range of the members' force magnitudes, and per conformer
 // the members' energies in float64 and the energy QBC factor.  Two small launches, no atomics: every output is written
 // by exactly one thread, so the results are deterministic.
-#include "common.cuh"
+#include "terms.cuh"
 
 namespace ani {
 
@@ -17,8 +17,8 @@ struct QbcArgs {
   float* atom_stats;           // [3][n]
   double* member_energies;     // [count][n_conf]
   double* qbc;                 // [n_conf]
-  int n, n_conf, n_per_conf, count;
-  int idx[ANI_MAX_MEMBERS];
+  int n, n_conf, n_per_conf;
+  ActiveMembers ms;            // output k of grad_members / member_energies is member ms.idx[k]
 };
 
 // one thread per atom: the mean gradient and the statistics of the members' force magnitudes (arch.py:543-576)
@@ -31,7 +31,7 @@ __global__ void __launch_bounds__(256) k_qbc_atoms(const __grid_constant__ QbcAr
 #pragma unroll
   for (int k = 0; k < ANI_MAX_MEMBERS; ++k) {
     mag[k] = 0.f;
-    if (k < q.count) {
+    if (k < q.ms.count) {
       const float* g = q.grad_members + ((size_t)k * q.n + a) * 3;
       const float x = g[0], y = g[1], z = g[2];
       gx += x;
@@ -43,18 +43,18 @@ __global__ void __launch_bounds__(256) k_qbc_atoms(const __grid_constant__ QbcAr
       mn = fminf(mn, mag[k]);
     }
   }
-  const float inv = 1.0f / (float)q.count;
+  const float inv = 1.0f / (float)q.ms.count;
   q.grad[3 * (size_t)a + 0] = gx * inv;
   q.grad[3 * (size_t)a + 1] = gy * inv;
   q.grad[3 * (size_t)a + 2] = gz * inv;
   const float mean = sum * inv;
   float rstd = 0.f, rrange = 1.f;  // one member: stdev 0, range 1
-  if (q.count > 1) {
+  if (q.ms.count > 1) {
     float ss = 0.f;
 #pragma unroll
     for (int k = 0; k < ANI_MAX_MEMBERS; ++k)
-      if (k < q.count) ss += (mag[k] - mean) * (mag[k] - mean);
-    const float sd = sqrtf(ss / (float)(q.count - 1));  // unbiased
+      if (k < q.ms.count) ss += (mag[k] - mean) * (mag[k] - mean);
+    const float sd = sqrtf(ss / (float)(q.ms.count - 1));  // unbiased
     rstd = (sd + eps) / (mean + eps);
     rrange = ((mx - mn) + eps) / (mean + eps);
   }
@@ -77,7 +77,7 @@ __global__ void __launch_bounds__(256) k_qbc_conformers(const __grid_constant__ 
     const double self = q.sae ? q.sae[sp] : 0.0;
 #pragma unroll
     for (int k = 0; k < ANI_MAX_MEMBERS; ++k)
-      if (k < q.count) e[k] += (double)q.member_atomic[(size_t)q.idx[k] * q.n + a] + self;
+      if (k < q.ms.count) e[k] += (double)q.member_atomic[(size_t)q.ms.idx[k] * q.n + a] + self;
     e[ANI_MAX_MEMBERS] += 1.0;
   }
 #pragma unroll
@@ -94,16 +94,16 @@ __global__ void __launch_bounds__(256) k_qbc_conformers(const __grid_constant__ 
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) em[k] += red[k][w];
   }
   double mean = 0.0;
-  for (int k = 0; k < q.count; ++k) {
+  for (int k = 0; k < q.ms.count; ++k) {
     q.member_energies[(size_t)k * q.n_conf + c] = em[k];
     mean += em[k];
   }
-  mean /= q.count;
+  mean /= q.ms.count;
   double sd = 0.0;
-  if (q.count > 1) {
+  if (q.ms.count > 1) {
     double ss = 0.0;
-    for (int k = 0; k < q.count; ++k) ss += (em[k] - mean) * (em[k] - mean);
-    sd = sqrt(ss / (q.count - 1));
+    for (int k = 0; k < q.ms.count; ++k) ss += (em[k] - mean) * (em[k] - mean);
+    sd = sqrt(ss / (q.ms.count - 1));
   }
   q.qbc[c] = sd / sqrt(em[ANI_MAX_MEMBERS]);
 }
@@ -118,8 +118,10 @@ extern "C" int ani_b200_ensemble_qbc(const float* grad_members, const int32_t* m
                                      double* qbc, void* stream) {
   if (!grad_members || !members || !member_atomic || !species || !grad || !atom_stats || !member_energies || !qbc)
     return ANI_ERR_BAD_ARG;
-  if (n_members < 1 || n_members > ANI_MAX_MEMBERS || n_conf < 1 || n_per_conf < 1) return ANI_ERR_BAD_ARG;
+  if (n_members < 1 || n_conf < 1 || n_per_conf < 1) return ANI_ERR_BAD_ARG;
   QbcArgs q;
+  const int rc = active_members(members, n_members, q.ms);
+  if (rc != ANI_OK) return rc;
   q.grad_members = grad_members;
   q.member_atomic = member_atomic;
   q.species = species;
@@ -131,12 +133,6 @@ extern "C" int ani_b200_ensemble_qbc(const float* grad_members, const int32_t* m
   q.n = n_conf * n_per_conf;
   q.n_conf = n_conf;
   q.n_per_conf = n_per_conf;
-  q.count = n_members;
-  for (int k = 0; k < ANI_MAX_MEMBERS; ++k) q.idx[k] = 0;
-  for (int k = 0; k < n_members; ++k) {
-    if (members[k] < 0 || members[k] >= ANI_MAX_MEMBERS) return ANI_ERR_BAD_ARG;
-    q.idx[k] = members[k];
-  }
   cudaStream_t st = (cudaStream_t)stream;
   k_qbc_atoms<<<(q.n + 255) / 256, 256, 0, st>>>(q);
   k_qbc_conformers<<<n_conf, 256, 0, st>>>(q);

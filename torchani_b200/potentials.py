@@ -46,13 +46,14 @@ def _cutoff_fn_name(cutoff_fn: tp.Any) -> str:
     return name
 
 
-class _PairEnergy(torch.autograd.Function):
-    """coords -> (energies (C,) float64, atomic energies (C, A)) over a half pair list; dE/dcoords is produced by the
-    forward launch (gradients reach ``coords`` only, as in ``AEVComputer.compute_from_neighbors``)."""
+class _HalfListEnergy(torch.autograd.Function):
+    """coords -> (energies (C,) float64, atomic energies (C, A)) of a term over a half pair list.  ``launch(species,
+    idx, dist, diff, ghost, atomic, energies, grad, stream)`` runs the term's half-list entry point; dE/dcoords is
+    produced by that forward launch (gradients reach ``coords`` only, as in ``AEVComputer.compute_from_neighbors``)."""
 
     @staticmethod
     def forward(ctx, coords: Tensor, elem_idxs: Tensor, neighbors: Neighbors, ghost_flags: tp.Optional[Tensor],
-                params: PairParams):
+                launch: tp.Callable[..., None]):
         n_conf, n_per_conf = elem_idxs.shape
         dev = coords.device
         species = elem_idxs.reshape(-1).to(torch.int32).contiguous()
@@ -65,10 +66,7 @@ class _PairEnergy(torch.autograd.Function):
         energies = torch.zeros(n_conf, dtype=torch.float64, device=dev)
         grad = torch.zeros(n_conf, n_per_conf, 3, dtype=torch.float32, device=dev) if want_grad else None
         with torch.cuda.device(dev):
-            check(_lib.lib().ani_b200_pair_potential_pairs(
-                _lib.C.byref(params), ptr(species), idx[0].data_ptr(), idx[1].data_ptr(), ptr(dist), ptr(diff),
-                ptr(ghost), idx.shape[1], n_conf, n_per_conf, ptr(atomic), ptr(energies), ptr(grad),
-                torch.cuda.current_stream(dev).cuda_stream), "pair_potential_pairs")
+            launch(species, idx, dist, diff, ghost, atomic, energies, grad, torch.cuda.current_stream(dev).cuda_stream)
         ctx.want_grad = want_grad
         if want_grad:
             ctx.save_for_backward(grad)
@@ -131,18 +129,29 @@ class PairPotential(torch.nn.Module):
             for b in range(v.shape[1]):
                 dst[a][b] = float(v[a, b])
 
+    def _half_list_launch(self, device: torch.device) -> tp.Callable[..., None]:
+        """The launch of this term over a half pair list, for ``_HalfListEnergy``."""
+        p = self.params()
+
+        def launch(species, idx, dist, diff, ghost, atomic, energies, grad, stream):
+            check(_lib.lib().ani_b200_pair_potential_pairs(
+                _lib.C.byref(p), ptr(species), idx[0].data_ptr(), idx[1].data_ptr(), ptr(dist), ptr(diff), ptr(ghost),
+                idx.shape[1], *atomic.shape, ptr(atomic), ptr(energies), ptr(grad), stream), "pair_potential_pairs")
+        return launch
+
     def compute_from_neighbors(self, elem_idxs: Tensor, coords: Tensor, neighbors: Neighbors, charge: int = 0,
                                atomic: bool = False, ensemble_values: bool = False,
                                ghost_flags: tp.Optional[Tensor] = None) -> Tensor:
         """Energies ``(C,)`` or ``(C, A)`` of the given half pair list (potentials/core.py:181-207; pairs beyond the
         cutoff are ignored, pairs that touch a ghost atom count half; ``ensemble_values`` is disregarded as in the
-        reference)."""
+        reference).  D3 (dftd3.py:221-246) counts every listed pair in the coordination numbers."""
         assert elem_idxs.dim() == 2 and coords.shape == (elem_idxs.shape[0], elem_idxs.shape[1], 3)
         if coords.device.type != "cuda":
             raise ValueError("torchani_b200 runs on CUDA tensors only (there is no CPU path)")
         if ghost_flags is not None and ghost_flags.numel() != elem_idxs.numel():
             raise ValueError("ghost_flags and species should have the same number of elements")
-        energies, atomic_e = _PairEnergy.apply(coords, elem_idxs, neighbors, ghost_flags, self.params())
+        energies, atomic_e = _HalfListEnergy.apply(coords, elem_idxs, neighbors, ghost_flags,
+                                                   self._half_list_launch(coords.device))
         return atomic_e.to(coords.dtype) if atomic else energies.to(coords.dtype)
 
     def forward(self, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor] = None,
@@ -235,42 +244,6 @@ class RepulsionZBL(PairPotential):
         for q in range(4):
             p.screen_coeff[q] = float(self._coeffs.view(-1)[q])
             p.screen_exp[q] = float(self._exponents.view(-1)[q])
-
-
-class _D3Energy(torch.autograd.Function):
-    """coords -> (energies (C,) float64, atomic energies (C, A)) of D3 over a half pair list; dE/dcoords (direct part
-    and coordination-number chain) is produced by the forward launches, as in ``_PairEnergy``."""
-
-    @staticmethod
-    def forward(ctx, coords: Tensor, elem_idxs: Tensor, neighbors: Neighbors, ghost_flags: tp.Optional[Tensor],
-                params: D3Params, tables: Tensor):
-        n_conf, n_per_conf = elem_idxs.shape
-        dev = coords.device
-        species = elem_idxs.reshape(-1).to(torch.int32).contiguous()
-        idx = neighbors.indices.to(torch.int64).contiguous()
-        dist = neighbors.distances.detach().to(torch.float32).contiguous()
-        diff = neighbors.diff_vectors.detach().to(torch.float32).contiguous()
-        ghost = None if ghost_flags is None else ghost_flags.reshape(-1).to(torch.uint8).contiguous()
-        want_grad = bool(coords.requires_grad)
-        n = n_conf * n_per_conf
-        cn = torch.empty(n, dtype=torch.float32, device=dev)
-        dedcn = torch.empty(n, dtype=torch.float32, device=dev) if want_grad else None
-        atomic = torch.zeros(n_conf, n_per_conf, dtype=torch.float32, device=dev)
-        energies = torch.zeros(n_conf, dtype=torch.float64, device=dev)
-        grad = torch.zeros(n_conf, n_per_conf, 3, dtype=torch.float32, device=dev) if want_grad else None
-        with torch.cuda.device(dev):
-            check(_lib.lib().ani_b200_dispersion_d3_pairs(
-                _lib.C.byref(params), ptr(tables), ptr(species), idx[0].data_ptr(), idx[1].data_ptr(), ptr(dist),
-                ptr(diff), ptr(ghost), idx.shape[1], n_conf, n_per_conf, ptr(cn), ptr(dedcn), ptr(atomic),
-                ptr(energies), ptr(grad), torch.cuda.current_stream(dev).cuda_stream), "dispersion_d3_pairs")
-        ctx.want_grad = want_grad
-        if want_grad:
-            ctx.save_for_backward(grad)
-        return energies, atomic
-
-    @staticmethod
-    def backward(ctx, g_energy, g_atomic):
-        return _PairEnergy.backward(ctx, g_energy, g_atomic) + (None,)
 
 
 class _BeckeJohnsonDamp(torch.nn.Module):
@@ -386,20 +359,17 @@ class TwoBodyDispersionD3(PairPotential):
         self._device_tables[key] = (self._versions(), t)
         return t
 
-    def compute_from_neighbors(self, elem_idxs: Tensor, coords: Tensor, neighbors: Neighbors, charge: int = 0,
-                               atomic: bool = False, ensemble_values: bool = False,
-                               ghost_flags: tp.Optional[Tensor] = None) -> Tensor:
-        """Energies ``(C,)`` or ``(C, A)`` of the given half pair list (potentials/core.py:181-207 over
-        dftd3.py:221-246): pairs beyond the cutoff are ignored, coordination numbers count every listed pair, pair
-        energies that touch a ghost atom count half."""
-        assert elem_idxs.dim() == 2 and coords.shape == (elem_idxs.shape[0], elem_idxs.shape[1], 3)
-        if coords.device.type != "cuda":
-            raise ValueError("torchani_b200 runs on CUDA tensors only (there is no CPU path)")
-        if ghost_flags is not None and ghost_flags.numel() != elem_idxs.numel():
-            raise ValueError("ghost_flags and species should have the same number of elements")
-        energies, atomic_e = _D3Energy.apply(coords, elem_idxs, neighbors, ghost_flags, self.params(),
-                                             self.tables(coords.device))
-        return atomic_e.to(coords.dtype) if atomic else energies.to(coords.dtype)
+    def _half_list_launch(self, device: torch.device) -> tp.Callable[..., None]:
+        p, tables = self.params(), self.tables(device)
+
+        def launch(species, idx, dist, diff, ghost, atomic, energies, grad, stream):
+            cn = torch.empty(atomic.numel(), dtype=torch.float32, device=device)
+            dedcn = torch.empty_like(cn) if grad is not None else None
+            check(_lib.lib().ani_b200_dispersion_d3_pairs(
+                _lib.C.byref(p), ptr(tables), ptr(species), idx[0].data_ptr(), idx[1].data_ptr(), ptr(dist),
+                ptr(diff), ptr(ghost), idx.shape[1], *atomic.shape, ptr(cn), ptr(dedcn), ptr(atomic), ptr(energies),
+                ptr(grad), stream), "dispersion_d3_pairs")
+        return launch
 
 
 def from_torchani(ref_pot) -> PairPotential:
