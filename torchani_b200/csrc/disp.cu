@@ -436,14 +436,16 @@ extern "C" int ani_b200_dispersion_d3_pairs(const ani_d3_params* params, const f
   const int rc = ani::check_d3_params(params, tables);
   if (rc != ANI_OK) return rc;
   if (num_pairs < 0 || n_conf < 1 || n_per_conf < 1) return ANI_ERR_BAD_ARG;
-  if (!cn || (grad_coords && (!dedcn || !diff_vectors))) return ANI_ERR_BAD_ARG;
+  if (!cn || (grad_coords && !dedcn)) return ANI_ERR_BAD_ARG;
   const size_t n = (size_t)n_conf * n_per_conf;
   cudaStream_t st = (cudaStream_t)stream;
   cudaMemsetAsync(cn, 0, n * sizeof(float), st);
   if (grad_coords) cudaMemsetAsync(dedcn, 0, n * sizeof(float), st);
   ANI_CUDA_CHECK_LAUNCH();
+  // an empty list has no pair arrays to point to (as in ani_b200_pair_potential_pairs)
   if (num_pairs == 0) return ANI_OK;
   if (!species || !idx0 || !idx1 || !distances) return ANI_ERR_BAD_ARG;
+  if (grad_coords && !diff_vectors) return ANI_ERR_BAD_ARG;
   const long long blocks = (num_pairs + 255) / 256;
   if (blocks > 0x7fffffffLL) return ANI_ERR_BAD_ARG;
   const float4* tab = reinterpret_cast<const float4*>(tables);
