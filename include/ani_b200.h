@@ -32,6 +32,8 @@
  *                               caller-supplied half list, with ghost weights
  *   ani_b200_dispersion_d3      potentials/dftd3.py:102-311 (TwoBodyDispersionD3, D3(BJ) two-body dispersion with its
  *                               own neighbour search); _pairs: over a caller-supplied half list, with ghost weights
+ *   ani_b200_charges            electro.py:29-156 (ChargeNormalizer.forward, DipoleComputer.forward) on the raw outputs of
+ *                               a charge network pass (potentials/nnp.py:75-102, SeparateChargesNNPotential)
  *   ani_b200_operand_format     (no counterpart: format of the tensor-core GEMM operands of this build)
  */
 #ifndef ANI_B200_H
@@ -652,6 +654,25 @@ int ani_b200_reduce_energies(const ani_mlp_model* model, const float* e_member, 
                              const int32_t* species, int n, int lo, int hi, int n_conf,
                              int n_per_conf, const double* sae, float* atomic_out,
                              float* member_atomic_out, double* energies_out, void* stream);
+
+/* 7b. Atomic charges and dipoles of a charge model (ANIq / ANImbis), one launch, one CTA per conformer.              */
+/*    q_raw        raw charges: with row_of / orig_to_sorted (outputs of the step preparation) the e_member row 0    */
+/*                 f32[rows_cap] of a one-member charge network pass, read at row_of[orig_to_sorted[a]]; with both   */
+/*                 NULL, f32[n] in flat input order                                                                 */
+/*    species      i32[n] element indices, -1 = padding;  coords f32[n][3] in flat INPUT order (not wrapped)         */
+/*    weights      HOST f32[num_species] normaliser weights (may be NULL if !normalize); scale_by_q2: w_i = W[e_i]   */
+/*                 * q_raw_i^2 (ChargeNormalizer's scale_weights_by_charges_squared); normalize == 0: q = q_raw      */
+/*                 (BaseChargeNormalizer)                                                                           */
+/*    total_charge Q: normalised charges are q_i = q_raw_i + (Q - sum q_raw) w_i / sum w                          */
+/*    masses       HOST f32[num_species], needed only for frame 0                                                    */
+/*    frame        dipole reference point: 0 centre of mass, 1 centre of geometry (real atoms), 2 origin           */
+/*    charges_out  f32[n], input order, 0 for padding                                                                */
+/*    dipoles_out  f64[n_conf][3] = sum_i q_i (r_i - r_ref) over the real atoms, in e * Angstrom, or NULL            */
+/*    Float64 sums in a fixed order (no atomics): repeated runs give identical bits.                                */
+int ani_b200_charges(const float* q_raw, const int32_t* row_of, const int32_t* orig_to_sorted, const int32_t* species,
+                     const float* coords, int n_conf, int n_per_conf, const float* weights, int num_species,
+                     int scale_by_q2, int normalize, double total_charge, const float* masses, int frame,
+                     float* charges_out, double* dipoles_out, void* stream);
 
 /* 8. Multi-GPU: one-shot all-reduce of the per-rank partial forces / energies over NVLink peer memory.   */
 /*    The path shards by central atom (one process per GPU); every rank accumulates dE_owned/dx_j into a      */

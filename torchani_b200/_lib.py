@@ -23,6 +23,7 @@ ANI_MAX_ANG = 96
 ANI_VIRIAL_SLOTS = 64
 ACT_CELU = 0                # ani_mlp_model::activation
 ACT_GELU = 1
+DIPOLE_FRAMES = ("center_of_mass", "center_of_geometry", "origin")   # the frame argument of ani_b200_charges
 ANI_LATTICE_STRIDE = 18   # floats per conformer of the lattice table of grid mode 3: cell, inverse
 
 STATUS_NBR_OVERFLOW = 1
@@ -154,6 +155,7 @@ _PROTOTYPES = {
     "ani_b200_comm_destroy": (C.c_int, [_P]),
     "ani_b200_active_aev_blocks": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "ani_b200_reduce_energies": (C.c_int, [_P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
+    "ani_b200_charges": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _P, _I, _I, _I, C.c_double, _P, _I, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

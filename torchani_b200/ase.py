@@ -34,6 +34,7 @@ except ImportError:
     ) from None
 
 from .calculator import HostCalculator
+from .nn import ATOMIC_NUMBER
 
 StressKind = str   # "scaling" | "fdotr" | "numerical"  (annotations.py of the reference)
 
@@ -65,6 +66,10 @@ class Calculator(AseCalculator):
         if self.qbc:
             self.implemented_properties = list(Calculator.implemented_properties) + [
                 "energy_qbc", "force_magnitudes", "force_relative_stdev", "force_relative_range"]
+        # a charge model (models.ANIq): atomic charges (e) and the dipole about the centre of mass (e * A, ASE's unit)
+        self._charges = hasattr(model, "charge_networks")
+        if self._charges:
+            self.implemented_properties = list(self.implemented_properties) + ["charges", "dipole"]
         self._host: tp.Optional[HostCalculator] = None
         self._host_key: tp.Any = None
 
@@ -113,13 +118,38 @@ class Calculator(AseCalculator):
         elif self.qbc:
             e, f, q = host.calculate_with_qbc(positions)
             self._store_qbc(q, ha)
+        elif self._charges:
+            self._set_masses(host)
+            e, f, charges, dipole = host.calculate_with_charges(positions)
+            self._store_charges(charges, dipole)
         else:
             e, f = host.calculate(positions)
+        if self._charges and (needs_stress or self.qbc) and ("charges" in properties or "dipole" in properties):
+            self._set_masses(host)
+            _, _, charges, dipole = host.calculate_with_charges(positions)
+            self._store_charges(charges, dipole)
         self.results["energy"] = e * ha
         self.results["free_energy"] = e * ha
         self.results["forces"] = f.astype(np.float64) * ha
         if needs_stress and self.stress_kind == "numerical":
             self.results["stress"] = self.calculate_numerical_stress(self.atoms)
+
+    def _set_masses(self, host: HostCalculator) -> None:
+        """The dipole is taken about the centre of mass of the Atoms: one mass per element of the model."""
+        numbers = np.asarray(self.atoms.get_atomic_numbers())
+        masses = np.asarray(self.atoms.get_masses(), dtype=np.float64)
+        per_symbol = []
+        for s in self.model.symbols:
+            m = masses[numbers == ATOMIC_NUMBER[s]]
+            if m.size and not np.all(m == m[0]):
+                raise ValueError(f"the atoms of element {s} carry different masses: the dipole kernel takes one mass "
+                                 "per element")
+            per_symbol.append(float(m[0]) if m.size else 1.0)
+        host.set_dipole_reference("center_of_mass", per_symbol)
+
+    def _store_charges(self, charges: np.ndarray, dipole: np.ndarray) -> None:
+        self.results["charges"] = charges.astype(np.float64)
+        self.results["dipole"] = dipole.astype(np.float64)
 
     def _store_qbc(self, q, ha: float) -> None:
         self.results["energy_qbc"] = q.energy_qbc * ha

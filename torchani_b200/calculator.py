@@ -109,7 +109,11 @@ class HostCalculator:
         q0, s0 = self.ws._out_qbc_off, self.ws._out_stats_off
         M = self.engine.nets.num_members
         self.h_energy_qbc = self.h_out_full[q0 + 8 * M * C_:q0 + 8 * (M + 1) * C_].view(torch.float64)
-        self.h_atom_stats = self.h_out_full[s0:].view(torch.float32).view((3,) + shape[:-1])
+        self.h_atom_stats = self.h_out_full[s0:s0 + 12 * C_ * self.n].view(torch.float32).view((3,) + shape[:-1])
+        c0 = self.ws._out_chg_off
+        self.h_dipoles = self.h_out_full[c0:c0 + 24 * C_].view(torch.float64).view(C_, 3)
+        self.h_charges = self.h_out_full[c0 + 24 * C_:].view(torch.float32).view(shape[:-1])
+        self._dipole: tp.Tuple[int, tp.Optional[tp.Tuple[float, ...]]] = (2, None)   # origin (set_dipole_reference)
         self.h_moved = torch.zeros(1, dtype=torch.int32).pin_memory()
         self._have_grid = False       # a grid built with the skin exists and may be reused
         self.rebuilds = 0             # steps that built the grid
@@ -240,6 +244,46 @@ class HostCalculator:
             return self.h_energy.numpy().copy(), np.negative(self.h_grad.numpy()), qbc
         return float(self.h_energy[0]), np.negative(self.h_grad.numpy()), qbc
 
+    def set_dipole_reference(self, reference: str = "origin", masses: tp.Optional[tp.Sequence[float]] = None) -> None:
+        """Reference point of the dipoles of ``calculate_with_charges``: "origin" (default), "center_of_geometry" or
+        "center_of_mass", which needs one mass per symbol of the model."""
+        from .electro import frame_index
+        frame = frame_index(reference)
+        if frame == 0 and (masses is None or len(masses) != len(self.model.symbols)):
+            raise ValueError("the center_of_mass reference needs one mass per symbol of the model")
+        self._dipole = (frame, tuple(float(m) for m in masses) if frame == 0 else None)
+
+    def calculate_with_charges(self, positions, cell=None) -> tp.Tuple[tp.Any, np.ndarray, np.ndarray, np.ndarray]:
+        """``calculate`` plus the atomic charges of a charge model (``models.ANIq``): (energy [Hartree], forces
+        [Hartree/A], charges (A,) [e], dipole (3,) [e * A], about the point of ``set_dipole_reference``).  One step
+        computes everything; like ``calculate`` it is one H2D and one D2H copy per call and, after a few calls, its own
+        captured CUDA graph.  Works with ``skin > 0`` and with batches (then (C,), (C, A, 3), (C, A), (C, 3)); not
+        with multi-GPU sharding: the normaliser needs every atom's raw charge."""
+        if getattr(self.engine, "charges", None) is None:
+            raise ValueError("calculate_with_charges needs a charge model (models.ANIq)")
+        if self.sharded is not None or tuple(self.shard) != (0, 1):
+            raise ValueError("calculate_with_charges runs on one GPU: no sharding")
+        if cell is not None:
+            self.set_cell(cell)
+        self._set_positions(positions)
+        eng = self.engine
+        self._calls += 1
+        if self._graphs and self._graph_version != eng.nets.active_key:
+            self._graphs = {}
+        reuse = self.skin > 0 and self._have_grid
+        self._run(reuse, charges=True)
+        if reuse and (int(self.h_moved[0]) & 1):
+            self.redone += 1   # an atom left its skin/2 sphere: rebuild, redo
+            self._run(False, charges=True)
+        elif reuse and int(self.h_moved[0]):
+            self._have_grid = False
+        if int(self.h_status[0]) and self._check_or_switch():
+            return self.calculate_with_charges(positions)
+        q, dip = self.h_charges.numpy().copy(), self.h_dipoles.numpy().copy()
+        if self.batch:
+            return self.h_energy.numpy().copy(), np.negative(self.h_grad.numpy()), q, dip
+        return float(self.h_energy[0]), np.negative(self.h_grad.numpy()), q, dip[0]
+
     def _check_or_switch(self) -> bool:
         """Raise what the reference raises for the status word of the last step.  If the 2 x fp16 operand format ran
         out of range, rebuild on the 3 x bfloat16 build of the library instead and return True: the caller redoes the
@@ -262,12 +306,15 @@ class HostCalculator:
             return True
         return False
 
-    def _run(self, reuse: bool, members: bool = False) -> None:
+    def _run(self, reuse: bool, members: bool = False, charges: bool = False) -> None:
         """One step (H2D, kernels, D2H, synchronise); after a few eager uses of a mode its whole sequence
-        is captured into one CUDA graph.  ``members``: the query-by-committee step (Engine.run(..., members=True))."""
+        is captured into one CUDA graph.  ``members``: the query-by-committee step (Engine.run(..., members=True)).
+        ``charges``: the step with the charge pass (Engine.run(..., charges=True))."""
         with torch.cuda.device(self.device):   # the C-ABI launches on the current device's stream
             if members:
                 self._run_members(reuse)
+            elif charges:
+                self._run_charges(reuse)
             else:
                 self._run_on_device(reuse)
 
@@ -292,6 +339,35 @@ class HostCalculator:
         else:
             self._copies_in(reuse)
             eng.run(ws, self.pbc, want_grad=True, reuse=reuse, conformer_cells=self.conformer_cells, members=True)
+            self._copies_out(reuse, members=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        if not reuse:
+            self._have_grid = self.skin > 0
+
+    def _run_charges(self, reuse: bool) -> None:
+        ws, eng = self.ws, self.engine
+        qn, qp = eng.charges
+        qp = qp._replace(frame=self._dipole[0], masses=self._dipole[1])
+        eng.set_charges((qn, qp))   # (the model's own calls may have left other dipole parameters on the engine)
+        key = ("charges", reuse, qn, qp)
+        self._mode_calls[key] = self._mode_calls.get(key, 0) + 1
+        if not reuse:
+            self.rebuilds += 1
+        eng.charge_buffers(ws)
+        graph = self._graphs.get(key)
+        if graph is None and eng.cuda_graph and not eng.profile and self._mode_calls[key] > self.graph_after:
+            eng.note_composition(ws)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                self._copies_in(reuse)
+                eng._launch(ws, self.pbc, True, 0, ws.n, reuse, conformer_cells=self.conformer_cells, charges=True)
+                self._copies_out(reuse, members=True)
+            self._graphs[key], self._graph_version = graph, eng.nets.active_key
+        if graph is not None:
+            graph.replay()
+        else:
+            self._copies_in(reuse)
+            eng.run(ws, self.pbc, want_grad=True, reuse=reuse, conformer_cells=self.conformer_cells, charges=True)
             self._copies_out(reuse, members=True)
         torch.cuda.current_stream(self.device).synchronize()
         if not reuse:
@@ -340,6 +416,7 @@ class HostCalculator:
         self.ws.in_block.copy_(self.h_in, non_blocking=True)
 
     def _copies_out(self, reuse: bool = False, members: bool = False) -> None:
+        # (members: the whole of out_full, with the query-by-committee and the charge outputs behind out_block)
         if members:
             self.h_out_full.copy_(self.ws.out_full, non_blocking=True)
         else:

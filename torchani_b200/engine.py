@@ -406,19 +406,28 @@ class Workspace:
         # followed, in the same allocation (out_full), by what the query-by-committee step adds (Engine.run(...,
         # members=True)), so that it too needs one D2H copy while the ordinary step still copies out_block only:
         #   [member energies f64 x M x n_conf | qbc f64 x n_conf | pad to 16 B | atom stats f32 x 3 n]
+        # and then by what a step with charges adds (Engine.run(..., charges=True), calculator.calculate_with_charges):
+        #   [pad to 16 B | dipoles f64 x 3 n_conf | charges f32 x n]
         self.in_coords_off = (9 * n_conf + 15) // 16 * 16
         self.in_block = torch.zeros(self.in_coords_off + 3 * n, **f32)
         self._out_grad_off = (8 * n_conf + 4 + 15) // 16 * 16
         out_len = self._out_grad_off + 12 * n
         self._out_qbc_off = (out_len + 15) // 16 * 16
         self._out_stats_off = (self._out_qbc_off + 8 * (num_members + 1) * n_conf + 15) // 16 * 16
-        self.out_full = torch.zeros(self._out_stats_off + 12 * n, dtype=torch.uint8, device=device)
+        self._out_chg_off = (self._out_stats_off + 12 * n + 15) // 16 * 16
+        self.out_full = torch.zeros(self._out_chg_off + 24 * n_conf + 4 * n, dtype=torch.uint8, device=device)
         self.out_block = self.out_full[:out_len]
         self.member_energies = self.out_full[self._out_qbc_off:self._out_qbc_off + 8 * num_members * n_conf].view(
             torch.float64).view(num_members, n_conf)
         self.qbc = self.out_full[self._out_qbc_off + 8 * num_members * n_conf:
                                  self._out_qbc_off + 8 * (num_members + 1) * n_conf].view(torch.float64)
-        self.atom_stats = self.out_full[self._out_stats_off:].view(torch.float32).view(3, n)
+        self.atom_stats = self.out_full[self._out_stats_off:self._out_stats_off + 12 * n].view(torch.float32).view(3, n)
+        self.dipoles = self.out_full[self._out_chg_off:self._out_chg_off + 24 * n_conf].view(torch.float64).view(n_conf, 3)
+        self.charges = self.out_full[self._out_chg_off + 24 * n_conf:].view(torch.float32)
+        # the charge networks' own activations and raw outputs (one member), allocated on the first step with charges
+        # (Engine.charge_buffers): the energy networks' act1..act3 / e_member are live until the energy reduction
+        self.q_act: tp.Optional[tp.Tuple[Tensor, Tensor, Tensor]] = None
+        self.q_raw: tp.Optional[Tensor] = None
         # per-member dE/dAEV slabs f32[M][rows_cap][ldx] and dE_m/dcoords f32[M][n][3] of the query-by-committee step:
         # allocated on its first use (Engine.members_buffers; at 10 k atoms the slabs of 8 members take ~340 MB)
         self.dx_members: tp.Optional[Tensor] = None
@@ -547,18 +556,41 @@ class MembersResult(tp.NamedTuple):
     force_relative_range: Tensor   # (C, A) float32: (max_m |F_m| - min_m |F_m| + 1e-8) / (mean + 1e-8)
 
 
+class ChargeParams(tp.NamedTuple):
+    """The normaliser and dipole parameters of a charge model (the host arguments of ``ani_b200_charges``)."""
+    weights: tp.Tuple[float, ...]        # per element (ChargeNormalizer.weights); unused without ``normalize``
+    scale_by_q2: bool = False            # ChargeNormalizer.scale_weights_by_charges_squared
+    normalize: bool = True               # False: BaseChargeNormalizer (raw charges)
+    masses: tp.Optional[tp.Tuple[float, ...]] = None   # per element; needed for the centre-of-mass frame only
+    frame: int = 2                       # dipole reference point: 0 centre of mass, 1 centre of geometry, 2 origin
+
+    def arrays(self) -> tp.Tuple[tp.Any, tp.Any]:
+        w = (C.c_float * len(self.weights))(*self.weights)
+        m = None if self.masses is None else (C.c_float * len(self.masses))(*self.masses)
+        return w, m
+
+
+class ChargesResult(tp.NamedTuple):
+    """What a step with charges (``Engine.run(..., charges=True)``) adds."""
+    charges: Tensor    # (C, A) float32: normalised atomic charges (e), 0 for padding
+    dipoles: Tensor    # (C, 3) float64: sum_i q_i (r_i - r_ref) (e * Angstrom)
+
+
 class Engine:
     """Fused ANI energy(+force) step on one GPU.  ``lo_frac/hi_frac`` select the slice of
     bucket-sorted atoms this engine owns (multi-GPU sharding, see parallel.py)."""
 
     def __init__(self, consts: AEVConstants, nets: PackedNetworks, sae: tp.Optional[tp.Sequence[float]] = None,
                  nbr_cap: int = 128, cuda_graph: bool = True, pairs: tp.Sequence[PairParams] = (),
-                 dispersion: tp.Optional[tp.Tuple[D3Params, Tensor]] = None):
+                 dispersion: tp.Optional[tp.Tuple[D3Params, Tensor]] = None,
+                 charges: tp.Optional[tp.Tuple[PackedNetworks, ChargeParams]] = None):
         """``pairs``: the ``ani_pair_params`` of the model's pair potentials (potentials.PairPotential.params()); each
         adds one launch to the step (``_pair_potentials``), a model without any issues exactly the launches it
         issued before.  ``dispersion``: the ``ani_d3_params`` and device tables of a D3 term
         (potentials.TwoBodyDispersionD3.params() / .tables(device)), or None; it adds three launches to a step with
-        forces and two to one without (``_dispersion``)."""
+        forces and two to one without (``_dispersion``).  ``charges``: the packed charge networks (one member) and the
+        normaliser / dipole parameters of a charge model; a step asked for charges (``run(..., charges=True)``) runs
+        them forward-only on the step's AEVs and adds the launches of ``_charge_pass``, any other step is unchanged."""
         if nets.in_dim != consts.out_dim:
             raise ValueError("network input width != AEV length")
         if nets.num_species != consts.num_species:
@@ -578,6 +610,8 @@ class Engine:
             if d3t.device != nets.device or d3t.dtype != torch.float32 or d3t.numel() != d3p.num_species ** 2 * 100:
                 raise ValueError("D3 tables must be float32 (S, S, 25, 4) on the engine's device")
         self.dispersion = dispersion
+        self.charges: tp.Optional[tp.Tuple[PackedNetworks, ChargeParams]] = None
+        self.set_charges(charges)
         self.device = nets.device
         self.params = consts.to_struct()
         # internal column order of the tiled AEV operand / dE/dAEV rows: must be the one the layer-1 weights were packed in
@@ -600,6 +634,10 @@ class Engine:
         self.variant = nets.variant
         self.lib = _lib.lib(self.variant)
         self.launches_per_step = 0
+        # The forward-only pass of the charge networks: "step" = ani_b200_mlp_step(..., want_backward=0) (one data-flow
+        # launch per window), "chained" = ani_b200_mlp_forward (three launches of the GEMM kernel).  On the H100 the
+        # data-flow form was 2-3 % faster at water 10 k and on the GDB batch of 256 (tools/charge_timing.py, DESIGN §4.8)
+        self.charge_mlp = os.environ.get("ANI_B200_CHARGE_MLP", "step")
         # per-stage CUDA-event timing (bench.py's roofline leg); off by default
         self.profile = False
         # zero-fill of dE/dAEV and the energy reduction on a forked side stream (see _launch); off by default --
@@ -679,7 +717,7 @@ class Engine:
     # -- one step --------------------------------------------------------------------------
     def step(self, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor] = None, pbc: bool = False,
              want_grad: bool = True, shard: tp.Tuple[int, int] = (0, 1), want_virial: bool = False,
-             check: bool = False) -> StepResult:
+             check: bool = False, want_charges: bool = False) -> StepResult:
         """species (C, A) int (element indices, -1 padding), coords (C, A, 3) on this device.
         ``shard = (rank, world)``: only atoms whose bucket-sorted position falls into this
         rank's slice are evaluated; gradients/energies are partial sums to be all-reduced.
@@ -690,14 +728,15 @@ class Engine:
         if species.device != dev or coords.device != dev:
             raise ValueError(f"inputs must live on {dev} (the engine has no CPU path)")
         ws, per_conf = self._stage_inputs(species, coords, cell, pbc)
-        res = self.run(ws, bool(pbc), want_grad, shard, want_virial=want_virial, conformer_cells=per_conf)
+        res = self.run(ws, bool(pbc), want_grad, shard, want_virial=want_virial, conformer_cells=per_conf,
+                       charges=want_charges)
         if check:   # one 4-byte D2H read: cell too small / neighbour overflow / operand range raise here
             self.check_status(ws)
         return res
 
     def run(self, ws: Workspace, pbc: bool, want_grad: bool = True, shard: tp.Tuple[int, int] = (0, 1),
             reuse: bool = False, want_virial: bool = False, conformer_cells: bool = False,
-            members: bool = False) -> StepResult:
+            members: bool = False, charges: bool = False) -> StepResult:
         """One step on inputs that are ALREADY in the workspace buffers (``ws.species_i32``,
         ``ws.coords``, ``ws.cell`` -- or, with ``conformer_cells``, one cell per conformer in ``ws.cells``) -- the
         entry point of host-driven loops that copy straight into them (calculator.HostCalculator).  The results alias
@@ -705,9 +744,21 @@ class Engine:
 
         ``members=True``: the query-by-committee step (``_launch_members``).  Besides the ordinary results (the
         gradient is the mean of the members' gradients) it leaves every active member's energy and gradient and the
-        force / energy disagreement statistics in the workspace (``members_result``).  One GPU only."""
+        force / energy disagreement statistics in the workspace (``members_result``).  One GPU only.
+
+        ``charges=True`` (an engine built with ``charges``): the step also leaves the normalised atomic charges and the
+        dipoles in the workspace (``charges_result``).  One GPU only, not in the query-by-committee step: the
+        normaliser needs every atom's raw charge."""
         n, n_conf, n_per_conf = ws.n, ws.n_conf, ws.n_per_conf
         members = bool(members)
+        charges = bool(charges)
+        if charges:
+            if self.charges is None:
+                raise ValueError("this engine has no charge networks")
+            if members or tuple(shard) != (0, 1) or ws.reducer is not None:
+                raise ValueError("charges are computed unsharded and outside the query-by-committee step: the "
+                                 "normaliser needs every atom's raw charge")
+            self.charge_buffers(ws)
         if members and (tuple(shard) != (0, 1) or not want_grad or want_virial):
             raise ValueError("the query-by-committee step runs unsharded, with forces and without the virial")
         rank, world = shard
@@ -726,13 +777,15 @@ class Engine:
             raise ValueError("reuse=True (Verlet skin) is not supported for periodic batches")
         key = (n_conf, n_per_conf, bool(pbc), bool(want_grad), lo, hi, self.nets.active_key, bool(reuse), self.skin,
                bool(want_virial), self.mlp_mode, conformer_cells, members)
+        if charges:   # (the charge networks' operands and the normaliser / dipole parameters are baked into the capture)
+            key = key + (self.charges[0], self.charges[1], self.charge_mlp)
         if reuse and not self.skin > 0:
             raise ValueError("reuse=True needs Engine.skin > 0 and a previous step that built the grid")
         if members:
             self.members_buffers(ws)
         with torch.cuda.device(self.device):   # the C-ABI launches on the CURRENT device's stream
             if not self.cuda_graph or self.profile:
-                self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells, members)
+                self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells, members, charges)
             else:
                 graph = self._graphs.get(key)
                 if graph is not None:
@@ -743,12 +796,12 @@ class Engine:
                     if len(self._graph_seen) > 4 * self.max_graphs:
                         self._graph_seen.clear()
                     self._graph_seen[key] = self._graph_seen.get(key, 0) + 1
-                    self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells, members)
+                    self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells, members, charges)
                 else:
                     self.note_composition(ws)
                     graph = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(graph):
-                        self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells, members)
+                        self._launch(ws, bool(pbc), want_grad, lo, hi, reuse, want_virial, conformer_cells, members, charges)
                     while len(self._graphs) >= self.max_graphs:   # evict the least recently used capture
                         self._graphs.pop(next(iter(self._graphs)))
                     self._graphs[key] = graph
@@ -772,6 +825,8 @@ class Engine:
                                   + len(self.pairs))
         if self.dispersion is not None:   # CN, energies + dE/dCN, and the chain where forces are wanted
             self.launches_per_step += 3 if (want_grad or members) else 2
+        if charges:
+            self.launches_per_step += self._charge_launches(ws)
         grad = ws.grad.view(n_conf, n_per_conf, 3) if want_grad else None
         virial = None
         if want_virial:
@@ -833,7 +888,8 @@ class Engine:
             ptr(ws.status), *lat, torch.cuda.current_stream(self.device).cuda_stream))
 
     def _launch(self, ws: Workspace, pbc: bool, want_grad: bool, lo: int, hi: int, reuse: bool = False,
-                want_virial: bool = False, conformer_cells: bool = False, members: bool = False) -> None:
+                want_virial: bool = False, conformer_cells: bool = False, members: bool = False,
+                charges: bool = False) -> None:
         """Enqueue the kernels of one step on the current stream (graph-capturable: no allocation,
         no synchronisation, only this library's launches and two memsets)."""
         if members:
@@ -926,6 +982,8 @@ class Engine:
         if self.dispersion is not None:
             self._dispersion(ws, lo, hi, lat, ws.grad_ptr if want_grad else None,
                              ptr(ws.virial) if want_virial else None, None, self._timed)
+        if charges:
+            self._charge_pass(ws, self._timed)
         if ws.reducer is not None:
             # multi-GPU: sum the partial forces / energies of all ranks over NVLink peer memory (one launch,
             # part of the captured graph); without forces only the energies matter but the buffer is small
@@ -970,6 +1028,76 @@ class Engine:
             C.byref(params), ptr(tables), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sorted_orig), ws.n, lo,
             hi, ws.n_conf, ws.n_per_conf, self.skin, ptr(ws.d3_cn), ptr(ws.d3_dedcn), ptr(ws.atomic), ws.energies_ptr,
             grad_ptr, virial_ptr, ptr(ws.member_atomic), grad_members_ptr, idx, len(active), ptr(ws.status), *lat, st))
+
+    def set_charges(self, charges: tp.Optional[tp.Tuple[PackedNetworks, ChargeParams]]) -> None:
+        """Attach (or replace) the charge networks and the normaliser / dipole parameters (see ``__init__``)."""
+        if charges is not None:
+            qn, qp = charges
+            nets = self.nets
+            if qn.num_members != 1:
+                raise ValueError("the charge networks must be one member")
+            if (qn.in_dim, qn.num_species, qn.ldx, qn.col_pad, qn.variant) != (
+                    nets.in_dim, nets.num_species, nets.ldx, nets.col_pad, nets.variant):
+                raise ValueError("the charge networks must read the energy networks' AEV operand: same AEV length, "
+                                 "elements, internal column order and operand format")
+            if len(qp.weights) != nets.num_species or (qp.masses is not None and len(qp.masses) != nets.num_species):
+                raise ValueError("one normaliser weight (and mass) per element is required")
+            if qp.frame not in (0, 1, 2) or (qp.frame == 0 and qp.masses is None):
+                raise ValueError("the centre-of-mass dipole frame needs one mass per element")
+        self.charges = charges
+
+    def charge_buffers(self, ws: Workspace) -> None:
+        """Allocate the charge networks' activations and raw outputs (once per workspace, before any capture)."""
+        if ws.q_raw is None:
+            qn = self.charges[0]
+            ws.q_act = tuple(operand_buffer(ws.rows_cap, w, self.device, self.variant) for w in qn.act_cols)
+            ws.q_raw = torch.zeros(1, ws.rows_cap, dtype=torch.float32, device=self.device)
+
+    def _charge_launches(self, ws: Workspace) -> int:
+        """Kernels a step with charges adds: the forward-only charge network pass and ani_b200_charges."""
+        if self.charge_mlp == "step":
+            return self.lib.ani_b200_mlp_step_windows(C.byref(self.charges[0].model), ws.rows_cap) + 1
+        return 3 + 1
+
+    def _charge_pass(self, ws: Workspace, run: tp.Callable[[str, tp.Callable[[], int]], None]) -> None:
+        """Enqueue the charge networks (forward only, one member) on the step's tiled AEVs ``ws.x`` and live column
+        blocks, then ani_b200_charges: normalised charges in input order and one dipole per conformer.  It goes after
+        every other kernel of the step: none of them writes ``ws.x`` after the AEV forward (the MLP reads it, the AEV
+        backward, the pair and D3 terms read ``dx`` / the neighbour words), so the energy step's own launches and
+        their order are those of a step without charges."""
+        if self.charge_mlp not in ("chained", "step"):
+            raise ValueError(f"ANI_B200_CHARGE_MLP={self.charge_mlp!r}: expected 'chained' or 'step'")
+        L = self.lib
+        qn, qp = self.charges
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        a1, a2, a3 = ws.q_act
+        if self.charge_mlp == "step":
+            run("charge_forward", lambda: L.ani_b200_mlp_step(
+                C.byref(qn.model), ptr(ws.x), None, ws.rows_cap, ptr(ws.row_atom), ptr(ws.layout_info),
+                ptr(ws.aev_blocks), ptr(a1), ptr(a2), ptr(a3), ptr(ws.q_raw), 0, ptr(ws.mlp_sync), ptr(ws.status), st))
+        else:
+            run("charge_forward", lambda: L.ani_b200_mlp_forward(
+                C.byref(qn.model), ptr(ws.x), ws.rows_cap, ptr(ws.row_atom), ptr(ws.layout_info), ptr(ws.aev_blocks),
+                ptr(a1), ptr(a2), ptr(a3), ptr(ws.q_raw), 0, ptr(ws.status), st))
+        w, m = qp.arrays()
+        run("charges", lambda: L.ani_b200_charges(
+            ptr(ws.q_raw), ptr(ws.row_of), ptr(ws.orig_to_sorted), ptr(ws.species_i32), ptr(ws.coords), ws.n_conf,
+            ws.n_per_conf, w, qn.num_species, int(qp.scale_by_q2), int(qp.normalize), 0.0, m, qp.frame,
+            ptr(ws.charges), ptr(ws.dipoles), st))
+
+    def charges_result(self, ws: Workspace) -> ChargesResult:
+        """Views of the charges and dipoles of the last ``run(..., charges=True)`` on ``ws``."""
+        assert ws.q_raw is not None, "no step with charges has run on this workspace"
+        return ChargesResult(ws.charges.view(ws.n_conf, ws.n_per_conf), ws.dipoles)
+
+    def raw_charges(self, ws: Workspace) -> Tensor:
+        """(C, A) float32 raw charges (the charge networks' outputs before the normaliser) of the last step with
+        charges, in input order, 0 for padding (a gather on the stream; for tests and diagnostics)."""
+        assert ws.q_raw is not None, "no step with charges has run on this workspace"
+        sp = ws.species_i32
+        rows = ws.row_of.long()[ws.orig_to_sorted.long().clamp(min=0)]
+        q = torch.where(sp >= 0, ws.q_raw[0][rows.clamp(min=0)], torch.zeros_like(ws.q_raw[0][:1]))
+        return q.view(ws.n_conf, ws.n_per_conf)
 
     def members_buffers(self, ws: Workspace) -> None:
         """Allocate the per-member slabs and gradients of the query-by-committee step (once per workspace, before any

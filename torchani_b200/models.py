@@ -591,6 +591,32 @@ def networks_from_torchani(netr) -> AtomicContainer:
     return nets
 
 
+def charge_networks_from_torchani(netr) -> "ChargeNetworks":
+    """The charge container of a reference ``SeparateChargesNNPotential`` -- ``ANINetworks`` with ``out_dim = 1`` or
+    ``_ANINetworksDiscardFirstScalar`` with ``out_dim = 2`` (column 1 kept) -- as a ``ChargeNetworks`` with the same
+    weights."""
+    from .nn import ChargeNetworks
+    if hasattr(netr, "members") or not hasattr(netr, "atomics"):
+        raise ValueError("charge networks: only one ANINetworks-style container is supported (no ensembles, SingleNN "
+                         "or shared networks)")
+    kept = 1 if type(netr).__name__ == "_ANINetworksDiscardFirstScalar" else 0
+    plain = networks_from_torchani(netr)
+    return ChargeNetworks(dict(plain.atomics.items()), kept_output=kept).requires_grad_(False)
+
+
+def charge_normalizer_from_torchani(norm, symbols):
+    """A reference ``ChargeNormalizer`` (its non-persistent ``weights`` buffer and scaling flag) or
+    ``BaseChargeNormalizer``."""
+    from .electro import BaseChargeNormalizer, ChargeNormalizer
+    name = type(norm).__name__
+    if name == "ChargeNormalizer":
+        return ChargeNormalizer(symbols, norm.weights.detach().double().cpu().tolist(),
+                                bool(norm.scale_weights_by_charges_squared))
+    if name == "BaseChargeNormalizer":
+        return BaseChargeNormalizer()
+    raise ValueError(f"charge normalizer {name!r} is not supported")
+
+
 def from_torchani(ref_model, device=None) -> ANI:
     """Convert a ``torchani.arch.ANI`` instance (reference, e.g. ``torchani.models.ANI2x()``) into
     the CUDA model: same symbols, AEV constants, network weights and self energies."""
@@ -611,7 +637,16 @@ def from_torchani(ref_model, device=None) -> ANI:
         except ValueError as exc:
             raise ValueError(f"cannot convert potential {name!r} of the reference model: {exc}; a converted model "
                              "without it would compute other energies and forces") from None
-    model = ANI(symbols, aevc, nets, sae, ref_model.periodic_table_index, extra)
+    nnp = ref_model.potentials["nnp"]
+    if type(nnp).__name__ == "MergedChargesNNPotential":
+        raise ValueError("merged charge networks (MergedChargesNNPotential) are not supported: their energy networks "
+                         "have out_dim = 2, which the fused backward does not run")
+    if hasattr(nnp, "charge_networks"):   # SeparateChargesNNPotential (arch.ANIq)
+        model: ANI = ANIq(symbols, aevc, nets, sae, extra, ref_model.periodic_table_index,
+                          charge_networks_from_torchani(nnp.charge_networks),
+                          charge_normalizer_from_torchani(nnp.charge_normalizer, symbols))
+    else:
+        model = ANI(symbols, aevc, nets, sae, ref_model.periodic_table_index, extra)
     model.requires_grad_(False)
     if device is None:
         device = ref_model.energy_shifter.self_energies.device
@@ -630,6 +665,10 @@ def accelerate_torchani_(ref_model):
     nets = networks_from_torchani(nnp.neural_networks).to(dev)
     nnp.aev_computer = aevc
     nnp.neural_networks = nets
+    if type(nnp).__name__ == "MergedChargesNNPotential":
+        raise ValueError("merged charge networks (MergedChargesNNPotential) are not supported")
+    if hasattr(nnp, "charge_networks"):   # SeparateChargesNNPotential: same AEV, forward-only charge networks
+        nnp.charge_networks = charge_networks_from_torchani(nnp.charge_networks).to(dev)
     ref_model.neighborlist = aevc.neighborlist
     # RepulsionXTB / RepulsionZBL / TwoBodyDispersionD3 members run through the CUDA pair-list kernels; any other
     # potential stays as it is
@@ -666,3 +705,242 @@ class _DropInPairPotential(torch.nn.Module):
         return self._Energies(self.potential.compute_from_neighbors(
             elem_idxs, coords, Neighbors(neighbors.indices, neighbors.distances, neighbors.diff_vectors), charge,
             atomic, ensemble_values, ghost_flags))
+
+
+# -- charge models (arch.py:579-680, models.py:201-252) -------------------------------------------------------------
+class SpeciesEnergiesAtomicCharges(tp.NamedTuple):   # tuples.py of the reference
+    species: Tensor
+    energies: Tensor
+    atomic_charges: Tensor
+
+
+class EnergiesScalars(tp.NamedTuple):
+    energies: Tensor
+    scalars: tp.Optional[Tensor] = None
+
+
+class _FusedEnergyCharges(torch.autograd.Function):
+    """``_FusedEnergy`` with the charge pass: coords -> (energies, atomic NN energies, member atomic, charges (C, A),
+    dipoles (C, 3)) from one step.  Charges and dipoles carry no gradient: a nonzero upstream gradient on them
+    raises."""
+
+    @staticmethod
+    def forward(ctx, coords: Tensor, species: Tensor, cell: tp.Optional[Tensor], pbc: bool, engine: Engine,
+                want_grad: bool):
+        res: StepResult = engine.step(species, coords.detach(), cell, pbc, want_grad=want_grad, check=True,
+                                      want_charges=True)
+        ws = engine.workspace(*species.shape)
+        q = engine.charges_result(ws)
+        ctx.want_grad = want_grad
+        if want_grad:
+            ctx.save_for_backward(res.grad.clone())
+        ctx.mark_non_differentiable(res.member_atomic)
+        return (res.energies.clone(), res.atomic_energies.clone(), res.member_atomic.clone(), q.charges.clone(),
+                q.dipoles.clone())
+
+    @staticmethod
+    def backward(ctx, g_energy, g_atomic, g_member, g_charges, g_dipoles):
+        for g in (g_charges, g_dipoles):
+            if g is not None and bool((g != 0).any()):
+                raise NotImplementedError("gradients of atomic charges and dipoles are not computed by the fused "
+                                          "engine (the charge networks run forward only)")
+        out, *_ = _FusedEnergy.backward(ctx, g_energy, g_atomic, g_member)
+        return out, None, None, None, None, None
+
+
+class ANIq(ANI):
+    r"""ANI-style model that computes atomic charges next to the energies (interface of arch.py:579-680), with
+    separate charge networks that read the energy networks' AEV (potentials/nnp.py:75-102,
+    ``SeparateChargesNNPotential``).
+
+    The charge networks run forward-only inside the fused step, on the AEVs it already built, and one more kernel
+    normalises the charges per conformer (``charge_normalizer``) and forms the dipoles.  Energies and forces are those
+    of an ``ANI`` with the same energy networks.  Merged charge networks (one container with ``out_dim = 2`` for
+    energies and charges) are not supported."""
+
+    def __init__(self, symbols: tp.Sequence[str], aev_computer: AEVComputer, neural_networks: AtomicContainer,
+                 energy_shifter: SelfEnergy, potentials: tp.Optional[tp.Mapping[str, PairPotential]] = None,
+                 periodic_table_index: bool = True, charge_networks: tp.Optional[AtomicContainer] = None,
+                 charge_normalizer: tp.Optional[torch.nn.Module] = None):
+        super().__init__(symbols, aev_computer, neural_networks, energy_shifter, periodic_table_index, potentials)
+        from .electro import BaseChargeNormalizer, ChargeNormalizer
+        from .nn import ChargeNetworks
+        if charge_networks is None:
+            raise ValueError("merged charge networks (MergedChargesNNPotential: energies and charges from one container "
+                             "with out_dim = 2) are not supported; pass separate charge_networks")
+        if not isinstance(charge_networks, ChargeNetworks):
+            raise ValueError("charge_networks must be a torchani_b200.nn.ChargeNetworks (one container, no ensemble)")
+        if charge_networks.num_species != len(symbols) or charge_networks.in_dim != neural_networks.member_networks()[0].in_dim:
+            raise ValueError("the charge networks must take the model's elements and AEV")
+        if charge_normalizer is None:
+            charge_normalizer = ChargeNormalizer(symbols)
+        if not isinstance(charge_normalizer, BaseChargeNormalizer):
+            raise ValueError("charge_normalizer must be a torchani_b200.electro.ChargeNormalizer or BaseChargeNormalizer")
+        self.charge_networks = charge_networks
+        self.charge_normalizer = charge_normalizer
+        # dipole frame of the step's charge pass (ANIq.dipoles sets it); forward reads only the charges
+        self._dipole_params: tp.Tuple[int, tp.Optional[tp.Tuple[float, ...]]] = (2, None)
+
+    def __getitem__(self, idx: int) -> "ANIq":
+        import copy
+        base = ANI.__getitem__(self, idx)
+        return ANIq(self.symbols, base.aev_computer, base.neural_networks, base.energy_shifter, dict(base.potentials),
+                    self.periodic_table_index, copy.deepcopy(self.charge_networks),
+                    copy.deepcopy(self.charge_normalizer))
+
+    def _charge_params(self):
+        from .electro import ChargeNormalizer
+        from .engine import ChargeParams
+        norm = self.charge_normalizer
+        frame, masses = self._dipole_params
+        if isinstance(norm, ChargeNormalizer):
+            w, q2 = norm.params()
+            return ChargeParams(w, q2, True, masses, frame)
+        return ChargeParams(tuple(1.0 for _ in self.symbols), False, False, masses, frame)
+
+    def engine(self, device: torch.device) -> Engine:
+        # the charge networks follow the energy networks' operand format (models.ANI._guarded switches both)
+        qnets = self.charge_networks
+        if qnets._variant != self.neural_networks._variant:
+            qnets.use_variant(self.neural_networks._variant)
+        eng = super().engine(device)
+        c = self.aev_computer.constants
+        qnets._radial_len = c.num_species * len(c.shf_r)
+        eng.set_charges((qnets.packed(device), self._charge_params()))
+        return eng
+
+    def _guarded(self, fn: tp.Callable[[], tp.Any]) -> tp.Any:
+        try:
+            return fn()
+        except _lib.OperandRangeError:
+            if self.neural_networks._variant == "bf16x3" or not _lib.available("bf16x3"):
+                raise
+            import warnings
+            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this model "
+                          "(energy and charge networks) to the 3 x bfloat16 build of the library")
+            self.neural_networks.use_variant("bf16x3")
+            self.charge_networks.use_variant("bf16x3")
+            return fn()
+
+    def _step_with_charges(self, species_coordinates, cell, pbc, charge: int, want_grad: tp.Optional[bool] = None):
+        """(elem_idxs, energies, atomic NN energies, member atomic, charges, dipoles) of one fused step, or, for a
+        periodic cell thinner than the cutoff, of a supercell (then normalised over the supercell; the first A atoms'
+        outputs are returned and the dipole is formed from their charges and the original coordinates)."""
+        species, coords = species_coordinates
+        self._check_inputs(species, coords, charge)
+        elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
+        _validate_inputs(self.cutoff, elem_idxs, coords, cell, pbc, conformer_cells=True)
+        sup = None if (isinstance(self.neighborlist, CellList) or _per_conformer(cell)) else \
+            supercell_for_thin_cell(species, coords, cell, pbc, self.cutoff)
+        if sup is not None:
+            sp_rep, co_rep, cell_rep, R = sup
+            a = elem_idxs.shape[1]
+            _, e, e_at, e_m, q, _ = self._step_with_charges((sp_rep, co_rep), cell_rep, pbc, charge, want_grad)
+            q = q[:, :a]
+            frame, masses = self._dipole_params
+            from .electro import run_charges
+            _, dip = run_charges(elem_idxs, q, coords, None, False, False, 0.0, masses, frame, True)
+            return elem_idxs, e / R, e_at[..., :a], e_m[..., :a], q, dip
+        cell = effective_periodic_cell(coords, cell, pbc, self.cutoff)
+        wg = bool(coords.requires_grad) if want_grad is None else want_grad
+        e, e_atomic, e_member, q, dip = self._guarded(lambda: _FusedEnergyCharges.apply(
+            coords, elem_idxs, cell, pbc is not None, self.engine(coords.device), wg))
+        return elem_idxs, e, e_atomic, e_member, q, dip
+
+    def forward(self, species_coordinates: tp.Tuple[Tensor, Tensor], cell: tp.Optional[Tensor] = None,
+                pbc: tp.Optional[Tensor] = None, charge: int = 0, atomic: bool = False,
+                ensemble_values: bool = False) -> SpeciesEnergiesAtomicCharges:
+        """arch.py:640-680: energies as ``ANI.forward`` and the normalised atomic charges (C, A) of the same step."""
+        coords = species_coordinates[1]
+        elem_idxs, e, e_atomic, e_member, q, _ = self._step_with_charges(species_coordinates, cell, pbc, charge)
+        if ensemble_values:
+            energies = e_member[self.neural_networks.active_members_idxs].to(coords.dtype)
+            if self.energy_shifter._enabled:
+                energies = energies + self.energy_shifter(elem_idxs, atomic=True).to(coords.dtype)
+            if not atomic:
+                energies = energies.sum(-1)
+        elif atomic:
+            energies = e_atomic.to(coords.dtype)
+            if self.energy_shifter._enabled:
+                energies = energies + self.energy_shifter(elem_idxs, atomic=True).to(coords.dtype)
+        else:
+            energies = e.to(coords.dtype)
+        return SpeciesEnergiesAtomicCharges(elem_idxs, energies, q.to(coords.dtype))
+
+    def dipoles(self, species_coordinates: tp.Tuple[Tensor, Tensor], cell: tp.Optional[Tensor] = None,
+                pbc: tp.Optional[Tensor] = None, charge: int = 0, reference: str = "center_of_mass",
+                masses: tp.Sequence[float] = ()) -> Tensor:
+        """Dipoles (C, 3) in e * Angstrom, ``sum_i q_i (r_i - r_ref)`` over the real atoms of the normalised charges of
+        the same fused step (electro.py:96-156, DipoleComputer), in the coordinates as given (not wrapped into the
+        cell).  ``masses``: one per symbol of the model, needed for ``reference="center_of_mass"`` (the reference's
+        mass table is not shipped)."""
+        from .electro import frame_index
+        frame = frame_index(reference)
+        if frame == 0 and len(masses) != len(self.symbols):
+            raise ValueError("the center_of_mass reference needs one mass per symbol of the model (masses=...): atomic "
+                             "masses are not shipped with torchani_b200")
+        self._dipole_params = (frame, tuple(float(m) for m in masses) if frame == 0 else None)
+        try:
+            coords = species_coordinates[1]
+            *_, dip = self._step_with_charges(species_coordinates, cell, pbc, charge, want_grad=False)
+        finally:
+            self._dipole_params = (2, None)
+        return dip.to(coords.dtype)
+
+    def compute_from_neighbors(self, elem_idxs: Tensor, coords: Tensor, neighbors: Neighbors, charge: int = 0,
+                               atomic: bool = False, ensemble_values: bool = False) -> EnergiesScalars:
+        """arch.py:620-660: energies as ``ANI.compute_from_neighbors`` and the normalised charges (C, A) of the charge
+        networks on the same AEVs."""
+        self._check_inputs(elem_idxs, coords, charge)
+        neighbors = discard_outside_cutoff(neighbors, self.cutoff)
+        rcr = self.aev_computer.radial.cutoff
+        aevs = self.aev_computer.compute_from_neighbors(
+            elem_idxs, coords, neighbors if self.cutoff <= rcr else discard_outside_cutoff(neighbors, rcr))
+        energies = self.neural_networks(elem_idxs, aevs, atomic, ensemble_values)
+        for pot in self._enabled_potentials():
+            energies = energies + pot.compute_from_neighbors(
+                elem_idxs, coords, discard_outside_cutoff(neighbors, pot.cutoff), charge, atomic,
+                ensemble_values).to(energies.dtype)
+        if self.energy_shifter._enabled:
+            energies = energies + self.energy_shifter(elem_idxs, atomic=atomic).to(energies.dtype)
+        if self.charge_networks._variant != self.neural_networks._variant:
+            self.charge_networks.use_variant(self.neural_networks._variant)
+        qs = self.charge_normalizer(elem_idxs, self.charge_networks(elem_idxs, aevs, atomic=True), charge)
+        return EnergiesScalars(energies, qs.to(coords.dtype))
+
+    def compute_from_full_neighborlist(self, *args, **kwargs):
+        raise NotImplementedError("charges over a full neighbour list with ghost atoms are not supported: the "
+                                  "normaliser needs every atom of the system")
+
+    def members_forces(self, *args, **kwargs):
+        raise ValueError("the query-by-committee step of an ANIq model computes no charges; call forward for the "
+                         "charges, or build an ANI from the same energy networks for the member forces")
+
+    def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs) -> None:
+        for old in list(state_dict.keys()):
+            if old.startswith(prefix + "potentials.nnp.charge_networks."):
+                state_dict[old.replace("potentials.nnp.charge_networks.", "charge_networks.", 1)] = state_dict.pop(old)
+        super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
+
+
+def ANImbis(model_index: tp.Optional[int] = None, neighborlist: NeighborlistArg = "cell_list",
+            periodic_table_index: bool = True, device=None, seed: tp.Optional[int] = 0,
+            electronegativity: tp.Sequence[float] = (), hardness: tp.Sequence[float] = ()) -> ANIq:
+    """The ANImbis architecture (models.py:201-252): ANI-2x energies (AEV, 8-member CELU ensemble, self energies) and
+    one set of charge networks with ANI-2x widths, GELU, no biases and ``out_dim = 2`` (column 1 is the charge), with a
+    ``ChargeNormalizer`` of weights (electronegativity / hardness)^2 scaled by the squared raw charges.  Weights are
+    seeded random (no download).  The electronegativities and hardnesses (one per symbol, ANI-2x order) are not
+    shipped: pass them, or convert a reference model with ``from_torchani``."""
+    from .electro import ChargeNormalizer
+    from .nn import ChargeNetworks
+    normalizer = ChargeNormalizer.from_electronegativity_and_hardness(
+        SYMBOLS_2X, electronegativity, hardness, scale_weights_by_charges_squared=True)
+    base = _assemble(SYMBOLS_2X, AEVComputer.like_2x, ANINetworks.like_2x, 8, neighborlist, periodic_table_index,
+                     seed, None)
+    qnets = ChargeNetworks.like_2x(SYMBOLS_2X, base.aev_computer.out_dim)
+    model = ANIq(SYMBOLS_2X, base.aev_computer, base.neural_networks, base.energy_shifter, None, periodic_table_index,
+                 qnets, normalizer)
+    model.requires_grad_(False)
+    if model_index is not None:
+        model = model[model_index]
+    return model.to(device) if device is not None else model

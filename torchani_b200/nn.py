@@ -257,7 +257,7 @@ class AtomicContainer(torch.nn.Module):
             params = self._packed_params = [p for m in members for p in m.parameters()]
             key = (str(device), self._variant, rl, tuple(p._version for p in params),
                    tuple(p.data_ptr() for p in params[:2]))
-            weights = [[m.atomics[s].linear_pairs() for s in m.atomics] for m in members]
+            weights = [[self._packing_pairs(m.atomics[s]) for s in m.atomics] for m in members]
             in_dim = members[0].in_dim
             self._packed = PackedNetworks(weights, in_dim, device, variant=self._variant,
                                           radial_len=getattr(self, "_radial_len", 0),
@@ -265,6 +265,10 @@ class AtomicContainer(torch.nn.Module):
             self._packed.set_active_members(self.active_members_idxs)
             self._packed_key = key
         return self._packed
+
+    def _packing_pairs(self, net: AtomicNetwork) -> tp.List[tp.Tuple[Tensor, tp.Optional[Tensor]]]:
+        """The (W, b) pairs of a network as the kernels get them (``ChargeNetworks`` keeps one output row)."""
+        return net.linear_pairs()
 
     def _run(self, elem_idxs: Tensor, aevs: Tensor, atomic: bool, ensemble_values: bool) -> Tensor:
         assert elem_idxs.shape == aevs.shape[:-1]
@@ -359,6 +363,47 @@ class ANINetworks(AtomicContainer):
                 activation: tp.Union[str, torch.nn.Module] = "celu", bias: bool = True):
         dims = {"H": (160, 128, 96), "C": (144, 112, 96), "N": (128, 112, 96), "O": (128, 112, 96)}
         return cls.build(symbols, in_dim, dims, out_dim, activation, bias, default_dims=(128, 112, 96))
+
+
+class ChargeNetworks(ANINetworks):
+    r"""Element-specific networks -> raw atomic charges, the charge networks of an ANIq model (potentials/nnp.py:75-102).
+
+    Two forms of the reference share this container and its module tree (``atomics.SYM.layers.K.weight``,
+    ``atomics.SYM.final_layer.weight``):
+
+    * ``ANINetworks`` with ``out_dim = 1`` (``simple_aniq``, arch.py:1071-1182): ``kept_output = 0``;
+    * ``_ANINetworksDiscardFirstScalar`` with ``out_dim = 2`` (ANImbis, nn/_internal.py:69-90): only output column 1
+      is used, ``kept_output = 1``.
+
+    The kernels get the kept row of every final layer.  Charges carry no gradient: ``forward`` evaluates the networks
+    forward-only."""
+
+    def __init__(self, modules: tp.Dict[str, AtomicNetwork], alias: bool = False, kept_output: tp.Optional[int] = None):
+        super().__init__(modules, alias)
+        if kept_output is None:
+            kept_output = 1 if self.out_dim == 2 else 0
+        if (self.out_dim, kept_output) not in ((1, 0), (2, 1)):
+            raise ValueError("charge networks have out_dim = 1, or out_dim = 2 of which column 1 is the charge "
+                             f"(_ANINetworksDiscardFirstScalar); got out_dim = {self.out_dim}, column {kept_output}")
+        self.kept_output = int(kept_output)
+
+    def _packing_pairs(self, net: AtomicNetwork) -> tp.List[tp.Tuple[Tensor, tp.Optional[Tensor]]]:
+        pairs = net.linear_pairs()
+        k = self.kept_output
+        w, b = pairs[-1]
+        return pairs[:-1] + [(w[k:k + 1], None if b is None else b[k:k + 1])]
+
+    def forward(self, elem_idxs: Tensor, aevs: tp.Optional[Tensor] = None, atomic: bool = True,
+                ensemble_values: bool = False) -> Tensor:
+        """Raw charges (C, A), 0 for padding atoms (or their sums per conformer with ``atomic=False``)."""
+        assert aevs is not None
+        return self._run(elem_idxs, aevs.detach(), atomic, False)
+
+    @classmethod
+    def like_2x(cls, symbols: tp.Sequence[str] = ("H", "C", "N", "O", "S", "F", "Cl"), in_dim: int = 1008,
+                out_dim: int = 2, activation: tp.Union[str, torch.nn.Module] = "gelu", bias: bool = False):
+        """ANImbis's charge networks (models.py:201-252): ANI-2x widths, GELU, no biases, ``out_dim = 2``."""
+        return super().like_2x(symbols, in_dim, out_dim, activation, bias)
 
 
 class ANIModel(ANINetworks):
