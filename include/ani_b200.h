@@ -30,6 +30,9 @@
  *   ani_b200_pair_potential     potentials/core.py:106-207, potentials/xtb.py:57-77, potentials/zbl.py:68-81
  *                               (RepulsionXTB / RepulsionZBL over the step's own neighbour list); _pairs: over a
  *                               caller-supplied half list, with ghost weights
+ *   ani_b200_pair_potential_search  the same and potentials/lj.py, potentials/fixed_coulomb.py (LennardJones,
+ *                               RepulsionLJ, DispersionLJ, FixedCoulomb, FixedMNOK) with a neighbour search of their own
+ *                               cutoff
  *   ani_b200_dispersion_d3      potentials/dftd3.py:102-311 (TwoBodyDispersionD3, D3(BJ) two-body dispersion with its
  *                               own neighbour search); _pairs: over a caller-supplied half list, with ghost weights
  *   ani_b200_charges            electro.py:29-156 (ChargeNormalizer.forward, DipoleComputer.forward) on the raw outputs of
@@ -279,6 +282,12 @@ int ani_b200_ensemble_qbc(const float* grad_members, const int32_t* members, int
 /*      kind 0 (xTB)  E = a[s][t] / d * exp(-b[s][t] * d^c[s][t])      a = y_ab, b = sqrt_alpha_ab, c = k_rep_ab          */
 /*      kind 1 (ZBL)  E = a[s][t] / d * sum_q screen_coeff[q] exp(-screen_exp[q] * b[s][t] * d)                          */
 /*                    a = Z_s Z_t, b = (Z_s^p + Z_t^p) / k                                                              */
+/*      kind 2 (LennardJones)  E = 4 a[s][t] (x^12 - x^6), x = b[s][t] / d     a = sqrt(eps_s eps_t),                  */
+/*      kind 3 (RepulsionLJ)   E = 4 a[s][t] x^12                                  b = (sigma_s + sigma_t) / 2 (A),       */
+/*      kind 4 (DispersionLJ)  E = -4 a[s][t] x^6                                  to_bohr = 1: the LJ kinds work in A    */
+/*      kind 5 (FixedCoulomb)  E = a[s][t] / d                                 a = q_s q_t / dielectric                 */
+/*      kind 6 (FixedMNOK)     E = a[s][t] / sqrt((R to_bohr)^2 + b[s][t]^2)   a = q_s q_t, b = 2 / (eta_s + eta_t);   */
+/*                             no clamp of R                                                                          */
 /*    times the envelope fc(R; cutoff): cutoff_fn 0 = cosine, 1 = smooth(2, 1e-10), 2 = none (then `cutoff` is not      */
 /*    read and no pair is screened out).  Pairs with R > cutoff contribute nothing.  The tables are symmetric.          */
 typedef struct ani_pair_params {
@@ -326,6 +335,25 @@ int ani_b200_pair_potential_pairs(const ani_pair_params* params, const int32_t* 
                                   const int64_t* idx1, const float* distances, const float* diff_vectors,
                                   const uint8_t* ghost_flags, int64_t num_pairs, int n_conf, int n_per_conf,
                                   float* atomic, double* energies, float* grad_coords, void* stream);
+/*    ani_b200_pair_potential_search evaluates one potential of any kind for the sorted atoms lo..hi-1 over a neighbour  */
+/*    search of its own cutoff on the grid of ani_b200_prepare_step (bin_start, spos, sorted_orig of that preparation),  */
+/*    the search of ani_b200_dispersion_d3 (4h): per lattice direction ceil((cutoff + skin) / bucket width) buckets, a   */
+/*    neighbour inside the cutoff at two images counts twice.  cutoff_fn 2 means no cutoff and is for open systems      */
+/*    (grid modes 0 and 1), whose stencil then spans the grid or the conformer's bucket.  Periodic widths must be >=      */
+/*    cutoff + skin, else ANI_STATUS_CELL_TOO_SMALL is OR-ed into status and the atoms of that cell write nothing.       */
+/*    Outputs, add-only contract, ordering and member rules are those of ani_b200_pair_potential.  One launch.  The      */
+/*    _cells form is for grid mode 3 and takes its lattice table (not NULL).                                             */
+int ani_b200_pair_potential_search(const ani_pair_params* params, const ani_grid* grid, const int32_t* bin_start,
+                                   const float* spos, const int32_t* sorted_orig, int n, int lo, int hi, int n_conf,
+                                   int n_per_conf, float skin, float* atomic, double* energies, float* grad_coords,
+                                   double* virial, float* member_atomic, float* grad_members, const int32_t* members,
+                                   int n_members, int32_t* status, void* stream);
+int ani_b200_pair_potential_search_cells(const ani_pair_params* params, const ani_grid* grid,
+                                         const int32_t* bin_start, const float* spos, const int32_t* sorted_orig,
+                                         int n, int lo, int hi, int n_conf, int n_per_conf, float skin, float* atomic,
+                                         double* energies, float* grad_coords, double* virial, float* member_atomic,
+                                         float* grad_members, const int32_t* members, int n_members, int32_t* status,
+                                         const float* lattice, void* stream);
 
 /* 4h. D3(BJ) two-body dispersion (potentials/dftd3.py:140-311, TwoBodyDispersionD3) with its own neighbour search    */
 /*    over the step's bucket grid (its cutoff, 8 A in the reference's models, is beyond Rcr).  With d = R * to_bohr:       */

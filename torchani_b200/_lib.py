@@ -98,6 +98,7 @@ _I = C.c_int
 _F = C.c_float
 _D3_ARGS = [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P]
 _PAIR_ARGS = [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I]
+_PAIR_SEARCH_ARGS = [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P, _P, _P, _P, _P, _P, _P, _I, _P]
 
 _PROTOTYPES = {
     "ani_b200_abi_version": (C.c_int, []),
@@ -128,6 +129,8 @@ _PROTOTYPES = {
     "ani_b200_ensemble_qbc": (C.c_int, [_P, _P, _I, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
     "ani_b200_pair_potential": (C.c_int, _PAIR_ARGS + [_P]),
     "ani_b200_pair_potential_cells": (C.c_int, _PAIR_ARGS + [_P, _P]),
+    "ani_b200_pair_potential_search": (C.c_int, _PAIR_SEARCH_ARGS + [_P]),
+    "ani_b200_pair_potential_search_cells": (C.c_int, _PAIR_SEARCH_ARGS + [_P, _P]),
     "ani_b200_pair_potential_pairs": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int64, _I, _I, _P, _P, _P, _P]),
     "ani_b200_dispersion_d3": (C.c_int, _D3_ARGS + [_P]),
     "ani_b200_dispersion_d3_cells": (C.c_int, _D3_ARGS + [_P, _P]),

@@ -18,14 +18,9 @@
 //   * No valid reference.  An element pair with no positive C6ref gets C6 = 1 and dC6/dCN = 0, as eps / eps does in
 //     the reference.
 //
-// The neighbour search is this file's own: the AEV's neighbour words end at Rcr, D3 reaches 8 A or more.  It runs on
-// the bucket grid of the step (bin_start, spos, ani_grid; the lattice table in grid mode 3) with a stencil of
-// `reach_d = ceil((cutoff + skin) / bucket width_d)` buckets per lattice direction, bucket width = perpendicular width
-// / dims.  Offsets -reach..reach are distinct (bucket, image) pairs, so a neighbour inside the cutoff at two images
-// (cells between 1x and 2x the cutoff) counts twice, as the reference's multi-image lists count it.  Image codes stay
-// the 27 codes of common.cuh, which needs reach_d <= dims_d, i.e. every periodic width >= cutoff + skin; below that
-// the first launch ORs ANI_STATUS_CELL_TOO_SMALL and nothing is written.  Open systems clip the stencil to the grid;
-// grid mode 1 (one bucket per conformer) walks the conformer's bucket.
+// The neighbour search is search_neighbours of terms.cuh: the AEV's neighbour words end at Rcr, D3 reaches 8 A or
+// more.  It needs every periodic width >= cutoff + skin; below that the first launch ORs ANI_STATUS_CELL_TOO_SMALL
+// and nothing is written.
 //
 // Three launches, each over the results of the previous one for ALL real atoms:
 //   1. CN of every real atom (plain stores into cn[sorted index]),
@@ -44,118 +39,6 @@ namespace ani {
 constexpr int D3_WARPS = 8;
 constexpr int D3_REFS = 25;   // 5 x 5 reference pairs per element pair
 constexpr float D3_LN_EPS = -80.5904782547916f;   // ln(1e-35), the eps of dftd3.py:177
-
-// largest bucket b with bin_start[b] <= i: the bucket of sorted atom i (empty buckets share their start with the next)
-__device__ __forceinline__ int bucket_of(const int32_t* __restrict__ bin_start, int nbins, int i) {
-  int lo = 0, hi = nbins - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (__ldg(bin_start + mid) <= i) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
-}
-
-// a neighbour inside the cutoff, queued in shared memory until the warp has 32 of them
-struct D3Hit {
-  int j, sj;
-  float dx, dy, dz, R;
-};
-constexpr int D3_QUEUE = 64;
-
-// Calls f(j, sj, dx, dy, dz, R) for every neighbour j of sorted atom i with R <= cutoff (Delta = r_j + shift - r_i).
-// The warp screens 32 candidates at a time (about one in eight is inside an 8 A cutoff on a 5 A bucket grid) and
-// queues the hits in `q` (D3_QUEUE entries of this warp's shared memory); f runs on 32 queued hits at a time, so the
-// per-pair work (the 25-term C6 interpolation) runs with all lanes busy.  The order of the hits, and so every lane's
-// partial sum, depends only on the grid.  Warp-uniform; returns false (nothing visited) if a periodic width is below
-// cutoff + skin.
-template <bool LAT, class F>
-__device__ __forceinline__ bool d3_neighbours(const ani_d3_params& P, const ani_grid& g,
-                                              const int32_t* __restrict__ bin_start, const float4* __restrict__ spos,
-                                              const float* __restrict__ lattice, int i, float4 pi, int conf,
-                                              float skin, D3Hit* __restrict__ q, F&& f) {
-  const int lane = threadIdx.x & 31;
-  const float cut2 = P.cutoff * P.cutoff;
-  int qn = 0;   // queued hits (warp-uniform)
-  auto drain = [&]() {
-    const int m = min(qn, 32);
-    if (lane < m) {
-      const D3Hit h = q[lane];
-      f(h.j, h.sj, h.dx, h.dy, h.dz, h.R);
-    }
-    __syncwarp();
-    if (lane < qn - 32) q[lane] = q[lane + 32];
-    __syncwarp();
-    qn -= m;
-  };
-  auto run = [&](int lo, int hi, int code) {
-    float3 sh = make_float3(0.f, 0.f, 0.f);
-    if (code != 13) sh = LAT ? image_shift(lattice, conf, code) : image_shift(g, code);
-    for (int b0 = lo; b0 < hi; b0 += 32) {
-      const int j = b0 + lane;
-      bool hit = false;
-      D3Hit h;
-      if (j < hi && !(code == 13 && j == i)) {
-        const float4 p = spos[j];
-        h.dx = (p.x + sh.x) - pi.x;
-        h.dy = (p.y + sh.y) - pi.y;
-        h.dz = (p.z + sh.z) - pi.z;
-        const float r2 = h.dx * h.dx + h.dy * h.dy + h.dz * h.dz;
-        hit = r2 <= cut2;
-        h.j = j;
-        h.sj = __float_as_int(p.w);
-        h.R = sqrtf(r2);
-      }
-      const unsigned m = __ballot_sync(ANI_FULL_MASK, hit);
-      if (hit) q[qn + __popc(m & ((1u << lane) - 1u))] = h;
-      __syncwarp();
-      qn += __popc(m);
-      if (qn >= 32) drain();
-    }
-  };
-  if (!LAT && g.mode == 1) {   // one bucket per conformer
-    run(__ldg(bin_start + conf), __ldg(bin_start + conf + 1), 13);
-    if (qn > 0) drain();
-    return true;
-  }
-  int ix, iy, iz;
-  const int base = bucket_coords(g, bucket_of(bin_start, g.nbins, i), ix, iy, iz);
-  const float* inv = LAT ? lattice + (size_t)conf * ANI_LATTICE_STRIDE + 9 : g.inv;
-  const float reach_len = P.cutoff + skin;
-  int r[3];
-#pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    const float perp = 1.0f / sqrtf(inv[d] * inv[d] + inv[3 + d] * inv[3 + d] + inv[6 + d] * inv[6 + d]);
-    r[d] = (int)ceilf(reach_len * (float)g.dims[d] / perp);
-    if (g.pbc) {
-      if (r[d] > g.dims[d]) return false;
-    } else {
-      r[d] = min(r[d], g.dims[d] - 1);
-    }
-  }
-  const int dx_ = g.dims[0], dy_ = g.dims[1], dz_ = g.dims[2];
-  for (int ox = -r[0]; ox <= r[0]; ++ox) {
-    int jx = ix + ox, wx = jx < 0 ? -1 : (jx >= dx_ ? 1 : 0);
-    if (wx && !g.pbc) continue;
-    jx -= wx * dx_;
-    for (int oy = -r[1]; oy <= r[1]; ++oy) {
-      int jy = iy + oy, wy = jy < 0 ? -1 : (jy >= dy_ ? 1 : 0);
-      if (wy && !g.pbc) continue;
-      jy -= wy * dy_;
-      const int row = base + (jx * dy_ + jy) * dz_;
-      // the z run iz-r..iz+r in up to three contiguous pieces, one per image
-      for (int wz = -1; wz <= 1; ++wz) {
-        if (wz && !g.pbc) continue;
-        const int zlo = max(iz - r[2], wz * dz_), zhi = min(iz + r[2], wz * dz_ + dz_ - 1);
-        if (zlo > zhi) continue;
-        run(__ldg(bin_start + row + zlo - wz * dz_), __ldg(bin_start + row + zhi - wz * dz_ + 1),
-            (wx + 1) * 9 + (wy + 1) * 3 + (wz + 1));
-      }
-    }
-  }
-  if (qn > 0) drain();
-  return true;
-}
 
 // coordination-number count of a pair and its derivative with respect to R (Angstrom)
 __device__ __forceinline__ void d3_count(const ani_d3_params& P, int a, int b, float R, float& c, float& dc) {
@@ -237,7 +120,7 @@ __global__ void __launch_bounds__(D3_WARPS * 32)
                     int hi, int n_per_conf, float skin, const float* __restrict__ lattice, float* __restrict__ cn,
                     float* __restrict__ dedcn, const __grid_constant__ TermOut out,
                     const __grid_constant__ ActiveMembers ms, int32_t* __restrict__ status) {
-  __shared__ D3Hit s_q[D3_WARPS][D3_QUEUE];
+  __shared__ SearchHit s_q[D3_WARPS][SEARCH_QUEUE];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const ani_grid g = *grid;
   const int end = min(PASS == 3 ? hi : n, g.n_real);
@@ -258,8 +141,8 @@ __global__ void __launch_bounds__(D3_WARPS * 32)
     const float dedcn_i = PASS == 3 ? dedcn[i] : 0.f;
     bool ok = true;
     if (si >= 0) {
-      ok = d3_neighbours<LAT>(P, g, bin_start, spos, lattice, i, pi, conf_i, skin, s_q[warp],
-                              [&](int j, int sj, float dx, float dy, float dz, float R) {
+      ok = search_neighbours<LAT>(P.cutoff, g, bin_start, spos, lattice, i, pi, conf_i, skin, s_q[warp],
+                                  [&](int j, int sj, float dx, float dy, float dz, float R) {
         if (sj < 0) return;
         if (PASS == 1) {
           float c, dc;

@@ -1,4 +1,4 @@
-// Pair potentials (short-range repulsion) evaluated over the neighbour list of the step.
+// Pair potentials evaluated over the neighbour list of the step, or over a neighbour search of their own cutoff.
 //
 // The AEV forward leaves, for every processed atom, the neighbours within Rcr as words (sorted index | image code
 // << 26), BOTH directions of every pair.  A pair potential with a cutoff <= Rcr therefore needs no neighbour search of
@@ -11,39 +11,100 @@
 // and central-atom shards need nothing new: an atom's gradient comes from the rank that owns it, a pair's energy is
 // split between the owners of its two ends.
 //
-// Functional forms (potentials/xtb.py:57-77, potentials/zbl.py:68-81), d = max(R, 1e-7) * to_bohr:
-//   xTB  E = y_ab / d * exp(-sqrt_alpha_ab * d^k_ab)
-//   ZBL  E = Z_a Z_b / d * sum_q c_q exp(-x_q * d * (Z_a^p + Z_b^p) / k)
+// Functional forms (potentials/xtb.py:57-77, potentials/zbl.py:68-81, potentials/lj.py:118-145,
+// potentials/fixed_coulomb.py:28-81), d = max(R, 1e-7) * to_bohr (to_bohr = 1 for the LJ kinds, which work in A):
+//   0 xTB           E = y_ab / d * exp(-sqrt_alpha_ab * d^k_ab)
+//   1 ZBL           E = Z_a Z_b / d * sum_q c_q exp(-x_q * d * (Z_a^p + Z_b^p) / k)
+//   2 LennardJones  E = 4 eps_ab (x^12 - x^6), x = sigma_ab / d
+//   3 RepulsionLJ   E = 4 eps_ab x^12
+//   4 DispersionLJ  E = -4 eps_ab x^6
+//   5 FixedCoulomb  E = qq_ab / d                         (qq_ab = q_a q_b / dielectric)
+//   6 FixedMNOK     E = qq_ab / sqrt(d^2 + inv_eta_ab^2), d = R * to_bohr without the clamp
 // Arithmetic: expf / sqrtf / powf and true divisions (the repulsion is of order 1 Ha at 0.4 A, so the approximate MUFU
 // forms of the AEV kernels would cost the 1e-5 relative bar on atomic energies); d^1.5 is d * sqrt(d).
+//
+// Kinds 0 and 1 run over the AEV's neighbour words (k_pair_potential, cutoff <= Rcr).  Every kind also runs over
+// search_neighbours of terms.cuh at its own cutoff (k_pair_potential_search): the LJ and Coulomb terms are used at
+// 8-12 A or without a cutoff, far beyond Rcr.
 #include "terms.cuh"
 
 namespace ani {
 
 constexpr int PAIR_WARPS = 8;
 
+// E and dE/dd of each kind at d (Bohr, or A for the LJ kinds)
+__device__ __forceinline__ float pair_xtb(const ani_pair_params& P, int a, int b, float d, float& dE) {
+  const float y = P.a[a][b], sa = P.b[a][b], k = P.c[a][b];
+  const float dk = (k == 1.5f) ? d * sqrtf(d) : (k == 1.0f) ? d : powf(d, k);
+  const float E = y / d * expf(-sa * dk);
+  dE = -E * (1.0f + sa * k * dk) / d;
+  return E;
+}
+
+__device__ __forceinline__ float pair_zbl(const ani_pair_params& P, int a, int b, float d, float& dE) {
+  const float zz = P.a[a][b], s = P.b[a][b];
+  float sum = 0.f, dsum = 0.f;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float t = P.screen_coeff[q] * expf(-P.screen_exp[q] * s * d);
+    sum += t;
+    dsum = fmaf(-P.screen_exp[q] * s, t, dsum);
+  }
+  const float E = zz / d * sum;
+  dE = (zz * dsum - E) / d;
+  return E;
+}
+
+__device__ __forceinline__ float pair_lj(const ani_pair_params& P, int a, int b, float d, float& dE) {
+  const float x = P.b[a][b] / d, x2 = x * x, x6 = x2 * x2 * x2, x12 = x6 * x6;
+  const float e4 = 4.f * P.a[a][b];
+  dE = e4 * (6.f * x6 - 12.f * x12) / d;
+  return e4 * (x12 - x6);
+}
+
+__device__ __forceinline__ float pair_lj_repulsion(const ani_pair_params& P, int a, int b, float d, float& dE) {
+  const float x = P.b[a][b] / d, x2 = x * x, x6 = x2 * x2 * x2;
+  const float E = 4.f * P.a[a][b] * (x6 * x6);
+  dE = -12.f * E / d;
+  return E;
+}
+
+__device__ __forceinline__ float pair_lj_dispersion(const ani_pair_params& P, int a, int b, float d, float& dE) {
+  const float x = P.b[a][b] / d, x2 = x * x, x6 = x2 * x2 * x2;
+  const float E = -4.f * P.a[a][b] * x6;
+  dE = -6.f * E / d;
+  return E;
+}
+
+__device__ __forceinline__ float pair_coulomb(const ani_pair_params& P, int a, int b, float d, float& dE) {
+  const float E = P.a[a][b] / d;
+  dE = -E / d;
+  return E;
+}
+
+__device__ __forceinline__ float pair_mnok(const ani_pair_params& P, int a, int b, float d, float& dE) {
+  const float ie = P.b[a][b];
+  const float u = fmaf(d, d, ie * ie);
+  const float E = P.a[a][b] / sqrtf(u);
+  dE = -E * d / u;
+  return E;
+}
+
 // E(R) fc(R) and its derivative with respect to R (Angstrom) for the element pair (a, b)
 __device__ __forceinline__ void pair_energy(const ani_pair_params& P, int a, int b, float R, float& e, float& de) {
-  const float d = fmaxf(R, 1e-7f) * P.to_bohr;   // potentials/core.py:137-139
+  const bool clamp = P.kind != 6;                // potentials/core.py:137-139; FixedMNOK does not clamp
+  const float d = (clamp ? fmaxf(R, 1e-7f) : R) * P.to_bohr;
   float E, dE;                                   // dE: dE/dd
-  if (P.kind == 0) {
-    const float y = P.a[a][b], sa = P.b[a][b], k = P.c[a][b];
-    const float dk = (k == 1.5f) ? d * sqrtf(d) : (k == 1.0f) ? d : powf(d, k);
-    E = y / d * expf(-sa * dk);
-    dE = -E * (1.0f + sa * k * dk) / d;
-  } else {
-    const float zz = P.a[a][b], s = P.b[a][b];
-    float sum = 0.f, dsum = 0.f;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float t = P.screen_coeff[q] * expf(-P.screen_exp[q] * s * d);
-      sum += t;
-      dsum = fmaf(-P.screen_exp[q] * s, t, dsum);
-    }
-    E = zz / d * sum;
-    dE = (zz * dsum - E) / d;
+  switch (P.kind) {
+    case 0: E = pair_xtb(P, a, b, d, dE); break;
+    case 1: E = pair_zbl(P, a, b, d, dE); break;
+    case 2: E = pair_lj(P, a, b, d, dE); break;
+    case 3: E = pair_lj_repulsion(P, a, b, d, dE); break;
+    case 4: E = pair_lj_dispersion(P, a, b, d, dE); break;
+    case 5: E = pair_coulomb(P, a, b, d, dE); break;
+    default: E = pair_mnok(P, a, b, d, dE); break;
   }
-  dE = (R >= 1e-7f) ? dE * P.to_bohr : 0.f;      // the clamp has no slope below its floor
+  dE = (!clamp || R >= 1e-7f) ? dE * P.to_bohr : 0.f;   // the clamp has no slope below its floor
   float f = 1.f, df = 0.f;
   if (P.cutoff_fn != 2) cutoff_value_grad(R, P.cutoff, P.cutoff_fn, f, df);
   e = E * f;
@@ -104,6 +165,58 @@ __global__ void __launch_bounds__(PAIR_WARPS * 32)
   add_conformer_energies<PAIR_WARPS>(out.energies, e_out, conf_out);
 }
 
+// The same sums over search_neighbours at the potential's own cutoff (cutoff_fn 2: no cutoff, open systems only): one
+// warp per owned sorted atom, both directions of every pair, outputs and ordering rules of k_pair_potential.  A periodic
+// width below cutoff + skin ORs ANI_STATUS_CELL_TOO_SMALL and the atom writes nothing.
+template <bool LAT, bool VIRIAL>
+__global__ void __launch_bounds__(PAIR_WARPS * 32)
+    k_pair_potential_search(const __grid_constant__ ani_pair_params P, const ani_grid* __restrict__ grid,
+                            const int32_t* __restrict__ bin_start, const float4* __restrict__ spos,
+                            const int32_t* __restrict__ sorted_orig, int n, int lo, int hi, int n_per_conf, float skin,
+                            const float* __restrict__ lattice, const __grid_constant__ TermOut out,
+                            const __grid_constant__ ActiveMembers ms, int32_t* __restrict__ status) {
+  __shared__ SearchHit s_q[PAIR_WARPS][SEARCH_QUEUE];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const ani_grid g = *grid;
+  hi = min(hi, g.n_real);
+  const int i = lo + blockIdx.x * PAIR_WARPS + warp;
+  const float cutoff = P.cutoff_fn == 2 ? INFINITY : P.cutoff;
+  int conf_out = -1;
+  float e_out = 0.f;
+  if (i < hi) {
+    const float4 pi = spos[i];
+    const int si = __float_as_int(pi.w);
+    const int oi = sorted_orig[i];
+    const int conf_i = oi / n_per_conf;
+    float e = 0.f, gx = 0.f, gy = 0.f, gz = 0.f;
+    float vir[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) vir[k] = 0.f;
+    if (si >= 0) {
+      const bool ok = search_neighbours<LAT>(cutoff, g, bin_start, spos, lattice, i, pi, conf_i, skin, s_q[warp],
+                                             [&](int j, int sj, float dx, float dy, float dz, float R) {
+        if (sj < 0) return;
+        float ep, de;
+        pair_energy(P, si, sj, R, ep, de);
+        e = fmaf(0.5f, ep, e);
+        const float sc = R >= 1e-7f ? de / R : 0.f;   // dE/dDelta = sc * Delta
+        const float fx = sc * dx, fy = sc * dy, fz = sc * dz;
+        gx -= fx;
+        gy -= fy;
+        gz -= fz;
+        if (VIRIAL) add_outer(vir, fx, fy, fz, dx, dy, dz);
+      });
+      if (!ok) {
+        if (lane == 0 && status) atomicOr(status, ANI_STATUS_CELL_TOO_SMALL);
+      } else {
+        e_out = add_atom_term<true, VIRIAL>(out, ms, n, g.mode, oi, conf_i, e, gx, gy, gz, vir);
+        conf_out = conf_i;
+      }
+    }
+  }
+  add_conformer_energies<PAIR_WARPS>(out.energies, e_out, conf_out);
+}
+
 // The same potential over a caller-supplied HALF pair list (the reference's Neighbors tuple; diff = x[idx0] - x[idx1] +
 // shift): one thread per pair, float atomics (not the hot path).  Pairs that touch a ghost atom count half
 // (potentials/core.py:170-177); pairs beyond the cutoff and pairs with a padding atom contribute nothing.
@@ -132,7 +245,7 @@ __global__ void k_pair_potential_pairs(const __grid_constant__ ani_pair_params P
 static int check_pair_params(const ani_pair_params* p) {
   const int rc = check_term_params(p);
   if (rc != ANI_OK) return rc;
-  return p->kind == 0 || p->kind == 1 ? ANI_OK : ANI_ERR_BAD_ARG;
+  return p->kind >= 0 && p->kind <= 6 ? ANI_OK : ANI_ERR_BAD_ARG;
 }
 
 static int launch_pair_potential(const ani_pair_params* params, const ani_grid* grid, const float* spos,
@@ -165,6 +278,36 @@ static int launch_pair_potential(const ani_pair_params* params, const ani_grid* 
   return ANI_OK;
 }
 
+static int launch_pair_potential_search(const ani_pair_params* params, const ani_grid* grid, const int32_t* bin_start,
+                                        const float* spos, const int32_t* sorted_orig, int n, int lo, int hi,
+                                        int n_conf, int n_per_conf, float skin, float* atomic, double* energies,
+                                        float* grad_coords, double* virial, float* member_atomic, float* grad_members,
+                                        const int32_t* members, int n_members, int32_t* status, const float* lattice,
+                                        bool want_lattice, void* stream) {
+  int rc = check_pair_params(params);
+  if (rc != ANI_OK) return rc;
+  ActiveMembers ms;
+  rc = check_step_term_args(grid, spos, sorted_orig, n, lo, hi, n_conf, n_per_conf, lattice, want_lattice,
+                            member_atomic, grad_members, members, n_members, ms);
+  if (rc != ANI_OK) return rc;
+  if (!bin_start || !(skin >= 0.f)) return ANI_ERR_BAD_ARG;
+  if (hi == lo) return ANI_OK;
+  const int blocks = (hi - lo + PAIR_WARPS - 1) / PAIR_WARPS;
+  const TermOut out{atomic, energies, grad_coords, virial, member_atomic, grad_members};
+  auto launch = [&](auto kernel) {
+    kernel<<<blocks, PAIR_WARPS * 32, 0, (cudaStream_t)stream>>>(
+        *params, grid, bin_start, reinterpret_cast<const float4*>(spos), sorted_orig, n, lo, hi, n_per_conf, skin,
+        lattice, out, ms, status);
+  };
+  if (want_lattice) {
+    virial ? launch(k_pair_potential_search<true, true>) : launch(k_pair_potential_search<true, false>);
+  } else {
+    virial ? launch(k_pair_potential_search<false, true>) : launch(k_pair_potential_search<false, false>);
+  }
+  ANI_CUDA_CHECK_LAUNCH();
+  return ANI_OK;
+}
+
 }  // namespace ani
 
 extern "C" int ani_b200_pair_potential(const ani_pair_params* params, const ani_grid* grid, const float* spos,
@@ -187,6 +330,29 @@ extern "C" int ani_b200_pair_potential_cells(const ani_pair_params* params, cons
   return ani::launch_pair_potential(params, grid, spos, sorted_orig, n, lo, hi, n_conf, n_per_conf, nbr_cnt, nbr_list,
                                     nbr_cap, atomic, energies, grad_coords, virial, member_atomic, grad_members,
                                     members, n_members, lattice, true, stream);
+}
+
+extern "C" int ani_b200_pair_potential_search(const ani_pair_params* params, const ani_grid* grid,
+                                              const int32_t* bin_start, const float* spos, const int32_t* sorted_orig,
+                                              int n, int lo, int hi, int n_conf, int n_per_conf, float skin,
+                                              float* atomic, double* energies, float* grad_coords, double* virial,
+                                              float* member_atomic, float* grad_members, const int32_t* members,
+                                              int n_members, int32_t* status, void* stream) {
+  return ani::launch_pair_potential_search(params, grid, bin_start, spos, sorted_orig, n, lo, hi, n_conf, n_per_conf,
+                                           skin, atomic, energies, grad_coords, virial, member_atomic, grad_members,
+                                           members, n_members, status, nullptr, false, stream);
+}
+
+extern "C" int ani_b200_pair_potential_search_cells(const ani_pair_params* params, const ani_grid* grid,
+                                                    const int32_t* bin_start, const float* spos,
+                                                    const int32_t* sorted_orig, int n, int lo, int hi, int n_conf,
+                                                    int n_per_conf, float skin, float* atomic, double* energies,
+                                                    float* grad_coords, double* virial, float* member_atomic,
+                                                    float* grad_members, const int32_t* members, int n_members,
+                                                    int32_t* status, const float* lattice, void* stream) {
+  return ani::launch_pair_potential_search(params, grid, bin_start, spos, sorted_orig, n, lo, hi, n_conf, n_per_conf,
+                                           skin, atomic, energies, grad_coords, virial, member_atomic, grad_members,
+                                           members, n_members, status, lattice, true, stream);
 }
 
 extern "C" int ani_b200_pair_potential_pairs(const ani_pair_params* params, const int32_t* species,

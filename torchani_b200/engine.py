@@ -585,8 +585,9 @@ class Engine:
                  dispersion: tp.Optional[tp.Tuple[D3Params, Tensor]] = None,
                  charges: tp.Optional[tp.Tuple[PackedNetworks, ChargeParams]] = None):
         """``pairs``: the ``ani_pair_params`` of the model's pair potentials (potentials.PairPotential.params()); each
-        adds one launch to the step (``_pair_potentials``), a model without any issues exactly the launches it
-        issued before.  ``dispersion``: the ``ani_d3_params`` and device tables of a D3 term
+        adds one launch to the step, a model without any issues exactly the launches it issued before.  The repulsion
+        kinds (0 xTB, 1 ZBL) run over the AEV's neighbour words and need cutoff <= Rcr (``_pair_potentials``); the LJ
+        and Coulomb kinds (2-6) run over a neighbour search of their own cutoff, at any cutoff (``_search_pairs``).  ``dispersion``: the ``ani_d3_params`` and device tables of a D3 term
         (potentials.TwoBodyDispersionD3.params() / .tables(device)), or None; it adds three launches to a step with
         forces and two to one without (``_dispersion``).  ``charges``: the packed charge networks (one member) and the
         normaliser / dipole parameters of a charge model; a step asked for charges (``run(..., charges=True)``) runs
@@ -597,10 +598,12 @@ class Engine:
             raise ValueError("network / AEV species mismatch")
         self.consts, self.nets = consts, nets
         for p in pairs:
-            check_pair_cutoff(math.inf if p.cutoff_fn == 2 else p.cutoff, consts.rcr)
+            if p.kind in (0, 1):
+                check_pair_cutoff(math.inf if p.cutoff_fn == 2 else p.cutoff, consts.rcr)
             if p.num_species != consts.num_species:
                 raise ValueError("pair potential / AEV species mismatch")
-        self.pairs = list(pairs)
+        self.pairs = [p for p in pairs if p.kind in (0, 1)]
+        self.search_pairs = [p for p in pairs if p.kind not in (0, 1)]
         if dispersion is not None:
             d3p, d3t = dispersion
             if d3p.cutoff_fn == 2 or not d3p.cutoff > 0:
@@ -775,8 +778,11 @@ class Engine:
             raise ValueError("the workspace of a periodic batch needs Workspace.make_periodic() first")
         if periodic_batch and reuse:
             raise ValueError("reuse=True (Verlet skin) is not supported for periodic batches")
+        if pbc and any(p.cutoff_fn == 2 for p in self.search_pairs):
+            raise ValueError("PBC can't use an infinite cutoff: a pair potential without a cutoff runs on open systems "
+                             "only")
         key = (n_conf, n_per_conf, bool(pbc), bool(want_grad), lo, hi, self.nets.active_key, bool(reuse), self.skin,
-               bool(want_virial), self.mlp_mode, conformer_cells, members)
+               bool(want_virial), self.mlp_mode, conformer_cells, members, tuple(p.kind for p in self.search_pairs))
         if charges:   # (the charge networks' operands and the normaliser / dipole parameters are baked into the capture)
             key = key + (self.charges[0], self.charges[1], self.charge_mlp)
         if reuse and not self.skin > 0:
@@ -822,7 +828,7 @@ class Engine:
         else:
             mlp = 3 + (4 if want_grad else 0)
         self.launches_per_step = (1 + (0 if (pbc or n_conf > 1) else 1) + 1 + mlp + (1 if want_grad else 0) + 1
-                                  + len(self.pairs))
+                                  + len(self.pairs) + len(self.search_pairs))
         if self.dispersion is not None:   # CN, energies + dE/dCN, and the chain where forces are wanted
             self.launches_per_step += 3 if (want_grad or members) else 2
         if charges:
@@ -979,6 +985,9 @@ class Engine:
         if self.pairs:
             self._pair_potentials(ws, lo, hi, lat, ws.grad_ptr if want_grad else None,
                                   ptr(ws.virial) if want_virial else None, None, self._timed)
+        if self.search_pairs:
+            self._search_pairs(ws, lo, hi, lat, ws.grad_ptr if want_grad else None,
+                               ptr(ws.virial) if want_virial else None, None, self._timed)
         if self.dispersion is not None:
             self._dispersion(ws, lo, hi, lat, ws.grad_ptr if want_grad else None,
                              ptr(ws.virial) if want_virial else None, None, self._timed)
@@ -1011,6 +1020,24 @@ class Engine:
                 C.byref(p), ptr(ws.grid), ptr(ws.spos), ptr(ws.sorted_orig), ws.n, lo, hi, ws.n_conf, ws.n_per_conf,
                 ptr(ws.nbr_cnt), ptr(ws.nbr_list), ws.nbr_cap, ptr(ws.atomic), ws.energies_ptr, grad_ptr, virial_ptr,
                 ptr(ws.member_atomic), grad_members_ptr, idx, len(active), *lat, st))
+
+    def _search_pairs(self, ws: Workspace, lo: int, hi: int, lat: tp.Tuple[tp.Any, ...], grad_ptr: tp.Optional[int],
+                      virial_ptr: tp.Optional[int], grad_members_ptr: tp.Optional[int],
+                      run: tp.Callable[[str, tp.Callable[[], int]], None]) -> None:
+        """Enqueue the LJ / Coulomb pair potentials for atoms [lo, hi): one launch each of
+        ani_b200_pair_potential_search (a neighbour search of the potential's own cutoff over the step's bucket grid,
+        reach cutoff + ``skin``), with the outputs and the ordering rules of ``_pair_potentials``.  A cell thinner than
+        the cutoff + skin raises ANI_STATUS_CELL_TOO_SMALL (``check_status``)."""
+        L = self.lib
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        active = list(self.nets.active)
+        idx = (C.c_int32 * len(active))(*active)
+        fn = L.ani_b200_pair_potential_search_cells if lat else L.ani_b200_pair_potential_search
+        for p in self.search_pairs:
+            run("pair_potential_search", lambda p=p: fn(
+                C.byref(p), ptr(ws.grid), ptr(ws.bin_start), ptr(ws.spos), ptr(ws.sorted_orig), ws.n, lo, hi,
+                ws.n_conf, ws.n_per_conf, self.skin, ptr(ws.atomic), ws.energies_ptr, grad_ptr, virial_ptr,
+                ptr(ws.member_atomic), grad_members_ptr, idx, len(active), ptr(ws.status), *lat, st))
 
     def _dispersion(self, ws: Workspace, lo: int, hi: int, lat: tp.Tuple[tp.Any, ...], grad_ptr: tp.Optional[int],
                     virial_ptr: tp.Optional[int], grad_members_ptr: tp.Optional[int],
@@ -1155,6 +1182,8 @@ class Engine:
             ws.energies_ptr, st), "reduce_energies")
         if self.pairs:   # before the statistics: they read the members' atomic energies and gradients
             self._pair_potentials(ws, 0, n, lat, None, None, gm, run)
+        if self.search_pairs:
+            self._search_pairs(ws, 0, n, lat, None, None, gm, run)
         if self.dispersion is not None:
             self._dispersion(ws, 0, n, lat, None, None, gm, run)
         check(L.ani_b200_ensemble_qbc(

@@ -129,10 +129,11 @@ class ANI(torch.nn.Module):
                  energy_shifter: SelfEnergy, periodic_table_index: bool = True,
                  potentials: tp.Optional[tp.Mapping[str, PairPotential]] = None):
         """``potentials``: pair potentials evaluated next to the networks (arch.py:116-127), e.g.
-        ``{"repulsion_xtb": RepulsionXTB(...)}``.  The repulsion terms run inside the fused step over the AEV's own
-        neighbour list, so each needs ``cutoff <=`` the radial AEV cutoff; a ``TwoBodyDispersionD3`` (at most one, any
-        name, a finite cutoff) runs its own neighbour search over the step's bucket grid.  ``self.cutoff`` is the
-        largest cutoff of the networks and the potentials (arch.py:125)."""
+        ``{"repulsion_xtb": RepulsionXTB(...)}``.  The repulsion terms (xTB, ZBL) run inside the fused step over the
+        AEV's own neighbour list, so each needs ``cutoff <=`` the radial AEV cutoff; the LJ and Coulomb terms run a
+        neighbour search of their own cutoff over the step's bucket grid, at any cutoff (``math.inf``: open systems
+        only); a ``TwoBodyDispersionD3`` (at most one, any name, a finite cutoff) runs its own neighbour search too.
+        ``self.cutoff`` is the largest cutoff of the networks and the potentials (arch.py:125)."""
         super().__init__()
         self.register_buffer("atomic_numbers", torch.tensor([ATOMIC_NUMBER[e] for e in symbols], dtype=torch.long))
         assert len(energy_shifter.self_energies) == len(symbols)
@@ -157,7 +158,7 @@ class ANI(torch.nn.Module):
                 if pot.cutoff == math.inf:
                     raise ValueError(f"potential {name!r}: D3 in a model needs a finite cutoff (its neighbour search "
                                      "runs on the step's bucket grid)")
-            else:
+            elif pot.kind in (0, 1):
                 check_pair_cutoff(pot.cutoff, self.cutoff)
         if n_d3 > 1:
             raise ValueError("a model takes at most one TwoBodyDispersionD3")
@@ -670,12 +671,16 @@ def accelerate_torchani_(ref_model):
     if hasattr(nnp, "charge_networks"):   # SeparateChargesNNPotential: same AEV, forward-only charge networks
         nnp.charge_networks = charge_networks_from_torchani(nnp.charge_networks).to(dev)
     ref_model.neighborlist = aevc.neighborlist
-    # RepulsionXTB / RepulsionZBL / TwoBodyDispersionD3 members run through the CUDA pair-list kernels; any other
-    # potential stays as it is
+    # the pair potentials with a CUDA counterpart run through the CUDA pair-list kernels; any other potential stays as
+    # it is
     for name, pot in list(ref_model.potentials.items()):
-        if name != "nnp" and type(pot).__name__ in ("RepulsionXTB", "RepulsionZBL", "TwoBodyDispersionD3"):
+        if name != "nnp" and type(pot).__name__ in _CONVERTED_POTENTIALS:
             ref_model.potentials[name] = _DropInPairPotential(_potentials.from_torchani(pot).to(dev))
     return ref_model
+
+
+_CONVERTED_POTENTIALS = ("RepulsionXTB", "RepulsionZBL", "LennardJones", "RepulsionLJ", "DispersionLJ", "FixedCoulomb",
+                         "FixedMNOK", "TwoBodyDispersionD3")
 
 
 class _DropInPairPotential(torch.nn.Module):

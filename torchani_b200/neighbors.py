@@ -12,6 +12,7 @@ either: the reference's argsort is unstable); compare as sets.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import typing as tp
 
 import torch
@@ -112,6 +113,8 @@ def effective_periodic_cell(coords: Tensor, cell: tp.Optional[Tensor], pbc: tp.O
     vector is replaced by one along the normal of the other two, long enough (extent of the atoms along it + cutoff +
     1 A) that no pair within the cutoff crosses it.  Same pair set, same shifts along the periodic vectors, zero
     shift along the others.  One host synchronisation (the extent), only in this case."""
+    if pbc is not None and cutoff == math.inf:
+        raise ValueError("PBC can't use an infinite cutoff")
     if pbc is None or cell is None or bool(pbc.all()):
         return cell
     c = cell.detach().to(torch.float64)
@@ -143,6 +146,8 @@ def supercell_for_thin_cell(species: Tensor, coords: Tensor, cell: tp.Optional[T
     (which autograd does by itself through the replication below).  One host sync (the cell widths)."""
     if pbc is None or cell is None:
         return None
+    if cutoff == math.inf:
+        raise ValueError("PBC can't use an infinite cutoff")
     c = cell.detach().to(torch.float64).cpu()
     inv = torch.linalg.inv(c)
     widths = 1.0 / inv.norm(dim=0)          # distance between the lattice planes of direction d

@@ -1,18 +1,22 @@
 """Pair potentials with the interface of ``torchani.potentials`` (potentials/core.py:106-207): the short-range
-repulsion terms ``RepulsionXTB`` (potentials/xtb.py) and ``RepulsionZBL`` (potentials/zbl.py), and the D3(BJ)
-two-body dispersion ``TwoBodyDispersionD3`` (potentials/dftd3.py).
+repulsion terms ``RepulsionXTB`` (potentials/xtb.py) and ``RepulsionZBL`` (potentials/zbl.py), the Lennard-Jones
+terms ``LennardJones``, ``RepulsionLJ`` and ``DispersionLJ`` (potentials/lj.py), the fixed-charge Coulomb terms
+``FixedCoulomb`` and ``FixedMNOK`` (potentials/fixed_coulomb.py), and the D3(BJ) two-body dispersion
+``TwoBodyDispersionD3`` (potentials/dftd3.py).
 
-Inside a model (``models.ANI(..., potentials={...})``) a pair potential is evaluated by the fused step over the
-neighbour list the AEV kernel has just built (``ani_b200_pair_potential``), which is why its cutoff may not exceed the
-radial AEV cutoff.  On its own a module evaluates a half pair list (``compute_from_neighbors``, ``forward``) through
+Inside a model (``models.ANI(..., potentials={...})``) the repulsion terms are evaluated by the fused step over the
+neighbour list the AEV kernel has just built (``ani_b200_pair_potential``), which is why their cutoff may not exceed
+the radial AEV cutoff.  The LJ and Coulomb terms run over a neighbour search of their own cutoff on the step's bucket
+grid (``ani_b200_pair_potential_search``), at any cutoff; without a cutoff (the reference's default) on open systems
+only.  On its own a module evaluates a half pair list (``compute_from_neighbors``, ``forward``) through
 ``ani_b200_pair_potential_pairs``.  CUDA float32 only; there is no CPU path.
 
 D3 has a cutoff beyond Rcr (8 A in the reference's models) and coordination numbers that make it many-body: inside a
 model it runs its own neighbour search over the step's bucket grid (``ani_b200_dispersion_d3``, three launches).
 
-The reference's per-element xTB ``alpha`` / ``yeff`` defaults and its D3 tables (C6 references, covalent radii,
-empirical charges) are not shipped: pass them, or convert a reference module (``from_torchani``), which reads its
-buffers.
+The reference's per-element xTB ``alpha`` / ``yeff`` defaults, its D3 tables (C6 references, covalent radii,
+empirical charges) and its ff19SB LJ table are not shipped; neither are atomic charges or hardnesses for the Coulomb
+terms: pass them, or convert a reference module (``from_torchani``), which reads its buffers.
 """
 from __future__ import annotations
 
@@ -28,6 +32,7 @@ from .neighbors import Neighbors, all_pairs
 from .nn import ATOMIC_NUMBER
 
 ANGSTROM_TO_BOHR = 1.8897261258369282   # units.py:41
+HARTREE_TO_KCALPERMOL = 627.5094738898777   # units.py:51
 _CUTOFF_FNS = {"cosine": 0, "smooth": 1, "dummy": 2}
 
 
@@ -92,6 +97,7 @@ class PairPotential(torch.nn.Module):
     element-pair tables of ``ani_pair_params`` in ``_fill``."""
 
     kind = -1
+    _to_bohr = ANGSTROM_TO_BOHR   # the length unit of the kernel's d (the LJ kinds work in A)
 
     def __init__(self, symbols: tp.Sequence[str], *, cutoff: float = math.inf, cutoff_fn: tp.Any = "smooth"):
         super().__init__()
@@ -117,7 +123,7 @@ class PairPotential(torch.nn.Module):
         p = PairParams()
         p.kind, p.cutoff_fn, p.num_species = self.kind, _CUTOFF_FNS[self.cutoff_fn], len(self.symbols)
         p.cutoff = self.cutoff if self.cutoff != math.inf else 0.0
-        p.to_bohr = ANGSTROM_TO_BOHR
+        p.to_bohr = self._to_bohr
         self._fill(p)
         return p
 
@@ -246,6 +252,101 @@ class RepulsionZBL(PairPotential):
             p.screen_exp[q] = float(self._exponents.view(-1)[q])
 
 
+def _per_symbol(cls_name: str, name: str, seq: tp.Sequence[float], symbols: tp.Sequence[str]) -> Tensor:
+    """One float32 value per symbol (the reference keeps these as float32 buffers, potentials/lj.py:84-88)."""
+    if not len(seq):
+        raise ValueError(f"{cls_name} needs `{name}` (one value per symbol): it has no default in torchani_b200; pass "
+                         "the values or convert a reference module (potentials.from_torchani / models.from_torchani), "
+                         "which reads its buffers")
+    if len(seq) != len(symbols):
+        raise ValueError(f"`{name}` needs one value per symbol")
+    return torch.tensor([float(v) for v in seq], dtype=torch.float32)
+
+
+class _LJ(PairPotential):
+    r"""Lennard-Jones style potentials (potentials/lj.py:60-115): ``eps`` in Hartree and ``sigma`` in Angstrom, one
+    value per symbol, combined by the Berthelot (``sqrt(eps_a eps_b)``) and Lorentz (``(sigma_a + sigma_b) / 2``)
+    rules.  The defaults are the reference's: sigma = 1.5 A and eps = 0.1 kcal/mol for every element."""
+
+    _to_bohr = 1.0
+
+    def __init__(self, symbols: tp.Sequence[str], eps: tp.Sequence[float] = (), sigma: tp.Sequence[float] = (), *,
+                 trainable: tp.Sequence[str] = (), cutoff: float = math.inf, cutoff_fn: tp.Any = "smooth"):
+        super().__init__(symbols, cutoff=cutoff, cutoff_fn=cutoff_fn)
+        if len(trainable):
+            raise ValueError(f"{type(self).__name__}: trainable pair-potential parameters are not supported by the "
+                             "CUDA kernels")
+        name = type(self).__name__
+        S = len(symbols)
+        eps = eps if len(eps) else [0.1 / HARTREE_TO_KCALPERMOL] * S
+        sigma = sigma if len(sigma) else [1.5] * S
+        self.register_buffer("_eps", _per_symbol(name, "eps", eps, symbols), persistent=False)
+        self.register_buffer("_sigma", _per_symbol(name, "sigma", sigma, symbols), persistent=False)
+
+    def _fill(self, p: PairParams) -> None:
+        eps = self._eps.detach().to("cpu", torch.float64)
+        sigma = self._sigma.detach().to("cpu", torch.float64)
+        self._table(p.a, torch.outer(eps, eps).sqrt())
+        self._table(p.b, (sigma.view(-1, 1) + sigma.view(1, -1)) / 2)
+
+
+class LennardJones(_LJ):
+    r"""``E = 4 eps_ab (x^12 - x^6)``, ``x = sigma_ab / max(R, 1e-7)`` (potentials/lj.py:138-145)."""
+
+    kind = 2
+
+
+class RepulsionLJ(_LJ):
+    r"""``E = 4 eps_ab x^12`` (potentials/lj.py:128-135)."""
+
+    kind = 3
+
+
+class DispersionLJ(_LJ):
+    r"""``E = -4 eps_ab x^6`` (potentials/lj.py:118-125)."""
+
+    kind = 4
+
+
+class FixedCoulomb(PairPotential):
+    r"""Coulomb energy of fixed per-element charges (potentials/fixed_coulomb.py:13-38):
+    ``E = q_a q_b / (dielectric * max(R, 1e-7) * to_bohr)``.  ``charges`` (e, one value per symbol) are required."""
+
+    kind = 5
+
+    def __init__(self, symbols: tp.Sequence[str], dielectric: float = 1.0, charges: tp.Sequence[float] = (), *,
+                 cutoff: float = math.inf, cutoff_fn: tp.Any = "smooth"):
+        super().__init__(symbols, cutoff=cutoff, cutoff_fn=cutoff_fn)
+        self._dielectric = float(dielectric)
+        self.register_buffer("_charges", _per_symbol("FixedCoulomb", "charges", charges, symbols), persistent=False)
+
+    def _fill(self, p: PairParams) -> None:
+        q = self._charges.detach().to("cpu", torch.float64)
+        self._table(p.a, torch.outer(q, q) / self._dielectric)
+
+
+class FixedMNOK(PairPotential):
+    r"""Mataga-Nishimoto-Ohno-Klopman screened Coulomb energy of fixed per-element charges
+    (potentials/fixed_coulomb.py:49-81): ``E = q_a q_b / sqrt((R to_bohr)^2 + (2 / (eta_a + eta_b))^2)``, R not
+    clamped.  As in the reference, ``dielectric`` is stored but does not enter the energy.  ``charges`` and ``eta`` (one
+    value per symbol) are required."""
+
+    kind = 6
+
+    def __init__(self, symbols: tp.Sequence[str], dielectric: float = 1.0, charges: tp.Sequence[float] = (),
+                 eta: tp.Sequence[float] = (), *, cutoff: float = math.inf, cutoff_fn: tp.Any = "smooth"):
+        super().__init__(symbols, cutoff=cutoff, cutoff_fn=cutoff_fn)
+        self._dielectric = float(dielectric)
+        self.register_buffer("_charges", _per_symbol("FixedMNOK", "charges", charges, symbols), persistent=False)
+        self.register_buffer("_eta", _per_symbol("FixedMNOK", "eta", eta, symbols), persistent=False)
+
+    def _fill(self, p: PairParams) -> None:
+        q = self._charges.detach().to("cpu", torch.float64)
+        eta = self._eta.detach().to("cpu", torch.float64)
+        self._table(p.a, torch.outer(q, q))
+        self._table(p.b, 2 / (eta.view(-1, 1) + eta.view(1, -1)))
+
+
 class _BeckeJohnsonDamp(torch.nn.Module):
     """Holds the damping radii of D3(BJ) under the reference's state-dict key ``_damp_fn.cutoff_radii``
     (potentials/dftd3.py:45-110): ``cutoff_radii = sqrt(3 outer(sqrt_q, sqrt_q))`` in Bohr, and ``_a1``, ``_a2``."""
@@ -267,8 +368,6 @@ class TwoBodyDispersionD3(PairPotential):
     5)``, -1 where a reference is missing.  None of them is shipped: pass them, or convert a reference module
     (``potentials.from_torchani``), or pass the buffers of a reference state dict (the keys are the reference's,
     ``load_state_dict`` accepts its legacy ``_damp_fn_6`` / ``_damp_fn_8`` keys)."""
-
-    kind = 2
 
     def __init__(self, symbols: tp.Sequence[str], s6: float, s8: float, damp_a1: float, damp_a2: float,
                  sqrt_empirical_charge: tp.Sequence[float] = (), covalent_radii: tp.Sequence[float] = (), *,
@@ -372,14 +471,35 @@ class TwoBodyDispersionD3(PairPotential):
         return launch
 
 
+def _buffer_values(ref_pot, key: str) -> tp.List[float]:
+    """A per-element buffer of a reference module; trainable parameters are refused (not supported by the kernels)."""
+    v = getattr(ref_pot, key)
+    if isinstance(v, torch.nn.Parameter):
+        raise ValueError(f"{type(ref_pot).__name__}: trainable pair-potential parameters ({key}) are not supported by "
+                         "the CUDA kernels")
+    return [float(x) for x in v.detach().to("cpu", torch.float32).tolist()]
+
+
 def from_torchani(ref_pot) -> PairPotential:
-    """A reference ``RepulsionXTB`` / ``RepulsionZBL`` / ``TwoBodyDispersionD3`` module -> the CUDA module with the
-    same parameters (read from the module's buffers).  Any other potential raises ``ValueError``."""
+    """A reference ``RepulsionXTB`` / ``RepulsionZBL`` / ``LennardJones`` / ``RepulsionLJ`` / ``DispersionLJ`` /
+    ``FixedCoulomb`` / ``FixedMNOK`` / ``TwoBodyDispersionD3`` module -> the CUDA module with the same parameters (read
+    from the module's buffers).  Any other potential raises ``ValueError``."""
     name = type(ref_pot).__name__
     symbols = tuple(ref_pot.symbols)
     cutoff_fn = ref_pot.cutoff_fn
-    if name == "RepulsionXTB":
-        out: PairPotential = RepulsionXTB(symbols, alpha=[1.0] * len(symbols), yeff=[1.0] * len(symbols),
+    lj = {"LennardJones": LennardJones, "RepulsionLJ": RepulsionLJ, "DispersionLJ": DispersionLJ}
+    if name in lj:
+        out: PairPotential = lj[name](symbols, eps=_buffer_values(ref_pot, "_eps"),
+                                      sigma=_buffer_values(ref_pot, "_sigma"), cutoff=ref_pot.cutoff,
+                                      cutoff_fn=cutoff_fn)
+    elif name == "FixedCoulomb":
+        out = FixedCoulomb(symbols, float(ref_pot._dielectric), _buffer_values(ref_pot, "_charges"),
+                           cutoff=ref_pot.cutoff, cutoff_fn=cutoff_fn)
+    elif name == "FixedMNOK":
+        out = FixedMNOK(symbols, float(ref_pot._dielectric), _buffer_values(ref_pot, "_charges"),
+                        _buffer_values(ref_pot, "_eta"), cutoff=ref_pot.cutoff, cutoff_fn=cutoff_fn)
+    elif name == "RepulsionXTB":
+        out = RepulsionXTB(symbols, alpha=[1.0] * len(symbols), yeff=[1.0] * len(symbols),
                                           cutoff=ref_pot.cutoff, cutoff_fn=cutoff_fn)
         for key in ("y_ab", "sqrt_alpha_ab", "k_rep_ab"):
             getattr(out, key).copy_(getattr(ref_pot, key).detach().to("cpu", torch.float32))
@@ -404,7 +524,7 @@ def from_torchani(ref_pot) -> PairPotential:
         out._damp_fn.cutoff_radii.copy_(damp.cutoff_radii.detach().to("cpu", torch.float32))
         out._k1, out._k2, out._k3 = ref_pot._k1, ref_pot._k2, ref_pot._k3
     else:
-        raise ValueError(f"potential {name} has no CUDA counterpart (RepulsionXTB, RepulsionZBL and "
-                         "TwoBodyDispersionD3 do)")
+        raise ValueError(f"potential {name} has no CUDA counterpart (RepulsionXTB, RepulsionZBL, LennardJones, "
+                         "RepulsionLJ, DispersionLJ, FixedCoulomb, FixedMNOK and TwoBodyDispersionD3 do)")
     out._enabled = bool(ref_pot._enabled)
     return out
