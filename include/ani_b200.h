@@ -720,6 +720,64 @@ int ani_b200_comm_buffers(void* comm, float** partial_f32, double** partial_f64,
 int ani_b200_comm_allreduce(void* comm, float* out_f32, double* out_f64, void* stream);
 int ani_b200_comm_destroy(void* comm);
 
+/* 9. Analytic Hessians of open systems (csrc/hessian.cu), after a step with gradients (grid mode 0 or 1, one rank):  */
+/*    they read what it left behind -- sorted positions, nbr_cnt / nbr_list, row_of, sorted_orig, the tiled AEVs x and */
+/*    the member-weighted dE/dAEV rows dx -- and change none of it.  Per central atom i with n_i = min(nbr_cnt, cap)   */
+/*    neighbour words, one block B_i (f32, 3 n_i x 3 n_i, row / column 3 n + c = component c of r_n - r_i of          */
+/*    neighbour n) collects the second derivatives of i's energy terms with respect to those relative vectors:        */
+/*      ani_b200_hessian_jacobian   the AEV Jacobian rows J_i (row 3 n + c = dA_i / d(r_n - r_i)_c, f32[ldx] in the     */
+/*                                  internal column order of x / dx; the chunk's rows are zeroed first)              */
+/*      ani_b200_hessian_network    B_i += J_i^T K_i J_i, K_i = sum over the members with member_scale[m] != 0 of      */
+/*                                  member_scale[m] times the network Hessian at A_i: one fp32 primal pass per         */
+/*                                  (atom, member), five tangent GEMMs over the rows and Zdot1 Deltadot1^T per atom.  */
+/*                                  scratch: 4 rows hmax + n_slots 5 hmax floats, hmax = ani_b200_hessian_hidden_max  */
+/*      ani_b200_hessian_geometric  with dx (pair_dev NULL): the Hessian of dx_i . A_i with dx_i held fixed; with a     */
+/*                                  DEVICE copy of one ani_pair_params of kind 0 or 1 (dx NULL): the Hessian of its    */
+/*                                  1/2 E(R) fc(R) per neighbour word within its cutoff                              */
+/*      ani_b200_hessian_assemble   hess[conf][3 A][3 A] (f64, input atom order, accumulated; the caller zeroes it)    */
+/*                                  += B_i mapped onto atoms {i} u nbrs(i): (j, k) += B, (i, k) and (j, i) -= the     */
+/*                                  sums over j / k, (i, i) += the sum of B                                          */
+/*    A chunk is a set of central atoms ("slots") processed together (device arrays):                                 */
+/*      atom[n_slots]        sorted index of each slot's atom                                                         */
+/*      row_off[n_slots]     first Jacobian row of the slot (3 n_i rows); slots of one species are contiguous and     */
+/*                           every species segment starts at a multiple of ANI_HESSIAN_ROW_ALIGN                     */
+/*      block_off[n_slots]   first float of B_i in `blocks`                                                          */
+/*      row_slot[rows]       slot of each row, -1 for the rows between the segments                                   */
+/*      tile_species[rows / ANI_HESSIAN_ROW_ALIGN]  species of each row tile                                           */
+/*      rows                 multiple of ANI_HESSIAN_ROW_ALIGN;  max_count: largest n_i of the chunk                    */
+/*    `blocks` must be zeroed before the network and geometric calls of a chunk, which add into it.                   */
+#define ANI_HESSIAN_ROW_ALIGN 64
+typedef struct ani_hessian_chunk {
+  const int32_t* atom;
+  const int32_t* row_off;
+  const long long* block_off;
+  const int32_t* row_slot;
+  const int32_t* tile_species;
+  int32_t n_slots, rows, max_count, pad_;
+} ani_hessian_chunk;
+/*    Plain fp32 weights of every member, per species, in the padded widths of ani_mlp_species (h1, h2, h3):        */
+/*      w1 [M][h1][ldx] (internal column order), w2 [M][h2][h1], w3 [M][h3][h2]; biases and w4 from ani_mlp_species.  */
+typedef struct ani_hessian_weights {
+  const float* w1[ANI_MAX_SPECIES];
+  const float* w2[ANI_MAX_SPECIES];
+  const float* w3[ANI_MAX_SPECIES];
+} ani_hessian_weights;
+int ani_b200_hessian_hidden_max(const ani_mlp_model* model);
+int ani_b200_hessian_jacobian(const ani_aev_params* params, const float* spos, const int32_t* nbr_cnt,
+                              const int32_t* nbr_list, int cap, const ani_hessian_chunk* chunk, float* jac, int ldx,
+                              void* stream);
+int ani_b200_hessian_network(const ani_mlp_model* model, const ani_hessian_weights* weights, const void* x,
+                             const int32_t* row_of, const float* spos, const int32_t* nbr_cnt, int cap,
+                             const ani_hessian_chunk* chunk, const float* jac, float* scratch, float* blocks,
+                             void* stream);
+int ani_b200_hessian_geometric(const ani_aev_params* params, const float* spos, const int32_t* nbr_cnt,
+                               const int32_t* nbr_list, int cap, const int32_t* row_of, const float* dx, int ldx,
+                               const ani_pair_params* pair_dev, const ani_hessian_chunk* chunk, float* blocks,
+                               void* stream);
+int ani_b200_hessian_assemble(const int32_t* nbr_cnt, const int32_t* nbr_list, int cap, const int32_t* sorted_orig,
+                              const ani_hessian_chunk* chunk, const float* blocks, int n_per_conf, double* hess,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -81,6 +81,22 @@ class PairParams(C.Structure):
     ]
 
 
+ANI_HESSIAN_ROW_ALIGN = 64
+
+
+class HessianChunk(C.Structure):
+    _fields_ = [
+        ("atom", C.c_void_p), ("row_off", C.c_void_p), ("block_off", C.c_void_p), ("row_slot", C.c_void_p),
+        ("tile_species", C.c_void_p), ("n_slots", C.c_int32), ("rows", C.c_int32), ("max_count", C.c_int32),
+        ("pad_", C.c_int32),
+    ]
+
+
+class HessianWeights(C.Structure):
+    _fields_ = [("w1", C.c_void_p * ANI_MAX_SPECIES), ("w2", C.c_void_p * ANI_MAX_SPECIES),
+                ("w3", C.c_void_p * ANI_MAX_SPECIES)]
+
+
 class D3Params(C.Structure):
     _fields_ = [
         ("cutoff_fn", C.c_int32), ("num_species", C.c_int32), ("cutoff", C.c_float), ("to_bohr", C.c_float),
@@ -159,6 +175,11 @@ _PROTOTYPES = {
     "ani_b200_active_aev_blocks": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "ani_b200_reduce_energies": (C.c_int, [_P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     "ani_b200_charges": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _P, _I, _I, _I, C.c_double, _P, _I, _P, _P, _P]),
+    "ani_b200_hessian_hidden_max": (C.c_int, [_P]),
+    "ani_b200_hessian_jacobian": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _I, _P]),
+    "ani_b200_hessian_network": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P]),
+    "ani_b200_hessian_geometric": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P]),
+    "ani_b200_hessian_assemble": (C.c_int, [_P, _P, _I, _P, _P, _P, _I, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)
@@ -240,6 +261,19 @@ def check(rc: int, what: str = "") -> None:
         if rc == -3:
             msg += " -- " + l.ani_b200_last_cuda_error().decode()
         raise ANIB200Error(f"{what}: {msg}" if what else msg)
+
+
+def forbid_create_graph(what: str) -> None:
+    """Raise when a custom autograd Function's backward runs under ``create_graph=True`` (grad mode is on inside a
+    backward only then): its gradient has no graph of its own, so a second derivative taken through it would silently
+    miss its term.  Called first in those backwards."""
+    import torch
+    if torch.is_grad_enabled():
+        raise NotImplementedError(
+            f"second derivatives through {what} are not supported (its backward has no graph of its own); for "
+            "Hessians convert the model with torchani_b200.models.from_torchani and use ANI.energies_forces_hessians "
+            "or torchani_b200.grad, which differentiate the fused step analytically (open systems, no D3, no LJ or "
+            "Coulomb terms, no external neighbour lists)")
 
 
 def ptr(t) -> int:

@@ -115,6 +115,7 @@ class _AEVFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_aev: Tensor):
+        _lib.forbid_create_graph("the CUDA AEV computer (_AEVFunction)")
         g, computer = ctx.g, ctx.computer
         consts = computer.constants
         grad_aev = grad_aev.reshape(g.n, consts.out_dim).to(torch.float32).contiguous()
@@ -170,6 +171,7 @@ class _AEVFromNeighbors(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_aev: Tensor):
+        _lib.forbid_create_graph("the CUDA AEV computer with a caller-supplied neighbour list (_AEVFromNeighbors)")
         grid, spos, ident, row_start, row_j, row_d, status = ctx.saved
         computer = ctx.computer
         consts = computer.constants
@@ -228,6 +230,7 @@ class _AEVFromFullList(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_aev: Tensor):
+        _lib.forbid_create_graph("the CUDA AEV computer with a full neighbour list (_AEVFromFullList)")
         grid, spos, ident, row_start, row_j, row_d, status = ctx.saved
         computer, n = ctx.computer, ctx.n
         consts = computer.constants

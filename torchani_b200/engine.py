@@ -350,6 +350,14 @@ class PackedNetworks:
         mdl.b1_compact = b1c.data_ptr()
         self._keep = [src, dst, b1c]
         self._plan = plan
+        # the plain fp32 weights next to the tiled operands (W1 in the internal column order), which the Hessian's
+        # tangent network pass reads (Engine.hessian)
+        self.plain_weights = _lib.HessianWeights()
+        for s in range(S):
+            q = plan[s]
+            self.plain_weights.w1[s] = sp0 + 4 * q["s_w1"]
+            self.plain_weights.w2[s] = sp0 + 4 * q["s_w2"]
+            self.plain_weights.w3[s] = sp0 + 4 * q["s_w3"]
         mdl.h1_max = max(q["p"][0] for q in plan)
         mdl.h2_max = max(q["p"][1] for q in plan)
         mdl.h3_max = max(q["p"][2] for q in plan)
@@ -537,6 +545,77 @@ def check_pair_cutoff(cutoff: float, rcr: float) -> None:
                          f"{cutoff}: it is evaluated over the AEV's neighbour list, which holds nothing beyond it")
 
 
+# Jacobian rows (3 per neighbour word) of one chunk of central atoms in Engine.hessian: at ldx = 1024 and ANI-2x widths,
+# 32 768 rows take about 130 MB of Jacobian and 130 MB of tangent scratch
+HESSIAN_ROW_BUDGET = 32768
+
+
+class _HessianPlan(tp.NamedTuple):
+    """One chunk of central atoms of Engine.hessian, in the layout of ani_hessian_chunk (include/ani_b200.h
+    section 9)."""
+    atom: np.ndarray          # i32 [n_slots] sorted index
+    row_off: np.ndarray       # i32 [n_slots]
+    row_slot: np.ndarray      # i32 [rows]
+    tile_species: np.ndarray  # i32 [rows / ANI_HESSIAN_ROW_ALIGN]
+    block_off: np.ndarray     # i64 [n_slots]
+    rows: int
+    block_floats: int
+    max_count: int
+
+
+def _hessian_chunks(cnt: np.ndarray, species: np.ndarray, row_budget: int) -> tp.Iterator[_HessianPlan]:
+    """Split the real sorted atoms (neighbour counts ``cnt``, element indices ``species``) into chunks whose Jacobian
+    rows, species segments aligned to ANI_HESSIAN_ROW_ALIGN, fit ``row_budget`` (a chunk holds at least one atom)."""
+    align = _lib.ANI_HESSIAN_ROW_ALIGN
+    if row_budget < align:
+        raise ValueError(f"row_budget must be at least {align}")
+    up = lambda v: (v + align - 1) // align * align  # noqa: E731
+    order = np.argsort(species, kind="stable")
+    chunk: tp.List[int] = []
+    seg: tp.Dict[int, int] = {}
+
+    def plan(atoms: tp.List[int]) -> _HessianPlan:
+        atom = np.asarray(atoms, dtype=np.int32)   # species-major (``order``)
+        row_off = np.zeros(len(atom), dtype=np.int32)
+        block_off = np.zeros(len(atom), dtype=np.int64)
+        slots, tiles = [], []
+        r, b, prev = 0, 0, None
+        for k, a in enumerate(atom):
+            s = int(species[a])
+            if s != prev and prev is not None:
+                pad = up(r) - r
+                slots.append(np.full(pad, -1, dtype=np.int32))
+                r += pad
+            if s != prev:
+                tiles.append((r // align, s))
+            prev = s
+            row_off[k], block_off[k] = r, b
+            m3 = 3 * int(cnt[a])
+            slots.append(np.full(m3, k, dtype=np.int32))
+            r += m3
+            b += m3 * m3
+        pad = up(max(r, 1)) - r
+        slots.append(np.full(pad, -1, dtype=np.int32))
+        rows = r + pad
+        tile_species = np.zeros(rows // align, dtype=np.int32)
+        for t0, s in tiles:
+            tile_species[t0:] = s
+        return _HessianPlan(atom, row_off, np.concatenate(slots), tile_species, block_off, rows, max(b, 1),
+                            int(cnt[atom].max()))
+
+    for a in order:
+        s, m3 = int(species[a]), 3 * int(cnt[a])
+        grown = dict(seg)
+        grown[s] = grown.get(s, 0) + m3
+        if chunk and sum(up(v) for v in grown.values()) > row_budget:
+            yield plan(chunk)
+            chunk, grown = [], {s: m3}
+        chunk.append(int(a))
+        seg = grown
+    if chunk:
+        yield plan(chunk)
+
+
 class StepResult(tp.NamedTuple):
     energies: Tensor          # (C,) float64: NN energy + self energies of the owned atoms
     atomic_energies: Tensor   # (C, A) float32: NN atomic energies (ensemble mean), 0 for padding
@@ -664,6 +743,7 @@ class Engine:
         self._side_stream: tp.Optional[torch.cuda.Stream] = None
         self._ev: tp.List[torch.cuda.Event] = []
         self.stage_events: tp.Dict[str, tp.List[tp.Tuple[torch.cuda.Event, torch.cuda.Event]]] = {}
+        self.hessian_count = 0   # Hessians computed by this engine (``hessian``)
 
     def _timed(self, name: str, fn: tp.Callable[[], int]) -> None:
         """Run one C-ABI stage; with ``profile`` on, bracket it with events on the launch stream."""
@@ -833,6 +913,8 @@ class Engine:
             self.launches_per_step += 3 if (want_grad or members) else 2
         if charges:
             self.launches_per_step += self._charge_launches(ws)
+        # what the workspace now holds, for Engine.hessian: (periodic, dE/dAEV rows written, sharded)
+        ws.last_run = (bool(pbc), bool(want_grad) and not members, (lo, hi) != (0, n) or ws.reducer is not None)
         grad = ws.grad.view(n_conf, n_per_conf, 3) if want_grad else None
         virial = None
         if want_virial:
@@ -1209,6 +1291,91 @@ class Engine:
         self.run(ws, bool(pbc), True, members=True, conformer_cells=per_conf)
         r = self.members_result(ws)
         return r.energies.clone(), r.grad.clone()
+
+    # -- analytic Hessians ------------------------------------------------------------------------
+    def hessian(self, ws: Workspace, row_budget: int = HESSIAN_ROW_BUDGET) -> Tensor:
+        """(C, 3A, 3A) float32 Hessian d^2E/dx^2 of the energies of the last ``run(ws, pbc=False, want_grad=True)`` on
+        ``ws`` (an open single molecule or conformer batch, unsharded), in input atom order, accumulated in float64;
+        padding atoms get zero rows and columns, conformers are independent blocks.  It reads what that step left in the
+        workspace (neighbour words, AEVs, dE/dAEV rows) and runs as eager launches of csrc/hessian.cu, per chunk of
+        central atoms whose Jacobian rows (3 per neighbour) fit ``row_budget``: AEV Jacobian rows, the tangent network
+        pass of every active member, the geometric and xTB / ZBL terms, and the assembly.  Synchronises once to plan the
+        chunks."""
+        last = getattr(ws, "last_run", None)
+        if last is None:
+            raise ValueError("Engine.hessian needs a step with gradients on this workspace first: "
+                             "run(ws, pbc=False, want_grad=True)")
+        periodic, have_dx, sharded = last
+        if periodic:
+            raise ValueError("Hessians of periodic systems are not supported (open molecules and conformer batches "
+                             "only)")
+        if sharded:
+            raise ValueError("Hessians are computed on one unsharded engine: every atom's neighbour words and dE/dAEV "
+                             "row are needed")
+        if not have_dx:
+            raise ValueError("Engine.hessian needs the dE/dAEV rows of an ordinary step with gradients "
+                             "(run(ws, pbc=False, want_grad=True))")
+        if self.dispersion is not None:
+            raise NotImplementedError("Hessians of models with D3 dispersion are not supported")
+        if self.search_pairs:
+            raise NotImplementedError("Hessians of models with Lennard-Jones or Coulomb pair potentials (kinds 2-6) "
+                                      "are not supported; only the xTB and ZBL repulsion terms have second "
+                                      "derivatives")
+        L, nets = self.lib, self.nets
+        dev = self.device
+        n_conf, A = ws.n_conf, ws.n_per_conf
+        with torch.cuda.device(dev):
+            st = torch.cuda.current_stream(dev).cuda_stream
+            n_real = int(self.grid_info(ws).n_real)
+            cnt = ws.nbr_cnt[:n_real].clamp(max=ws.nbr_cap).cpu().numpy().astype(np.int64)
+            species = ws.spos[:n_real, 3].contiguous().view(torch.int32).cpu().numpy()
+            hess = torch.zeros(n_conf, 3 * A, 3 * A, dtype=torch.float64, device=dev)
+            hmax = L.ani_b200_hessian_hidden_max(C.byref(nets.model))
+            pairs = [torch.frombuffer(bytearray(bytes(p)), dtype=torch.uint8).to(dev) for p in self.pairs]
+            for chunk in _hessian_chunks(cnt, species, int(row_budget)):
+                self._hessian_chunk(ws, chunk, hmax, pairs, hess, st)
+        self.hessian_count += 1
+        return hess.to(torch.float32)
+
+    def hessian_chunk_args(self, plan: "_HessianPlan") -> tp.Tuple[_lib.HessianChunk, tp.List[Tensor]]:
+        """The ani_hessian_chunk of ``plan`` and the device arrays it points into (keep them alive while it is used)."""
+        dev = self.device
+        i32 = torch.from_numpy(np.concatenate([plan.atom, plan.row_off, plan.row_slot, plan.tile_species])).to(dev)
+        b_off = torch.from_numpy(plan.block_off).to(dev)
+        ns, rows = len(plan.atom), plan.rows
+        ch = _lib.HessianChunk()
+        ch.atom, ch.row_off = i32.data_ptr(), i32.data_ptr() + 4 * ns
+        ch.row_slot, ch.tile_species = i32.data_ptr() + 8 * ns, i32.data_ptr() + 4 * (2 * ns + rows)
+        ch.block_off = b_off.data_ptr()
+        ch.n_slots, ch.rows, ch.max_count = ns, rows, plan.max_count
+        return ch, [i32, b_off]
+
+    def _hessian_chunk(self, ws: Workspace, plan: "_HessianPlan", hmax: int, pairs: tp.List[Tensor], hess: Tensor,
+                       st: int) -> None:
+        """Enqueue the four stages of one chunk of central atoms (see ``hessian``)."""
+        L, nets, dev = self.lib, self.nets, self.device
+        ch, _keep = self.hessian_chunk_args(plan)
+        ns, rows = len(plan.atom), plan.rows
+        jac = torch.empty(rows, nets.ldx, dtype=torch.float32, device=dev)
+        scratch = torch.empty(4 * rows * hmax + ns * 5 * hmax, dtype=torch.float32, device=dev)
+        blocks = torch.zeros(plan.block_floats, dtype=torch.float32, device=dev)
+        cap = ws.nbr_cap
+        self._timed("hessian_jacobian", lambda: L.ani_b200_hessian_jacobian(
+            C.byref(self.params), ptr(ws.spos), ptr(ws.nbr_cnt), ptr(ws.nbr_list), cap, C.byref(ch), ptr(jac),
+            nets.ldx, st))
+        self._timed("hessian_network", lambda: L.ani_b200_hessian_network(
+            C.byref(nets.model), C.byref(nets.plain_weights), ptr(ws.x), ptr(ws.row_of), ptr(ws.spos), ptr(ws.nbr_cnt),
+            cap, C.byref(ch), ptr(jac), ptr(scratch), ptr(blocks), st))
+        self._timed("hessian_geometric", lambda: L.ani_b200_hessian_geometric(
+            C.byref(self.params), ptr(ws.spos), ptr(ws.nbr_cnt), ptr(ws.nbr_list), cap, ptr(ws.row_of), ptr(ws.dx),
+            nets.ldx, None, C.byref(ch), ptr(blocks), st))
+        for p in pairs:
+            self._timed("hessian_geometric", lambda p=p: L.ani_b200_hessian_geometric(
+                C.byref(self.params), ptr(ws.spos), ptr(ws.nbr_cnt), ptr(ws.nbr_list), cap, None, None, 0, ptr(p),
+                C.byref(ch), ptr(blocks), st))
+        self._timed("hessian_assemble", lambda: L.ani_b200_hessian_assemble(
+            ptr(ws.nbr_cnt), ptr(ws.nbr_list), cap, ptr(ws.sorted_orig), C.byref(ch), ptr(blocks), ws.n_per_conf,
+            ptr(hess), st))
 
     def _use_dataflow_mlp(self, owned: int) -> bool:
         """One data-flow launch (True) or six chained launches (False) for `owned` atoms; see __init__."""

@@ -91,7 +91,11 @@ class SelfEnergy(torch.nn.Module):
 
 class _FusedEnergy(torch.autograd.Function):
     """coords -> (energies (C,), atomic NN energies (C, A), member atomic (M, C, A)); the
-    gradient of the ensemble-mean energy is produced by the forward launch sequence."""
+    gradient of the ensemble-mean energy is produced by the forward launch sequence.
+
+    Under ``create_graph=True`` the backward returns that gradient through ``_HessianProduct``: it re-runs the step on
+    the saved coordinates (the workspace may have been reused since the forward), computes the analytic Hessian once
+    (``Engine.hessian``) and differentiates the gradient as the product with it."""
 
     @staticmethod
     def forward(ctx, coords: Tensor, species: Tensor, cell: tp.Optional[Tensor], pbc: bool, engine: Engine,
@@ -99,7 +103,8 @@ class _FusedEnergy(torch.autograd.Function):
         res: StepResult = engine.step(species, coords.detach(), cell, pbc, want_grad=want_grad, check=True)
         ctx.want_grad = want_grad
         if want_grad:
-            ctx.save_for_backward(res.grad.clone())
+            ctx.save_for_backward(res.grad.clone(), coords)
+            ctx.step_args = (species, cell, pbc, engine)
         ctx.mark_non_differentiable(res.member_atomic)
         return res.energies.clone(), res.atomic_energies.clone(), res.member_atomic.clone()
 
@@ -107,14 +112,48 @@ class _FusedEnergy(torch.autograd.Function):
     def backward(ctx, g_energy, g_atomic, g_member):
         if not ctx.want_grad:
             raise RuntimeError("energies were computed without forces (coords.requires_grad was False)")
-        (grad,) = ctx.saved_tensors
-        out = None
-        if g_energy is not None:
-            out = grad * g_energy.to(grad.dtype).view(-1, 1, 1)
+        grad, coords = ctx.saved_tensors
         if g_atomic is not None and bool((g_atomic != 0).any()):
             raise NotImplementedError("per-atom upstream gradients are not supported by the fused engine; "
                                       "use AEVComputer + Ensemble modules directly")
-        return out, None, None, None, None, None
+        if g_energy is None:
+            return None, None, None, None, None, None
+        if torch.is_grad_enabled():   # create_graph=True: a gradient that can be differentiated again
+            species, cell, pbc, engine = ctx.step_args
+            hess = _step_hessian(engine, species, coords, cell, pbc)
+            return _HessianProduct.apply(coords, g_energy, grad, hess), None, None, None, None, None
+        return grad * g_energy.to(grad.dtype).view(-1, 1, 1), None, None, None, None, None
+
+
+def _step_hessian(engine: Engine, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor], pbc: bool) -> Tensor:
+    """(C, 3A, 3A) float32 Hessian of one step on ``coords`` (eager launches; open systems only)."""
+    if pbc:
+        raise ValueError("Hessians of periodic systems are not supported (open molecules and conformer batches only)")
+    engine.step(species, coords.detach(), cell, False, want_grad=True, check=True)
+    return engine.hessian(engine.workspace(*species.shape))
+
+
+class _HessianProduct(torch.autograd.Function):
+    """(coords, g_energy) -> g_energy * dE/dcoords with the step's gradient and Hessian precomputed: the backward is
+    the batched product with the Hessian (one per conformer), so every component of a Hessian taken through autograd
+    reuses the one Hessian computation of the step."""
+
+    @staticmethod
+    def forward(ctx, coords: Tensor, g_energy: Tensor, grad: Tensor, hess: Tensor):
+        ctx.save_for_backward(g_energy, grad, hess)
+        ctx.coords_dtype = coords.dtype
+        return grad * g_energy.to(grad.dtype).view(-1, 1, 1)
+
+    @staticmethod
+    def backward(ctx, v: Tensor):
+        if torch.is_grad_enabled():
+            raise NotImplementedError("third derivatives of the fused step are not supported")
+        g_energy, grad, hess = ctx.saved_tensors
+        n_conf = v.shape[0]
+        hv = torch.bmm(hess, v.reshape(n_conf, -1, 1).to(hess.dtype)).view_as(v)
+        d_coords = hv * g_energy.to(hv.dtype).view(-1, 1, 1)
+        d_g = (grad.to(v.dtype) * v).sum((1, 2)).to(g_energy.dtype)
+        return d_coords.to(ctx.coords_dtype), d_g, None, None
 
 
 def _per_conformer(cell: tp.Optional[Tensor]) -> bool:
@@ -445,6 +484,22 @@ class ANI(torch.nn.Module):
             elem_idxs, coords.detach(), cell, pbc is not None, want_grad=True, check=True))
         return res.energies.clone(), -res.grad
 
+    def energies_forces_hessians(self, species: Tensor, coords: Tensor) -> tp.Tuple[Tensor, Tensor, Tensor]:
+        """(energies f64 (C,), forces f32 (C, A, 3), Hessians d^2E/dx^2 f32 (C, 3A, 3A)) of open molecules or conformer
+        batches (grad.py:239-260 without the autograd round trip): one step with gradients and its analytic Hessian
+        (``Engine.hessian``).  Padding atoms get zero rows and columns.  Periodic input, D3, Lennard-Jones and Coulomb
+        terms are not supported; the xTB and ZBL repulsion terms are included.  A charge model gives the Hessian of its
+        energy (the charges are not differentiated)."""
+        elem_idxs = self.species_converter(species, nop=not self.periodic_table_index)
+        _validate_inputs(self.cutoff, elem_idxs, coords, None, None)
+
+        def run():
+            eng = self.engine(coords.device)
+            res = eng.step(elem_idxs, coords.detach(), None, False, want_grad=True, check=True)
+            e, f = res.energies.clone(), -res.grad
+            return e, f, eng.hessian(eng.workspace(*elem_idxs.shape))
+        return self._guarded(run)
+
     def energies_forces_stress(self, species: Tensor, coords: Tensor, cell: Tensor,
                                pbc: tp.Optional[Tensor] = None) -> tp.Tuple[Tensor, Tensor, Tensor]:
         """(energies f64 (C,), forces f32 (C, A, 3), stress f64 in Hartree/A^3) of periodic systems in one cell: (3, 3)
@@ -737,14 +792,15 @@ class _FusedEnergyCharges(torch.autograd.Function):
         ws = engine.workspace(*species.shape)
         q = engine.charges_result(ws)
         ctx.want_grad = want_grad
-        if want_grad:
-            ctx.save_for_backward(res.grad.clone())
+        if want_grad:   # (what _FusedEnergy.backward reads)
+            ctx.save_for_backward(res.grad.clone(), coords)
         ctx.mark_non_differentiable(res.member_atomic)
         return (res.energies.clone(), res.atomic_energies.clone(), res.member_atomic.clone(), q.charges.clone(),
                 q.dipoles.clone())
 
     @staticmethod
     def backward(ctx, g_energy, g_atomic, g_member, g_charges, g_dipoles):
+        _lib.forbid_create_graph("the fused step with charges (_FusedEnergyCharges)")
         for g in (g_charges, g_dipoles):
             if g is not None and bool((g != 0).any()):
                 raise NotImplementedError("gradients of atomic charges and dipoles are not computed by the fused "

@@ -162,6 +162,7 @@ class _MLPFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out: Tensor):
+        _lib.forbid_create_graph("the CUDA atomic networks (_MLPFunction)")
         if not ctx.want_grad:
             raise RuntimeError("this evaluation was run without the backward-to-input pass")
         (g,) = ctx.saved_tensors

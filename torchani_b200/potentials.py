@@ -79,6 +79,7 @@ class _HalfListEnergy(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_energy, g_atomic):
+        _lib.forbid_create_graph("the CUDA pair potentials over a half neighbour list (_HalfListEnergy)")
         if not ctx.want_grad:
             raise RuntimeError("energies were computed without forces (coords.requires_grad was False)")
         (grad,) = ctx.saved_tensors
