@@ -38,6 +38,7 @@
  *   ani_b200_charges            electro.py:29-156 (ChargeNormalizer.forward, DipoleComputer.forward) on the raw outputs of
  *                               a charge network pass (potentials/nnp.py:75-102, SeparateChargesNNPotential)
  *   ani_b200_operand_format     (no counterpart: format of the tensor-core GEMM operands of this build)
+ *   ani_b200_md_*               (no counterpart: the reference's MD loop is ASE's VelocityVerlet / Langevin on the host)
  */
 #ifndef ANI_B200_H
 #define ANI_B200_H
@@ -777,6 +778,67 @@ int ani_b200_hessian_geometric(const ani_aev_params* params, const float* spos, 
 int ani_b200_hessian_assemble(const int32_t* nbr_cnt, const int32_t* nbr_list, int cap, const int32_t* sorted_orig,
                               const ani_hessian_chunk* chunk, const float* blocks, int n_per_conf, double* hess,
                               void* stream);
+
+/* 10. Molecular dynamics on the device (csrc/md.cu): velocity Verlet (NVE) and BAOAB Langevin integrators whose       */
+/*    state stays in device memory, so that K whole MD steps (integrator + force step) capture into one CUDA graph.   */
+/*    Units: A, fs, amu, Hartree, K.  The caller owns every buffer (ani_md_state, device pointers unless noted):       */
+/*      x, v        f64[n][3] master positions (unwrapped, input order) and velocities (A / fs)                         */
+/*      inv_mass    f64[n] 1 / mass (1 / amu); 0 for padding atoms, which never move                                  */
+/*      params      f64[n_conf][ANI_MD_PARAMS] per conformer: dt (fs), temperature (K), friction (1 / fs), the energy  */
+/*                  QBC and the force relative-stdev stop thresholds (+inf: never), 3 N_real, two unused               */
+/*      counter     i64[2] step counter t (counter[0]; counter[1] is the launches' own copy)                           */
+/*      stop_step   i64[n_conf] -1 while running, else the step at which the conformer stopped                         */
+/*      trigger     f64[2][n][3] x, v of a conformer at its stop step (written then only), or NULL                     */
+/*      thermo      f64[thermo_rows][n_conf][ANI_MD_THERMO]: step t's record {t, E_pot, E_kin (Hartree), T (K)} goes    */
+/*                  to row t % thermo_rows; T = 2 E_kin / (3 N_real k_B)                                                */
+/*      frames      f64[frame_slots][1 + frame_velocities][n][3]: x (and v) of step t, where t % record_every == 0, in  */
+/*                  slot (t / record_every) % frame_slots; unused with record_every == 0                              */
+/*      partials    f64[n_conf][ceil(n_per_conf / ANI_MD_BLOCK)][2] scratch of ani_b200_md_step                        */
+/*      seed        key of the Langevin noise;  accel = Hartree / (amu A^2) in fs^-2;  kb = k_B in Hartree / K         */
+/*  ani_b200_md_init   per conformer, with zero_momentum: v -= total momentum / total mass (real atoms); then the      */
+/*                     f32 coords (flat input order) of x, wrapped into the cell: cell_mode 0 open, 1 one cell f32[9]   */
+/*                     (rows are lattice vectors), 2 one cell per conformer f32[n_conf][9].  One launch.               */
+/*  ani_b200_md_step   after the force step at x(t) (grad f32[n][3] dE/dx, energies f64[n_conf]), two launches: the   */
+/*                     final half kick B(dt/2) giving v(t) (none at t = 0: v(0) is the initial velocity), the thermo    */
+/*                     record and frame of step t, the stop check, then B(dt/2) A(dt) (ANI_MD_VERLET) or              */
+/*                     B(dt/2) A(dt/2) O(dt) A(dt/2) (ANI_MD_LANGEVIN, O: v = c v + sqrt((1 - c^2) k_B T / m) xi,      */
+/*                     c = exp(-friction dt), xi = ani_b200_md_noise(seed, t)) to x(t+1), the f32 coords of x(t+1)      */
+/*                     (wrapped into `cell` f32[9] when not NULL), and t += 1.  Stop check (qbc f64[n_conf] and          */
+/*                     force_stdev f32[n], the query-by-committee step's energy QBC and force_relative_stdev, both or  */
+/*                     neither): a running conformer whose qbc or largest force_stdev exceeds its threshold stops at     */
+/*                     t: stop_step = t, trigger = x(t), v(t); its x and v never change again.  Sums are float64 in a   */
+/*                     fixed order: the same state and forces give the same bits.                                     */
+/*  ani_b200_md_step_cells  the same with one cell per conformer: the lattice table of grid mode 3                     */
+/*                     (f32[n_conf][ANI_LATTICE_STRIDE], written by ani_b200_prepare_step_cells) in place of `cell`.    */
+/*  ani_b200_md_noise  out f64[n][3]: the standard normals the O step of step `step` draws for atoms 0..n-1 (flat index */
+/*                     over the conformers): Philox4x32-10 keyed on the seed, counter (step, atom, component), Box-Muller. */
+#define ANI_MD_BLOCK 256
+#define ANI_MD_PARAMS 8
+#define ANI_MD_THERMO 4
+#define ANI_MD_VERLET 0
+#define ANI_MD_LANGEVIN 1
+typedef struct ani_md_state {
+  double* x;
+  double* v;
+  const double* inv_mass;
+  const double* params;
+  long long* counter;
+  long long* stop_step;
+  double* trigger;
+  double* thermo;
+  double* frames;
+  double* partials;
+  unsigned long long seed;
+  double accel, kb;
+  int32_t n_conf, n_per_conf, integrator, thermo_rows, record_every, frame_slots, frame_velocities, pad_;
+} ani_md_state;
+int ani_b200_md_init(const ani_md_state* state, const float* cells, int cell_mode, int zero_momentum, float* coords,
+                     void* stream);
+int ani_b200_md_step(const ani_md_state* state, const float* grad, const double* energies, const double* qbc,
+                     const float* force_stdev, const float* cell, float* coords, void* stream);
+int ani_b200_md_step_cells(const ani_md_state* state, const float* grad, const double* energies, const double* qbc,
+                           const float* force_stdev, const float* lattice, float* coords, void* stream);
+int ani_b200_md_noise(unsigned long long seed, long long step, int n, double* out, void* stream);
 
 #ifdef __cplusplus
 }

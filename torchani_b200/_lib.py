@@ -97,6 +97,21 @@ class HessianWeights(C.Structure):
                 ("w3", C.c_void_p * ANI_MAX_SPECIES)]
 
 
+ANI_MD_BLOCK = 256
+ANI_MD_PARAMS = 8
+ANI_MD_THERMO = 4
+MD_VERLET = 0
+MD_LANGEVIN = 1
+
+
+class MDState(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in ("x", "v", "inv_mass", "params", "counter", "stop_step", "trigger", "thermo",
+                                          "frames", "partials")] + [
+        ("seed", C.c_uint64), ("accel", C.c_double), ("kb", C.c_double)] + [
+        (k, C.c_int32) for k in ("n_conf", "n_per_conf", "integrator", "thermo_rows", "record_every", "frame_slots",
+                                 "frame_velocities", "pad_")]
+
+
 class D3Params(C.Structure):
     _fields_ = [
         ("cutoff_fn", C.c_int32), ("num_species", C.c_int32), ("cutoff", C.c_float), ("to_bohr", C.c_float),
@@ -180,6 +195,10 @@ _PROTOTYPES = {
     "ani_b200_hessian_network": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P]),
     "ani_b200_hessian_geometric": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P]),
     "ani_b200_hessian_assemble": (C.c_int, [_P, _P, _I, _P, _P, _P, _I, _P, _P]),
+    "ani_b200_md_init": (C.c_int, [_P, _P, _I, _I, _P, _P]),
+    "ani_b200_md_step": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
+    "ani_b200_md_step_cells": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
+    "ani_b200_md_noise": (C.c_int, [C.c_uint64, C.c_longlong, _I, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -766,12 +766,19 @@ class Engine:
         key = (n_conf, n_per_conf)
         ws = self._ws.get(key)
         if ws is None:
-            ws = Workspace(n_conf, n_per_conf, self.consts.num_species, self.nets.ldx, self.nets.act_cols,
-                           self.nets.num_members, self.nbr_cap, self.device, variant=self.variant)
-            if self.dispersion is not None:   # coordination numbers and dE/dCN of every atom (D3 scratch)
-                ws.d3_cn = torch.zeros(ws.n, dtype=torch.float32, device=self.device)
-                ws.d3_dedcn = torch.zeros(ws.n, dtype=torch.float32, device=self.device)
+            ws = self.new_workspace(n_conf, n_per_conf)
             self._ws[key] = ws
+        return ws
+
+    def new_workspace(self, n_conf: int, n_per_conf: int) -> Workspace:
+        """A workspace of this shape that the engine does not cache, for a caller that keeps state in it from one step
+        to the next (md: the forces of the current positions); run it through ``_launch``, whose captured graphs are
+        the caller's (``run`` keys its graphs by shape, not by workspace)."""
+        ws = Workspace(n_conf, n_per_conf, self.consts.num_species, self.nets.ldx, self.nets.act_cols,
+                       self.nets.num_members, self.nbr_cap, self.device, variant=self.variant)
+        if self.dispersion is not None:   # coordination numbers and dE/dCN of every atom (D3 scratch)
+            ws.d3_cn = torch.zeros(ws.n, dtype=torch.float32, device=self.device)
+            ws.d3_dedcn = torch.zeros(ws.n, dtype=torch.float32, device=self.device)
         return ws
 
     def _stage_inputs(self, species: Tensor, coords: Tensor, cell: tp.Optional[Tensor], pbc: bool
@@ -858,9 +865,7 @@ class Engine:
             raise ValueError("the workspace of a periodic batch needs Workspace.make_periodic() first")
         if periodic_batch and reuse:
             raise ValueError("reuse=True (Verlet skin) is not supported for periodic batches")
-        if pbc and any(p.cutoff_fn == 2 for p in self.search_pairs):
-            raise ValueError("PBC can't use an infinite cutoff: a pair potential without a cutoff runs on open systems "
-                             "only")
+        self.check_pair_cutoffs(pbc)
         key = (n_conf, n_per_conf, bool(pbc), bool(want_grad), lo, hi, self.nets.active_key, bool(reuse), self.skin,
                bool(want_virial), self.mlp_mode, conformer_cells, members, tuple(p.kind for p in self.search_pairs))
         if charges:   # (the charge networks' operands and the normaliser / dipole parameters are baked into the capture)
@@ -923,6 +928,11 @@ class Engine:
                 virial = virial[0]
         return StepResult(ws.energies, ws.atomic.view(n_conf, n_per_conf),
                           ws.member_atomic.view(-1, n_conf, n_per_conf), grad, virial)
+
+    def check_pair_cutoffs(self, pbc: bool) -> None:
+        if pbc and any(p.cutoff_fn == 2 for p in self.search_pairs):
+            raise ValueError("PBC can't use an infinite cutoff: a pair potential without a cutoff runs on open systems "
+                             "only")
 
     def _prepare(self, ws: Workspace, pbc: bool, conformer_cells: bool, lo: int, hi: int, reuse: bool,
                  zero_ptr: tp.Optional[int], zero_count: int, virial: tp.Optional[Tensor],

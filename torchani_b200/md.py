@@ -1,0 +1,437 @@
+"""Molecular dynamics on the device: velocity Verlet (NVE) and Langevin (BAOAB) loops whose positions and velocities stay
+in device memory, with K whole MD steps -- the integrator launches of csrc/md.cu and the fused force step -- captured
+into one CUDA graph.  The host touches the GPU once per K steps: one replay, one copy of the replay's thermo records
+and frames into pinned memory, one synchronisation.
+
+    dyn = md.Langevin(model, atomic_numbers, positions, masses, dt=0.5, temperature=300.0, friction=0.02, seed=0)
+    dyn.run(10_000)
+    dyn.positions, dyn.velocities, dyn.thermo, dyn.frames
+
+Units: Angstrom, fs, amu, Hartree, K.  ``friction`` is in fs^-1: ASE's ``Langevin(..., friction=f)`` takes f in units
+of the inverse ASE time unit (``ASE_TIME_FS`` = 10.1805 fs), so ASE's ``friction=0.2`` is ``0.2 / ASE_TIME_FS`` =
+0.0196 fs^-1 here.  The BAOAB splitting samples the same distribution as ASE's Langevin but is not the same trajectory
+(another scheme, other random numbers).
+
+Every MD step rebuilds the bucket grid (no Verlet skin); the cell is fixed, and the system fully periodic or open.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import math
+import typing as tp
+import warnings
+
+import numpy as np
+import torch
+from torch import Tensor
+
+from . import _lib
+from ._lib import check, ptr
+from .engine import conformer_cells
+from .grad import HARTREE_TO_JOULE, _AMU, _E
+
+__all__ = ["VelocityVerlet", "Langevin", "maxwell_boltzmann", "Thermo", "Frames", "ACCEL", "KB", "ASE_TIME_FS"]
+
+K_B_JOULE = 1.38064852e-23                     # Boltzmann constant, J / K (CODATA 2014)
+ACCEL = HARTREE_TO_JOULE / _AMU * 1e-10        # Hartree / (amu A^2) in fs^-2: acceleration = -dE/dx / m * ACCEL
+KB = K_B_JOULE / HARTREE_TO_JOULE              # k_B in Hartree / K
+ASE_TIME_FS = 1e5 * math.sqrt(_AMU / _E)       # ASE's time unit, A sqrt(amu / eV), in fs
+
+
+class Thermo(tp.NamedTuple):
+    """One record per step and conformer (steps ascending)."""
+    step: np.ndarray          # (S,) int64
+    potential: np.ndarray     # (S, C) Hartree: the model's energy
+    kinetic: np.ndarray       # (S, C) Hartree
+    temperature: np.ndarray   # (S, C) K: 2 E_kin / (3 N_real k_B), as ASE reports it
+
+
+class Frames(tp.NamedTuple):
+    step: np.ndarray                    # (F,) int64: the recorded steps (multiples of record_every)
+    positions: np.ndarray               # (F, C, A, 3) float64, unwrapped
+    velocities: tp.Optional[np.ndarray]  # (F, C, A, 3) float64 with record_velocities, else None
+
+
+def maxwell_boltzmann(masses, temperature, seed: int = 0) -> np.ndarray:
+    """Velocities (..., A, 3) float64 in A / fs drawn from the Maxwell-Boltzmann distribution at ``temperature`` (K; a
+    scalar, or one per conformer for masses (C, A)), with the centre-of-mass momentum of every conformer set to zero.
+    Atoms with mass 0 (padding) get zero velocity."""
+    m = np.asarray(masses, dtype=np.float64)
+    batch = m.ndim == 2
+    m2 = m.reshape(-1, m.shape[-1])
+    T = np.broadcast_to(np.asarray(temperature, dtype=np.float64).reshape(-1, 1), (m2.shape[0], 1))
+    if (T <= 0).any() or (m2 < 0).any():
+        raise ValueError("temperature must be > 0 and masses >= 0")
+    real = m2 > 0
+    inv = np.where(real, 1.0 / np.where(real, m2, 1.0), 0.0)
+    rng = np.random.default_rng(seed)
+    v = rng.standard_normal(m2.shape + (3,)) * np.sqrt(KB * T * ACCEL * inv)[..., None]
+    p = (m2[..., None] * v).sum(1, keepdims=True)
+    v = np.where(real[..., None], v - p / m2.sum(1, keepdims=True)[..., None], 0.0)
+    return v if batch else v[0]
+
+
+class _Dynamics:
+    """The device MD loop shared by ``VelocityVerlet`` and ``Langevin`` (see the module docstring)."""
+
+    integrator = _lib.MD_VERLET
+
+    def __init__(self, model, atomic_numbers, positions, masses, dt: float, temperature, friction, seed: int,
+                 cell, pbc, velocities, steps_per_replay: int, record_every: int, record_velocities: bool,
+                 qbc_stop, zero_momentum: bool):
+        dev = next(model.buffers()).device
+        if dev.type != "cuda":
+            raise ValueError("the device MD loop needs a model on a CUDA device")
+        self.model, self.device = model, dev
+        if not (math.isfinite(dt) and dt > 0):
+            raise ValueError(f"dt must be > 0 fs, got {dt}")
+        pb = np.asarray(pbc if not isinstance(pbc, Tensor) else pbc.cpu(), dtype=bool).reshape(-1)
+        if pb.size not in (1, 3) or (pb.any() and not pb.all()):
+            raise ValueError("partial PBC is not supported: the system is fully periodic or open")
+        self.pbc = bool(pb.all())
+        if self.pbc and cell is None:
+            raise ValueError("If pbc is not None, cell should be present")
+        z = torch.as_tensor(np.asarray(atomic_numbers if not isinstance(atomic_numbers, Tensor)
+                                       else atomic_numbers.cpu()))
+        C_ = z.shape[0] if z.dim() == 2 else 1
+        z = z.reshape(C_, -1).to(dev)
+        A = z.shape[1]
+        self.n_conf, self.n_per_conf, n = C_, A, C_ * A
+        self.species = model.species_converter(z, nop=not model.periodic_table_index)
+        real = (self.species >= 0).cpu().numpy()
+        m = np.asarray(masses, dtype=np.float64)
+        m = np.broadcast_to(m.reshape(-1, A), (C_, A))
+        if not (np.isfinite(m[real]) & (m[real] > 0)).all():
+            raise ValueError("masses must be > 0 (amu) for every real atom")
+        n_real = real.sum(1)
+        if (n_real == 0).any():
+            raise ValueError("every conformer needs at least one real atom")
+        T = np.broadcast_to(np.asarray(temperature, dtype=np.float64).reshape(-1), (C_,))
+        g = np.broadcast_to(np.asarray(friction, dtype=np.float64).reshape(-1), (C_,))
+        if self.integrator == _lib.MD_LANGEVIN:
+            if not (np.isfinite(T) & (T > 0)).all():
+                raise ValueError("temperature must be > 0 K")
+            if not (np.isfinite(g) & (g >= 0)).all():
+                raise ValueError("friction must be >= 0 (1 / fs)")
+        self.qbc = qbc_stop is not None
+        e_thr, f_thr = (None, None) if qbc_stop is None else qbc_stop
+        e_thr = np.broadcast_to(np.asarray(math.inf if e_thr is None else e_thr, dtype=np.float64).reshape(-1), (C_,))
+        f_thr = np.broadcast_to(np.asarray(math.inf if f_thr is None else f_thr, dtype=np.float64).reshape(-1), (C_,))
+        self.K = int(steps_per_replay)
+        self.record_every = int(record_every)
+        if self.K < 1 or self.record_every < 0:
+            raise ValueError("steps_per_replay must be >= 1 and record_every >= 0")
+        self.dt = float(dt)
+
+        # the cell, in the form the engine takes it
+        self.per_conf = False
+        self.cell = None
+        if self.pbc:
+            c = torch.as_tensor(np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float32))
+            if c.dim() == 3 and C_ == 1:
+                c = c.reshape(3, 3)
+            self.per_conf = conformer_cells(c, C_)
+            self.cell = c.to(dev)
+
+        f64 = dict(dtype=torch.float64, device=dev)
+        # [x 3n | v 3n | counter 2 | stop_step C | thermo K C 4 | frames]: the head up to stop_step is what a redone
+        # replay restores, the tail from stop_step on is what a replay copies to the host
+        self.frame_slots = -(-self.K // self.record_every) if self.record_every else 0
+        self.frame_f = 2 if record_velocities else 1
+        head = 6 * n + 2 + C_
+        rec = C_ + self.K * C_ * _lib.ANI_MD_THERMO + self.frame_slots * self.frame_f * 3 * n
+        self._buf = torch.zeros(head + rec - C_, **f64)
+        self.x = self._buf[:3 * n].view(C_, A, 3)
+        self.v = self._buf[3 * n:6 * n].view(C_, A, 3)
+        self._counter = self._buf[6 * n:6 * n + 2].view(torch.int64)
+        self._stop = self._buf[6 * n + 2:head].view(torch.int64)
+        self._rec = self._buf[6 * n + 2:]
+        self._head = self._buf[:head]
+        self._backup = torch.empty_like(self._head)
+        self._thermo_dev = self._buf[head:head + self.K * C_ * _lib.ANI_MD_THERMO]
+        self._frames_dev = self._buf[head + self.K * C_ * _lib.ANI_MD_THERMO:]
+        self._h_rec = torch.zeros(self._rec.numel(), dtype=torch.float64).pin_memory()
+        self._h_status = torch.zeros(1, dtype=torch.int32).pin_memory()
+        pos = torch.as_tensor(positions if not isinstance(positions, Tensor) else positions.detach().cpu()
+                              ).to(torch.float64).reshape(C_, A, 3)
+        self.x.copy_(pos.to(dev))
+        if velocities is not None:
+            vel = torch.as_tensor(velocities if not isinstance(velocities, Tensor) else velocities.detach().cpu()
+                                  ).to(torch.float64).reshape(C_, A, 3)
+            self.v.copy_(vel.to(dev))
+        self._stop.fill_(-1)
+        inv = np.where(real, 1.0 / np.where(real, m, 1.0), 0.0)
+        self.inv_mass = torch.from_numpy(np.ascontiguousarray(inv)).to(**f64).reshape(-1)
+        params = np.zeros((C_, _lib.ANI_MD_PARAMS))
+        params[:, 0], params[:, 1], params[:, 2], params[:, 3], params[:, 4] = self.dt, T, g, e_thr, f_thr
+        params[:, 5] = 3 * n_real
+        self.params = torch.from_numpy(params).to(**f64)
+        self.trigger = torch.zeros(2, C_, A, 3, **f64) if self.qbc else None
+        nb = -(-A // _lib.ANI_MD_BLOCK)
+        self._partials = torch.zeros(C_ * nb * 2, **f64)
+        st = _lib.MDState()
+        st.x, st.v, st.inv_mass, st.params = ptr(self.x), ptr(self.v), ptr(self.inv_mass), ptr(self.params)
+        st.counter, st.stop_step, st.trigger = ptr(self._counter), ptr(self._stop), ptr(self.trigger)
+        st.thermo, st.frames, st.partials = ptr(self._thermo_dev), ptr(self._frames_dev), ptr(self._partials)
+        st.seed = int(seed) & (2 ** 64 - 1)
+        st.accel, st.kb = ACCEL, KB
+        st.n_conf, st.n_per_conf, st.integrator = C_, A, self.integrator
+        st.thermo_rows, st.record_every = self.K, self.record_every
+        st.frame_slots, st.frame_velocities = self.frame_slots, int(self.frame_f == 2)
+        self._state = st
+        self.step = 0   # steps done (the device counter, mirrored)
+        self._stop_host = np.full(C_, -1, dtype=np.int64)
+        self._thermo: tp.List[np.ndarray] = []
+        self._frames: tp.List[tp.Tuple[int, np.ndarray]] = []
+        self._graph: tp.Optional[torch.cuda.CUDAGraph] = None
+        with torch.cuda.device(dev):
+            self._attach_engine()
+            self._begin(bool(zero_momentum))
+
+    # -- engine and workspace ----------------------------------------------------------------
+    def _attach_engine(self) -> None:
+        eng = self.model.engine(self.device)
+        if eng.skin > 0:
+            raise ValueError("the device MD loop rebuilds the bucket grid every step: Verlet-skin reuse "
+                             "(Engine.skin > 0) is not supported")
+        if any(w.reducer is not None for w in eng._ws.values()):
+            raise ValueError("the device MD loop runs on one GPU: this engine is sharded")
+        eng.check_pair_cutoffs(self.pbc)
+        # a workspace of its own: between two runs it holds the forces of the current positions
+        ws = eng.new_workspace(self.n_conf, self.n_per_conf)
+        if self.pbc and self.n_conf > 1:
+            ws.make_periodic()
+        ws.species_i32.copy_(self.species.reshape(-1))
+        if self.qbc:
+            eng.members_buffers(ws)
+        if self.per_conf:
+            ws.cells.copy_(self.cell.reshape(self.n_conf, 9))
+        elif self.pbc:
+            ws.cell.copy_(self.cell.reshape(-1))
+        self.engine, self.ws = eng, ws
+        self._graph = None
+
+    def _begin(self, zero_momentum: bool) -> None:
+        """Write the float32 coordinates of the current positions and run the force step there (eagerly); on an operand
+        range overflow switch to the 3 x bfloat16 build, restore the state and start again."""
+        while True:
+            self._backup.copy_(self._head)
+            mode = 2 if self.per_conf else (1 if self.pbc else 0)
+            check(self.engine.lib.ani_b200_md_init(
+                C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, mode,
+                int(zero_momentum), ptr(self.ws.coords), self._stream()), "md_init")
+            self._force_step()
+            self._h_status.copy_(self.ws.status, non_blocking=True)
+            torch.cuda.current_stream(self.device).synchronize()
+            if not self._switched():
+                return
+            self._head.copy_(self._backup)
+
+    def _stream(self) -> int:
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def _switched(self) -> bool:
+        """Raise for the status word of the last force steps as Engine.check_status does; if the 2 x fp16 operand
+        format ran out of range, move to the 3 x bfloat16 build instead and return True (the caller redoes the work)."""
+        if int(self._h_status[0]) == 0:
+            return False
+        try:
+            self.engine.check_status(self.ws)
+        except _lib.OperandRangeError:
+            nets = self.model.neural_networks
+            if nets._variant == "bf16x3" or not _lib.available("bf16x3"):
+                raise
+            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this model "
+                          "to the 3 x bfloat16 build of the library")
+            nets.use_variant("bf16x3")
+            self._attach_engine()
+            return True
+        return False
+
+    # -- the loop -------------------------------------------------------------------------------
+    def _integrate(self) -> None:
+        """The integrator launches of one step (ani_b200_md_step: finish step t, start step t + 1)."""
+        ws, L = self.ws, self.engine.lib
+        qbc = ptr(ws.qbc) if self.qbc else None
+        stdev = ptr(ws.atom_stats[1]) if self.qbc else None
+        if self.per_conf:
+            rc = L.ani_b200_md_step_cells(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), qbc, stdev,
+                                          ptr(ws.lattice), ptr(ws.coords), self._stream())
+        else:
+            rc = L.ani_b200_md_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), qbc, stdev,
+                                    ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
+        check(rc, "md_step")
+
+    def _force_step(self) -> None:
+        self.engine._launch(self.ws, self.pbc, True, 0, self.ws.n, False, conformer_cells=self.per_conf,
+                            members=self.qbc)
+
+    def _body(self, k: int) -> None:
+        """k MD steps on the stream (graph-capturable): save the state, k x (integrator, force step), copies out."""
+        self._backup.copy_(self._head)
+        for _ in range(k):
+            self._integrate()
+            self._force_step()
+        self._h_rec.copy_(self._rec, non_blocking=True)
+        self._h_status.copy_(self.ws.status, non_blocking=True)
+
+    def _advance(self, k: int) -> None:
+        """k steps: one replay of the captured K-step graph (k == K) or eager launches of the same sequence."""
+        while True:
+            if k == self.K and self.engine.cuda_graph:
+                if self._graph is None:
+                    self.engine.note_composition(self.ws)
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        self._body(k)
+                    self._graph = g
+                self._graph.replay()
+            else:
+                self._body(k)
+            torch.cuda.current_stream(self.device).synchronize()
+            if not self._switched():
+                break
+            self._head.copy_(self._backup)   # redo the replay on the new build from the state it started with
+            self._begin(False)
+        self._collect(self.step, k)
+        self.step += k
+
+    def _collect(self, t0: int, k: int) -> None:
+        C_, K = self.n_conf, self.K
+        h = self._h_rec.numpy()
+        th = h[C_:C_ + K * C_ * _lib.ANI_MD_THERMO].reshape(K, C_, _lib.ANI_MD_THERMO)
+        self._thermo.append(th[[(t0 + i) % K for i in range(k)]].copy())
+        if self.record_every:
+            fr = h[C_ + K * C_ * _lib.ANI_MD_THERMO:].reshape(self.frame_slots, self.frame_f, C_, self.n_per_conf, 3)
+            for t in range(t0, t0 + k):
+                if t % self.record_every == 0:
+                    self._frames.append((t, fr[(t // self.record_every) % self.frame_slots].copy()))
+        self._stop_host = h[:C_].view(np.int64).copy()
+
+    def run(self, steps: int, callback: tp.Optional[tp.Callable[..., tp.Any]] = None) -> None:
+        """Run ``steps`` MD steps: replays of ``steps_per_replay`` steps, the remainder as eager launches of the same
+        sequence (bitwise the same result).  ``callback(step, positions, velocities, thermo)`` runs after every replay
+        (``thermo``: that replay's records).  With ``qbc_stop`` the run ends early once every conformer has stopped;
+        the force steps of stopped conformers go on to the end of their replay (at most K - 1 wasted steps each)."""
+        steps = int(steps)
+        if steps < 0:
+            raise ValueError("steps must be >= 0")
+        with torch.cuda.device(self.device):
+            done = 0
+            while done < steps:
+                k = min(self.K, steps - done)
+                self._advance(k)
+                done += k
+                if callback is not None:
+                    callback(self.step, self.positions, self.velocities, self._as_thermo(self._thermo[-1]))
+                if self.qbc and bool((self._stop_host >= 0).all()):
+                    break
+
+    # -- results ----------------------------------------------------------------------------------
+    @property
+    def positions(self) -> Tensor:
+        """(C, A, 3) float64 master positions of the current step, unwrapped (device)."""
+        return self.x
+
+    @property
+    def velocities(self) -> Tensor:
+        """(C, A, 3) float64 velocities of the current step t (device): the stored velocities lack the final half kick
+        of step t until the next step applies it, so it is applied here from the forces of the last force step (not at
+        t = 0 and not for stopped conformers, whose velocities are those of their stop step)."""
+        if self.step == 0:
+            return self.v.clone()
+        h = (0.5 * self.params[:, 0] * ACCEL).view(-1, 1, 1) * self.inv_mass.view(self.n_conf, -1, 1)
+        kicked = self.v - h * self.ws.grad.view(self.n_conf, self.n_per_conf, 3).double()
+        stopped = (self._stop >= 0).view(-1, 1, 1)
+        return torch.where(stopped, self.v, kicked)
+
+    @staticmethod
+    def _as_thermo(th: np.ndarray) -> Thermo:
+        return Thermo(th[:, 0, 0].astype(np.int64), th[..., 1].copy(), th[..., 2].copy(), th[..., 3].copy())
+
+    @property
+    def thermo(self) -> Thermo:
+        if not self._thermo:
+            z = np.zeros((0, self.n_conf))
+            return Thermo(np.zeros(0, dtype=np.int64), z, z.copy(), z.copy())
+        return self._as_thermo(np.concatenate(self._thermo))
+
+    @property
+    def frames(self) -> Frames:
+        shape = (0, self.n_conf, self.n_per_conf, 3)
+        if not self._frames:
+            return Frames(np.zeros(0, dtype=np.int64), np.zeros(shape), np.zeros(shape) if self.frame_f == 2 else None)
+        f = np.stack([fr for _, fr in self._frames])
+        return Frames(np.array([t for t, _ in self._frames], dtype=np.int64), f[:, 0],
+                      f[:, 1] if self.frame_f == 2 else None)
+
+    @property
+    def stop_step(self) -> np.ndarray:
+        """(C,) int64: the step at which each conformer stopped, -1 while it runs (``qbc_stop``)."""
+        return self._stop.cpu().numpy()
+
+    @property
+    def stopped(self) -> np.ndarray:
+        return self.stop_step >= 0
+
+    @property
+    def trigger_frame(self) -> tp.Tuple[Tensor, Tensor]:
+        """(positions, velocities), each (C, A, 3) float64 on the device, of every conformer at its stop step (zeros
+        for a conformer that has not stopped); ``qbc_stop`` only."""
+        if self.trigger is None:
+            raise ValueError("no qbc_stop was given")
+        return self.trigger[0], self.trigger[1]
+
+
+class VelocityVerlet(_Dynamics):
+    """NVE: B(dt/2) A(dt) forces B(dt/2), as ASE's ``VelocityVerlet``.
+
+    Args:
+        model: a ``torchani_b200.models.ANI`` on a CUDA device
+        atomic_numbers: (A,) or (C, A) (element indices if the model has ``periodic_table_index=False``); -1 pads
+        positions: (A, 3) or (C, A, 3) Angstrom; masses: (A,) or (C, A) amu (ignored for padding)
+        dt: time step, fs
+        cell: None, (3, 3) shared or (C, 3, 3) one per conformer; pbc: fully periodic (True) or open
+        velocities: initial velocities (A / fs), default zero (see ``maxwell_boltzmann``)
+        steps_per_replay: K, the MD steps of one CUDA graph replay
+        record_every: a frame every so many steps (0: none); record_velocities: frames hold the velocities too
+        qbc_stop: None, or (energy QBC threshold, force relative-stdev threshold) -- scalars or one per conformer, None
+            for a check that is not wanted: a conformer stops, and its x and v freeze, at the first step whose ensemble
+            disagreement exceeds either (``stopped``, ``stop_step``, ``trigger_frame``); the steps run the
+            query-by-committee force step
+        zero_momentum: remove the centre-of-mass momentum of every conformer at the start
+    """
+
+    integrator = _lib.MD_VERLET
+
+    def __init__(self, model, atomic_numbers, positions, masses, dt: float = 0.5, cell=None, pbc=False,
+                 velocities=None, steps_per_replay: int = 20, record_every: int = 10, record_velocities: bool = False,
+                 qbc_stop=None, zero_momentum: bool = False):
+        super().__init__(model, atomic_numbers, positions, masses, dt, 0.0, 0.0, 0, cell, pbc, velocities,
+                         steps_per_replay, record_every, record_velocities, qbc_stop, zero_momentum)
+
+
+class Langevin(_Dynamics):
+    """NVT: BAOAB (Leimkuhler-Matthews), B(dt/2) A(dt/2) O(dt) A(dt/2) forces B(dt/2), with
+    O: v = c v + sqrt((1 - c^2) k_B T / m) xi, c = exp(-friction dt), and xi from a counter-based generator keyed on
+    (seed, step, atom, component): the noise does not depend on K or on replay boundaries.  ``temperature`` (K) and
+    ``friction`` (1 / fs) may be one per conformer (replicas at different temperatures in one batch).  The other
+    arguments are those of ``VelocityVerlet``."""
+
+    integrator = _lib.MD_LANGEVIN
+
+    def __init__(self, model, atomic_numbers, positions, masses, dt: float = 0.5, temperature=300.0,
+                 friction=0.02, seed: int = 0, cell=None, pbc=False, velocities=None, steps_per_replay: int = 20,
+                 record_every: int = 10, record_velocities: bool = False, qbc_stop=None, zero_momentum: bool = False):
+        super().__init__(model, atomic_numbers, positions, masses, dt, temperature, friction, seed, cell, pbc,
+                         velocities, steps_per_replay, record_every, record_velocities, qbc_stop, zero_momentum)
+
+
+def noise(seed: int, step: int, n: int, device) -> Tensor:
+    """(n, 3) float64: the standard normals the Langevin O step of ``step`` draws for atoms 0..n-1 (flat index over
+    the conformers), from ani_b200_md_noise."""
+    out = torch.empty(n, 3, dtype=torch.float64, device=device)
+    with torch.cuda.device(out.device):
+        check(_lib.lib().ani_b200_md_noise(int(seed) & (2 ** 64 - 1), int(step), int(n), ptr(out),
+                                           torch.cuda.current_stream(out.device).cuda_stream), "md_noise")
+    return out
