@@ -779,8 +779,9 @@ int ani_b200_hessian_assemble(const int32_t* nbr_cnt, const int32_t* nbr_list, i
                               const ani_hessian_chunk* chunk, const float* blocks, int n_per_conf, double* hess,
                               void* stream);
 
-/* 10. Molecular dynamics on the device (csrc/md.cu): velocity Verlet (NVE) and BAOAB Langevin integrators whose       */
-/*    state stays in device memory, so that K whole MD steps (integrator + force step) capture into one CUDA graph.   */
+/* 10. Molecular dynamics on the device (csrc/md.cu): velocity Verlet (NVE), BAOAB Langevin (NVT) and Langevin with   */
+/*    stochastic cell rescaling (NPT) integrators whose state stays in device memory, so that K whole MD steps          */
+/*    (integrator + force step) capture into one CUDA graph.                                                          */
 /*    Units: A, fs, amu, Hartree, K.  The caller owns every buffer (ani_md_state, device pointers unless noted):       */
 /*      x, v        f64[n][3] master positions (unwrapped, input order) and velocities (A / fs)                         */
 /*      inv_mass    f64[n] 1 / mass (1 / amu); 0 for padding atoms, which never move                                  */
@@ -812,9 +813,32 @@ int ani_b200_hessian_assemble(const int32_t* nbr_cnt, const int32_t* nbr_list, i
 /*                     (f32[n_conf][ANI_LATTICE_STRIDE], written by ani_b200_prepare_step_cells) in place of `cell`.    */
 /*  ani_b200_md_noise  out f64[n][3]: the standard normals the O step of step `step` draws for atoms 0..n-1 (flat index */
 /*                     over the conformers): Philox4x32-10 keyed on the seed, counter (step, atom, component), Box-Muller. */
+/*  ani_b200_md_step_npt  ani_b200_md_step (ANI_MD_LANGEVIN only, no stop check) with isotropic stochastic cell        */
+/*                     rescaling (Bernetti & Bussi, J. Chem. Phys. 153, 114107 (2020)), every conformer fully periodic.  */
+/*                     With h(t) the master cell, V = |det h|, K = E_kin(t), W = the virial of the force step at x(t)    */
+/*                     (its slots summed in a fixed order), T, dt from params and P0, tau_p, beta_T from baro->params:    */
+/*                       P_int = (2 K - tr W) / (3 V)                                                                 */
+/*                       de = -(beta_T / tau_p) (P0 - P_int) dt + sqrt(2 k_B T beta_T dt / (V tau_p)) xi  (de = d ln V)  */
+/*                       mu = exp(de / 3);  after B A O A:  x(t+1) = mu x',  v <- v / mu,  h(t+1) = mu h(t)           */
+/*                     xi = ani_b200_md_cell_noise(seed, t)[c].  The f32 coords of x(t+1) are wrapped into the           */
+/*                     float32-rounded h(t+1), which is written to cell_out for the next force step (never read by this   */
+/*                     launch).  ani_md_barostat (device pointers; units A, fs, Hartree):                                 */
+/*                       master       f64[2][n_conf][9] master cell rows by step parity: step t reads slot t % 2 and      */
+/*                                    writes slot (t + 1) % 2                                                          */
+/*                       params       f64[n_conf][ANI_MD_BARO_PARAMS]: P0 (Hartree / A^3), tau_p (fs), beta_T (A^3 / Hartree) */
+/*                       cell_out     f32 cell rows of conformer c at cell_out + c * cell_stride (>= 9): the cell the      */
+/*                                    next preparation reads (the workspace's cell, or its cells of grid mode 3)          */
+/*                       virial       f64[n_conf][virial_slots][9] the force step's virial slots (its W_ab partial sums)   */
+/*                       record       f64[thermo_rows][n_conf][ANI_MD_BARO]: {V (A^3), P_int (Hartree / A^3)} of step t,   */
+/*                                    in row t % thermo_rows, beside the thermo record                                 */
+/*                       frame_cells  f64[frame_slots][n_conf][9] h(t) of each frame (not NULL with record_every > 0)      */
+/*  ani_b200_md_cell_noise  out f64[n_conf]: the standard normals xi of the cell rescaling of step `step`: Philox      */
+/*                     counter (step, conformer, component 3), a counter no atom draws.                                  */
 #define ANI_MD_BLOCK 256
 #define ANI_MD_PARAMS 8
 #define ANI_MD_THERMO 4
+#define ANI_MD_BARO_PARAMS 3
+#define ANI_MD_BARO 2
 #define ANI_MD_VERLET 0
 #define ANI_MD_LANGEVIN 1
 typedef struct ani_md_state {
@@ -839,6 +863,18 @@ int ani_b200_md_step(const ani_md_state* state, const float* grad, const double*
 int ani_b200_md_step_cells(const ani_md_state* state, const float* grad, const double* energies, const double* qbc,
                            const float* force_stdev, const float* lattice, float* coords, void* stream);
 int ani_b200_md_noise(unsigned long long seed, long long step, int n, double* out, void* stream);
+typedef struct ani_md_barostat {
+  double* master;
+  const double* params;
+  float* cell_out;
+  const double* virial;
+  double* record;
+  double* frame_cells;
+  int32_t cell_stride, virial_slots;
+} ani_md_barostat;
+int ani_b200_md_step_npt(const ani_md_state* state, const ani_md_barostat* baro, const float* grad,
+                         const double* energies, float* coords, void* stream);
+int ani_b200_md_cell_noise(unsigned long long seed, long long step, int n_conf, double* out, void* stream);
 
 #ifdef __cplusplus
 }

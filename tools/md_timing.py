@@ -9,12 +9,16 @@ Arms, per workload, velocity Verlet at dt = 0.5 fs:
     host                   HostCalculator.calculate (one H2D, graph replay, one D2H, synchronise per step) driven by the
                            oracle's float64 velocity Verlet in numpy -- the reference's ASE pattern without ASE
 
+With --npt the arms are instead, on water 1 k and 10 k at K = 10 and 50, Langevin (BAOAB, NVT) against LangevinNPT
+(the same with stochastic cell rescaling at 1.01325 bar: the force step also accumulates the virial), timed the same
+way, with the integrator launches of both.
+
 Every arm is warmed up (captures happen before timing).  The device arms are timed with a host clock around run()
 (which ends in a synchronisation) and with CUDA events around the same call; the host arm with a host clock.  The
 integrator's own launches (ani_b200_md_step, two kernels) are timed separately with CUDA events over 200 eager calls.
 The arms alternate over --reps rounds; medians are reported with the device name and power limit, as JSON in --out.
 
-    python tools/md_timing.py --out <dir> [--reps 5] [--steps 500]
+    python tools/md_timing.py --out <dir> [--reps 5] [--steps 500] [--npt]
 """
 from __future__ import annotations
 
@@ -46,12 +50,17 @@ def workload(name):
     return idx.numpy(), co.double().numpy(), cell.double().numpy(), True
 
 
-def device_arm(model, name, K, steps):
+def device_arm(model, name, K, steps, kind="verlet"):
     from torchani_b200 import md
     sp, co, cell, pbc = workload(name)
     m = MASSES_2X[np.maximum(sp, 0)] * (sp >= 0)
-    dyn = md.VelocityVerlet(model, sp, co, m, dt=DT, cell=cell, pbc=pbc, velocities=md.maxwell_boltzmann(m, 300.0, 1),
-                            steps_per_replay=K, record_every=0)
+    kw = dict(dt=DT, velocities=md.maxwell_boltzmann(m, 300.0, 1), steps_per_replay=K, record_every=0)
+    if kind == "verlet":
+        dyn = md.VelocityVerlet(model, sp, co, m, cell=cell, pbc=pbc, **kw)
+    elif kind == "nvt":
+        dyn = md.Langevin(model, sp, co, m, cell=cell, pbc=pbc, **kw)
+    else:
+        dyn = md.LangevinNPT(model, sp, co, m, cell, **kw)
     steps = steps // K * K
     dyn.run(2 * K)   # capture + warm-up
 
@@ -118,8 +127,10 @@ def main() -> None:
     ap.add_argument("--out", required=True)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--steps", type=int, default=500)
-    ap.add_argument("--workloads", default="water1k,water10k,gdb256")
+    ap.add_argument("--workloads", default=None)
+    ap.add_argument("--npt", action="store_true", help="Langevin against LangevinNPT at K = 10 and 50")
     args = ap.parse_args()
+    workloads = args.workloads or ("water1k,water10k" if args.npt else "water1k,water10k,gdb256")
     if not torch.cuda.is_available():
         raise SystemExit("md_timing needs a GPU")
     from torchani_b200 import models
@@ -129,12 +140,17 @@ def main() -> None:
                          capture_output=True, text=True).stdout.strip()
     result = {"device": torch.cuda.get_device_name(0), "nvidia_smi": smi, "dt_fs": DT, "steps": args.steps,
               "workloads": {}}
-    for name in args.workloads.split(","):
+    for name in workloads.split(","):
         arms = {}
         dyns = {}
-        for K in (1, 10, 50):
-            dyns[K], arms[f"device K={K}"] = device_arm(model, name, K, args.steps)
-        arms["host"] = host_arm(model, name, max(50, args.steps // 5))
+        if args.npt:
+            for kind in ("nvt", "npt"):
+                for K in (10, 50):
+                    dyns[(kind, K)], arms[f"{kind} K={K}"] = device_arm(model, name, K, args.steps, kind)
+        else:
+            for K in (1, 10, 50):
+                dyns[K], arms[f"device K={K}"] = device_arm(model, name, K, args.steps)
+            arms["host"] = host_arm(model, name, max(50, args.steps // 5))
         times = {k: ([], []) for k in arms}
         for _ in range(args.reps):
             for k, fn in arms.items():
@@ -148,11 +164,15 @@ def main() -> None:
             rec[k] = {"ms_per_step": ms, "spread_ms": [min(wall), max(wall)],
                       "device_ms_per_step": statistics.median(dev) if dev else None,
                       "ns_per_day": DT * 1e-6 * 86400e3 / ms}
-        rec["integrator_ms_per_step"] = integrator_ms(dyns[50])
+        if args.npt:
+            for kind in ("nvt", "npt"):
+                rec[f"{kind} integrator_ms_per_step"] = integrator_ms(dyns[(kind, 50)])
+        else:
+            rec["integrator_ms_per_step"] = integrator_ms(dyns[50])
         result["workloads"][name] = rec
         print(name, json.dumps(rec, indent=1), flush=True)
     os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "md_timing.json"), "w") as fh:
+    with open(os.path.join(args.out, "md_timing_npt.json" if args.npt else "md_timing.json"), "w") as fh:
         json.dump(result, fh, indent=1)
     print(json.dumps(result))
 

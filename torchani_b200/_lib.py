@@ -100,6 +100,8 @@ class HessianWeights(C.Structure):
 ANI_MD_BLOCK = 256
 ANI_MD_PARAMS = 8
 ANI_MD_THERMO = 4
+ANI_MD_BARO_PARAMS = 3
+ANI_MD_BARO = 2
 MD_VERLET = 0
 MD_LANGEVIN = 1
 
@@ -110,6 +112,11 @@ class MDState(C.Structure):
         ("seed", C.c_uint64), ("accel", C.c_double), ("kb", C.c_double)] + [
         (k, C.c_int32) for k in ("n_conf", "n_per_conf", "integrator", "thermo_rows", "record_every", "frame_slots",
                                  "frame_velocities", "pad_")]
+
+
+class MDBarostat(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in ("master", "params", "cell_out", "virial", "record", "frame_cells")] + [
+        ("cell_stride", C.c_int32), ("virial_slots", C.c_int32)]
 
 
 class D3Params(C.Structure):
@@ -199,6 +206,8 @@ _PROTOTYPES = {
     "ani_b200_md_step": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "ani_b200_md_step_cells": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "ani_b200_md_noise": (C.c_int, [C.c_uint64, C.c_longlong, _I, _P, _P]),
+    "ani_b200_md_step_npt": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "ani_b200_md_cell_noise": (C.c_int, [C.c_uint64, C.c_longlong, _I, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -13,6 +13,13 @@
 // Every sum is float64 in a fixed order (block trees of fixed shape, no atomics): two runs from the same state and
 // forces give identical bits.  The step counter lives on the device (counter[0] is read by k_md_finish, which copies
 // it to counter[1] for k_md_start, which advances counter[0]), so a replayed graph needs no argument changes.
+//
+// Constant pressure (ani_b200_md_step_npt): k_md_start also forms the conformer's internal pressure from E_kin, the
+// trace of the force step's virial and the volume of its float64 master cell, draws the isotropic stochastic cell
+// rescaling (Bernetti & Bussi 2020) factor mu, and after B A (O A) scales x and the cell by mu and v by 1 / mu.  The
+// master cell is double-buffered by step parity (step t reads slot t % 2, block 0 writes slot (t + 1) % 2), and the
+// float32 coordinates are wrapped into the float32-rounded new cell, which block 0 also writes for the next force
+// step's preparation: no launch reads a word another block of the same launch writes.
 #include "common.cuh"
 
 namespace ani {
@@ -29,6 +36,7 @@ struct MdArgs {
   int cell_stride;
   float* coords;              // f32[n][3]
   int zero_momentum;          // (ani_b200_md_init)
+  ani_md_barostat baro;       // ani_b200_md_step_npt; baro.master == nullptr for NVE / NVT
 };
 
 // ---- counter-based normals: Philox4x32-10 keyed on the seed, counter (step, atom, component) ----------------------
@@ -61,32 +69,41 @@ __device__ __forceinline__ double md_normal(unsigned long long seed, long long s
   return sqrt(-2.0 * log(u1)) * cospi(2.0 * u2);
 }
 
-// float64 cell rows and inverse of conformer c (frac = r @ inv), by thread 0 into shared memory
+// determinant of the cell rows m
+__device__ __forceinline__ double det3(const double* m) {
+  return m[0] * (m[4] * m[8] - m[5] * m[7]) + m[1] * (m[5] * m[6] - m[3] * m[8]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
+}
+
+// inverse of the cell rows m (frac = r @ inv)
+__device__ __forceinline__ void invert3(const double* m, double* inv) {
+  const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6];
+  const double det = m[0] * c00 + m[1] * c01 + m[2] * c02;
+  const double r = 1.0 / det;
+  inv[0] = c00 * r;
+  inv[1] = (m[2] * m[7] - m[1] * m[8]) * r;
+  inv[2] = (m[1] * m[5] - m[2] * m[4]) * r;
+  inv[3] = c01 * r;
+  inv[4] = (m[0] * m[8] - m[2] * m[6]) * r;
+  inv[5] = (m[2] * m[3] - m[0] * m[5]) * r;
+  inv[6] = c02 * r;
+  inv[7] = (m[1] * m[6] - m[0] * m[7]) * r;
+  inv[8] = (m[0] * m[4] - m[1] * m[3]) * r;
+}
+
+// float64 cell rows and inverse of conformer c, by thread 0 into shared memory
 __device__ __forceinline__ void load_cell(const MdArgs& a, int c, double* cell, double* inv) {
   if (threadIdx.x == 0 && a.cells) {
     const float* f = a.cells + (size_t)c * a.cell_stride;
     for (int k = 0; k < 9; ++k) cell[k] = (double)f[k];
-    const double* m = cell;
-    const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6];
-    const double det = m[0] * c00 + m[1] * c01 + m[2] * c02;
-    const double r = 1.0 / det;
-    inv[0] = c00 * r;
-    inv[1] = (m[2] * m[7] - m[1] * m[8]) * r;
-    inv[2] = (m[1] * m[5] - m[2] * m[4]) * r;
-    inv[3] = c01 * r;
-    inv[4] = (m[0] * m[8] - m[2] * m[6]) * r;
-    inv[5] = (m[2] * m[3] - m[0] * m[5]) * r;
-    inv[6] = c02 * r;
-    inv[7] = (m[1] * m[6] - m[0] * m[7]) * r;
-    inv[8] = (m[0] * m[4] - m[1] * m[3]) * r;
+    invert3(cell, inv);
   }
 }
 
 // float32 coordinates of master position x: wrapped into the cell (fractional coordinates minus their floor) when
 // periodic, so that the float32 copy never holds a far-away image
-__device__ __forceinline__ void write_coords(const MdArgs& a, size_t i, double x, double y, double z,
+__device__ __forceinline__ void write_coords(const MdArgs& a, size_t i, double x, double y, double z, bool periodic,
                                              const double* cell, const double* inv) {
-  if (a.cells) {
+  if (periodic) {
     const double f0 = floor(x * inv[0] + y * inv[3] + z * inv[6]);
     const double f1 = floor(x * inv[1] + y * inv[4] + z * inv[7]);
     const double f2 = floor(x * inv[2] + y * inv[5] + z * inv[8]);
@@ -152,10 +169,47 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_finish(const __grid_constant__ 
   }
 }
 
-// launch 2 of a step: totals, thermo, frame, stop check, and the move to x(t+1)
-__global__ void __launch_bounds__(MD_BLOCK) k_md_start(const __grid_constant__ MdArgs a) {
-  __shared__ double cell[9], inv[9], tot[2];
+// isotropic stochastic cell rescaling of conformer c at step t (Euler-Maruyama in eps = ln V), by thread 0 of every
+// block of the conformer (the same inputs, so the same mu everywhere): tot = {sum 1/2 m v^2 (E_kin in amu A^2 / fs^2),
+// -, tr W}; mu goes to tot[3], the float32-rounded new cell and its inverse to cell / inv.  Block 0 writes the master cell of step t + 1, the float32
+// cell of the next force step, the record {V, P_int} of step t and the cell of step t's frame.
+__device__ void rescale_cell(const MdArgs& a, int c, long long t, const double* par, double* tot, double* cell,
+                             double* inv) {
   const ani_md_state& s = a.s;
+  const ani_md_barostat& b = a.baro;
+  const double* h = b.master + ((size_t)(t & 1) * s.n_conf + c) * 9;
+  const double* bp = b.params + (size_t)c * ANI_MD_BARO_PARAMS;   // P0 (Hartree / A^3), tau_p (fs), beta_T (A^3 / Hartree)
+  const double vol = fabs(det3(h));
+  const double p_int = (2.0 * tot[0] / s.accel - tot[2]) / (3.0 * vol);
+  const double kt = s.kb * par[1], dt = par[0], bt = bp[2] / bp[1];
+  // (the k_B T / V term of the volume form, dV = -(beta_T V / tau_p)(P0 - P_int - k_B T / V) dt + ..., cancels against
+  // the Ito correction of eps = ln V: keeping it here would sample V^(N+1) exp(-P0 V / k_B T), one power too many)
+  const double de = -bt * (bp[0] - p_int) * dt + sqrt(2.0 * kt * bt * dt / vol) * md_normal(s.seed, t, c, 3);
+  const double mu = exp(de / 3.0);
+  tot[3] = mu;
+  for (int k = 0; k < 9; ++k) cell[k] = (double)(float)(mu * h[k]);
+  invert3(cell, inv);
+  if (blockIdx.x != 0) return;
+  double* hn = b.master + ((size_t)((t + 1) & 1) * s.n_conf + c) * 9;
+  float* out = b.cell_out + (size_t)c * b.cell_stride;
+  for (int k = 0; k < 9; ++k) {
+    hn[k] = mu * h[k];
+    out[k] = (float)(mu * h[k]);
+  }
+  double* rec = b.record + ((size_t)(t % s.thermo_rows) * s.n_conf + c) * ANI_MD_BARO;
+  rec[0] = vol;
+  rec[1] = p_int;
+  if (s.record_every > 0 && t % s.record_every == 0) {
+    double* fc = b.frame_cells + ((size_t)((t / s.record_every) % s.frame_slots) * s.n_conf + c) * 9;
+    for (int k = 0; k < 9; ++k) fc[k] = h[k];
+  }
+}
+
+// launch 2 of a step: totals, thermo, frame, stop check, (the cell rescaling,) and the move to x(t+1)
+__global__ void __launch_bounds__(MD_BLOCK) k_md_start(const __grid_constant__ MdArgs a) {
+  __shared__ double cell[9], inv[9], tot[4];
+  const ani_md_state& s = a.s;
+  const bool npt = a.baro.master != nullptr;
   const int c = blockIdx.y, j = blockIdx.x * MD_BLOCK + threadIdx.x, nb = gridDim.x;
   const long long t = s.counter[1];
   const double* par = s.params + (size_t)c * ANI_MD_PARAMS;
@@ -174,8 +228,21 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_start(const __grid_constant__ M
       tot[0] = ke;
       tot[1] = fm;
     }
+  } else if (npt && threadIdx.x < 64) {   // the trace of the conformer's virial slots, in the same fixed order
+    const int l = threadIdx.x - 32;
+    const double* w = a.baro.virial + (size_t)c * a.baro.virial_slots * 9;
+    double tr = 0.0;
+    for (int k = l; k < a.baro.virial_slots; k += 32) tr += w[9 * k] + w[9 * k + 4] + w[9 * k + 8];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) tr += __shfl_down_sync(ANI_FULL_MASK, tr, o);
+    if (l == 0) tot[2] = tr;
   }
-  load_cell(a, c, cell, inv);
+  if (npt) {
+    __syncthreads();
+    if (threadIdx.x == 0) rescale_cell(a, c, t, par, tot, cell, inv);
+  } else {
+    load_cell(a, c, cell, inv);
+  }
   __syncthreads();
   // stop_step[c] is written below by block 0 of this conformer only, and only with the value t: a block that reads it
   // concurrently sees -1 or t, and "stopped before this step" is false for both
@@ -242,13 +309,22 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_start(const __grid_constant__ M
     y += hd * vy;
     z += hd * vz;
   }
+  if (npt) {   // x(t+1) = mu x', v / mu
+    const double mu = tot[3];
+    x *= mu;
+    y *= mu;
+    z *= mu;
+    vx /= mu;
+    vy /= mu;
+    vz /= mu;
+  }
   s.x[3 * i + 0] = x;
   s.x[3 * i + 1] = y;
   s.x[3 * i + 2] = z;
   s.v[3 * i + 0] = vx;
   s.v[3 * i + 1] = vy;
   s.v[3 * i + 2] = vz;
-  write_coords(a, i, x, y, z, cell, inv);
+  write_coords(a, i, x, y, z, npt || a.cells, cell, inv);
 }
 
 // one CTA per conformer: optional removal of the centre-of-mass momentum, then the coordinates of step 0
@@ -277,7 +353,7 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_init(const __grid_constant__ Md
   __syncthreads();
   for (int j = threadIdx.x; j < A; j += MD_BLOCK) {
     const size_t i = base + j;
-    write_coords(a, i, s.x[3 * i + 0], s.x[3 * i + 1], s.x[3 * i + 2], cell, inv);
+    write_coords(a, i, s.x[3 * i + 0], s.x[3 * i + 1], s.x[3 * i + 2], a.cells, cell, inv);
   }
 }
 
@@ -287,12 +363,18 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_noise(unsigned long long seed, 
   for (int k = 0; k < 3; ++k) out[3 * (size_t)i + k] = md_normal(seed, step, i, k);
 }
 
+__global__ void __launch_bounds__(MD_BLOCK) k_md_cell_noise(unsigned long long seed, long long step, int n, double* out) {
+  const int c = blockIdx.x * MD_BLOCK + threadIdx.x;
+  if (c < n) out[c] = md_normal(seed, step, c, 3);
+}
+
 bool md_state_ok(const ani_md_state* s) {
   return s && s->x && s->v && s->inv_mass && s->n_conf >= 1 && s->n_per_conf >= 1;
 }
 
 int md_step(const ani_md_state* s, const float* grad, const double* energies, const double* qbc,
-            const float* force_stdev, const float* cells, int cell_stride, float* coords, void* stream) {
+            const float* force_stdev, const float* cells, int cell_stride, float* coords, void* stream,
+            const ani_md_barostat* baro = nullptr) {
   if (!md_state_ok(s) || !s->params || !s->counter || !s->stop_step || !s->thermo || !s->partials) return ANI_ERR_BAD_ARG;
   if (!grad || !energies || !coords || (!qbc != !force_stdev)) return ANI_ERR_BAD_ARG;
   if ((s->integrator != ANI_MD_VERLET && s->integrator != ANI_MD_LANGEVIN) || s->thermo_rows < 1) return ANI_ERR_BAD_ARG;
@@ -309,6 +391,7 @@ int md_step(const ani_md_state* s, const float* grad, const double* energies, co
   a.cell_stride = cell_stride;
   a.coords = coords;
   a.zero_momentum = 0;
+  a.baro = baro ? *baro : ani_md_barostat{};
   const dim3 grid((s->n_per_conf + MD_BLOCK - 1) / MD_BLOCK, s->n_conf);
   cudaStream_t st = (cudaStream_t)stream;
   k_md_finish<<<grid, MD_BLOCK, 0, st>>>(a);
@@ -349,9 +432,26 @@ extern "C" int ani_b200_md_step_cells(const ani_md_state* state, const float* gr
   return md_step(state, grad, energies, qbc, force_stdev, lattice, ANI_LATTICE_STRIDE, coords, stream);
 }
 
+extern "C" int ani_b200_md_step_npt(const ani_md_state* state, const ani_md_barostat* baro, const float* grad,
+                                    const double* energies, float* coords, void* stream) {
+  if (!md_state_ok(state) || !baro || state->integrator != ANI_MD_LANGEVIN) return ANI_ERR_BAD_ARG;
+  const ani_md_barostat& b = *baro;
+  if (!b.master || !b.params || !b.cell_out || !b.virial || !b.record || b.cell_stride < 9 || b.virial_slots < 1)
+    return ANI_ERR_BAD_ARG;
+  if (state->record_every > 0 && !b.frame_cells) return ANI_ERR_BAD_ARG;
+  return md_step(state, grad, energies, nullptr, nullptr, nullptr, 0, coords, stream, baro);
+}
+
 extern "C" int ani_b200_md_noise(unsigned long long seed, long long step, int n, double* out, void* stream) {
   if (n < 1 || !out) return ANI_ERR_BAD_ARG;
   k_md_noise<<<(n + MD_BLOCK - 1) / MD_BLOCK, MD_BLOCK, 0, (cudaStream_t)stream>>>(seed, step, n, out);
+  ANI_CUDA_CHECK_LAUNCH();
+  return ANI_OK;
+}
+
+extern "C" int ani_b200_md_cell_noise(unsigned long long seed, long long step, int n_conf, double* out, void* stream) {
+  if (n_conf < 1 || !out) return ANI_ERR_BAD_ARG;
+  k_md_cell_noise<<<(n_conf + MD_BLOCK - 1) / MD_BLOCK, MD_BLOCK, 0, (cudaStream_t)stream>>>(seed, step, n_conf, out);
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;
 }

@@ -40,6 +40,8 @@ SQRT_MHESSIAN_TO_INVCM = math.sqrt(HARTREE_TO_JOULE / _AMU) / 1e-10 / _C / 100.0
 SQRT_MHESSIAN_TO_MILLIEV = SQRT_MHESSIAN_TO_INVCM * INVCM_TO_EV * 1000.0
 # Hartree / A^2 -> N / m -> mDyne / A (1 N = 1e8 mDyne, 1 m = 1e10 A)
 MHESSIAN_TO_FCONST = HARTREE_TO_JOULE * 1e8 / 1e-10
+# 1 bar = 1e5 Pa = 1e5 J / m^3 in Hartree / A^3 (1 m^3 = 1e30 A^3)
+BAR_TO_HARTREE_A3 = 1e5 / HARTREE_TO_JOULE / 1e30
 
 
 class EnergiesForces(tp.NamedTuple):

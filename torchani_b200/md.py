@@ -1,7 +1,8 @@
-"""Molecular dynamics on the device: velocity Verlet (NVE) and Langevin (BAOAB) loops whose positions and velocities stay
-in device memory, with K whole MD steps -- the integrator launches of csrc/md.cu and the fused force step -- captured
-into one CUDA graph.  The host touches the GPU once per K steps: one replay, one copy of the replay's thermo records
-and frames into pinned memory, one synchronisation.
+"""Molecular dynamics on the device: velocity Verlet (NVE), Langevin (BAOAB, NVT) and Langevin with stochastic cell
+rescaling (NPT) loops whose positions, velocities and cells stay in device memory, with K whole MD steps -- the
+integrator launches of csrc/md.cu and the fused force step -- captured into one CUDA graph.  The host touches the GPU
+once per K steps: one replay, one copy of the replay's thermo records and frames into pinned memory, one
+synchronisation.
 
     dyn = md.Langevin(model, atomic_numbers, positions, masses, dt=0.5, temperature=300.0, friction=0.02, seed=0)
     dyn.run(10_000)
@@ -12,7 +13,9 @@ of the inverse ASE time unit (``ASE_TIME_FS`` = 10.1805 fs), so ASE's ``friction
 0.0196 fs^-1 here.  The BAOAB splitting samples the same distribution as ASE's Langevin but is not the same trajectory
 (another scheme, other random numbers).
 
-Every MD step rebuilds the bucket grid (no Verlet skin); the cell is fixed, and the system fully periodic or open.
+Every MD step rebuilds the bucket grid (no Verlet skin).  ``VelocityVerlet`` and ``Langevin`` keep the cell fixed, and
+the system fully periodic or open; ``LangevinNPT`` rescales the cell of every conformer of a fully periodic system.
+Pressures are in bar and compressibilities in 1 / bar (``BAR_TO_HARTREE_A3`` converts).
 """
 from __future__ import annotations
 
@@ -28,9 +31,10 @@ from torch import Tensor
 from . import _lib
 from ._lib import check, ptr
 from .engine import conformer_cells
-from .grad import HARTREE_TO_JOULE, _AMU, _E
+from .grad import BAR_TO_HARTREE_A3, HARTREE_TO_JOULE, _AMU, _E
 
-__all__ = ["VelocityVerlet", "Langevin", "maxwell_boltzmann", "Thermo", "Frames", "ACCEL", "KB", "ASE_TIME_FS"]
+__all__ = ["VelocityVerlet", "Langevin", "LangevinNPT", "maxwell_boltzmann", "Thermo", "Frames", "NPT", "ACCEL", "KB",
+           "ASE_TIME_FS", "BAR_TO_HARTREE_A3"]
 
 K_B_JOULE = 1.38064852e-23                     # Boltzmann constant, J / K (CODATA 2014)
 ACCEL = HARTREE_TO_JOULE / _AMU * 1e-10        # Hartree / (amu A^2) in fs^-2: acceleration = -dE/dx / m * ACCEL
@@ -50,6 +54,13 @@ class Frames(tp.NamedTuple):
     step: np.ndarray                    # (F,) int64: the recorded steps (multiples of record_every)
     positions: np.ndarray               # (F, C, A, 3) float64, unwrapped
     velocities: tp.Optional[np.ndarray]  # (F, C, A, 3) float64 with record_velocities, else None
+
+
+class NPT(tp.NamedTuple):
+    """One barostat record per step and conformer (``LangevinNPT``; steps ascending, those of ``Thermo``)."""
+    step: np.ndarray          # (S,) int64
+    volume: np.ndarray        # (S, C) A^3: the cell of the step
+    pressure: np.ndarray      # (S, C) bar: the internal pressure (2 E_kin - tr W) / (3 V), W the force step's virial
 
 
 def maxwell_boltzmann(masses, temperature, seed: int = 0) -> np.ndarray:
@@ -78,7 +89,7 @@ class _Dynamics:
 
     def __init__(self, model, atomic_numbers, positions, masses, dt: float, temperature, friction, seed: int,
                  cell, pbc, velocities, steps_per_replay: int, record_every: int, record_velocities: bool,
-                 qbc_stop, zero_momentum: bool):
+                 qbc_stop, zero_momentum: bool, barostat: tp.Optional[tp.Tuple[np.ndarray, float, np.ndarray]] = None):
         dev = next(model.buffers()).device
         if dev.type != "cuda":
             raise ValueError("the device MD loop needs a model on a CUDA device")
@@ -114,6 +125,7 @@ class _Dynamics:
             if not (np.isfinite(g) & (g >= 0)).all():
                 raise ValueError("friction must be >= 0 (1 / fs)")
         self.qbc = qbc_stop is not None
+        self.isobaric = barostat is not None
         e_thr, f_thr = (None, None) if qbc_stop is None else qbc_stop
         e_thr = np.broadcast_to(np.asarray(math.inf if e_thr is None else e_thr, dtype=np.float64).reshape(-1), (C_,))
         f_thr = np.broadcast_to(np.asarray(math.inf if f_thr is None else f_thr, dtype=np.float64).reshape(-1), (C_,))
@@ -125,31 +137,46 @@ class _Dynamics:
 
         # the cell, in the form the engine takes it
         self.per_conf = False
-        self.cell = None
+        self._cell32 = None
         if self.pbc:
-            c = torch.as_tensor(np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float32))
+            c64 = np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float64)
+            c = torch.as_tensor(c64.astype(np.float32))
             if c.dim() == 3 and C_ == 1:
                 c = c.reshape(3, 3)
             self.per_conf = conformer_cells(c, C_)
-            self.cell = c.to(dev)
+            if self.isobaric and C_ > 1 and not self.per_conf:   # every replica's box evolves on its own: grid mode 3
+                c, self.per_conf = c.expand(C_, 3, 3).contiguous(), True
+            self._cell32 = c.to(dev)
+            if self.isobaric:
+                c64 = np.broadcast_to(c64.reshape(-1, 3, 3), (C_, 3, 3))
+                if not (np.isfinite(c64).all() and (np.abs(np.linalg.det(c64)) > 0).all()):
+                    raise ValueError("constant pressure needs a finite cell of volume > 0 for every conformer")
 
         f64 = dict(dtype=torch.float64, device=dev)
-        # [x 3n | v 3n | counter 2 | stop_step C | thermo K C 4 | frames]: the head up to stop_step is what a redone
-        # replay restores, the tail from stop_step on is what a replay copies to the host
+        # [x 3n | v 3n | counter 2 | master cells 2 C 9 (NPT) | stop_step C | thermo K C 4 | frames | NPT records K C 2 |
+        # frame cells F C 9]: the head up to stop_step is what a redone replay restores, the tail from stop_step on is
+        # what a replay copies to the host
         self.frame_slots = -(-self.K // self.record_every) if self.record_every else 0
         self.frame_f = 2 if record_velocities else 1
-        head = 6 * n + 2 + C_
-        rec = C_ + self.K * C_ * _lib.ANI_MD_THERMO + self.frame_slots * self.frame_f * 3 * n
-        self._buf = torch.zeros(head + rec - C_, **f64)
+        nm = 18 * C_ if self.isobaric else 0
+        head = 6 * n + 2 + nm + C_
+        n_th, n_fr = self.K * C_ * _lib.ANI_MD_THERMO, self.frame_slots * self.frame_f * 3 * n
+        n_bar, n_fc = (self.K * C_ * _lib.ANI_MD_BARO, self.frame_slots * C_ * 9) if self.isobaric else (0, 0)
+        self._buf = torch.zeros(head + n_th + n_fr + n_bar + n_fc, **f64)
         self.x = self._buf[:3 * n].view(C_, A, 3)
         self.v = self._buf[3 * n:6 * n].view(C_, A, 3)
         self._counter = self._buf[6 * n:6 * n + 2].view(torch.int64)
-        self._stop = self._buf[6 * n + 2:head].view(torch.int64)
-        self._rec = self._buf[6 * n + 2:]
+        self._master = self._buf[6 * n + 2:6 * n + 2 + nm].view(2, C_, 3, 3) if self.isobaric else None
+        self._stop = self._buf[head - C_:head].view(torch.int64)
+        self._rec = self._buf[head - C_:]
         self._head = self._buf[:head]
         self._backup = torch.empty_like(self._head)
-        self._thermo_dev = self._buf[head:head + self.K * C_ * _lib.ANI_MD_THERMO]
-        self._frames_dev = self._buf[head + self.K * C_ * _lib.ANI_MD_THERMO:]
+        self._thermo_dev = self._buf[head:head + n_th]
+        self._frames_dev = self._buf[head + n_th:head + n_th + n_fr]
+        self._baro_dev = self._buf[head + n_th + n_fr:head + n_th + n_fr + n_bar]
+        self._fcells_dev = self._buf[head + n_th + n_fr + n_bar:]
+        if self.isobaric:
+            self._master[0].copy_(torch.from_numpy(np.array(c64)).to(dev))
         self._h_rec = torch.zeros(self._rec.numel(), dtype=torch.float64).pin_memory()
         self._h_status = torch.zeros(1, dtype=torch.int32).pin_memory()
         pos = torch.as_tensor(positions if not isinstance(positions, Tensor) else positions.detach().cpu()
@@ -166,6 +193,11 @@ class _Dynamics:
         params[:, 0], params[:, 1], params[:, 2], params[:, 3], params[:, 4] = self.dt, T, g, e_thr, f_thr
         params[:, 5] = 3 * n_real
         self.params = torch.from_numpy(params).to(**f64)
+        if self.isobaric:
+            p0, tau, beta = barostat
+            bp = np.zeros((C_, _lib.ANI_MD_BARO_PARAMS))
+            bp[:, 0], bp[:, 1], bp[:, 2] = p0, tau, beta
+            self.baro_params = torch.from_numpy(bp).to(**f64)
         self.trigger = torch.zeros(2, C_, A, 3, **f64) if self.qbc else None
         nb = -(-A // _lib.ANI_MD_BLOCK)
         self._partials = torch.zeros(C_ * nb * 2, **f64)
@@ -183,6 +215,8 @@ class _Dynamics:
         self._stop_host = np.full(C_, -1, dtype=np.int64)
         self._thermo: tp.List[np.ndarray] = []
         self._frames: tp.List[tp.Tuple[int, np.ndarray]] = []
+        self._npt_rec: tp.List[np.ndarray] = []
+        self._frame_cells: tp.List[np.ndarray] = []
         self._graph: tp.Optional[torch.cuda.CUDAGraph] = None
         with torch.cuda.device(dev):
             self._attach_engine()
@@ -204,18 +238,33 @@ class _Dynamics:
         ws.species_i32.copy_(self.species.reshape(-1))
         if self.qbc:
             eng.members_buffers(ws)
-        if self.per_conf:
-            ws.cells.copy_(self.cell.reshape(self.n_conf, 9))
+        if self.isobaric:
+            pass   # the float32 cell(s) of the current master cell, written by _begin
+        elif self.per_conf:
+            ws.cells.copy_(self._cell32.reshape(self.n_conf, 9))
         elif self.pbc:
-            ws.cell.copy_(self.cell.reshape(-1))
+            ws.cell.copy_(self._cell32.reshape(-1))
         self.engine, self.ws = eng, ws
         self._graph = None
+        if self.isobaric:
+            b = _lib.MDBarostat()
+            b.master, b.params, b.virial = ptr(self._master), ptr(self.baro_params), ptr(ws.virial)
+            b.cell_out, b.cell_stride = ptr(ws.cells) if self.per_conf else ptr(ws.cell), 9
+            b.record, b.frame_cells = ptr(self._baro_dev), ptr(self._fcells_dev)
+            b.virial_slots = _lib.ANI_VIRIAL_SLOTS
+            self._baro = b
 
     def _begin(self, zero_momentum: bool) -> None:
         """Write the float32 coordinates of the current positions and run the force step there (eagerly); on an operand
         range overflow switch to the 3 x bfloat16 build, restore the state and start again."""
         while True:
             self._backup.copy_(self._head)
+            if self.isobaric:   # the float32 cell(s) of the current step's master cell
+                h = self._master[self.step % 2]
+                if self.per_conf:
+                    self.ws.cells.copy_(h.reshape(self.n_conf, 9))
+                else:
+                    self.ws.cell.copy_(h.reshape(-1))
             mode = 2 if self.per_conf else (1 if self.pbc else 0)
             check(self.engine.lib.ani_b200_md_init(
                 C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, mode,
@@ -252,6 +301,10 @@ class _Dynamics:
     def _integrate(self) -> None:
         """The integrator launches of one step (ani_b200_md_step: finish step t, start step t + 1)."""
         ws, L = self.ws, self.engine.lib
+        if self.isobaric:
+            check(L.ani_b200_md_step_npt(C.byref(self._state), C.byref(self._baro), ptr(ws.grad), ptr(ws.energies),
+                                         ptr(ws.coords), self._stream()), "md_step_npt")
+            return
         qbc = ptr(ws.qbc) if self.qbc else None
         stdev = ptr(ws.atom_stats[1]) if self.qbc else None
         if self.per_conf:
@@ -263,8 +316,8 @@ class _Dynamics:
         check(rc, "md_step")
 
     def _force_step(self) -> None:
-        self.engine._launch(self.ws, self.pbc, True, 0, self.ws.n, False, conformer_cells=self.per_conf,
-                            members=self.qbc)
+        self.engine._launch(self.ws, self.pbc, True, 0, self.ws.n, False, want_virial=self.isobaric,
+                            conformer_cells=self.per_conf, members=self.qbc)
 
     def _body(self, k: int) -> None:
         """k MD steps on the stream (graph-capturable): save the state, k x (integrator, force step), copies out."""
@@ -299,13 +352,23 @@ class _Dynamics:
     def _collect(self, t0: int, k: int) -> None:
         C_, K = self.n_conf, self.K
         h = self._h_rec.numpy()
-        th = h[C_:C_ + K * C_ * _lib.ANI_MD_THERMO].reshape(K, C_, _lib.ANI_MD_THERMO)
-        self._thermo.append(th[[(t0 + i) % K for i in range(k)]].copy())
+        o_fr = C_ + self._thermo_dev.numel()
+        o_bar = o_fr + self._frames_dev.numel()
+        o_fc = o_bar + self._baro_dev.numel()
+        rows = [(t0 + i) % K for i in range(k)]
+        th = h[C_:o_fr].reshape(K, C_, _lib.ANI_MD_THERMO)
+        self._thermo.append(th[rows].copy())
+        if self.isobaric:
+            self._npt_rec.append(h[o_bar:o_fc].reshape(K, C_, _lib.ANI_MD_BARO)[rows].copy())
         if self.record_every:
-            fr = h[C_ + K * C_ * _lib.ANI_MD_THERMO:].reshape(self.frame_slots, self.frame_f, C_, self.n_per_conf, 3)
+            fr = h[o_fr:o_bar].reshape(self.frame_slots, self.frame_f, C_, self.n_per_conf, 3)
+            fc = h[o_fc:].reshape(self.frame_slots, C_, 3, 3) if self.isobaric else None
             for t in range(t0, t0 + k):
                 if t % self.record_every == 0:
-                    self._frames.append((t, fr[(t // self.record_every) % self.frame_slots].copy()))
+                    slot = (t // self.record_every) % self.frame_slots
+                    self._frames.append((t, fr[slot].copy()))
+                    if self.isobaric:
+                        self._frame_cells.append(fc[slot].copy())
         self._stop_host = h[:C_].view(np.int64).copy()
 
     def run(self, steps: int, callback: tp.Optional[tp.Callable[..., tp.Any]] = None) -> None:
@@ -328,6 +391,12 @@ class _Dynamics:
                     break
 
     # -- results ----------------------------------------------------------------------------------
+    @property
+    def cell(self) -> tp.Optional[Tensor]:
+        """The fixed cell in the form the engine takes it: (3, 3) or, one per conformer, (C, 3, 3) float32 (device);
+        None for an open system."""
+        return self._cell32
+
     @property
     def positions(self) -> Tensor:
         """(C, A, 3) float64 master positions of the current step, unwrapped (device)."""
@@ -427,6 +496,87 @@ class Langevin(_Dynamics):
                          velocities, steps_per_replay, record_every, record_velocities, qbc_stop, zero_momentum)
 
 
+class LangevinNPT(_Dynamics):
+    """NPT: ``Langevin`` (BAOAB) with isotropic stochastic cell rescaling (C-rescale; Bernetti & Bussi, J. Chem. Phys.
+    153, 114107 (2020)).  With eps = ln V, per conformer and step t:
+
+        P_int = (2 E_kin - tr W) / (3 V)                 W = sum (dE/dDelta)_a Delta_b, the force step's virial
+        d eps = -(beta_T / tau_p) (P0 - P_int) dt + sqrt(2 k_B T beta_T dt / (V tau_p)) xi
+        mu    = exp(d eps / 3):   h <- mu h,   x <- mu x,   v <- v / mu
+
+    (Euler-Maruyama in eps.  The paper's k_B T / V drift term belongs to its volume form, dV = ...; in eps it cancels
+    against the Ito correction; keeping it would sample Gamma(N + 2) instead of Gamma(N + 1), whose mean is
+    1 / (N + 1) = 1.5 % larger for an ideal gas of 64 atoms.)
+
+    P_int is formed from E_kin, W and V of step t; the rescaling follows the B A O A moves of the step, so the next force
+    step sees the positions and the cell it is used with.  The noise xi is keyed on (seed, step, conformer) apart from
+    the atoms' (``cell_noise``).  Isotropic scaling keeps the cell's shape (triclinic cells included).  The sampled
+    volume distribution is that of the isothermal-isobaric ensemble (an ideal gas of N atoms: Gamma(N + 1, k_B T / P0)).
+
+    Args: those of ``Langevin`` without ``pbc`` (always fully periodic); ``qbc_stop`` is rejected (the
+    query-by-committee step computes no virial); and
+        cell: (3, 3) or (C, 3, 3) lattice vectors as rows; a shared cell of a batch becomes one cell per conformer, since
+            every replica's box evolves on its own
+        pressure: P0, bar (scalar or one per conformer)
+        tau_p: the barostat's relaxation time, fs
+        compressibility: beta_T, 1 / bar (scalar or one per conformer; 4.5e-5 is water's)
+    A box that shrinks below the cutoff raises ``ANI_STATUS_CELL_TOO_SMALL`` at the end of the replay, as does a
+    neighbour-list overflow as the density rises.
+    """
+
+    integrator = _lib.MD_LANGEVIN
+
+    def __init__(self, model, atomic_numbers, positions, masses, cell, dt: float = 0.5, temperature=300.0,
+                 friction=0.02, pressure=1.01325, tau_p: float = 1000.0, compressibility=4.5e-5, seed: int = 0,
+                 velocities=None, steps_per_replay: int = 20, record_every: int = 10, record_velocities: bool = False,
+                 qbc_stop=None, zero_momentum: bool = False):
+        if cell is None:
+            raise ValueError("constant pressure needs a fully periodic cell")
+        if qbc_stop is not None:
+            raise ValueError("qbc_stop is not supported at constant pressure: the query-by-committee step computes no "
+                             "virial")
+        n_conf = np.shape(atomic_numbers)[0] if np.ndim(atomic_numbers) == 2 else 1
+        p0 = np.broadcast_to(np.asarray(pressure, dtype=np.float64).reshape(-1), (n_conf,))
+        beta = np.broadcast_to(np.asarray(compressibility, dtype=np.float64).reshape(-1), (n_conf,))
+        tau_p = float(tau_p)
+        if not np.isfinite(p0).all():
+            raise ValueError("pressure must be finite (bar)")
+        if not (math.isfinite(tau_p) and tau_p > 0):
+            raise ValueError(f"tau_p must be > 0 fs, got {tau_p}")
+        if not (np.isfinite(beta) & (beta > 0)).all():
+            raise ValueError("compressibility must be > 0 (1 / bar)")
+        super().__init__(model, atomic_numbers, positions, masses, dt, temperature, friction, seed, cell, True,
+                         velocities, steps_per_replay, record_every, record_velocities, None, zero_momentum,
+                         (p0 * BAR_TO_HARTREE_A3, tau_p, beta / BAR_TO_HARTREE_A3))
+
+    @property
+    def cell(self) -> Tensor:
+        """(C, 3, 3) float64 cell of the current step, lattice vectors as rows: a copy on the device (the master cells
+        are rewritten by every step)."""
+        return self._master[self.step % 2].clone()
+
+    @property
+    def volume(self) -> Tensor:
+        """(C,) float64 volume of the current cell, A^3 (device)."""
+        return torch.linalg.det(self._master[self.step % 2]).abs()
+
+    @property
+    def npt(self) -> NPT:
+        th = self.thermo
+        if not self._npt_rec:
+            z = np.zeros((0, self.n_conf))
+            return NPT(th.step, z, z.copy())
+        r = np.concatenate(self._npt_rec)
+        return NPT(th.step, r[..., 0].copy(), r[..., 1] / BAR_TO_HARTREE_A3)
+
+    @property
+    def frame_cells(self) -> np.ndarray:
+        """(F, C, 3, 3) float64: the cell of every frame of ``frames``."""
+        if not self._frame_cells:
+            return np.zeros((0, self.n_conf, 3, 3))
+        return np.stack(self._frame_cells)
+
+
 def noise(seed: int, step: int, n: int, device) -> Tensor:
     """(n, 3) float64: the standard normals the Langevin O step of ``step`` draws for atoms 0..n-1 (flat index over
     the conformers), from ani_b200_md_noise."""
@@ -434,4 +584,14 @@ def noise(seed: int, step: int, n: int, device) -> Tensor:
     with torch.cuda.device(out.device):
         check(_lib.lib().ani_b200_md_noise(int(seed) & (2 ** 64 - 1), int(step), int(n), ptr(out),
                                            torch.cuda.current_stream(out.device).cuda_stream), "md_noise")
+    return out
+
+
+def cell_noise(seed: int, step: int, n_conf: int, device) -> Tensor:
+    """(n_conf,) float64: the standard normals the cell rescaling of ``step`` draws for conformers 0..n_conf-1, from
+    ani_b200_md_cell_noise."""
+    out = torch.empty(n_conf, dtype=torch.float64, device=device)
+    with torch.cuda.device(out.device):
+        check(_lib.lib().ani_b200_md_cell_noise(int(seed) & (2 ** 64 - 1), int(step), int(n_conf), ptr(out),
+                                                torch.cuda.current_stream(out.device).cuda_stream), "md_cell_noise")
     return out
