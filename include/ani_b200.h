@@ -876,6 +876,61 @@ int ani_b200_md_step_npt(const ani_md_state* state, const ani_md_barostat* baro,
                          const double* energies, float* coords, void* stream);
 int ani_b200_md_cell_noise(unsigned long long seed, long long step, int n_conf, double* out, void* stream);
 
+/* 11. Geometry optimisation on the device (csrc/opt.cu): FIRE (Bitzek et al., PRL 97, 170201 (2006)) as ASE's        */
+/*    ase.optimize.FIRE defines it, without its downhill check, one independent optimisation per conformer.  The state */
+/*    stays in device memory, so that K whole steps (FIRE + force step) capture into one CUDA graph, as in section 10.  */
+/*    Units: A, eV, Hartree.  The caller owns every buffer (ani_opt_state, device pointers):                            */
+/*      x, v        f64[n][3] master positions (unwrapped, input order) and FIRE velocities (eV / A x the time unit)     */
+/*      force_scale f64[n] f = -dE/dx * force_scale: HARTREE_TO_EV for movable real atoms, 0 for fixed or padding atoms  */
+/*      params      f64[n_conf][ANI_OPT_PARAMS] per conformer: dt0, maxstep (A), dtmax, Nmin, finc, fdec, astart, fa,  */
+/*                  the fmax threshold (eV / A).  Not read by the validation of the entry points (device memory): the     */
+/*                  caller keeps 0 < fdec < 1 <= finc, 0 < fa <= 1, dt0, maxstep, dtmax > 0 and fmax >= 0               */
+/*      scalars     f64[2][n_conf][ANI_OPT_SCALARS] {dt, a, n} by step parity: step t reads slot t % 2 and writes slot    */
+/*                  (t + 1) % 2                                                                                     */
+/*      counter     i64[2] step counter t (counter[0]; counter[1] is the launches' own copy)                           */
+/*      conv_step   i64[n_conf] -1 while the conformer runs, else the step at which it converged                        */
+/*      record      f64[record_rows][n_conf][ANI_OPT_RECORD]: step t's record {t, E (Hartree), fmax (eV / A)} goes to    */
+/*                  row t % record_rows                                                                              */
+/*      partials    f64[n_conf][ceil(n_per_conf / ANI_MD_BLOCK)][4] scratch of ani_b200_opt_step                       */
+/*  ani_b200_opt_init  with reset: v = 0 and the scalars of slot counter[0] % 2 = {dt0, astart, 0}; then the f32       */
+/*                     coords of x, wrapped into the cell: cell_mode 0 open, 1 one cell f32[9], 2 one cell per          */
+/*                     conformer f32[n_conf][9].  One launch.                                                         */
+/*  ani_b200_opt_step  after the force step at x(t) (grad f32[n][3] dE/dx, energies f64[n_conf]), two launches, per    */
+/*                     conformer with fmax(t) = max_i |f_i|:                                                           */
+/*                       record {t, E, fmax(t)};  fmax(t) < threshold (and running): conv_step = t, and from then on    */
+/*                       x, v, dt, a, n never change;  else P = f.v, F2 = f.f, V2 = v.v and                            */
+/*                       t > 0, P > 0:  c1 = 1 - a, c2 = a sqrt(V2 / F2);  n > Nmin: dt = min(dt finc, dtmax), a *= fa; */
+/*                                      n += 1                                                                       */
+/*                       t > 0, P <= 0: c1 = c2 = 0, a = astart, dt *= fdec, n = 0                                   */
+/*                       t = 0:         c1 = 1, c2 = 0                                                               */
+/*                       v' = c1 v + (c2 + dt) f,  |dr| = dt sqrt(c1^2 V2 + 2 c1 (c2 + dt) P + (c2 + dt)^2 F2),        */
+/*                       x(t+1) = x(t) + dt v' min(1, maxstep / |dr|)                                                   */
+/*                     then the f32 coords of x(t+1) (wrapped into `cell` f32[9] when not NULL), and t += 1.  Sums are   */
+/*                     float64 in a fixed order: the same state and forces give the same bits.                         */
+/*  ani_b200_opt_step_cells  the same with one cell per conformer: the lattice table of grid mode 3                    */
+/*                     (f32[n_conf][ANI_LATTICE_STRIDE], written by ani_b200_prepare_step_cells) in place of `cell`.    */
+#define ANI_OPT_PARAMS 9
+#define ANI_OPT_SCALARS 3
+#define ANI_OPT_RECORD 3
+typedef struct ani_opt_state {
+  double* x;
+  double* v;
+  const double* force_scale;
+  const double* params;
+  double* scalars;
+  long long* counter;
+  long long* conv_step;
+  double* record;
+  double* partials;
+  int32_t n_conf, n_per_conf, record_rows, pad_;
+} ani_opt_state;
+int ani_b200_opt_init(const ani_opt_state* state, const float* cells, int cell_mode, int reset, float* coords,
+                      void* stream);
+int ani_b200_opt_step(const ani_opt_state* state, const float* grad, const double* energies, const float* cell,
+                      float* coords, void* stream);
+int ani_b200_opt_step_cells(const ani_opt_state* state, const float* grad, const double* energies,
+                            const float* lattice, float* coords, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -119,6 +119,17 @@ class MDBarostat(C.Structure):
         ("cell_stride", C.c_int32), ("virial_slots", C.c_int32)]
 
 
+ANI_OPT_PARAMS = 9
+ANI_OPT_SCALARS = 3
+ANI_OPT_RECORD = 3
+
+
+class OptState(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in ("x", "v", "force_scale", "params", "scalars", "counter", "conv_step", "record",
+                                          "partials")] + [
+        (k, C.c_int32) for k in ("n_conf", "n_per_conf", "record_rows", "pad_")]
+
+
 class D3Params(C.Structure):
     _fields_ = [
         ("cutoff_fn", C.c_int32), ("num_species", C.c_int32), ("cutoff", C.c_float), ("to_bohr", C.c_float),
@@ -208,6 +219,9 @@ _PROTOTYPES = {
     "ani_b200_md_noise": (C.c_int, [C.c_uint64, C.c_longlong, _I, _P, _P]),
     "ani_b200_md_step_npt": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "ani_b200_md_cell_noise": (C.c_int, [C.c_uint64, C.c_longlong, _I, _P, _P]),
+    "ani_b200_opt_init": (C.c_int, [_P, _P, _I, _I, _P, _P]),
+    "ani_b200_opt_step": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "ani_b200_opt_step_cells": (C.c_int, [_P, _P, _P, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

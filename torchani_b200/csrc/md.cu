@@ -20,7 +20,7 @@
 // master cell is double-buffered by step parity (step t reads slot t % 2, block 0 writes slot (t + 1) % 2), and the
 // float32 coordinates are wrapped into the float32-rounded new cell, which block 0 also writes for the next force
 // step's preparation: no launch reads a word another block of the same launch writes.
-#include "common.cuh"
+#include "md_common.cuh"
 
 namespace ani {
 
@@ -74,65 +74,6 @@ __device__ __forceinline__ double det3(const double* m) {
   return m[0] * (m[4] * m[8] - m[5] * m[7]) + m[1] * (m[5] * m[6] - m[3] * m[8]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
 }
 
-// inverse of the cell rows m (frac = r @ inv)
-__device__ __forceinline__ void invert3(const double* m, double* inv) {
-  const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6];
-  const double det = m[0] * c00 + m[1] * c01 + m[2] * c02;
-  const double r = 1.0 / det;
-  inv[0] = c00 * r;
-  inv[1] = (m[2] * m[7] - m[1] * m[8]) * r;
-  inv[2] = (m[1] * m[5] - m[2] * m[4]) * r;
-  inv[3] = c01 * r;
-  inv[4] = (m[0] * m[8] - m[2] * m[6]) * r;
-  inv[5] = (m[2] * m[3] - m[0] * m[5]) * r;
-  inv[6] = c02 * r;
-  inv[7] = (m[1] * m[6] - m[0] * m[7]) * r;
-  inv[8] = (m[0] * m[4] - m[1] * m[3]) * r;
-}
-
-// float64 cell rows and inverse of conformer c, by thread 0 into shared memory
-__device__ __forceinline__ void load_cell(const MdArgs& a, int c, double* cell, double* inv) {
-  if (threadIdx.x == 0 && a.cells) {
-    const float* f = a.cells + (size_t)c * a.cell_stride;
-    for (int k = 0; k < 9; ++k) cell[k] = (double)f[k];
-    invert3(cell, inv);
-  }
-}
-
-// float32 coordinates of master position x: wrapped into the cell (fractional coordinates minus their floor) when
-// periodic, so that the float32 copy never holds a far-away image
-__device__ __forceinline__ void write_coords(const MdArgs& a, size_t i, double x, double y, double z, bool periodic,
-                                             const double* cell, const double* inv) {
-  if (periodic) {
-    const double f0 = floor(x * inv[0] + y * inv[3] + z * inv[6]);
-    const double f1 = floor(x * inv[1] + y * inv[4] + z * inv[7]);
-    const double f2 = floor(x * inv[2] + y * inv[5] + z * inv[8]);
-    x -= f0 * cell[0] + f1 * cell[3] + f2 * cell[6];
-    y -= f0 * cell[1] + f1 * cell[4] + f2 * cell[7];
-    z -= f0 * cell[2] + f1 * cell[5] + f2 * cell[8];
-  }
-  a.coords[3 * i + 0] = (float)x;
-  a.coords[3 * i + 1] = (float)y;
-  a.coords[3 * i + 2] = (float)z;
-}
-
-// fixed-shape tree over the block (blockDim.x == MD_BLOCK): sum of `v`, max of `w`; thread 0 gets the results
-__device__ __forceinline__ void block_reduce(double& v, double& w, double* sv, double* sw) {
-  sv[threadIdx.x] = v;
-  sw[threadIdx.x] = w;
-  __syncthreads();
-#pragma unroll
-  for (int s = MD_BLOCK / 2; s > 0; s >>= 1) {
-    if (threadIdx.x < s) {
-      sv[threadIdx.x] += sv[threadIdx.x + s];
-      sw[threadIdx.x] = fmax(sw[threadIdx.x], sw[threadIdx.x + s]);
-    }
-    __syncthreads();
-  }
-  v = sv[0];
-  w = sw[0];
-}
-
 // launch 1 of a step: the final half kick and the per-block partial sums (grid: blocks per conformer x conformers)
 __global__ void __launch_bounds__(MD_BLOCK) k_md_finish(const __grid_constant__ MdArgs a) {
   __shared__ double sv[MD_BLOCK], sw[MD_BLOCK];
@@ -161,7 +102,7 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_finish(const __grid_constant__ 
       if (a.force_stdev) fmax_ = (double)a.force_stdev[i];
     }
   }
-  block_reduce(ke, fmax_, sv, sw);
+  block_reduce<1>(&ke, fmax_, sv, sw);
   if (threadIdx.x == 0) {
     double* p = s.partials + 2 * ((size_t)c * gridDim.x + blockIdx.x);
     p[0] = ke;
@@ -241,7 +182,7 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_start(const __grid_constant__ M
     __syncthreads();
     if (threadIdx.x == 0) rescale_cell(a, c, t, par, tot, cell, inv);
   } else {
-    load_cell(a, c, cell, inv);
+    load_cell(a.cells, a.cell_stride, c, cell, inv);
   }
   __syncthreads();
   // stop_step[c] is written below by block 0 of this conformer only, and only with the value t: a block that reads it
@@ -324,7 +265,7 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_start(const __grid_constant__ M
   s.v[3 * i + 0] = vx;
   s.v[3 * i + 1] = vy;
   s.v[3 * i + 2] = vz;
-  write_coords(a, i, x, y, z, npt || a.cells, cell, inv);
+  write_coords(a.coords, i, x, y, z, npt || a.cells, cell, inv);
 }
 
 // one CTA per conformer: optional removal of the centre-of-mass momentum, then the coordinates of step 0
@@ -340,7 +281,7 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_init(const __grid_constant__ Md
         const double im = s.inv_mass[base + j];
         if (im > 0.0) p += (k < 3 ? s.v[3 * (base + j) + k] : 1.0) / im;
       }
-      block_reduce(p, unused, sv, sw);
+      block_reduce<1>(&p, unused, sv, sw);
       if (threadIdx.x == 0) tot[k] = p;
       __syncthreads();   // (sv is reused by the next reduction)
     }
@@ -349,11 +290,11 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_init(const __grid_constant__ Md
         for (int k = 0; k < 3; ++k) s.v[3 * (base + j) + k] -= tot[k] / tot[3];
     }
   }
-  load_cell(a, c, cell, inv);
+  load_cell(a.cells, a.cell_stride, c, cell, inv);
   __syncthreads();
   for (int j = threadIdx.x; j < A; j += MD_BLOCK) {
     const size_t i = base + j;
-    write_coords(a, i, s.x[3 * i + 0], s.x[3 * i + 1], s.x[3 * i + 2], a.cells, cell, inv);
+    write_coords(a.coords, i, s.x[3 * i + 0], s.x[3 * i + 1], s.x[3 * i + 2], a.cells, cell, inv);
   }
 }
 

@@ -1,0 +1,74 @@
+// Pieces shared by the device loops of md.cu (MD integrators) and opt.cu (FIRE): the float64 cell inverse, the float32
+// coordinates of a master position wrapped into the cell, and the fixed-shape block tree their per-block partial sums
+// go through.
+#pragma once
+#include "common.cuh"
+
+namespace ani {
+
+// inverse of the cell rows m (frac = r @ inv)
+__device__ __forceinline__ void invert3(const double* m, double* inv) {
+  const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6];
+  const double det = m[0] * c00 + m[1] * c01 + m[2] * c02;
+  const double r = 1.0 / det;
+  inv[0] = c00 * r;
+  inv[1] = (m[2] * m[7] - m[1] * m[8]) * r;
+  inv[2] = (m[1] * m[5] - m[2] * m[4]) * r;
+  inv[3] = c01 * r;
+  inv[4] = (m[0] * m[8] - m[2] * m[6]) * r;
+  inv[5] = (m[2] * m[3] - m[0] * m[5]) * r;
+  inv[6] = c02 * r;
+  inv[7] = (m[1] * m[6] - m[0] * m[7]) * r;
+  inv[8] = (m[0] * m[4] - m[1] * m[3]) * r;
+}
+
+// float64 cell rows and inverse of conformer c (f32 rows at cells + c * stride; nullptr = open), by thread 0 into
+// shared memory
+__device__ __forceinline__ void load_cell(const float* cells, int stride, int c, double* cell, double* inv) {
+  if (threadIdx.x == 0 && cells) {
+    const float* f = cells + (size_t)c * stride;
+    for (int k = 0; k < 9; ++k) cell[k] = (double)f[k];
+    invert3(cell, inv);
+  }
+}
+
+// float32 coordinates of master position x of atom i: wrapped into the cell (fractional coordinates minus their floor)
+// when periodic, so that the float32 copy never holds a far-away image
+__device__ __forceinline__ void write_coords(float* coords, size_t i, double x, double y, double z, bool periodic,
+                                             const double* cell, const double* inv) {
+  if (periodic) {
+    const double f0 = floor(x * inv[0] + y * inv[3] + z * inv[6]);
+    const double f1 = floor(x * inv[1] + y * inv[4] + z * inv[7]);
+    const double f2 = floor(x * inv[2] + y * inv[5] + z * inv[8]);
+    x -= f0 * cell[0] + f1 * cell[3] + f2 * cell[6];
+    y -= f0 * cell[1] + f1 * cell[4] + f2 * cell[7];
+    z -= f0 * cell[2] + f1 * cell[5] + f2 * cell[8];
+  }
+  coords[3 * i + 0] = (float)x;
+  coords[3 * i + 1] = (float)y;
+  coords[3 * i + 2] = (float)z;
+}
+
+// fixed-shape tree over the block (blockDim.x == ANI_MD_BLOCK): the sums of v[0..NS), the max of w; thread 0 gets the
+// results.  sv holds NS * ANI_MD_BLOCK doubles, sw ANI_MD_BLOCK.
+template <int NS>
+__device__ __forceinline__ void block_reduce(double* v, double& w, double* sv, double* sw) {
+#pragma unroll
+  for (int k = 0; k < NS; ++k) sv[k * ANI_MD_BLOCK + threadIdx.x] = v[k];
+  sw[threadIdx.x] = w;
+  __syncthreads();
+#pragma unroll
+  for (int s = ANI_MD_BLOCK / 2; s > 0; s >>= 1) {
+    if (threadIdx.x < s) {
+#pragma unroll
+      for (int k = 0; k < NS; ++k) sv[k * ANI_MD_BLOCK + threadIdx.x] += sv[k * ANI_MD_BLOCK + threadIdx.x + s];
+      sw[threadIdx.x] = fmax(sw[threadIdx.x], sw[threadIdx.x + s]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int k = 0; k < NS; ++k) v[k] = sv[k * ANI_MD_BLOCK];
+  w = sw[0];
+}
+
+}  // namespace ani

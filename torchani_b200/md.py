@@ -82,20 +82,26 @@ def maxwell_boltzmann(masses, temperature, seed: int = 0) -> np.ndarray:
     return v if batch else v[0]
 
 
-class _Dynamics:
-    """The device MD loop shared by ``VelocityVerlet`` and ``Langevin`` (see the module docstring)."""
+class _DeviceLoop:
+    """The machinery every device loop shares (the MD integrators here, FIRE in ``optimize``): the model's engine with a
+    workspace of its own, the initial force step, the status check with the switch to the 3 x bfloat16 build and the
+    redo of the work from a saved state, and K steps -- the loop's own launches (``_integrate``) and the fused force
+    step -- captured into one CUDA graph.
 
-    integrator = _lib.MD_VERLET
+    A subclass holds its state in ``_head`` (restored on a redo; ``_backup`` is the saved copy), the records a replay
+    copies to the host in ``_rec`` (to ``_h_rec``), and defines ``_init_launch(reset)`` (the coordinates of the current
+    state and, with ``reset``, its initial values), ``_integrate()`` and ``_collect(t0, k)``."""
 
-    def __init__(self, model, atomic_numbers, positions, masses, dt: float, temperature, friction, seed: int,
-                 cell, pbc, velocities, steps_per_replay: int, record_every: int, record_velocities: bool,
-                 qbc_stop, zero_momentum: bool, barostat: tp.Optional[tp.Tuple[np.ndarray, float, np.ndarray]] = None):
+    isobaric = False   # the force step accumulates the virial, and the cells are the loop's (LangevinNPT)
+    qbc = False        # the force step is the query-by-committee step
+    _what = "the device MD loop"
+
+    def _set_system(self, model, atomic_numbers, cell, pbc, steps_per_replay: int) -> tp.Optional[np.ndarray]:
+        """Model, device, species, PBC and the fixed cell (``per_conf``, ``_cell32``); returns the float64 cell."""
         dev = next(model.buffers()).device
         if dev.type != "cuda":
-            raise ValueError("the device MD loop needs a model on a CUDA device")
+            raise ValueError(f"{self._what} needs a model on a CUDA device")
         self.model, self.device = model, dev
-        if not (math.isfinite(dt) and dt > 0):
-            raise ValueError(f"dt must be > 0 fs, got {dt}")
         pb = np.asarray(pbc if not isinstance(pbc, Tensor) else pbc.cpu(), dtype=bool).reshape(-1)
         if pb.size not in (1, 3) or (pb.any() and not pb.all()):
             raise ValueError("partial PBC is not supported: the system is fully periodic or open")
@@ -106,9 +112,134 @@ class _Dynamics:
                                        else atomic_numbers.cpu()))
         C_ = z.shape[0] if z.dim() == 2 else 1
         z = z.reshape(C_, -1).to(dev)
-        A = z.shape[1]
-        self.n_conf, self.n_per_conf, n = C_, A, C_ * A
+        self.n_conf, self.n_per_conf = C_, z.shape[1]
         self.species = model.species_converter(z, nop=not model.periodic_table_index)
+        self.K = int(steps_per_replay)
+        # the cell, in the form the engine takes it
+        self.per_conf = False
+        self._cell32 = None
+        if not self.pbc:
+            return None
+        c64 = np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float64)
+        c = torch.as_tensor(c64.astype(np.float32))
+        if c.dim() == 3 and C_ == 1:
+            c = c.reshape(3, 3)
+        self.per_conf = conformer_cells(c, C_)
+        self._cell32 = c.to(dev)
+        return c64
+
+    # -- engine and workspace ----------------------------------------------------------------
+    def _attach_engine(self) -> None:
+        eng = self.model.engine(self.device)
+        if eng.skin > 0:
+            raise ValueError(f"{self._what} rebuilds the bucket grid every step: Verlet-skin reuse "
+                             "(Engine.skin > 0) is not supported")
+        if any(w.reducer is not None for w in eng._ws.values()):
+            raise ValueError(f"{self._what} runs on one GPU: this engine is sharded")
+        eng.check_pair_cutoffs(self.pbc)
+        # a workspace of its own: between two runs it holds the forces of the current positions
+        ws = eng.new_workspace(self.n_conf, self.n_per_conf)
+        if self.pbc and self.n_conf > 1:
+            ws.make_periodic()
+        ws.species_i32.copy_(self.species.reshape(-1))
+        if self.isobaric:
+            pass   # the float32 cell(s) of the current master cell, written by _begin
+        elif self.per_conf:
+            ws.cells.copy_(self._cell32.reshape(self.n_conf, 9))
+        elif self.pbc:
+            ws.cell.copy_(self._cell32.reshape(-1))
+        self.engine, self.ws = eng, ws
+        self._graph = None
+        self._attached()
+
+    def _attached(self) -> None:
+        """What a loop adds to a newly attached engine and workspace."""
+
+    def _begin(self, reset: bool) -> None:
+        """Write the float32 coordinates of the current positions and run the force step there (eagerly); on an operand
+        range overflow switch to the 3 x bfloat16 build, restore the state and start again."""
+        while True:
+            self._backup.copy_(self._head)
+            self._init_launch(reset)
+            self._force_step()
+            self._h_status.copy_(self.ws.status, non_blocking=True)
+            torch.cuda.current_stream(self.device).synchronize()
+            if not self._switched():
+                return
+            self._head.copy_(self._backup)
+
+    def _stream(self) -> int:
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def _switched(self) -> bool:
+        """Raise for the status word of the last force steps as Engine.check_status does; if the 2 x fp16 operand
+        format ran out of range, move to the 3 x bfloat16 build instead and return True (the caller redoes the work)."""
+        if int(self._h_status[0]) == 0:
+            return False
+        try:
+            self.engine.check_status(self.ws)
+        except _lib.OperandRangeError:
+            nets = self.model.neural_networks
+            if nets._variant == "bf16x3" or not _lib.available("bf16x3"):
+                raise
+            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this model "
+                          "to the 3 x bfloat16 build of the library")
+            nets.use_variant("bf16x3")
+            self._attach_engine()
+            return True
+        return False
+
+    # -- the loop -------------------------------------------------------------------------------
+    def _force_step(self) -> None:
+        self.engine._launch(self.ws, self.pbc, True, 0, self.ws.n, False, want_virial=self.isobaric,
+                            conformer_cells=self.per_conf, members=self.qbc)
+
+    def _body(self, k: int) -> None:
+        """k steps on the stream (graph-capturable): save the state, k x (the loop's launches, force step), copies
+        out."""
+        self._backup.copy_(self._head)
+        for _ in range(k):
+            self._integrate()
+            self._force_step()
+        self._h_rec.copy_(self._rec, non_blocking=True)
+        self._h_status.copy_(self.ws.status, non_blocking=True)
+
+    def _advance(self, k: int) -> None:
+        """k steps: one replay of the captured K-step graph (k == K) or eager launches of the same sequence."""
+        while True:
+            if k == self.K and self.engine.cuda_graph:
+                if self._graph is None:
+                    self.engine.note_composition(self.ws)
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        self._body(k)
+                    self._graph = g
+                self._graph.replay()
+            else:
+                self._body(k)
+            torch.cuda.current_stream(self.device).synchronize()
+            if not self._switched():
+                break
+            self._head.copy_(self._backup)   # redo the replay on the new build from the state it started with
+            self._begin(False)
+        self._collect(self.step, k)
+        self.step += k
+
+
+class _Dynamics(_DeviceLoop):
+    """The device MD loop shared by ``VelocityVerlet`` and ``Langevin`` (see the module docstring)."""
+
+    integrator = _lib.MD_VERLET
+
+    def __init__(self, model, atomic_numbers, positions, masses, dt: float, temperature, friction, seed: int,
+                 cell, pbc, velocities, steps_per_replay: int, record_every: int, record_velocities: bool,
+                 qbc_stop, zero_momentum: bool, barostat: tp.Optional[tp.Tuple[np.ndarray, float, np.ndarray]] = None):
+        if not (math.isfinite(dt) and dt > 0):
+            raise ValueError(f"dt must be > 0 fs, got {dt}")
+        self.isobaric = barostat is not None
+        c64 = self._set_system(model, atomic_numbers, cell, pbc, steps_per_replay)
+        dev, C_, A = self.device, self.n_conf, self.n_per_conf
+        n = C_ * A
         real = (self.species >= 0).cpu().numpy()
         m = np.asarray(masses, dtype=np.float64)
         m = np.broadcast_to(m.reshape(-1, A), (C_, A))
@@ -125,32 +256,20 @@ class _Dynamics:
             if not (np.isfinite(g) & (g >= 0)).all():
                 raise ValueError("friction must be >= 0 (1 / fs)")
         self.qbc = qbc_stop is not None
-        self.isobaric = barostat is not None
         e_thr, f_thr = (None, None) if qbc_stop is None else qbc_stop
         e_thr = np.broadcast_to(np.asarray(math.inf if e_thr is None else e_thr, dtype=np.float64).reshape(-1), (C_,))
         f_thr = np.broadcast_to(np.asarray(math.inf if f_thr is None else f_thr, dtype=np.float64).reshape(-1), (C_,))
-        self.K = int(steps_per_replay)
         self.record_every = int(record_every)
         if self.K < 1 or self.record_every < 0:
             raise ValueError("steps_per_replay must be >= 1 and record_every >= 0")
         self.dt = float(dt)
 
-        # the cell, in the form the engine takes it
-        self.per_conf = False
-        self._cell32 = None
-        if self.pbc:
-            c64 = np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float64)
-            c = torch.as_tensor(c64.astype(np.float32))
-            if c.dim() == 3 and C_ == 1:
-                c = c.reshape(3, 3)
-            self.per_conf = conformer_cells(c, C_)
-            if self.isobaric and C_ > 1 and not self.per_conf:   # every replica's box evolves on its own: grid mode 3
-                c, self.per_conf = c.expand(C_, 3, 3).contiguous(), True
-            self._cell32 = c.to(dev)
-            if self.isobaric:
-                c64 = np.broadcast_to(c64.reshape(-1, 3, 3), (C_, 3, 3))
-                if not (np.isfinite(c64).all() and (np.abs(np.linalg.det(c64)) > 0).all()):
-                    raise ValueError("constant pressure needs a finite cell of volume > 0 for every conformer")
+        if self.isobaric and self.pbc:
+            if C_ > 1 and not self.per_conf:   # every replica's box evolves on its own: grid mode 3
+                self._cell32, self.per_conf = self._cell32.expand(C_, 3, 3).contiguous(), True
+            c64 = np.broadcast_to(c64.reshape(-1, 3, 3), (C_, 3, 3))
+            if not (np.isfinite(c64).all() and (np.abs(np.linalg.det(c64)) > 0).all()):
+                raise ValueError("constant pressure needs a finite cell of volume > 0 for every conformer")
 
         f64 = dict(dtype=torch.float64, device=dev)
         # [x 3n | v 3n | counter 2 | master cells 2 C 9 (NPT) | stop_step C | thermo K C 4 | frames | NPT records K C 2 |
@@ -218,34 +337,15 @@ class _Dynamics:
         self._npt_rec: tp.List[np.ndarray] = []
         self._frame_cells: tp.List[np.ndarray] = []
         self._graph: tp.Optional[torch.cuda.CUDAGraph] = None
+        self._zero_momentum = bool(zero_momentum)
         with torch.cuda.device(dev):
             self._attach_engine()
-            self._begin(bool(zero_momentum))
+            self._begin(True)
 
-    # -- engine and workspace ----------------------------------------------------------------
-    def _attach_engine(self) -> None:
-        eng = self.model.engine(self.device)
-        if eng.skin > 0:
-            raise ValueError("the device MD loop rebuilds the bucket grid every step: Verlet-skin reuse "
-                             "(Engine.skin > 0) is not supported")
-        if any(w.reducer is not None for w in eng._ws.values()):
-            raise ValueError("the device MD loop runs on one GPU: this engine is sharded")
-        eng.check_pair_cutoffs(self.pbc)
-        # a workspace of its own: between two runs it holds the forces of the current positions
-        ws = eng.new_workspace(self.n_conf, self.n_per_conf)
-        if self.pbc and self.n_conf > 1:
-            ws.make_periodic()
-        ws.species_i32.copy_(self.species.reshape(-1))
+    def _attached(self) -> None:
+        ws = self.ws
         if self.qbc:
-            eng.members_buffers(ws)
-        if self.isobaric:
-            pass   # the float32 cell(s) of the current master cell, written by _begin
-        elif self.per_conf:
-            ws.cells.copy_(self._cell32.reshape(self.n_conf, 9))
-        elif self.pbc:
-            ws.cell.copy_(self._cell32.reshape(-1))
-        self.engine, self.ws = eng, ws
-        self._graph = None
+            self.engine.members_buffers(ws)
         if self.isobaric:
             b = _lib.MDBarostat()
             b.master, b.params, b.virial = ptr(self._master), ptr(self.baro_params), ptr(ws.virial)
@@ -254,50 +354,19 @@ class _Dynamics:
             b.virial_slots = _lib.ANI_VIRIAL_SLOTS
             self._baro = b
 
-    def _begin(self, zero_momentum: bool) -> None:
-        """Write the float32 coordinates of the current positions and run the force step there (eagerly); on an operand
-        range overflow switch to the 3 x bfloat16 build, restore the state and start again."""
-        while True:
-            self._backup.copy_(self._head)
-            if self.isobaric:   # the float32 cell(s) of the current step's master cell
-                h = self._master[self.step % 2]
-                if self.per_conf:
-                    self.ws.cells.copy_(h.reshape(self.n_conf, 9))
-                else:
-                    self.ws.cell.copy_(h.reshape(-1))
-            mode = 2 if self.per_conf else (1 if self.pbc else 0)
-            check(self.engine.lib.ani_b200_md_init(
-                C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, mode,
-                int(zero_momentum), ptr(self.ws.coords), self._stream()), "md_init")
-            self._force_step()
-            self._h_status.copy_(self.ws.status, non_blocking=True)
-            torch.cuda.current_stream(self.device).synchronize()
-            if not self._switched():
-                return
-            self._head.copy_(self._backup)
+    def _init_launch(self, reset: bool) -> None:
+        """ani_b200_md_init (with the momentum removal when asked for, at the start only)."""
+        if self.isobaric:   # the float32 cell(s) of the current step's master cell
+            h = self._master[self.step % 2]
+            if self.per_conf:
+                self.ws.cells.copy_(h.reshape(self.n_conf, 9))
+            else:
+                self.ws.cell.copy_(h.reshape(-1))
+        mode = 2 if self.per_conf else (1 if self.pbc else 0)
+        check(self.engine.lib.ani_b200_md_init(
+            C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, mode,
+            int(reset and self._zero_momentum), ptr(self.ws.coords), self._stream()), "md_init")
 
-    def _stream(self) -> int:
-        return torch.cuda.current_stream(self.device).cuda_stream
-
-    def _switched(self) -> bool:
-        """Raise for the status word of the last force steps as Engine.check_status does; if the 2 x fp16 operand
-        format ran out of range, move to the 3 x bfloat16 build instead and return True (the caller redoes the work)."""
-        if int(self._h_status[0]) == 0:
-            return False
-        try:
-            self.engine.check_status(self.ws)
-        except _lib.OperandRangeError:
-            nets = self.model.neural_networks
-            if nets._variant == "bf16x3" or not _lib.available("bf16x3"):
-                raise
-            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this model "
-                          "to the 3 x bfloat16 build of the library")
-            nets.use_variant("bf16x3")
-            self._attach_engine()
-            return True
-        return False
-
-    # -- the loop -------------------------------------------------------------------------------
     def _integrate(self) -> None:
         """The integrator launches of one step (ani_b200_md_step: finish step t, start step t + 1)."""
         ws, L = self.ws, self.engine.lib
@@ -314,40 +383,6 @@ class _Dynamics:
             rc = L.ani_b200_md_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), qbc, stdev,
                                     ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
         check(rc, "md_step")
-
-    def _force_step(self) -> None:
-        self.engine._launch(self.ws, self.pbc, True, 0, self.ws.n, False, want_virial=self.isobaric,
-                            conformer_cells=self.per_conf, members=self.qbc)
-
-    def _body(self, k: int) -> None:
-        """k MD steps on the stream (graph-capturable): save the state, k x (integrator, force step), copies out."""
-        self._backup.copy_(self._head)
-        for _ in range(k):
-            self._integrate()
-            self._force_step()
-        self._h_rec.copy_(self._rec, non_blocking=True)
-        self._h_status.copy_(self.ws.status, non_blocking=True)
-
-    def _advance(self, k: int) -> None:
-        """k steps: one replay of the captured K-step graph (k == K) or eager launches of the same sequence."""
-        while True:
-            if k == self.K and self.engine.cuda_graph:
-                if self._graph is None:
-                    self.engine.note_composition(self.ws)
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
-                        self._body(k)
-                    self._graph = g
-                self._graph.replay()
-            else:
-                self._body(k)
-            torch.cuda.current_stream(self.device).synchronize()
-            if not self._switched():
-                break
-            self._head.copy_(self._backup)   # redo the replay on the new build from the state it started with
-            self._begin(False)
-        self._collect(self.step, k)
-        self.step += k
 
     def _collect(self, t0: int, k: int) -> None:
         C_, K = self.n_conf, self.K
