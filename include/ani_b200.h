@@ -930,6 +930,56 @@ int ani_b200_opt_step(const ani_opt_state* state, const float* grad, const doubl
                       float* coords, void* stream);
 int ani_b200_opt_step_cells(const ani_opt_state* state, const float* grad, const double* energies,
                             const float* lattice, float* coords, void* stream);
+/*  Variable cell (ani_b200_opt_cell_step): FIRE on the degrees of freedom of ASE's FrechetCellFilter, every conformer  */
+/*    fully periodic, over A + 3 rows: A atom rows u_i = F^-1 r_i (state->x holds u) and 3 cell rows d = c logm(F),     */
+/*    where F is the deformation gradient (cell h = h0 F^T, rows are lattice vectors) and c = params[1].  Per conformer  */
+/*    and step t, with W the force step's virial (its slots summed in a fixed order, Hartree), V = |det h|, L = d / c:  */
+/*      atom rows   g_i = F^T f_i  (f = -dE/dr * force_scale, eV / A)                                                 */
+/*      cell rows   Phi = D_expm(L^T)[G] / c,  G = -(W + p0 V I) F^-T * params[2]   (the Frechet derivative of expm at  */
+/*                  L^T in the direction G: -dH/dd of the enthalpy H = E + p0 V, in eV with params[2] = HARTREE_TO_EV) */
+/*                  projection 1: Phi -> (tr Phi / 3) I (hydrostatic strain);  2: Phi -> Phi - (tr Phi / 3) I          */
+/*                  (constant volume)                                                                                */
+/*    and then ani_b200_opt_step's FIRE over the A + 3 rows: P, F2, V2 and fmax include the cell rows, the maxstep      */
+/*    clamp is over all of them, and a converged conformer freezes its cell too.  d(t+1) = d + s v_cell',               */
+/*    F(t+1) = expm(d(t+1) / c), u(t+1) = u + s v'; the f32 coords of F(t+1) u(t+1) are wrapped into the               */
+/*    float32-rounded h0 F(t+1)^T, which is also written to cell_out for the next force step (never read by this        */
+/*    step).  Both exponentials run in float64 (Taylor series with scaling and squaring, ~1e-15 relative).             */
+/*    ani_opt_cell (device pointers):                                                                                 */
+/*      master      f64[2][n_conf][ANI_OPT_CELL_MASTER] {d, v_cell, F} (3 x 3 each, row-major) by step parity: step t   */
+/*                  reads slot t % 2 and block 0 writes slot (t + 1) % 2 (v_cell too: every block of step t reads it)   */
+/*      h0          f64[n_conf][9] the cell of construction (rows)                                                    */
+/*      params      f64[n_conf][ANI_OPT_CELL_PARAMS] {p0 (Hartree / A^3), c (> 0), the unit of the cell forces per     */
+/*                  Hartree (HARTREE_TO_EV, as force_scale)}                                                           */
+/*      cell_out    f32 cell rows of conformer c at cell_out + c * cell_stride (>= 9): the workspace's cell, or its     */
+/*                  cells of grid mode 3                                                                              */
+/*      virial      f64[n_conf][virial_slots][9] the force step's virial slots                                         */
+/*      cell_force  f64[n_conf][9] scratch: Phi of step t, written by the first launch, read by the second           */
+/*      record      f64[record_rows][n_conf][ANI_OPT_CELL_RECORD] {V (A^3), -tr W / (3 V) (Hartree / A^3),            */
+/*                  H = E + p0 V (Hartree)} of step t, in row t % record_rows, beside state->record                    */
+/*      projection  0 none, 1 hydrostatic strain, 2 constant volume                                                   */
+/*  ani_b200_opt_cell_init  one launch: with reset, v = 0, the scalars of slot counter[0] % 2 = {dt0, astart, 0} and    */
+/*                     the master slot counter[0] % 2 = {0, 0, I}; then, from that slot's F, the f32 cell h0 F^T to     */
+/*                     cell_out and the f32 coords of F u wrapped into it.                                            */
+/*  ani_b200_opt_cell_step  after the force step at u(t), d(t) (grad, energies, and the virial slots): two launches,   */
+/*                     the same two as ani_b200_opt_step.  Sums are float64 in a fixed order without atomics: the same  */
+/*                     state and forces give the same bits.                                                           */
+#define ANI_OPT_CELL_MASTER 27
+#define ANI_OPT_CELL_PARAMS 3
+#define ANI_OPT_CELL_RECORD 3
+typedef struct ani_opt_cell {
+  double* master;
+  const double* h0;
+  const double* params;
+  float* cell_out;
+  const double* virial;
+  double* cell_force;
+  double* record;
+  int32_t cell_stride, virial_slots, projection, pad_;
+} ani_opt_cell;
+int ani_b200_opt_cell_init(const ani_opt_state* state, const ani_opt_cell* cell, int reset, float* coords,
+                           void* stream);
+int ani_b200_opt_cell_step(const ani_opt_state* state, const ani_opt_cell* cell, const float* grad,
+                           const double* energies, float* coords, void* stream);
 
 #ifdef __cplusplus
 }

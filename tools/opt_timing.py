@@ -20,7 +20,12 @@ of the last 500 steps (where float32 noise of the forces, not the geometry, sets
 
 Results go to --out as JSON, with the device name and power limit read in the same run.
 
-    python tools/opt_timing.py --out <dir> [--reps 5] [--steps 500]
+With --cell: variable-cell FIRE (optimize.CellFIRE) against fixed-cell FIRE per step at K = 1, 10 and 50 on water 1 k
+and on a 256-atom fcc Lennard-Jones crystal (a pure-LJ model: zero networks, sigma 2.5 A, eps 0.5 eV, smooth cutoff
+6.25 A), arms alternated over --reps rounds, medians; and the two launches of each step form alone under CUDA events
+(ani_b200_opt_cell_step against ani_b200_opt_step, 200 eager calls each).  Results go to opt_cell_timing.json.
+
+    python tools/opt_timing.py --out <dir> [--reps 5] [--steps 500] [--cell]
 """
 from __future__ import annotations
 
@@ -41,6 +46,13 @@ sys.path.insert(0, ROOT)
 
 def workload(name):
     from torchani_b200 import synthetic
+    if name == "ljfcc":   # 4 x 4 x 4 conventional cells, strained and sheared, atoms displaced by 0.02 A
+        a, shear = 1.56 * 2.5, np.array([[1.03, 0.04, 0.0], [-0.02, 0.98, 0.03], [0.01, 0.0, 1.02]])
+        base = np.array([[0, 0, 0], [0, 0.5, 0.5], [0.5, 0, 0.5], [0.5, 0.5, 0]])
+        cells = np.array([(i, j, k) for i in range(4) for j in range(4) for k in range(4)])
+        r = a * (cells[:, None] + base[None]).reshape(-1, 3) @ shear
+        r += 0.02 * np.random.default_rng(0).standard_normal(r.shape)
+        return np.zeros((1, len(r)), dtype=np.int64), r[None], 4 * a * np.eye(3) @ shear, True
     if name == "gdb256":
         sp, co = synthetic.conformer_batch(256)
         return sp.numpy(), co.double().numpy(), None, False
@@ -48,10 +60,13 @@ def workload(name):
     return idx.numpy(), co.double().numpy(), cell.double().numpy(), True
 
 
-def device_arm(model, name, K, steps):
+def device_arm(model, name, K, steps, variable_cell=False):
     from torchani_b200 import optimize
     sp, co, cell, pbc = workload(name)
-    opt = optimize.FIRE(model, sp, co, cell=cell, pbc=pbc, steps_per_replay=K)
+    if variable_cell:
+        opt = optimize.CellFIRE(model, sp, co, cell, steps_per_replay=K)
+    else:
+        opt = optimize.FIRE(model, sp, co, cell=cell, pbc=pbc, steps_per_replay=K)
     steps = steps // K * K
     opt.run(0.0, 2 * K)   # capture + warm-up
 
@@ -164,6 +179,44 @@ def floor(model, steps):
             "fmax_at": {str(s): float(f[s]) for s in (100, 300, 1000, 3000) if s < len(f)}}
 
 
+def lj_model():
+    """Zero networks, no self energies and one Lennard-Jones term (sigma 2.5 A, eps 0.5 eV, smooth cutoff 6.25 A)."""
+    from torchani_b200 import models, potentials
+    from torchani_b200.grad import HARTREE_TO_EV
+    base = models.ANI2x(seed=0)
+    with torch.no_grad():
+        for p in base.neural_networks.parameters():
+            p.zero_()
+    S = len(base.symbols)
+    lj = potentials.LennardJones(base.symbols, eps=[0.5 / HARTREE_TO_EV] * S, sigma=[2.5] * S, cutoff=6.25,
+                                 cutoff_fn="smooth")
+    return models.ANI(base.symbols, base.aev_computer, base.neural_networks, models.SelfEnergy(base.symbols, [0.0] * S),
+                      False, {"lj": lj}).cuda()
+
+
+def cell_main(args, model, result) -> None:
+    for name in ("water1k", "ljfcc"):
+        mdl = lj_model() if name == "ljfcc" else model
+        arms, opts = {}, {}
+        for K in (1, 10, 50):
+            for cell in (False, True):
+                key = f"{'CellFIRE' if cell else 'FIRE'} K={K}"
+                opts[key], arms[key] = device_arm(mdl, name, K, args.steps, cell)
+        times = {k: [] for k in arms}
+        for _ in range(args.reps):
+            for k, fn in arms.items():
+                times[k].append(fn())
+        rec = {k: {"ms_per_step": statistics.median(v), "spread_ms": [min(v), max(v)]} for k, v in times.items()}
+        rec["launches_ms_per_step"] = {"FIRE": fire_launch_ms(opts["FIRE K=50"]),
+                                       "CellFIRE": fire_launch_ms(opts["CellFIRE K=50"])}
+        result["workloads"][name] = rec
+        print(name, json.dumps(rec, indent=1), flush=True)
+    os.makedirs(args.out, exist_ok=True)
+    with open(os.path.join(args.out, "opt_cell_timing.json"), "w") as fh:
+        json.dump(result, fh, indent=1)
+    print(json.dumps(result))
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True)
@@ -172,6 +225,7 @@ def main() -> None:
     ap.add_argument("--max-steps", type=int, default=3000)
     ap.add_argument("--floor-steps", type=int, default=5000)
     ap.add_argument("--workloads", default="gdb256,water1k")
+    ap.add_argument("--cell", action="store_true", help="variable-cell FIRE against FIRE (see the docstring)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("opt_timing needs a GPU")
@@ -181,6 +235,9 @@ def main() -> None:
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
     result = {"device": torch.cuda.get_device_name(0), "nvidia_smi": smi, "steps": args.steps, "workloads": {}}
+    if args.cell:
+        cell_main(args, model, result)
+        return
     for name in args.workloads.split(","):
         arms, opts = {}, {}
         for K in (1, 10, 50):

@@ -130,6 +130,16 @@ class OptState(C.Structure):
         (k, C.c_int32) for k in ("n_conf", "n_per_conf", "record_rows", "pad_")]
 
 
+ANI_OPT_CELL_MASTER = 27
+ANI_OPT_CELL_PARAMS = 3
+ANI_OPT_CELL_RECORD = 3
+
+
+class OptCell(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in ("master", "h0", "params", "cell_out", "virial", "cell_force", "record")] + [
+        (k, C.c_int32) for k in ("cell_stride", "virial_slots", "projection", "pad_")]
+
+
 class D3Params(C.Structure):
     _fields_ = [
         ("cutoff_fn", C.c_int32), ("num_species", C.c_int32), ("cutoff", C.c_float), ("to_bohr", C.c_float),
@@ -222,6 +232,8 @@ _PROTOTYPES = {
     "ani_b200_opt_init": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "ani_b200_opt_step": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "ani_b200_opt_step_cells": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "ani_b200_opt_cell_init": (C.c_int, [_P, _P, _I, _P, _P]),
+    "ani_b200_opt_cell_step": (C.c_int, [_P, _P, _P, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

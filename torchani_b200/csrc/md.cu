@@ -69,11 +69,6 @@ __device__ __forceinline__ double md_normal(unsigned long long seed, long long s
   return sqrt(-2.0 * log(u1)) * cospi(2.0 * u2);
 }
 
-// determinant of the cell rows m
-__device__ __forceinline__ double det3(const double* m) {
-  return m[0] * (m[4] * m[8] - m[5] * m[7]) + m[1] * (m[5] * m[6] - m[3] * m[8]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
-}
-
 // launch 1 of a step: the final half kick and the per-block partial sums (grid: blocks per conformer x conformers)
 __global__ void __launch_bounds__(MD_BLOCK) k_md_finish(const __grid_constant__ MdArgs a) {
   __shared__ double sv[MD_BLOCK], sw[MD_BLOCK];

@@ -1,10 +1,15 @@
-// Pieces shared by the device loops of md.cu (MD integrators) and opt.cu (FIRE): the float64 cell inverse, the float32
-// coordinates of a master position wrapped into the cell, and the fixed-shape block tree their per-block partial sums
-// go through.
+// Pieces shared by the device loops of md.cu (MD integrators) and opt.cu (FIRE): the float64 cell determinant and
+// inverse, the float32 coordinates of a master position wrapped into the cell, and the fixed-shape block tree their
+// per-block partial sums go through.
 #pragma once
 #include "common.cuh"
 
 namespace ani {
+
+// determinant of the cell rows m
+__device__ __forceinline__ double det3(const double* m) {
+  return m[0] * (m[4] * m[8] - m[5] * m[7]) + m[1] * (m[5] * m[6] - m[3] * m[8]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
+}
 
 // inverse of the cell rows m (frac = r @ inv)
 __device__ __forceinline__ void invert3(const double* m, double* inv) {

@@ -23,7 +23,8 @@ The step of a conformer is clamped as a whole (ASE's global norm), not atom by a
 Units: ``fmax`` and ``log.fmax`` are in eV / A, ASE's unit, so ASE's thresholds and FIRE parameters keep their meaning
 (``maxstep`` in A).  ``energies`` is in Hartree and ``forces`` in Hartree / A, like every other output of the package.
 
-Every step rebuilds the bucket grid (no Verlet skin), and the cell stays fixed.
+Every step rebuilds the bucket grid (no Verlet skin).  ``FIRE`` keeps the cell fixed; ``CellFIRE`` relaxes the lattice
+vectors with the atoms, as ASE's ``FIRE(FrechetCellFilter(atoms))`` does (see its docstring).
 """
 from __future__ import annotations
 
@@ -37,10 +38,10 @@ from torch import Tensor
 
 from . import _lib
 from ._lib import check, ptr
-from .grad import HARTREE_TO_EV
+from .grad import BAR_TO_HARTREE_A3, HARTREE_TO_EV
 from .md import _DeviceLoop
 
-__all__ = ["FIRE", "Log", "HARTREE_TO_EV"]
+__all__ = ["FIRE", "CellFIRE", "Log", "CellLog", "HARTREE_TO_EV", "BAR_TO_HARTREE_A3"]
 
 
 class Log(tp.NamedTuple):
@@ -48,6 +49,16 @@ class Log(tp.NamedTuple):
     step: np.ndarray     # (S,) int64
     energy: np.ndarray   # (S, C) Hartree: the energy at the step's positions
     fmax: np.ndarray     # (S, C) eV / A: the largest force on a movable atom there
+
+
+class CellLog(tp.NamedTuple):
+    """One record per step and conformer of ``CellFIRE`` (steps ascending)."""
+    step: np.ndarray       # (S,) int64
+    energy: np.ndarray     # (S, C) Hartree
+    fmax: np.ndarray       # (S, C) eV / A: the largest row norm of the atom and cell forces (FrechetCellFilter's)
+    volume: np.ndarray     # (S, C) A^3
+    pressure: np.ndarray   # (S, C) bar: -tr W / (3 V), the virial pressure of the force step
+    enthalpy: np.ndarray   # (S, C) Hartree: E + p0 V
 
 
 class FIRE(_DeviceLoop):
@@ -88,7 +99,7 @@ class FIRE(_DeviceLoop):
             raise ValueError("n_min must be >= 0")
         if int(steps_per_replay) < 1:
             raise ValueError("steps_per_replay must be >= 1")
-        self._set_system(model, atomic_numbers, cell, pbc, steps_per_replay)
+        c64 = self._set_system(model, atomic_numbers, cell, pbc, steps_per_replay)
         dev, C_, A = self.device, self.n_conf, self.n_per_conf
         n = C_ * A
         real = (self.species >= 0).cpu().numpy()
@@ -102,20 +113,24 @@ class FIRE(_DeviceLoop):
         self.fixed = fix
 
         f64 = dict(dtype=torch.float64, device=dev)
-        # [x 3n | v 3n | scalars 2 C 3 | counter 2 | conv_step C | records K C 3]: the head up to conv_step is what a
-        # redone replay restores, the tail from conv_step on is what a replay copies to the host
-        ns = 2 * C_ * _lib.ANI_OPT_SCALARS
-        head = 6 * n + ns + 2 + C_
-        self._buf = torch.zeros(head + self.K * C_ * _lib.ANI_OPT_RECORD, **f64)
+        # [x 3n | v 3n | scalars 2 C 3 | counter 2 | (CellFIRE: master 2 C 27) | conv_step C | records K C 3 |
+        # (CellFIRE: cell records K C 3)]: the head up to conv_step is what a redone replay restores, the tail from
+        # conv_step on is what a replay copies to the host
+        ns, nm = 2 * C_ * _lib.ANI_OPT_SCALARS, C_ * self._master_words
+        head = 6 * n + ns + 2 + nm + C_
+        n_rec = self.K * C_ * _lib.ANI_OPT_RECORD
+        self._buf = torch.zeros(head + n_rec + self.K * C_ * self._cell_record_words, **f64)
         self.x = self._buf[:3 * n].view(C_, A, 3)
         self.v = self._buf[3 * n:6 * n].view(C_, A, 3)
         self._scalars = self._buf[6 * n:6 * n + ns].view(2, C_, _lib.ANI_OPT_SCALARS)
         self._counter = self._buf[6 * n + ns:6 * n + ns + 2].view(torch.int64)
+        self._master = self._buf[6 * n + ns + 2:6 * n + ns + 2 + nm]
         self._conv = self._buf[head - C_:head].view(torch.int64)
         self._rec = self._buf[head - C_:]
         self._head = self._buf[:head]
         self._backup = torch.empty_like(self._head)
-        self._record_dev = self._buf[head:]
+        self._record_dev = self._buf[head:head + n_rec]
+        self._cell_record_dev = self._buf[head + n_rec:]
         self._h_rec = torch.zeros(self._rec.numel(), dtype=torch.float64).pin_memory()
         self._h_status = torch.zeros(1, dtype=torch.int32).pin_memory()
         pos = torch.as_tensor(positions if not isinstance(positions, Tensor) else positions.detach().cpu()
@@ -138,9 +153,16 @@ class FIRE(_DeviceLoop):
         self._conv_host = np.full(C_, -1, dtype=np.int64)
         self._log: tp.List[np.ndarray] = []
         self._graph: tp.Optional[torch.cuda.CUDAGraph] = None
+        self._setup(c64)
         with torch.cuda.device(dev):
             self._attach_engine()
             self._begin(True)
+
+    _master_words = 0        # per conformer: state a redo restores beyond FIRE's own (CellFIRE's master)
+    _cell_record_words = 0   # per conformer and step: records beyond FIRE's own (CellFIRE's)
+
+    def _setup(self, cell64: tp.Optional[np.ndarray]) -> None:
+        """What a subclass adds to the state before the engine is attached."""
 
     # -- the device loop ------------------------------------------------------------------------
     def _init_launch(self, reset: bool) -> None:
@@ -165,7 +187,7 @@ class FIRE(_DeviceLoop):
         C_ = self.n_conf
         h = self._h_rec.numpy()
         rows = [(t0 + i) % self.K for i in range(k)]
-        self._log.append(h[C_:].reshape(self.K, C_, _lib.ANI_OPT_RECORD)[rows].copy())
+        self._log.append(h[C_:C_ + self._record_dev.numel()].reshape(self.K, C_, _lib.ANI_OPT_RECORD)[rows].copy())
         self._conv_host = h[:C_].view(np.int64).copy()
 
     def run(self, fmax: float = 0.05, steps: int = 1000,
@@ -230,4 +252,150 @@ class FIRE(_DeviceLoop):
         if not self._log:
             z = np.zeros((0, self.n_conf))
             return Log(np.zeros(0, dtype=np.int64), z, z.copy())
+        return self._as_log(np.concatenate(self._log))
+
+
+class CellFIRE(FIRE):
+    """FIRE over positions and lattice vectors: ASE's ``FIRE(FrechetCellFilter(atoms, scalar_pressure=...))`` on the
+    device, one relaxation per conformer of a fully periodic batch.
+
+    Per conformer, with h0 the cell at construction (rows are lattice vectors), F the deformation gradient (the cell is
+    h = h0 F^T), c = ``cell_factor`` and p0 = ``pressure``, FIRE runs over A + 3 rows:
+
+        atom rows   u_i = F^-1 r_i,        forces g_i = F^T f_i              (f = -dE/dr, eV / A)
+        cell rows   d = c logm F,          forces Phi = D_expm(L^T)[G] / c,  L = d / c,  G = -(W + p0 V I) F^-T
+        enthalpy    H = E + p0 V,          V = |det h|
+
+    W is the force step's virial (eV here), D_expm the Frechet derivative of the matrix exponential; g and Phi are
+    -dH/du and -dH/dd.  P, F2, V2, fmax and the maxstep clamp of ``FIRE`` include the cell rows, so ``fmax`` means what
+    it means for ASE's filtered ``Atoms``; a converged conformer keeps its positions and cell.
+
+    Args: those of ``FIRE`` (pbc is always fully periodic, and ``fixed`` is rejected: ASE's ``FixAtoms`` acts on
+    Cartesian positions, which the filter's coordinates do not express), and
+        cell: (3, 3) or (C, 3, 3) lattice vectors as rows; a shared cell of a batch becomes one cell per conformer
+        pressure: p0, bar (scalar or one per conformer; 1 eV / A^3 = 1.6021766208e6 bar)
+        cell_factor: c (scalar or one per conformer); default the number of real atoms, as ASE's
+        hydrostatic_strain: keep only the isotropic part (tr Phi / 3) I of the cell force: the shape is kept
+        constant_volume: keep only its traceless part: det F = 1
+    A box that shrinks below the cutoff raises ``ANI_STATUS_CELL_TOO_SMALL`` at the end of the replay.
+    """
+
+    isobaric = True   # the force step accumulates the virial, and the cells are the loop's
+    _what = "the device cell optimiser"
+    _master_words = 2 * _lib.ANI_OPT_CELL_MASTER
+    _cell_record_words = _lib.ANI_OPT_CELL_RECORD
+
+    def __init__(self, model, atomic_numbers, positions, cell, pbc=True, pressure=0.0, cell_factor=None,
+                 hydrostatic_strain: bool = False, constant_volume: bool = False, fixed=None, **fire):
+        pb = np.asarray(pbc if not isinstance(pbc, Tensor) else pbc.cpu(), dtype=bool).reshape(-1)
+        if cell is None or pb.size not in (1, 3) or not pb.all():
+            raise ValueError("variable-cell relaxation needs a fully periodic cell")
+        if fixed is not None:
+            raise ValueError("fixed atoms are not supported with a variable cell: the filter's coordinates do not "
+                             "express Cartesian constraints")
+        if hydrostatic_strain and constant_volume:
+            raise ValueError("hydrostatic_strain and constant_volume are mutually exclusive")
+        z = np.asarray(atomic_numbers if not isinstance(atomic_numbers, Tensor) else atomic_numbers.cpu())
+        n_conf = z.shape[0] if z.ndim == 2 else 1
+        h = np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float64)
+        if h.shape not in ((3, 3), (n_conf, 3, 3)) and not (n_conf == 1 and h.shape == (1, 3, 3)):
+            raise ValueError(f"cell must be (3, 3) or ({n_conf}, 3, 3), got {h.shape}")
+        h = np.broadcast_to(h.reshape(-1, 3, 3), (n_conf, 3, 3))
+        if not (np.isfinite(h).all() and (np.abs(np.linalg.det(h)) > 0).all()):
+            raise ValueError("variable-cell relaxation needs a finite cell of volume > 0 for every conformer")
+        p0 = np.broadcast_to(np.asarray(pressure, dtype=np.float64).reshape(-1), (n_conf,))
+        if not np.isfinite(p0).all():
+            raise ValueError("pressure must be finite (bar)")
+        n_real = (z.reshape(n_conf, -1) >= 0).sum(1).astype(np.float64)
+        cf = n_real if cell_factor is None else np.broadcast_to(
+            np.asarray(cell_factor, dtype=np.float64).reshape(-1), (n_conf,))
+        if not (np.isfinite(cf) & (cf > 0)).all():
+            raise ValueError("cell_factor must be > 0 (and every conformer needs a real atom)")
+        self._p0 = p0 * BAR_TO_HARTREE_A3
+        self._cell_factor = np.array(cf)
+        self._projection = 1 if hydrostatic_strain else (2 if constant_volume else 0)
+        # every conformer's cell evolves on its own: a batch always runs one cell per conformer (grid mode 3)
+        super().__init__(model, atomic_numbers, positions, cell=np.array(h, order="C") if n_conf > 1 else cell,
+                         pbc=True, **fire)
+
+    def _setup(self, cell64) -> None:
+        dev, C_ = self.device, self.n_conf
+        f64 = dict(dtype=torch.float64, device=dev)
+        # (a C-order copy: numpy's default copy of a broadcast keeps the conformer axis innermost)
+        self.h0 = torch.from_numpy(np.array(np.broadcast_to(cell64.reshape(-1, 3, 3), (C_, 3, 3)), order="C")).to(**f64)
+        par = np.stack([self._p0, self._cell_factor, np.full(C_, HARTREE_TO_EV)], 1)
+        self.cell_params = torch.from_numpy(par).to(**f64)
+        self._cell_force = torch.zeros(C_, 9, **f64)
+        self._master = self._master.view(2, C_, _lib.ANI_OPT_CELL_MASTER)
+
+    def _attached(self) -> None:
+        q = _lib.OptCell()
+        q.master, q.h0, q.params = ptr(self._master), ptr(self.h0), ptr(self.cell_params)
+        q.cell_out, q.cell_stride = (ptr(self.ws.cells) if self.per_conf else ptr(self.ws.cell)), 9
+        q.virial, q.virial_slots = ptr(self.ws.virial), _lib.ANI_VIRIAL_SLOTS
+        q.cell_force, q.record, q.projection = ptr(self._cell_force), ptr(self._cell_record_dev), self._projection
+        self._cell = q
+
+    def _init_launch(self, reset: bool) -> None:
+        """ani_b200_opt_cell_init: (with reset, v = 0, the initial scalars and F = I,) the float32 cell and coordinates
+        of the current state."""
+        check(self.engine.lib.ani_b200_opt_cell_init(C.byref(self._state), C.byref(self._cell), int(reset),
+                                                     ptr(self.ws.coords), self._stream()), "opt_cell_init")
+
+    def _integrate(self) -> None:
+        """The launches of one step (ani_b200_opt_cell_step: u(t), d(t) to u(t+1), d(t+1))."""
+        ws = self.ws
+        check(self.engine.lib.ani_b200_opt_cell_step(C.byref(self._state), C.byref(self._cell), ptr(ws.grad),
+                                                     ptr(ws.energies), ptr(ws.coords), self._stream()),
+              "opt_cell_step")
+
+    def _collect(self, t0: int, k: int) -> None:
+        super()._collect(t0, k)
+        h = self._h_rec.numpy()
+        rows = [(t0 + i) % self.K for i in range(k)]
+        cr = h[self.n_conf + self._record_dev.numel():].reshape(self.K, self.n_conf, _lib.ANI_OPT_CELL_RECORD)
+        self._log[-1] = np.concatenate([self._log[-1], cr[rows]], -1)
+
+    # -- results ----------------------------------------------------------------------------------
+    @property
+    def deformation(self) -> Tensor:
+        """(C, 3, 3) float64 deformation gradient F of the current step (device, a copy)."""
+        return self._master[self.step % 2, :, 18:].reshape(self.n_conf, 3, 3).clone()
+
+    @property
+    def positions(self) -> Tensor:
+        """(C, A, 3) float64 Cartesian positions r = F u of the current step, unwrapped (device)."""
+        return self.x @ self.deformation.transpose(1, 2)
+
+    @property
+    def cell(self) -> Tensor:
+        """(C, 3, 3) float64 cell h0 F^T of the current step, lattice vectors as rows (device)."""
+        return self.h0 @ self.deformation.transpose(1, 2)
+
+    @property
+    def volume(self) -> Tensor:
+        """(C,) float64 volume of the current cell, A^3 (device)."""
+        return torch.linalg.det(self.cell).abs()
+
+    @property
+    def stress(self) -> Tensor:
+        """(C, 3, 3) float64 W / V (Hartree / A^3) of the last force step, at the current positions and cell: the
+        convention of ``HostCalculator.calculate_with_stress``."""
+        w = self.ws.virial.view(self.n_conf, -1, 9).sum(1).view(self.n_conf, 3, 3)
+        return w / self.volume.view(-1, 1, 1)
+
+    @property
+    def enthalpies(self) -> Tensor:
+        """(C,) float64 E + p0 V (Hartree) of the current step (device)."""
+        return self.ws.energies + torch.from_numpy(self._p0).to(self.device) * self.volume
+
+    @staticmethod
+    def _as_log(r: np.ndarray) -> CellLog:
+        return CellLog(r[:, 0, 0].astype(np.int64), r[..., 1].copy(), r[..., 2].copy(), r[..., 3].copy(),
+                       r[..., 4] / BAR_TO_HARTREE_A3, r[..., 5].copy())
+
+    @property
+    def log(self) -> CellLog:
+        if not self._log:
+            return self._as_log(np.zeros((0, self.n_conf, _lib.ANI_OPT_RECORD + _lib.ANI_OPT_CELL_RECORD)))
         return self._as_log(np.concatenate(self._log))
