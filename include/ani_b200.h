@@ -980,6 +980,70 @@ int ani_b200_opt_cell_init(const ani_opt_state* state, const ani_opt_cell* cell,
                            void* stream);
 int ani_b200_opt_cell_step(const ani_opt_state* state, const ani_opt_cell* cell, const float* grad,
                            const double* energies, float* coords, void* stream);
+/*  L-BFGS (csrc/lbfgs.cu): ASE's ase.optimize.LBFGS without its line search, one independent optimisation per        */
+/*    conformer, with the direction from the compact representation of the inverse BFGS matrix (Byrd, Nocedal &      */
+/*    Schnabel, Math. Prog. 63 (1994)).  Units: A, eV, Hartree.  ani_lbfgs_state (device pointers; M = memory + 1):    */
+/*      x, x_prev, g_prev  f64[n][3] positions (unwrapped, input order), those of the last step and its gradient       */
+/*                  g = dE/dx * force_scale (eV / A)                                                                 */
+/*      s, y        f64[n_conf][M][n_per_conf][3] ring of the pairs s = x(t) - x(t-1), y = g(t) - g(t-1): with head    */
+/*                  the pairs ever stored and L = min(memory, head), chronological pair j is in slot (head - L + j) % M; */
+/*                  the spare slot takes the next pair before it is known whether y.s == 0                           */
+/*      sy, yy      f64[n_conf][M][M] slot-indexed s_i.y_j (for i not newer than j) and y_i.y_j                        */
+/*      coef        f64[n_conf][2][memory] scratch: a and b of the step (chronological)                               */
+/*      p           f64[n][3] scratch: the step's direction                                                          */
+/*      iter        i64[n_conf][2] {k, head}: the steps taken (ASE's iteration) and the pairs ever stored              */
+/*      force_scale f64[n] as in ani_opt_state                                                                        */
+/*      params      f64[n_conf][ANI_LBFGS_PARAMS] per conformer: maxstep (A), damping, H0 = 1 / alpha (A^2 / eV), the  */
+/*                  fmax threshold (eV / A); not read by the validation (device memory): the caller keeps them > 0     */
+/*      counter, conv_step, record (ANI_LBFGS_RECORD = {t, E, fmax}) as in ani_opt_state                               */
+/*      partials    f64[ANI_LBFGS_PARTIALS(n_conf, n_per_conf, memory)] scratch of ani_b200_lbfgs_step                  */
+/*      memory      1 .. ANI_LBFGS_MAX_MEMORY (R of the solve, memory^2 doubles, sits in shared memory)                */
+/*  ani_b200_lbfgs_init  with reset: x_prev = x, g_prev = 0, {k, head} = {0, 0}; then the f32 coords of x, wrapped     */
+/*                     into the cell (cell_mode as ani_b200_opt_init).  One launch.                                   */
+/*  ani_b200_lbfgs_step  after the force step at x(t) (grad f32[n][3] dE/dx, energies f64[n_conf]), four launches, per   */
+/*                     conformer with fmax(t) = max_i |g_i|:                                                          */
+/*                       record {t, E, fmax(t)};  fmax(t) < threshold (and running): conv_step = t, and from then on    */
+/*                       nothing of the conformer changes;  else                                                      */
+/*                       k >= 1: the pair s = x - x_prev, y = g - g_prev joins the history (the oldest leaves a full     */
+/*                               one), unless y.s == 0, where it is skipped                                           */
+/*                       p = -H g, H the inverse BFGS matrix of the live pairs with H0 (the two-loop recursion's p)     */
+/*                       x(t+1) = x + damping p min(1, maxstep / max_i |p_i|)  (the factor applies when >= maxstep)   */
+/*                       x_prev = x, g_prev = g, k += 1                                                               */
+/*                     then the f32 coords of x(t+1) (wrapped into `cell` f32[9] when not NULL), and t += 1.  Sums are   */
+/*                     float64 in a fixed order without atomics: the same state and forces give the same bits.          */
+/*  ani_b200_lbfgs_step_cells  the same with one cell per conformer: the lattice table of grid mode 3                  */
+/*                     (f32[n_conf][ANI_LATTICE_STRIDE], written by ani_b200_prepare_step_cells) in place of `cell`.    */
+#define ANI_LBFGS_PARAMS 4
+#define ANI_LBFGS_RECORD 3
+#define ANI_LBFGS_MAX_MEMORY 128
+#define ANI_LBFGS_TILE 32 /* atoms per tile of the dot sweep and per block of the direction launch */
+#define ANI_LBFGS_PARTIALS(n_conf, n_per_conf, memory) \
+  ((size_t)(n_conf) * (((n_per_conf) + ANI_LBFGS_TILE - 1) / ANI_LBFGS_TILE) * (4 * ((size_t)(memory) + 1) + 2))
+typedef struct ani_lbfgs_state {
+  double* x;
+  double* x_prev;
+  double* g_prev;
+  double* s;
+  double* y;
+  double* sy;
+  double* yy;
+  double* coef;
+  double* p;
+  long long* iter;
+  const double* force_scale;
+  const double* params;
+  long long* counter;
+  long long* conv_step;
+  double* record;
+  double* partials;
+  int32_t n_conf, n_per_conf, memory, record_rows;
+} ani_lbfgs_state;
+int ani_b200_lbfgs_init(const ani_lbfgs_state* state, const float* cells, int cell_mode, int reset, float* coords,
+                        void* stream);
+int ani_b200_lbfgs_step(const ani_lbfgs_state* state, const float* grad, const double* energies, const float* cell,
+                        float* coords, void* stream);
+int ani_b200_lbfgs_step_cells(const ani_lbfgs_state* state, const float* grad, const double* energies,
+                              const float* lattice, float* coords, void* stream);
 
 #ifdef __cplusplus
 }

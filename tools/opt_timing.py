@@ -25,7 +25,13 @@ and on a 256-atom fcc Lennard-Jones crystal (a pure-LJ model: zero networks, sig
 6.25 A), arms alternated over --reps rounds, medians; and the two launches of each step form alone under CUDA events
 (ani_b200_opt_cell_step against ani_b200_opt_step, 200 eager calls each).  Results go to opt_cell_timing.json.
 
-    python tools/opt_timing.py --out <dir> [--reps 5] [--steps 500] [--cell]
+With --lbfgs: L-BFGS (optimize.LBFGS, ASE's defaults, memory 100) against FIRE per step at K = 1, 10 and 50 on the GDB
+batch and water 1 k, the arms alternated over --reps rounds, medians; the four L-BFGS launches alone with a full
+history (after 110 steps; ani_b200_lbfgs_step under CUDA events, 200 eager calls) against the two FIRE launches; and
+the steps and wall time (K = 50) of both optimisers to fmax 0.05 eV / A on the GDB batch and to 1e-4 and 1e-6 eV / A
+on the 26-atom molecule of the floor run.  Results go to opt_lbfgs_timing.json.
+
+    python tools/opt_timing.py --out <dir> [--reps 5] [--steps 500] [--cell | --lbfgs]
 """
 from __future__ import annotations
 
@@ -60,10 +66,12 @@ def workload(name):
     return idx.numpy(), co.double().numpy(), cell.double().numpy(), True
 
 
-def device_arm(model, name, K, steps, variable_cell=False):
+def device_arm(model, name, K, steps, variable_cell=False, lbfgs=False):
     from torchani_b200 import optimize
     sp, co, cell, pbc = workload(name)
-    if variable_cell:
+    if lbfgs:
+        opt = optimize.LBFGS(model, sp, co, cell=cell, pbc=pbc, steps_per_replay=K)
+    elif variable_cell:
         opt = optimize.CellFIRE(model, sp, co, cell, steps_per_replay=K)
     else:
         opt = optimize.FIRE(model, sp, co, cell=cell, pbc=pbc, steps_per_replay=K)
@@ -217,6 +225,58 @@ def cell_main(args, model, result) -> None:
     print(json.dumps(result))
 
 
+def lbfgs_to_fmax(model, sp, co, cell, pbc, fmax, max_steps):
+    from torchani_b200 import optimize
+    out = {}
+    for cls in (optimize.FIRE, optimize.LBFGS):
+        cls(model, sp, co, cell=cell, pbc=pbc, steps_per_replay=50).run(0.0, 50)   # this shape's warm-up
+        opt = cls(model, sp, co, cell=cell, pbc=pbc, steps_per_replay=50)
+        t0 = time.perf_counter()
+        done = opt.run(fmax, max_steps)
+        ms = (time.perf_counter() - t0) * 1e3
+        out[cls.__name__] = {"ms": ms, "steps": opt.step, "last_converged_step": int(opt.converged_step.max()),
+                             "converged": float(opt.converged.mean()), "all": done,
+                             "energy_Ha": float(opt.energies.max())}
+    return out
+
+
+def lbfgs_main(args, model, result) -> None:
+    for name in ("gdb256", "water1k"):
+        arms, opts = {}, {}
+        for K in (1, 10, 50):
+            for lb in (False, True):
+                key = f"{'LBFGS' if lb else 'FIRE'} K={K}"
+                opts[key], arms[key] = device_arm(model, name, K, args.steps, lbfgs=lb)
+        times = {k: [] for k in arms}
+        for _ in range(args.reps):
+            for k, fn in arms.items():
+                times[k].append(fn())
+        rec = {k: {"ms_per_step": statistics.median(v), "spread_ms": [min(v), max(v)]} for k, v in times.items()}
+        lb = opts["LBFGS K=50"]
+        if lb.step < 110:
+            lb.run(0.0, 110 // 50 * 50 + 50)
+        pairs = int(lb._iter[:, 1].min())
+        rec["launches_ms_per_step"] = {"FIRE": fire_launch_ms(opts["FIRE K=50"]), "LBFGS": fire_launch_ms(lb),
+                                       "LBFGS pairs stored": pairs}
+        del opts, arms
+        sp, co, cell, pbc = workload(name)
+        if name == "gdb256":
+            rec["to_fmax_0.05"] = lbfgs_to_fmax(model, sp, co, cell, pbc, 0.05, args.max_steps)
+        result["workloads"][name] = rec
+        print(name, json.dumps(rec, indent=1), flush=True)
+    sp, co, _, _ = workload("gdb256")
+    n = int((sp[0] >= 0).sum())
+    result["molecule"] = {"atoms": n}
+    for fmax in (1e-4, 1e-6):
+        result["molecule"][f"to_fmax_{fmax:g}"] = lbfgs_to_fmax(model, sp[0, :n], co[0, :n], None, False, fmax,
+                                                                args.floor_steps)
+    print("molecule", json.dumps(result["molecule"]), flush=True)
+    os.makedirs(args.out, exist_ok=True)
+    with open(os.path.join(args.out, "opt_lbfgs_timing.json"), "w") as fh:
+        json.dump(result, fh, indent=1)
+    print(json.dumps(result))
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True)
@@ -226,6 +286,7 @@ def main() -> None:
     ap.add_argument("--floor-steps", type=int, default=5000)
     ap.add_argument("--workloads", default="gdb256,water1k")
     ap.add_argument("--cell", action="store_true", help="variable-cell FIRE against FIRE (see the docstring)")
+    ap.add_argument("--lbfgs", action="store_true", help="L-BFGS against FIRE (see the docstring)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("opt_timing needs a GPU")
@@ -237,6 +298,9 @@ def main() -> None:
     result = {"device": torch.cuda.get_device_name(0), "nvidia_smi": smi, "steps": args.steps, "workloads": {}}
     if args.cell:
         cell_main(args, model, result)
+        return
+    if args.lbfgs:
+        lbfgs_main(args, model, result)
         return
     for name in args.workloads.split(","):
         arms, opts = {}, {}

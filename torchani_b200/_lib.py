@@ -140,6 +140,23 @@ class OptCell(C.Structure):
         (k, C.c_int32) for k in ("cell_stride", "virial_slots", "projection", "pad_")]
 
 
+ANI_LBFGS_PARAMS = 4
+ANI_LBFGS_RECORD = 3
+ANI_LBFGS_MAX_MEMORY = 128
+ANI_LBFGS_TILE = 32
+
+
+def lbfgs_partials(n_conf: int, n_per_conf: int, memory: int) -> int:
+    """ANI_LBFGS_PARTIALS: the doubles of the scratch of ani_b200_lbfgs_step."""
+    return n_conf * -(-n_per_conf // ANI_LBFGS_TILE) * (4 * (memory + 1) + 2)
+
+
+class LbfgsState(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in ("x", "x_prev", "g_prev", "s", "y", "sy", "yy", "coef", "p", "iter",
+                                          "force_scale", "params", "counter", "conv_step", "record", "partials")] + [
+        (k, C.c_int32) for k in ("n_conf", "n_per_conf", "memory", "record_rows")]
+
+
 class D3Params(C.Structure):
     _fields_ = [
         ("cutoff_fn", C.c_int32), ("num_species", C.c_int32), ("cutoff", C.c_float), ("to_bohr", C.c_float),
@@ -234,6 +251,9 @@ _PROTOTYPES = {
     "ani_b200_opt_step_cells": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "ani_b200_opt_cell_init": (C.c_int, [_P, _P, _I, _P, _P]),
     "ani_b200_opt_cell_step": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "ani_b200_lbfgs_init": (C.c_int, [_P, _P, _I, _I, _P, _P]),
+    "ani_b200_lbfgs_step": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "ani_b200_lbfgs_step_cells": (C.c_int, [_P, _P, _P, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -1,7 +1,7 @@
-"""Geometry optimisation on the device: FIRE for every conformer of a batch at once, with the positions, the FIRE
-velocities and the per-conformer scalars in device memory, and K whole optimisation steps -- the two launches of
-csrc/opt.cu and the fused force step -- captured into one CUDA graph.  The host touches the GPU once per K steps: one
-replay, one copy of the replay's records into pinned memory, one synchronisation.
+"""Geometry optimisation on the device: FIRE or L-BFGS for every conformer of a batch at once, with the positions and
+the optimiser's state in device memory, and K whole optimisation steps -- the launches of csrc/opt.cu (FIRE) or
+csrc/lbfgs.cu (L-BFGS) and the fused force step -- captured into one CUDA graph.  The host touches the GPU once per K
+steps: one replay, one copy of the replay's records into pinned memory, one synchronisation.
 
     opt = optimize.FIRE(model, atomic_numbers, positions)
     done = opt.run(fmax=0.05, steps=1000)
@@ -24,13 +24,15 @@ Units: ``fmax`` and ``log.fmax`` are in eV / A, ASE's unit, so ASE's thresholds 
 (``maxstep`` in A).  ``energies`` is in Hartree and ``forces`` in Hartree / A, like every other output of the package.
 
 Every step rebuilds the bucket grid (no Verlet skin).  ``FIRE`` keeps the cell fixed; ``CellFIRE`` relaxes the lattice
-vectors with the atoms, as ASE's ``FIRE(FrechetCellFilter(atoms))`` does (see its docstring).
+vectors with the atoms, as ASE's ``FIRE(FrechetCellFilter(atoms))`` does (see its docstring).  ``LBFGS`` is ASE's
+``LBFGS`` without its line search, with the inputs, ``run`` and results of ``FIRE`` (see its docstring).
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
 import typing as tp
+import warnings
 
 import numpy as np
 import torch
@@ -41,7 +43,7 @@ from ._lib import check, ptr
 from .grad import BAR_TO_HARTREE_A3, HARTREE_TO_EV
 from .md import _DeviceLoop
 
-__all__ = ["FIRE", "CellFIRE", "Log", "CellLog", "HARTREE_TO_EV", "BAR_TO_HARTREE_A3"]
+__all__ = ["FIRE", "CellFIRE", "LBFGS", "Log", "CellLog", "HARTREE_TO_EV", "BAR_TO_HARTREE_A3"]
 
 
 class Log(tp.NamedTuple):
@@ -61,42 +63,21 @@ class CellLog(tp.NamedTuple):
     enthalpy: np.ndarray   # (S, C) Hartree: E + p0 V
 
 
-class FIRE(_DeviceLoop):
-    """FIRE on the device (see the module docstring).
+class _Optimizer(_DeviceLoop):
+    """What the device optimisers share: the system, the fixed mask and ``force_scale``, one float64 buffer
+    [x 3n | the optimiser's state | conv_step C | records K C 3 | extra records] whose head up to conv_step is what a
+    redone replay restores and whose tail from conv_step on is what a replay copies to the host, ``run``, ``_collect``
+    and the results.  A subclass sizes its state (``_state_words``), carves it, and names its parameter column of the
+    fmax threshold (``_fmax_col``)."""
 
-    Args:
-        model: a ``torchani_b200.models.ANI`` on a CUDA device
-        atomic_numbers: (A,) or (C, A) (element indices if the model has ``periodic_table_index=False``); -1 pads
-        positions: (A, 3) or (C, A, 3) Angstrom
-        cell: None, (3, 3) shared or (C, 3, 3) one per conformer (fixed); pbc: fully periodic (True) or open
-        fixed: None, or an (A,) or (C, A) boolean mask of atoms that never move (ASE's ``FixAtoms``); they are left
-            out of fmax
-        dt, maxstep, dtmax, n_min, finc, fdec, astart, fa: ASE's FIRE parameters (maxstep in A), with
-            0 < fdec < 1 <= finc, 0 < fa <= 1, dt, maxstep, dtmax > 0, n_min >= 0 and 0 <= astart <= 1
-        steps_per_replay: K, the steps of one CUDA graph replay
+    _fmax_col = 0
+    _cell_record_words = 0   # per conformer and step: records beyond the optimiser's own (CellFIRE's)
 
-    ``run`` returns after the replay in which the last conformer converged: the force steps of a converged conformer
-    go on to the end of that replay (at most K - 1 steps each), while its positions stay where they converged.
-    """
+    def _state_words(self) -> int:
+        raise NotImplementedError
 
-    _what = "the device optimiser"
-
-    def __init__(self, model, atomic_numbers, positions, cell=None, pbc=False, fixed=None, dt: float = 0.1,
-                 maxstep: float = 0.2, dtmax: float = 1.0, n_min: int = 5, finc: float = 1.1, fdec: float = 0.5,
-                 astart: float = 0.1, fa: float = 0.99, steps_per_replay: int = 20):
-        dt, maxstep, dtmax, n_min = float(dt), float(maxstep), float(dtmax), float(n_min)
-        finc, fdec, astart, fa = float(finc), float(fdec), float(astart), float(fa)
-        par = (dt, maxstep, dtmax, n_min, finc, fdec, astart, fa)
-        if not all(math.isfinite(p) for p in par):
-            raise ValueError("the FIRE parameters must be finite")
-        if not (dt > 0 and maxstep > 0 and dtmax > 0):
-            raise ValueError("dt, maxstep and dtmax must be > 0")
-        if not (0 < fdec < 1 <= finc):
-            raise ValueError("FIRE needs 0 < fdec < 1 <= finc")
-        if not (0 < fa <= 1 and 0 <= astart <= 1):
-            raise ValueError("FIRE needs 0 < fa <= 1 and 0 <= astart <= 1")
-        if n_min < 0:
-            raise ValueError("n_min must be >= 0")
+    def _allocate(self, model, atomic_numbers, positions, cell, pbc, fixed, steps_per_replay):
+        """The system and the buffer; returns the float64 cell and the state words of the buffer."""
         if int(steps_per_replay) < 1:
             raise ValueError("steps_per_replay must be >= 1")
         c64 = self._set_system(model, atomic_numbers, cell, pbc, steps_per_replay)
@@ -113,18 +94,11 @@ class FIRE(_DeviceLoop):
         self.fixed = fix
 
         f64 = dict(dtype=torch.float64, device=dev)
-        # [x 3n | v 3n | scalars 2 C 3 | counter 2 | (CellFIRE: master 2 C 27) | conv_step C | records K C 3 |
-        # (CellFIRE: cell records K C 3)]: the head up to conv_step is what a redone replay restores, the tail from
-        # conv_step on is what a replay copies to the host
-        ns, nm = 2 * C_ * _lib.ANI_OPT_SCALARS, C_ * self._master_words
-        head = 6 * n + ns + 2 + nm + C_
+        ns = self._state_words()
+        head = 3 * n + ns + C_
         n_rec = self.K * C_ * _lib.ANI_OPT_RECORD
         self._buf = torch.zeros(head + n_rec + self.K * C_ * self._cell_record_words, **f64)
         self.x = self._buf[:3 * n].view(C_, A, 3)
-        self.v = self._buf[3 * n:6 * n].view(C_, A, 3)
-        self._scalars = self._buf[6 * n:6 * n + ns].view(2, C_, _lib.ANI_OPT_SCALARS)
-        self._counter = self._buf[6 * n + ns:6 * n + ns + 2].view(torch.int64)
-        self._master = self._buf[6 * n + ns + 2:6 * n + ns + 2 + nm]
         self._conv = self._buf[head - C_:head].view(torch.int64)
         self._rec = self._buf[head - C_:]
         self._head = self._buf[:head]
@@ -139,49 +113,16 @@ class FIRE(_DeviceLoop):
         self._conv.fill_(-1)
         scale = np.where(real & ~fix, HARTREE_TO_EV, 0.0)
         self.force_scale = torch.from_numpy(scale).to(**f64).reshape(-1)
-        params = np.zeros((C_, _lib.ANI_OPT_PARAMS))
-        params[:, :8] = par
-        self.params = torch.from_numpy(params).to(**f64)
-        self._partials = torch.zeros(C_ * -(-A // _lib.ANI_MD_BLOCK) * 4, **f64)
-        st = _lib.OptState()
-        st.x, st.v, st.force_scale, st.params = ptr(self.x), ptr(self.v), ptr(self.force_scale), ptr(self.params)
-        st.scalars, st.counter, st.conv_step = ptr(self._scalars), ptr(self._counter), ptr(self._conv)
-        st.record, st.partials = ptr(self._record_dev), ptr(self._partials)
-        st.n_conf, st.n_per_conf, st.record_rows = C_, A, self.K
-        self._state = st
         self.step = 0   # steps done (the device counter, mirrored)
         self._conv_host = np.full(C_, -1, dtype=np.int64)
         self._log: tp.List[np.ndarray] = []
         self._graph: tp.Optional[torch.cuda.CUDAGraph] = None
-        self._setup(c64)
-        with torch.cuda.device(dev):
+        return c64, self._buf[3 * n:3 * n + ns]
+
+    def _start(self) -> None:
+        with torch.cuda.device(self.device):
             self._attach_engine()
             self._begin(True)
-
-    _master_words = 0        # per conformer: state a redo restores beyond FIRE's own (CellFIRE's master)
-    _cell_record_words = 0   # per conformer and step: records beyond FIRE's own (CellFIRE's)
-
-    def _setup(self, cell64: tp.Optional[np.ndarray]) -> None:
-        """What a subclass adds to the state before the engine is attached."""
-
-    # -- the device loop ------------------------------------------------------------------------
-    def _init_launch(self, reset: bool) -> None:
-        """ani_b200_opt_init (v = 0 and the initial scalars at the start only)."""
-        mode = 2 if self.per_conf else (1 if self.pbc else 0)
-        check(self.engine.lib.ani_b200_opt_init(
-            C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, mode,
-            int(reset), ptr(self.ws.coords), self._stream()), "opt_init")
-
-    def _integrate(self) -> None:
-        """The FIRE launches of one step (ani_b200_opt_step: step t to x(t+1))."""
-        ws, L = self.ws, self.engine.lib
-        if self.per_conf:
-            rc = L.ani_b200_opt_step_cells(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), ptr(ws.lattice),
-                                           ptr(ws.coords), self._stream())
-        else:
-            rc = L.ani_b200_opt_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies),
-                                     ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
-        check(rc, "opt_step")
 
     def _collect(self, t0: int, k: int) -> None:
         C_ = self.n_conf
@@ -194,16 +135,16 @@ class FIRE(_DeviceLoop):
             callback: tp.Optional[tp.Callable[..., tp.Any]] = None) -> bool:
         """Optimise until every conformer has max_i |f_i| < ``fmax`` (eV / A) or ``steps`` steps have run: replays of
         ``steps_per_replay`` steps, the remainder as eager launches of the same sequence.  Returns True when every
-        conformer converged.  A new ``run`` starts a new convergence check and keeps the FIRE state (v, dt, a, n), so
-        a second ``run`` with a smaller ``fmax`` continues the optimisation, as ASE's does.  ``callback(step,
-        positions, log)`` runs after every replay (``log``: that replay's records)."""
+        conformer converged.  A new ``run`` starts a new convergence check and keeps the optimiser's state (FIRE's v,
+        dt, a, n; L-BFGS's history), so a second ``run`` with a smaller ``fmax`` continues the optimisation, as ASE's
+        does.  ``callback(step, positions, log)`` runs after every replay (``log``: that replay's records)."""
         fmax, steps = float(fmax), int(steps)
         if not (math.isfinite(fmax) and fmax >= 0):
             raise ValueError(f"fmax must be >= 0 eV/A, got {fmax}")
         if steps < 0:
             raise ValueError("steps must be >= 0")
         with torch.cuda.device(self.device):
-            self.params[:, 8].fill_(fmax)
+            self.params[:, self._fmax_col].fill_(fmax)
             self._conv.fill_(-1)
             self._conv_host[:] = -1
             done = 0
@@ -216,6 +157,10 @@ class FIRE(_DeviceLoop):
                 if bool((self._conv_host >= 0).all()):
                     break
         return bool((self._conv_host >= 0).all())
+
+    def _cell_mode(self) -> int:
+        """The cell_mode of the init entry points: 0 open, 1 one cell, 2 one cell per conformer."""
+        return 2 if self.per_conf else (1 if self.pbc else 0)
 
     # -- results ----------------------------------------------------------------------------------
     @property
@@ -253,6 +198,94 @@ class FIRE(_DeviceLoop):
             z = np.zeros((0, self.n_conf))
             return Log(np.zeros(0, dtype=np.int64), z, z.copy())
         return self._as_log(np.concatenate(self._log))
+
+
+class FIRE(_Optimizer):
+    """FIRE on the device (see the module docstring).
+
+    Args:
+        model: a ``torchani_b200.models.ANI`` on a CUDA device
+        atomic_numbers: (A,) or (C, A) (element indices if the model has ``periodic_table_index=False``); -1 pads
+        positions: (A, 3) or (C, A, 3) Angstrom
+        cell: None, (3, 3) shared or (C, 3, 3) one per conformer (fixed); pbc: fully periodic (True) or open
+        fixed: None, or an (A,) or (C, A) boolean mask of atoms that never move (ASE's ``FixAtoms``); they are left
+            out of fmax
+        dt, maxstep, dtmax, n_min, finc, fdec, astart, fa: ASE's FIRE parameters (maxstep in A), with
+            0 < fdec < 1 <= finc, 0 < fa <= 1, dt, maxstep, dtmax > 0, n_min >= 0 and 0 <= astart <= 1
+        steps_per_replay: K, the steps of one CUDA graph replay
+
+    ``run`` returns after the replay in which the last conformer converged: the force steps of a converged conformer
+    go on to the end of that replay (at most K - 1 steps each), while its positions stay where they converged.
+    """
+
+    _what = "the device optimiser"
+    _fmax_col = 8
+
+    def __init__(self, model, atomic_numbers, positions, cell=None, pbc=False, fixed=None, dt: float = 0.1,
+                 maxstep: float = 0.2, dtmax: float = 1.0, n_min: int = 5, finc: float = 1.1, fdec: float = 0.5,
+                 astart: float = 0.1, fa: float = 0.99, steps_per_replay: int = 20):
+        dt, maxstep, dtmax, n_min = float(dt), float(maxstep), float(dtmax), float(n_min)
+        finc, fdec, astart, fa = float(finc), float(fdec), float(astart), float(fa)
+        par = (dt, maxstep, dtmax, n_min, finc, fdec, astart, fa)
+        if not all(math.isfinite(p) for p in par):
+            raise ValueError("the FIRE parameters must be finite")
+        if not (dt > 0 and maxstep > 0 and dtmax > 0):
+            raise ValueError("dt, maxstep and dtmax must be > 0")
+        if not (0 < fdec < 1 <= finc):
+            raise ValueError("FIRE needs 0 < fdec < 1 <= finc")
+        if not (0 < fa <= 1 and 0 <= astart <= 1):
+            raise ValueError("FIRE needs 0 < fa <= 1 and 0 <= astart <= 1")
+        if n_min < 0:
+            raise ValueError("n_min must be >= 0")
+        # state: [v 3n | scalars 2 C 3 | counter 2 | (CellFIRE: master 2 C 27)]
+        c64, st_words = self._allocate(model, atomic_numbers, positions, cell, pbc, fixed, steps_per_replay)
+        dev, C_, A = self.device, self.n_conf, self.n_per_conf
+        n = C_ * A
+        ns = 2 * C_ * _lib.ANI_OPT_SCALARS
+        self.v = st_words[:3 * n].view(C_, A, 3)
+        self._scalars = st_words[3 * n:3 * n + ns].view(2, C_, _lib.ANI_OPT_SCALARS)
+        self._counter = st_words[3 * n + ns:3 * n + ns + 2].view(torch.int64)
+        self._master = st_words[3 * n + ns + 2:]
+        f64 = dict(dtype=torch.float64, device=dev)
+        params = np.zeros((C_, _lib.ANI_OPT_PARAMS))
+        params[:, :8] = par
+        self.params = torch.from_numpy(params).to(**f64)
+        self._partials = torch.zeros(C_ * -(-A // _lib.ANI_MD_BLOCK) * 4, **f64)
+        st = _lib.OptState()
+        st.x, st.v, st.force_scale, st.params = ptr(self.x), ptr(self.v), ptr(self.force_scale), ptr(self.params)
+        st.scalars, st.counter, st.conv_step = ptr(self._scalars), ptr(self._counter), ptr(self._conv)
+        st.record, st.partials = ptr(self._record_dev), ptr(self._partials)
+        st.n_conf, st.n_per_conf, st.record_rows = C_, A, self.K
+        self._state = st
+        self._setup(c64)
+        self._start()
+
+    _master_words = 0        # per conformer: state a redo restores beyond FIRE's own (CellFIRE's master)
+
+    def _state_words(self) -> int:
+        return 3 * self.n_conf * self.n_per_conf + 2 * self.n_conf * _lib.ANI_OPT_SCALARS + 2 + \
+            self.n_conf * self._master_words
+
+    def _setup(self, cell64: tp.Optional[np.ndarray]) -> None:
+        """What a subclass adds to the state before the engine is attached."""
+
+    # -- the device loop ------------------------------------------------------------------------
+    def _init_launch(self, reset: bool) -> None:
+        """ani_b200_opt_init (v = 0 and the initial scalars at the start only)."""
+        check(self.engine.lib.ani_b200_opt_init(
+            C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, self._cell_mode(),
+            int(reset), ptr(self.ws.coords), self._stream()), "opt_init")
+
+    def _integrate(self) -> None:
+        """The FIRE launches of one step (ani_b200_opt_step: step t to x(t+1))."""
+        ws, L = self.ws, self.engine.lib
+        if self.per_conf:
+            rc = L.ani_b200_opt_step_cells(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), ptr(ws.lattice),
+                                           ptr(ws.coords), self._stream())
+        else:
+            rc = L.ani_b200_opt_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies),
+                                     ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
+        check(rc, "opt_step")
 
 
 class CellFIRE(FIRE):
@@ -399,3 +432,111 @@ class CellFIRE(FIRE):
         if not self._log:
             return self._as_log(np.zeros((0, self.n_conf, _lib.ANI_OPT_RECORD + _lib.ANI_OPT_CELL_RECORD)))
         return self._as_log(np.concatenate(self._log))
+
+
+class LBFGS(_Optimizer):
+    """L-BFGS on the device: ASE's ``ase.optimize.LBFGS(atoms, maxstep, memory, damping, alpha)`` without its line
+    search, one optimisation per conformer of a batch.  Per conformer and step t, with f the forces in eV / A (zero for
+    fixed and padding atoms), g = -f and H0 = 1 / alpha:
+
+        fmax(t) = max_i |f_i| < fmax:  converged at t; nothing of the conformer changes again
+        k >= 1:   s = x(t) - x(t-1), y = g(t) - g(t-1) join the history; the oldest pair leaves when more than
+                  ``memory`` are kept
+        p = -H g  (H the inverse BFGS matrix of the kept pairs with H0: the two-loop recursion's p; p = f / alpha at
+                  k = 0)
+        x(t+1) = x(t) + damping p min(1, maxstep / max_i |p_i|)   (the factor applies when max_i |p_i| >= maxstep:
+                  the longest atom step, not FIRE's global norm);   k += 1
+
+    One deviation from ASE: a pair with y.s == 0 exactly, where ASE divides by zero, is skipped.  Pairs with y.s < 0
+    are kept, as ASE keeps them.  The device forms p from the compact representation of H (Byrd, Nocedal & Schnabel,
+    Math. Prog. 63 (1994)) in four launches (csrc/lbfgs.cu), not by the two-loop recursion; both give the same p up to
+    rounding.
+
+    Args: those of ``FIRE`` without FIRE's parameters, and ASE's
+        maxstep: the longest atom step, A (> 1 warns, as ASE does)
+        memory: the pairs kept, 1 .. 128
+        damping: the factor of every step
+        alpha: the initial Hessian guess 1 / H0, eV / A^2
+    The history is C x memory x 3A x 2 doubles on the device (and as much again for the copy a 3 x bfloat16 redo
+    restores).  A second ``run`` keeps the history and k, as ASE's optimiser does.
+    """
+
+    _what = "the device optimiser"
+    _fmax_col = 3
+
+    def __init__(self, model, atomic_numbers, positions, cell=None, pbc=False, fixed=None, maxstep: float = 0.2,
+                 memory: int = 100, damping: float = 1.0, alpha: float = 70.0, steps_per_replay: int = 20):
+        maxstep, damping, alpha = float(maxstep), float(damping), float(alpha)
+        for name, v in (("maxstep", maxstep), ("damping", damping), ("alpha", alpha)):
+            if not (math.isfinite(v) and v > 0):
+                raise ValueError(f"{name} must be finite and > 0, got {v}")
+        if int(memory) != memory or not 1 <= int(memory) <= _lib.ANI_LBFGS_MAX_MEMORY:
+            raise ValueError(f"memory must be an integer in 1..{_lib.ANI_LBFGS_MAX_MEMORY}, got {memory}")
+        if maxstep > 1.0:
+            warnings.warn(f"a much too large maximum step size for L-BFGS: {maxstep:.1f} A")
+        self.memory = int(memory)
+        # state: [x_prev 3n | g_prev 3n | s C M 3A | y C M 3A | SY C M M | YY C M M | {k, head} 2 C | counter 2]
+        c64, st_words = self._allocate(model, atomic_numbers, positions, cell, pbc, fixed, steps_per_replay)
+        dev, C_, A, M = self.device, self.n_conf, self.n_per_conf, self.memory + 1
+        n = C_ * A
+        o = np.cumsum([0, 3 * n, 3 * n, C_ * M * 3 * A, C_ * M * 3 * A, C_ * M * M, C_ * M * M, 2 * C_, 2])
+        self.x_prev = st_words[o[0]:o[1]].view(C_, A, 3)
+        self.g_prev = st_words[o[1]:o[2]].view(C_, A, 3)
+        self._s = st_words[o[2]:o[3]].view(C_, M, A, 3)
+        self._y = st_words[o[3]:o[4]].view(C_, M, A, 3)
+        self._sy = st_words[o[4]:o[5]].view(C_, M, M)
+        self._yy = st_words[o[5]:o[6]].view(C_, M, M)
+        self._iter = st_words[o[6]:o[7]].view(torch.int64).view(C_, 2)
+        self._counter = st_words[o[7]:o[8]].view(torch.int64)
+        f64 = dict(dtype=torch.float64, device=dev)
+        params = np.zeros((C_, _lib.ANI_LBFGS_PARAMS))
+        params[:, :3] = (maxstep, damping, 1.0 / alpha)
+        self.params = torch.from_numpy(params).to(**f64)
+        self._coef = torch.zeros(C_, 2, self.memory, **f64)
+        self._p = torch.zeros(C_, A, 3, **f64)
+        self._partials = torch.zeros(_lib.lbfgs_partials(C_, A, self.memory), **f64)
+        st = _lib.LbfgsState()
+        st.x, st.x_prev, st.g_prev = ptr(self.x), ptr(self.x_prev), ptr(self.g_prev)
+        st.s, st.y, st.sy, st.yy = ptr(self._s), ptr(self._y), ptr(self._sy), ptr(self._yy)
+        st.coef, st.p, st.iter = ptr(self._coef), ptr(self._p), ptr(self._iter)
+        st.force_scale, st.params, st.counter = ptr(self.force_scale), ptr(self.params), ptr(self._counter)
+        st.conv_step, st.record, st.partials = ptr(self._conv), ptr(self._record_dev), ptr(self._partials)
+        st.n_conf, st.n_per_conf, st.memory, st.record_rows = C_, A, self.memory, self.K
+        self._state = st
+        self._start()
+
+    def _state_words(self) -> int:
+        C_, A, M = self.n_conf, self.n_per_conf, self.memory + 1
+        return 6 * C_ * A + 2 * C_ * M * 3 * A + 2 * C_ * M * M + 2 * C_ + 2
+
+    def _init_launch(self, reset: bool) -> None:
+        """ani_b200_lbfgs_init (x_prev = x, g_prev = 0 and an empty history at the start only)."""
+        check(self.engine.lib.ani_b200_lbfgs_init(
+            C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, self._cell_mode(),
+            int(reset), ptr(self.ws.coords), self._stream()), "lbfgs_init")
+
+    def _integrate(self) -> None:
+        """The L-BFGS launches of one step (ani_b200_lbfgs_step: step t to x(t+1))."""
+        ws, L = self.ws, self.engine.lib
+        if self.per_conf:
+            rc = L.ani_b200_lbfgs_step_cells(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), ptr(ws.lattice),
+                                             ptr(ws.coords), self._stream())
+        else:
+            rc = L.ani_b200_lbfgs_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies),
+                                       ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
+        check(rc, "lbfgs_step")
+
+    @property
+    def iteration(self) -> np.ndarray:
+        """(C,) int64: the steps each conformer has taken (ASE's ``iteration``)."""
+        return self._iter[:, 0].cpu().numpy()
+
+    def _history(self) -> tp.Tuple[Tensor, Tensor]:
+        """(S, Y), each (C, L, A, 3) float64 on the device: the kept pairs of every conformer in chronological order,
+        L = min(memory, pairs stored) of the conformer with the fewest (a copy)."""
+        head = self._iter[:, 1].cpu().numpy()
+        M = self.memory + 1
+        L = int(min(self.memory, head.min()))
+        idx = torch.as_tensor(np.stack([(h - L + np.arange(L)) % M for h in head]), device=self.device)
+        take = idx.view(self.n_conf, L, 1, 1).expand(-1, -1, self.n_per_conf, 3)
+        return torch.gather(self._s, 1, take), torch.gather(self._y, 1, take)
