@@ -31,6 +31,52 @@ ASE_KB = K_B / E_CHARGE                             # ASE's units.kB, eV / K
 VERLET, LANGEVIN = 0, 1
 
 
+_PHILOX_M = (np.uint64(0xD2511F53), np.uint64(0xCD9E8D57))
+_PHILOX_W = (np.uint32(0x9E3779B9), np.uint32(0xBB67AE85))
+_LO32 = np.uint64(0xFFFFFFFF)
+
+
+def philox4x32_10(counter, key) -> np.ndarray:
+    """Philox4x32-10 (Salmon et al., SC'11, as in Random123): counter (..., 4) and key (..., 2) uint32 words, broadcast
+    against each other; returns the (..., 4) uint32 output block."""
+    c = np.asarray(counter, dtype=np.uint32)
+    k = np.asarray(key, dtype=np.uint32)
+    lead = np.broadcast_shapes(c.shape[:-1], k.shape[:-1])
+    c = [np.broadcast_to(c[..., j], lead).astype(np.uint64) for j in range(4)]
+    k0 = np.broadcast_to(k[..., 0], lead).astype(np.uint32)
+    k1 = np.broadcast_to(k[..., 1], lead).astype(np.uint32)
+    with np.errstate(over="ignore"):
+        for _ in range(10):
+            p0, p1 = _PHILOX_M[0] * c[0], _PHILOX_M[1] * c[2]
+            c = [(p1 >> np.uint64(32)) ^ c[1] ^ k0.astype(np.uint64), p1 & _LO32,
+                 (p0 >> np.uint64(32)) ^ c[3] ^ k1.astype(np.uint64), p0 & _LO32]
+            k0 = k0 + _PHILOX_W[0]
+            k1 = k1 + _PHILOX_W[1]
+    return np.stack([w.astype(np.uint32) for w in c], -1)
+
+
+def unit_open(a, b) -> np.ndarray:
+    """A uniform double in (0, 1) from the top 53 bits of the words (a, b): (m + 1/2) 2^-53."""
+    m = ((np.asarray(a, dtype=np.uint64) << np.uint64(32)) | np.asarray(b, dtype=np.uint64)) >> np.uint64(11)
+    return (m.astype(np.float64) + 0.5) * 2.0 ** -53
+
+
+def normal(seed, step, atom, comp) -> np.ndarray:
+    """The device's standard normal of (seed, step, atom, component), broadcast over its arguments: one Philox4x32-10
+    block with counter (step low, step high, atom, component) and key (seed low, seed high), two uniforms from its
+    words (0, 1) and (2, 3), and the cosine branch of Box-Muller."""
+    step = np.asarray(step, dtype=np.int64).astype(np.uint64)
+    seed = np.asarray(seed, dtype=np.uint64)
+    atom = np.asarray(atom, dtype=np.int64).astype(np.uint32)
+    comp = np.asarray(comp, dtype=np.int64).astype(np.uint32)
+    step, seed, atom, comp = np.broadcast_arrays(step, seed, atom, comp)
+    ctr = np.stack([(step & _LO32).astype(np.uint32), (step >> np.uint64(32)).astype(np.uint32), atom, comp], -1)
+    key = np.stack([(seed & _LO32).astype(np.uint32), (seed >> np.uint64(32)).astype(np.uint32)], -1)
+    w = philox4x32_10(ctr, key)
+    u1, u2 = unit_open(w[..., 0], w[..., 1]), unit_open(w[..., 2], w[..., 3])
+    return np.sqrt(-2.0 * np.log(u1)) * np.cos(2.0 * np.pi * u2)
+
+
 def kick(v, grad, inv_mass, dt):
     """B(dt/2): v + dt/2 a, a = -grad / m * ACCEL."""
     h = (0.5 * dt * ACCEL * inv_mass)[..., None]

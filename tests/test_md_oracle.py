@@ -107,6 +107,39 @@ def test_maxwell_boltzmann():
         md.maxwell_boltzmann(m, 0.0)
 
 
+@pytest.mark.parametrize("counter, key, out", [
+    ((0, 0, 0, 0), (0, 0), (0x6627E8D5, 0xE169C58D, 0xBC57AC4C, 0x9B00DBD8)),
+    ((0xFFFFFFFF,) * 4, (0xFFFFFFFF,) * 2, (0x408F276D, 0x41C83B0E, 0xA20BC7C6, 0x6D5451FD)),
+    ((0x243F6A88, 0x85A308D3, 0x13198A2E, 0x03707344), (0xA4093822, 0x299F31D0),
+     (0xD16CFE09, 0x94FDCCEB, 0x5001E420, 0x24126EA1)),
+])
+def test_philox_known_answers(counter, key, out):
+    """The Philox4x32-10 restatement against the Random123 known-answer vectors (counter -> output, key words last),
+    one at a time and broadcast over a batch."""
+    assert tuple(int(w) for w in mo.philox4x32_10(counter, key)) == out
+    batch = mo.philox4x32_10(np.tile(np.array(counter, dtype=np.uint32), (3, 1)), key)
+    assert batch.shape == (3, 4) and (batch == np.array(out, dtype=np.uint32)).all()
+
+
+def test_normal_counter_layout():
+    """``normal`` draws from the block of counter (step low, step high, atom, component) and key (seed low, seed
+    high): each word changes the draw, the step's high word included, and the words (0, 1) and (2, 3) of the block
+    give the two uniforms of Box-Muller's cosine branch."""
+    seed, step = 0x0123456789ABCDEF, (5 << 32) + 7
+    z = mo.normal(seed, step, 11, 2)
+    w = mo.philox4x32_10((7, 5, 11, 2), (0x89ABCDEF, 0x01234567))
+    u1, u2 = mo.unit_open(w[0], w[1]), mo.unit_open(w[2], w[3])
+    assert 0.0 < u1 < 1.0 and 0.0 < u2 < 1.0
+    assert z == pytest.approx(math.sqrt(-2.0 * math.log(u1)) * math.cos(2.0 * math.pi * u2), rel=1e-15, abs=1e-15)
+    others = [mo.normal(seed ^ 1, step, 11, 2), mo.normal(seed ^ (1 << 32), step, 11, 2), mo.normal(seed, step + 1, 11, 2),
+              mo.normal(seed, step + (1 << 32), 11, 2), mo.normal(seed, step, 12, 2), mo.normal(seed, step, 11, 3)]
+    assert len({float(z)} | {float(o) for o in others}) == 7
+    assert mo.unit_open(0, 0) == 2.0 ** -54 and mo.unit_open(0, 0x800) == 1.5 * 2.0 ** -53
+    # moments of a large batch: mean 0 and variance 1 to a few standard errors
+    zs = mo.normal(seed, np.arange(4)[:, None, None], np.arange(5000)[None, :, None], np.arange(4)[None, None, :])
+    assert abs(zs.mean()) < 5.0 / math.sqrt(zs.size) and abs(zs.var() - 1.0) < 5.0 * math.sqrt(2.0 / zs.size)
+
+
 def test_md_state_layout_matches_header(tmp_path):
     from torchani_b200 import _lib
     prog = tmp_path / "md.c"
