@@ -43,6 +43,45 @@ def energy_fn(model: orc.Model, species: Tensor, networks: str = "celu", pairs: 
     return energy
 
 
+def center_aev(spec: orc.AEVSpec, s_center: int, s_nbrs: tp.Sequence[int], vectors: Tensor) -> Tensor:
+    """The AEV (out_dim,) of one central atom of element ``s_center`` as a function of its neighbour vectors ``vectors``
+    (n, 3) = r_n - r_i (elements ``s_nbrs``), in the column order of ``aev_from_neighbors``: radial terms of the
+    neighbours within Rcr, angular terms of every pair of neighbours within Rca (both inclusive, the cosine's
+    denominator clamped at 1e-10).  Every neighbour and pair is summed in the order given, so the per-stage references
+    are ``torch.func`` derivatives of this function with respect to ``vectors``.  ``s_center`` does not enter (an AEV
+    row holds the neighbours' elements only); it is kept for the symmetry of the call with ``center_pair_energy``."""
+    S = spec.num_species
+    sp = torch.as_tensor(list(s_nbrs), dtype=torch.long).view(-1)
+    d = vectors.norm(dim=-1)
+    nr = len(spec.shf_r)
+    radial = vectors.new_zeros(S, nr)
+    r_in = d.detach() <= spec.rcr
+    if bool(r_in.any()):
+        radial = radial.index_add(0, sp[r_in], orc.radial_terms(spec, d[r_in]))
+    npairs = S * (S + 1) // 2
+    angular = vectors.new_zeros(npairs, spec.angular_sub)
+    close = torch.nonzero(d.detach() <= spec.rca).view(-1)
+    if close.numel() >= 2:
+        ja, jb = torch.triu_indices(close.numel(), close.numel(), 1)
+        a, b = close[ja], close[jb]
+        terms = orc.angular_terms(spec, d[a], d[b], vectors[a], vectors[b])
+        angular = angular.index_add(0, orc.triu_index(S)[sp[a], sp[b]], terms)
+    return torch.cat([radial.reshape(-1), angular.reshape(-1)])
+
+
+def center_pair_energy(pair: porc.PairSpec, s_center: int, s_nbrs: tp.Sequence[int], vectors: Tensor) -> Tensor:
+    """Half of the pair energy E(R) fc(R) of one central atom (element ``s_center``) with each of its neighbours
+    (``vectors`` (n, 3) = r_n - r_i, elements ``s_nbrs``) within the term's cutoff (inclusive): the atomic split of a
+    full neighbour list, a scalar.  Summed over every atom of a system it is ``pair_oracle.energies_from_neighbors``."""
+    n = vectors.shape[0]
+    species = torch.tensor([[int(s_center)] + [int(s) for s in s_nbrs]], dtype=torch.long)
+    d = vectors.norm(dim=-1)
+    keep = d.detach() <= pair.cutoff
+    idx = torch.stack([torch.zeros(n, dtype=torch.long), torch.arange(1, n + 1)])[:, keep]
+    nb = orc.Neighbors(idx, d[keep], vectors[keep])
+    return 0.5 * porc.pair_energies(pair, species, nb).sum()
+
+
 def hessian(energy: tp.Callable[[Tensor], Tensor], coords: Tensor) -> Tensor:
     """(C, 3A, 3A) d^2E/dx^2 in the dtype of ``coords`` (conformers are independent: one backward per component)."""
     x = coords.detach().clone().requires_grad_(True)

@@ -1,6 +1,7 @@
 """Hessian infrastructure without a GPU: the float64 oracle's Hessians against finite differences of its forces,
 ``torchani_b200.grad.vibrational_analysis`` against the oracle's float64 restatement in every mode kind and unit,
-the chunk planner of Engine.hessian and the rejections that need no device."""
+the chunk planner of Engine.hessian, the rejections that need no device, and the per-atom restatements
+``center_aev`` / ``center_pair_energy`` that the kernel-level GPU tests differentiate."""
 import numpy as np
 import pytest
 import torch
@@ -171,3 +172,82 @@ def test_vibrational_analysis_reproduces_the_reference(name):
                 g, r = got.modes.numpy()[keep].reshape(int(keep.sum()), -1), ref["modes"][keep].reshape(int(keep.sum()), -1)
                 sign = np.sign(np.sum(g * r, axis=1, keepdims=True))
                 np.testing.assert_allclose(g * sign, r, atol=1e-10 * np.abs(r).max(), err_msg=f"{name} {c} {kind}")
+
+
+# ---- per-atom restatements: center_aev and center_pair_energy ------------------------------------------------------
+def _aev_specs():
+    """ANI-1x, ANI-2x, the smooth-cutoff GELU spec and test_gpu_aev's covering configurations (ShfA x ShfZ = 32)."""
+    import oracle.gelu_oracle as gor
+    from test_gpu_aev import CONFIGS, spec_of
+    specs = {"1x": orc.aev_spec_1x(), "2x": orc.aev_spec_2x(), "gelu": gor.gelu_spec()}
+    specs.update({c.name: spec_of(c) for c in CONFIGS})
+    return specs
+
+
+AEV_SPECS = _aev_specs()
+
+
+def _cluster(n, S, radius, seed, min_dist=0.9):
+    """n float64 points in a ball (random sequential placement), random elements 0..S-1."""
+    rng = np.random.default_rng(seed)
+    pts = np.zeros((0, 3))
+    while len(pts) < n:
+        p = rng.uniform(-radius, radius, 3)
+        if np.linalg.norm(p) <= radius and (len(pts) == 0 or np.linalg.norm(pts - p, axis=1).min() >= min_dist):
+            pts = np.vstack([pts, p])
+    return torch.tensor(rng.integers(0, S, n)).view(1, -1), torch.tensor(pts).view(1, -1, 3)
+
+
+@pytest.mark.parametrize("name", list(AEV_SPECS))
+def test_center_aev_matches_aev_from_neighbors(name):
+    spec = AEV_SPECS[name]
+    sp, co = _cluster(18, spec.num_species, 3.2, 11)
+    ref = orc.aev_from_neighbors(spec, sp, orc.neighborlist("all_pairs", spec.rcr, sp, co))[0]
+    x = co[0]
+    rng = np.random.default_rng(5)
+    for i in range(x.shape[0]):
+        d = (x - x[i]).norm(dim=-1)
+        nbrs = [j for j in rng.permutation(x.shape[0]).tolist() if j != i and float(d[j]) <= spec.rcr]
+        got = hor.center_aev(spec, int(sp[0, i]), sp[0, nbrs].tolist(), x[nbrs] - x[i])
+        assert float((got - ref[i]).abs().max()) <= 1e-12 * (1.0 + float(ref[i].abs().max())), (name, i)
+
+
+def test_center_aev_derivatives_through_torch_func():
+    """jacrev of center_aev (the per-stage references of the GPU kernels) equals the full-system Jacobian with respect
+    to the neighbours' positions, and is zero in every column block a neighbour cannot touch."""
+    spec = orc.aev_spec_2x()
+    sp, co = _cluster(10, 7, 2.6, 3)
+    x, i = co[0], 4
+    nbrs = [j for j in range(10) if j != i]
+    jac = torch.func.jacrev(lambda v: hor.center_aev(spec, int(sp[0, i]), sp[0, nbrs].tolist(), v))(x[nbrs] - x[i])
+
+    def row(xx):
+        return orc.aev_from_neighbors(spec, sp, orc.neighborlist("all_pairs", spec.rcr, sp, xx.view(1, -1, 3)))[0, i]
+    full = torch.autograd.functional.jacobian(row, x)
+    assert float((jac - full[:, nbrs]).abs().max()) <= 1e-12 * float(full.abs().max())
+    nr = len(spec.shf_r)
+    for n, j in enumerate(nbrs):
+        other = torch.ones(spec.radial_len, dtype=torch.bool)
+        other[int(sp[0, j]) * nr:(int(sp[0, j]) + 1) * nr] = False
+        assert float(jac[:spec.radial_len][other, n].abs().sum()) == 0.0
+
+
+@pytest.mark.parametrize("kind", ["xtb", "zbl"])
+@pytest.mark.parametrize("fn", ["cosine", "smooth"])
+@pytest.mark.parametrize("cutoff", [3.0, 4.6, 5.1])
+def test_center_pair_energy_sums_to_energies_from_neighbors(kind, fn, cutoff):
+    import os
+    import oracle.pair_oracle as porc
+    if kind == "xtb":
+        z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pair_params.npz"))
+        pair = porc.PairSpec("xtb", cutoff, fn, tuple(torch.tensor(z[k]) for k in ("y_ab", "sqrt_alpha_ab", "k_rep_ab")))
+    else:
+        pair = porc.zbl_spec(orc.SYMBOLS_2X, cutoff, fn)
+    sp, co = _cluster(16, 7, 3.4, 8)
+    ref = porc.energies_from_neighbors(pair, sp, orc.neighborlist("all_pairs", cutoff, sp, co))[0]
+    x = co[0]
+    tot = 0.0
+    for i in range(x.shape[0]):
+        nbrs = [j for j in range(x.shape[0]) if j != i]
+        tot = tot + hor.center_pair_energy(pair, int(sp[0, i]), sp[0, nbrs].tolist(), x[nbrs] - x[i])
+    assert abs(float(tot - ref)) <= 1e-12 * abs(float(ref))

@@ -153,8 +153,9 @@ enum { VEC_S1 = 0, VEC_R1 = 1, VEC_S2 = 2, VEC_R2 = 3, VEC_Q3 = 4, VEC_COUNT = 5
 
 __device__ __forceinline__ void activation_d(int act, float alpha, float z, float& y, float& d1, float& d2) {
   if (act == ANI_ACT_CELU) {
-    // CELU: the z <= 0 branch at z = 0, as torch's first and second derivatives take it
-    if (z > 0.f) {
+    // CELU: at z = 0 both branches give y = 0 and sigma' = 1; sigma'' takes the linear branch's 0 there, as torch's
+    // double backward does (its second derivative is non-zero for z < 0 only)
+    if (z >= 0.f) {
       y = z;
       d1 = 1.f;
       d2 = 0.f;
@@ -686,6 +687,7 @@ extern "C" int ani_b200_hessian_network(const ani_mlp_model* model, const ani_he
   }
   const dim3 grid_g((hmax + G_BN - 1) / G_BN, chunk->rows / G_BM);
   const int tiles = (3 * min(chunk->max_count, cap) + 31) / 32;
+  if (tiles == 0) return ANI_OK;   // no atom of the chunk has a neighbour: every B_i is empty (and a 0-tile grid invalid)
   const float4* sp4 = reinterpret_cast<const float4*>(spos);
   for (int m = 0; m < model->num_members; ++m) {
     const float scale = model->member_scale[m];
