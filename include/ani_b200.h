@@ -1044,6 +1044,65 @@ int ani_b200_lbfgs_step(const ani_lbfgs_state* state, const float* grad, const d
                         float* coords, void* stream);
 int ani_b200_lbfgs_step_cells(const ani_lbfgs_state* state, const float* grad, const double* energies,
                               const float* lattice, float* coords, void* stream);
+/*  Nudged elastic band (csrc/neb.cu): ASE's NEB ("aseneb" or "improvedtangent", optionally with a climbing image)     */
+/*    relaxed by ASE's FIRE over each band's interior rows.  A band has n = n_images >= 3 images; images 0 and n - 1    */
+/*    never move.  Interior image i (1 .. n - 2) of band b is conformer b (n - 2) + i - 1 of the force step, so the   */
+/*    force step's flat atom index and the band's FIRE row index are the same.  Units: A, eV, Hartree.                 */
+/*    ani_neb_state (device pointers):                                                                                */
+/*      fire        the FIRE state of ani_opt_state with n_conf = B bands and n_per_conf = (n - 2) n_atoms rows: x, v,  */
+/*                  force_scale, params (ANI_OPT_PARAMS per band), scalars, counter and conv_step as there; record      */
+/*                  f64[record_rows][B][ANI_NEB_RECORD] {t, E_imax (Hartree), fmax (eV / A), imax}; partials           */
+/*                  f64[B (n - 2)][ceil(n_atoms / ANI_MD_BLOCK)][4] scratch                                            */
+/*      endpoints   f64[B][2][n_atoms][3] images 0 and n - 1                                                          */
+/*      end_energies f64[B][2] their energies (Hartree)                                                               */
+/*      springs     f64[B][n - 1] k_j (eV / A^2) of the spring between images j and j + 1                             */
+/*      climb       f64[B] 1: image imax of the band climbs, 0: it does not                                           */
+/*      neb_force   f64[B (n - 2) n_atoms][3] scratch: the NEB forces f (eV / A) of the step                          */
+/*      dots        f64[B (n - 2)][ceil(n_atoms / ANI_MD_BLOCK)][ANI_NEB_DOTS] scratch                                 */
+/*      method      ANI_NEB_ASENEB or ANI_NEB_IMPROVED_TANGENT                                                        */
+/*    Per interior image i, with F = -dE/dx * force_scale, t- = x_i - x_{i-1}, t+ = x_{i+1} - x_i (both 0 where        */
+/*    force_scale is 0), k- = k_{i-1}, k+ = k_i, imax = 1 + the first index of the largest of E_1 .. E_{n-2}, the       */
+/*    tangent tau = alpha t- + beta t+ and f = F + gamma- t- + gamma+ t+:                                             */
+/*      ASENEB       (alpha, beta) = (0, 1) for i < imax, (1, 0) for i > imax, (1, 1) at imax; m = tau.tau (1 if 0);  */
+/*                   climbing: f = F - 2 (F.tau / m) tau;  else f = F - ((F.tau + (k- t- - k+ t+).tau) / m) tau        */
+/*      IMPROVED_TANGENT  (Henkelman & Jonsson 2000) E_{i+1} > E_i > E_{i-1}: (0, 1);  E_{i+1} < E_i < E_{i-1}: (1, 0); */
+/*                   else (dmin, dmax) if E_{i+1} > E_{i-1}, (dmax, dmin) if not, of |E_{i+1} - E_i|, |E_{i-1} - E_i|;  */
+/*                   u = tau / |tau| (0 if |tau| = 0); climbing: f = F - 2 (F.u) u;                                  */
+/*                   else f = F - (F.u) u + (k+ |t+| - k- |t-|) u                                                     */
+/*    and then ani_b200_opt_step's FIRE per band over all its (n - 2) n_atoms rows (P, F2, V2, fmax and the maxstep     */
+/*    clamp over the whole band; a converged band's x and v freeze).                                                  */
+/*  ani_b200_neb_init  with reset: v = 0 and the scalars of slot counter[0] % 2 = {dt0, astart, 0}; then the f32       */
+/*                     coords of x: cell_mode 0 open, 1 one cell f32[9], 2 one cell per force-step conformer            */
+/*                     f32[B (n - 2)][9].  One launch.                                                                */
+/*  ani_b200_neb_step  after the force step at x(t) (grad f32[B (n - 2) n_atoms][3] dE/dx, energies f64[B (n - 2)]),   */
+/*                     three launches: the five dot products {t-.t-, t+.t+, t-.t+, F.t-, F.t+} per image, the NEB       */
+/*                     forces and their FIRE partials, and FIRE's update; then the f32 coords of x(t+1) (wrapped into   */
+/*                     `cell` f32[9] when not NULL), and t += 1.  Sums are float64 in a fixed order without atomics:    */
+/*                     the same state and forces give the same bits.                                                 */
+/*  ani_b200_neb_step_cells  the same with the lattice table of grid mode 3 (f32[B (n - 2)][ANI_LATTICE_STRIDE]) in    */
+/*                     place of `cell`.                                                                              */
+/*  ani_b200_neb_project  the first two launches only: neb_force of the current forces; writes nothing but scratch.    */
+#define ANI_NEB_RECORD 4
+#define ANI_NEB_DOTS 5
+#define ANI_NEB_ASENEB 0
+#define ANI_NEB_IMPROVED_TANGENT 1
+typedef struct ani_neb_state {
+  ani_opt_state fire;
+  const double* endpoints;
+  const double* end_energies;
+  const double* springs;
+  const double* climb;
+  double* neb_force;
+  double* dots;
+  int32_t n_images, n_atoms, method, pad_;
+} ani_neb_state;
+int ani_b200_neb_init(const ani_neb_state* state, const float* cells, int cell_mode, int reset, float* coords,
+                      void* stream);
+int ani_b200_neb_step(const ani_neb_state* state, const float* grad, const double* energies, const float* cell,
+                      float* coords, void* stream);
+int ani_b200_neb_step_cells(const ani_neb_state* state, const float* grad, const double* energies,
+                            const float* lattice, float* coords, void* stream);
+int ani_b200_neb_project(const ani_neb_state* state, const float* grad, const double* energies, void* stream);
 
 #ifdef __cplusplus
 }

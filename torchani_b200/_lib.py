@@ -157,6 +157,18 @@ class LbfgsState(C.Structure):
         (k, C.c_int32) for k in ("n_conf", "n_per_conf", "memory", "record_rows")]
 
 
+ANI_NEB_RECORD = 4
+ANI_NEB_DOTS = 5
+ANI_NEB_ASENEB = 0
+ANI_NEB_IMPROVED_TANGENT = 1
+
+
+class NebState(C.Structure):
+    _fields_ = [("fire", OptState)] + [(k, C.c_void_p) for k in ("endpoints", "end_energies", "springs", "climb",
+                                                                  "neb_force", "dots")] + [
+        (k, C.c_int32) for k in ("n_images", "n_atoms", "method", "pad_")]
+
+
 class D3Params(C.Structure):
     _fields_ = [
         ("cutoff_fn", C.c_int32), ("num_species", C.c_int32), ("cutoff", C.c_float), ("to_bohr", C.c_float),
@@ -254,6 +266,10 @@ _PROTOTYPES = {
     "ani_b200_lbfgs_init": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "ani_b200_lbfgs_step": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "ani_b200_lbfgs_step_cells": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "ani_b200_neb_init": (C.c_int, [_P, _P, _I, _I, _P, _P]),
+    "ani_b200_neb_step": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "ani_b200_neb_step_cells": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "ani_b200_neb_project": (C.c_int, [_P, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -70,9 +70,9 @@ def _fingerprint(extra=()) -> str:
 
 
 # translation units without any of the profiled kernels (preparation, communicator, pair potentials, dispersion, ABI
-# glue, Hessians, MD integrators, FIRE, L-BFGS): a change there does not touch the AEV / GEMM kernels whose measured DRAM traffic bench.py reports
+# glue, Hessians, MD integrators, FIRE, L-BFGS, NEB): a change there does not touch the AEV / GEMM kernels whose measured DRAM traffic bench.py reports
 _NOT_PROFILED = ("cells.cu", "comm.cu", "api.cu", "pair.cu", "disp.cu", "charges.cu", "hessian.cu", "md.cu",
-                "opt.cu", "lbfgs.cu")
+                "opt.cu", "lbfgs.cu", "neb.cu")
 
 
 def build_id(variant: str = "", kernels_only: bool = False) -> str:

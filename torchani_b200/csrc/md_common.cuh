@@ -1,6 +1,6 @@
-// Pieces shared by the device loops of md.cu (MD integrators) and opt.cu (FIRE): the float64 cell determinant and
-// inverse, the float32 coordinates of a master position wrapped into the cell, and the fixed-shape block tree their
-// per-block partial sums go through.
+// Pieces shared by the device loops of md.cu (MD integrators), opt.cu (FIRE) and neb.cu (NEB under FIRE): the float64
+// cell determinant and inverse, the float32 coordinates of a master position wrapped into the cell, the fixed-shape
+// block tree their per-block partial sums go through, and FIRE's scalar update.
 #pragma once
 #include "common.cuh"
 
@@ -74,6 +74,60 @@ __device__ __forceinline__ void block_reduce(double* v, double& w, double* sv, d
 #pragma unroll
   for (int k = 0; k < NS; ++k) v[k] = sv[k * ANI_MD_BLOCK];
   w = sw[0];
+}
+
+// FIRE's scalar update of optimisation c (a conformer of opt.cu, a band of neb.cu) at step t from the totals
+// {P, F2, V2, max |f_i|^2}, by thread 0 of every block of the optimisation (the same inputs, so the same results
+// everywhere): mix = {c1, c2 + dt, dt * min(1, maxstep / |dr|), frozen}.  The leader block (one per optimisation)
+// writes the record {t, *energy, fmax} of step t (rows of RECORD words), the convergence step and the scalars of step
+// t + 1, and the leader of optimisation 0 the step counter.
+template <int RECORD>
+__device__ inline void fire_scalars(const ani_opt_state& s, int c, long long t, const double* tot, bool leader,
+                                    const double* energy, double* mix) {
+  const double* par = s.params + (size_t)c * ANI_OPT_PARAMS;   // dt0, maxstep, dtmax, Nmin, finc, fdec, astart, fa, fmax
+  const double* sc = s.scalars + ((size_t)(t & 1) * s.n_conf + c) * ANI_OPT_SCALARS;
+  const double p = tot[0], f2 = tot[1], v2 = tot[2], fmax_ = sqrt(tot[3]);
+  double dt = sc[0], al = sc[1], n = sc[2];
+  // conv_step[c] is written below by the leader block of this optimisation only, and only with the value t: a block
+  // that reads it concurrently sees -1 or t, and "converged before this step" is false for both
+  const long long cs = s.conv_step[c];
+  const bool before = cs >= 0 && cs < t;
+  const bool conv = !before && fmax_ < par[8];
+  const bool frozen = before || conv;
+  double c1 = 1.0, c2 = 0.0;   // t = 0: v' = v + dt f, and dt is not shrunk
+  if (!frozen && t > 0) {
+    if (p > 0.0) {
+      c1 = 1.0 - al;
+      c2 = al * sqrt(v2 / f2);
+      if (n > par[3]) {
+        dt = fmin(dt * par[4], par[2]);
+        al *= par[7];
+      }
+      n += 1.0;
+    } else {
+      c1 = 0.0;
+      al = par[6];
+      dt *= par[5];
+      n = 0.0;
+    }
+  }
+  const double cf = c2 + dt;
+  const double dr = dt * sqrt(c1 * c1 * v2 + 2.0 * c1 * cf * p + cf * cf * f2);   // |dt v'|: every term is >= 0
+  mix[0] = c1;
+  mix[1] = cf;
+  mix[2] = dt * (dr > par[1] ? par[1] / dr : 1.0);
+  mix[3] = frozen ? 1.0 : 0.0;
+  if (!leader) return;
+  double* nx = s.scalars + ((size_t)((t + 1) & 1) * s.n_conf + c) * ANI_OPT_SCALARS;
+  nx[0] = dt;
+  nx[1] = al;
+  nx[2] = n;
+  double* row = s.record + ((size_t)(t % s.record_rows) * s.n_conf + c) * RECORD;
+  row[0] = (double)t;
+  row[1] = *energy;
+  row[2] = fmax_;
+  if (conv) s.conv_step[c] = t;
+  if (c == 0) s.counter[0] = t + 1;
 }
 
 }  // namespace ani

@@ -225,57 +225,6 @@ __global__ void __launch_bounds__(OPT_BLOCK) k_opt_reduce(const __grid_constant_
   }
 }
 
-// FIRE's scalar update of conformer c at step t from the totals {P, F2, V2, max |f_i|^2}, by thread 0 of every block
-// of the conformer (the same inputs, so the same results everywhere): mix = {c1, c2 + dt, dt * min(1, maxstep / |dr|),
-// frozen}.  Block 0 writes the record of step t, the convergence step and the scalars of step t + 1.
-__device__ void fire_scalars(const OptArgs& a, int c, long long t, const double* tot, double* mix) {
-  const ani_opt_state& s = a.s;
-  const double* par = s.params + (size_t)c * ANI_OPT_PARAMS;   // dt0, maxstep, dtmax, Nmin, finc, fdec, astart, fa, fmax
-  const double* sc = s.scalars + ((size_t)(t & 1) * s.n_conf + c) * ANI_OPT_SCALARS;
-  const double p = tot[0], f2 = tot[1], v2 = tot[2], fmax_ = sqrt(tot[3]);
-  double dt = sc[0], al = sc[1], n = sc[2];
-  // conv_step[c] is written below by block 0 of this conformer only, and only with the value t: a block that reads it
-  // concurrently sees -1 or t, and "converged before this step" is false for both
-  const long long cs = s.conv_step[c];
-  const bool before = cs >= 0 && cs < t;
-  const bool conv = !before && fmax_ < par[8];
-  const bool frozen = before || conv;
-  double c1 = 1.0, c2 = 0.0;   // t = 0: v' = v + dt f, and dt is not shrunk
-  if (!frozen && t > 0) {
-    if (p > 0.0) {
-      c1 = 1.0 - al;
-      c2 = al * sqrt(v2 / f2);
-      if (n > par[3]) {
-        dt = fmin(dt * par[4], par[2]);
-        al *= par[7];
-      }
-      n += 1.0;
-    } else {
-      c1 = 0.0;
-      al = par[6];
-      dt *= par[5];
-      n = 0.0;
-    }
-  }
-  const double cf = c2 + dt;
-  const double dr = dt * sqrt(c1 * c1 * v2 + 2.0 * c1 * cf * p + cf * cf * f2);   // |dt v'|: every term is >= 0
-  mix[0] = c1;
-  mix[1] = cf;
-  mix[2] = dt * (dr > par[1] ? par[1] / dr : 1.0);
-  mix[3] = frozen ? 1.0 : 0.0;
-  if (blockIdx.x != 0) return;
-  double* nx = s.scalars + ((size_t)((t + 1) & 1) * s.n_conf + c) * ANI_OPT_SCALARS;
-  nx[0] = dt;
-  nx[1] = al;
-  nx[2] = n;
-  double* row = s.record + ((size_t)(t % s.record_rows) * s.n_conf + c) * ANI_OPT_RECORD;
-  row[0] = (double)t;
-  row[1] = a.energies[c];
-  row[2] = fmax_;
-  if (conv) s.conv_step[c] = t;
-  if (c == 0) s.counter[0] = t + 1;
-}
-
 // the cell rows' move of conformer c at step t by thread 0 of every block (k_opt_update), after fire_scalars: from
 // slot t % 2 and cell_force, v_cell' = c1 v_cell + (c2 + dt) Phi, d(t+1) = d + s v_cell' and F(t+1) = expm(d(t+1) / c)
 // (all unchanged for a frozen conformer); F(t) to cell[9..18), F(t+1) to cell[18..27), the float32-rounded
@@ -336,7 +285,7 @@ __global__ void __launch_bounds__(OPT_BLOCK) k_opt_update(const __grid_constant_
       tot[3] = fmax(tot[3], __shfl_down_sync(ANI_FULL_MASK, tot[3], o));
     }
     if (threadIdx.x == 0) {
-      fire_scalars(a, c, s.counter[1], tot, mix);
+      fire_scalars<ANI_OPT_RECORD>(s, c, s.counter[1], tot, blockIdx.x == 0, a.energies + c, mix);
       if constexpr (CELL) cell_move(a, c, s.counter[1], mix, cell, inv);
     }
   }

@@ -25,7 +25,9 @@ Units: ``fmax`` and ``log.fmax`` are in eV / A, ASE's unit, so ASE's thresholds 
 
 Every step rebuilds the bucket grid (no Verlet skin).  ``FIRE`` keeps the cell fixed; ``CellFIRE`` relaxes the lattice
 vectors with the atoms, as ASE's ``FIRE(FrechetCellFilter(atoms))`` does (see its docstring).  ``LBFGS`` is ASE's
-``LBFGS`` without its line search, with the inputs, ``run`` and results of ``FIRE`` (see its docstring).
+``LBFGS`` without its line search, with the inputs, ``run`` and results of ``FIRE`` (see its docstring).  ``NEB`` is
+ASE's nudged elastic band under FIRE, one FIRE optimisation per band, with the interior images of every band in one
+force step (csrc/neb.cu; see its docstring).
 """
 from __future__ import annotations
 
@@ -43,7 +45,8 @@ from ._lib import check, ptr
 from .grad import BAR_TO_HARTREE_A3, HARTREE_TO_EV
 from .md import _DeviceLoop
 
-__all__ = ["FIRE", "CellFIRE", "LBFGS", "Log", "CellLog", "HARTREE_TO_EV", "BAR_TO_HARTREE_A3"]
+__all__ = ["FIRE", "CellFIRE", "LBFGS", "NEB", "interpolate", "Log", "CellLog", "NEBLog", "HARTREE_TO_EV",
+           "BAR_TO_HARTREE_A3"]
 
 
 class Log(tp.NamedTuple):
@@ -65,13 +68,19 @@ class CellLog(tp.NamedTuple):
 
 class _Optimizer(_DeviceLoop):
     """What the device optimisers share: the system, the fixed mask and ``force_scale``, one float64 buffer
-    [x 3n | the optimiser's state | conv_step C | records K C 3 | extra records] whose head up to conv_step is what a
+    [x 3n | the optimiser's state | conv_step O | records K O R | extra records] whose head up to conv_step is what a
     redone replay restores and whose tail from conv_step on is what a replay copies to the host, ``run``, ``_collect``
-    and the results.  A subclass sizes its state (``_state_words``), carves it, and names its parameter column of the
-    fmax threshold (``_fmax_col``)."""
+    and the results.  O is the number of optimisations (``_n_opt``: one per conformer, one per band for ``NEB``) and R
+    the words of a record (``_record_words``).  A subclass sizes its state (``_state_words``), carves it, and names its
+    parameter column of the fmax threshold (``_fmax_col``)."""
 
     _fmax_col = 0
+    _record_words = _lib.ANI_OPT_RECORD
     _cell_record_words = 0   # per conformer and step: records beyond the optimiser's own (CellFIRE's)
+
+    @property
+    def _n_opt(self) -> int:
+        return self.n_conf
 
     def _state_words(self) -> int:
         raise NotImplementedError
@@ -81,7 +90,7 @@ class _Optimizer(_DeviceLoop):
         if int(steps_per_replay) < 1:
             raise ValueError("steps_per_replay must be >= 1")
         c64 = self._set_system(model, atomic_numbers, cell, pbc, steps_per_replay)
-        dev, C_, A = self.device, self.n_conf, self.n_per_conf
+        dev, C_, A, O = self.device, self.n_conf, self.n_per_conf, self._n_opt
         n = C_ * A
         real = (self.species >= 0).cpu().numpy()
         fix = np.zeros((C_, A), dtype=bool)
@@ -95,12 +104,12 @@ class _Optimizer(_DeviceLoop):
 
         f64 = dict(dtype=torch.float64, device=dev)
         ns = self._state_words()
-        head = 3 * n + ns + C_
-        n_rec = self.K * C_ * _lib.ANI_OPT_RECORD
+        head = 3 * n + ns + O
+        n_rec = self.K * O * self._record_words
         self._buf = torch.zeros(head + n_rec + self.K * C_ * self._cell_record_words, **f64)
         self.x = self._buf[:3 * n].view(C_, A, 3)
-        self._conv = self._buf[head - C_:head].view(torch.int64)
-        self._rec = self._buf[head - C_:]
+        self._conv = self._buf[head - O:head].view(torch.int64)
+        self._rec = self._buf[head - O:]
         self._head = self._buf[:head]
         self._backup = torch.empty_like(self._head)
         self._record_dev = self._buf[head:head + n_rec]
@@ -114,7 +123,7 @@ class _Optimizer(_DeviceLoop):
         scale = np.where(real & ~fix, HARTREE_TO_EV, 0.0)
         self.force_scale = torch.from_numpy(scale).to(**f64).reshape(-1)
         self.step = 0   # steps done (the device counter, mirrored)
-        self._conv_host = np.full(C_, -1, dtype=np.int64)
+        self._conv_host = np.full(O, -1, dtype=np.int64)
         self._log: tp.List[np.ndarray] = []
         self._graph: tp.Optional[torch.cuda.CUDAGraph] = None
         return c64, self._buf[3 * n:3 * n + ns]
@@ -125,11 +134,11 @@ class _Optimizer(_DeviceLoop):
             self._begin(True)
 
     def _collect(self, t0: int, k: int) -> None:
-        C_ = self.n_conf
+        O = self._n_opt
         h = self._h_rec.numpy()
         rows = [(t0 + i) % self.K for i in range(k)]
-        self._log.append(h[C_:C_ + self._record_dev.numel()].reshape(self.K, C_, _lib.ANI_OPT_RECORD)[rows].copy())
-        self._conv_host = h[:C_].view(np.int64).copy()
+        self._log.append(h[O:O + self._record_dev.numel()].reshape(self.K, O, self._record_words)[rows].copy())
+        self._conv_host = h[:O].view(np.int64).copy()
 
     def run(self, fmax: float = 0.05, steps: int = 1000,
             callback: tp.Optional[tp.Callable[..., tp.Any]] = None) -> bool:
@@ -181,7 +190,8 @@ class _Optimizer(_DeviceLoop):
 
     @property
     def converged_step(self) -> np.ndarray:
-        """(C,) int64: the step at which each conformer converged in the current ``run``, -1 if it has not."""
+        """(O,) int64: the step at which each optimisation (conformer, or band of ``NEB``) converged in the current
+        ``run``, -1 if it has not."""
         return self._conv.cpu().numpy()
 
     @property
@@ -198,6 +208,24 @@ class _Optimizer(_DeviceLoop):
             z = np.zeros((0, self.n_conf))
             return Log(np.zeros(0, dtype=np.int64), z, z.copy())
         return self._as_log(np.concatenate(self._log))
+
+
+def _fire_params(dt, maxstep, dtmax, n_min, finc, fdec, astart, fa) -> tp.Tuple[float, ...]:
+    """ASE's FIRE parameters, checked: the first eight columns of the parameter row of ani_opt_state."""
+    dt, maxstep, dtmax, n_min = float(dt), float(maxstep), float(dtmax), float(n_min)
+    finc, fdec, astart, fa = float(finc), float(fdec), float(astart), float(fa)
+    par = (dt, maxstep, dtmax, n_min, finc, fdec, astart, fa)
+    if not all(math.isfinite(p) for p in par):
+        raise ValueError("the FIRE parameters must be finite")
+    if not (dt > 0 and maxstep > 0 and dtmax > 0):
+        raise ValueError("dt, maxstep and dtmax must be > 0")
+    if not (0 < fdec < 1 <= finc):
+        raise ValueError("FIRE needs 0 < fdec < 1 <= finc")
+    if not (0 < fa <= 1 and 0 <= astart <= 1):
+        raise ValueError("FIRE needs 0 < fa <= 1 and 0 <= astart <= 1")
+    if n_min < 0:
+        raise ValueError("n_min must be >= 0")
+    return par
 
 
 class FIRE(_Optimizer):
@@ -224,19 +252,7 @@ class FIRE(_Optimizer):
     def __init__(self, model, atomic_numbers, positions, cell=None, pbc=False, fixed=None, dt: float = 0.1,
                  maxstep: float = 0.2, dtmax: float = 1.0, n_min: int = 5, finc: float = 1.1, fdec: float = 0.5,
                  astart: float = 0.1, fa: float = 0.99, steps_per_replay: int = 20):
-        dt, maxstep, dtmax, n_min = float(dt), float(maxstep), float(dtmax), float(n_min)
-        finc, fdec, astart, fa = float(finc), float(fdec), float(astart), float(fa)
-        par = (dt, maxstep, dtmax, n_min, finc, fdec, astart, fa)
-        if not all(math.isfinite(p) for p in par):
-            raise ValueError("the FIRE parameters must be finite")
-        if not (dt > 0 and maxstep > 0 and dtmax > 0):
-            raise ValueError("dt, maxstep and dtmax must be > 0")
-        if not (0 < fdec < 1 <= finc):
-            raise ValueError("FIRE needs 0 < fdec < 1 <= finc")
-        if not (0 < fa <= 1 and 0 <= astart <= 1):
-            raise ValueError("FIRE needs 0 < fa <= 1 and 0 <= astart <= 1")
-        if n_min < 0:
-            raise ValueError("n_min must be >= 0")
+        par = _fire_params(dt, maxstep, dtmax, n_min, finc, fdec, astart, fa)
         # state: [v 3n | scalars 2 C 3 | counter 2 | (CellFIRE: master 2 C 27)]
         c64, st_words = self._allocate(model, atomic_numbers, positions, cell, pbc, fixed, steps_per_replay)
         dev, C_, A = self.device, self.n_conf, self.n_per_conf
@@ -540,3 +556,278 @@ class LBFGS(_Optimizer):
         idx = torch.as_tensor(np.stack([(h - L + np.arange(L)) % M for h in head]), device=self.device)
         take = idx.view(self.n_conf, L, 1, 1).expand(-1, -1, self.n_per_conf, 3)
         return torch.gather(self._s, 1, take), torch.gather(self._y, 1, take)
+
+
+class NEBLog(tp.NamedTuple):
+    """One record per step and band of ``NEB`` (steps ascending)."""
+    step: np.ndarray   # (S,) int64
+    emax: np.ndarray   # (S, B) Hartree: the largest interior energy at the step, E_imax
+    fmax: np.ndarray   # (S, B) eV / A: the largest NEB force on a movable atom of the band's interior images
+    imax: np.ndarray   # (S, B) int64: the image of E_imax (1 .. n - 2)
+
+
+_NEB_METHODS = {"aseneb": _lib.ANI_NEB_ASENEB, "improvedtangent": _lib.ANI_NEB_IMPROVED_TANGENT}
+
+
+class NEB(_Optimizer):
+    """A nudged elastic band relaxed by FIRE on the device: ASE's ``FIRE(NEB(images, k, climb, method))`` for every
+    band of a batch, with the interior images of all bands evaluated by one force step.
+
+    A band has images 0 .. n - 1 (n >= 3); the endpoints never move.  Interior image i of band b is conformer
+    b (n - 2) + i - 1 of the force step.  Per interior image, with F its forces (eV / A; zero for fixed and padding
+    atoms), t- = x_i - x_{i-1}, t+ = x_{i+1} - x_i (zero on those atoms), k- = k_{i-1}, k+ = k_i and imax = 1 + the
+    first index of the largest of E_1 .. E_{n-2}, the tangent is tau = alpha t- + beta t+ and
+
+        method="aseneb" (ASE's default): (alpha, beta) = (0, 1) below imax, (1, 0) above it and (1, 1) at imax;
+            m = tau.tau (1 if 0); climbing image f = F - 2 (F.tau / m) tau, every other image
+            f = F - ((F.tau + (k- t- - k+ t+).tau) / m) tau
+        method="improvedtangent" (Henkelman & Jonsson, J. Chem. Phys. 113, 9978 (2000)): (0, 1) where the energy rises
+            through the image, (1, 0) where it falls, else weights |dE| max / min by the higher neighbour;
+            u = tau / |tau|; climbing image f = F - 2 (F.u) u, every other image f = F - (F.u) u + (k+ |t+| - k- |t-|) u
+
+    The one deviation from ASE: |tau| = 0 with "improvedtangent", where ASE divides by zero, gives u = 0.  The climbing
+    image (Henkelman, Uberuaga & Jonsson, J. Chem. Phys. 113, 9901 (2000)) is image imax of each band when ``climb``
+    is set; ``neb.climb = True`` before a second ``run`` continues with the FIRE state kept, as ASE's second
+    ``opt.run()`` does.  FIRE (that of ``FIRE``) runs per band over the rows of its interior images: P, F2, V2, the
+    maxstep clamp and fmax = max_i |f_i| (row norms of the NEB forces, as ASE 3.22's ``Optimizer.converged``) are the
+    band's; a converged band's positions freeze.  The endpoint energies come from one force step at construction.
+
+    Args:
+        model: a ``torchani_b200.models.ANI`` on a CUDA device
+        atomic_numbers: (A,) or (B, A); -1 pads
+        images: (n, A, 3) or (B, n, A, 3) Angstrom, endpoints included (``interpolate`` makes a linear band)
+        cell: None, (3, 3) shared by every band, or (B, 3, 3) one per band (fixed); pbc: fully periodic or open
+        fixed: None, or an (A,) or (B, A) boolean mask of atoms that never move; their positions must be the same in
+            every image of a band
+        k: spring constants, eV / A^2: a scalar, (n - 1,) or (B, n - 1); spring j joins images j and j + 1
+        climb: the climbing image; method: "aseneb" or "improvedtangent"
+        dt, maxstep, dtmax, n_min, finc, fdec, astart, fa, steps_per_replay: those of ``FIRE``
+    ASE's ``remove_rotation_and_translation`` and ``precon`` are rejected, as are its "eb", "spline" and "string"
+    methods.
+    """
+
+    _what = "the device NEB"
+    _fmax_col = 8
+    _record_words = _lib.ANI_NEB_RECORD
+
+    def __init__(self, model, atomic_numbers, images, cell=None, pbc=False, fixed=None, k=0.1, climb: bool = False,
+                 method: str = "aseneb", dt: float = 0.1, maxstep: float = 0.2, dtmax: float = 1.0, n_min: int = 5,
+                 finc: float = 1.1, fdec: float = 0.5, astart: float = 0.1, fa: float = 0.99,
+                 steps_per_replay: int = 20, remove_rotation_and_translation: bool = False, precon=None):
+        if method not in _NEB_METHODS:
+            raise ValueError(f"method must be 'aseneb' or 'improvedtangent', got {method!r} (ASE's 'eb', 'spline' and "
+                             "'string' are not supported)")
+        if remove_rotation_and_translation:
+            raise ValueError("remove_rotation_and_translation is not supported")
+        if precon is not None:
+            raise ValueError("preconditioned NEB is not supported")
+        par = _fire_params(dt, maxstep, dtmax, n_min, finc, fdec, astart, fa)
+        x = np.asarray(images if not isinstance(images, Tensor) else images.detach().cpu(), dtype=np.float64)
+        if x.ndim == 3:
+            x = x[None]
+        if x.ndim != 4 or x.shape[-1] != 3:
+            raise ValueError(f"images must be (n, A, 3) or (B, n, A, 3), got {x.shape}")
+        B, n, A = x.shape[:3]
+        if n < 3:
+            raise ValueError(f"a band needs n >= 3 images, got {n}")
+        m = n - 2
+        if B * m > 65535:
+            raise ValueError(f"B (n - 2) = {B * m} interior images exceed 65535")
+        if not np.isfinite(x).all():
+            raise ValueError("images must be finite")
+        z = np.asarray(atomic_numbers if not isinstance(atomic_numbers, Tensor) else atomic_numbers.cpu())
+        if z.shape not in ((A,), (B, A)):
+            raise ValueError(f"atomic_numbers must be ({A},) or ({B}, {A}), got {z.shape}")
+        z = np.broadcast_to(z.reshape(-1, A), (B, A))
+        fix = np.zeros((B, A), dtype=bool)
+        if fixed is not None:
+            f = np.asarray(fixed if not isinstance(fixed, Tensor) else fixed.cpu())
+            if f.dtype != bool or f.shape not in ((A,), (B, A)):
+                raise ValueError(f"fixed must be a boolean mask of shape ({A},) or ({B}, {A}), got {f.dtype} {f.shape}")
+            fix[:] = f
+        for b in range(B):   # t is zeroed on fixed atoms: ASE's result only if they sit still along the band
+            if not (x[b][:, fix[b]] == x[b, 0][fix[b]]).all():
+                raise ValueError(f"fixed atoms must have the same positions in every image of a band (band {b})")
+        kk = np.asarray(k, dtype=np.float64)
+        if kk.shape not in ((), (n - 1,), (B, n - 1)):
+            raise ValueError(f"k must be a scalar, ({n - 1},) or ({B}, {n - 1}), got {kk.shape}")
+        kk = np.array(np.broadcast_to(kk, (B, n - 1)), order="C")   # (numpy's copy of a broadcast is not C-order)
+        if not (np.isfinite(kk) & (kk > 0)).all():
+            raise ValueError("k must be finite and > 0 (eV / A^2)")
+        # the cell of the force step: shared (grid mode 2) or one per interior image (grid mode 3)
+        fcell = None
+        if cell is not None:
+            h = np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float64)
+            if h.shape not in ((3, 3), (B, 3, 3)):
+                raise ValueError(f"cell must be (3, 3) or ({B}, 3, 3), got {h.shape}")
+            fcell = h.reshape(3, 3) if h.ndim == 2 or B == 1 else np.repeat(h, m, 0)
+        self.n_bands, self.n_images, self.method = B, n, method
+        self._climb = bool(climb)
+        c64, st_words = self._allocate(model, np.repeat(z, m, 0), x[:, 1:-1].reshape(B * m, A, 3), fcell, pbc,
+                                       np.repeat(fix, m, 0), steps_per_replay)
+        dev, C_ = self.device, self.n_conf
+        nn_ = C_ * A
+        ns = 2 * B * _lib.ANI_OPT_SCALARS
+        self.v = st_words[:3 * nn_].view(C_, A, 3)
+        self._scalars = st_words[3 * nn_:3 * nn_ + ns].view(2, B, _lib.ANI_OPT_SCALARS)
+        self._counter = st_words[3 * nn_ + ns:3 * nn_ + ns + 2].view(torch.int64)
+        f64 = dict(dtype=torch.float64, device=dev)
+        params = np.zeros((B, _lib.ANI_OPT_PARAMS))
+        params[:, :8] = par
+        self.params = torch.from_numpy(params).to(**f64)
+        nb = -(-A // _lib.ANI_MD_BLOCK)
+        self._partials = torch.zeros(C_ * nb * 4, **f64)
+        self._dots = torch.zeros(C_ * nb * _lib.ANI_NEB_DOTS, **f64)
+        self._neb_force = torch.zeros(C_, A, 3, **f64)
+        self.endpoints = torch.from_numpy(np.ascontiguousarray(x[:, [0, n - 1]])).to(**f64)
+        self.end_energies = torch.zeros(B, 2, **f64)
+        self.springs = torch.from_numpy(kk).to(**f64)
+        self._climb_dev = torch.full((B,), 1.0 if self._climb else 0.0, **f64)
+        st = _lib.NebState()
+        fs = st.fire
+        fs.x, fs.v, fs.force_scale, fs.params = ptr(self.x), ptr(self.v), ptr(self.force_scale), ptr(self.params)
+        fs.scalars, fs.counter, fs.conv_step = ptr(self._scalars), ptr(self._counter), ptr(self._conv)
+        fs.record, fs.partials = ptr(self._record_dev), ptr(self._partials)
+        fs.n_conf, fs.n_per_conf, fs.record_rows = B, m * A, self.K
+        st.endpoints, st.end_energies, st.springs = ptr(self.endpoints), ptr(self.end_energies), ptr(self.springs)
+        st.climb, st.neb_force, st.dots = ptr(self._climb_dev), ptr(self._neb_force), ptr(self._dots)
+        st.n_images, st.n_atoms, st.method = n, A, _NEB_METHODS[method]
+        self._state = st
+        self._endpoint_energies()
+        self._start()
+
+    @property
+    def _n_opt(self) -> int:
+        return self.n_bands
+
+    def _state_words(self) -> int:
+        return 3 * self.n_conf * self.n_per_conf + 2 * self.n_bands * _lib.ANI_OPT_SCALARS + 2
+
+    def _endpoint_energies(self) -> None:
+        """One force step on the 2B endpoint conformers, at float32 coordinates wrapped as the loop writes them."""
+        B, A, dev = self.n_bands, self.n_per_conf, self.device
+        m = self.n_images - 2
+        z = self.species.view(B, m, A)[:, :1].expand(B, 2, A).reshape(2 * B, A)
+        xe = self.endpoints.reshape(2 * B, A, 3)
+        cell = None
+        if self.pbc:
+            h = self._cell32.double().view(-1, 3, 3)
+            h = h[::m].repeat_interleave(2, 0) if self.per_conf else h.expand(2 * B, 3, 3)
+            xe = xe - torch.floor(xe @ torch.linalg.inv(h)) @ h
+            cell = self._cell32.view(-1, 3, 3)[::m].repeat_interleave(2, 0) if self.per_conf else self._cell32
+        with torch.cuda.device(dev):
+            while True:
+                try:
+                    r = self.model.engine(dev).step(z, xe.float(), cell, self.pbc, check=True)
+                    break
+                except _lib.OperandRangeError:
+                    nets = self.model.neural_networks
+                    if nets._variant == "bf16x3" or not _lib.available("bf16x3"):
+                        raise
+                    warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this "
+                                  "model to the 3 x bfloat16 build of the library")
+                    nets.use_variant("bf16x3")
+            self.end_energies.copy_(r.energies.view(B, 2))
+        self._end_variant = self.model.neural_networks._variant
+
+    def _attached(self) -> None:
+        if self.model.neural_networks._variant != self._end_variant:   # switched to 3 x bfloat16: endpoints too
+            self._endpoint_energies()
+
+    @property
+    def climb(self) -> bool:
+        """Whether image imax of every band climbs.  Setting it writes the device word the next step and
+        ``neb_forces`` read, so ``neb.climb = True; neb.run(...)`` continues with the FIRE state kept."""
+        return self._climb
+
+    @climb.setter
+    def climb(self, value: bool) -> None:
+        self._climb = bool(value)
+        self._climb_dev.fill_(1.0 if self._climb else 0.0)
+
+    # -- the device loop ------------------------------------------------------------------------
+    def _init_launch(self, reset: bool) -> None:
+        """ani_b200_neb_init (v = 0 and the initial scalars at the start only)."""
+        check(self.engine.lib.ani_b200_neb_init(
+            C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, self._cell_mode(),
+            int(reset), ptr(self.ws.coords), self._stream()), "neb_init")
+
+    def _integrate(self) -> None:
+        """The NEB launches of one step (ani_b200_neb_step: step t to x(t+1))."""
+        ws, L = self.ws, self.engine.lib
+        if self.per_conf:
+            rc = L.ani_b200_neb_step_cells(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), ptr(ws.lattice),
+                                           ptr(ws.coords), self._stream())
+        else:
+            rc = L.ani_b200_neb_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies),
+                                     ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
+        check(rc, "neb_step")
+
+    # -- results ----------------------------------------------------------------------------------
+    @property
+    def positions(self) -> Tensor:
+        """(B, n, A, 3) float64 positions of the current step, endpoints included, unwrapped (device, a copy)."""
+        B, m, A = self.n_bands, self.n_images - 2, self.n_per_conf
+        e = self.endpoints
+        return torch.cat([e[:, :1], self.x.view(B, m, A, 3), e[:, 1:]], 1)
+
+    @property
+    def energies(self) -> Tensor:
+        """(B, n) float64 energies (Hartree) of the images at the current positions (device, a copy)."""
+        B, m = self.n_bands, self.n_images - 2
+        return torch.cat([self.end_energies[:, :1], self.ws.energies.view(B, m), self.end_energies[:, 1:]], 1)
+
+    @property
+    def forces(self) -> Tensor:
+        """(B, n - 2, A, 3) float32 forces -dE/dx (Hartree / A) of the interior images at the current positions,
+        fixed atoms included (device, a copy)."""
+        return -self.ws.grad.view(self.n_bands, self.n_images - 2, self.n_per_conf, 3)
+
+    @property
+    def neb_forces(self) -> Tensor:
+        """(B, n - 2, A, 3) float64 NEB forces (eV / A) at the current positions: ani_b200_neb_project of the last
+        force step (device, a copy)."""
+        with torch.cuda.device(self.device):
+            check(self.engine.lib.ani_b200_neb_project(C.byref(self._state), ptr(self.ws.grad),
+                                                       ptr(self.ws.energies), self._stream()), "neb_project")
+        return self._neb_force.view(self.n_bands, self.n_images - 2, self.n_per_conf, 3).clone()
+
+    @property
+    def imax(self) -> np.ndarray:
+        """(B,) int64: the image of the largest interior energy at the current positions (the first of equal ones)."""
+        e = self.ws.energies.view(self.n_bands, self.n_images - 2).cpu().numpy()
+        return 1 + np.argmax(e, 1)
+
+    @property
+    def barrier(self) -> np.ndarray:
+        """(B,) float64: E_imax - E_0 (Hartree) at the current positions."""
+        e = self.energies.cpu().numpy()
+        return e[np.arange(self.n_bands), self.imax] - e[:, 0]
+
+    @staticmethod
+    def _as_log(r: np.ndarray) -> NEBLog:
+        return NEBLog(r[:, 0, 0].astype(np.int64), r[..., 1].copy(), r[..., 2].copy(), r[..., 3].astype(np.int64))
+
+    @property
+    def log(self) -> NEBLog:
+        if not self._log:
+            return self._as_log(np.zeros((0, self.n_bands, _lib.ANI_NEB_RECORD)))
+        return self._as_log(np.concatenate(self._log))
+
+
+def interpolate(initial, final, n_images: int, cell=None, mic: bool = False) -> np.ndarray:
+    """ASE's linear ``NEB.interpolate()`` on the host: (n_images, A, 3) float64 images from ``initial`` to ``final``
+    (each (A, 3)), endpoints included.  With ``mic`` the displacement of every atom is taken to its nearest periodic
+    image under ``cell`` (rows are lattice vectors), as ASE's ``interpolate(mic=True)``."""
+    a = np.asarray(initial, dtype=np.float64)
+    d = np.asarray(final, dtype=np.float64) - a
+    if int(n_images) < 2 or a.shape != d.shape or a.ndim != 2 or a.shape[1] != 3:
+        raise ValueError("interpolate needs n_images >= 2 and initial, final of the same (A, 3) shape")
+    if mic:
+        if cell is None:
+            raise ValueError("mic needs a cell")
+        h = np.asarray(cell, dtype=np.float64).reshape(3, 3)
+        f = d @ np.linalg.inv(h)
+        d = (f - np.round(f)) @ h
+    s = np.arange(int(n_images)).reshape(-1, 1, 1) / (int(n_images) - 1)
+    return a[None] + s * d[None]
