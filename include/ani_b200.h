@@ -808,7 +808,8 @@ int ani_b200_hessian_assemble(const int32_t* nbr_cnt, const int32_t* nbr_list, i
 /*                     force_stdev f32[n], the query-by-committee step's energy QBC and force_relative_stdev, both or  */
 /*                     neither): a running conformer whose qbc or largest force_stdev exceeds its threshold stops at     */
 /*                     t: stop_step = t, trigger = x(t), v(t); its x and v never change again.  Sums are float64 in a   */
-/*                     fixed order: the same state and forces give the same bits.                                     */
+/*                     fixed order: the same state and forces give the same bits.  n_conf > 65535 or n_conf n_per_conf  */
+/*                     > INT_MAX: ANI_ERR_UNSUPPORTED (before any CUDA call).                                          */
 /*  ani_b200_md_step_cells  the same with one cell per conformer: the lattice table of grid mode 3                     */
 /*                     (f32[n_conf][ANI_LATTICE_STRIDE], written by ani_b200_prepare_step_cells) in place of `cell`.    */
 /*  ani_b200_md_noise  out f64[n][3]: the standard normals the O step of step `step` draws for atoms 0..n-1 (flat index */

@@ -122,6 +122,14 @@ def test_argument_validation_without_gpu():
     # the _cells form of D3 without its lattice table
     assert d3(ok_list, 3, cells=True, lattice=None) == -1
 
+    # an MD step over more conformers than a grid's y extent holds
+    st = _lib.MDState()
+    for name in ("x", "v", "inv_mass", "params", "counter", "stop_step", "thermo", "partials"):
+        setattr(st, name, h.value)
+    st.accel, st.kb, st.integrator, st.thermo_rows = 1.0, 1.0, _lib.MD_VERLET, 1
+    st.n_conf, st.n_per_conf = 65536, 1
+    assert L.ani_b200_md_step(C.byref(st), h, h, None, None, None, h, None) == -2
+
 
 def test_product_package_does_not_import_the_oracle():
     """The oracle is test infrastructure: nothing under torchani_b200/ may reference it."""

@@ -19,6 +19,7 @@ from torch import Tensor
 
 from . import _lib
 from .models import ANI
+from .nn import fall_back_to_bf16x3
 
 HARTREE_TO_EV = 27.211386024367243  # units.py (CODATA 2014, as used by the reference's ASE interface)
 
@@ -291,13 +292,8 @@ class HostCalculator:
         try:
             self.engine.check_status(self.ws)
         except _lib.OperandRangeError:
-            nets = self.model.neural_networks
-            if nets._variant == "bf16x3" or not _lib.available("bf16x3") or self.sharded is not None:
+            if self.sharded is not None or not fall_back_to_bf16x3(self.model.neural_networks):
                 raise
-            import warnings
-            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this "
-                          "model to the 3 x bfloat16 build of the library")
-            nets.use_variant("bf16x3")
             self.engine = self.model.engine(self.device)
             self.engine.skin = self.skin
             self.ws = self._workspace()

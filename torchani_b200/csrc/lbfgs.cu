@@ -39,14 +39,8 @@ constexpr int LB_TILE = ANI_LBFGS_TILE;          // atoms per dot-sweep tile and
 constexpr int LB_ROWS = LB_THREADS / ANI_WARP;   // rows per dot-sweep block: one warp each
 constexpr int LB_SOLVE = 128;                    // threads of a solve block
 
-struct LbfgsArgs {
+struct LbfgsArgs : LoopArgs {
   ani_lbfgs_state s;
-  const float* grad;          // f32[n][3] dE/dx (Hartree / A), input order
-  const double* energies;     // f64[n_conf]
-  const float* cells;         // cell rows (f32[9]) of conformer c at cells + c * cell_stride; nullptr = open
-  int cell_stride;
-  float* coords;              // f32[n][3]
-  int reset;                  // (ani_b200_lbfgs_init)
 };
 
 __device__ __forceinline__ int ring_slots(const ani_lbfgs_state& s) { return s.memory + 1; }
@@ -75,13 +69,6 @@ __device__ __forceinline__ void grad_of(const LbfgsArgs& a, size_t i, double* g)
   g[0] = (double)a.grad[3 * i + 0] * fs;
   g[1] = (double)a.grad[3 * i + 1] * fs;
   g[2] = (double)a.grad[3 * i + 2] * fs;
-}
-
-// the maximum over a warp by a fixed tree towards lane 0
-__device__ __forceinline__ double warp_max(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_down_sync(ANI_FULL_MASK, v, o));
-  return v;
 }
 
 // launch 1: the new pair and the dot products of every row with g and y_new, per tile of atoms (see the file comment)
@@ -121,7 +108,7 @@ __global__ void __launch_bounds__(LB_THREADS) k_lbfgs_dots(const __grid_constant
       }
     }
     if (grp == 0) {
-      f2 = warp_max(f2);
+      warp_tree<0, 1>(&f2);
       if (lane == 0) wmax[threadIdx.x / ANI_WARP] = f2;
     }
   }
@@ -149,21 +136,11 @@ __global__ void __launch_bounds__(LB_THREADS) k_lbfgs_dots(const __grid_constant
       d[3] += ye * sy[e];
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-    for (int q = 0; q < 4; ++q) d[q] += __shfl_down_sync(ANI_FULL_MASK, d[q], o);
+  warp_tree<4, 0>(d);
   if (lane == 0) {
     double* out = dot_partials(s, c, tile) + 4 * r;
     for (int q = 0; q < 4; ++q) out[q] = d[q];
   }
-}
-
-// the sum of a lane-strided partial over warp 0 by a fixed tree, broadcast to every lane
-__device__ __forceinline__ double warp_sum_all(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(ANI_FULL_MASK, v, o);
-  return __shfl_sync(ANI_FULL_MASK, v, 0);
 }
 
 // launch 2: one block per conformer (see the file comment); dynamic shared memory: R f64[memory][memory], then the
@@ -183,10 +160,10 @@ __global__ void __launch_bounds__(LB_SOLVE) k_lbfgs_solve(const __grid_constant_
   const long long t = s.counter[1], k = s.iter[2 * c], head = s.iter[2 * c + 1];
   const double* par = s.params + (size_t)c * ANI_LBFGS_PARAMS;   // maxstep, damping, H0, fmax
   const double h0 = par[2];
-  if (threadIdx.x < ANI_WARP) {   // fmax(t): the tiles' maxima, lane-strided, then a fixed tree
-    double m = 0.0;
-    for (int b = threadIdx.x; b < nt; b += ANI_WARP) m = fmax(m, fmax_partials(s, c)[b]);
-    m = warp_max(m);
+  if (threadIdx.x < ANI_WARP) {   // fmax(t): warp_reduce of the tiles' maxima
+    const double* fp = fmax_partials(s, c);
+    double m;
+    warp_reduce<0, 1>(threadIdx.x, nt, [&](int b, double* v) { v[0] = fp[b]; }, &m);
     if (threadIdx.x == 0) {
       const double fm = sqrt(m);
       double* row = s.record + ((size_t)(t % s.record_rows) * s.n_conf + c) * ANI_LBFGS_RECORD;
@@ -255,7 +232,8 @@ __global__ void __launch_bounds__(LB_SOLVE) k_lbfgs_solve(const __grid_constant_
     const double* yrow = YY + (size_t)slot[i] * M;
     double acc = 0.0;
     for (int j = threadIdx.x % ANI_WARP; j < L; j += ANI_WARP) acc += yrow[slot[j]] * rv[j];
-    acc = warp_sum_all(acc);
+    warp_tree<1, 0>(&acc);
+    acc = __shfl_sync(ANI_FULL_MASK, acc, 0);   // (to every lane: the row loop compiles shorter than for lane 0 only)
     if (threadIdx.x % ANI_WARP == 0) av[i] = R[i * L + i] * rv[i] + h0 * acc - h0 * tot[M + drop + i];
   }
   __syncthreads();
@@ -336,7 +314,7 @@ __global__ void __launch_bounds__(LB_THREADS) k_lbfgs_direction(const __grid_con
       const double* v = part[0] + 3 * threadIdx.x;
       p2 = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
     }
-    p2 = warp_max(p2);
+    warp_tree<0, 1>(&p2);
     if (threadIdx.x == 0) pmax_partials(s, c)[blockIdx.x] = p2;
   }
 }
@@ -347,10 +325,10 @@ __global__ void __launch_bounds__(LB_THREADS) k_lbfgs_move(const __grid_constant
   const ani_lbfgs_state& s = a.s;
   const int c = blockIdx.y, j = blockIdx.x * LB_THREADS + threadIdx.x;
   if (s.conv_step[c] >= 0) return;   // converged at this step or before: nothing moves
-  if (threadIdx.x < ANI_WARP) {   // max_i |p_i|^2: the direction blocks' maxima, lane-strided, then a fixed tree
-    double m = 0.0;
-    for (int b = threadIdx.x; b < n_tiles(s); b += ANI_WARP) m = fmax(m, pmax_partials(s, c)[b]);
-    m = warp_max(m);
+  if (threadIdx.x < ANI_WARP) {   // max_i |p_i|^2: warp_reduce of the direction blocks' maxima
+    const double* pp = pmax_partials(s, c);
+    double m;
+    warp_reduce<0, 1>(threadIdx.x, n_tiles(s), [&](int b, double* v) { v[0] = pp[b]; }, &m);
     if (threadIdx.x == 0) {
       const double maxstep = s.params[(size_t)c * ANI_LBFGS_PARAMS], longest = sqrt(m);
       scale = longest >= maxstep ? maxstep / longest : 1.0;   // ASE's determine_step: the longest atom step
@@ -376,7 +354,6 @@ __global__ void __launch_bounds__(LB_THREADS) k_lbfgs_move(const __grid_constant
 
 // one CTA per conformer: with reset, x_prev = x, g_prev = 0 and {k, head} = {0, 0}; then the coordinates of x
 __global__ void __launch_bounds__(LB_THREADS) k_lbfgs_init(const __grid_constant__ LbfgsArgs a) {
-  __shared__ double cell[9], inv[9];
   const ani_lbfgs_state& s = a.s;
   const int c = blockIdx.x, A = s.n_per_conf;
   const size_t base = (size_t)c * A;
@@ -390,12 +367,7 @@ __global__ void __launch_bounds__(LB_THREADS) k_lbfgs_init(const __grid_constant
       s.iter[2 * c + 1] = 0;
     }
   }
-  load_cell(a.cells, a.cell_stride, c, cell, inv);
-  __syncthreads();
-  for (int j = threadIdx.x; j < A; j += LB_THREADS) {
-    const size_t i = base + j;
-    write_coords(a.coords, i, s.x[3 * i + 0], s.x[3 * i + 1], s.x[3 * i + 2], a.cells, cell, inv);
-  }
+  conformer_coords(a, c, A, s.x);
 }
 
 size_t solve_smem(int memory) {
@@ -412,14 +384,9 @@ int lbfgs_step(const ani_lbfgs_state* s, const float* grad, const double* energi
                int cell_stride, float* coords, void* stream) {
   if (!lbfgs_state_ok(s) || !s->conv_step || !s->record || !s->partials || s->record_rows < 1) return ANI_ERR_BAD_ARG;
   if (!grad || !energies || !coords) return ANI_ERR_BAD_ARG;
-  if ((long long)s->n_conf * s->n_per_conf > 0x7fffffffLL || s->n_conf > 65535) return ANI_ERR_UNSUPPORTED;
-  LbfgsArgs a = {};
-  a.s = *s;
-  a.grad = grad;
-  a.energies = energies;
-  a.cells = cells;
-  a.cell_stride = cell_stride;
-  a.coords = coords;
+  const int rc = launch_shape(s->n_conf, s->n_per_conf);
+  if (rc != ANI_OK) return rc;
+  const LbfgsArgs a = {{grad, energies, cells, cell_stride, coords, 0}, *s};
   const int tiles = (s->n_per_conf + LB_TILE - 1) / LB_TILE, groups = (s->memory + 1 + LB_ROWS - 1) / LB_ROWS;
   const size_t smem = solve_smem(s->memory);
   if (cudaFuncSetAttribute(k_lbfgs_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
@@ -439,12 +406,9 @@ using namespace ani;
 
 extern "C" int ani_b200_lbfgs_init(const ani_lbfgs_state* state, const float* cells, int cell_mode, int reset,
                                    float* coords, void* stream) {
-  if (!lbfgs_state_ok(state) || !coords || cell_mode < 0 || cell_mode > 2 || (cell_mode && !cells))
-    return ANI_ERR_BAD_ARG;
   LbfgsArgs a = {};
+  if (!lbfgs_state_ok(state) || !coords || !init_cells(a, cells, cell_mode)) return ANI_ERR_BAD_ARG;
   a.s = *state;
-  a.cells = cell_mode ? cells : nullptr;
-  a.cell_stride = cell_mode == 2 ? 9 : 0;
   a.coords = coords;
   a.reset = reset != 0;
   k_lbfgs_init<<<state->n_conf, LB_THREADS, 0, (cudaStream_t)stream>>>(a);

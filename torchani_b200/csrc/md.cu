@@ -26,16 +26,10 @@ namespace ani {
 
 constexpr int MD_BLOCK = ANI_MD_BLOCK;
 
-struct MdArgs {
+struct MdArgs : LoopArgs {
   ani_md_state s;
-  const float* grad;          // f32[n][3] dE/dx (Hartree / A), input order
-  const double* energies;     // f64[n_conf]
   const double* qbc;          // f64[n_conf] or nullptr (no stop check)
   const float* force_stdev;   // f32[n] force_relative_stdev or nullptr
-  const float* cells;         // cell rows (f32[9]) of conformer c at cells + c * cell_stride; nullptr = open
-  int cell_stride;
-  float* coords;              // f32[n][3]
-  int zero_momentum;          // (ani_b200_md_init)
   ani_md_barostat baro;       // ani_b200_md_step_npt; baro.master == nullptr for NVE / NVT
 };
 
@@ -149,29 +143,24 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_start(const __grid_constant__ M
   const int c = blockIdx.y, j = blockIdx.x * MD_BLOCK + threadIdx.x, nb = gridDim.x;
   const long long t = s.counter[1];
   const double* par = s.params + (size_t)c * ANI_MD_PARAMS;
-  if (threadIdx.x < 32) {   // the conformer's partials: lane-strided in order, then a fixed tree towards lane 0
-    double ke = 0.0, fm = 0.0;
-    for (int b = threadIdx.x; b < nb; b += 32) {
-      ke += s.partials[2 * ((size_t)c * nb + b)];
-      fm = fmax(fm, s.partials[2 * ((size_t)c * nb + b) + 1]);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      ke += __shfl_down_sync(ANI_FULL_MASK, ke, o);
-      fm = fmax(fm, __shfl_down_sync(ANI_FULL_MASK, fm, o));
-    }
+  if (threadIdx.x < 32) {   // the conformer's {E_kin, max force stdev}, by warp_reduce of its partials
+    const double* p = s.partials + 2 * (size_t)c * nb;
+    double r[2];
+    warp_reduce<1, 1>(threadIdx.x, nb, [&](int b, double* v) {
+      v[0] = p[2 * b];
+      v[1] = p[2 * b + 1];
+    }, r);
     if (threadIdx.x == 0) {
-      tot[0] = ke;
-      tot[1] = fm;
+      tot[0] = r[0];
+      tot[1] = r[1];
     }
   } else if (npt && threadIdx.x < 64) {   // the trace of the conformer's virial slots, in the same fixed order
-    const int l = threadIdx.x - 32;
     const double* w = a.baro.virial + (size_t)c * a.baro.virial_slots * 9;
-    double tr = 0.0;
-    for (int k = l; k < a.baro.virial_slots; k += 32) tr += w[9 * k] + w[9 * k + 4] + w[9 * k + 8];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) tr += __shfl_down_sync(ANI_FULL_MASK, tr, o);
-    if (l == 0) tot[2] = tr;
+    double tr;
+    warp_reduce<1, 0>(threadIdx.x - 32, a.baro.virial_slots, [&](int k, double* v) {
+      v[0] = w[9 * k] + w[9 * k + 4] + w[9 * k + 8];
+    }, &tr);
+    if (threadIdx.x == 32) tot[2] = tr;
   }
   if (npt) {
     __syncthreads();
@@ -265,11 +254,11 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_start(const __grid_constant__ M
 
 // one CTA per conformer: optional removal of the centre-of-mass momentum, then the coordinates of step 0
 __global__ void __launch_bounds__(MD_BLOCK) k_md_init(const __grid_constant__ MdArgs a) {
-  __shared__ double sv[MD_BLOCK], sw[MD_BLOCK], cell[9], inv[9], tot[4];
+  __shared__ double sv[MD_BLOCK], sw[MD_BLOCK], tot[4];
   const ani_md_state& s = a.s;
   const int c = blockIdx.x, A = s.n_per_conf;
   const size_t base = (size_t)c * A;
-  if (a.zero_momentum) {
+  if (a.reset) {
     for (int k = 0; k < 4; ++k) {   // the momentum components sum m v_k, then the total mass
       double p = 0.0, unused = 0.0;
       for (int j = threadIdx.x; j < A; j += MD_BLOCK) {
@@ -285,12 +274,7 @@ __global__ void __launch_bounds__(MD_BLOCK) k_md_init(const __grid_constant__ Md
         for (int k = 0; k < 3; ++k) s.v[3 * (base + j) + k] -= tot[k] / tot[3];
     }
   }
-  load_cell(a.cells, a.cell_stride, c, cell, inv);
-  __syncthreads();
-  for (int j = threadIdx.x; j < A; j += MD_BLOCK) {
-    const size_t i = base + j;
-    write_coords(a.coords, i, s.x[3 * i + 0], s.x[3 * i + 1], s.x[3 * i + 2], a.cells, cell, inv);
-  }
+  conformer_coords(a, c, A, s.x);
 }
 
 __global__ void __launch_bounds__(MD_BLOCK) k_md_noise(unsigned long long seed, long long step, int n, double* out) {
@@ -316,18 +300,9 @@ int md_step(const ani_md_state* s, const float* grad, const double* energies, co
   if ((s->integrator != ANI_MD_VERLET && s->integrator != ANI_MD_LANGEVIN) || s->thermo_rows < 1) return ANI_ERR_BAD_ARG;
   if (s->record_every < 0 || (s->record_every > 0 && (!s->frames || s->frame_slots < 1))) return ANI_ERR_BAD_ARG;
   if (!(s->accel > 0.0) || !(s->kb > 0.0)) return ANI_ERR_BAD_ARG;
-  if ((long long)s->n_conf * s->n_per_conf > 0x7fffffffLL) return ANI_ERR_UNSUPPORTED;
-  MdArgs a;
-  a.s = *s;
-  a.grad = grad;
-  a.energies = energies;
-  a.qbc = qbc;
-  a.force_stdev = force_stdev;
-  a.cells = cells;
-  a.cell_stride = cell_stride;
-  a.coords = coords;
-  a.zero_momentum = 0;
-  a.baro = baro ? *baro : ani_md_barostat{};
+  const int rc = launch_shape(s->n_conf, s->n_per_conf);
+  if (rc != ANI_OK) return rc;
+  MdArgs a = {{grad, energies, cells, cell_stride, coords, 0}, *s, qbc, force_stdev, baro ? *baro : ani_md_barostat{}};
   const dim3 grid((s->n_per_conf + MD_BLOCK - 1) / MD_BLOCK, s->n_conf);
   cudaStream_t st = (cudaStream_t)stream;
   k_md_finish<<<grid, MD_BLOCK, 0, st>>>(a);
@@ -342,14 +317,11 @@ using namespace ani;
 
 extern "C" int ani_b200_md_init(const ani_md_state* state, const float* cells, int cell_mode, int zero_momentum,
                                 float* coords, void* stream) {
-  if (!md_state_ok(state) || !coords || cell_mode < 0 || cell_mode > 2 || (cell_mode && !cells))
-    return ANI_ERR_BAD_ARG;
   MdArgs a = {};
+  if (!md_state_ok(state) || !coords || !init_cells(a, cells, cell_mode)) return ANI_ERR_BAD_ARG;
   a.s = *state;
-  a.cells = cell_mode ? cells : nullptr;
-  a.cell_stride = cell_mode == 2 ? 9 : 0;
   a.coords = coords;
-  a.zero_momentum = zero_momentum != 0;
+  a.reset = zero_momentum != 0;
   k_md_init<<<state->n_conf, MD_BLOCK, 0, (cudaStream_t)stream>>>(a);
   ANI_CUDA_CHECK_LAUNCH();
   return ANI_OK;

@@ -1,10 +1,39 @@
-// Pieces shared by the device loops of md.cu (MD integrators), opt.cu (FIRE) and neb.cu (NEB under FIRE): the float64
-// cell determinant and inverse, the float32 coordinates of a master position wrapped into the cell, the fixed-shape
-// block tree their per-block partial sums go through, and FIRE's scalar update.
+// Pieces shared by the device loops of md.cu (MD integrators), opt.cu (FIRE, cell FIRE), lbfgs.cu (L-BFGS) and neb.cu
+// (NEB under FIRE):
+//   host      the arguments every loop launch takes (LoopArgs), the cell_mode decoding of the init entry points and the
+//             launch-shape check of the step entry points
+//   device    the float64 cell determinant and inverse; the float32 coordinates of a master position wrapped into the
+//             cell, and of a whole conformer (the tail of the one-CTA-per-conformer init kernels); the fixed-shape
+//             block tree and the ordered warp reduction their per-block partials go through; FIRE's scalar reset,
+//             scalar update and move
 #pragma once
 #include "common.cuh"
 
 namespace ani {
+
+// what every loop launch takes besides its state
+struct LoopArgs {
+  const float* grad;          // f32[n][3] dE/dx (Hartree / A), input order
+  const double* energies;     // f64[n_conf]
+  const float* cells;         // cell rows (f32[9]) of conformer c at cells + c * cell_stride; nullptr = open
+  int cell_stride;
+  float* coords;              // f32[n][3]
+  int reset;                  // the init entry point's flag (ani_b200_md_init: the centre-of-mass momentum removal)
+};
+
+// the cells of an init entry point's cell_mode (0 open, 1 one cell, 2 one per conformer) into a; false when invalid
+inline bool init_cells(LoopArgs& a, const float* cells, int cell_mode) {
+  if (cell_mode < 0 || cell_mode > 2 || (cell_mode && !cells)) return false;
+  a.cells = cell_mode ? cells : nullptr;
+  a.cell_stride = cell_mode == 2 ? 9 : 0;
+  return true;
+}
+
+// a step launch over (blocks of a conformer's atoms) x conformers: n_conf * n_per_conf atoms must fit an int and
+// n_conf the grid's y (or z) extent
+inline int launch_shape(long long n_conf, long long n_per_conf) {
+  return n_conf * n_per_conf > 0x7fffffffLL || n_conf > 65535 ? ANI_ERR_UNSUPPORTED : ANI_OK;
+}
 
 // determinant of the cell rows m
 __device__ __forceinline__ double det3(const double* m) {
@@ -54,6 +83,53 @@ __device__ __forceinline__ void write_coords(float* coords, size_t i, double x, 
   coords[3 * i + 2] = (float)z;
 }
 
+// the float32 coordinates of the master positions x of conformer c (A atoms), wrapped into its cell: the tail of the
+// one-CTA-per-conformer init kernels, after their own writes to x
+__device__ __forceinline__ void conformer_coords(const LoopArgs& a, int c, int A, const double* x) {
+  __shared__ double cell[9], inv[9];
+  load_cell(a.cells, a.cell_stride, c, cell, inv);
+  __syncthreads();
+  for (int j = threadIdx.x; j < A; j += blockDim.x) {
+    const size_t i = (size_t)c * A + j;
+    write_coords(a.coords, i, x[3 * i + 0], x[3 * i + 1], x[3 * i + 2], a.cells, cell, inv);
+  }
+}
+
+// the fixed shuffle tree towards lane 0 over a warp: the sums of v[0..NS), the maxima of v[NS..NS+NM)
+template <int NS, int NM>
+__device__ __forceinline__ void warp_tree(double* v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+    for (int k = 0; k < NS + NM; ++k) {
+      const double u = __shfl_down_sync(ANI_FULL_MASK, v[k], o);
+      v[k] = k < NS ? v[k] + u : fmax(v[k], u);
+    }
+}
+
+// the ordered reduction of n partials by one warp (lane = the thread's lane): lane l sums (and takes maxima of)
+// partials l, l + 32, ... in order, then warp_tree; lane 0 gets the totals.  part(b, v) writes partial b's NS summed
+// and then NM maximised values to v.
+template <int NS, int NM, class Part>
+__device__ __forceinline__ void warp_reduce(int lane, int n, Part part, double* tot) {
+#pragma unroll
+  for (int k = 0; k < NS + NM; ++k) tot[k] = 0.0;
+  for (int b = lane; b < n; b += ANI_WARP) {
+    double v[NS + NM];
+    part(b, v);
+#pragma unroll
+    for (int k = 0; k < NS + NM; ++k) tot[k] = k < NS ? tot[k] + v[k] : fmax(tot[k], v[k]);
+  }
+  warp_tree<NS, NM>(tot);
+}
+
+// warp_reduce of n FIRE partials {P, F2, V2, max |f_i|^2} at p (4 words each)
+__device__ __forceinline__ void fire_totals(const double* p, int n, double* tot) {
+  warp_reduce<3, 1>(threadIdx.x, n, [&](int b, double* v) {
+    for (int k = 0; k < 4; ++k) v[k] = p[4 * (unsigned)b + k];
+  }, tot);
+}
+
 // fixed-shape tree over the block (blockDim.x == ANI_MD_BLOCK): the sums of v[0..NS), the max of w; thread 0 gets the
 // results.  sv holds NS * ANI_MD_BLOCK doubles, sw ANI_MD_BLOCK.
 template <int NS>
@@ -74,6 +150,30 @@ __device__ __forceinline__ void block_reduce(double* v, double& w, double* sv, d
 #pragma unroll
   for (int k = 0; k < NS; ++k) v[k] = sv[k * ANI_MD_BLOCK];
   w = sw[0];
+}
+
+// FIRE's scalars {dt0, astart, 0} of optimisation c at the parity slot of step t
+__device__ __forceinline__ void fire_reset(const ani_opt_state& s, int c, long long t) {
+  const double* par = s.params + (size_t)c * ANI_OPT_PARAMS;
+  double* sc = s.scalars + ((size_t)(t & 1) * s.n_conf + c) * ANI_OPT_SCALARS;
+  sc[0] = par[0];
+  sc[1] = par[6];
+  sc[2] = 0.0;
+}
+
+// FIRE's move of one atom with force f by mix (fire_scalars): v' = c1 v + (c2 + dt) f, x += st v'; returns x(t+1) in xn
+__device__ __forceinline__ void fire_move(const double* mix, const double* f, double* v, double* x, double* xn) {
+  const double c1 = mix[0], cf = mix[1], st = mix[2];
+  const double vx = c1 * v[0] + cf * f[0], vy = c1 * v[1] + cf * f[1], vz = c1 * v[2] + cf * f[2];
+  xn[0] = x[0] + st * vx;
+  xn[1] = x[1] + st * vy;
+  xn[2] = x[2] + st * vz;
+  v[0] = vx;
+  v[1] = vy;
+  v[2] = vz;
+  x[0] = xn[0];
+  x[1] = xn[1];
+  x[2] = xn[2];
 }
 
 // FIRE's scalar update of optimisation c (a conformer of opt.cu, a band of neb.cu) at step t from the totals

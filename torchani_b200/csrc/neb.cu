@@ -11,8 +11,8 @@
 //   k_neb_project  every block sums its image's partials in order; thread 0 reads the band's energies, forms imax,
 //                  (alpha, beta) and gamma-, gamma+; every thread writes f to neb_force, and the block its FIRE
 //                  partials {f.v, f.f, v.v, max |f_i|^2}
-//   k_neb_update   every block sums all of its band's FIRE partials (lane-strided in order, then a shuffle tree, as
-//                  k_opt_update does) and runs FIRE's scalar rule (fire_scalars); the band's first block writes the
+//   k_neb_update   every block sums all of its band's FIRE partials (fire_totals, as k_opt_update does) and runs
+//                  FIRE's scalar rule (fire_scalars); the band's first block writes the
 //                  record {t, E_imax, fmax, imax}, conv_step and the scalars of t + 1; every block moves its atoms with
 //                  neb_force and writes their float32 coordinates, wrapped into the cell of its image's conformer
 // Race rules: the scalars are double-buffered by step parity; conv_step[b] and the record have one writer, the band's
@@ -25,15 +25,9 @@ namespace ani {
 
 constexpr int NEB_BLOCK = ANI_MD_BLOCK;
 
-struct NebArgs {
+struct NebArgs : LoopArgs {   // energies: f64[B (n - 2)] the interior images' energies
   ani_neb_state s;
-  const float* grad;          // f32[n][3] dE/dx (Hartree / A)
-  const double* energies;     // f64[B (n - 2)] the interior images' energies
-  const float* cells;         // cell rows (f32[9]) of conformer c at cells + c * cell_stride; nullptr = open
-  int cell_stride;
-  float* coords;              // f32[n][3]
   int step;                   // k_neb_dots copies the counter (a step, not ani_b200_neb_project)
-  int reset;                  // (ani_b200_neb_init)
 };
 
 // F, t- and t+ of atom j of interior conformer ci; returns its force_scale (0: F, t- and t+ are all 0)
@@ -180,24 +174,10 @@ __global__ void __launch_bounds__(NEB_BLOCK) k_neb_update(const __grid_constant_
   __shared__ double cell[9], inv[9], mix[4];
   const ani_neb_state& s = a.s;
   const int m = s.n_images - 2, ci = blockIdx.y, b = ci / m, j = blockIdx.x * NEB_BLOCK + threadIdx.x;
-  if (threadIdx.x < 32) {   // the band's partials: lane-strided in order, then a fixed tree towards lane 0
+  if (threadIdx.x < 32) {   // all of the band's partials, by fire_totals
     const int np = m * gridDim.x;
-    const double* base = s.fire.partials + 4 * (size_t)b * np;
-    double tot[4] = {0.0, 0.0, 0.0, 0.0};
-    for (int q = threadIdx.x; q < np; q += 32) {
-      const double* p = base + 4 * q;
-      tot[0] += p[0];
-      tot[1] += p[1];
-      tot[2] += p[2];
-      tot[3] = fmax(tot[3], p[3]);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      tot[0] += __shfl_down_sync(ANI_FULL_MASK, tot[0], o);
-      tot[1] += __shfl_down_sync(ANI_FULL_MASK, tot[1], o);
-      tot[2] += __shfl_down_sync(ANI_FULL_MASK, tot[2], o);
-      tot[3] = fmax(tot[3], __shfl_down_sync(ANI_FULL_MASK, tot[3], o));
-    }
+    double tot[4];
+    fire_totals(s.fire.partials + 4 * (size_t)b * np, np, tot);
     if (threadIdx.x == 0) {
       const long long t = s.fire.counter[1];
       const bool leader = blockIdx.x == 0 && ci == b * m;
@@ -213,19 +193,9 @@ __global__ void __launch_bounds__(NEB_BLOCK) k_neb_update(const __grid_constant_
   if (mix[3] != 0.0 || j >= s.n_atoms) return;
   const size_t i = (size_t)ci * s.n_atoms + j;
   if (s.fire.force_scale[i] == 0.0) return;   // fixed and padding atoms: f = 0 and v = 0, so x never moves
-  const double c1 = mix[0], cf = mix[1], st = mix[2];
-  double* v = s.fire.v + 3 * i;
-  double* x = s.fire.x + 3 * i;
-  const double* f = s.neb_force + 3 * i;
-  const double vx = c1 * v[0] + cf * f[0], vy = c1 * v[1] + cf * f[1], vz = c1 * v[2] + cf * f[2];
-  const double px = x[0] + st * vx, py = x[1] + st * vy, pz = x[2] + st * vz;
-  v[0] = vx;
-  v[1] = vy;
-  v[2] = vz;
-  x[0] = px;
-  x[1] = py;
-  x[2] = pz;
-  write_coords(a.coords, i, px, py, pz, a.cells, cell, inv);
+  double xn[3];
+  fire_move(mix, s.neb_force + 3 * i, s.fire.v + 3 * i, s.fire.x + 3 * i, xn);
+  write_coords(a.coords, i, xn[0], xn[1], xn[2], a.cells, cell, inv);
 }
 
 // grid (blocks per image x interior images): with reset, v = 0 and the band's scalars of the current step; then the
@@ -238,14 +208,7 @@ __global__ void __launch_bounds__(NEB_BLOCK) k_neb_init(const __grid_constant__ 
   if (a.reset) {
     if (j < s.n_atoms)
       for (int d = 0; d < 3; ++d) s.fire.v[3 * i + d] = 0.0;
-    if (ci % m == 0 && blockIdx.x == 0 && threadIdx.x == 0) {
-      const int b = ci / m;
-      const double* par = s.fire.params + (size_t)b * ANI_OPT_PARAMS;
-      double* sc = s.fire.scalars + ((size_t)(s.fire.counter[0] & 1) * s.fire.n_conf + b) * ANI_OPT_SCALARS;
-      sc[0] = par[0];
-      sc[1] = par[6];
-      sc[2] = 0.0;
-    }
+    if (ci % m == 0 && blockIdx.x == 0 && threadIdx.x == 0) fire_reset(s.fire, ci / m, s.fire.counter[0]);
   }
   load_cell(a.cells, a.cell_stride, ci, cell, inv);
   __syncthreads();
@@ -265,7 +228,8 @@ bool neb_state_ok(const ani_neb_state* p) {
 // the grid of every launch: (blocks per image, interior images); 0 when it does not fit
 int neb_grid(const ani_neb_state* p, dim3* grid) {
   const long long imgs = (long long)p->fire.n_conf * (p->n_images - 2);
-  if (imgs > 65535 || imgs * p->n_atoms > 0x7fffffffLL) return ANI_ERR_UNSUPPORTED;
+  const int rc = launch_shape(imgs, p->n_atoms);
+  if (rc != ANI_OK) return rc;
   *grid = dim3((p->n_atoms + NEB_BLOCK - 1) / NEB_BLOCK, (unsigned)imgs);
   return ANI_OK;
 }
@@ -276,14 +240,7 @@ int neb_launch(const ani_neb_state* state, const float* grad, const double* ener
   dim3 grid;
   const int rc = neb_grid(state, &grid);
   if (rc != ANI_OK) return rc;
-  NebArgs a = {};
-  a.s = *state;
-  a.grad = grad;
-  a.energies = energies;
-  a.cells = cells;
-  a.cell_stride = cell_stride;
-  a.coords = coords;
-  a.step = step;
+  const NebArgs a = {{grad, energies, cells, cell_stride, coords, 0}, *state, step};
   cudaStream_t st = (cudaStream_t)stream;
   k_neb_dots<<<grid, NEB_BLOCK, 0, st>>>(a);
   k_neb_project<<<grid, NEB_BLOCK, 0, st>>>(a);
@@ -298,15 +255,12 @@ using namespace ani;
 
 extern "C" int ani_b200_neb_init(const ani_neb_state* state, const float* cells, int cell_mode, int reset,
                                  float* coords, void* stream) {
-  if (!neb_state_ok(state) || !coords || cell_mode < 0 || cell_mode > 2 || (cell_mode && !cells))
-    return ANI_ERR_BAD_ARG;
+  NebArgs a = {};
+  if (!neb_state_ok(state) || !coords || !init_cells(a, cells, cell_mode)) return ANI_ERR_BAD_ARG;
   dim3 grid;
   const int rc = neb_grid(state, &grid);
   if (rc != ANI_OK) return rc;
-  NebArgs a = {};
   a.s = *state;
-  a.cells = cell_mode ? cells : nullptr;
-  a.cell_stride = cell_mode == 2 ? 9 : 0;
   a.coords = coords;
   a.reset = reset != 0;
   k_neb_init<<<grid, NEB_BLOCK, 0, (cudaStream_t)stream>>>(a);

@@ -30,14 +30,8 @@ namespace ani {
 
 constexpr int OPT_BLOCK = ANI_MD_BLOCK;
 
-struct OptArgs {
+struct OptArgs : LoopArgs {
   ani_opt_state s;
-  const float* grad;          // f32[n][3] dE/dx (Hartree / A), input order
-  const double* energies;     // f64[n_conf]
-  const float* cells;         // cell rows (f32[9]) of conformer c at cells + c * cell_stride; nullptr = open
-  int cell_stride;
-  float* coords;              // f32[n][3]
-  int reset;                  // (ani_b200_opt_init)
 };
 
 struct OptCellArgs : OptArgs {
@@ -124,16 +118,12 @@ __device__ __forceinline__ void deformed_cell(const double* h0, const double* f,
 // {V, -tr W / (3 V), E + p0 V} of step t, and returns the cell rows' {P, F2, V2, max row^2} in part
 __device__ void cell_rows(const OptCellArgs& a, int c, long long t, double* part) {
   const ani_opt_cell& q = a.q;
-  const int l = threadIdx.x;
-  double w[9];
-  for (int k = 0; k < 9; ++k) w[k] = 0.0;
   const double* vs = q.virial + (size_t)c * q.virial_slots * 9;
-  for (int b = l; b < q.virial_slots; b += 32)
-    for (int k = 0; k < 9; ++k) w[k] += vs[9 * b + k];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1)
-    for (int k = 0; k < 9; ++k) w[k] += __shfl_down_sync(ANI_FULL_MASK, w[k], o);
-  if (l != 0) return;
+  double w[9];
+  warp_reduce<9, 0>(threadIdx.x, q.virial_slots, [&](int b, double* v) {
+    for (int k = 0; k < 9; ++k) v[k] = vs[9 * b + k];
+  }, w);
+  if (threadIdx.x != 0) return;
   const double* m = cell_slot(q, a.s.n_conf, c, t);
   const double *d = m, *vc = m + 9, *f = m + 18;
   const double* par = q.params + (size_t)c * ANI_OPT_CELL_PARAMS;   // p0, c, unit
@@ -268,22 +258,9 @@ __global__ void __launch_bounds__(OPT_BLOCK) k_opt_update(const __grid_constant_
   __shared__ double cell[CELL ? 27 : 9], inv[9], mix[4];   // CELL: then F(t), F(t+1)
   const ani_opt_state& s = a.s;
   const int c = blockIdx.y, j = blockIdx.x * OPT_BLOCK + threadIdx.x, nb = gridDim.x;
-  if (threadIdx.x < 32) {   // the conformer's partials: lane-strided in order, then a fixed tree towards lane 0
-    double tot[4] = {0.0, 0.0, 0.0, 0.0};
-    for (int b = threadIdx.x; b < nb; b += 32) {
-      const double* q = s.partials + 4 * ((size_t)c * nb + b);
-      tot[0] += q[0];
-      tot[1] += q[1];
-      tot[2] += q[2];
-      tot[3] = fmax(tot[3], q[3]);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      tot[0] += __shfl_down_sync(ANI_FULL_MASK, tot[0], o);
-      tot[1] += __shfl_down_sync(ANI_FULL_MASK, tot[1], o);
-      tot[2] += __shfl_down_sync(ANI_FULL_MASK, tot[2], o);
-      tot[3] = fmax(tot[3], __shfl_down_sync(ANI_FULL_MASK, tot[3], o));
-    }
+  if (threadIdx.x < 32) {   // the conformer's partials, by fire_totals
+    double tot[4];
+    fire_totals(s.partials + 4 * (size_t)c * nb, nb, tot);
     if (threadIdx.x == 0) {
       fire_scalars<ANI_OPT_RECORD>(s, c, s.counter[1], tot, blockIdx.x == 0, a.energies + c, mix);
       if constexpr (CELL) cell_move(a, c, s.counter[1], mix, cell, inv);
@@ -295,7 +272,6 @@ __global__ void __launch_bounds__(OPT_BLOCK) k_opt_update(const __grid_constant_
   const size_t i = (size_t)c * s.n_per_conf + j;
   const double fs = s.force_scale[i];
   if (fs == 0.0) return;   // fixed and padding atoms: f = 0 and v = 0, so x never moves
-  const double c1 = mix[0], cf = mix[1], st = mix[2];
   double fx = -(double)a.grad[3 * i + 0] * fs, fy = -(double)a.grad[3 * i + 1] * fs,
          fz = -(double)a.grad[3 * i + 2] * fs;
   if constexpr (CELL) {   // g = f F(t), as in k_opt_reduce
@@ -305,16 +281,10 @@ __global__ void __launch_bounds__(OPT_BLOCK) k_opt_update(const __grid_constant_
     fx = gx;
     fy = gy;
   }
-  const double vx = c1 * s.v[3 * i + 0] + cf * fx;
-  const double vy = c1 * s.v[3 * i + 1] + cf * fy;
-  const double vz = c1 * s.v[3 * i + 2] + cf * fz;
-  const double x = s.x[3 * i + 0] + st * vx, y = s.x[3 * i + 1] + st * vy, z = s.x[3 * i + 2] + st * vz;
-  s.v[3 * i + 0] = vx;
-  s.v[3 * i + 1] = vy;
-  s.v[3 * i + 2] = vz;
-  s.x[3 * i + 0] = x;
-  s.x[3 * i + 1] = y;
-  s.x[3 * i + 2] = z;
+  const double f[3] = {fx, fy, fz};
+  double xn[3];
+  fire_move(mix, f, s.v + 3 * i, s.x + 3 * i, xn);
+  const double x = xn[0], y = xn[1], z = xn[2];
   if constexpr (CELL) {   // r = F(t+1) u(t+1), wrapped into the float32-rounded h0 F(t+1)^T
     const double* f = cell + 18;
     write_coords(a.coords, i, f[0] * x + f[1] * y + f[2] * z, f[3] * x + f[4] * y + f[5] * z,
@@ -326,26 +296,13 @@ __global__ void __launch_bounds__(OPT_BLOCK) k_opt_update(const __grid_constant_
 
 // one CTA per conformer: with reset, v = 0 and the scalars of the current step; then the coordinates of x
 __global__ void __launch_bounds__(OPT_BLOCK) k_opt_init(const __grid_constant__ OptArgs a) {
-  __shared__ double cell[9], inv[9];
   const ani_opt_state& s = a.s;
   const int c = blockIdx.x, A = s.n_per_conf;
-  const size_t base = (size_t)c * A;
   if (a.reset) {
-    for (int j = threadIdx.x; j < 3 * A; j += OPT_BLOCK) s.v[3 * base + j] = 0.0;
-    if (threadIdx.x == 0) {
-      const double* par = s.params + (size_t)c * ANI_OPT_PARAMS;
-      double* sc = s.scalars + ((size_t)(s.counter[0] & 1) * s.n_conf + c) * ANI_OPT_SCALARS;
-      sc[0] = par[0];
-      sc[1] = par[6];
-      sc[2] = 0.0;
-    }
+    for (int j = threadIdx.x; j < 3 * A; j += OPT_BLOCK) s.v[3 * (size_t)c * A + j] = 0.0;
+    if (threadIdx.x == 0) fire_reset(s, c, s.counter[0]);
   }
-  load_cell(a.cells, a.cell_stride, c, cell, inv);
-  __syncthreads();
-  for (int j = threadIdx.x; j < A; j += OPT_BLOCK) {
-    const size_t i = base + j;
-    write_coords(a.coords, i, s.x[3 * i + 0], s.x[3 * i + 1], s.x[3 * i + 2], a.cells, cell, inv);
-  }
+  conformer_coords(a, c, A, s.x);
 }
 
 // one CTA per conformer: with reset, v = 0, the scalars of the current step and the master {0, 0, I}; then the float32
@@ -361,11 +318,7 @@ __global__ void __launch_bounds__(OPT_BLOCK) k_opt_cell_init(const __grid_consta
   if (a.reset) {
     for (int j = threadIdx.x; j < 3 * A; j += OPT_BLOCK) s.v[3 * base + j] = 0.0;
     if (threadIdx.x == 0) {
-      const double* par = s.params + (size_t)c * ANI_OPT_PARAMS;
-      double* sc = s.scalars + ((size_t)(t & 1) * s.n_conf + c) * ANI_OPT_SCALARS;
-      sc[0] = par[0];
-      sc[1] = par[6];
-      sc[2] = 0.0;
+      fire_reset(s, c, t);
       for (int k = 0; k < 18; ++k) m[k] = 0.0;
       for (int k = 0; k < 9; ++k) m[18 + k] = (k % 4 == 0) ? 1.0 : 0.0;
     }
@@ -399,14 +352,9 @@ int opt_step(const ani_opt_state* s, const float* grad, const double* energies, 
              float* coords, void* stream) {
   if (!opt_state_ok(s) || !s->conv_step || !s->record || !s->partials || s->record_rows < 1) return ANI_ERR_BAD_ARG;
   if (!grad || !energies || !coords) return ANI_ERR_BAD_ARG;
-  if ((long long)s->n_conf * s->n_per_conf > 0x7fffffffLL || s->n_conf > 65535) return ANI_ERR_UNSUPPORTED;
-  OptArgs a = {};
-  a.s = *s;
-  a.grad = grad;
-  a.energies = energies;
-  a.cells = cells;
-  a.cell_stride = cell_stride;
-  a.coords = coords;
+  const int rc = launch_shape(s->n_conf, s->n_per_conf);
+  if (rc != ANI_OK) return rc;
+  const OptArgs a = {{grad, energies, cells, cell_stride, coords, 0}, *s};
   const dim3 grid((s->n_per_conf + OPT_BLOCK - 1) / OPT_BLOCK, s->n_conf);
   cudaStream_t st = (cudaStream_t)stream;
   k_opt_reduce<false><<<grid, OPT_BLOCK, 0, st>>>(a);
@@ -426,12 +374,9 @@ using namespace ani;
 
 extern "C" int ani_b200_opt_init(const ani_opt_state* state, const float* cells, int cell_mode, int reset,
                                  float* coords, void* stream) {
-  if (!opt_state_ok(state) || !coords || cell_mode < 0 || cell_mode > 2 || (cell_mode && !cells))
-    return ANI_ERR_BAD_ARG;
   OptArgs a = {};
+  if (!opt_state_ok(state) || !coords || !init_cells(a, cells, cell_mode)) return ANI_ERR_BAD_ARG;
   a.s = *state;
-  a.cells = cell_mode ? cells : nullptr;
-  a.cell_stride = cell_mode == 2 ? 9 : 0;
   a.coords = coords;
   a.reset = reset != 0;
   k_opt_init<<<state->n_conf, OPT_BLOCK, 0, (cudaStream_t)stream>>>(a);
@@ -468,13 +413,9 @@ extern "C" int ani_b200_opt_cell_step(const ani_opt_state* state, const ani_opt_
   const ani_opt_state* s = state;
   if (!opt_state_ok(s) || !s->conv_step || !s->record || !s->partials || s->record_rows < 1) return ANI_ERR_BAD_ARG;
   if (!opt_cell_ok(cell) || !grad || !energies || !coords) return ANI_ERR_BAD_ARG;
-  if ((long long)s->n_conf * s->n_per_conf > 0x7fffffffLL || s->n_conf > 65535) return ANI_ERR_UNSUPPORTED;
-  OptCellArgs a = {};
-  a.s = *s;
-  a.q = *cell;
-  a.grad = grad;
-  a.energies = energies;
-  a.coords = coords;
+  const int rc = launch_shape(s->n_conf, s->n_per_conf);
+  if (rc != ANI_OK) return rc;
+  const OptCellArgs a = {{{grad, energies, nullptr, 0, coords, 0}, *s}, *cell};
   const dim3 grid((s->n_per_conf + OPT_BLOCK - 1) / OPT_BLOCK, s->n_conf);
   cudaStream_t st = (cudaStream_t)stream;
   k_opt_reduce<true><<<grid, OPT_BLOCK, 0, st>>>(a);

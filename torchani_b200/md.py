@@ -22,7 +22,6 @@ from __future__ import annotations
 import ctypes as C
 import math
 import typing as tp
-import warnings
 
 import numpy as np
 import torch
@@ -32,6 +31,7 @@ from . import _lib
 from ._lib import check, ptr
 from .engine import conformer_cells
 from .grad import BAR_TO_HARTREE_A3, HARTREE_TO_JOULE, _AMU, _E
+from .nn import fall_back_to_bf16x3
 
 __all__ = ["VelocityVerlet", "Langevin", "LangevinNPT", "maxwell_boltzmann", "Thermo", "Frames", "NPT", "ACCEL", "KB",
            "ASE_TIME_FS", "BAR_TO_HARTREE_A3"]
@@ -63,6 +63,16 @@ class NPT(tp.NamedTuple):
     pressure: np.ndarray      # (S, C) bar: the internal pressure (2 E_kin - tr W) / (3 V), W the force step's virial
 
 
+def _host(x, dtype=None) -> np.ndarray:
+    """An input as a numpy array (a tensor is copied to the host)."""
+    return np.asarray(x.detach().cpu() if isinstance(x, Tensor) else x, dtype=dtype)
+
+
+def _per_conf(x, n: int) -> np.ndarray:
+    """A scalar or one value per conformer as (n,) float64."""
+    return np.broadcast_to(np.asarray(x, dtype=np.float64).reshape(-1), (n,))
+
+
 def maxwell_boltzmann(masses, temperature, seed: int = 0) -> np.ndarray:
     """Velocities (..., A, 3) float64 in A / fs drawn from the Maxwell-Boltzmann distribution at ``temperature`` (K; a
     scalar, or one per conformer for masses (C, A)), with the centre-of-mass momentum of every conformer set to zero.
@@ -88,9 +98,8 @@ class _DeviceLoop:
     redo of the work from a saved state, and K steps -- the loop's own launches (``_integrate``) and the fused force
     step -- captured into one CUDA graph.
 
-    A subclass holds its state in ``_head`` (restored on a redo; ``_backup`` is the saved copy), the records a replay
-    copies to the host in ``_rec`` (to ``_h_rec``), and defines ``_init_launch(reset)`` (the coordinates of the current
-    state and, with ``reset``, its initial values), ``_integrate()`` and ``_collect(t0, k)``."""
+    A subclass lays out its float64 buffer with ``_layout`` and defines ``_init_launch(reset)`` (the coordinates of the
+    current state and, with ``reset``, its initial values) and ``_integrate()``."""
 
     isobaric = False   # the force step accumulates the virial, and the cells are the loop's (LangevinNPT)
     qbc = False        # the force step is the query-by-committee step
@@ -102,14 +111,13 @@ class _DeviceLoop:
         if dev.type != "cuda":
             raise ValueError(f"{self._what} needs a model on a CUDA device")
         self.model, self.device = model, dev
-        pb = np.asarray(pbc if not isinstance(pbc, Tensor) else pbc.cpu(), dtype=bool).reshape(-1)
+        pb = _host(pbc, bool).reshape(-1)
         if pb.size not in (1, 3) or (pb.any() and not pb.all()):
             raise ValueError("partial PBC is not supported: the system is fully periodic or open")
         self.pbc = bool(pb.all())
         if self.pbc and cell is None:
             raise ValueError("If pbc is not None, cell should be present")
-        z = torch.as_tensor(np.asarray(atomic_numbers if not isinstance(atomic_numbers, Tensor)
-                                       else atomic_numbers.cpu()))
+        z = torch.as_tensor(_host(atomic_numbers))
         C_ = z.shape[0] if z.dim() == 2 else 1
         z = z.reshape(C_, -1).to(dev)
         self.n_conf, self.n_per_conf = C_, z.shape[1]
@@ -120,13 +128,93 @@ class _DeviceLoop:
         self._cell32 = None
         if not self.pbc:
             return None
-        c64 = np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float64)
+        c64 = _host(cell, np.float64)
         c = torch.as_tensor(c64.astype(np.float32))
         if c.dim() == 3 and C_ == 1:
             c = c.reshape(3, 3)
         self.per_conf = conformer_cells(c, C_)
         self._cell32 = c.to(dev)
         return c64
+
+    def _layout(self, head, flags, records) -> tp.Dict[str, Tensor]:
+        """Lay out the float64 buffer ``_buf`` from named segments (name, shape[, dtype]) in this order: ``head``, the
+        state a redone replay restores (``_head``, saved in ``_backup``); ``flags``, the stop or convergence words, -1
+        until set, which end the head and start what a replay copies to the host (``_rec`` to ``_h_rec``); and
+        ``records``, the record rings and frames ``_collect`` gathers.  Returns the device views by name."""
+        segs = [(s[0], s[1], s[2] if len(s) > 2 else torch.float64) for s in (*head, *flags, *records)]
+        ends = np.cumsum([math.prod(shape) for _, shape, _ in segs]).tolist()
+        n_head, r0 = ends[len(head) + len(flags) - 1], ends[len(head) - 1]
+        self._buf = torch.zeros(ends[-1], dtype=torch.float64, device=self.device)
+        self._head, self._rec = self._buf[:n_head], self._buf[r0:]
+        self._backup = torch.empty_like(self._head)
+        self._h_rec = torch.zeros(self._rec.numel(), dtype=torch.float64).pin_memory()
+        self._h_status = torch.zeros(1, dtype=torch.int32).pin_memory()
+        views, host = {}, {}
+        for (name, shape, dtype), b in zip(segs, ends):
+            a = b - math.prod(shape)
+            views[name] = self._buf[a:b].view(dtype).view(shape)
+            if a >= r0:
+                host[name] = self._h_rec[a - r0:b - r0].view(dtype).view(shape).numpy()
+        for s in flags:
+            views[s[0]].fill_(-1)
+        self._h_flags = self._h_rec[:n_head - r0].view(torch.int64).numpy()
+        self._flags = np.full(self._h_flags.shape, -1, dtype=np.int64)   # as of the last replay
+        self._h_records = {s[0]: host[s[0]] for s in records}
+        self._records: tp.Dict[str, tp.List[np.ndarray]] = {s[0]: [] for s in records}
+        self.step = 0   # steps done (the device counter, mirrored)
+        self._graph: tp.Optional[torch.cuda.CUDAGraph] = None
+        return views
+
+    def _rows(self, name: str, t0: int, k: int) -> tp.List[int]:
+        """The rows of record segment ``name`` that steps t0 .. t0 + k - 1 wrote: those of a ring of K rows."""
+        return [(t0 + i) % self.K for i in range(k)]
+
+    def _collect(self, t0: int, k: int) -> None:
+        for name, h in self._h_records.items():
+            self._records[name].append(h[self._rows(name, t0, k)].copy())
+        self._flags = self._h_flags.copy()
+
+    def _joined(self, name: str, last: bool = False) -> np.ndarray:
+        """The collected rows of record segment ``name`` (``last``: of the last replay only), steps ascending."""
+        parts = self._records[name][-1:] if last else self._records[name]
+        return np.concatenate([np.zeros((0,) + self._h_records[name].shape[1:])] + parts)
+
+    def _run(self, steps: int, callback, args: tp.Callable[[], tuple],
+             start: tp.Optional[tp.Callable[[], None]] = None) -> bool:
+        """``start()``, then ``steps`` steps: replays of ``steps_per_replay`` steps, the remainder as eager launches of
+        the same sequence (bitwise the same result), each followed by ``callback(step, *args())``; the run ends early
+        once every flag word is set.  Returns whether they all are."""
+        steps = int(steps)
+        if steps < 0:
+            raise ValueError("steps must be >= 0")
+        with torch.cuda.device(self.device):
+            if start is not None:
+                start()
+            done = 0
+            while done < steps:
+                k = min(self.K, steps - done)
+                self._advance(k)
+                done += k
+                if callback is not None:
+                    callback(self.step, *args())
+                if bool((self._flags >= 0).all()):
+                    break
+        return bool((self._flags >= 0).all())
+
+    def _init_cell(self) -> tuple:
+        """(cell pointer, cell_mode) of the init entry points: cell_mode 0 open, 1 one cell, 2 one per conformer."""
+        return ptr(self.ws.cell) if self.pbc else None, 2 if self.per_conf else (1 if self.pbc else 0)
+
+    def _step_call(self, name: str, *args) -> None:
+        """ani_b200_<name>(state, grad, energies, *args, cell, coords, stream) with the fixed cell, or its ``_cells``
+        twin with the lattice table of one cell per conformer."""
+        ws, L = self.ws, self.engine.lib
+        if self.per_conf:
+            fn, cell = getattr(L, f"ani_b200_{name}_cells"), ptr(ws.lattice)
+        else:
+            fn, cell = getattr(L, f"ani_b200_{name}"), ptr(ws.cell) if self.pbc else None
+        check(fn(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), *args, cell, ptr(ws.coords), self._stream()),
+              name)
 
     # -- engine and workspace ----------------------------------------------------------------
     def _attach_engine(self) -> None:
@@ -179,12 +267,8 @@ class _DeviceLoop:
         try:
             self.engine.check_status(self.ws)
         except _lib.OperandRangeError:
-            nets = self.model.neural_networks
-            if nets._variant == "bf16x3" or not _lib.available("bf16x3"):
+            if not fall_back_to_bf16x3(self.model.neural_networks):
                 raise
-            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this model "
-                          "to the 3 x bfloat16 build of the library")
-            nets.use_variant("bf16x3")
             self._attach_engine()
             return True
         return False
@@ -239,7 +323,6 @@ class _Dynamics(_DeviceLoop):
         self.isobaric = barostat is not None
         c64 = self._set_system(model, atomic_numbers, cell, pbc, steps_per_replay)
         dev, C_, A = self.device, self.n_conf, self.n_per_conf
-        n = C_ * A
         real = (self.species >= 0).cpu().numpy()
         m = np.asarray(masses, dtype=np.float64)
         m = np.broadcast_to(m.reshape(-1, A), (C_, A))
@@ -248,8 +331,7 @@ class _Dynamics(_DeviceLoop):
         n_real = real.sum(1)
         if (n_real == 0).any():
             raise ValueError("every conformer needs at least one real atom")
-        T = np.broadcast_to(np.asarray(temperature, dtype=np.float64).reshape(-1), (C_,))
-        g = np.broadcast_to(np.asarray(friction, dtype=np.float64).reshape(-1), (C_,))
+        T, g = _per_conf(temperature, C_), _per_conf(friction, C_)
         if self.integrator == _lib.MD_LANGEVIN:
             if not (np.isfinite(T) & (T > 0)).all():
                 raise ValueError("temperature must be > 0 K")
@@ -257,8 +339,8 @@ class _Dynamics(_DeviceLoop):
                 raise ValueError("friction must be >= 0 (1 / fs)")
         self.qbc = qbc_stop is not None
         e_thr, f_thr = (None, None) if qbc_stop is None else qbc_stop
-        e_thr = np.broadcast_to(np.asarray(math.inf if e_thr is None else e_thr, dtype=np.float64).reshape(-1), (C_,))
-        f_thr = np.broadcast_to(np.asarray(math.inf if f_thr is None else f_thr, dtype=np.float64).reshape(-1), (C_,))
+        e_thr = _per_conf(math.inf if e_thr is None else e_thr, C_)
+        f_thr = _per_conf(math.inf if f_thr is None else f_thr, C_)
         self.record_every = int(record_every)
         if self.K < 1 or self.record_every < 0:
             raise ValueError("steps_per_replay must be >= 1 and record_every >= 0")
@@ -272,40 +354,23 @@ class _Dynamics(_DeviceLoop):
                 raise ValueError("constant pressure needs a finite cell of volume > 0 for every conformer")
 
         f64 = dict(dtype=torch.float64, device=dev)
-        # [x 3n | v 3n | counter 2 | master cells 2 C 9 (NPT) | stop_step C | thermo K C 4 | frames | NPT records K C 2 |
-        # frame cells F C 9]: the head up to stop_step is what a redone replay restores, the tail from stop_step on is
-        # what a replay copies to the host
         self.frame_slots = -(-self.K // self.record_every) if self.record_every else 0
         self.frame_f = 2 if record_velocities else 1
-        nm = 18 * C_ if self.isobaric else 0
-        head = 6 * n + 2 + nm + C_
-        n_th, n_fr = self.K * C_ * _lib.ANI_MD_THERMO, self.frame_slots * self.frame_f * 3 * n
-        n_bar, n_fc = (self.K * C_ * _lib.ANI_MD_BARO, self.frame_slots * C_ * 9) if self.isobaric else (0, 0)
-        self._buf = torch.zeros(head + n_th + n_fr + n_bar + n_fc, **f64)
-        self.x = self._buf[:3 * n].view(C_, A, 3)
-        self.v = self._buf[3 * n:6 * n].view(C_, A, 3)
-        self._counter = self._buf[6 * n:6 * n + 2].view(torch.int64)
-        self._master = self._buf[6 * n + 2:6 * n + 2 + nm].view(2, C_, 3, 3) if self.isobaric else None
-        self._stop = self._buf[head - C_:head].view(torch.int64)
-        self._rec = self._buf[head - C_:]
-        self._head = self._buf[:head]
-        self._backup = torch.empty_like(self._head)
-        self._thermo_dev = self._buf[head:head + n_th]
-        self._frames_dev = self._buf[head + n_th:head + n_th + n_fr]
-        self._baro_dev = self._buf[head + n_th + n_fr:head + n_th + n_fr + n_bar]
-        self._fcells_dev = self._buf[head + n_th + n_fr + n_bar:]
-        if self.isobaric:
+        npt = self.isobaric
+        seg = self._layout(
+            [("x", (C_, A, 3)), ("v", (C_, A, 3)), ("counter", (2,), torch.int64)] +
+            ([("master", (2, C_, 3, 3))] if npt else []),
+            [("stop", (C_,), torch.int64)],
+            [("thermo", (self.K, C_, _lib.ANI_MD_THERMO)), ("frames", (self.frame_slots, self.frame_f, C_, A, 3))] +
+            ([("npt", (self.K, C_, _lib.ANI_MD_BARO)), ("frame_cells", (self.frame_slots, C_, 3, 3))] if npt else []))
+        self.x, self.v, self._counter, self._stop = seg["x"], seg["v"], seg["counter"], seg["stop"]
+        self._master = seg.get("master")
+        self._seg = seg
+        if npt:
             self._master[0].copy_(torch.from_numpy(np.array(c64)).to(dev))
-        self._h_rec = torch.zeros(self._rec.numel(), dtype=torch.float64).pin_memory()
-        self._h_status = torch.zeros(1, dtype=torch.int32).pin_memory()
-        pos = torch.as_tensor(positions if not isinstance(positions, Tensor) else positions.detach().cpu()
-                              ).to(torch.float64).reshape(C_, A, 3)
-        self.x.copy_(pos.to(dev))
+        self.x.copy_(torch.from_numpy(_host(positions, np.float64)).reshape(C_, A, 3).to(dev))
         if velocities is not None:
-            vel = torch.as_tensor(velocities if not isinstance(velocities, Tensor) else velocities.detach().cpu()
-                                  ).to(torch.float64).reshape(C_, A, 3)
-            self.v.copy_(vel.to(dev))
-        self._stop.fill_(-1)
+            self.v.copy_(torch.from_numpy(_host(velocities, np.float64)).reshape(C_, A, 3).to(dev))
         inv = np.where(real, 1.0 / np.where(real, m, 1.0), 0.0)
         self.inv_mass = torch.from_numpy(np.ascontiguousarray(inv)).to(**f64).reshape(-1)
         params = np.zeros((C_, _lib.ANI_MD_PARAMS))
@@ -323,20 +388,13 @@ class _Dynamics(_DeviceLoop):
         st = _lib.MDState()
         st.x, st.v, st.inv_mass, st.params = ptr(self.x), ptr(self.v), ptr(self.inv_mass), ptr(self.params)
         st.counter, st.stop_step, st.trigger = ptr(self._counter), ptr(self._stop), ptr(self.trigger)
-        st.thermo, st.frames, st.partials = ptr(self._thermo_dev), ptr(self._frames_dev), ptr(self._partials)
+        st.thermo, st.frames, st.partials = ptr(seg["thermo"]), ptr(seg["frames"]), ptr(self._partials)
         st.seed = int(seed) & (2 ** 64 - 1)
         st.accel, st.kb = ACCEL, KB
         st.n_conf, st.n_per_conf, st.integrator = C_, A, self.integrator
         st.thermo_rows, st.record_every = self.K, self.record_every
         st.frame_slots, st.frame_velocities = self.frame_slots, int(self.frame_f == 2)
         self._state = st
-        self.step = 0   # steps done (the device counter, mirrored)
-        self._stop_host = np.full(C_, -1, dtype=np.int64)
-        self._thermo: tp.List[np.ndarray] = []
-        self._frames: tp.List[tp.Tuple[int, np.ndarray]] = []
-        self._npt_rec: tp.List[np.ndarray] = []
-        self._frame_cells: tp.List[np.ndarray] = []
-        self._graph: tp.Optional[torch.cuda.CUDAGraph] = None
         self._zero_momentum = bool(zero_momentum)
         with torch.cuda.device(dev):
             self._attach_engine()
@@ -350,7 +408,7 @@ class _Dynamics(_DeviceLoop):
             b = _lib.MDBarostat()
             b.master, b.params, b.virial = ptr(self._master), ptr(self.baro_params), ptr(ws.virial)
             b.cell_out, b.cell_stride = ptr(ws.cells) if self.per_conf else ptr(ws.cell), 9
-            b.record, b.frame_cells = ptr(self._baro_dev), ptr(self._fcells_dev)
+            b.record, b.frame_cells = ptr(self._seg["npt"]), ptr(self._seg["frame_cells"])
             b.virial_slots = _lib.ANI_VIRIAL_SLOTS
             self._baro = b
 
@@ -362,68 +420,31 @@ class _Dynamics(_DeviceLoop):
                 self.ws.cells.copy_(h.reshape(self.n_conf, 9))
             else:
                 self.ws.cell.copy_(h.reshape(-1))
-        mode = 2 if self.per_conf else (1 if self.pbc else 0)
-        check(self.engine.lib.ani_b200_md_init(
-            C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, mode,
-            int(reset and self._zero_momentum), ptr(self.ws.coords), self._stream()), "md_init")
+        check(self.engine.lib.ani_b200_md_init(C.byref(self._state), *self._init_cell(),
+                                               int(reset and self._zero_momentum), ptr(self.ws.coords),
+                                               self._stream()), "md_init")
 
     def _integrate(self) -> None:
         """The integrator launches of one step (ani_b200_md_step: finish step t, start step t + 1)."""
-        ws, L = self.ws, self.engine.lib
+        ws = self.ws
         if self.isobaric:
-            check(L.ani_b200_md_step_npt(C.byref(self._state), C.byref(self._baro), ptr(ws.grad), ptr(ws.energies),
-                                         ptr(ws.coords), self._stream()), "md_step_npt")
-            return
-        qbc = ptr(ws.qbc) if self.qbc else None
-        stdev = ptr(ws.atom_stats[1]) if self.qbc else None
-        if self.per_conf:
-            rc = L.ani_b200_md_step_cells(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), qbc, stdev,
-                                          ptr(ws.lattice), ptr(ws.coords), self._stream())
+            check(self.engine.lib.ani_b200_md_step_npt(C.byref(self._state), C.byref(self._baro), ptr(ws.grad),
+                                                       ptr(ws.energies), ptr(ws.coords), self._stream()), "md_step_npt")
         else:
-            rc = L.ani_b200_md_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), qbc, stdev,
-                                    ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
-        check(rc, "md_step")
+            self._step_call("md_step", ptr(ws.qbc) if self.qbc else None, ptr(ws.atom_stats[1]) if self.qbc else None)
 
-    def _collect(self, t0: int, k: int) -> None:
-        C_, K = self.n_conf, self.K
-        h = self._h_rec.numpy()
-        o_fr = C_ + self._thermo_dev.numel()
-        o_bar = o_fr + self._frames_dev.numel()
-        o_fc = o_bar + self._baro_dev.numel()
-        rows = [(t0 + i) % K for i in range(k)]
-        th = h[C_:o_fr].reshape(K, C_, _lib.ANI_MD_THERMO)
-        self._thermo.append(th[rows].copy())
-        if self.isobaric:
-            self._npt_rec.append(h[o_bar:o_fc].reshape(K, C_, _lib.ANI_MD_BARO)[rows].copy())
-        if self.record_every:
-            fr = h[o_fr:o_bar].reshape(self.frame_slots, self.frame_f, C_, self.n_per_conf, 3)
-            fc = h[o_fc:].reshape(self.frame_slots, C_, 3, 3) if self.isobaric else None
-            for t in range(t0, t0 + k):
-                if t % self.record_every == 0:
-                    slot = (t // self.record_every) % self.frame_slots
-                    self._frames.append((t, fr[slot].copy()))
-                    if self.isobaric:
-                        self._frame_cells.append(fc[slot].copy())
-        self._stop_host = h[:C_].view(np.int64).copy()
+    def _rows(self, name: str, t0: int, k: int) -> tp.List[int]:
+        if name in ("frames", "frame_cells"):   # the slot of every recorded step
+            re = self.record_every
+            return [(t // re) % self.frame_slots for t in range(t0, t0 + k) if t % re == 0] if re else []
+        return super()._rows(name, t0, k)
 
     def run(self, steps: int, callback: tp.Optional[tp.Callable[..., tp.Any]] = None) -> None:
         """Run ``steps`` MD steps: replays of ``steps_per_replay`` steps, the remainder as eager launches of the same
         sequence (bitwise the same result).  ``callback(step, positions, velocities, thermo)`` runs after every replay
         (``thermo``: that replay's records).  With ``qbc_stop`` the run ends early once every conformer has stopped;
         the force steps of stopped conformers go on to the end of their replay (at most K - 1 wasted steps each)."""
-        steps = int(steps)
-        if steps < 0:
-            raise ValueError("steps must be >= 0")
-        with torch.cuda.device(self.device):
-            done = 0
-            while done < steps:
-                k = min(self.K, steps - done)
-                self._advance(k)
-                done += k
-                if callback is not None:
-                    callback(self.step, self.positions, self.velocities, self._as_thermo(self._thermo[-1]))
-                if self.qbc and bool((self._stop_host >= 0).all()):
-                    break
+        self._run(steps, callback, lambda: (self.positions, self.velocities, self._as_thermo(self._joined("thermo", True))))
 
     # -- results ----------------------------------------------------------------------------------
     @property
@@ -455,19 +476,13 @@ class _Dynamics(_DeviceLoop):
 
     @property
     def thermo(self) -> Thermo:
-        if not self._thermo:
-            z = np.zeros((0, self.n_conf))
-            return Thermo(np.zeros(0, dtype=np.int64), z, z.copy(), z.copy())
-        return self._as_thermo(np.concatenate(self._thermo))
+        return self._as_thermo(self._joined("thermo"))
 
     @property
     def frames(self) -> Frames:
-        shape = (0, self.n_conf, self.n_per_conf, 3)
-        if not self._frames:
-            return Frames(np.zeros(0, dtype=np.int64), np.zeros(shape), np.zeros(shape) if self.frame_f == 2 else None)
-        f = np.stack([fr for _, fr in self._frames])
-        return Frames(np.array([t for t, _ in self._frames], dtype=np.int64), f[:, 0],
-                      f[:, 1] if self.frame_f == 2 else None)
+        f = self._joined("frames")
+        steps = np.arange(0, self.step, self.record_every) if self.record_every else np.zeros(0, dtype=np.int64)
+        return Frames(steps, f[:, 0], f[:, 1] if self.frame_f == 2 else None)
 
     @property
     def stop_step(self) -> np.ndarray:
@@ -571,8 +586,7 @@ class LangevinNPT(_Dynamics):
             raise ValueError("qbc_stop is not supported at constant pressure: the query-by-committee step computes no "
                              "virial")
         n_conf = np.shape(atomic_numbers)[0] if np.ndim(atomic_numbers) == 2 else 1
-        p0 = np.broadcast_to(np.asarray(pressure, dtype=np.float64).reshape(-1), (n_conf,))
-        beta = np.broadcast_to(np.asarray(compressibility, dtype=np.float64).reshape(-1), (n_conf,))
+        p0, beta = _per_conf(pressure, n_conf), _per_conf(compressibility, n_conf)
         tau_p = float(tau_p)
         if not np.isfinite(p0).all():
             raise ValueError("pressure must be finite (bar)")
@@ -597,19 +611,13 @@ class LangevinNPT(_Dynamics):
 
     @property
     def npt(self) -> NPT:
-        th = self.thermo
-        if not self._npt_rec:
-            z = np.zeros((0, self.n_conf))
-            return NPT(th.step, z, z.copy())
-        r = np.concatenate(self._npt_rec)
-        return NPT(th.step, r[..., 0].copy(), r[..., 1] / BAR_TO_HARTREE_A3)
+        r = self._joined("npt")
+        return NPT(self.thermo.step, r[..., 0].copy(), r[..., 1] / BAR_TO_HARTREE_A3)
 
     @property
     def frame_cells(self) -> np.ndarray:
         """(F, C, 3, 3) float64: the cell of every frame of ``frames``."""
-        if not self._frame_cells:
-            return np.zeros((0, self.n_conf, 3, 3))
-        return np.stack(self._frame_cells)
+        return self._joined("frame_cells")
 
 
 def noise(seed: int, step: int, n: int, device) -> Tensor:

@@ -26,7 +26,7 @@ from .engine import Engine, StepResult, check_pair_cutoff
 from .neighbors import (CellList, Neighbors, NeighborlistArg, _validate_inputs, discard_outside_cutoff,
                         effective_periodic_cell, narrow_down, supercell_for_thin_cell)
 from .nn import (ANINetworks, ATOMIC_NUMBER, AtomicContainer, AtomicNetwork, Ensemble, SpeciesConverter,
-                 SpeciesEnergies)
+                 SpeciesEnergies, fall_back_to_bf16x3)
 from .potentials import PairPotential, TwoBodyDispersionD3
 from . import potentials as _potentials
 
@@ -281,13 +281,8 @@ class ANI(torch.nn.Module):
         try:
             return fn()
         except _lib.OperandRangeError:
-            nets = self.neural_networks
-            if nets._variant == "bf16x3" or not _lib.available("bf16x3"):
+            if not fall_back_to_bf16x3(self.neural_networks):
                 raise
-            import warnings
-            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this model "
-                          "to the 3 x bfloat16 build of the library")
-            nets.use_variant("bf16x3")
             return fn()
 
     @staticmethod
@@ -874,13 +869,8 @@ class ANIq(ANI):
         try:
             return fn()
         except _lib.OperandRangeError:
-            if self.neural_networks._variant == "bf16x3" or not _lib.available("bf16x3"):
+            if not fall_back_to_bf16x3(self.neural_networks, self.charge_networks):
                 raise
-            import warnings
-            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this model "
-                          "(energy and charge networks) to the 3 x bfloat16 build of the library")
-            self.neural_networks.use_variant("bf16x3")
-            self.charge_networks.use_variant("bf16x3")
             return fn()
 
     def _step_with_charges(self, species_coordinates, cell, pbc, charge: int, want_grad: tp.Optional[bool] = None):

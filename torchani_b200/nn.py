@@ -278,12 +278,8 @@ class AtomicContainer(torch.nn.Module):
         try:
             e_m = _MLPFunction.apply(aevs, elem_idxs, self.packed(aevs.device), bool(aevs.requires_grad))  # (M, C, A)
         except _lib.OperandRangeError:
-            # a value left the range of the fp16 operand pieces: switch to the 3 x bfloat16 build and redo
-            if self._variant == "bf16x3" or not _lib.available("bf16x3"):
+            if not fall_back_to_bf16x3(self):
                 raise
-            warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this "
-                          "container to the 3 x bfloat16 build of the library")
-            self.use_variant("bf16x3")
             e_m = _MLPFunction.apply(aevs, elem_idxs, self.packed(aevs.device), bool(aevs.requires_grad))
         nets = self._packed
         if ensemble_values:
@@ -293,6 +289,20 @@ class AtomicContainer(torch.nn.Module):
                              dtype=e_m.dtype, device=e_m.device).view(-1, 1, 1)
         out = (e_m * scale).sum(0)
         return out if atomic else out.sum(-1)
+
+
+def fall_back_to_bf16x3(*containers: AtomicContainer) -> bool:
+    """The response to ANI_STATUS_OPERAND_RANGE (a value left the range of the 2 x fp16 operand pieces): False when the
+    first container already runs on the 3 x bfloat16 build or that build is missing (the caller re-raises); otherwise
+    warn, move every container to the 3 x bfloat16 build -- same kernels, 6 instead of 4 bytes per operand element, no
+    range limit -- and return True (the caller redoes its work)."""
+    if containers[0]._variant == "bf16x3" or not _lib.available("bf16x3"):
+        return False
+    warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching to the 3 x bfloat16 "
+                  "build of the library")
+    for c in containers:
+        c.use_variant("bf16x3")
+    return True
 
 
 class ANINetworks(AtomicContainer):

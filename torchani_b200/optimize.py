@@ -43,7 +43,8 @@ from torch import Tensor
 from . import _lib
 from ._lib import check, ptr
 from .grad import BAR_TO_HARTREE_A3, HARTREE_TO_EV
-from .md import _DeviceLoop
+from .md import _DeviceLoop, _host, _per_conf
+from .nn import fall_back_to_bf16x3
 
 __all__ = ["FIRE", "CellFIRE", "LBFGS", "NEB", "interpolate", "Log", "CellLog", "NEBLog", "HARTREE_TO_EV",
            "BAR_TO_HARTREE_A3"]
@@ -66,79 +67,57 @@ class CellLog(tp.NamedTuple):
     enthalpy: np.ndarray   # (S, C) Hartree: E + p0 V
 
 
+def _fixed_mask(fixed, n: int, A: int) -> np.ndarray:
+    """``fixed`` (None, or an (A,) or (n, A) boolean mask) as an (n, A) mask."""
+    fix = np.zeros((n, A), dtype=bool)
+    if fixed is not None:
+        f = _host(fixed)
+        if f.dtype != bool or f.shape not in ((A,), (n, A)):
+            raise ValueError(f"fixed must be a boolean mask of shape ({A},) or ({n}, {A}), got {f.dtype} {f.shape}")
+        fix[:] = f
+    return fix
+
+
 class _Optimizer(_DeviceLoop):
     """What the device optimisers share: the system, the fixed mask and ``force_scale``, one float64 buffer
-    [x 3n | the optimiser's state | conv_step O | records K O R | extra records] whose head up to conv_step is what a
-    redone replay restores and whose tail from conv_step on is what a replay copies to the host, ``run``, ``_collect``
-    and the results.  O is the number of optimisations (``_n_opt``: one per conformer, one per band for ``NEB``) and R
-    the words of a record (``_record_words``).  A subclass sizes its state (``_state_words``), carves it, and names its
-    parameter column of the fmax threshold (``_fmax_col``)."""
+    [x | the optimiser's state | conv_step O | log K O R | further records], ``run`` and the results.  O is the number
+    of optimisations (``_n_opt``: one per conformer, one per band for ``NEB``) and R the words of a record
+    (``_record_words``).  A subclass lists its state (``_state_segments``) and further records (``_record_segments``)
+    and names its parameter column of the fmax threshold (``_fmax_col``)."""
 
     _fmax_col = 0
     _record_words = _lib.ANI_OPT_RECORD
-    _cell_record_words = 0   # per conformer and step: records beyond the optimiser's own (CellFIRE's)
 
     @property
     def _n_opt(self) -> int:
         return self.n_conf
 
-    def _state_words(self) -> int:
+    def _state_segments(self) -> tp.List[tuple]:
         raise NotImplementedError
 
+    def _record_segments(self) -> tp.List[tuple]:
+        return []
+
     def _allocate(self, model, atomic_numbers, positions, cell, pbc, fixed, steps_per_replay):
-        """The system and the buffer; returns the float64 cell and the state words of the buffer."""
+        """The system and the buffer; returns the float64 cell and the buffer's views by name."""
         if int(steps_per_replay) < 1:
             raise ValueError("steps_per_replay must be >= 1")
         c64 = self._set_system(model, atomic_numbers, cell, pbc, steps_per_replay)
-        dev, C_, A, O = self.device, self.n_conf, self.n_per_conf, self._n_opt
-        n = C_ * A
+        C_, A = self.n_conf, self.n_per_conf
+        self.fixed = _fixed_mask(fixed, C_, A)
+        seg = self._layout([("x", (C_, A, 3))] + self._state_segments(), [("conv", (self._n_opt,), torch.int64)],
+                           [("log", (self.K, self._n_opt, self._record_words))] + self._record_segments())
+        self.x, self._conv = seg["x"], seg["conv"]
+        self.x.copy_(torch.from_numpy(_host(positions, np.float64)).reshape(C_, A, 3).to(self.device))
         real = (self.species >= 0).cpu().numpy()
-        fix = np.zeros((C_, A), dtype=bool)
-        if fixed is not None:
-            f = np.asarray(fixed if not isinstance(fixed, Tensor) else fixed.cpu())
-            if f.dtype != bool or f.shape not in ((A,), (C_, A)):
-                raise ValueError(f"fixed must be a boolean mask of shape ({A},) or ({C_}, {A}), got {f.dtype} "
-                                 f"{f.shape}")
-            fix[:] = f
-        self.fixed = fix
-
-        f64 = dict(dtype=torch.float64, device=dev)
-        ns = self._state_words()
-        head = 3 * n + ns + O
-        n_rec = self.K * O * self._record_words
-        self._buf = torch.zeros(head + n_rec + self.K * C_ * self._cell_record_words, **f64)
-        self.x = self._buf[:3 * n].view(C_, A, 3)
-        self._conv = self._buf[head - O:head].view(torch.int64)
-        self._rec = self._buf[head - O:]
-        self._head = self._buf[:head]
-        self._backup = torch.empty_like(self._head)
-        self._record_dev = self._buf[head:head + n_rec]
-        self._cell_record_dev = self._buf[head + n_rec:]
-        self._h_rec = torch.zeros(self._rec.numel(), dtype=torch.float64).pin_memory()
-        self._h_status = torch.zeros(1, dtype=torch.int32).pin_memory()
-        pos = torch.as_tensor(positions if not isinstance(positions, Tensor) else positions.detach().cpu()
-                              ).to(torch.float64).reshape(C_, A, 3)
-        self.x.copy_(pos.to(dev))
-        self._conv.fill_(-1)
-        scale = np.where(real & ~fix, HARTREE_TO_EV, 0.0)
-        self.force_scale = torch.from_numpy(scale).to(**f64).reshape(-1)
-        self.step = 0   # steps done (the device counter, mirrored)
-        self._conv_host = np.full(O, -1, dtype=np.int64)
-        self._log: tp.List[np.ndarray] = []
-        self._graph: tp.Optional[torch.cuda.CUDAGraph] = None
-        return c64, self._buf[3 * n:3 * n + ns]
+        scale = np.where(real & ~self.fixed, HARTREE_TO_EV, 0.0)
+        self.force_scale = torch.from_numpy(scale).to(dtype=torch.float64, device=self.device).reshape(-1)
+        return c64, seg
 
     def _start(self) -> None:
         with torch.cuda.device(self.device):
             self._attach_engine()
             self._begin(True)
-
-    def _collect(self, t0: int, k: int) -> None:
-        O = self._n_opt
-        h = self._h_rec.numpy()
-        rows = [(t0 + i) % self.K for i in range(k)]
-        self._log.append(h[O:O + self._record_dev.numel()].reshape(self.K, O, self._record_words)[rows].copy())
-        self._conv_host = h[:O].view(np.int64).copy()
 
     def run(self, fmax: float = 0.05, steps: int = 1000,
             callback: tp.Optional[tp.Callable[..., tp.Any]] = None) -> bool:
@@ -147,29 +126,20 @@ class _Optimizer(_DeviceLoop):
         conformer converged.  A new ``run`` starts a new convergence check and keeps the optimiser's state (FIRE's v,
         dt, a, n; L-BFGS's history), so a second ``run`` with a smaller ``fmax`` continues the optimisation, as ASE's
         does.  ``callback(step, positions, log)`` runs after every replay (``log``: that replay's records)."""
-        fmax, steps = float(fmax), int(steps)
+        fmax = float(fmax)
         if not (math.isfinite(fmax) and fmax >= 0):
             raise ValueError(f"fmax must be >= 0 eV/A, got {fmax}")
-        if steps < 0:
-            raise ValueError("steps must be >= 0")
-        with torch.cuda.device(self.device):
+
+        def start() -> None:
             self.params[:, self._fmax_col].fill_(fmax)
             self._conv.fill_(-1)
-            self._conv_host[:] = -1
-            done = 0
-            while done < steps:
-                k = min(self.K, steps - done)
-                self._advance(k)
-                done += k
-                if callback is not None:
-                    callback(self.step, self.positions, self._as_log(self._log[-1]))
-                if bool((self._conv_host >= 0).all()):
-                    break
-        return bool((self._conv_host >= 0).all())
+            self._flags[:] = -1
 
-    def _cell_mode(self) -> int:
-        """The cell_mode of the init entry points: 0 open, 1 one cell, 2 one cell per conformer."""
-        return 2 if self.per_conf else (1 if self.pbc else 0)
+        return self._run(steps, callback, lambda: (self.positions, self._as_log(self._log_rows(True))), start)
+
+    def _log_rows(self, last: bool = False) -> np.ndarray:
+        """The collected records of ``log`` (``last``: of the last replay only)."""
+        return self._joined("log", last)
 
     # -- results ----------------------------------------------------------------------------------
     @property
@@ -204,10 +174,7 @@ class _Optimizer(_DeviceLoop):
 
     @property
     def log(self) -> Log:
-        if not self._log:
-            z = np.zeros((0, self.n_conf))
-            return Log(np.zeros(0, dtype=np.int64), z, z.copy())
-        return self._as_log(np.concatenate(self._log))
+        return self._as_log(self._log_rows())
 
 
 def _fire_params(dt, maxstep, dtmax, n_min, finc, fdec, astart, fa) -> tp.Tuple[float, ...]:
@@ -253,55 +220,44 @@ class FIRE(_Optimizer):
                  maxstep: float = 0.2, dtmax: float = 1.0, n_min: int = 5, finc: float = 1.1, fdec: float = 0.5,
                  astart: float = 0.1, fa: float = 0.99, steps_per_replay: int = 20):
         par = _fire_params(dt, maxstep, dtmax, n_min, finc, fdec, astart, fa)
-        # state: [v 3n | scalars 2 C 3 | counter 2 | (CellFIRE: master 2 C 27)]
-        c64, st_words = self._allocate(model, atomic_numbers, positions, cell, pbc, fixed, steps_per_replay)
-        dev, C_, A = self.device, self.n_conf, self.n_per_conf
-        n = C_ * A
-        ns = 2 * C_ * _lib.ANI_OPT_SCALARS
-        self.v = st_words[:3 * n].view(C_, A, 3)
-        self._scalars = st_words[3 * n:3 * n + ns].view(2, C_, _lib.ANI_OPT_SCALARS)
-        self._counter = st_words[3 * n + ns:3 * n + ns + 2].view(torch.int64)
-        self._master = st_words[3 * n + ns + 2:]
-        f64 = dict(dtype=torch.float64, device=dev)
-        params = np.zeros((C_, _lib.ANI_OPT_PARAMS))
+        c64, seg = self._allocate(model, atomic_numbers, positions, cell, pbc, fixed, steps_per_replay)
+        self._state = self._fire_state(par, seg)
+        self._setup(c64, seg)
+        self._start()
+
+    def _state_segments(self) -> tp.List[tuple]:
+        return [("v", (self.n_conf, self.n_per_conf, 3)), ("scalars", (2, self._n_opt, _lib.ANI_OPT_SCALARS)),
+                ("counter", (2,), torch.int64)]
+
+    def _fire_state(self, par: tp.Tuple[float, ...], seg: tp.Dict[str, Tensor]) -> _lib.OptState:
+        """FIRE's views of the buffer, parameters and scratch, and its ani_opt_state: one optimisation over the rows
+        of each conformer (or of each band's interior images)."""
+        C_, A, O = self.n_conf, self.n_per_conf, self._n_opt
+        f64 = dict(dtype=torch.float64, device=self.device)
+        self.v, self._scalars, self._counter = seg["v"], seg["scalars"], seg["counter"]
+        params = np.zeros((O, _lib.ANI_OPT_PARAMS))
         params[:, :8] = par
         self.params = torch.from_numpy(params).to(**f64)
         self._partials = torch.zeros(C_ * -(-A // _lib.ANI_MD_BLOCK) * 4, **f64)
         st = _lib.OptState()
         st.x, st.v, st.force_scale, st.params = ptr(self.x), ptr(self.v), ptr(self.force_scale), ptr(self.params)
         st.scalars, st.counter, st.conv_step = ptr(self._scalars), ptr(self._counter), ptr(self._conv)
-        st.record, st.partials = ptr(self._record_dev), ptr(self._partials)
-        st.n_conf, st.n_per_conf, st.record_rows = C_, A, self.K
-        self._state = st
-        self._setup(c64)
-        self._start()
+        st.record, st.partials = ptr(seg["log"]), ptr(self._partials)
+        st.n_conf, st.n_per_conf, st.record_rows = O, C_ // O * A, self.K
+        return st
 
-    _master_words = 0        # per conformer: state a redo restores beyond FIRE's own (CellFIRE's master)
-
-    def _state_words(self) -> int:
-        return 3 * self.n_conf * self.n_per_conf + 2 * self.n_conf * _lib.ANI_OPT_SCALARS + 2 + \
-            self.n_conf * self._master_words
-
-    def _setup(self, cell64: tp.Optional[np.ndarray]) -> None:
+    def _setup(self, cell64: tp.Optional[np.ndarray], seg: tp.Dict[str, Tensor]) -> None:
         """What a subclass adds to the state before the engine is attached."""
 
     # -- the device loop ------------------------------------------------------------------------
     def _init_launch(self, reset: bool) -> None:
         """ani_b200_opt_init (v = 0 and the initial scalars at the start only)."""
-        check(self.engine.lib.ani_b200_opt_init(
-            C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, self._cell_mode(),
-            int(reset), ptr(self.ws.coords), self._stream()), "opt_init")
+        check(self.engine.lib.ani_b200_opt_init(C.byref(self._state), *self._init_cell(), int(reset),
+                                                ptr(self.ws.coords), self._stream()), "opt_init")
 
     def _integrate(self) -> None:
         """The FIRE launches of one step (ani_b200_opt_step: step t to x(t+1))."""
-        ws, L = self.ws, self.engine.lib
-        if self.per_conf:
-            rc = L.ani_b200_opt_step_cells(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), ptr(ws.lattice),
-                                           ptr(ws.coords), self._stream())
-        else:
-            rc = L.ani_b200_opt_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies),
-                                     ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
-        check(rc, "opt_step")
+        self._step_call("opt_step")
 
 
 class CellFIRE(FIRE):
@@ -331,12 +287,10 @@ class CellFIRE(FIRE):
 
     isobaric = True   # the force step accumulates the virial, and the cells are the loop's
     _what = "the device cell optimiser"
-    _master_words = 2 * _lib.ANI_OPT_CELL_MASTER
-    _cell_record_words = _lib.ANI_OPT_CELL_RECORD
 
     def __init__(self, model, atomic_numbers, positions, cell, pbc=True, pressure=0.0, cell_factor=None,
                  hydrostatic_strain: bool = False, constant_volume: bool = False, fixed=None, **fire):
-        pb = np.asarray(pbc if not isinstance(pbc, Tensor) else pbc.cpu(), dtype=bool).reshape(-1)
+        pb = _host(pbc, bool).reshape(-1)
         if cell is None or pb.size not in (1, 3) or not pb.all():
             raise ValueError("variable-cell relaxation needs a fully periodic cell")
         if fixed is not None:
@@ -344,20 +298,19 @@ class CellFIRE(FIRE):
                              "express Cartesian constraints")
         if hydrostatic_strain and constant_volume:
             raise ValueError("hydrostatic_strain and constant_volume are mutually exclusive")
-        z = np.asarray(atomic_numbers if not isinstance(atomic_numbers, Tensor) else atomic_numbers.cpu())
+        z = _host(atomic_numbers)
         n_conf = z.shape[0] if z.ndim == 2 else 1
-        h = np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float64)
+        h = _host(cell, np.float64)
         if h.shape not in ((3, 3), (n_conf, 3, 3)) and not (n_conf == 1 and h.shape == (1, 3, 3)):
             raise ValueError(f"cell must be (3, 3) or ({n_conf}, 3, 3), got {h.shape}")
         h = np.broadcast_to(h.reshape(-1, 3, 3), (n_conf, 3, 3))
         if not (np.isfinite(h).all() and (np.abs(np.linalg.det(h)) > 0).all()):
             raise ValueError("variable-cell relaxation needs a finite cell of volume > 0 for every conformer")
-        p0 = np.broadcast_to(np.asarray(pressure, dtype=np.float64).reshape(-1), (n_conf,))
+        p0 = _per_conf(pressure, n_conf)
         if not np.isfinite(p0).all():
             raise ValueError("pressure must be finite (bar)")
         n_real = (z.reshape(n_conf, -1) >= 0).sum(1).astype(np.float64)
-        cf = n_real if cell_factor is None else np.broadcast_to(
-            np.asarray(cell_factor, dtype=np.float64).reshape(-1), (n_conf,))
+        cf = n_real if cell_factor is None else _per_conf(cell_factor, n_conf)
         if not (np.isfinite(cf) & (cf > 0)).all():
             raise ValueError("cell_factor must be > 0 (and every conformer needs a real atom)")
         self._p0 = p0 * BAR_TO_HARTREE_A3
@@ -367,7 +320,13 @@ class CellFIRE(FIRE):
         super().__init__(model, atomic_numbers, positions, cell=np.array(h, order="C") if n_conf > 1 else cell,
                          pbc=True, **fire)
 
-    def _setup(self, cell64) -> None:
+    def _state_segments(self) -> tp.List[tuple]:
+        return super()._state_segments() + [("master", (2, self.n_conf, _lib.ANI_OPT_CELL_MASTER))]
+
+    def _record_segments(self) -> tp.List[tuple]:
+        return [("cell_log", (self.K, self.n_conf, _lib.ANI_OPT_CELL_RECORD))]
+
+    def _setup(self, cell64, seg) -> None:
         dev, C_ = self.device, self.n_conf
         f64 = dict(dtype=torch.float64, device=dev)
         # (a C-order copy: numpy's default copy of a broadcast keeps the conformer axis innermost)
@@ -375,14 +334,14 @@ class CellFIRE(FIRE):
         par = np.stack([self._p0, self._cell_factor, np.full(C_, HARTREE_TO_EV)], 1)
         self.cell_params = torch.from_numpy(par).to(**f64)
         self._cell_force = torch.zeros(C_, 9, **f64)
-        self._master = self._master.view(2, C_, _lib.ANI_OPT_CELL_MASTER)
+        self._master, self._cell_log_dev = seg["master"], seg["cell_log"]
 
     def _attached(self) -> None:
         q = _lib.OptCell()
         q.master, q.h0, q.params = ptr(self._master), ptr(self.h0), ptr(self.cell_params)
         q.cell_out, q.cell_stride = (ptr(self.ws.cells) if self.per_conf else ptr(self.ws.cell)), 9
         q.virial, q.virial_slots = ptr(self.ws.virial), _lib.ANI_VIRIAL_SLOTS
-        q.cell_force, q.record, q.projection = ptr(self._cell_force), ptr(self._cell_record_dev), self._projection
+        q.cell_force, q.record, q.projection = ptr(self._cell_force), ptr(self._cell_log_dev), self._projection
         self._cell = q
 
     def _init_launch(self, reset: bool) -> None:
@@ -398,12 +357,8 @@ class CellFIRE(FIRE):
                                                      ptr(ws.energies), ptr(ws.coords), self._stream()),
               "opt_cell_step")
 
-    def _collect(self, t0: int, k: int) -> None:
-        super()._collect(t0, k)
-        h = self._h_rec.numpy()
-        rows = [(t0 + i) % self.K for i in range(k)]
-        cr = h[self.n_conf + self._record_dev.numel():].reshape(self.K, self.n_conf, _lib.ANI_OPT_CELL_RECORD)
-        self._log[-1] = np.concatenate([self._log[-1], cr[rows]], -1)
+    def _log_rows(self, last: bool = False) -> np.ndarray:
+        return np.concatenate([self._joined("log", last), self._joined("cell_log", last)], -1)
 
     # -- results ----------------------------------------------------------------------------------
     @property
@@ -442,12 +397,6 @@ class CellFIRE(FIRE):
     def _as_log(r: np.ndarray) -> CellLog:
         return CellLog(r[:, 0, 0].astype(np.int64), r[..., 1].copy(), r[..., 2].copy(), r[..., 3].copy(),
                        r[..., 4] / BAR_TO_HARTREE_A3, r[..., 5].copy())
-
-    @property
-    def log(self) -> CellLog:
-        if not self._log:
-            return self._as_log(np.zeros((0, self.n_conf, _lib.ANI_OPT_RECORD + _lib.ANI_OPT_CELL_RECORD)))
-        return self._as_log(np.concatenate(self._log))
 
 
 class LBFGS(_Optimizer):
@@ -491,19 +440,10 @@ class LBFGS(_Optimizer):
         if maxstep > 1.0:
             warnings.warn(f"a much too large maximum step size for L-BFGS: {maxstep:.1f} A")
         self.memory = int(memory)
-        # state: [x_prev 3n | g_prev 3n | s C M 3A | y C M 3A | SY C M M | YY C M M | {k, head} 2 C | counter 2]
-        c64, st_words = self._allocate(model, atomic_numbers, positions, cell, pbc, fixed, steps_per_replay)
-        dev, C_, A, M = self.device, self.n_conf, self.n_per_conf, self.memory + 1
-        n = C_ * A
-        o = np.cumsum([0, 3 * n, 3 * n, C_ * M * 3 * A, C_ * M * 3 * A, C_ * M * M, C_ * M * M, 2 * C_, 2])
-        self.x_prev = st_words[o[0]:o[1]].view(C_, A, 3)
-        self.g_prev = st_words[o[1]:o[2]].view(C_, A, 3)
-        self._s = st_words[o[2]:o[3]].view(C_, M, A, 3)
-        self._y = st_words[o[3]:o[4]].view(C_, M, A, 3)
-        self._sy = st_words[o[4]:o[5]].view(C_, M, M)
-        self._yy = st_words[o[5]:o[6]].view(C_, M, M)
-        self._iter = st_words[o[6]:o[7]].view(torch.int64).view(C_, 2)
-        self._counter = st_words[o[7]:o[8]].view(torch.int64)
+        _, seg = self._allocate(model, atomic_numbers, positions, cell, pbc, fixed, steps_per_replay)
+        dev, C_, A = self.device, self.n_conf, self.n_per_conf
+        self.x_prev, self.g_prev, self._s, self._y = seg["x_prev"], seg["g_prev"], seg["s"], seg["y"]
+        self._sy, self._yy, self._iter, self._counter = seg["sy"], seg["yy"], seg["iter"], seg["counter"]
         f64 = dict(dtype=torch.float64, device=dev)
         params = np.zeros((C_, _lib.ANI_LBFGS_PARAMS))
         params[:, :3] = (maxstep, damping, 1.0 / alpha)
@@ -516,31 +456,24 @@ class LBFGS(_Optimizer):
         st.s, st.y, st.sy, st.yy = ptr(self._s), ptr(self._y), ptr(self._sy), ptr(self._yy)
         st.coef, st.p, st.iter = ptr(self._coef), ptr(self._p), ptr(self._iter)
         st.force_scale, st.params, st.counter = ptr(self.force_scale), ptr(self.params), ptr(self._counter)
-        st.conv_step, st.record, st.partials = ptr(self._conv), ptr(self._record_dev), ptr(self._partials)
+        st.conv_step, st.record, st.partials = ptr(self._conv), ptr(seg["log"]), ptr(self._partials)
         st.n_conf, st.n_per_conf, st.memory, st.record_rows = C_, A, self.memory, self.K
         self._state = st
         self._start()
 
-    def _state_words(self) -> int:
+    def _state_segments(self) -> tp.List[tuple]:
         C_, A, M = self.n_conf, self.n_per_conf, self.memory + 1
-        return 6 * C_ * A + 2 * C_ * M * 3 * A + 2 * C_ * M * M + 2 * C_ + 2
+        return [("x_prev", (C_, A, 3)), ("g_prev", (C_, A, 3)), ("s", (C_, M, A, 3)), ("y", (C_, M, A, 3)),
+                ("sy", (C_, M, M)), ("yy", (C_, M, M)), ("iter", (C_, 2), torch.int64), ("counter", (2,), torch.int64)]
 
     def _init_launch(self, reset: bool) -> None:
         """ani_b200_lbfgs_init (x_prev = x, g_prev = 0 and an empty history at the start only)."""
-        check(self.engine.lib.ani_b200_lbfgs_init(
-            C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, self._cell_mode(),
-            int(reset), ptr(self.ws.coords), self._stream()), "lbfgs_init")
+        check(self.engine.lib.ani_b200_lbfgs_init(C.byref(self._state), *self._init_cell(), int(reset),
+                                                  ptr(self.ws.coords), self._stream()), "lbfgs_init")
 
     def _integrate(self) -> None:
         """The L-BFGS launches of one step (ani_b200_lbfgs_step: step t to x(t+1))."""
-        ws, L = self.ws, self.engine.lib
-        if self.per_conf:
-            rc = L.ani_b200_lbfgs_step_cells(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), ptr(ws.lattice),
-                                             ptr(ws.coords), self._stream())
-        else:
-            rc = L.ani_b200_lbfgs_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies),
-                                       ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
-        check(rc, "lbfgs_step")
+        self._step_call("lbfgs_step")
 
     @property
     def iteration(self) -> np.ndarray:
@@ -569,7 +502,7 @@ class NEBLog(tp.NamedTuple):
 _NEB_METHODS = {"aseneb": _lib.ANI_NEB_ASENEB, "improvedtangent": _lib.ANI_NEB_IMPROVED_TANGENT}
 
 
-class NEB(_Optimizer):
+class NEB(FIRE):
     """A nudged elastic band relaxed by FIRE on the device: ASE's ``FIRE(NEB(images, k, climb, method))`` for every
     band of a batch, with the interior images of all bands evaluated by one force step.
 
@@ -607,7 +540,6 @@ class NEB(_Optimizer):
     """
 
     _what = "the device NEB"
-    _fmax_col = 8
     _record_words = _lib.ANI_NEB_RECORD
 
     def __init__(self, model, atomic_numbers, images, cell=None, pbc=False, fixed=None, k=0.1, climb: bool = False,
@@ -622,7 +554,7 @@ class NEB(_Optimizer):
         if precon is not None:
             raise ValueError("preconditioned NEB is not supported")
         par = _fire_params(dt, maxstep, dtmax, n_min, finc, fdec, astart, fa)
-        x = np.asarray(images if not isinstance(images, Tensor) else images.detach().cpu(), dtype=np.float64)
+        x = _host(images, np.float64)
         if x.ndim == 3:
             x = x[None]
         if x.ndim != 4 or x.shape[-1] != 3:
@@ -635,16 +567,11 @@ class NEB(_Optimizer):
             raise ValueError(f"B (n - 2) = {B * m} interior images exceed 65535")
         if not np.isfinite(x).all():
             raise ValueError("images must be finite")
-        z = np.asarray(atomic_numbers if not isinstance(atomic_numbers, Tensor) else atomic_numbers.cpu())
+        z = _host(atomic_numbers)
         if z.shape not in ((A,), (B, A)):
             raise ValueError(f"atomic_numbers must be ({A},) or ({B}, {A}), got {z.shape}")
         z = np.broadcast_to(z.reshape(-1, A), (B, A))
-        fix = np.zeros((B, A), dtype=bool)
-        if fixed is not None:
-            f = np.asarray(fixed if not isinstance(fixed, Tensor) else fixed.cpu())
-            if f.dtype != bool or f.shape not in ((A,), (B, A)):
-                raise ValueError(f"fixed must be a boolean mask of shape ({A},) or ({B}, {A}), got {f.dtype} {f.shape}")
-            fix[:] = f
+        fix = _fixed_mask(fixed, B, A)
         for b in range(B):   # t is zeroed on fixed atoms: ASE's result only if they sit still along the band
             if not (x[b][:, fix[b]] == x[b, 0][fix[b]]).all():
                 raise ValueError(f"fixed atoms must have the same positions in every image of a band (band {b})")
@@ -657,38 +584,24 @@ class NEB(_Optimizer):
         # the cell of the force step: shared (grid mode 2) or one per interior image (grid mode 3)
         fcell = None
         if cell is not None:
-            h = np.asarray(cell if not isinstance(cell, Tensor) else cell.cpu(), dtype=np.float64)
+            h = _host(cell, np.float64)
             if h.shape not in ((3, 3), (B, 3, 3)):
                 raise ValueError(f"cell must be (3, 3) or ({B}, 3, 3), got {h.shape}")
             fcell = h.reshape(3, 3) if h.ndim == 2 or B == 1 else np.repeat(h, m, 0)
         self.n_bands, self.n_images, self.method = B, n, method
         self._climb = bool(climb)
-        c64, st_words = self._allocate(model, np.repeat(z, m, 0), x[:, 1:-1].reshape(B * m, A, 3), fcell, pbc,
-                                       np.repeat(fix, m, 0), steps_per_replay)
-        dev, C_ = self.device, self.n_conf
-        nn_ = C_ * A
-        ns = 2 * B * _lib.ANI_OPT_SCALARS
-        self.v = st_words[:3 * nn_].view(C_, A, 3)
-        self._scalars = st_words[3 * nn_:3 * nn_ + ns].view(2, B, _lib.ANI_OPT_SCALARS)
-        self._counter = st_words[3 * nn_ + ns:3 * nn_ + ns + 2].view(torch.int64)
-        f64 = dict(dtype=torch.float64, device=dev)
-        params = np.zeros((B, _lib.ANI_OPT_PARAMS))
-        params[:, :8] = par
-        self.params = torch.from_numpy(params).to(**f64)
+        _, seg = self._allocate(model, np.repeat(z, m, 0), x[:, 1:-1].reshape(B * m, A, 3), fcell, pbc,
+                                np.repeat(fix, m, 0), steps_per_replay)
+        C_, f64 = self.n_conf, dict(dtype=torch.float64, device=self.device)
+        st = _lib.NebState()
+        st.fire = self._fire_state(par, seg)
         nb = -(-A // _lib.ANI_MD_BLOCK)
-        self._partials = torch.zeros(C_ * nb * 4, **f64)
         self._dots = torch.zeros(C_ * nb * _lib.ANI_NEB_DOTS, **f64)
         self._neb_force = torch.zeros(C_, A, 3, **f64)
         self.endpoints = torch.from_numpy(np.ascontiguousarray(x[:, [0, n - 1]])).to(**f64)
         self.end_energies = torch.zeros(B, 2, **f64)
         self.springs = torch.from_numpy(kk).to(**f64)
         self._climb_dev = torch.full((B,), 1.0 if self._climb else 0.0, **f64)
-        st = _lib.NebState()
-        fs = st.fire
-        fs.x, fs.v, fs.force_scale, fs.params = ptr(self.x), ptr(self.v), ptr(self.force_scale), ptr(self.params)
-        fs.scalars, fs.counter, fs.conv_step = ptr(self._scalars), ptr(self._counter), ptr(self._conv)
-        fs.record, fs.partials = ptr(self._record_dev), ptr(self._partials)
-        fs.n_conf, fs.n_per_conf, fs.record_rows = B, m * A, self.K
         st.endpoints, st.end_energies, st.springs = ptr(self.endpoints), ptr(self.end_energies), ptr(self.springs)
         st.climb, st.neb_force, st.dots = ptr(self._climb_dev), ptr(self._neb_force), ptr(self._dots)
         st.n_images, st.n_atoms, st.method = n, A, _NEB_METHODS[method]
@@ -699,9 +612,6 @@ class NEB(_Optimizer):
     @property
     def _n_opt(self) -> int:
         return self.n_bands
-
-    def _state_words(self) -> int:
-        return 3 * self.n_conf * self.n_per_conf + 2 * self.n_bands * _lib.ANI_OPT_SCALARS + 2
 
     def _endpoint_energies(self) -> None:
         """One force step on the 2B endpoint conformers, at float32 coordinates wrapped as the loop writes them."""
@@ -721,12 +631,8 @@ class NEB(_Optimizer):
                     r = self.model.engine(dev).step(z, xe.float(), cell, self.pbc, check=True)
                     break
                 except _lib.OperandRangeError:
-                    nets = self.model.neural_networks
-                    if nets._variant == "bf16x3" or not _lib.available("bf16x3"):
+                    if not fall_back_to_bf16x3(self.model.neural_networks):
                         raise
-                    warnings.warn("torchani_b200: operand range of the 2 x fp16 GEMM format exceeded; switching this "
-                                  "model to the 3 x bfloat16 build of the library")
-                    nets.use_variant("bf16x3")
             self.end_energies.copy_(r.energies.view(B, 2))
         self._end_variant = self.model.neural_networks._variant
 
@@ -748,20 +654,12 @@ class NEB(_Optimizer):
     # -- the device loop ------------------------------------------------------------------------
     def _init_launch(self, reset: bool) -> None:
         """ani_b200_neb_init (v = 0 and the initial scalars at the start only)."""
-        check(self.engine.lib.ani_b200_neb_init(
-            C.byref(self._state), ptr(self.ws.cell) if self.pbc else None, self._cell_mode(),
-            int(reset), ptr(self.ws.coords), self._stream()), "neb_init")
+        check(self.engine.lib.ani_b200_neb_init(C.byref(self._state), *self._init_cell(), int(reset),
+                                                ptr(self.ws.coords), self._stream()), "neb_init")
 
     def _integrate(self) -> None:
         """The NEB launches of one step (ani_b200_neb_step: step t to x(t+1))."""
-        ws, L = self.ws, self.engine.lib
-        if self.per_conf:
-            rc = L.ani_b200_neb_step_cells(C.byref(self._state), ptr(ws.grad), ptr(ws.energies), ptr(ws.lattice),
-                                           ptr(ws.coords), self._stream())
-        else:
-            rc = L.ani_b200_neb_step(C.byref(self._state), ptr(ws.grad), ptr(ws.energies),
-                                     ptr(ws.cell) if self.pbc else None, ptr(ws.coords), self._stream())
-        check(rc, "neb_step")
+        self._step_call("neb_step")
 
     # -- results ----------------------------------------------------------------------------------
     @property
@@ -807,12 +705,6 @@ class NEB(_Optimizer):
     @staticmethod
     def _as_log(r: np.ndarray) -> NEBLog:
         return NEBLog(r[:, 0, 0].astype(np.int64), r[..., 1].copy(), r[..., 2].copy(), r[..., 3].astype(np.int64))
-
-    @property
-    def log(self) -> NEBLog:
-        if not self._log:
-            return self._as_log(np.zeros((0, self.n_bands, _lib.ANI_NEB_RECORD)))
-        return self._as_log(np.concatenate(self._log))
 
 
 def interpolate(initial, final, n_images: int, cell=None, mic: bool = False) -> np.ndarray:
